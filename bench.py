@@ -5,7 +5,8 @@ A "step" = one evaluation of the exact-GP marginal log likelihood through the BB
 preconditioner (rank 100) -> N(0,P) probes -> mBCG (t = 10 probes + y, J = 21 iterations) -> SLQ log-det ->
 log_prob, on synthetic data (BASELINE.md section 2): X ~ U[0,1]^{N x d}, y = sin(3 sum x) + 0.1 eps, RBF.
 
-    python bench.py --gpus 1 --steps 10 --warmup 3            # our engine (libgpbbmm, sm_100a)
+    python bench.py --gpus 1 --steps 10 --warmup 3            # our engine (libgpbbmm, sm_90a)
+    python bench.py ... --dump-outputs DIR                    # also write the last timed step's results as DIR/<name>.npy
     python bench.py --impl reference --steps 2 --warmup 1     # the reference algorithm on the host CPU cores, full N
     torchrun ... bench.py --gpus N ...                        # rows of K sharded over N GPUs (strong scaling)
 
@@ -95,11 +96,11 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "sm_max_mhz": 1980.0}, "fallback (NVIDIA H100 SXM data sheet, 700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     def __init__(self, index=0):
         self.index = index
@@ -143,6 +144,28 @@ class ClockSampler:
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def dump_outputs(out_dir, arrays):
+    """Write the results of the last timed step as out_dir/<name>.npy (float64 for host scalars, float32 otherwise), so that
+    two builds run with the same arguments (hence the same seeded inputs) can be compared output for output."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float32 if a.dtype == np.float32 else np.float64)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
+def mll_result_arrays(res):
+    """The fields of an MllResult as arrays: what a caller of Plan.mll receives."""
+    import numpy as np
+
+    out = {k: np.array([getattr(res, k)], dtype=np.float64)
+           for k in ("mll", "log_prob", "inv_quad", "logdet", "logdet_precond", "cg_iters", "tridiag_size", "precond_rank")}
+    out["resid"] = np.array(list(res.resid), dtype=np.float32)
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------
@@ -270,6 +293,8 @@ def run_reference(args, w):
         "e2e": {"value": val, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
     }
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {k: [float(getattr(r, k))] for k in ("mll", "log_prob", "inv_quad", "logdet", "iters")})
     emit(line)
 
 
@@ -302,7 +327,7 @@ def measure_workload(w, args, env, steps, warmup, sample_clocks=False):
         plan.set_ski(w["grid"], [float(a[0]) for a in axes], [float(a[1] - a[0]) for a in axes])
     plan.set_hypers(w["kind"], w["lengthscale"], w["outputscale"], w["noise"])
     info = plan.info()
-    l2_flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    l2_flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def step():
         l2_flush.zero_()  # evict the L2 between steps (timing rule); ~60 us of the step
@@ -346,12 +371,8 @@ def measure_workload(w, args, env, steps, warmup, sample_clocks=False):
     ach = flops / (kms * 1e-3) / 1e12
     peak = float(peaks["bf16_tflops"])
     trans = (2 if w["kind"] != "rbf" else 1) * rc * n  # transcendental ops per launch (ex2, + sqrt for Matern)
-    mufu_peak = 16.0 * info["n_sm"] * float(peaks.get("sm_max_mhz", 1965.0)) * 1e6  # 16 MUFU/clk/SM (tools/mufu_bench.cu: 15.99)
+    mufu_peak = 16.0 * info["n_sm"] * float(peaks.get("sm_max_mhz", 1980.0)) * 1e6  # 16 ex2 / clk / SM
     traffic = None
-    tpath = os.path.join(ROOT, "profiles", "kmv_tc2_dram_bytes.json")
-    if os.path.exists(tpath) and world == 1 and w is WORKLOADS["c2"] and info["backend"] == "tcgen05":
-        with open(tpath) as f:
-            traffic = json.load(f).get("dram_bytes_per_launch")
     if info["backend"] == "ski":
         nnz = 4 ** d
         abytes = float(n) * nnz * (4 + 8)          # SURVEY.md section 8f: W stored as (int64 index, fp32 value) per non-zero
@@ -365,14 +386,14 @@ def measure_workload(w, args, env, steps, warmup, sample_clocks=False):
                 "info": info, "res": res, "flops": 0.0, "kms": kms,
                 "ctx": dict(plan=plan, x=x, y=y, xd=xd, y_loc=y_loc, e1d=e1d, e2d=e2d, radd=radd, rb=rb, rc=rc, l2_flush=l2_flush, barrier=barrier)}
     roofline = {
-        "bound": "tensor", "kernel": info.get("kernel", "gp::v2::kmv_tc2_kernel" if info["backend"] == "tcgen05" else "gp::kmv_simt_kernel"),
+        "bound": "tensor", "kernel": info.get("kernel", "gp::kmv_tc_kernel" if info["backend"] == "tcgen05" else "gp::kmv_simt_kernel"),
         "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic,
-        "peak_source": f"bf16 dense burst, {peak_src}; the kernel runs kind::tf32 (nominal half of bf16) with a 3xTF32 split",
+        "peak_source": f"bf16 dense burst, {peak_src}; the kernel runs wgmma tf32 (nominal half of bf16) with a 3xTF32 split",
         "ms_per_launch": kms, "algorithmic_flops_per_launch": flops,
         "gpairs_per_s": rc * n / (kms * 1e-3) / 1e9,
         "mufu_bound": {"transcendentals_per_launch": trans, "achieved_per_s": trans / (kms * 1e-3),
                        "peak_per_s_at_max_clock": mufu_peak, "frac": trans / (kms * 1e-3) / mufu_peak,
-                       "note": "all-MUFU ceiling; the kernel evaluates part of the ex2 on the FMA pipe, so frac may exceed 1"},
+                       "note": "all-MUFU ceiling: every ex2 (and Matern sqrt) runs on the MUFU"},
         "algorithmic_bytes_per_launch": 4.0 * (n * d + 2 * n * tt),
     }
     out = {
@@ -452,6 +473,8 @@ def run_c4(args, w):
     torch.cuda.synchronize(dev)
     ms_step = e0.elapsed_time(e1) / args.steps
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"mll": out.detach().float().cpu().numpy()})
     line = {
         "metric": METRIC, "value": B * 1e3 / ms_step, "unit": UNIT, "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -582,8 +605,10 @@ def run_ours(args, w):
         m3["ctx"]["plan"].close()
 
     if rank == 0:
-        cpu = cpu_baseline(w) if not args.no_cpu else None
         res = m["res"]
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, mll_result_arrays(res))
+        cpu = cpu_baseline(w) if not args.no_cpu else None
         parity = None
         if cpu and cpu.get("value"):
             rel = lambda a, b: abs(a - b) / max(abs(b), 1e-300)  # noqa: E731
@@ -614,6 +639,8 @@ def main():
     ap.add_argument("--backend", default="auto", choices=["auto", "tcgen05", "simt"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-c3", action="store_true", help="skip the secondary N=200k record")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the results of the last timed step as DIR/<name>.npy (same arguments => same inputs)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     w = WORKLOADS[args.workload]

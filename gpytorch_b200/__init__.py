@@ -1,5 +1,5 @@
-"""gpytorch_b200 -- B200-native BBMM exact-GP inference behind the gpytorch kernels / LinearOperator /
-ExactMarginalLogLikelihood API surface.  The arithmetic lives in libgpbbmm.so (hand-written sm_100a CUDA,
+"""gpytorch_b200 -- H100-native BBMM exact-GP inference behind the gpytorch kernels / LinearOperator /
+ExactMarginalLogLikelihood API surface.  The arithmetic lives in libgpbbmm.so (hand-written sm_90a CUDA,
 C ABI in include/gp_bbmm.h); this package is the thin Python host mirroring the reference interface.
 """
 from . import _lib, constraints, distributions, functions, kernels, likelihoods, means, mlls, models, operators, settings  # noqa: F401

@@ -86,7 +86,6 @@ PROTOTYPES = {
     "gp_plan_set_comm": (_I, [_P, _P]),
     "gp_kernel_launches": (_L, [_P]),
     "gp_plan_info": (_I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
-    "gp_plan_set_trace": (_I, [_P, _P]),
     "gp_time_kmv_kernel": (_I, [_P, _P, _L, _I, _I, _I, C.POINTER(_F)]),
 }
 

@@ -59,7 +59,7 @@ int nccl_allreduce_double(gp_comm* c, double* buf, size_t count, cudaStream_t st
 
 using namespace gp;
 
-extern "C" const char* gp_version(void) { return "gpbbmm 0.1 (sm_100a; tcgen05 3xTF32 fused K.V, device mBCG, pivoted-Cholesky precond, SLQ)"; }
+extern "C" const char* gp_version(void) { return "gpbbmm 0.1 (sm_90a; wgmma 3xTF32 fused K.V, device mBCG, pivoted-Cholesky precond, SLQ)"; }
 extern "C" const char* gp_last_error(void) { return g_err; }
 extern "C" const char* gp_status_string(int s) {
   switch (s) {
@@ -81,14 +81,14 @@ extern "C" int gp_plan_create(gp_plan** out, int device, void* stream) {
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev == 0) {
-    set_error("libgpbbmm needs a CUDA device (sm_100a); there is no CPU fallback: %s", cudaGetErrorString(e));
+    set_error("libgpbbmm needs a CUDA device (sm_90a); there is no CPU fallback: %s", cudaGetErrorString(e));
     return GP_E_CUDA;
   }
   GP_REQUIRE(device >= 0 && device < ndev, GP_E_SHAPE, "device %d out of range", device);
   GP_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   GP_CUDA(cudaGetDeviceProperties(&prop, device));
-  GP_REQUIRE(prop.major == 10, GP_E_CUDA, "libgpbbmm is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+  GP_REQUIRE(prop.major == 9 && prop.minor == 0, GP_E_CUDA, "libgpbbmm is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
   gp_plan* p = new gp_plan();
   p->device = device;
   p->stream = reinterpret_cast<cudaStream_t>(stream);
@@ -197,12 +197,6 @@ extern "C" int gp_kmv(gp_plan* p, const float* V, int64_t ldv, int t, float* OUT
 extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   p->comm = comm;
-  return GP_OK;
-}
-
-extern "C" int gp_plan_set_trace(gp_plan* p, long long* trace) {
-  GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
-  p->tc_trace = trace;
   return GP_OK;
 }
 

@@ -9,7 +9,7 @@
 // device and later launches become no-ops, so the host never synchronises inside the loop.
 //
 // One iteration = 6 launches and TWO global reductions (round 1: 10 launches, three reductions):
-//   K.V            fused kernel-matmul on the packed direction tiles                          (kmv_tc2.cu)
+//   K.V            fused kernel-matmul on the packed direction tiles                          (kmv_tc.cu) 
 //   finishv_wtv    V = os sum_s partial_s + D P ; per-CTA partials of p.V and of W^T V        (W streamed once)
 //   sum            fixed-order fp64 sums of the partials  -> message 1: [ pV (16) | W^T V (16 k) ]     (all-reduce)
 //   update_precond alpha = gamma / pV ; U += alpha P ; R -= alpha V ; w = W^T R_k - alpha o W^T V ;
@@ -273,7 +273,7 @@ cg_finishv_wtv_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_
 // Z = a_r R - s W w with (a_r, s) = (1/sigma^2, 1/sigma^2) for the constant diagonal, (1/d_r, 1) for a per-row diagonal whose
 // factor W is pre-scaled (pivchol.cu).  Without a preconditioner (k == 0) Z aliases R and z.r = r.r.
 template <bool INIT>
-__global__ void __launch_bounds__(CG_THREADS)
+__global__ void __launch_bounds__(CG_THREADS, 2)   // sm_90 ptxas otherwise caps the INIT variant at 64 registers and spills
 cg_update_precond_kernel(const double* __restrict__ sums1, int iter, float eps, const float* __restrict__ P,
                          const float* __restrict__ V, float* __restrict__ U, float* __restrict__ R, float* __restrict__ Z,
                          const float* __restrict__ W, int k, int wp, const double* __restrict__ wprev,

@@ -1,4 +1,4 @@
-// gp_common.cuh -- shared declarations for libgpbbmm (sm_100a only).
+// gp_common.cuh -- shared declarations for libgpbbmm (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,9 +8,9 @@
 
 #include "../../include/gp_bbmm.h"
 
-#ifndef __CUDA_ARCH_FEAT_SM100_ALL
+#ifndef __CUDA_ARCH_FEAT_SM90_ALL
 #if defined(__CUDA_ARCH__)
-#error "libgpbbmm is written for sm_100a only: compile with -gencode arch=compute_100a,code=sm_100a"
+#error "libgpbbmm is written for sm_90a only: compile with -gencode arch=compute_90a,code=sm_90a"
 #endif
 #endif
 
@@ -18,9 +18,9 @@ namespace gp {
 
 // ---- compile-time geometry ------------------------------------------------------------
 constexpr int TP = 16;         // padded column count of every [N, t] block (t <= 16)
-constexpr int TILE_I = 128;    // rows of K per CTA tile (UMMA M)
-constexpr int TILE_J = 64;     // columns of K per pipeline step (UMMA N of GEMM1, K of GEMM2)
-constexpr int KP_MAX = 128;    // max padded augmented feature width of the tcgen05 path (3d+4 <= 128)
+constexpr int TILE_I = 128;    // rows of K per CTA tile (two wgmma M = 64 warpgroups)
+constexpr int TILE_J = 64;     // columns of K per pipeline step (wgmma N of GEMM1, K of GEMM2)
+constexpr int KP_MAX = 128;    // max padded augmented feature width of the tensor-core path (3d+4 <= 128)
 constexpr int SIMT_TI = 128;   // rows per CTA in the SIMT kernel
 constexpr int SIMT_TJ = 64;    // staged columns per step in the SIMT kernel
 constexpr float LOG2E = 1.4426950408889634f;
@@ -114,7 +114,7 @@ struct gp_comm {
 struct gp_plan {
   int device = 0;
   cudaStream_t stream = nullptr;
-  int n_sm = 148;
+  int n_sm = 132;
   int backend_req = GP_BACKEND_AUTO;
   int backend = GP_BACKEND_SIMT;
   int64_t launches = 0;
@@ -133,13 +133,11 @@ struct gp_plan {
   const float* noise_diag = nullptr;  // optional per-row diagonal D [n2] (FixedNoiseGaussianLikelihood); replaces the scalar noise
   // derived geometry
   int DP = 0;      // padded feature width of the SIMT arrays
-  int KP = 0;      // padded augmented width (3d+4 -> multiple of 8) of the tcgen05 tiles
-  int nsplit = 1;  // column splits of the K.V work (load balance over 148 SMs)
-  int nparts = 1;  // partial-sum slots written by the K.V kernel (nsplit, x2 for the tcgen05 kernel)
+  int KP = 0;      // padded augmented width (3d+4 -> multiple of 8) of the tensor-core tiles
+  int nsplit = 1;  // column splits of the K.V work (load balance over the SMs)
+  int nparts = 1;  // partial-sum slots written by the K.V kernel (nsplit)
   int64_t ntile_i = 0, ntile_j = 0, tiles_per_split = 0;
-  int64_t rows_pad = 0;  // local rows padded to the 256-row CTA block of the tcgen05 kernel: pitch of `partial`, rows of XA
-  bool tc2 = false;      // second-generation tcgen05 kernel (kmv_tc2.cu); the round-1 kernel (kmv_tc.cu) serves KP > 64
-  int npoly = 2;         // of every 8 ex2 evaluations, how many run as a polynomial on the FMA pipe (0, 2, 4)
+  int64_t rows_pad = 0;  // local rows padded to 256: pitch of `partial`, rows of XA
   // device buffers
   int* xbad = nullptr;  // device flag: non-finite value in the packed inputs (lives behind mean[])
   gp::DevBuf mean, scale, Z1, Z2, XA, XB, V16, Vtiles, partial, out16;
@@ -150,14 +148,13 @@ struct gp_plan {
   // kernel sums (GP_BACKEND_SUM): the terms (caller-owned plans over the same rows); while the parent launches a term's K.V
   // kernel the term writes into the parent's partial slots and reads the parent's packed V tiles
   std::vector<gp_plan*> terms;
-  bool sum_tc = false;            // every term runs the tcgen05 kernel (the direction block is packed once for all of them)
+  bool sum_tc = false;            // every term runs the tensor-core kernel (the direction block is packed once for all of them)
   bool sum_any_tc = false;        // at least one term reads the packed V tiles
   float* partial_ext = nullptr;   // set on a TERM for the duration of one launch by its parent
   float* vtiles_ext = nullptr;
   gp::DevBuf part_scale;          // [nparts] outputscale of the term that owns each partial slot
   std::vector<float> part_scale_host;
   void* pinned = nullptr;  // small pinned host scratch
-  long long* tc_trace = nullptr;  // optional device buffer [256][8] for the pipeline event trace of CTA (0,0)
 };
 
 namespace gp {
@@ -165,10 +162,9 @@ namespace gp {
 // ---- launches implemented across the .cu files -------------------------------------------
 int pack_inputs(gp_plan* p);                                            // pack.cu
 int to_v16(gp_plan* p, const float* V, int64_t ldv, int t, int64_t n, float* V16);
-int pack_v_tiles(gp_plan* p, const float* V16);                         // pack.cu (tcgen05 B operand of GEMM2)
-int kmv_partials(gp_plan* p, const float* V16, const int* done_flag);   // dispatch simt / tcgen05
+int pack_v_tiles(gp_plan* p, const float* V16);                         // pack.cu (tensor-core B operand of GEMM2)
+int kmv_partials(gp_plan* p, const float* V16, const int* done_flag);   // dispatch simt / tensor cores
 int kmv_tc_launch_kind(gp_plan* p, int kind, const int* done_flag);     // kind may be GP_DERIV + kind
-int kmv_tc2_launch_kind(gp_plan* p, int kind, const int* done_flag);    // kmv_tc2.cu
 int kmv_simt_launch(gp_plan* p, const float* V16, const int* done_flag);
 int kmv_tc_launch(gp_plan* p, const int* done_flag);
 int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t, int add_noise);

@@ -1,7 +1,7 @@
 // kmv_simt.cu -- fp32 CUDA-core fused kernel-matmul, row extraction, diagonal and the
 // bilinear hyper-parameter gradient.
 //
-// The SIMT K.V kernel is the bring-up / cross-check path for the tcgen05 kernel (kmv_tc.cu) and
+// The SIMT K.V kernel is the bring-up / cross-check path for the tensor-core kernel (kmv_tc.cu) and
 // the backend for d > 41.  It evaluates a_ij = -0.5 |z_i - z_j|^2 by direct differences (no
 // cancellation), so it is also the more accurate of the two.
 // Reference semantics: LazyEvaluatedKernelTensor._matmul (lazy/lazy_evaluated_kernel_tensor.py:245-276),
@@ -290,7 +290,7 @@ __global__ void sum_partials_double_kernel(const double* __restrict__ in, int64_
   out[o] = s;
 }
 
-// tcgen05 path of the bilinear derivative: gout[block][o] = sum_{r,c} L16[r][c] * sum_split partial[split][r][c]
+// tensor-core path of the bilinear derivative: gout[block][o] = sum_{r,c} L16[r][c] * sum_split partial[split][r][c]
 __global__ void bilin_dot_kernel(const float* __restrict__ partial, int nsplit, int64_t rows, int64_t rows_pad,
                                  const float* __restrict__ L16, double* __restrict__ gout, int gstride, int o) {
   __shared__ double red[256];

@@ -1,33 +1,28 @@
-// kmv_tc.cu -- the fused kernel-matmul  out = K(X1,X2) V  on tcgen05 tensor cores (sm_100a).
+// kmv_tc.cu -- the fused kernel-matmul  out = K(X1,X2) V  on Hopper tensor cores (wgmma, sm_90a).
 //
-// Replaces (reference, paths under /root/reference/gpytorch):
+// Replaces (reference, paths relative to the gpytorch package):
 //   sq_dist GEMM + exp over N^2          kernels/kernel.py:26-49, functions/rbf_covariance.py:14-19
 //   Matern poly*exp passes               functions/matern_covariance.py:21-47
 //   dense K @ V inside linear_cg         lazy/lazy_evaluated_kernel_tensor.py:245-276 (chunked form)
-// The N x N matrix K never exists in HBM: per 128 x 64 tile it lives in TMEM only.
+// The N x N matrix K never exists in HBM: per 64 x 64 tile it lives in the registers of one warpgroup.
 //
-// One CTA (320 threads; TWO CTAs are resident per SM) owns one work unit = (128-row tile of K) x (a contiguous range of
-// 64-column tiles).  Per column tile u (TMEM slot u % 2, epilogue warpgroup u % 2):
-//   GEMM1  S  = A_i . B_j^T            tcgen05.mma kind::tf32, M=128 N=64 K=KP (3xTF32 split operands packed by pack.cu so
-//                                      that S_ij = -0.5|z_i - z_j|^2 directly)
-//   EPI    P  = cov(S)                 software pipeline over 8-column groups: tcgen05.ld (two groups ahead) -> ex2/sqrt
-//                                      (MUFU, one group ahead) -> P_hi (tf32, IN PLACE of S) + P_lo (bf16 pairs) -> tcgen05.st
-//   GEMM2  O  = P_hi [V_hi;V_lo] (tf32, N=32) + P_lo V (bf16 x bf16, N=16)   A operand from TMEM, B = V^T tiles in smem;
-//          O[u % 2] is a fresh accumulator per tile, folded into fp32 registers by the epilogue warps two tiles later
-// Operands arrive by bulk TMA (cp.async.bulk, mbarrier complete_tx) from tiles pre-packed in HBM in the exact UMMA
-// K-major no-swizzle layout, through a NS-deep smem ring.  Warp roles: 0-3 / 4-7 the two epilogue warpgroups, 8 TMA
-// producer, 9 TMEM allocator + MMA issuer (converged warp, one elect.sync per batch; GEMM2(u) then GEMM1(u+2) from the
-// same thread => pipe-ordered, which is what makes the in-place P safe without a "slot drained" barrier).
-//
-// What bounds it (tools/mufu_bench.cu, tools/tc_trace.py, profiles/NOTES_r01.md): the MUFU unit does 16 ex2/clk/SM
-// (measured 15.99), i.e. 512 cycles per 128x64 tile.  TMEM holds 4 tile slots per SM (128 columns each: S/P_hi 64,
-// P_lo 32, O 32), every slot is a dependent chain  GEMM1 -> s_full -> ld -> MUFU -> st -> p_full -> GEMM2 -> GEMM1'
-// with ~1000 cycles of fixed latency (mbarrier hand-offs 100-400 each, SS-mode MMA 48 cycles, queueing in the tensor
-// pipe) and the MUFU phases of all slots share one unit, so the tile time is ~512 + 1000/4 cycles.  Two small CTAs per
-// SM instead of one big one: warpgroups inside one CTA fall into lockstep on shared barriers, independent CTAs do not.
-// Every barrier is private to one slot, so an epilogue warp may run one tile ahead of its siblings.
-//
-// TMEM columns (256 per CTA): S / P_hi slots [0,64) [64,128) | P_lo slots [128,160) [160,192) | O slots [192,224) [224,256)
+// One CTA (two warpgroups, two CTAs resident per SM) owns one work unit = (128-row tile of K) x (a contiguous range of
+// 64-column tiles).  Warpgroup w owns rows [64 w, +64) of the tile; both share one B / V stream.  Per column tile:
+//   GEMM1  S  = A_i . B_j^T     wgmma m64n64k8 tf32, both operands in shared memory (3xTF32 split operands packed by
+//                               pack.cu so that S_ij = -0.5|z_i - z_j|^2 directly); S lands in 32 fp32 registers per thread
+//   EPI    P  = cov(S)          ex2 / sqrt on the MUFU, in registers; P = P_hi + P_lo, both tf32 (P_hi: P with the low 13
+//                               bits cleared, P_lo: the exact fp32 residual)
+//   GEMM2  O  = P_hi [V_hi;V_lo] (m64n32k8) + P_lo V_hi (m64n16k8), A operand from registers, B = V^T tiles in shared memory;
+//          a fresh accumulator per tile, folded into fp32 registers after every tile
+// The accumulator of GEMM1 is used directly as the register A operand of GEMM2.  That works because pack.cu stores the
+// columns of every 8-column group of XB in the order 0 4 1 5 2 6 3 7: a thread's accumulator pair (2t, 2t+1) then holds
+// the columns (t, t+4) the tf32 A fragment expects, and the V tiles keep their natural row order.
+// Operands arrive by bulk TMA (cp.async.bulk, mbarrier complete_tx) from tiles pre-packed in HBM in the wgmma K-major
+// no-swizzle layout, through an NS-deep shared-memory ring that thread 0 refills: a stage is reloaded at the start of the
+// tile after the one that used it, once both warpgroups have released it.  There is no separate producer warp: 8 warps
+// per CTA leave 128 registers per thread at two CTAs per SM (a ninth warp puts five warps on one SM sub-partition and
+// caps them at 96, where the wgmma chain spills and is serialised).  The two CTAs per SM keep the tensor core busy while
+// the other CTA's warpgroups are in their MUFU-bound epilogue.
 #include "gp_common.cuh"
 #include "tc_ptx.cuh"
 
@@ -35,93 +30,33 @@ namespace gp {
 
 using namespace ptx;
 
-constexpr int TC_THREADS = 320;  // 2 epilogue warpgroups (one per TMEM slot) + TMA producer + MMA issuer; TWO CTAs per SM
-constexpr int W_PROD = 8, W_MMA = 9;
-// TMEM columns (256 allocated per CTA; two CTAs share the SM's 512)
-constexpr int NSTG = 2;                         // S / P_hi slots (64 columns each): tile u lives in slot u % 2
-constexpr int COL_LO = NSTG * TILE_J;           // 128: P_lo slot u % 2 at COL_LO + (u % 2) * 32 (bf16 pairs)
-constexpr int COL_O = COL_LO + NSTG * (TILE_J / 2);  // 192: O accumulator (32 columns)
-constexpr int TMEM_COLS = 256;
-constexpr int NO = 2;                           // O accumulators (32 columns each): tile u accumulates into O[u % 2]
-static_assert(TILE_J == 64 && COL_O + NO * 2 * TP <= TMEM_COLS, "TMEM budget is laid out for TILE_J = 64");
-constexpr int V_TF32_BYTES = 2 * TILE_J * TP * 4;  // [64/4][32 rows: V_hi(16) | V_lo(16)][4 tf32] = 8192
-constexpr int V_BF16_BYTES = TILE_J * TP * 2;      // [64/8][16 rows][8 bf16]                       = 2048
-constexpr int V_TILE_BYTES = V_TF32_BYTES + V_BF16_BYTES;
-constexpr int MAX_NS = 6;
+constexpr int TC_THREADS = 256;                     // 2 warpgroups
+constexpr int V_TF32_BYTES = 2 * TILE_J * TP * 4;   // [64/4][32 rows: V_hi(16) | V_lo(16)][4 tf32] = 8192
+constexpr int V_TILE_BYTES = V_TF32_BYTES + TILE_J * TP * 2;   // pitch of the packed V tiles in HBM (pack.cu)
+constexpr int MAX_NS = 8;
 
 struct TcBars {
   uint64_t a_full;
   uint64_t b_full[MAX_NS];
-  uint64_t b_empty[MAX_NS];
-  uint64_t s_full[NSTG];
-  uint64_t p_full[NSTG];   // per slot: an epilogue warp may run one tile ahead of its siblings (never two: tile u+2 needs
-                           // GEMM1(u+2), issued after p_full(u) completed), so consecutive tiles must not share a barrier
-  uint64_t o_full[NO];
-  uint32_t tmem_base;
-  uint32_t pad;
+  uint64_t b_empty[MAX_NS];   // 256 arrivals: every consumer thread, after its warpgroup's GEMM2 has read the stage
 };
 
-// P = cov(S), split P = P_hi (tf32, stored in place of S) + P_lo (bf16 pairs), for the 64 columns one thread holds.
-//   RBF: k = 2^a with NO clamp of a at 0: a = -0.5|z_i - z_j|^2 can only come out > 0 through rounding for (near-)duplicate
-//   points, where it is < 2e-6, i.e. k <= 1 + 1.4e-6 -- inside the stated entry tolerance; dropping the FMNMX relieves the
-//   ALU pipe (second-busiest after the XU pipe).  The exact diagonal is still forced to a = 0 in diagonal tiles.
-// The tile is processed as a software pipeline over groups of 8 columns: the MUFU ops of group g+1 are issued BEFORE
-// the split of group g, so that every consumer sits >= 8 MUFU slots (64 pipe cycles) behind its producer -- an in-order
-// warp that reads a MUFU result 2-3 slots after issuing it stalls ~20 cycles each time and lets the XU pipe run dry
-// (measured: one warp alone reached 57 % of the XU rate with the straightforward per-pair loop).
 template <int KIND>
-__device__ __forceinline__ void cov_group8(const uint32_t* __restrict__ s, float (&p)[8]) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-    p[i] = (KIND == GP_RBF) ? ex2_approx(__uint_as_float(s[i])) : cov_from_arg<KIND>(__uint_as_float(s[i]));
-}
-// tf32 truncation (one LOP3 each), residual in [0, 2^-10 p) by one packed FADD2 per pair, rounded to bf16 (RN), two per
-// TMEM column: P is kept to ~2^-19 relative, random sign
-__device__ __forceinline__ void split_group8(const float (&p)[8], uint32_t* __restrict__ hi, uint32_t* __restrict__ lo) {
-#pragma unroll
-  for (int i = 0; i < 8; i += 2) {
-    const uint32_t h0 = __float_as_uint(p[i]) & 0xFFFFE000u, h1 = __float_as_uint(p[i + 1]) & 0xFFFFE000u;
-    float l0, l1;
-    sub_f32x2(p[i], p[i + 1], __uint_as_float(h0), __uint_as_float(h1), l0, l1);
-    lo[i >> 1] = pack_bf16x2(l0, l1);
-    hi[i] = h0;
-    hi[i + 1] = h1;
-  }
-}
-// One step of the pipeline: (1) the S columns of group g+1 (loaded during the previous step) go through the MUFU into
-// pn, (2) the load of group g+2 is put in flight into sn2, (3) group g (MUFU results from the previous step, in pc) is
-// split and stored.  The loop over steps is a REAL loop (not unrolled): ptxas schedules inside one step only, so a MUFU
-// result is never consumed in the step that issued it.
-template <int KIND, bool HAS_NEXT, bool HAS_NEXT2>
-__device__ __forceinline__ void epi_step(int g, uint32_t t_hi, uint32_t t_lo, const float (&pc)[8], uint32_t (&sn)[8], float (&pn)[8],
-                                         uint32_t (&sn2)[8], bool diag_tile, int cd) {
-  if (HAS_NEXT) {
-    tmem_wait_ld();                                      // sn = S columns of group g+1 has arrived
-    if (diag_tile) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        if (8 * (g + 1) + i == cd) sn[i] = 0u;           // a_ii = 0 exactly (kernel.py:44-45 fills the diagonal with 0)
-    }
-  }
-  if (HAS_NEXT2) GP_TMEM_LD8(t_hi + 8 * (g + 2), sn2);
-  if (HAS_NEXT) cov_group8<KIND>(sn, pn);
-  uint32_t hi[8], lo[4];
-  split_group8(pc, hi, lo);
-  GP_TMEM_ST8(t_hi + 8 * g, hi);
-  GP_TMEM_ST4(t_lo + 4 * g, lo);
+__device__ __forceinline__ float cov_tc(float a) {
+  // RBF: k = 2^a with NO clamp of a at 0: a = -0.5|z_i - z_j|^2 can only come out > 0 through rounding for (near-)duplicate
+  // points, where it is < 2e-6, i.e. k <= 1 + 1.4e-6 -- inside the stated entry tolerance.  The exact diagonal is forced to
+  // a = 0 in diagonal tiles.
+  return (KIND == GP_RBF) ? ex2_approx(a) : cov_from_arg<KIND>(a);
 }
 
 template <int KIND>
 __global__ void __launch_bounds__(TC_THREADS, 2)
 kmv_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const float* __restrict__ Vt,
               float* __restrict__ partial, int KP, int NS, int64_t ntile_j, int64_t tiles_per_split,
-              int64_t rows_pad, int same, int64_t row_begin, const int* __restrict__ done_flag, long long* __restrict__ trace) {
-  if (done_flag && *done_flag) return;  // CTA-uniform, before any barrier / TMEM state exists
-  // optional event trace of CTA (0,0): trace[tile][8] = {g1_issue, g2_issue, sfull_wait, sfull_done, c0_done, ofull_done, tile_end, -}
-  const bool tr = trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0;
-#define GP_TR(tile, ev) do { if (tr && lane == 0 && (tile) < 256) trace[(tile) * 8 + (ev)] = clock64(); } while (0)
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int warp = (int)warp_idx_uniform();
+              int64_t rows_pad, int same, int64_t row_begin, const int* __restrict__ done_flag) {
+  if (done_flag && *done_flag) return;  // CTA-uniform, before any barrier exists
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int64_t it = blockIdx.x;
   const int split = blockIdx.y;
@@ -131,7 +66,7 @@ kmv_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const 
 
   const uint32_t a_bytes = (uint32_t)KP * TILE_I * 4;
   const uint32_t b_bytes = (uint32_t)KP * TILE_J * 4;
-  const uint32_t stage_bytes = b_bytes + V_TILE_BYTES;
+  const uint32_t stage_bytes = b_bytes + V_TF32_BYTES;
   uint8_t* sA = smem;
   uint8_t* sStage = smem + a_bytes;
   TcBars* bars = reinterpret_cast<TcBars*>(smem + a_bytes + (size_t)NS * stage_bytes);
@@ -140,245 +75,153 @@ kmv_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const 
     mbar_init(smem_u32(&bars->a_full), 1);
     for (int s = 0; s < MAX_NS; ++s) {
       mbar_init(smem_u32(&bars->b_full[s]), 1);
-      mbar_init(smem_u32(&bars->b_empty[s]), 1);
+      mbar_init(smem_u32(&bars->b_empty[s]), 256);
     }
-    for (int s = 0; s < NSTG; ++s) mbar_init(smem_u32(&bars->s_full[s]), 1);
-    for (int i = 0; i < NSTG; ++i) mbar_init(smem_u32(&bars->p_full[i]), 128);
-    for (int i = 0; i < NO; ++i) mbar_init(smem_u32(&bars->o_full[i]), 1);
     fence_mbar_init();
   }
-  if (warp == W_MMA) tmem_alloc(smem_u32(&bars->tmem_base), TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
+  if (T == 0) return;
 
-  if (warp == W_PROD) {
-    // ===================== TMA producer (one lane) =====================
-    if (lane == 0 && T > 0) {
-      mbar_arrive_expect_tx(smem_u32(&bars->a_full), a_bytes);
-      bulk_g2s(smem_u32(sA), XA + it * (int64_t)TILE_I * KP, a_bytes, smem_u32(&bars->a_full));
-      int sb = 0;
-      uint32_t par = 1;
-      for (int u = 0; u < T; ++u) {
-        mbar_wait(smem_u32(&bars->b_empty[sb]), par);
-        const uint32_t full = smem_u32(&bars->b_full[sb]);
-        uint8_t* st = sStage + (size_t)sb * stage_bytes;
-        const int64_t jt = jt0 + u;
-        mbar_arrive_expect_tx(full, stage_bytes);
-        bulk_g2s(smem_u32(st), XB + jt * (int64_t)TILE_J * KP, b_bytes, full);
-        bulk_g2s(smem_u32(st + b_bytes), reinterpret_cast<const uint8_t*>(Vt) + jt * (int64_t)V_TILE_BYTES, V_TILE_BYTES, full);
-        if (++sb == NS) { sb = 0; par ^= 1; }
-      }
-    }
-  } else if (warp == W_MMA) {
-    // ===================== MMA issuer (converged warp, one elected lane issues each batch) ==========
-    // Program order per tile u:  wait P(u) -> GEMM2(u) -> GEMM1(u+2) into the slot GEMM2(u) has just read.  One thread
-    // issues both, so the tensor pipe orders them and no "slot drained" barrier is needed; GEMM1 runs one tile ahead of
-    // the epilogue, whose math overlaps GEMM2(u-1) + GEMM1(u+1).
-    if (T > 0) {
-      constexpr uint32_t IDESC1 = idesc_tf32(TILE_I, TILE_J);    // S = A B^T                       128 x 64
-      constexpr uint32_t IDESC2A = idesc_tf32(TILE_I, 2 * TP);   // O  = P_hi [V_hi;V_lo]^T  (tf32) 128 x 32
-      constexpr uint32_t IDESC2B = idesc_bf16(TILE_I, TP);       // O += P_lo V^T            (bf16) 128 x 16
-      const int ksteps1 = KP / 8;
-      const uint64_t a_desc0 = smem_desc(smem_u32(sA), TILE_I * 16, 128);
-      mbar_wait(smem_u32(&bars->a_full), 0);
-      int sb1 = 0;          // smem ring slot of the next GEMM1
-      uint32_t par1 = 0;
-      int g1 = 0;           // next tile GEMM1 produces
-      auto issue_g1 = [&]() {
-        const int slot = g1 % NSTG;
-        mbar_wait(smem_u32(&bars->b_full[sb1]), par1);
-        tc_fence_after();
-        GP_TR(g1, 0);
-        const uint64_t b_desc0 = smem_desc(smem_u32(sStage + (size_t)sb1 * stage_bytes), TILE_J * 16, 128);
-        const uint32_t d_s = tmem + (uint32_t)(slot * TILE_J);
-        const uint32_t sfull = smem_u32(&bars->s_full[slot]);
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < KP_MAX / 8; ++ks)  // fully unrolled + predicated: every operand stays in uniform registers
-            if (ks < ksteps1)
-              mma_tf32_ss_1t(d_s, a_desc0 + (uint64_t)(ks * ((2 * TILE_I * 16) >> 4)), b_desc0 + (uint64_t)(ks * ((2 * TILE_J * 16) >> 4)),
-                             IDESC1, ks > 0 ? 1u : 0u);
-          tc_commit_1t(sfull);
-        }
-        __syncwarp();
-        if (++sb1 == NS) { sb1 = 0; par1 ^= 1; }
-        ++g1;
-      };
-      issue_g1();
-      if (T > 1) issue_g1();
-      int sb2 = 0;
-      for (int u = 0; u < T; ++u) {
-        const int slot = u % NSTG;
-        mbar_wait(smem_u32(&bars->p_full[slot]), (uint32_t)((u / NSTG) & 1));
-        tc_fence_after();
-        GP_TR(u, 1);
-        const uint32_t v_addr = smem_u32(sStage + (size_t)sb2 * stage_bytes + b_bytes);
-        const uint64_t v_desc0 = smem_desc(v_addr, 2 * TP * 16, 128);                 // tf32 tile, 32 rows
-        const uint64_t w_desc0 = smem_desc(v_addr + V_TF32_BYTES, TP * 16, 128);      // bf16 tile, 16 rows
-        const uint32_t p_hi = tmem + (uint32_t)(slot * TILE_J);
-        const uint32_t p_lo = tmem + (uint32_t)(COL_LO + slot * (TILE_J / 2));
-        const uint32_t bempty = smem_u32(&bars->b_empty[sb2]), ofull = smem_u32(&bars->o_full[u % NO]);
-        const uint32_t d_o = tmem + (uint32_t)(COL_O + (u % NO) * 2 * TP);
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < TILE_J / 8; ++ks)
-            mma_tf32_ts_1t(d_o, p_hi + ks * 8, v_desc0 + (uint64_t)(ks * ((2 * 2 * TP * 16) >> 4)), IDESC2A, ks > 0 ? 1u : 0u);
-#pragma unroll
-          for (int ks = 0; ks < TILE_J / 16; ++ks)
-            mma_bf16_ts_1t(d_o, p_lo + ks * 8, w_desc0 + (uint64_t)(ks * ((2 * TP * 16) >> 4)), IDESC2B, 1u);
-          tc_commit_1t(bempty);   // smem slot (B + V) is free again
-          tc_commit_1t(ofull);    // O holds tile u's product
-        }
-        __syncwarp();
-        if (++sb2 == NS) sb2 = 0;
-        if (g1 < T) issue_g1();   // refill the TMEM slot GEMM2(u) has just consumed (same thread => ordered)
-      }
-    }
-  } else {
-    // ===================== epilogue warpgroups (warps 0-3: even tiles / slot 0, warps 4-7: odd tiles / slot 1) =========
-    const int wg = warp >> 2;
-    const int q = warp & 3;            // TMEM lane quadrant of this warp
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const int64_t gi = row_begin + it * TILE_I + q * 32 + lane;  // global row of this thread
-    const uint32_t t_o = tmem + lane_off + (uint32_t)COL_O;
-    // O is folded into fp32 registers after EVERY tile: the tensor core's accumulator truncates on each add, so long
-    // TMEM accumulation chains drift (1e-4 at N = 50k); 12 adds per tile keep the product at fp32 level.
-    float acc[TP];
-#pragma unroll
-    for (int c = 0; c < TP; ++c) acc[c] = 0.f;
-    for (int u = wg; u < T; u += 2) {
-      const int slot = wg;
-      if (q == 0) GP_TR(u, 2);
-      mbar_wait(smem_u32(&bars->s_full[slot]), (uint32_t)((u / NSTG) & 1));
-      tc_fence_after();
-      if (q == 0) GP_TR(u, 3);
-      const uint32_t t_s = tmem + lane_off + (uint32_t)(slot * TILE_J);   // S, overwritten in place by P_hi
-      const uint32_t t_lo = tmem + lane_off + (uint32_t)(COL_LO + slot * (TILE_J / 2));
-      const int64_t jbase = (jt0 + u) * TILE_J;
-      const bool diag_tile = same && (row_begin + it * TILE_I < jbase + TILE_J) && (jbase < row_begin + (it + 1) * TILE_I);
-      const int cd = (int)(gi - jbase);
-      uint32_t sa[8], sb[8];
-      float pa[8], pb[8];
-      GP_TMEM_LD8(t_s, sa);
-      GP_TMEM_LD8(t_s + 8, sb);
-      if (u >= 2) {
-        // fold O(u-2): its TMEM load rides with the first S loads and its adds are scheduled into the MUFU-bound steps.
-        // No o_full wait: s_full(u) was committed by the issuer thread AFTER it issued GEMM2(u-2), and tcgen05.commit tracks
-        // all prior MMAs of that thread.  O[u % 2] is next written by GEMM2(u), issued after this thread's arrive on
-        // p_full(u).  (Waiting for GEMM2(u-1) instead, issued only when THIS tile started, costs ~500 cycles.)
-        uint32_t o[32];
-        GP_TMEM_LD32(t_o + (uint32_t)((u % NO) * 2 * TP), o);
-        tmem_wait_ld();
-#pragma unroll
-        for (int c = 0; c < TP; ++c) acc[c] += __uint_as_float(o[c]) + __uint_as_float(o[TP + c]);
-      } else {
-        tmem_wait_ld();
-      }
-      if (diag_tile) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if (i == cd) sa[i] = 0u;
-      }
-      cov_group8<KIND>(sa, pa);                          // group 0 in pa; group 1's S in sb
-      if (q == 0) GP_TR(u, 4);
-#pragma unroll 1
-      for (int g = 0; g < 6; g += 2) {
-        epi_step<KIND, true, true>(g, t_s, t_lo, pa, sb, pb, sa, diag_tile, cd);      // MUFU g+1 -> pb, load g+2 -> sa, split g
-        epi_step<KIND, true, true>(g + 1, t_s, t_lo, pb, sa, pa, sb, diag_tile, cd);  // MUFU g+2 -> pa, load g+3 -> sb, split g+1
-      }
-      epi_step<KIND, true, false>(6, t_s, t_lo, pa, sb, pb, sa, diag_tile, cd);
-      epi_step<KIND, false, false>(7, t_s, t_lo, pb, sa, pa, sb, diag_tile, cd);
-      if (q == 0) GP_TR(u, 5);
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(smem_u32(&bars->p_full[slot]));  // GEMM2(u) may now read P (this slot); it accumulates into O[u % 2]
-      if (q == 0) GP_TR(u, 6);
-    }
-    {
-      const int w = ((T - 1 - wg) >= 0) ? (T - 1 - ((T - 1 - wg) & 1)) : -1;   // this warpgroup's last tile: still in TMEM
-      if (w >= 0) {
-        mbar_wait(smem_u32(&bars->o_full[wg]), (uint32_t)((w / NO) & 1));
-        tc_fence_after();
-        uint32_t o[32];
-        GP_TMEM_LD32(t_o + (uint32_t)(wg * 2 * TP), o);
-        tmem_wait_ld();
-#pragma unroll
-        for (int c = 0; c < TP; ++c) acc[c] += __uint_as_float(o[c]) + __uint_as_float(o[TP + c]);
-      }
-    }
-    // combine the two warpgroups' partial sums through smem.  The exchange buffer reuses ring slot 0, so the OTHER
-    // warpgroup's last GEMM2 (which may still be reading its B / V stage) must have completed too.
-    {
-      const int og = wg ^ 1;
-      const int wo = ((T - 1 - og) >= 0) ? (T - 1 - ((T - 1 - og) & 1)) : -1;
-      if (wo >= 0) mbar_wait(smem_u32(&bars->o_full[og]), (uint32_t)((wo / NO) & 1));
-    }
-    float* xch = reinterpret_cast<float*>(sStage);
-    const int rloc = q * 32 + lane;
-    if (wg == 1) {
-#pragma unroll
-      for (int c = 0; c < TP; ++c) xch[c * TILE_I + rloc] = acc[c];
-    }
-    named_bar_sync(1, 256);
-    if (wg == 0) {
-#pragma unroll
-      for (int c = 0; c < TP; ++c) acc[c] += xch[c * TILE_I + rloc];
-    }
-    if (wg == 0) {
-    const int64_t row = it * TILE_I + q * 32 + lane;
-    float4* dst = reinterpret_cast<float4*>(partial + ((int64_t)split * rows_pad + row) * TP);
-#pragma unroll
-    for (int qq = 0; qq < 4; ++qq) dst[qq] = make_float4(acc[4 * qq], acc[4 * qq + 1], acc[4 * qq + 2], acc[4 * qq + 3]);
-    }
+  // load tile u into ring stage u % NS (thread 0 only)
+  auto load_stage = [&](int u) {
+    const uint32_t full = smem_u32(&bars->b_full[u % NS]);
+    uint8_t* st = sStage + (size_t)(u % NS) * stage_bytes;
+    const int64_t jt = jt0 + u;
+    mbar_arrive_expect_tx(full, stage_bytes);
+    bulk_g2s(smem_u32(st), XB + jt * (int64_t)TILE_J * KP, b_bytes, full);
+    // only the tf32 part of the packed V tile: the products run in tf32 (P_lo is multiplied by V_hi)
+    bulk_g2s(smem_u32(st + b_bytes), reinterpret_cast<const uint8_t*>(Vt) + jt * (int64_t)V_TILE_BYTES, V_TF32_BYTES, full);
+  };
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(smem_u32(&bars->a_full), a_bytes);
+    bulk_g2s(smem_u32(sA), XA + it * (int64_t)TILE_I * KP, a_bytes, smem_u32(&bars->a_full));
+    for (int u = 0; u < NS && u < T; ++u) load_stage(u);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem, TMEM_COLS);
+
+  // accumulator fragment of wgmma m64nN (fp32): register i of thread (warp wq of the warpgroup, lane = 4 g + t) holds row
+  // 16 wq + g + 8 ((i >> 1) & 1) and column position 8 (i >> 2) + 2 t + (i & 1); with the XB column order of pack.cu the
+  // position 2 t + e of an 8-column group is column t + 4 e of the tile.
+  const int wg = warp >> 2;
+  const int wq = warp & 3;
+  const int g = lane >> 2, t = lane & 3;
+  const int64_t rloc0 = it * TILE_I + wg * 64 + wq * 16 + g;   // local (padded) rows rloc0 and rloc0 + 8 of this thread
+  const int64_t gi0 = row_begin + rloc0;
+  const uint64_t a_desc0 = gmma_desc(smem_u32(sA) + (uint32_t)wg * 8 * 128, TILE_I * 16, 128);
+  constexpr uint64_t A_KSTEP = (2 * TILE_I * 16) >> 4, B_KSTEP = (2 * TILE_J * 16) >> 4, V_KSTEP = (2 * 2 * TP * 16) >> 4;
+  const int ksteps1 = KP / 8;
+
+  float acc[8];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) acc[c] = 0.f;
+  mbar_wait(smem_u32(&bars->a_full), 0);
+  int sb = 0;
+  uint32_t par = 0;
+#pragma unroll 1
+  for (int u = 0; u < T; ++u) {
+    if (threadIdx.x == 0 && u >= 1 && u - 1 + NS < T) {
+      // stage (u - 1) % NS: released by both warpgroups after tile u - 1 (phase (u - 1) / NS of its empty barrier)
+      mbar_wait(smem_u32(&bars->b_empty[(u - 1) % NS]), (uint32_t)(((u - 1) / NS) & 1));
+      load_stage(u - 1 + NS);
+    }
+    mbar_wait(smem_u32(&bars->b_full[sb]), par);
+    const uint32_t st = smem_u32(sStage + (size_t)sb * stage_bytes);
+    const uint64_t b_desc0 = gmma_desc(st, TILE_J * 16, 128);
+    const uint64_t v_desc0 = gmma_desc(st + b_bytes, 2 * TP * 16, 128);   // rows 0-15 V_hi, 16-31 V_lo
+    float s[32];
+    fence_regs(s);
+    wgmma_fence();
+#pragma unroll 1
+    for (int ks = 0; ks < ksteps1; ++ks)
+      wgmma_m64n64k8_ss(s, a_desc0 + ks * A_KSTEP, b_desc0 + ks * B_KSTEP, ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_regs(s);
+
+    const int64_t jbase = (jt0 + u) * TILE_J;
+    const bool diag_tile = same && (gi0 - wq * 16 - g < jbase + TILE_J) && (jbase < gi0 - wq * 16 - g + 64);
+    if (diag_tile) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int64_t gi = gi0 + 8 * ((i >> 1) & 1);
+        const int64_t gj = jbase + 8 * (i >> 2) + t + 4 * (i & 1);
+        if (gi == gj) s[i] = 0.f;   // a_ii = 0 exactly (kernel.py:44-45 fills the diagonal with 0)
+      }
+    }
+    // P = cov(S) split into tf32 P_hi (in hi) and the fp32 residual P_lo (in place of S)
+    uint32_t hi[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float pv = cov_tc<KIND>(s[i]);
+      hi[i] = __float_as_uint(pv) & 0xFFFFE000u;
+      s[i] = pv - __uint_as_float(hi[i]);
+    }
+    float o1[16], o2[8];
+    fence_regs(s);
+    fence_regs(o1);
+    fence_regs(o2);
+    wgmma_fence();
+#pragma unroll
+    for (int jb = 0; jb < TILE_J / 8; ++jb)
+      wgmma_m64n32k8_rs(o1, hi[4 * jb], hi[4 * jb + 2], hi[4 * jb + 1], hi[4 * jb + 3], v_desc0 + jb * V_KSTEP, jb > 0 ? 1u : 0u);
+#pragma unroll
+    for (int jb = 0; jb < TILE_J / 8; ++jb)
+      wgmma_m64n16k8_rs(o2, __float_as_uint(s[4 * jb]), __float_as_uint(s[4 * jb + 2]), __float_as_uint(s[4 * jb + 1]),
+                        __float_as_uint(s[4 * jb + 3]), v_desc0 + jb * V_KSTEP, jb > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_regs(o1);
+    fence_regs(o2);
+    mbar_arrive(smem_u32(&bars->b_empty[sb]));   // this thread's share of the stage has been read
+    if (++sb == NS) { sb = 0; par ^= 1; }
+    // O is folded into fp32 registers after every tile: long accumulation chains inside the tensor core drift
+#pragma unroll
+    for (int c = 0; c < 8; ++c) acc[c] += o1[c] + o1[c + 8] + o2[c];
+  }
+  // columns 2 t, 2 t + 1 (c even) and 8 + 2 t, 9 + 2 t of rows rloc0 (c & 2 == 0) and rloc0 + 8
+#pragma unroll
+  for (int c = 0; c < 8; c += 2) {
+    const int64_t row = rloc0 + 8 * ((c >> 1) & 1);
+    float2* dst = reinterpret_cast<float2*>(partial + ((int64_t)split * rows_pad + row) * TP + 8 * (c >> 2) + 2 * t);
+    *dst = make_float2(acc[c], acc[c + 1]);
   }
 }
 
 static int tc_smem_bytes(int KP, int* ns_out) {
   const int a_bytes = KP * TILE_I * 4;
-  const int stage = KP * TILE_J * 4 + V_TILE_BYTES;
-  // preferred: two CTAs per SM (<= ~112 KB each); wide feature vectors fall back to one CTA per SM
+  const int stage = KP * TILE_J * 4 + V_TF32_BYTES;
+  // preferred: two CTAs per SM (<= ~113 KB each of the 228 KB); wide feature vectors fall back to one CTA per SM
   int budget = 112 * 1024 - a_bytes - (int)sizeof(TcBars) - 1024;
   int ns = budget / stage;
   if (ns < 3) {
-    budget = 220 * 1024 - a_bytes - (int)sizeof(TcBars) - 1024;
+    budget = 226 * 1024 - a_bytes - (int)sizeof(TcBars) - 1024;
     ns = budget / stage;
   }
   if (ns > MAX_NS) ns = MAX_NS;
   *ns_out = ns;
-  return a_bytes + ns * stage + (int)sizeof(TcBars) + 64;
+  return a_bytes + ns * stage + (int)sizeof(TcBars);
 }
 
 template <int KIND>
 static int launch_tc_kind(gp_plan* p, const int* done_flag) {
   int ns = 0;
   int smem_bytes = tc_smem_bytes(p->KP, &ns);
-  GP_REQUIRE(ns >= 3, GP_E_SHAPE, "tcgen05 path: smem ring too small for KP=%d", p->KP);
+  GP_REQUIRE(ns >= 2, GP_E_SHAPE, "tensor-core path: smem ring too small for KP=%d", p->KP);
   static bool attr_done[64] = {};   // function attributes are per device
   const int dev_slot = p->device & 63;
   if (!attr_done[dev_slot]) {
     GP_CUDA(cudaFuncSetAttribute(kmv_tc_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_done[dev_slot] = true;
   }
-  int64_t rows_pad = p->rows_pad;
   dim3 grid((unsigned)p->ntile_i, (unsigned)p->nsplit);
   kmv_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
       p->XA.as<float>(), p->XB.as<float>(), vtiles_ptr(p), partial_ptr(p), p->KP, ns, p->ntile_j,
-      p->tiles_per_split, rows_pad, p->same ? 1 : 0, p->row_begin, done_flag, p->tc_trace);
+      p->tiles_per_split, p->rows_pad, p->same ? 1 : 0, p->row_begin, done_flag);
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
 
 int kmv_tc_launch_kind(gp_plan* p, int kind, const int* done_flag) {
-  if (p->tc2) return kmv_tc2_launch_kind(p, kind, done_flag);
   switch (kind) {
     case GP_RBF: return launch_tc_kind<GP_RBF>(p, done_flag);
     case GP_MATERN12: return launch_tc_kind<GP_MATERN12>(p, done_flag);

@@ -8,9 +8,11 @@
 // HBM layouts produced here
 //   Z2   [n2][DP]            fp32, zero padded features           (SIMT kernel, row extraction)
 //   Z1   [n1_local][DP]      only when X2 != X1 (otherwise Z1 aliases Z2 + row_begin*DP)
-//   XA   [ntile_i][KP/4][128][4]   UMMA K-major no-swizzle tiles of the A operand
+//   XA   [ntile_i][KP/4][128][4]   wgmma K-major no-swizzle tiles of the A operand
 //                                  [z_hi | z_lo | z_hi | n_hi n_lo 1 1 | 0..]   (3xTF32 split)
-//   XB   [ntile_j][KP/4][ 64][4]   B operand  [z_hi | z_hi | z_lo | 1 1 n_hi n_lo | 0..]
+//   XB   [ntile_j][KP/4][ 64][4]   B operand  [z_hi | z_hi | z_lo | 1 1 n_hi n_lo | 0..], the columns of every 8-column
+//                                  group stored in the order 0 4 1 5 2 6 3 7 (kmv_tc.cu: the GEMM1 accumulator is then the
+//                                  tf32 A fragment of GEMM2)
 //   so that  sum_k A_ik B_jk = z_i.z_j (to ~2^-22) + n_i + n_j,  n = -0.5 |z|^2  = a_ij.
 //   Vt   per 64-row tile: [64/4][32][4] tf32 (rows 0-15 hi, 16-31 lo) + [64/8][16][8] bf16  (B operands of GEMM2)
 #include <stdlib.h>
@@ -55,6 +57,7 @@ __global__ void pack_tc_kernel(const float* __restrict__ Z, int64_t row0, int64_
   if (r >= nrows_pad) return;
   int64_t tile = r / tile_rows;
   int rr = (int)(r % tile_rows);
+  if (!IS_A) rr = (rr & ~7) | ((rr & 4) ? 2 * (rr & 3) + 1 : 2 * (rr & 3));   // column c of a group -> position 2 (c % 4) + c / 4
   float4* dst = reinterpret_cast<float4*>(out + tile * (int64_t)tile_rows * KP);
   const bool valid = r < nrows_valid;
   const float* z = Z + (row0 + r) * DP;
@@ -147,21 +150,13 @@ int choose_geometry(gp_plan* p) {
   int want = p->backend_req;
   if (want == GP_BACKEND_AUTO) want = (p->KP <= KP_MAX) ? GP_BACKEND_TCGEN05 : GP_BACKEND_SIMT;
   GP_REQUIRE(!(want == GP_BACKEND_TCGEN05 && p->KP > KP_MAX), GP_E_SHAPE,
-             "tcgen05 backend needs 3d+4 <= %d (d=%d)", KP_MAX, p->d);
+             "tcgen05 (tensor-core) backend needs 3d+4 <= %d (d=%d)", KP_MAX, p->d);
   p->backend = want;
   p->rows_pad = cdiv(p->row_count, 2 * TILE_I) * 2 * TILE_I;
   p->ntile_i = p->rows_pad / TILE_I;
   p->ntile_j = cdiv(p->n2, TILE_J);
-  p->tc2 = p->backend == GP_BACKEND_TCGEN05 && p->KP <= 64 && getenv("GP_KMV_V1") == nullptr;
-  {
-    // share of the ex2 evaluations on the FMA pipe (of 8): measured best at C2 / C3 shapes (profiles/NOTES_r02.md): RBF is bound by
-    // the issuer <-> epilogue hand-off, not by the MUFU, so the polynomial only adds issue slots; Matern (sqrt + ex2 per entry) gains
-    const char* e = getenv("GP_NPOLY");
-    p->npoly = e ? atoi(e) : (p->kind == GP_RBF ? 0 : 2);
-    if (p->npoly != 0 && p->npoly != 2 && p->npoly != 4) p->npoly = 0;
-  }
   // column splits: pick the smallest nsplit whose unit count fills the SMs best
-  int64_t nti = (p->backend == GP_BACKEND_TCGEN05) ? (p->tc2 ? p->rows_pad / (2 * TILE_I) : p->ntile_i) : cdiv(p->row_count, SIMT_TI);
+  int64_t nti = (p->backend == GP_BACKEND_TCGEN05) ? p->ntile_i : cdiv(p->row_count, SIMT_TI);
   int64_t ntj = (p->backend == GP_BACKEND_TCGEN05) ? p->ntile_j : cdiv(p->n2, SIMT_TJ);
   int best = 1;
   double best_eff = -1.0;
@@ -170,7 +165,7 @@ int choose_geometry(gp_plan* p) {
     int64_t per = cdiv(ntj, s);
     if (s > 1 && per < 8) break;  // keep units long enough to amortise the prologue
     int64_t units = nti * s;
-    const int64_t slots = (int64_t)p->n_sm * ((p->backend == GP_BACKEND_TCGEN05 && !p->tc2) ? 2 : 1);  // resident CTAs
+    const int64_t slots = (int64_t)p->n_sm * (p->backend == GP_BACKEND_TCGEN05 ? 2 : 1);  // resident CTAs
     int64_t waves = cdiv(units, slots);
     double eff = (double)(nti * ntj) / (double)(waves * slots * per);
     if (eff > best_eff + 0.02) { best_eff = eff; best = s; }

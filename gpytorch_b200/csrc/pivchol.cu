@@ -167,7 +167,7 @@ __device__ __forceinline__ void pc_grid_barrier(unsigned int* bar, unsigned int 
   __syncthreads();
 }
 
-constexpr int PCP_THREADS = 384;  // persistent kernel: one CTA per SM keeps the grid barrier small (148 arrivals)
+constexpr int PCP_THREADS = 384;  // persistent kernel: one CTA per SM keeps the grid barrier small (one arrival per SM)
 constexpr int PCP_RED = 512;
 
 // Persistent kernel with ONE grid barrier per step.  Every CTA reduces the per-CTA partials itself (same loads, same tree => the

@@ -361,7 +361,7 @@ ski_gather_tiled_kernel(const int* __restrict__ first_s, const float* __restrict
 // fp32-level accuracy at a small multiple of the tf32 rate, so the pass is bound by streaming the grid block, not by FMAs
 // (the fp32 CUDA-core version of this kernel took 249 us per pass at G = 100, M = 10^6: 13 TFLOP/s).  Warp-level
 // mma.sync.m16n8k8 is the right tool for these skinny products (M = G <= 128 rows, one 64-column slab per CTA step): there is
-// no accumulator reuse across slabs for a tcgen05 / TMEM pipeline to amortise.
+// no accumulator reuse across slabs for an asynchronous wgmma pipeline to amortise.
 constexpr int SKI_MT = 64;          // slab width (positions)
 constexpr int SKI_BP = SKI_MT + 8;  // pitch of the staged slab: 72 = 8 mod 32 -> conflict-free B fragments
 __device__ __forceinline__ uint32_t tf32_rna(float x) {

@@ -1,5 +1,5 @@
-// tc_ptx.cuh -- thin inline-PTX wrappers for sm_100a: mbarrier, bulk TMA (cp.async.bulk),
-// tcgen05 alloc / mma / commit / ld / st / fences, UMMA shared-memory + instruction descriptors.
+// tc_ptx.cuh -- thin inline-PTX wrappers for sm_90a: mbarrier, bulk TMA (cp.async.bulk), wgmma (warpgroup MMA) and its
+// shared-memory matrix descriptor.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,42 +31,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// bounded wait: a protocol bug traps (context error) instead of hanging the GPU box.
+// bounded wait: a protocol bug traps (context error) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > 8000000000LL) __trap();
   }
-}
-
-// polling wait (no hardware suspend): for the MMA issuer, whose wake-up latency is on the critical path of every tile
-// (try_wait parks the thread and took 200-300 cycles to notice a completed phase; profiles/NOTES_r02.md)
-__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_poll(uint32_t bar, uint32_t parity) {
-  if (mbar_test_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_test_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) __trap();
-  }
-}
-
-// ---- named barriers (bar.sync / bar.arrive on ids 1..15; id 0 is __syncthreads) --------------
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // ---- bulk TMA: contiguous global -> shared, completion on an mbarrier (SASS: UBLKCP) -------
@@ -76,180 +47,64 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src_gmem
                : "memory");
 }
 
-// ---- tcgen05 ------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {  // converged warp; one elected lane commits
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar)
-      : "memory");
-}
-// All tcgen05 issue wrappers below are meant to be executed by a fully converged warp with warp-uniform
-// operands; exactly one elected lane issues (elect.sync), so ptxas keeps descriptors in uniform registers
-// and emits a bare UTCHMMA instead of a per-lane R2UR election loop.
-__device__ __forceinline__ uint32_t warp_idx_uniform() { return __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0); }
-
-// returns true in exactly one lane of a converged warp (cute::elect_one_sync)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, q;\n\t}"
-      : "=r"(pred)::"memory");
-  return pred != 0;
-}
-// single-thread issue forms: call ONLY from inside `if (elect_one()) { ... }` of a converged warp
-__device__ __forceinline__ void mma_tf32_ss_1t(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_tf32_ts_1t(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem, bf16 packed 2/column] * B[smem desc, bf16]^T   (kind::f16, fp32 accumulate)
-__device__ __forceinline__ void mma_bf16_ts_1t(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_1t(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, tf32 inputs, fp32 accumulate
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]^T
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// K-major, no-swizzle ("interleave") operand: 8-row x 16-byte core matrices;
-// lbo = byte stride between the two 16 B K-chunks of one K=8 (tf32) step,
-// sbo = byte stride between successive 8-row groups.  (cute::UMMA::SmemDescriptor, version 1)
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// ---- wgmma --------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major, no-swizzle ("interleave") operand: 8-row x 16-byte core matrices;
+// lbo = byte stride between the two 16 B K-chunks of one K = 8 (tf32) step, sbo = byte stride between successive 8-row
+// groups.  Layout type 0 (no swizzle) and base offset 0 in bits 49-51 / 62-63.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// instruction descriptor: fp32 accumulate, tf32 x tf32, both K-major, M x N
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving reads / writes of an accumulator register across a wgmma fence / wait
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
-// instruction descriptor: fp32 accumulate, bf16 x bf16, both K-major, M x N (K = 16 per instruction)
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// D[64 x 64] (+)= A[smem desc, 64 x 8 tf32] * B[smem desc, 64 x 8 tf32]^T   (fp32 accumulate; D: 32 registers per thread)
+__device__ __forceinline__ void wgmma_m64n64k8_ss(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
-// {upper, lower} = {bf16(hi_elem), bf16(lo_elem)}: the LOWER half is the even (lower-k) element of a packed TMEM column
-// (a0, a1) - (b0, b1) as ONE packed fp32x2 instruction (FADD2, sm_100)
-__device__ __forceinline__ void sub_f32x2(float a0, float a1, float b0, float b1, float& d0, float& d1) {
-  uint64_t a, b, d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(a0), "f"(a1));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(b) : "f"(b0), "f"(b1));
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(d));
+// D[64 x 32] (+)= A[registers, 64 x 8 tf32] * B[smem desc, 32 x 8 tf32]^T   (D: 16 registers per thread)
+__device__ __forceinline__ void wgmma_m64n32k8_rs(float (&d)[16], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc,
+                                                  uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(accumulate));
 }
-__device__ __forceinline__ uint32_t pack_bf16x2(float lower, float upper) {
-  uint32_t d;
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(upper), "f"(lower));
-  return d;
+// D[64 x 16] (+)= A[registers, 64 x 8 tf32] * B[smem desc, 16 x 8 tf32]^T   (D: 8 registers per thread)
+__device__ __forceinline__ void wgmma_m64n16k8_rs(float (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc,
+                                                  uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(accumulate));
 }
-
-#define GP_TMEM_ST16(taddr, r)                                                                                        \
-  asm volatile(                                                                                                       \
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "                                                                 \
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),                        \
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),   \
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])                                          \
-      : "memory")
-
-#define GP_TMEM_LD32(taddr, r)                                                                                        \
-  asm volatile(                                                                                                       \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                       \
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                       \
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"                       \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),   \
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),        \
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),       \
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])                     \
-      : "r"(taddr)                                                                                                    \
-      : "memory")
-
-#define GP_TMEM_ST32(taddr, r)                                                                                        \
-  asm volatile(                                                                                                       \
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "                                                                 \
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "                                      \
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),                \
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),   \
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),     \
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),     \
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])                                                                  \
-      : "memory")
-
-#define GP_TMEM_LD16(taddr, r)                                                                                        \
-  asm volatile(                                                                                                       \
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                                                       \
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"                                \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),   \
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])                      \
-      : "r"(taddr)                                                                                                    \
-      : "memory")
-
-#define GP_TMEM_LD8(taddr, r)                                                                                         \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"                          \
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])           \
-               : "r"(taddr)                                                                                              \
-               : "memory")
-#define GP_TMEM_ST8(taddr, r)                                                                                         \
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),  \
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])                               \
-               : "memory")
-#define GP_TMEM_ST4(taddr, r)                                                                                         \
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),       \
-               "r"(r[2]), "r"(r[3])                                                                                      \
-               : "memory")
-
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 }  // namespace ptx
 }  // namespace gp

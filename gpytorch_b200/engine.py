@@ -18,7 +18,7 @@ def _require_cuda_f32(t: torch.Tensor, name: str):
     if not t.is_cuda:
         raise RuntimeError(f"{name} must live on a CUDA device: gpytorch_b200 has no CPU path")
     if t.dtype != torch.float32:
-        raise RuntimeError(f"{name} must be float32 (got {t.dtype}); the sm_100a engine computes in fp32/3xTF32")
+        raise RuntimeError(f"{name} must be float32 (got {t.dtype}); the sm_90a engine computes in fp32/3xTF32")
 
 
 @dataclass

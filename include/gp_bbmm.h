@@ -1,5 +1,5 @@
 /*
- * gp_bbmm.h -- C ABI of the B200-native BBMM exact-GP engine (libgpbbmm.so).
+ * gp_bbmm.h -- C ABI of the H100-native BBMM exact-GP engine (libgpbbmm.so).
  *
  * Drop-in boundary for ONE hot path of cornellius-gp/gpytorch: the mBCG / SLQ evaluation of
  * the exact-GP marginal log likelihood.  Plain pointers and sizes only; no torch types.
@@ -43,7 +43,8 @@ enum {
 /* covariance function kinds: kernels/rbf_kernel.py:68-85, kernels/matern_kernel.py:85-110 */
 enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3 };
 
-/* which fused K.V kernel runs: GP_BACKEND_TCGEN05 = tcgen05/TMEM/bulk-TMA 3xTF32 kernel,
+/* which fused K.V kernel runs: GP_BACKEND_TCGEN05 = wgmma/bulk-TMA 3xTF32 tensor-core kernel
+ * (the name is historical),
  * GP_BACKEND_SIMT = fp32 CUDA-core kernel (bring-up / cross-check / d > 41). */
 enum { GP_BACKEND_AUTO = 0, GP_BACKEND_TCGEN05 = 1, GP_BACKEND_SIMT = 2, GP_BACKEND_SKI = 3 /* set by gp_plan_set_ski */,
        GP_BACKEND_SUM = 4 /* set by gp_plan_set_sum */ };
@@ -194,9 +195,6 @@ int64_t gp_kernel_launches(gp_plan* plan);               /* kernels launched by 
 int gp_plan_info(gp_plan* plan, int* backend, int* nsplit, int* kpad, int* n_sm);
 /* Times `reps` back-to-back launches of the fused K.V kernel ALONE (after `warmup` untimed ones) with CUDA
  * events on the plan's stream; V [n2, t].  *ms_per_launch is the average device time of one launch. */
-/* Debug: device buffer of 256*8 int64 receiving clock64() stamps of the tcgen05 pipeline events of CTA (0,0)
- * (NULL disables).  Used by tools/tc_trace.py to study pipeline bubbles. */
-int gp_plan_set_trace(gp_plan* plan, long long* trace);
 int gp_time_kmv_kernel(gp_plan* plan, const float* V, int64_t ldv, int t, int warmup, int reps, float* ms_per_launch);
 
 #ifdef __cplusplus

@@ -40,7 +40,7 @@ def test_every_declared_symbol_is_exported_and_bound():
         assert s in syms, f"{s} bound but not declared in the header"
 
 
-def test_sass_is_blackwell_native():
+def test_sass_is_hopper_native():
     import shutil, subprocess
 
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
@@ -48,8 +48,8 @@ def test_sass_is_blackwell_native():
         pytest.skip("cuobjdump not available")
     obj = os.path.join(ROOT, "gpytorch_b200", "build", "kmv_tc.o")
     sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "LDTM", "STTM", "UBLKCP", "MUFU.EX2"):
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "WARPGROUP.ARRIVE", "UBLKCP", "SYNCS.ARRIVE", "MUFU.EX2"):
         assert mnemonic in sass, f"{mnemonic} missing from the fused K.V kernel"
 
 

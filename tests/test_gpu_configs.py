@@ -1,9 +1,9 @@
-"""GPU parity at the REAL configurations (run with -m gpu on a B200).
+"""GPU parity at the REAL configurations (run with -m gpu on an H100).
 
 * C2 at full size (N = 50 000, d = 10, RBF, rank-100 preconditioner): the whole MLL evaluation against the oracle run in
   the reference's default dtype (fp32) on identical inputs and probe base samples -- size-dependent paths (nsplit = 3, 391
   row tiles / 782 column tiles, ring wrap-around) are only exercised here.
-* C3-shaped (Matern-5/2, d = 20 => KP = 64, the widest-feature regime of the tcgen05 kernel), multi-tile, ragged N: K.V and the
+* C3-shaped (Matern-5/2, d = 20 => KP = 64, three shared-memory stages in the tensor-core kernel), multi-tile, ragged N: K.V and the
   MLL against the fp64 oracle, both backends.
 * third-party anchors that are NOT this repository's restatement: scikit-learn's GaussianProcessRegressor log marginal
   likelihood (dense Cholesky) and scipy.sparse.linalg.cg.

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path through the C ABI vs the CPU oracle on the same
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C ABI vs the CPU oracle on the same
 seeded inputs, vs the committed golden vectors (outputs of the reference's own code), and -- at the BASELINE
 C2 size -- through size-independent properties (linearity, symmetry, row extraction, noise shift).
 
