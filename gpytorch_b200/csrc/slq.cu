@@ -16,10 +16,18 @@ __global__ void slq_kernel(const float* __restrict__ TMAT, int n_tridiag, int ld
   if (i >= n_tridiag) return;
   const float* T = TMAT + (size_t)i * ldt * ldt;
   double d[SLQ_JMAX], e[SLQ_JMAX], z[SLQ_JMAX];
+  bool finite = true;
   for (int a = 0; a < J; ++a) {
     d[a] = (double)T[(size_t)a * ldt + a];
     e[a] = (a + 1 < J) ? (double)T[(size_t)(a + 1) * ldt + a] : 0.0;
     z[a] = (a == 0) ? 1.0 : 0.0;
+    finite = finite && isfinite(d[a]) && isfinite(e[a]);
+  }
+  // A NaN / Inf entry would not stop the QL sweeps (fabs(NaN) <= x is false) and the mask below would then drop every NaN
+  // eigenvalue, turning the probe's term into a silent 0.  The reference gets NaN (eigh of a non-finite T), so write NaN.
+  if (!finite) {
+    out_per_probe[i] = __longlong_as_double(0x7ff8000000000000LL);
+    return;
   }
   const int n = J;
   for (int l = 0; l < n; ++l) {
@@ -82,7 +90,7 @@ extern "C" int gp_slq_logdet(gp_plan* p, const float* TMAT, int n_tridiag, int l
   GP_CUDA(cudaStreamSynchronize(p->stream));
   double s = 0.0;
   for (int i = 0; i < n_tridiag; ++i) s += h[i];
-  *logdet_out = s;  // NaN tridiagonals propagate to a NaN log-det, as in InvQuadLogdet.forward
+  *logdet_out = s;  // a probe whose leading block holds a NaN / Inf wrote NaN: the log-det is NaN, as in InvQuadLogdet.forward
   if (*reinterpret_cast<int*>(h + 64)) {
     set_error("tridiagonal eigen-solver (implicit QL) did not converge within 100 sweeps for at least one probe; the SLQ log-determinant is unreliable");
     return GP_W_EIG_NOT_CONVERGED;

@@ -145,7 +145,9 @@ def test_rows_diag_and_getitem(Plan, cuda_dev):
 # ---------------------------------------------------------------------------------------------------------
 # solver seam
 # ---------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("n,d,kind,ls,rank", [(1000, 3, "rbf", 0.5, 15), (3000, 10, "rbf", 1.0, 100), (2000, 4, "matern52", 0.7, 50)])
+@pytest.mark.parametrize("n,d,kind,ls,rank", [(1000, 3, "rbf", 0.5, 15), (3000, 10, "rbf", 1.0, 100), (2000, 4, "matern52", 0.7, 50),
+                                              (1500, 8, "matern32", 0.8, 64), (1500, 8, "matern32", 0.8, 65),
+                                              (4097, 10, "rbf", 1.0, 128)])
 def test_pivoted_cholesky_bit_exact_pivots_and_preconditioner(Plan, cuda_dev, n, d, kind, ls, rank):
     x, y = om.synthetic_problem(n, d, 0, torch.float64)
     K = ok.kernel_matrix(kind, x, x, ls, 1.0, True)
