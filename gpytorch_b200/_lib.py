@@ -28,6 +28,11 @@ class NanError(RuntimeError):
     """Mirror of gpytorch.utils.errors.NanError (utils/errors.py:8-22)."""
 
 
+class NotPSDError(RuntimeError):
+    """Mirror of linear_operator.utils.errors.NotPSDError (re-exported by gpytorch/utils/errors.py): a Cholesky factorisation
+    failed even after adding jitter to the diagonal."""
+
+
 class MllOpts(C.Structure):
     _fields_ = [
         ("num_probes", C.c_int),
@@ -79,6 +84,8 @@ PROTOTYPES = {
     "gp_mbcg": (_I, [_P, _P, _L, _I, _I, _F, _I, _I, _P, _I, _P, _L, _P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_F)]),
     "gp_slq_logdet": (_I, [_P, _P, _I, _I, _I, _L, C.POINTER(C.c_double)]),
     "gp_lanczos": (_I, [_P, _P, _I, _F, _P, _P, C.POINTER(_I)]),
+    "gp_ciq_sqrt_matmul": (_I, [_P, _P, _L, _I, C.POINTER(C.c_double), C.POINTER(C.c_double), _I, _F, _I, _P, _L,
+                                C.POINTER(_I), C.POINTER(_F)]),
     "gp_mll": (_I, [_P, _P, _P, _P, _P, C.POINTER(MllOpts), _P, C.POINTER(MllResult)]),
     "gp_comm_unique_id": (_I, [C.POINTER(C.c_uint8)]),
     "gp_comm_init": (_I, [C.POINTER(_P), C.POINTER(C.c_uint8), _I, _I]),

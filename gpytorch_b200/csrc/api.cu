@@ -106,7 +106,7 @@ extern "C" int gp_plan_destroy(gp_plan* p) {
   gp::DevBuf* bufs[] = {&p->mean, &p->scale, &p->Z1, &p->Z2, &p->XA, &p->XB, &p->V16, &p->Vtiles, &p->partial, &p->out16,
                         &p->cgU, &p->cgR, &p->cgZ, &p->cgP, &p->cgV, &p->cgPfull, &p->red, &p->sums, &p->qtr, &p->state,
                         &p->tmat_tmp, &p->misc, &p->misc2, &p->misc3, &p->pcdiag, &p->pcperm, &p->pcpos, &p->pcstate,
-                        &p->pcpart, &p->gram, &p->cholC, &p->part_scale};
+                        &p->pcpart, &p->gram, &p->cholC, &p->part_scale, &p->msw};
   for (auto* b : bufs) b->release();
   if (p->ski) {
     gp::DevBuf* sb[] = {&p->ski->first, &p->ski->wts, &p->ski->gridA, &p->ski->gridB, &p->ski->gridC, &p->ski->gridD, &p->ski->T, &p->ski->dT, &p->ski->flag,

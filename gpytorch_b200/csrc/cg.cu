@@ -557,6 +557,14 @@ __global__ void cg_finalize_kernel(const float* __restrict__ U, const CgState* _
   if (c < t) S[r * lds + c] = U[idx] * st->rhs_norm[c];
 }
 
+// the two reductions above, for the multi-shift MINRES loop (minres.cu)
+void cg_sum_launch(const float* in, int G, int L, double* out, const int* done, cudaStream_t st) {
+  cg_sum_kernel<<<(unsigned)cdiv(L, 32), 32 * SUM_GROUPS, 0, st>>>(in, G, L, out, done);
+}
+void cg_rhs_sq_launch(const float* RHS, int64_t ldr, int t, int64_t n, float* part, int G, cudaStream_t st) {
+  cg_rhs_sq_kernel<<<G, CG_THREADS, 0, st>>>(RHS, ldr, t, n, part);
+}
+
 static int allreduce(gp_plan* p, double* buf, size_t count) {
   if (p->comm && p->comm->world > 1) return nccl_allreduce_double(p->comm, buf, count, p->stream);
   return GP_OK;

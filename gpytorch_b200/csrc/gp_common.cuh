@@ -143,6 +143,7 @@ struct gp_plan {
   gp::DevBuf mean, scale, Z1, Z2, XA, XB, V16, Vtiles, partial, out16;
   gp::DevBuf cgU, cgR, cgZ, cgP, cgV, cgPfull, red, sums, qtr, state, tmat_tmp, misc, misc2, misc3;
   gp::DevBuf pcdiag, pcperm, pcpos, pcstate, pcpart, gram, cholC;
+  gp::DevBuf msw;   // multi-shift MINRES: Lanczos / direction blocks, partials, scalar state (minres.cu)
   gp_comm* comm = nullptr;
   gp_ski_state* ski = nullptr;   // non-null: backend == GP_BACKEND_SKI
   // kernel sums (GP_BACKEND_SUM): the terms (caller-owned plans over the same rows); while the parent launches a term's K.V

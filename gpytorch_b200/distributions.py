@@ -1,8 +1,9 @@
-"""MultivariateNormal with a lazy covariance (gpytorch/distributions/multivariate_normal.py:44-64, :221-252)."""
+"""MultivariateNormal with a lazy covariance (gpytorch/distributions/multivariate_normal.py:44-64, :221-252, :254-337)."""
 import math
 
 import torch
 
+from .sampling import psd_safe_cholesky
 
 
 class MultivariateNormal:
@@ -47,3 +48,46 @@ class MultivariateNormal:
             covar = covar.evaluate_kernel()
             inv_quad, logdet = covar.inv_quad_logdet(inv_quad_rhs=diff.unsqueeze(-1), logdet=True)
         return -0.5 * sum([inv_quad, logdet, diff.size(-1) * math.log(2 * math.pi)])
+
+    def _root(self):
+        """A root L with L L^T = covariance: the psd-safe Cholesky factor of a dense covariance (every posterior ExactGP returns),
+        the operator's root_decomposition otherwise."""
+        c = self._covar
+        return psd_safe_cholesky(c) if torch.is_tensor(c) else c.root_decomposition().root
+
+    def rsample(self, sample_shape=torch.Size(), base_samples=None):
+        """sample_shape x batch_shape x N reparameterised samples mean + L eps (multivariate_normal.py:254-320).
+
+        Gradients reach the mean always, and a dense covariance tensor through torch's Cholesky.  Samples of an engine operator
+        (Cholesky / Lanczos root of the operator, or CIQ with settings.ciq_samples) are detached from its hyper-parameters."""
+        sample_shape = torch.Size(sample_shape)
+        covar = self._covar
+        if base_samples is None:
+            num_samples = sample_shape.numel() or 1
+            if torch.is_tensor(covar):
+                root = psd_safe_cholesky(covar)
+                eps = torch.randn(*root.shape[:-1], num_samples, device=root.device, dtype=root.dtype)
+                res = (root @ eps).permute(-1, *range(root.dim() - 2), root.dim() - 2)
+            else:
+                res = covar.zero_mean_mvn_samples(num_samples)
+            res = res + self.loc.unsqueeze(0)
+            return res.reshape(sample_shape + self.loc.shape)
+
+        covar_root = self._root()
+        if self.loc.shape != base_samples.shape[-self.loc.dim():] and covar_root.shape[-1] < base_samples.shape[-1]:
+            raise RuntimeError(
+                "The size of base_samples (minus sample shape dimensions) should agree with the size "
+                "of self.loc. Expected ...{} but got {}".format(self.loc.shape, base_samples.shape))
+        sample_shape = base_samples.shape[: base_samples.dim() - self.loc.dim()]
+        base_samples = base_samples.reshape(-1, *self.loc.shape)
+        base_samples = base_samples.permute(*range(1, self.loc.dim() + 1), 0)
+        if covar_root.shape[-1] < base_samples.shape[-2]:          # a low-rank root uses the leading base samples
+            base_samples = base_samples[..., : covar_root.shape[-1], :]
+        res = covar_root.matmul(base_samples.to(covar_root.dtype)) + self.loc.unsqueeze(-1)
+        res = res.permute(-1, *range(self.loc.dim())).contiguous()
+        return res.reshape(sample_shape + self.loc.shape)
+
+    def sample(self, sample_shape=torch.Size(), base_samples=None):
+        """rsample without gradients (multivariate_normal.py:322-337)."""
+        with torch.no_grad():
+            return self.rsample(sample_shape=sample_shape, base_samples=base_samples)

@@ -29,6 +29,13 @@ class MbcgInfo:
     status: int
 
 
+@dataclass
+class CiqInfo:
+    iters: int
+    residual_norms: list      # [Q][t]: final |phibar| / |b_c| per shift and column
+    status: int
+
+
 class Plan:
     """Owns a gp_plan: inputs, hyper-parameters and workspaces for one covariance operator K(X1, X2)."""
 
@@ -238,6 +245,30 @@ class Plan:
         j = C.c_int()
         check(self.lib.gp_lanczos(self._h, _ptr(init), int(max_iter), float(tol), _ptr(qt), _ptr(tm), C.byref(j)))
         return qt[: j.value].t(), tm[: j.value, : j.value]
+
+    def ciq_sqrt_matmul(self, b: torch.Tensor, tau, w, tol: float = 1e-4, max_iter: int = 1000, warn: bool = True):
+        """K_hat sum_q w_q (K_hat + tau_q I)^{-1} b ~= K_hat^{1/2} b by multi-shift MINRES (csrc/minres.cu); K_hat is this plan's
+        operator with its noise.  b [n, t], t <= 16; tau / w host sequences of Q <= 32 floats.  Returns (out [n, t], CiqInfo)."""
+        _require_cuda_f32(b, "rhs")
+        vec = b.dim() == 1
+        b2 = b.unsqueeze(-1) if vec else b
+        if b2.stride(-1) != 1:
+            b2 = b2.contiguous()
+        n, t = b2.shape
+        Q = len(tau)
+        out = torch.empty(n, t, device=self.device, dtype=torch.float32)
+        ta = (C.c_double * max(Q, 1))(*[float(v) for v in tau])
+        wa = (C.c_double * max(Q, 1))(*[float(v) for v in w])
+        it = C.c_int()
+        resid = (C.c_float * max(Q * t, 1))()
+        with torch.cuda.device(self.device):
+            st = self.lib.gp_ciq_sqrt_matmul(self._h, _ptr(b2), b2.stride(0), t, ta, wa, Q, float(tol), int(max_iter),
+                                             _ptr(out), out.stride(0), C.byref(it), resid)
+        if st == _lib.GP_E_NAN_MVM:
+            raise _lib.NanError(_lib.last_error())
+        check(st, warn=warn)
+        info = CiqInfo(it.value, [[resid[q * t + c] for c in range(t)] for q in range(Q)], st)
+        return (out.squeeze(-1) if vec else out), info
 
     def mll(self, y_minus_mean, eps1, eps2, rademacher, num_probes=10, precond_rank=15, min_precond_size=2000,
             precond_tol=1e-3, cg_tol=1.0, max_cg_iter=1000, max_tridiag_iter=20, want_solve=False, warn=True):

@@ -8,7 +8,8 @@ test/lazy/test_lazy_evaluated_kernel_tensor.py:82-83), restricted to operators t
 import torch
 
 from . import settings
-from .operators import AddedDiagLinearOperator, ConstantDiagLinearOperator, KernelLinearOperator
+from .operators import AddedDiagLinearOperator, ConstantDiagLinearOperator, KernelLinearOperator, RootLinearOperator
+from .sampling import psd_safe_cholesky
 
 
 def _as_operator(obj):
@@ -55,6 +56,14 @@ def inv_quad_logdet(mat, inv_quad_rhs=None, logdet=False, reduce_inv_quad=True):
 def solve(mat, rhs, lhs=None):
     """gpytorch.solve (gpytorch/__init__.py:215-249)."""
     return mat.solve(rhs, lhs)
+
+
+def root_decomposition(mat, method=None):
+    """gpytorch.root_decomposition (gpytorch/__init__.py:176-188): R with R R^T ~= mat ("cholesky" or "lanczos"; None picks by
+    size as sampling does).  A dense tensor gets the psd-safe Cholesky factor."""
+    if torch.is_tensor(mat):
+        return RootLinearOperator(psd_safe_cholesky(mat))
+    return mat.root_decomposition(method=method)
 
 
 def lanczos_tridiag(mat, max_iter, init_vecs=None, tol=1e-5):

@@ -17,7 +17,9 @@ from __future__ import annotations
 import torch
 
 from . import settings
+from ._lib import NanError
 from .engine import Plan
+from .sampling import contour_quadrature, psd_safe_cholesky
 
 
 def _as_list(ls: torch.Tensor):
@@ -114,7 +116,108 @@ class DiagLinearOperator:
         return NotImplemented
 
 
-class KernelLinearOperator:
+class RootLinearOperator:
+    """R R^T held as its dense root R [..., n, r] (what root_decomposition returns; `.root` as in linear_operator)."""
+
+    def __init__(self, root: torch.Tensor):
+        self.root = root
+
+    @property
+    def shape(self):
+        return torch.Size([*self.root.shape[:-1], self.root.shape[-2]])
+
+    def matmul(self, rhs):
+        return self.root @ (self.root.transpose(-1, -2) @ rhs)
+
+    __matmul__ = matmul
+
+    def to_dense(self):
+        return self.root @ self.root.transpose(-1, -2)
+
+
+class _SamplingMixin:
+    """zero_mean_mvn_samples / root_decomposition of an engine operator K_hat (the kernel alone, or kernel + noise).
+
+    Three paths, as the reference picks them (linear_operator LinearOperator.zero_mean_mvn_samples / root_decomposition):
+      * settings.ciq_samples on: K_hat^{1/2} xi by contour integral quadrature, the shifted solves by multi-shift MINRES on the
+        device (csrc/minres.cu), xi ~ N(0, I) from torch's global generator, 16 columns per engine call;
+      * n <= max_cholesky_size or fast_computations(covar_root_decomposition=False): a dense psd-safe Cholesky root;
+      * otherwise a Lanczos root R = Q V Lambda^{1/2} of rank <= max_root_decomposition_size (negative Ritz values masked).
+    Samples of these paths are detached from the hyper-parameters: their gradients are not implemented."""
+
+    def _sampling_plan(self) -> Plan:
+        raise NotImplementedError
+
+    def _noise_floor(self):
+        """A proven lower bound of the spectrum of K_hat from its noise (None without noise)."""
+        return None
+
+    def _ciq_bounds(self, plan: Plan, start: torch.Tensor):
+        """(m, M) for the quadrature: M from the largest Ritz value of 20 Lanczos steps (raised by 1%: a Ritz value is a lower
+        bound of the largest eigenvalue), m the noise floor, else the smallest Ritz value."""
+        n = self.shape[0]
+        if not bool(torch.isfinite(start).all()) or float(start.abs().max()) == 0.0:
+            start = torch.ones(n, device=self.device)
+        _, t = plan.lanczos(start.float().contiguous(), min(20, n))
+        t = t.double().cpu()
+        if not bool(torch.isfinite(t).all()):
+            raise NanError("NaNs encountered when trying to perform matrix-vector multiplication")
+        ritz = torch.linalg.eigvalsh(t)
+        M = 1.01 * float(ritz.max())
+        floor = self._noise_floor()
+        if floor is not None and floor > 0.0:
+            m = floor
+        else:
+            m = float(ritz.min())
+            if m <= 0.0:
+                m = 1e-6 * M
+        return m, max(M, m)
+
+    def _ciq_samples(self, xi: torch.Tensor):
+        """K_hat^{1/2} xi for xi [n, s]; returns ([n, s], list of CiqInfo)."""
+        plan = self._sampling_plan()
+        m, M = self._ciq_bounds(plan, xi[:, 0])
+        tau, w = contour_quadrature(m, M, settings.num_contour_quadrature.value())
+        outs, infos = [], []
+        for c0 in range(0, xi.size(1), 16):
+            o, info = plan.ciq_sqrt_matmul(xi[:, c0:c0 + 16].contiguous(), tau, w, settings.minres_tolerance.value(),
+                                           settings.max_cg_iterations.value())
+            outs.append(o)
+            infos.append(info)
+        self.last_ciq = (m, M, infos)
+        return (outs[0] if len(outs) == 1 else torch.cat(outs, -1)), infos
+
+    def zero_mean_mvn_samples(self, num_samples: int) -> torch.Tensor:
+        """[num_samples, n] draws from N(0, K_hat)."""
+        n = self.shape[0]
+        if settings.ciq_samples.on():
+            xi = torch.randn(n, num_samples, device=self.device)
+            return self._ciq_samples(xi)[0].t()
+        root = self.root_decomposition().root
+        eps = torch.randn(root.size(-1), num_samples, device=root.device, dtype=root.dtype)
+        return (root @ eps).t()
+
+    def root_decomposition(self, method=None) -> RootLinearOperator:
+        """R with R R^T ~= K_hat: "cholesky" (dense, psd-safe) or "lanczos"; None picks as zero_mean_mvn_samples does."""
+        if method not in (None, "cholesky", "lanczos"):
+            raise RuntimeError(f"root_decomposition: unknown method {method!r} (the engine offers 'cholesky' and 'lanczos')")
+        n = self.shape[0]
+        if method == "cholesky" or (method is None and _dense_branch(n, settings.fast_computations.covar_root_decomposition)):
+            return RootLinearOperator(psd_safe_cholesky(self.to_dense().detach().float()))
+        return RootLinearOperator(self._lanczos_root())
+
+    def _lanczos_root(self, init=None) -> torch.Tensor:
+        p = self._sampling_plan()
+        init = init if init is not None else torch.randn(self.shape[0], device=self.device)
+        q, t = p.lanczos(init.float().contiguous(), settings.max_root_decomposition_size.value())
+        evals, evecs = torch.linalg.eigh(t.double())
+        mask = evals >= 0                                 # lanczos_tridiag_to_diag masks negative Ritz values
+        evecs = evecs * mask
+        evals = evals.masked_fill(~mask, 0.0)
+        return (q.double() @ (evecs * evals.sqrt())).float()
+
+
+class KernelLinearOperator(_SamplingMixin):
     """K(x1, x2) (outputscale folded in) that never materialises: every product is the fused CUDA kernel."""
 
     def __init__(self, x1, x2, kind, lengthscale, outputscale=None, plan: Plan | None = None, comm=None,
@@ -280,6 +383,15 @@ class KernelLinearOperator:
 
     def add_jitter(self, jitter_val=1e-3):
         return AddedDiagLinearOperator(self, ConstantDiagLinearOperator(torch.tensor(jitter_val, device=self.device), self.shape[0]))
+
+    def _sampling_plan(self) -> Plan:
+        """The plan of K alone: no noise, no per-row diagonal left over from an earlier K + D."""
+        if not self.same:
+            raise RuntimeError("sampling needs a square covariance operator (x2 == x1)")
+        p = self.plan(0.0)
+        if getattr(p, "_noise_diag", None) is not None:
+            p.set_noise_diag(None)
+        return p
 
     def _bilinear_derivative(self, left, right):
         """(d/d lengthscale, d/d outputscale) of sum(left * (K @ right)); lazy_evaluated_kernel_tensor.py:69-105."""
@@ -528,7 +640,7 @@ class _KernelMatmul(torch.autograd.Function):
         return (None, grad_rhs, *grads)
 
 
-class AddedDiagLinearOperator:
+class AddedDiagLinearOperator(_SamplingMixin):
     """K + D with the BBMM solves (linear_operator AddedDiagLinearOperator): D = sigma^2 I (constant-diagonal branch, Appendix
     A.4) or a per-row diagonal (FixedNoiseGaussianLikelihood; the non-constant-diagonal branch of the preconditioner)."""
 
@@ -588,6 +700,12 @@ class AddedDiagLinearOperator:
             p.set_noise_diag(None)
         self.kernel_op._last_noise = p.noise
         return p
+
+    def _sampling_plan(self) -> Plan:
+        return self._plan()
+
+    def _noise_floor(self):
+        return float(self.diag.diag_vec.detach().min()) if self.per_row else float(self.diag.diag_value.detach().reshape(-1)[0])
 
     def matmul(self, rhs):
         d = self._noise_col() if (self.per_row and rhs.dim() > 1) else self.noise
@@ -813,6 +931,24 @@ class BatchLinearOperator:
 
     def matmul(self, rhs):
         return torch.stack(self._map(lambda b, op: op.matmul(rhs[b] if rhs.dim() == 3 else rhs)))
+
+    def zero_mean_mvn_samples(self, num_samples: int) -> torch.Tensor:
+        """[num_samples, B, n]: every element samples concurrently on its own stream; the base samples are drawn here, in element
+        order, so that a reseeded generator reproduces them."""
+        n = self._mshape[-1]
+        if settings.ciq_samples.on():
+            xi = torch.randn(len(self.ops), n, num_samples, device=self.device)
+            outs = self._map(lambda b, op: op._ciq_samples(xi[b])[0])
+            return torch.stack(outs).permute(2, 0, 1)
+        root = self.root_decomposition().root
+        eps = torch.randn(len(self.ops), root.size(-1), num_samples, device=root.device, dtype=root.dtype)
+        return (root @ eps).permute(2, 0, 1)
+
+    def root_decomposition(self, method=None) -> RootLinearOperator:
+        """Stacked roots [B, n, r]; Lanczos roots of different ranks are padded with zero columns."""
+        roots = self._map(lambda b, op: op.root_decomposition(method).root)
+        r = max(x.size(-1) for x in roots)
+        return RootLinearOperator(torch.stack([torch.nn.functional.pad(x, (0, r - x.size(-1))) for x in roots]))
 
     __matmul__ = matmul
 

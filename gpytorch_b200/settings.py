@@ -108,6 +108,22 @@ class max_root_decomposition_size(_value_context):
     _global_value = 100
 
 
+class ciq_samples(_feature_flag):
+    """Draw MultivariateNormal samples of an engine operator as K_hat^{1/2} xi by contour integral quadrature and multi-shift
+    MINRES (linear_operator settings; off by default).  Off: Cholesky up to max_cholesky_size, a Lanczos root above it."""
+    _default = False
+
+
+class num_contour_quadrature(_value_context):
+    """Quadrature points Q of the CIQ square root (linear_operator settings; default 15)."""
+    _global_value = 15
+
+
+class minres_tolerance(_value_context):
+    """Relative residual at which msMINRES stops (linear_operator settings; default 1e-4)."""
+    _global_value = 1e-4
+
+
 class skip_logdet_forward(_feature_flag):
     _default = False
 

@@ -161,6 +161,15 @@ int gp_slq_logdet(gp_plan* plan, const float* TMAT, int n_tridiag, int ldt, int 
 int gp_lanczos(gp_plan* plan, const float* INIT, int max_iter, float tol, float* Qt, float* T,
                int* J_out);
 
+/* OUT = K_hat * sum_q w_q (K_hat + tau_q I)^{-1} B  ~=  K_hat^{1/2} B  (contour integral quadrature);
+ * B, OUT [n, t] (t <= 16), tau/w host double[Q] (1 <= Q <= 32, tau_q >= 0, finite);
+ * resid_out host float[Q*t]: final |phi| / ||b_c|| per shift and column; *iters_out = iterations run.
+ * Multi-shift MINRES on K_hat = the plan's operator with its noise (the closure of gp_mbcg), one Lanczos process per column
+ * shared by all shifts (msMINRES, Pleiss et al. 2020, arXiv 2006.11267; the reference's CIQ sampler,
+ * linear_operator.utils.contour_integral_quad / minres, behind settings.ciq_samples).  Square, unsharded plans only. */
+int gp_ciq_sqrt_matmul(gp_plan* plan, const float* B, int64_t ldb, int t, const double* tau, const double* w, int Q,
+                       float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out, float* resid_out);
+
 /* one-shot: MultivariateNormal.log_prob (distributions/multivariate_normal.py:221-252) through
  * inv_quad_logdet (:249), i.e. pivoted Cholesky -> preconditioner -> probes -> mBCG -> SLQ. */
 typedef struct gp_mll_opts {
