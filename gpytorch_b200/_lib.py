@@ -86,6 +86,9 @@ PROTOTYPES = {
     "gp_lanczos": (_I, [_P, _P, _I, _F, _P, _P, C.POINTER(_I)]),
     "gp_ciq_sqrt_matmul": (_I, [_P, _P, _L, _I, C.POINTER(C.c_double), C.POINTER(C.c_double), _I, _F, _I, _P, _L,
                                 C.POINTER(_I), C.POINTER(_F)]),
+    "gp_ciq_precond_build": (_I, [_P, _P, _I, _P, C.POINTER(C.c_double)]),
+    "gp_ciq_sqrt_matmul_precond": (_I, [_P, _P, _L, _I, _P, _I, C.POINTER(C.c_double), C.POINTER(C.c_double), _I, _F, _I, _P,
+                                        _L, C.POINTER(_I), C.POINTER(_F)]),
     "gp_mll": (_I, [_P, _P, _P, _P, _P, C.POINTER(MllOpts), _P, C.POINTER(MllResult)]),
     "gp_comm_unique_id": (_I, [C.POINTER(C.c_uint8)]),
     "gp_comm_init": (_I, [C.POINTER(_P), C.POINTER(C.c_uint8), _I, _I]),

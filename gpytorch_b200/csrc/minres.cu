@@ -21,6 +21,26 @@
 // MINRES on the shifted system), or on a Lanczos breakdown (beta_{k+1} below 1e-6 of the column's |T| entries: the Krylov space
 // is exhausted and every shifted residual is exactly zero), or when b_c = 0 (Z = 0, OUT = 0).  The loop ends when every column
 // has converged or at max_iter; the host reads the done flag one iteration behind (look-ahead, as cg.cu).
+//
+// Split preconditioning (gp_ciq_sqrt_matmul_precond).  P = L L^T + D is the pivoted-Cholesky preconditioner of K_hat = K + D
+// (D = sigma^2 I or the per-row diagonal, > 0).  For any F with F F^T = P, A = F^-1 K_hat F^-T satisfies F A F^T = K_hat, so
+// F A^{1/2} xi ~ N(0, K_hat), and by CIQ on A
+//     F A sum_q w_q (A + tau_q I)^-1 xi = K_hat F^-T Z ,   Z = sum_q w_q (A + tau_q I)^-1 xi :
+// only F^-1 and F^-T are ever applied.  F = D^{1/2} (I + M M^T)^{1/2} with M = D^{-1/2} L; with (V, s) = eigh(M^T M),
+//     (I + M M^T)^{-1/2} = I - U U^T ,  U = D^{-1/2} L V diag(h) ,  h_j = (sqrt(1 + s_j) (1 + sqrt(1 + s_j)))^{-1/2}
+// (gp_ciq_precond_build, pivchol.cu), so F^-1 = (I - U U^T) D^{-1/2} and F^-T = D^{-1/2} (I - U U^T).  E = K - L L^T >= 0 (the
+// Schur complement pivoted Cholesky leaves) gives A = I + F^-1 E F^-T, hence 1 <= lambda(A) <= 1 + tr(E) / min d: the quadrature
+// interval needs no Lanczos run.  One preconditioned iteration (c_k = U^T q_k, carried from the previous reduction):
+//   pre        x_k = D^-1/2 (q_k - U c_k) = F^-T q_k                                       (ms_scale_kernel, preconditioned overload)
+//   K.V        on x_k
+//   finish     y = D^-1/2 K_hat x_k ; v = y - beta_k q_{k-1} ; partials of [ q_k . v | U^T y ]
+//   sum        alpha_k = q_k . v - c_k . (U^T y)          (A q_k = y - U U^T y)
+//   orth       v -= U (U^T y) + alpha_k q_k ; partials of [ v . v | U^T v ]
+//   sum        beta_{k+1}^2 ; c_{k+1} = U^T v / beta_{k+1}  (re-based on the actual vector every iteration)
+//   update     as above, with x_k in place of q_k in the direction recurrence: the directions and Z are then the F^-T images
+//              of A's, and the tail OUT = K_hat (|b| Z) is the unpreconditioned one unchanged.
+// The preconditioned kernels are overloads of the kernels they replace (same names, so per-kernel resource checks cover both);
+// their row passes walk 64-row chunks, staging the chunk's rows of U [n][k] in shared memory for U c and U^T v.
 #include <math.h>
 
 #include <algorithm>
@@ -33,6 +53,7 @@ namespace gp {
 constexpr int MS_THREADS = 256;
 constexpr int MS_ROWS = 64;     // rows per pass of a CTA (4 float4 column groups x 64 row lanes)
 constexpr int MS_QMAX = 32;     // shifts per call
+constexpr int MS_KMAX = 128;    // preconditioner rank (the range of gp_precond_build)
 
 void cg_sum_launch(const float* in, int G, int L, double* out, const int* done, cudaStream_t st);   // cg.cu
 void cg_rhs_sq_launch(const float* RHS, int64_t ldr, int t, int64_t n, float* part, int G, cudaStream_t st);
@@ -179,37 +200,240 @@ ms_orth_kernel(const double* __restrict__ sums, const float* __restrict__ Qcur, 
   ms_block_reduce(acc, red, part + (size_t)blockIdx.x * TP);
 }
 
+// ---- preconditioned row passes ----------------------------------------------------------------------------------------------
+// dynamic shared memory: U rows of one chunk [64][kp] (kp = k | 1: an odd pitch puts the 8 rows a warp reads in 8 banks; the
+// region is at least [64][16] and doubles as the reduction scratch after the last chunk) | X block [64][16] | coefficients [k][16]
+__host__ __device__ inline int ms_upitch(int k) { return k | 1; }
+__host__ __device__ inline int ms_urows(int k) { return MS_ROWS * (ms_upitch(k) > TP ? ms_upitch(k) : TP); }
+inline size_t ms_pre_smem(int k) { return sizeof(float) * ((size_t)ms_urows(k) + MS_ROWS * TP + (size_t)k * TP); }
+
+// rows [r0, r0 + nr) of U [n][k] (one contiguous block) -> us [nr][kp]
+__device__ __forceinline__ int ms_stage_u(const float* __restrict__ U, int k, int64_t r0, int64_t n, float* __restrict__ us) {
+  const int nr = (int)min((int64_t)MS_ROWS, n - r0);
+  const int kp = ms_upitch(k);
+  const float* src = U + r0 * k;
+  for (int e = threadIdx.x; e < nr * k; e += MS_THREADS) {
+    const int r = e / k;
+    us[r * kp + (e - r * k)] = src[e];
+  }
+  return nr;
+}
+
+// acc[j] += sum_{r < nr} U[r][a0 + 16 j] xs[r][c]  (thread: c = tid & 15, a0 = tid >> 4)
+__device__ __forceinline__ void ms_ut_acc(const float* __restrict__ us, int k, const float* __restrict__ xs, int nr,
+                                          float (&acc)[MS_KMAX / 16]) {
+  const int c = threadIdx.x & 15, a0 = threadIdx.x >> 4, kp = ms_upitch(k);
+  for (int r = 0; r < nr; ++r) {
+    const float xv = xs[r * TP + c];
+#pragma unroll
+    for (int j = 0; j < MS_KMAX / 16; ++j)
+      if (a0 + 16 * j < k) acc[j] = fmaf(us[r * kp + a0 + 16 * j], xv, acc[j]);
+  }
+}
+
+__device__ __forceinline__ void ms_ut_store(const float (&acc)[MS_KMAX / 16], int k, float* __restrict__ out /*[k][16]*/) {
+  const int c = threadIdx.x & 15, a0 = threadIdx.x >> 4;
+#pragma unroll
+  for (int j = 0; j < MS_KMAX / 16; ++j)
+    if (a0 + 16 * j < k) out[(a0 + 16 * j) * TP + c] = acc[j];
+}
+
+// sum_a U[rl][a] cs[a][4 cg .. 4 cg + 4)
+__device__ __forceinline__ float4 ms_uc(const float* __restrict__ us, int k, const float* __restrict__ cs, int rl, int cg) {
+  const float* u = us + rl * ms_upitch(k);
+  float4 s = make_float4(0, 0, 0, 0);
+  for (int a = 0; a < k; ++a) {
+    const float ua = u[a];
+    const float4 c4 = reinterpret_cast<const float4*>(cs)[a * 4 + cg];
+    s.x = fmaf(ua, c4.x, s.x); s.y = fmaf(ua, c4.y, s.y); s.z = fmaf(ua, c4.z, s.z); s.w = fmaf(ua, c4.w, s.w);
+  }
+  return s;
+}
+
+// alpha_k of column c from [ q_k . v (16) | U^T y (16 k) ] and c_k = U^T q_k [k][16] (fp64, fixed order: every CTA of orth and
+// update computes the same value)
+__device__ __forceinline__ double ms_pre_alpha(const double* __restrict__ sums, const double* __restrict__ cvec, int k, int c) {
+  double a = sums[c];
+  for (int j = 0; j < k; ++j) a -= cvec[j * TP + c] * sums[TP + j * TP + c];
+  return a;
+}
+
+// pre: X = D^-1/2 (Q - U c) = F^-T Q   (c = U^T Q, fp64 [k][16])
+__global__ void __launch_bounds__(MS_THREADS)
+ms_scale_kernel(const float* __restrict__ Qin, const double* __restrict__ cvec, const float* __restrict__ U, int k, float noise,
+                const float* __restrict__ dvec, float* __restrict__ X, int64_t n, const int* __restrict__ done) {
+  if (done && *done) return;
+  extern __shared__ __align__(16) float msh[];
+  float* us = msh;
+  float* cs = msh + ms_urows(k) + MS_ROWS * TP;
+  const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
+  for (int e = tid; e < k * TP; e += MS_THREADS) cs[e] = (float)cvec[e];
+  for (int64_t r0 = (int64_t)blockIdx.x * MS_ROWS; r0 < n; r0 += (int64_t)gridDim.x * MS_ROWS) {
+    ms_stage_u(U, k, r0, n, us);
+    __syncthreads();
+    const int64_t r = r0 + rl;
+    if (r < n) {
+      const float4 uc = ms_uc(us, k, cs, rl, cg);
+      const float4 q = reinterpret_cast<const float4*>(Qin)[r * 4 + cg];
+      const float rs = 1.f / sqrtf(dvec ? dvec[r] : noise);
+      reinterpret_cast<float4*>(X)[r * 4 + cg] = make_float4((q.x - uc.x) * rs, (q.y - uc.y) * rs, (q.z - uc.z) * rs, (q.w - uc.w) * rs);
+    }
+    __syncthreads();
+  }
+}
+
+// finish: y = D^-1/2 (os sum_s partial_s + D x_k) ; v = y - beta_k q_{k-1} ; partials [ q_k . v | U^T y ]  (row pitch 16 (k + 1))
+__global__ void __launch_bounds__(MS_THREADS)
+ms_finish_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_pad, float os, const float* __restrict__ pscale,
+                 float noise, const float* __restrict__ dvec, const float* __restrict__ X, const float* __restrict__ Qcur,
+                 const float* __restrict__ Qprev, float* __restrict__ V, int64_t n, const MsState* __restrict__ st, int kk,
+                 const float* __restrict__ U, int k, float* __restrict__ part, const int* __restrict__ done,
+                 const int* __restrict__ xbad) {
+  if (*done) return;
+  extern __shared__ __align__(16) float msh[];
+  float* us = msh;
+  float* ys = msh + ms_urows(k);
+  __shared__ __align__(16) float bk[TP];
+  const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
+  if (tid < TP) bk[tid] = (float)st->beta[kk & 1][tid];
+  __syncthreads();
+  const float poison = *xbad ? __int_as_float(0x7fc00000) : 0.f;
+  const float4 b4 = reinterpret_cast<const float4*>(bk)[cg];
+  float4 acc = make_float4(0, 0, 0, 0);
+  float uacc[MS_KMAX / 16] = {};
+  for (int64_t r0 = (int64_t)blockIdx.x * MS_ROWS; r0 < n; r0 += (int64_t)gridDim.x * MS_ROWS) {
+    const int nr = ms_stage_u(U, k, r0, n, us);
+    const int64_t r = r0 + rl;
+    float4 y = make_float4(0, 0, 0, 0);
+    if (r < n) {
+      float4 s = make_float4(poison, poison, poison, poison);
+      float osr = os;
+      if (pscale) {
+        for (int sp = 0; sp < nsplit; ++sp) {
+          const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
+          const float w = pscale[sp];
+          s.x = fmaf(w, a.x, s.x); s.y = fmaf(w, a.y, s.y); s.z = fmaf(w, a.z, s.z); s.w = fmaf(w, a.w, s.w);
+        }
+        osr = 1.f;
+      } else {
+        for (int sp = 0; sp < nsplit; ++sp) {
+          const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
+          s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
+        }
+      }
+      const float4 x = reinterpret_cast<const float4*>(X)[r * 4 + cg];
+      const float d = dvec ? dvec[r] : noise;
+      const float rs = 1.f / sqrtf(d);
+      y = make_float4(fmaf(d, x.x, osr * s.x) * rs, fmaf(d, x.y, osr * s.y) * rs, fmaf(d, x.z, osr * s.z) * rs,
+                      fmaf(d, x.w, osr * s.w) * rs);
+      const float4 q = reinterpret_cast<const float4*>(Qcur)[r * 4 + cg];
+      const float4 qp = reinterpret_cast<const float4*>(Qprev)[r * 4 + cg];
+      float4 v;
+      v.x = fmaf(-b4.x, qp.x, y.x); v.y = fmaf(-b4.y, qp.y, y.y); v.z = fmaf(-b4.z, qp.z, y.z); v.w = fmaf(-b4.w, qp.w, y.w);
+      reinterpret_cast<float4*>(V)[r * 4 + cg] = v;
+      acc.x = fmaf(q.x, v.x, acc.x); acc.y = fmaf(q.y, v.y, acc.y); acc.z = fmaf(q.z, v.z, acc.z); acc.w = fmaf(q.w, v.w, acc.w);
+    }
+    reinterpret_cast<float4*>(ys)[rl * 4 + cg] = y;
+    __syncthreads();
+    ms_ut_acc(us, k, ys, nr, uacc);
+    __syncthreads();
+  }
+  float* out = part + (size_t)blockIdx.x * TP * (k + 1);
+  ms_block_reduce(acc, us, out);
+  ms_ut_store(uacc, k, out + TP);
+}
+
+// orth: v -= U (U^T y) + alpha_k q_k ; partials [ v . v | U^T v ]  (sums = [ q_k . v | U^T y ], cvec = c_k).
+// Without sums (start-up pass) V is only read: partials [ v . v | U^T v ] of the block as it is.
+__global__ void __launch_bounds__(MS_THREADS)
+ms_orth_kernel(const double* __restrict__ sums, const double* __restrict__ cvec, const float* __restrict__ Qcur,
+               float* __restrict__ V, int64_t n, const float* __restrict__ U, int k, float* __restrict__ part,
+               const int* __restrict__ done) {
+  if (done && *done) return;
+  extern __shared__ __align__(16) float msh[];
+  float* us = msh;
+  float* vs = msh + ms_urows(k);
+  float* cs = vs + MS_ROWS * TP;
+  __shared__ __align__(16) float al[TP];
+  const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
+  if (sums) {
+    for (int e = tid; e < k * TP; e += MS_THREADS) cs[e] = (float)sums[TP + e];
+    if (tid < TP) al[tid] = (float)ms_pre_alpha(sums, cvec, k, tid);
+  }
+  __syncthreads();
+  const float4 a4 = reinterpret_cast<const float4*>(al)[cg];
+  float4 acc = make_float4(0, 0, 0, 0);
+  float uacc[MS_KMAX / 16] = {};
+  for (int64_t r0 = (int64_t)blockIdx.x * MS_ROWS; r0 < n; r0 += (int64_t)gridDim.x * MS_ROWS) {
+    const int nr = ms_stage_u(U, k, r0, n, us);
+    __syncthreads();
+    const int64_t r = r0 + rl;
+    float4 v = make_float4(0, 0, 0, 0);
+    if (r < n) {
+      v = reinterpret_cast<const float4*>(V)[r * 4 + cg];
+      if (sums) {
+        const float4 uc = ms_uc(us, k, cs, rl, cg);
+        const float4 q = reinterpret_cast<const float4*>(Qcur)[r * 4 + cg];
+        v.x = fmaf(-a4.x, q.x, v.x - uc.x); v.y = fmaf(-a4.y, q.y, v.y - uc.y);
+        v.z = fmaf(-a4.z, q.z, v.z - uc.z); v.w = fmaf(-a4.w, q.w, v.w - uc.w);
+        reinterpret_cast<float4*>(V)[r * 4 + cg] = v;
+      }
+      acc.x = fmaf(v.x, v.x, acc.x); acc.y = fmaf(v.y, v.y, acc.y); acc.z = fmaf(v.z, v.z, acc.z); acc.w = fmaf(v.w, v.w, acc.w);
+    }
+    reinterpret_cast<float4*>(vs)[rl * 4 + cg] = v;
+    __syncthreads();
+    ms_ut_acc(us, k, vs, nr, uacc);
+    __syncthreads();
+  }
+  float* out = part + (size_t)blockIdx.x * TP * (k + 1);
+  ms_block_reduce(acc, us, out);
+  ms_ut_store(uacc, k, out + TP);
+}
+
 // rotations + q_{k+1} + direction blocks + Z + stop rule.  sums = [ alpha_k (16) | beta_{k+1}^2 (16) ].
+// Preconditioned (PRE): sums = [ q_k . v | U^T y ] (alpha_k through ms_pre_alpha with cprev = c_k), sums2 = [ v . v | U^T v ],
+// Qcur = x_k = F^-T q_k (the direction recurrence runs on the F^-T images), and block 0 writes c_{k+1} = U^T v / beta_{k+1} to
+// cnext (0 for a converged or broken-down column, whose q_{k+1} is 0).
 // D holds 2 blocks per shift: at iteration kk, d_{k-1} is block 2q + ((kk + 1) & 1) and d_{k-2} is block 2q + (kk & 1); the new
 // direction overwrites d_{k-2}.
+template <bool PRE>
 __global__ void __launch_bounds__(MS_THREADS)
-ms_update_kernel(const double* __restrict__ sums, int kk, int Q, int t, float tol, const float* __restrict__ V,
+ms_update_kernel(const double* __restrict__ sums, const double* __restrict__ sums2, const double* __restrict__ cprev,
+                 double* __restrict__ cnext, int k, int kk, int Q, int t, float tol, const float* __restrict__ V,
                  const float* __restrict__ Qcur, float* __restrict__ Qnext, float* __restrict__ D, float* __restrict__ Z, int64_t n,
                  MsState* __restrict__ st) {
   if (st->done_iter < kk) return;
   __shared__ __align__(16) float cD[MS_QMAX * TP], cE[MS_QMAX * TP], cG[MS_QMAX * TP], cW[MS_QMAX * TP];
   __shared__ float aphi[MS_QMAX * TP];
   __shared__ __align__(16) float invb[TP];
-  __shared__ int brk_s[TP];
-  __shared__ double bnext_s[TP];
+  __shared__ int brk_s[TP], nan_s[TP];
+  __shared__ double bnext_s[TP], alpha_s[TP];
   const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
   const int P = kk & 1, Pn = P ^ 1;
   const bool writer = blockIdx.x == 0;
   if (tid < TP) {
-    const double alpha = sums[tid];
-    double bn = sqrt(fmax(sums[TP + tid], 0.0));
+    const double alpha = PRE ? ms_pre_alpha(sums, cprev, k, tid) : sums[tid];
+    const double bn2 = PRE ? sums2[tid] : sums[TP + tid];
+    double bn = sqrt(fmax(bn2, 0.0));
     const double bk = st->beta[P][tid];
     // breakdown: the Krylov space of this column is exhausted (also taken for a NaN column, which the nan flag reports)
     const bool brk = !(bn > 1e-6 * sqrt(alpha * alpha + bk * bk + bn * bn));
     if (brk) bn = 0.0;
     bnext_s[tid] = bn;
+    alpha_s[tid] = alpha;
     brk_s[tid] = brk;
+    nan_s[tid] = !(alpha == alpha && bn2 == bn2);
     invb[tid] = (brk || st->conv[P][tid]) ? 0.f : (float)(1.0 / bn);
   }
   __syncthreads();
+  if (PRE && writer)
+    for (int e = tid; e < k * TP; e += MS_THREADS) {
+      const int c = e % TP;
+      cnext[e] = (brk_s[c] || st->conv[P][c]) ? 0.0 : sums2[TP + e] / bnext_s[c];
+    }
   for (int e = tid; e < Q * TP; e += MS_THREADS) {
     const int q = e / TP, c = e % TP;
-    const double a = sums[c] + st->tau[q];
+    const double a = alpha_s[c] + st->tau[q];
     const double bk = st->beta[P][c], bn = bnext_s[c];
     const double c1 = st->c1[P][e], s1 = st->s1[P][e], c2 = st->c2[P][e], s2 = st->s2[P][e], pb = st->phibar[P][e];
     const double eps = s2 * bk, dbar = c2 * bk;           // G_{k-2} applied to (0, beta_k)
@@ -273,7 +497,7 @@ ms_update_kernel(const double* __restrict__ sums, int kk, int Q, int t, float to
       st->conv[Pn][c] = conv;
       st->beta[Pn][c] = bnext_s[c];
     }
-    const bool bad = kk == 0 && c < t && !(sums[c] == sums[c] && sums[TP + c] == sums[TP + c]);
+    const bool bad = kk == 0 && c < t && nan_s[c];
     const bool all = __all_sync(0xffffffffu, conv);
     const bool anybad = __any_sync(0xffffffffu, bad);
     if (c == 0) {
@@ -295,9 +519,16 @@ __global__ void ms_scale_kernel(float* __restrict__ Z, const MsState* __restrict
   if (idx < n * TP) Z[idx] *= st->rhs_norm[idx % TP];
 }
 
-int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const double* tau, const double* w, int Q, float tol, int max_iter,
-            float* OUT, int64_t ldo, int* iters_out, float* resid_out) {
+// U == nullptr: OUT = K_hat sum_q w_q (K_hat + tau_q I)^-1 B.  U [n][k]: OUT = K_hat F^-T sum_q w_q (A + tau_q I)^-1 B (header).
+int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int k, const double* tau, const double* w, int Q,
+            float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out, float* resid_out) {
   GP_REQUIRE(p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  const bool pre = U != nullptr || k != 0;
+  if (pre) {
+    GP_REQUIRE(U != nullptr && k >= 1 && k <= MS_KMAX, GP_E_SHAPE, "preconditioner factor U [n, k] with k in [1,%d] (k=%d, U %s)",
+               MS_KMAX, k, U ? "set" : "null");
+    GP_REQUIRE(p->noise_diag != nullptr || p->noise > 0.f, GP_E_SHAPE, "the preconditioned CIQ needs noise > 0");
+  }
   GP_REQUIRE(p->same, GP_E_SHAPE, "CIQ needs a square operator (X2 == X1)");
   GP_REQUIRE(!(p->comm && p->comm->world > 1) && p->row_begin == 0 && p->row_count == p->n2, GP_E_SHAPE,
              "gp_ciq_sqrt_matmul is not supported on row-sharded plans");
@@ -313,13 +544,17 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const double* tau, c
   GP_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = p->stream;
   const int64_t n = p->n2;
-  const int G = (int)std::min<int64_t>(cdiv(n, MS_ROWS), (int64_t)8 * p->n_sm);
+  // the preconditioned row passes hold ~45 KB of shared memory (k = 128): 4 CTAs per SM
+  const int G = (int)std::min<int64_t>(cdiv(n, MS_ROWS), (int64_t)(pre ? 4 : 8) * p->n_sm);
   const size_t blk = (size_t)n * TP;
-  // workspace: q (2 blocks) | v | Z | directions (2 Q blocks) | partials [2][G][16] | sums [48] | tau, w | state
-  const size_t vec_floats = blk * (4 + 2 * (size_t)Q);
+  const int L = pre ? TP * (k + 1) : TP;   // partial row: [ dot (16) | U^T block (16 k) ]
+  // workspace: q (2 blocks) | v | Z | directions (2 Q blocks) | x (preconditioned) | partials [2][G][L] | sums | tau, w | state
+  // sums: [16] |b|^2 | [32] alpha | beta^2 ; preconditioned: [16] |b|^2 | A, B, start-up sums [3][L] | c_k buffer [16 k]
+  const size_t vec_floats = blk * (4 + 2 * (size_t)Q + (pre ? 1 : 0));
+  const size_t nsums = pre ? TP + 3 * (size_t)L + (size_t)TP * k : 48;
   const size_t off_part = vec_floats * sizeof(float);
-  const size_t off_sums = off_part + sizeof(float) * 2 * (size_t)G * TP;
-  const size_t off_tw = off_sums + sizeof(double) * 48;
+  const size_t off_sums = off_part + sizeof(float) * 2 * (size_t)G * L;
+  const size_t off_tw = off_sums + sizeof(double) * nsums;
   const size_t off_state = off_tw + sizeof(double) * 2 * MS_QMAX;
   GP_CHECK(p->msw.ensure(off_state + sizeof(MsState)));
   char* base = p->msw.as<char>();
@@ -327,10 +562,15 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const double* tau, c
   float* V = Qb[1] + blk;
   float* Z = V + blk;
   float* D = Z + blk;
+  float* X = D + 2 * (size_t)Q * blk;   // x_k = F^-T q_k (preconditioned only)
   float* part1 = reinterpret_cast<float*>(base + off_part);
-  float* part2 = part1 + (size_t)G * TP;
+  float* part2 = part1 + (size_t)G * L;
   double* sums0 = reinterpret_cast<double*>(base + off_sums);   // [16] |b|^2
   double* sums = sums0 + TP;                                    // [32] alpha | beta^2
+  double* sumsA = sums0 + TP;                                   // preconditioned: [ q.v | U^T y ]
+  double* sumsB = sumsA + L;                                    //                 [ v.v | U^T v ]
+  double* sumsI = sumsB + L;                                    //                 [ q_1.q_1 | U^T q_1 ]
+  double* cbuf[2] = {sumsI + TP, sumsI + L};                    // c_k = U^T q_k by iteration parity (c_1 from the start-up pass)
   double* d_tw = reinterpret_cast<double*>(base + off_tw);
   MsState* S = reinterpret_cast<MsState*>(base + off_state);
   const int* done = &S->done;
@@ -346,6 +586,12 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const double* tau, c
   cg_sum_launch(part1, G, TP, sums0, nullptr, st);
   ms_init_kernel<<<G, MS_THREADS, 0, st>>>(B, ldb, t, n, sums0, Q, d_tw, Qb[0], Qb[1], Z, S);
   p->launches += 3;
+  const size_t shp = pre ? ms_pre_smem(k) : 0;
+  if (pre) {   // c_1 = U^T q_1
+    ms_orth_kernel<<<G, MS_THREADS, shp, st>>>(nullptr, nullptr, nullptr, Qb[0], n, U, k, part2, nullptr);
+    cg_sum_launch(part2, G, L, sumsI, nullptr, st);
+    p->launches += 2;
+  }
   GP_CUDA(cudaGetLastError());
 
   // ---- iterations ----
@@ -358,14 +604,27 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const double* tau, c
   for (int kk = 0; kk < max_iter && !finished; ++kk) {
     float* Qcur = Qb[kk & 1];
     float* Qoth = Qb[(kk + 1) & 1];   // q_{k-1} on entry, q_{k+1} on exit
-    if ((status = kmv_partials(p, Qcur, done)) != GP_OK) break;
-    ms_finish_kernel<<<G, MS_THREADS, 0, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p),
-                                               p->noise, dvec, Qcur, Qoth, V, n, S, kk, part1, done, p->xbad);
-    cg_sum_launch(part1, G, TP, sums, done, st);
-    ms_orth_kernel<<<G, MS_THREADS, 0, st>>>(sums, Qcur, V, n, part2, done);
-    cg_sum_launch(part2, G, TP, sums + TP, done, st);
-    ms_update_kernel<<<G, MS_THREADS, 0, st>>>(sums, kk, Q, t, tol, V, Qcur, Qoth, D, Z, n, S);
-    p->launches += 5;
+    if (pre) {
+      const double* ck = cbuf[kk & 1];
+      ms_scale_kernel<<<G, MS_THREADS, shp, st>>>(Qcur, ck, U, k, p->noise, dvec, X, n, done);
+      if ((status = kmv_partials(p, X, done)) != GP_OK) break;
+      ms_finish_kernel<<<G, MS_THREADS, shp, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p),
+                                                   p->noise, dvec, X, Qcur, Qoth, V, n, S, kk, U, k, part1, done, p->xbad);
+      cg_sum_launch(part1, G, L, sumsA, done, st);
+      ms_orth_kernel<<<G, MS_THREADS, shp, st>>>(sumsA, ck, Qcur, V, n, U, k, part2, done);
+      cg_sum_launch(part2, G, L, sumsB, done, st);
+      ms_update_kernel<true><<<G, MS_THREADS, 0, st>>>(sumsA, sumsB, ck, cbuf[(kk + 1) & 1], k, kk, Q, t, tol, V, X, Qoth, D, Z, n, S);
+      p->launches += 6;
+    } else {
+      if ((status = kmv_partials(p, Qcur, done)) != GP_OK) break;
+      ms_finish_kernel<<<G, MS_THREADS, 0, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p),
+                                                 p->noise, dvec, Qcur, Qoth, V, n, S, kk, part1, done, p->xbad);
+      cg_sum_launch(part1, G, TP, sums, done, st);
+      ms_orth_kernel<<<G, MS_THREADS, 0, st>>>(sums, Qcur, V, n, part2, done);
+      cg_sum_launch(part2, G, TP, sums + TP, done, st);
+      ms_update_kernel<false><<<G, MS_THREADS, 0, st>>>(sums, nullptr, nullptr, nullptr, 0, kk, Q, t, tol, V, Qcur, Qoth, D, Z, n, S);
+      p->launches += 5;
+    }
     // look-ahead stop check: read the flag of iteration kk after iteration kk + 1 has been enqueued
     cudaMemcpyAsync(&h_done[kk & 1], &S->done, sizeof(int), cudaMemcpyDeviceToHost, st);
     cudaEventRecord(ev[kk & 1], st);
@@ -380,7 +639,7 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const double* tau, c
     status = GP_E_CUDA;
   }
   if (status == GP_OK) {
-    // OUT = K_hat (|b| Z)
+    // OUT = K_hat (|b| Z)   (preconditioned: Z already holds F^-T sum_q w_q (A + tau_q I)^-1 q_1)
     ms_scale_kernel<<<(unsigned)cdiv((int64_t)blk, 256), 256, 0, st>>>(Z, S, n);
     p->launches++;
     status = kmv_partials(p, Z, nullptr);
@@ -423,5 +682,13 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const double* tau, c
 extern "C" int gp_ciq_sqrt_matmul(gp_plan* plan, const float* B, int64_t ldb, int t, const double* tau, const double* w, int Q,
                                   float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out, float* resid_out) {
   GP_REQUIRE(plan != nullptr, GP_E_STATE, "null plan");
-  return gp::ciq_run(plan, B, ldb, t, tau, w, Q, tol, max_iter, OUT, ldo, iters_out, resid_out);
+  return gp::ciq_run(plan, B, ldb, t, nullptr, 0, tau, w, Q, tol, max_iter, OUT, ldo, iters_out, resid_out);
+}
+
+extern "C" int gp_ciq_sqrt_matmul_precond(gp_plan* plan, const float* B, int64_t ldb, int t, const float* U, int k, const double* tau,
+                                          const double* w, int Q, float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out,
+                                          float* resid_out) {
+  GP_REQUIRE(plan != nullptr, GP_E_STATE, "null plan");
+  GP_REQUIRE(U != nullptr, GP_E_SHAPE, "preconditioned CIQ without a factor U (k=%d)", k);
+  return gp::ciq_run(plan, B, ldb, t, U, k, tau, w, Q, tol, max_iter, OUT, ldo, iters_out, resid_out);
 }

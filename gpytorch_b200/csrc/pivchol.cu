@@ -8,6 +8,10 @@
 // through the k x k Cholesky of (L^T L + sigma^2 I) in fp64 instead of a QR of [L; sigma I]:
 // W = L C^{-T} spans the same column space as Q[:n] with W W^T == Q Q^T, and
 // log det P = log det(L^T L + sigma^2 I) + (n - k) log sigma^2.
+// gp_ciq_precond_build turns the same L into the split factor U of the preconditioned CIQ sampler (minres.cu header).
+#include <algorithm>
+#include <cmath>
+
 #include "gp_common.cuh"
 
 namespace gp {
@@ -556,6 +560,94 @@ __global__ void logsum_kernel(const float* __restrict__ d, int64_t n, double* __
   if (threadIdx.x == 0) *out = sh[0];
 }
 
+// ---- split-preconditioner factor of the CIQ sampler (gp_ciq_precond_build, minres.cu header) ----
+// U[r][j] = s_r sum_b T[j][b] L[b][r]  (T = diag(h) V^T, s_r = d_r^{-1/2}); the row / j-group mapping of wsolve_kernel, all b
+__global__ void __launch_bounds__(128)
+usolve_kernel(const float* __restrict__ Lt, int k, int64_t n, const double* __restrict__ T, const float* __restrict__ dvec,
+              double sigma_inv, float* __restrict__ U) {
+  extern __shared__ double shw[];
+  double* Ts = shw;                        // [k][k]
+  double* Ls = shw + (size_t)k * k;        // [k][32]
+  for (int e = threadIdx.x; e < k * k; e += 128) Ts[e] = T[e];
+  const int rl = threadIdx.x & 31, ag = threadIdx.x >> 5;
+  for (int blk = 0; blk < WS_BLOCKS; ++blk) {
+    const int64_t r0 = ((int64_t)blockIdx.x * WS_BLOCKS + blk) * 32;
+    if (r0 >= n) break;
+    __syncthreads();
+    for (int e = threadIdx.x; e < k * 32; e += 128) {
+      int b = e >> 5, rr = e & 31;
+      Ls[e] = (r0 + rr < n) ? (double)Lt[(int64_t)b * n + r0 + rr] : 0.0;
+    }
+    __syncthreads();
+    const int64_t r = r0 + rl;
+    if (r >= n) continue;
+    const double sr = dvec ? 1.0 / sqrt((double)dvec[r]) : sigma_inv;
+    for (int a = ag; a < k; a += 4) {
+      double s = 0.0;
+      for (int b = 0; b < k; ++b) s = fma(Ts[a * k + b], Ls[b * 32 + rl], s);
+      U[r * k + a] = (float)(s * sr);
+    }
+  }
+}
+
+// per-CTA fp64 partials [sum Lt^2 | min d] (min d = -1 once a d is <= 0 or NaN), reduced on the host in CTA order
+__global__ void __launch_bounds__(256)
+ciq_stats_kernel(const float* __restrict__ Lt, int64_t total, const float* __restrict__ dvec, int64_t n, double* __restrict__ part) {
+  __shared__ double s_sum[256], s_min[256];
+  const int tid = threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * 256;
+  double s = 0.0, m = INFINITY;
+  for (int64_t e = (int64_t)blockIdx.x * 256 + tid; e < total; e += stride) {
+    const double v = Lt[e];
+    s = fma(v, v, s);
+  }
+  if (dvec)
+    for (int64_t j = (int64_t)blockIdx.x * 256 + tid; j < n; j += stride) {
+      const float v = dvec[j];
+      m = (v > 0.f) ? fmin(m, (double)v) : -1.0;
+    }
+  s_sum[tid] = s; s_min[tid] = m;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (tid < h) { s_sum[tid] += s_sum[tid + h]; s_min[tid] = fmin(s_min[tid], s_min[tid + h]); }
+    __syncthreads();
+  }
+  if (tid == 0) { part[2 * blockIdx.x] = s_sum[0]; part[2 * blockIdx.x + 1] = s_min[0]; }
+}
+
+// Cyclic Jacobi eigen-decomposition of the symmetric k x k matrix A (fp64, fixed rotation order: deterministic).  On return the
+// diagonal of A holds the eigenvalues and the columns of V the eigenvectors.
+static void jacobi_eigh(int k, double* A, double* V) {
+  double fro = 0.0;
+  for (int e = 0; e < k * k; ++e) { V[e] = (e / k == e % k) ? 1.0 : 0.0; fro += A[e] * A[e]; }
+  for (int sweep = 0; sweep < 64; ++sweep) {
+    double off = 0.0;
+    for (int p = 0; p < k; ++p)
+      for (int q = p + 1; q < k; ++q) off += A[p * k + q] * A[p * k + q];
+    if (off <= 1e-32 * fro) break;
+    for (int p = 0; p < k - 1; ++p)
+      for (int q = p + 1; q < k; ++q) {
+        const double apq = A[p * k + q];
+        if (apq == 0.0) continue;
+        const double theta = (A[q * k + q] - A[p * k + p]) / (2.0 * apq);
+        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int r = 0; r < k; ++r) {   // A J
+          const double arp = A[r * k + p], arq = A[r * k + q];
+          A[r * k + p] = c * arp - s * arq; A[r * k + q] = s * arp + c * arq;
+        }
+        for (int r = 0; r < k; ++r) {   // J^T (A J)
+          const double apr = A[p * k + r], aqr = A[q * k + r];
+          A[p * k + r] = c * apr - s * aqr; A[q * k + r] = s * apr + c * aqr;
+        }
+        for (int r = 0; r < k; ++r) {   // V J
+          const double vrp = V[r * k + p], vrq = V[r * k + q];
+          V[r * k + p] = c * vrp - s * vrq; V[r * k + q] = s * vrp + c * vrq;
+        }
+      }
+  }
+}
+
 // Z[r][c] = sum_a L[a][r] eps1[a][c] + sigma eps2[r][c]
 __global__ void probes_kernel(const float* __restrict__ Lt, int k, int64_t n_total, int64_t row_begin, int64_t n_local,
                               const float* __restrict__ eps1, const float* __restrict__ eps2, int tp, float sigma,
@@ -720,6 +812,80 @@ extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, do
   if (logdet_out) *logdet_out = h[0];
   int fail = *reinterpret_cast<int*>(h + 2);
   GP_REQUIRE(!fail, GP_W_PIVCHOL_NAN, "preconditioner Gram matrix is not positive definite");
+  return GP_OK;
+}
+
+extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U, double* trace_resid_out) {
+  GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  GP_REQUIRE(k >= 1 && k <= 128, GP_E_SHAPE, "preconditioner rank %d not in [1,128]", k);
+  GP_REQUIRE(Lt != nullptr && U != nullptr, GP_E_SHAPE, "Lt / U missing");
+  GP_REQUIRE(p->same, GP_E_SHAPE, "the CIQ preconditioner needs a square operator");
+  GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "the CIQ preconditioner is not available for the SKI backend");
+  GP_REQUIRE(!(p->comm && p->comm->world > 1) && p->row_begin == 0 && p->row_count == p->n2, GP_E_SHAPE,
+             "gp_ciq_precond_build is not supported on row-sharded plans");
+  const float* dvec = p->noise_diag;
+  GP_REQUIRE(dvec != nullptr || p->noise > 0.f, GP_E_SHAPE, "the CIQ preconditioner needs noise > 0");
+  cudaStream_t st = p->stream;
+  const int64_t n = p->n2;
+  // Gram G = L^T D^-1 L (per-row noise) or L^T L (scalar noise, divided by sigma^2 below): gram_kernel with precond_build's split
+  const int ntile = (int)cdiv(k, GT);
+  const int nz = (int)std::min<int64_t>(64, std::max<int64_t>(1, std::min<int64_t>(n / 1024, (2 * p->n_sm) / (ntile * (ntile + 1) / 2))));
+  const int64_t jslice = cdiv(cdiv(n, nz), 64) * 64;
+  const int gs = (int)std::max<int64_t>(1, std::min<int64_t>(cdiv((int64_t)k * n, 4096), (int64_t)2 * p->n_sm));
+  GP_CHECK(p->gram.ensure(sizeof(double) * ((size_t)nz * k * k + 2 * (size_t)gs)));
+  GP_CHECK(p->cholC.ensure(sizeof(double) * ((size_t)2 * k * k + 4) + 64));
+  double* gpart = p->gram.as<double>();
+  double* spart = gpart + (size_t)nz * k * k;
+  double* d_T = p->cholC.as<double>();
+  gram_kernel<<<dim3((unsigned)ntile, (unsigned)ntile, (unsigned)nz), 256, 0, st>>>(Lt, k, n, jslice, dvec, gpart);
+  ciq_stats_kernel<<<gs, 256, 0, st>>>(Lt, (int64_t)k * n, dvec, n, spart);
+  p->launches += 2;
+  GP_CUDA(cudaGetLastError());
+  std::vector<double> hpart((size_t)nz * k * k + 2 * (size_t)gs);
+  GP_CUDA(cudaMemcpyAsync(hpart.data(), gpart, sizeof(double) * hpart.size(), cudaMemcpyDeviceToHost, st));
+  GP_CUDA(cudaStreamSynchronize(st));
+  const double* hs = hpart.data() + (size_t)nz * k * k;
+  double lsq = 0.0, dmin = INFINITY;
+  for (int b = 0; b < gs; ++b) { lsq += hs[2 * b]; dmin = std::min(dmin, hs[2 * b + 1]); }
+  GP_REQUIRE(!dvec || dmin > 0.0, GP_E_SHAPE, "the CIQ preconditioner needs a per-row noise diagonal > 0");
+  const double sig2 = dvec ? 1.0 : (double)p->noise;
+  std::vector<double> A((size_t)k * k), V((size_t)k * k), T((size_t)k * k);
+  bool finite = std::isfinite(lsq);
+  for (int e = 0; e < k * k; ++e) {
+    double s = 0.0;
+    for (int z = 0; z < nz; ++z) s += hpart[(size_t)z * k * k + e];
+    A[e] = s / sig2;
+    finite = finite && std::isfinite(A[e]);
+  }
+  if (!finite) {
+    set_error("NaNs encountered in the CIQ preconditioner factor. Attempting to continue without preconditioning.");
+    return GP_W_PIVCHOL_NAN;
+  }
+  // (V, s) = eigh(M^T M), M = D^-1/2 L ; T = diag(h) V^T with h_j = (sqrt(1 + s_j) (1 + sqrt(1 + s_j)))^-1/2 (no 1/s, no subtraction)
+  jacobi_eigh(k, A.data(), V.data());
+  for (int j = 0; j < k; ++j) {
+    const double r1 = sqrt(1.0 + std::max(A[(size_t)j * k + j], 0.0));
+    const double h = 1.0 / sqrt(r1 * (1.0 + r1));
+    for (int b = 0; b < k; ++b) T[(size_t)j * k + b] = h * V[(size_t)b * k + j];
+  }
+  GP_CUDA(cudaMemcpyAsync(d_T, T.data(), sizeof(double) * k * k, cudaMemcpyHostToDevice, st));   // pageable: copied before return
+  const size_t shu = sizeof(double) * ((size_t)k * k + (size_t)k * 32);
+  static bool attr_done[64] = {};
+  if (!attr_done[p->device & 63]) {
+    GP_CUDA(cudaFuncSetAttribute(usolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 168 * 1024));   // 128 KB + 32 KB
+    attr_done[p->device & 63] = true;
+  }
+  usolve_kernel<<<(unsigned)cdiv(n, 32 * WS_BLOCKS), 128, shu, st>>>(Lt, k, n, d_T, dvec, 1.0 / sqrt((double)p->noise), U);
+  p->launches += 1;
+  GP_CUDA(cudaGetLastError());
+  // tr(K - L L^T): the diagonal of a stationary kernel (sum) is its (summed) outputscale, as gp_kdiag fills it
+  double os_total = p->outputscale;
+  if (p->backend == GP_BACKEND_SUM) {
+    os_total = 0.0;
+    for (const gp_plan* q : p->terms) os_total += q->outputscale;
+  }
+  if (trace_resid_out) *trace_resid_out = (double)n * os_total - lsq;
+  GP_CUDA(cudaStreamSynchronize(st));
   return GP_OK;
 }
 

@@ -34,6 +34,7 @@ class CiqInfo:
     iters: int
     residual_norms: list      # [Q][t]: final |phibar| / |b_c| per shift and column
     status: int
+    precond_rank: int = 0     # k of the split preconditioner (0: unpreconditioned)
 
 
 class Plan:
@@ -201,6 +202,15 @@ class Plan:
         st = check(self.lib.gp_precond_build(self._h, _ptr(lt), k, _ptr(w), C.byref(ld)))
         return w, ld.value, st
 
+    def ciq_precond_build(self, lt: torch.Tensor):
+        """U [n, k], tr(K - L L^T) and the status: the split factor of P = L L^T + D for ciq_sqrt_matmul(precond_u=U)."""
+        lt = lt.contiguous()
+        k = lt.size(0)
+        u = torch.empty(self.n2, k, device=self.device, dtype=torch.float32)
+        tr = C.c_double()
+        st = check(self.lib.gp_ciq_precond_build(self._h, _ptr(lt), k, _ptr(u), C.byref(tr)))
+        return u, tr.value, st
+
     def precond_probes(self, lt, eps1, eps2):
         lt = lt.contiguous(); eps1 = eps1.contiguous(); eps2 = eps2.contiguous()
         k, tp = lt.size(0), eps2.size(1)
@@ -246,9 +256,12 @@ class Plan:
         check(self.lib.gp_lanczos(self._h, _ptr(init), int(max_iter), float(tol), _ptr(qt), _ptr(tm), C.byref(j)))
         return qt[: j.value].t(), tm[: j.value, : j.value]
 
-    def ciq_sqrt_matmul(self, b: torch.Tensor, tau, w, tol: float = 1e-4, max_iter: int = 1000, warn: bool = True):
+    def ciq_sqrt_matmul(self, b: torch.Tensor, tau, w, tol: float = 1e-4, max_iter: int = 1000, warn: bool = True,
+                        precond_u: torch.Tensor | None = None):
         """K_hat sum_q w_q (K_hat + tau_q I)^{-1} b ~= K_hat^{1/2} b by multi-shift MINRES (csrc/minres.cu); K_hat is this plan's
-        operator with its noise.  b [n, t], t <= 16; tau / w host sequences of Q <= 32 floats.  Returns (out [n, t], CiqInfo)."""
+        operator with its noise.  b [n, t], t <= 16; tau / w host sequences of Q <= 32 floats.  Returns (out [n, t], CiqInfo).
+        With precond_u = U [n, k] from ciq_precond_build: K_hat F^-T sum_q w_q (A + tau_q I)^{-1} b ~= F A^{1/2} b, A = F^-1 K_hat F^-T
+        (tau / w then belong to A's spectrum)."""
         _require_cuda_f32(b, "rhs")
         vec = b.dim() == 1
         b2 = b.unsqueeze(-1) if vec else b
@@ -262,12 +275,18 @@ class Plan:
         it = C.c_int()
         resid = (C.c_float * max(Q * t, 1))()
         with torch.cuda.device(self.device):
-            st = self.lib.gp_ciq_sqrt_matmul(self._h, _ptr(b2), b2.stride(0), t, ta, wa, Q, float(tol), int(max_iter),
-                                             _ptr(out), out.stride(0), C.byref(it), resid)
+            if precond_u is None:
+                st = self.lib.gp_ciq_sqrt_matmul(self._h, _ptr(b2), b2.stride(0), t, ta, wa, Q, float(tol), int(max_iter),
+                                                 _ptr(out), out.stride(0), C.byref(it), resid)
+            else:
+                u = precond_u.contiguous()
+                st = self.lib.gp_ciq_sqrt_matmul_precond(self._h, _ptr(b2), b2.stride(0), t, _ptr(u), u.size(-1), ta, wa, Q,
+                                                         float(tol), int(max_iter), _ptr(out), out.stride(0), C.byref(it), resid)
         if st == _lib.GP_E_NAN_MVM:
             raise _lib.NanError(_lib.last_error())
         check(st, warn=warn)
-        info = CiqInfo(it.value, [[resid[q * t + c] for c in range(t)] for q in range(Q)], st)
+        info = CiqInfo(it.value, [[resid[q * t + c] for c in range(t)] for q in range(Q)], st,
+                       0 if precond_u is None else precond_u.size(-1))
         return (out.squeeze(-1) if vec else out), info
 
     def mll(self, y_minus_mean, eps1, eps2, rademacher, num_probes=10, precond_rank=15, min_precond_size=2000,

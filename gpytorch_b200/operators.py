@@ -173,15 +173,24 @@ class _SamplingMixin:
                 m = 1e-6 * M
         return m, max(M, m)
 
+    def _ciq_precond(self):
+        """(U [n, k], m, M) of the split preconditioner F (csrc/minres.cu header) when settings.ciq_preconditioner applies, else None."""
+        return None
+
     def _ciq_samples(self, xi: torch.Tensor):
-        """K_hat^{1/2} xi for xi [n, s]; returns ([n, s], list of CiqInfo)."""
+        """K_hat^{1/2} xi for xi [n, s] (F A^{1/2} xi with settings.ciq_preconditioner); returns ([n, s], list of CiqInfo)."""
         plan = self._sampling_plan()
-        m, M = self._ciq_bounds(plan, xi[:, 0])
+        pre = self._ciq_precond() if settings.ciq_preconditioner.on() else None
+        if pre is None:
+            u = None
+            m, M = self._ciq_bounds(plan, xi[:, 0])
+        else:
+            u, m, M = pre
         tau, w = contour_quadrature(m, M, settings.num_contour_quadrature.value())
         outs, infos = [], []
         for c0 in range(0, xi.size(1), 16):
             o, info = plan.ciq_sqrt_matmul(xi[:, c0:c0 + 16].contiguous(), tau, w, settings.minres_tolerance.value(),
-                                           settings.max_cg_iterations.value())
+                                           settings.max_cg_iterations.value(), precond_u=u)
             outs.append(o)
             infos.append(info)
         self.last_ciq = (m, M, infos)
@@ -793,6 +802,23 @@ class AddedDiagLinearOperator(_SamplingMixin):
                 w, logdet, st2 = p.precond_build(lt)
                 self._precond_cache = (None, None, 0.0) if st2 != 0 else (w, lt, logdet)
         return self._precond_cache
+
+    def _ciq_precond(self):
+        """The split factor of the solves' preconditioner P = L L^T + D, built from the Lt of _preconditioner() (no second pivoted
+        Cholesky) and rebuilt whenever that cache is.  Interval: 1 <= lambda(F^-1 K_hat F^-T) <= 1 + tr(K - L L^T) / min d; the
+        bounds used are [1/2, 2 (1 + max(tr, 1e-6 tr K) / min d)], the margins absorbing the fp32 rounding of L."""
+        cache = self._preconditioner()
+        lt = cache[1]
+        if lt is None:
+            return None
+        if getattr(self, "_ciq_cache", None) is None or self._ciq_cache[0] is not cache:
+            u, tr_e, st = self._plan().ciq_precond_build(lt)
+            if st != 0:
+                self._ciq_cache = (cache, None)
+            else:
+                tr_k = tr_e + float(lt.double().square().sum())
+                self._ciq_cache = (cache, (u, 0.5, 2.0 * (1.0 + max(tr_e, 1e-6 * tr_k) / self._noise_floor())))
+        return self._ciq_cache[1]
 
     def _probes(self, lt, tp):
         n = self.shape[0]

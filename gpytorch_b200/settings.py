@@ -114,6 +114,16 @@ class ciq_samples(_feature_flag):
     _default = False
 
 
+class ciq_preconditioner(_feature_flag):
+    """With ciq_samples on, run CIQ on A = F^-1 K_hat F^-T, F F^T = P the pivoted-Cholesky preconditioner of the solves (same knobs:
+    max_preconditioner_size, min_preconditioning_size, preconditioner_tolerance), and return F A^{1/2} xi (off by default).
+    msMINRES then needs about sqrt(kappa(A)) instead of sqrt(kappa(K_hat)) iterations.  The draw has the same distribution
+    N(0, K_hat) but is a different root applied to the same xi: off, samples are K_hat^{1/2} xi, continuous in the
+    hyper-parameters (common random numbers across a sweep); on, they jump where the pivot order changes.  No effect where the
+    solves have no preconditioner (SKI, no noise, n < min_preconditioning_size, max_preconditioner_size(0), a failed build)."""
+    _default = False
+
+
 class num_contour_quadrature(_value_context):
     """Quadrature points Q of the CIQ square root (linear_operator settings; default 15)."""
     _global_value = 15

@@ -170,6 +170,19 @@ int gp_lanczos(gp_plan* plan, const float* INIT, int max_iter, float tol, float*
 int gp_ciq_sqrt_matmul(gp_plan* plan, const float* B, int64_t ldb, int t, const double* tau, const double* w, int Q,
                        float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out, float* resid_out);
 
+/* Split factor of the pivoted-Cholesky preconditioner P = L L^T + D for the CIQ sampler, from Lt [k, n] (1 <= k <= 128):
+ * U [n, k] with F^-1 = (I - U U^T) D^-1/2 for F = D^1/2 (I + M M^T)^1/2, M = D^-1/2 L (eigh of L^T D^-1 L in fp64 on the host);
+ * *trace_resid_out = tr(K - L L^T) in fp64.  Needs noise > 0 (all d > 0); square, unsharded, non-SKI plans.
+ * A non-finite Gram returns GP_W_PIVCHOL_NAN (the caller drops the preconditioner). */
+int gp_ciq_precond_build(gp_plan* plan, const float* Lt, int k, float* U, double* trace_resid_out);
+
+/* Preconditioned CIQ: OUT = K_hat F^-T sum_q w_q (A + tau_q I)^-1 B with A = F^-1 K_hat F^-T and U [n, k] from
+ * gp_ciq_precond_build, i.e. OUT ~= F A^{1/2} B ~ N(0, K_hat) for B ~ N(0, I) (a different root than gp_ciq_sqrt_matmul's).
+ * Arguments, status codes and the stop rule (on A's shifted residuals) as gp_ciq_sqrt_matmul. */
+int gp_ciq_sqrt_matmul_precond(gp_plan* plan, const float* B, int64_t ldb, int t, const float* U, int k, const double* tau,
+                               const double* w, int Q, float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out,
+                               float* resid_out);
+
 /* one-shot: MultivariateNormal.log_prob (distributions/multivariate_normal.py:221-252) through
  * inv_quad_logdet (:249), i.e. pivoted Cholesky -> preconditioner -> probes -> mBCG -> SLQ. */
 typedef struct gp_mll_opts {

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """sample_bench.py -- CIQ sampling (gp_ciq_sqrt_matmul, csrc/minres.cu) at three workloads, one JSON file.
 
-    python tools/sample_bench.py --out sample_bench.json [--reps 3] [--skip c3,c5]
+    python tools/sample_bench.py --out sample_bench.json [--reps 3] [--skip c3,c5] [--precond-rank 0,100]
 
 Workloads (Q = 15 quadrature points, msMINRES tolerance 1e-4, 16 samples, X ~ U[0,1]^{N x d}, outputscale 1, noise 0.1):
   c2  N = 50 000,  d = 10, RBF,        lengthscale 1
@@ -11,6 +11,10 @@ For each: ms for 16 samples (CUDA events; the L2 is evicted by a 192 MiB memset 
 outside the timed region), msMINRES iterations, the quadrature interval (m, M), ms per iteration from the slope between
 fixed 10- and 30-iteration runs next to the fused K.V launch alone (gp_time_kmv_kernel), and kernel launches per iteration from
 the same two runs.  At c2 it also times dense fp32 Cholesky sampling of the same xi and reports the largest difference.
+--precond-rank takes a comma-separated list of ranks k (default 0: the unpreconditioned run only).  For k > 0 the run uses the
+split preconditioner of settings.ciq_preconditioner (gp_ciq_sqrt_matmul_precond) and also reports k, the build time (pivoted
+Cholesky + gp_ciq_precond_build, CUDA events) and the trace interval [m, M]; c5 (SKI) has no pivoted-Cholesky preconditioner and
+is reported as skipped.
 """
 from __future__ import annotations
 
@@ -73,25 +77,41 @@ def _timed(fn, flush, reps):
     return out, min(ms), ms
 
 
-def run(name, cfg, reps, dev):
+def run(name, cfg, reps, dev, rank=0):
     gen = torch.Generator().manual_seed(0)
     op = _operator(cfg, dev, gen)
     n, s, Q, tol = cfg["n"], 16, 15, 1e-4
     xi = torch.randn(n, s, generator=gen).to(dev)
     flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)
     plan = op._sampling_plan()
-    m, M = op._ciq_bounds(plan, xi[:, 0])
+    u, extra = None, {}
+    if rank == 0:
+        m, M = op._ciq_bounds(plan, xi[:, 0])
+    else:
+        with settings.max_preconditioner_size(rank):
+            pre = op._ciq_precond()
+            if pre is None:
+                raise RuntimeError(f"{name}: no preconditioner at rank {rank}")
+            u, m, M = pre
+
+            def build():
+                lt, _, _ = plan.pivoted_cholesky(rank, settings.preconditioner_tolerance.value())
+                return plan.ciq_precond_build(lt)
+
+            build()                                                         # warm-up
+            _, build_ms, _ = _timed(build, flush, reps)
+        extra = {"precond_rank": int(u.size(1)), "build_ms_pivchol_plus_factor": build_ms}
     tau, w = contour_quadrature(m, M, Q)
-    plan.ciq_sqrt_matmul(xi, tau, w, tol, 1000)                         # warm-up
-    (out, info), best, all_ms = _timed(lambda: plan.ciq_sqrt_matmul(xi, tau, w, tol, 1000), flush, reps)
-    # the full public call (interval estimate included), same xi
-    with settings.ciq_samples(True):
+    plan.ciq_sqrt_matmul(xi, tau, w, tol, 1000, precond_u=u)               # warm-up
+    (out, info), best, all_ms = _timed(lambda: plan.ciq_sqrt_matmul(xi, tau, w, tol, 1000, precond_u=u), flush, reps)
+    # the full public call, same xi: the interval estimate included (k = 0), the cached factor reused (k > 0)
+    with settings.ciq_samples(True), settings.ciq_preconditioner(rank > 0), settings.max_preconditioner_size(max(rank, 1)):
         _, api_ms, _ = _timed(lambda: op._ciq_samples(xi), flush, reps)
     # per-iteration cost and launches: slope between fixed-length runs (tol = 0 never stops early)
     per = {}
     for k in (10, 30):
         l0 = plan.launches()
-        _, t_k, _ = _timed(lambda: plan.ciq_sqrt_matmul(xi, tau, w, 0.0, k, warn=False), flush, reps)
+        _, t_k, _ = _timed(lambda: plan.ciq_sqrt_matmul(xi, tau, w, 0.0, k, warn=False, precond_u=u), flush, reps)
         per[k] = (t_k, plan.launches() - l0)
     ms_it = (per[30][0] - per[10][0]) / 20
     launches_it = (per[30][1] - per[10][1]) / (20 * reps)
@@ -99,10 +119,10 @@ def run(name, cfg, reps, dev):
     res = {"n": n, "d": cfg["d"], "kind": cfg["kind"], "samples": s, "Q": Q, "tol": tol, "ms_16_samples": best, "ms_all_reps": all_ms,
            "ms_16_samples_api_incl_bounds": api_ms, "iters": info.iters, "m": m, "M": M, "ms_per_iter": ms_it,
            "ms_kmv_launch": kmv_ms, "launches_per_iter": launches_it,
-           "max_resid": max(max(r) for r in info.residual_norms)}
+           "max_resid": max(max(r) for r in info.residual_norms), **extra}
     if "grid" in cfg:
         res["grid"] = [cfg["grid"]] * cfg["d"]
-    if name == "c2":
+    if name == "c2" and rank == 0:
         dense = op.to_dense()
         torch.cuda.synchronize()
 
@@ -126,14 +146,21 @@ def main():
     ap.add_argument("--out", default="sample_bench.json")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip", default="")
+    ap.add_argument("--precond-rank", default="0", help="comma-separated preconditioner ranks k (0: unpreconditioned)")
     a = ap.parse_args()
+    ranks = [int(r) for r in a.precond_rank.split(",")]
     dev = torch.device("cuda:0")
     result = {"gpu": _gpu_info(), "l2_policy": "192 MiB memset before every timed call, outside the timed region", "workloads": {}}
     for name, cfg in WORKLOADS.items():
         if name in a.skip.split(","):
             continue
-        result["workloads"][name] = run(name, cfg, a.reps, dev)
-        print(name, json.dumps(result["workloads"][name]), flush=True)
+        for rank in ranks:
+            key = name if rank == 0 else f"{name}_k{rank}"
+            if rank > 0 and "grid" in cfg:
+                result["workloads"][key] = {"skipped": "SKI has no pivoted-Cholesky preconditioner"}
+            else:
+                result["workloads"][key] = run(name, cfg, a.reps, dev, rank)
+            print(key, json.dumps(result["workloads"][key]), flush=True)
     with open(a.out, "w") as f:
         json.dump(result, f, indent=1)
     print(json.dumps(result))
