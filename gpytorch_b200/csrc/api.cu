@@ -18,10 +18,6 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,
-             int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
-             int* tridiag_size, float* resid_out);
-
 __global__ void concat_rhs_kernel(const float* __restrict__ probes, int tp, const float* __restrict__ y, int64_t n,
                                   float* __restrict__ rhs, float* __restrict__ pn_part) {
   // rhs[r][0..tp) = probes (normalised later), rhs[r][tp] = y
@@ -52,8 +48,6 @@ __global__ void extract_col_kernel(const float* __restrict__ solves, int ld, int
   int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r < n) out[r] = solves[r * ld + col];
 }
-
-int nccl_allreduce_double(gp_comm* c, double* buf, size_t count, cudaStream_t st);
 
 }  // namespace gp
 
@@ -93,8 +87,8 @@ extern "C" int gp_plan_create(gp_plan** out, int device, void* stream) {
   p->device = device;
   p->stream = reinterpret_cast<cudaStream_t>(stream);
   p->n_sm = prop.multiProcessorCount;
-  GP_CUDA(cudaMallocHost(&p->pinned, 32768));
-  memset(p->pinned, 0, 32768);
+  GP_CUDA(cudaMallocHost(&p->pinned, PINNED_BYTES));
+  memset(p->pinned, 0, PINNED_BYTES);
   *out = p;
   return GP_OK;
 }
@@ -332,7 +326,7 @@ extern "C" int gp_mll(gp_plan* p, const float* y_minus_mean, const float* eps1, 
     extract_col_kernel<<<(unsigned)cdiv(n, 256), 256, 0, st>>>(solves, t, tp, n, solve_out);
     p->launches++;
   }
-  double* h = reinterpret_cast<double*>(reinterpret_cast<char*>(p->pinned) + 4096);
+  double* h = reinterpret_cast<double*>(static_cast<char*>(p->pinned) + PIN_SCALARS);
   GP_CUDA(cudaMemcpyAsync(h, iq_part, sizeof(double) * 64, cudaMemcpyDeviceToHost, st));
   GP_CUDA(cudaStreamSynchronize(st));
   double iq = 0.0;

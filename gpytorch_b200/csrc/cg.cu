@@ -26,16 +26,11 @@
 #include <algorithm>
 #include <dlfcn.h>
 
-#include "gp_common.cuh"
+#include "rowpass.cuh"
 
 namespace gp {
 
-constexpr int CG_THREADS = 256;
-constexpr int CG_ROWS = 64;   // rows per pass of a CTA (4 float4 column groups x 64 row lanes)
 constexpr int KMAX = 128;     // max preconditioner rank handled by the fused apply
-
-int nccl_allreduce_double(gp_comm* c, double* buf, size_t count, cudaStream_t st);   // comm.cu
-int nccl_allgather_float(gp_comm* c, float* buf, size_t count_per_rank, cudaStream_t st);
 
 // shared-memory row pitch of a staged W chunk: a multiple of 4 floats with pitch % 32 == 4, so that the 8 rows a warp touches
 // with one LDS.128 fall into 8 different 4-bank groups (conflict free)
@@ -43,22 +38,6 @@ static inline int w_pitch(int k) {
   int p = (k + 3) & ~3;
   while (p % 32 != 4) p += 4;
   return p;
-}
-
-__device__ __forceinline__ void block_reduce_cols(float4 acc, float* red /*[CG_ROWS][TP]*/, float* out /*[TP] global*/) {
-  // thread layout: cg = tid & 3 (float4 column group), rl = tid >> 2 (row lane)
-  const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
-  reinterpret_cast<float4*>(red)[rl * 4 + cg] = acc;
-  __syncthreads();
-  for (int s = CG_ROWS / 2; s > 0; s >>= 1) {
-    if (rl < s) {
-      float4 a = reinterpret_cast<float4*>(red)[rl * 4 + cg];
-      float4 b = reinterpret_cast<float4*>(red)[(rl + s) * 4 + cg];
-      reinterpret_cast<float4*>(red)[rl * 4 + cg] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-    }
-    __syncthreads();
-  }
-  if (tid < TP) out[tid] = red[tid];
 }
 
 // sum G partial vectors of length L (fp32) into fp64, fixed order.  Block = 32 outputs x 8 partial groups.
@@ -91,10 +70,10 @@ __global__ void __launch_bounds__(32 * SUM_GROUPS) cg_sum_kernel(const float* __
 }
 
 __global__ void cg_rhs_sq_kernel(const float* __restrict__ RHS, int64_t ldr, int t, int64_t n, float* __restrict__ part) {
-  __shared__ __align__(16) float red[CG_ROWS * TP];
+  __shared__ __align__(16) float red[RP_ROWS * TP];
   const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
   float4 acc = make_float4(0, 0, 0, 0);
-  for (int64_t r = (int64_t)blockIdx.x * CG_ROWS + rl; r < n; r += (int64_t)gridDim.x * CG_ROWS) {
+  for (int64_t r = (int64_t)blockIdx.x * RP_ROWS + rl; r < n; r += (int64_t)gridDim.x * RP_ROWS) {
     float v[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
@@ -128,7 +107,7 @@ __global__ void cg_init_kernel(const float* __restrict__ RHS, int64_t ldr, int t
     }
   }
   __syncthreads();
-  for (int64_t r = (int64_t)blockIdx.x * CG_ROWS + rl; r < n; r += (int64_t)gridDim.x * CG_ROWS) {
+  for (int64_t r = (int64_t)blockIdx.x * RP_ROWS + rl; r < n; r += (int64_t)gridDim.x * RP_ROWS) {
     float v[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
@@ -146,13 +125,13 @@ __device__ __forceinline__ void stage_w(const float* __restrict__ W, int k, int 
   const int tot = nr * k;
   const int tid = threadIdx.x;
   if ((k & 3) == 0) {
-    for (int e = tid * 4; e < tot; e += CG_THREADS * 4) {
+    for (int e = tid * 4; e < tot; e += RP_THREADS * 4) {
       const float4 v4 = *reinterpret_cast<const float4*>(wsrc + e);
       const int rr = e / k, kk = e - rr * k;
       *reinterpret_cast<float4*>(&Ws[rr * wp + kk]) = v4;
     }
   } else {
-    for (int e = tid; e < tot; e += CG_THREADS) {
+    for (int e = tid; e < tot; e += RP_THREADS) {
       const int rr = e / k, kk = e - rr * k;
       Ws[rr * wp + kk] = wsrc[e];
     }
@@ -165,7 +144,7 @@ __device__ __forceinline__ void stage_w(const float* __restrict__ W, int k, int 
 // tiles from the W chunk staged in shared memory.
 // out: part[blockIdx][0..16) = sum p.V (FINISH only) ; part[blockIdx][16 + kk*16 + c] = sum_r W[r][kk] X[r][c]
 template <bool FINISH>
-__global__ void __launch_bounds__(CG_THREADS)
+__global__ void __launch_bounds__(RP_THREADS)
 cg_finishv_wtv_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_pad, float os, const float* __restrict__ pscale, float noise,
                       const float* __restrict__ dvec, const float* __restrict__ P, float* __restrict__ V,
                       const float* __restrict__ Xin, const float* __restrict__ W, int k, int wp, int64_t n,
@@ -173,8 +152,8 @@ cg_finishv_wtv_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_
   if (done && *done) return;
   extern __shared__ __align__(16) float sh[];
   float* Xs = sh;                       // [64][16]
-  float* red = sh + CG_ROWS * TP;       // [64][16]
-  float* Ws = red + CG_ROWS * TP;       // [64][wp]  (reused as the [128][16] exchange buffer at the end)
+  float* red = sh + RP_ROWS * TP;       // [64][16]
+  float* Ws = red + RP_ROWS * TP;       // [64][wp]  (reused as the [128][16] exchange buffer at the end)
   const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
   const int kg = (tid >> 2) & 31, half = tid >> 7;
   const bool act = kg * 4 < k;
@@ -185,10 +164,10 @@ cg_finishv_wtv_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_
   for (int a = 0; a < 4; ++a)
 #pragma unroll
     for (int b = 0; b < 4; ++b) wacc[a][b] = 0.f;
-  const int64_t nchunk = cdiv(n, CG_ROWS);
+  const int64_t nchunk = cdiv(n, RP_ROWS);
   for (int64_t ch = blockIdx.x; ch < nchunk; ch += gridDim.x) {
-    const int64_t r0 = ch * CG_ROWS;
-    const int nr = (int)min((int64_t)CG_ROWS, n - r0);
+    const int64_t r0 = ch * RP_ROWS;
+    const int nr = (int)min((int64_t)RP_ROWS, n - r0);
     __syncthreads();   // previous chunk's phase 2 has finished with Xs / Ws
     if (k > 0) stage_w(W, k, wp, r0, nr, Ws);
     // phase 1: X rows
@@ -197,24 +176,8 @@ cg_finishv_wtv_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_
       float4 x = make_float4(0, 0, 0, 0);
       if (rl < nr) {
         if (FINISH) {
-          float4 s = make_float4(poison, poison, poison, poison);
-          float osr = os;
-          if (pscale) {   // kernel sum: slot sp belongs to the term with outputscale pscale[sp]
-            for (int sp = 0; sp < nsplit; ++sp) {
-              const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
-              const float w = pscale[sp];
-              s.x = fmaf(w, a.x, s.x); s.y = fmaf(w, a.y, s.y); s.z = fmaf(w, a.z, s.z); s.w = fmaf(w, a.w, s.w);
-            }
-            osr = 1.f;
-          } else {
-            for (int sp = 0; sp < nsplit; ++sp) {
-              const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
-              s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
-            }
-          }
+          x = khat_row(kpart, nsplit, rows_pad, os, pscale, poison, P, dvec, noise, r, cg);
           const float4 p = reinterpret_cast<const float4*>(P)[r * 4 + cg];
-          const float d = dvec ? dvec[r] : noise;
-          x = make_float4(fmaf(d, p.x, osr * s.x), fmaf(d, p.y, osr * s.y), fmaf(d, p.z, osr * s.z), fmaf(d, p.w, osr * s.w));
           reinterpret_cast<float4*>(V)[r * 4 + cg] = x;
           acc.x = fmaf(p.x, x.x, acc.x); acc.y = fmaf(p.y, x.y, acc.y); acc.z = fmaf(p.z, x.z, acc.z); acc.w = fmaf(p.w, x.w, acc.w);
         } else {
@@ -273,7 +236,7 @@ cg_finishv_wtv_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_
 // Z = a_r R - s W w with (a_r, s) = (1/sigma^2, 1/sigma^2) for the constant diagonal, (1/d_r, 1) for a per-row diagonal whose
 // factor W is pre-scaled (pivchol.cu).  Without a preconditioner (k == 0) Z aliases R and z.r = r.r.
 template <bool INIT>
-__global__ void __launch_bounds__(CG_THREADS, 2)   // sm_90 ptxas otherwise caps the INIT variant at 64 registers and spills
+__global__ void __launch_bounds__(RP_THREADS, 2)   // sm_90 ptxas otherwise caps the INIT variant at 64 registers and spills
 cg_update_precond_kernel(const double* __restrict__ sums1, int iter, float eps, const float* __restrict__ P,
                          const float* __restrict__ V, float* __restrict__ U, float* __restrict__ R, float* __restrict__ Z,
                          const float* __restrict__ W, int k, int wp, const double* __restrict__ wprev,
@@ -282,8 +245,8 @@ cg_update_precond_kernel(const double* __restrict__ sums1, int iter, float eps, 
   if (!INIT && st->done) return;
   extern __shared__ __align__(16) float sh[];
   float* red = sh;                                  // [64][16]
-  float* Xs = red + CG_ROWS * TP;                   // [64][16] the new residual rows of the chunk
-  float* ws = Xs + CG_ROWS * TP;                    // [k][16] w (float)
+  float* Xs = red + RP_ROWS * TP;                   // [64][16] the new residual rows of the chunk
+  float* ws = Xs + RP_ROWS * TP;                    // [k][16] w (float)
   float* Ws = ws + (size_t)k * TP;                  // [64][wp]  (reused as the [128][16] exchange buffer at the end)
   __shared__ float alpha_s[TP];
   const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
@@ -310,16 +273,16 @@ cg_update_precond_kernel(const double* __restrict__ sums1, int iter, float eps, 
     alpha_s[tid] = a;
   }
   __syncthreads();
-  for (int e = tid; e < k * TP; e += CG_THREADS) {
+  for (int e = tid; e < k * TP; e += RP_THREADS) {
     const double w = INIT ? sums1[TP + e] : wprev[e] - (double)alpha_s[e & (TP - 1)] * sums1[TP + e];
     ws[e] = (float)w;
   }
   const float4 al = reinterpret_cast<float4*>(alpha_s)[cg];
   float4 arr = make_float4(0, 0, 0, 0), azr = make_float4(0, 0, 0, 0);
-  const int64_t nchunk = cdiv(n, CG_ROWS);
+  const int64_t nchunk = cdiv(n, RP_ROWS);
   for (int64_t ch = blockIdx.x; ch < nchunk; ch += gridDim.x) {
-    const int64_t r0 = ch * CG_ROWS;
-    const int nr = (int)min((int64_t)CG_ROWS, n - r0);
+    const int64_t r0 = ch * RP_ROWS;
+    const int nr = (int)min((int64_t)RP_ROWS, n - r0);
     __syncthreads();   // ws ready / previous chunk done with Ws
     if (k > 0) stage_w(W, k, wp, r0, nr, Ws);
     const int64_t r = r0 + rl;
@@ -411,7 +374,7 @@ cg_update_precond_kernel(const double* __restrict__ sums1, int iter, float eps, 
 // INIT: beta = 0 (P = Z), gamma[0] = z.r, no bookkeeping.
 constexpr int V_TILE_FLOATS_CG = (2 * TILE_J * TP * 4 + TILE_J * TP * 2) / 4;  // 2560 floats per 64-row tile
 template <bool INIT>
-__global__ void __launch_bounds__(CG_THREADS)
+__global__ void __launch_bounds__(RP_THREADS)
 cg_dir_pack_kernel(const double* __restrict__ sums2, int iter, float eps,
                    float stop_after, float tol, int t, int n_tridiag, int n_tridiag_iter, int max_iter,
                    const float* __restrict__ Z, float* __restrict__ P, int64_t n, int64_t nchunk_pack,
@@ -557,12 +520,11 @@ __global__ void cg_finalize_kernel(const float* __restrict__ U, const CgState* _
   if (c < t) S[r * lds + c] = U[idx] * st->rhs_norm[c];
 }
 
-// the two reductions above, for the multi-shift MINRES loop (minres.cu)
 void cg_sum_launch(const float* in, int G, int L, double* out, const int* done, cudaStream_t st) {
   cg_sum_kernel<<<(unsigned)cdiv(L, 32), 32 * SUM_GROUPS, 0, st>>>(in, G, L, out, done);
 }
 void cg_rhs_sq_launch(const float* RHS, int64_t ldr, int t, int64_t n, float* part, int G, cudaStream_t st) {
-  cg_rhs_sq_kernel<<<G, CG_THREADS, 0, st>>>(RHS, ldr, t, n, part);
+  cg_rhs_sq_kernel<<<G, RP_THREADS, 0, st>>>(RHS, ldr, t, n, part);
 }
 
 static int allreduce(gp_plan* p, double* buf, size_t count) {
@@ -600,9 +562,8 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   const int wp = precond ? w_pitch(k) : 0;
   // CTAs per SM of the row-pass kernels: 2 with a preconditioner (the W chunk staged in shared memory bounds residency; 3 or 4
   // measured no faster at C2), 8 without one (pure streaming over the vectors: N = 10^6 rows at BASELINE C5)
-  static const int grid_mult_env = getenv("GP_CG_GRID_MULT") ? std::max(1, atoi(getenv("GP_CG_GRID_MULT"))) : 0;
-  const int grid_mult = grid_mult_env ? grid_mult_env : (precond ? 2 : 8);
-  const int G = (int)std::min<int64_t>(cdiv(n, CG_ROWS), (int64_t)grid_mult * p->n_sm);
+  const int grid_mult = precond ? 2 : 8;
+  const int G = (int)std::min<int64_t>(cdiv(n, RP_ROWS), (int64_t)grid_mult * p->n_sm);
   const int L1 = TP + k * TP;           // message 1: pV | W^T V
   const float* dvec = p->noise_diag ? p->noise_diag + p->row_begin : nullptr;
   GP_REQUIRE(!precond || dvec != nullptr || p->noise > 0.f, GP_E_SHAPE, "the preconditioner needs noise > 0");
@@ -630,16 +591,12 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   CgState* S = p->state.as<CgState>();
   const int* done = &S->done;
   const float inv_noise = p->noise > 0.f ? 1.f / p->noise : 0.f;
-  const size_t sh_b = sizeof(float) * ((size_t)2 * CG_ROWS * TP + std::max<size_t>((size_t)CG_ROWS * wp, 128 * TP));
-  const size_t sh_d = sizeof(float) * ((size_t)2 * CG_ROWS * TP + (size_t)k * TP + std::max<size_t>((size_t)CG_ROWS * wp, 128 * TP));
-  static bool attr_done[64] = {};
-  if (!attr_done[p->device & 63]) {
-    GP_CUDA(cudaFuncSetAttribute(cg_finishv_wtv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    GP_CUDA(cudaFuncSetAttribute(cg_finishv_wtv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    GP_CUDA(cudaFuncSetAttribute(cg_update_precond_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    GP_CUDA(cudaFuncSetAttribute(cg_update_precond_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr_done[p->device & 63] = true;
-  }
+  const size_t sh_b = sizeof(float) * ((size_t)2 * RP_ROWS * TP + std::max<size_t>((size_t)RP_ROWS * wp, 128 * TP));
+  const size_t sh_d = sizeof(float) * ((size_t)2 * RP_ROWS * TP + (size_t)k * TP + std::max<size_t>((size_t)RP_ROWS * wp, 128 * TP));
+  GP_CHECK(opt_in_smem<cg_finishv_wtv_kernel<true>>(p->device, 100 * 1024));
+  GP_CHECK(opt_in_smem<cg_finishv_wtv_kernel<false>>(p->device, 100 * 1024));
+  GP_CHECK(opt_in_smem<cg_update_precond_kernel<true>>(p->device, 100 * 1024));
+  GP_CHECK(opt_in_smem<cg_update_precond_kernel<false>>(p->device, 100 * 1024));
   if (n_tridiag > 0) GP_CUDA(cudaMemsetAsync(TMAT, 0, sizeof(float) * (size_t)n_tridiag * max_tridiag_iter * max_tridiag_iter, st));
 
   // the direction block is written straight into the packed K.V tiles when this rank owns all rows and the tensor-core
@@ -648,7 +605,7 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   const bool fuse_pack = tc && !sharded;
   float* Vt = fuse_pack ? p->Vtiles.as<float>() : nullptr;
   const int64_t nchunk_pack = fuse_pack ? p->ntile_j * (TILE_J / 4) : 0;
-  const int Gd = (int)std::min<int64_t>(cdiv(std::max<int64_t>(nchunk_pack, cdiv(n, (int64_t)4)) * 4, (int64_t)CG_THREADS), 4 * p->n_sm);
+  const int Gd = (int)std::min<int64_t>(cdiv(std::max<int64_t>(nchunk_pack, cdiv(n, (int64_t)4)) * 4, (int64_t)RP_THREADS), 4 * p->n_sm);
   auto kmv = [&]() -> int {
     if (fuse_pack) return kmv_tc_launch(p, done);
     if (sharded) GP_CHECK(nccl_allgather_float(p->comm, Pfull, (size_t)n * TP, st));
@@ -656,75 +613,57 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   };
 
   // ---- init: normalise rhs, R, U ; w = W^T R ; Z = P^-1 R ; P = Z ; gamma = z.r ----
-  cg_rhs_sq_kernel<<<G, CG_THREADS, 0, st>>>(RHS, ldr, t, n, red1);
-  cg_sum_kernel<<<1, 32 * SUM_GROUPS, 0, st>>>(red1, G, TP, sums0, nullptr);
+  cg_rhs_sq_launch(RHS, ldr, t, n, red1, G, st);
+  cg_sum_launch(red1, G, TP, sums0, nullptr, st);
   GP_CHECK(allreduce(p, sums0, TP));
-  cg_init_kernel<<<G, CG_THREADS, 0, st>>>(RHS, ldr, t, n, sums0, eps, U, R, S);
+  cg_init_kernel<<<G, RP_THREADS, 0, st>>>(RHS, ldr, t, n, sums0, eps, U, R, S);
   p->launches += 3;
   if (precond) {
-    cg_finishv_wtv_kernel<false><<<G, CG_THREADS, sh_b, st>>>(nullptr, 0, 0, 0.f, nullptr, 0.f, nullptr, nullptr, nullptr, R, W, k, wp, n, red1, L1,
+    cg_finishv_wtv_kernel<false><<<G, RP_THREADS, sh_b, st>>>(nullptr, 0, 0, 0.f, nullptr, 0.f, nullptr, nullptr, nullptr, R, W, k, wp, n, red1, L1,
                                                            nullptr, p->xbad);
-    cg_sum_kernel<<<(unsigned)cdiv(L1, 32), 32 * SUM_GROUPS, 0, st>>>(red1, G, L1, sums1, nullptr);
+    cg_sum_launch(red1, G, L1, sums1, nullptr, st);
     GP_CHECK(allreduce(p, sums1, L1));
     p->launches += 2;
   }
-  cg_update_precond_kernel<true><<<G, CG_THREADS, sh_d, st>>>(sums1, 0, eps, nullptr, nullptr, U, R, Z, W, k, wp, nullptr, inv_noise, dvec, n, S,
+  cg_update_precond_kernel<true><<<G, RP_THREADS, sh_d, st>>>(sums1, 0, eps, nullptr, nullptr, U, R, Z, W, k, wp, nullptr, inv_noise, dvec, n, S,
                                                              red2, L2);
-  cg_sum_kernel<<<(unsigned)cdiv(L2, 32), 32 * SUM_GROUPS, 0, st>>>(red2, G, L2, sums2, nullptr);
+  cg_sum_launch(red2, G, L2, sums2, nullptr, st);
   GP_CHECK(allreduce(p, sums2, L2));
-  cg_dir_pack_kernel<true><<<Gd, CG_THREADS, 0, st>>>(sums2, 0, eps, stop_after, tol, t, n_tridiag, n_tridiag_iter, max_iter, Z, P, n,
+  cg_dir_pack_kernel<true><<<Gd, RP_THREADS, 0, st>>>(sums2, 0, eps, stop_after, tol, t, n_tridiag, n_tridiag_iter, max_iter, Z, P, n,
                                                      nchunk_pack, Vt, S, TMAT, max_tridiag_iter);
   p->launches += 3;
   GP_CUDA(cudaGetLastError());
 
   // ---- iterations ----
-  int* h_done = reinterpret_cast<int*>(p->pinned);  // [0..3] ring of done flags
-  cudaEvent_t ev[2];
-  GP_CUDA(cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming));
-  GP_CUDA(cudaEventCreateWithFlags(&ev[1], cudaEventDisableTiming));
   const int first_stop = std::max(std::min(10, max_iter - 1), n_tridiag ? std::min(n_tridiag_iter, max_iter - 1) : 0);
+  SolverLoop loop(p, "mBCG", done, first_stop);
+  GP_CHECK(loop.create_events());
   int status = GP_OK;
-  int kk = 0;
   bool finished = false;
-  for (kk = 0; kk < max_iter && !finished; ++kk) {
+  for (int kk = 0; kk < max_iter && !finished; ++kk) {
     if ((status = kmv()) != GP_OK) break;
-    cg_finishv_wtv_kernel<true><<<G, CG_THREADS, sh_b, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p), p->noise, dvec, P, V,
+    cg_finishv_wtv_kernel<true><<<G, RP_THREADS, sh_b, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p), p->noise, dvec, P, V,
                                                           nullptr, W, k, wp, n, red1, L1, done, p->xbad);
-    cg_sum_kernel<<<(unsigned)cdiv(L1, 32), 32 * SUM_GROUPS, 0, st>>>(red1, G, L1, sums1, done);
+    cg_sum_launch(red1, G, L1, sums1, done, st);
     if ((status = allreduce(p, sums1, L1)) != GP_OK) break;
     // w_kk = W^T R_kk: the direct product shipped in message 2 of the previous launch of this kernel (start-up pass for kk = 0)
-    cg_update_precond_kernel<false><<<G, CG_THREADS, sh_d, st>>>(sums1, kk, eps, P, V, U, R, Z, W, k, wp, sums2 + 2 * TP, inv_noise, dvec, n, S,
+    cg_update_precond_kernel<false><<<G, RP_THREADS, sh_d, st>>>(sums1, kk, eps, P, V, U, R, Z, W, k, wp, sums2 + 2 * TP, inv_noise, dvec, n, S,
                                                                 red2, L2);
-    cg_sum_kernel<<<(unsigned)cdiv(L2, 32), 32 * SUM_GROUPS, 0, st>>>(red2, G, L2, sums2, done);
+    cg_sum_launch(red2, G, L2, sums2, done, st);
     if ((status = allreduce(p, sums2, L2)) != GP_OK) break;
-    cg_dir_pack_kernel<false><<<Gd, CG_THREADS, 0, st>>>(sums2, kk, eps, stop_after, tol, t, n_tridiag, n_tridiag_iter, max_iter, Z, P, n,
+    cg_dir_pack_kernel<false><<<Gd, RP_THREADS, 0, st>>>(sums2, kk, eps, stop_after, tol, t, n_tridiag, n_tridiag_iter, max_iter, Z, P, n,
                                                         nchunk_pack, Vt, S, TMAT, max_tridiag_iter);
     p->launches += 5;
-    if (kk >= first_stop) {
-      // look-ahead stop check: read the flag of iteration kk after iteration kk+1 has been enqueued
-      cudaMemcpyAsync(&h_done[kk & 1], &S->done, sizeof(int), cudaMemcpyDeviceToHost, st);
-      cudaEventRecord(ev[kk & 1], st);
-      if (kk > first_stop) {
-        cudaEventSynchronize(ev[(kk - 1) & 1]);
-        if (h_done[(kk - 1) & 1]) finished = true;
-      }
-    }
+    finished = loop.finished(kk);
   }
-  cudaError_t le = cudaGetLastError();
-  if (status == GP_OK && le != cudaSuccess) {
-    set_error("mBCG launch failed: %s", cudaGetErrorString(le));
-    status = GP_E_CUDA;
-  }
+  status = loop.launch_status(status);
   if (status == GP_OK) {
     cg_finalize_kernel<<<(unsigned)cdiv(n * TP, 256), 256, 0, st>>>(U, S, n, t, SOLVES, lds);
     p->launches += 1;
-    CgState* hs = reinterpret_cast<CgState*>(reinterpret_cast<char*>(p->pinned) + 64);
+    CgState* hs = reinterpret_cast<CgState*>(static_cast<char*>(p->pinned) + PIN_CG_STATE);
     cudaMemcpyAsync(hs, S, sizeof(CgState), cudaMemcpyDeviceToHost, st);
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) {
-      set_error("mBCG execution failed: %s", cudaGetErrorString(se));
-      status = GP_E_CUDA;
-    } else {
+    status = loop.sync();
+    if (status == GP_OK) {
       if (iters_out) *iters_out = hs->done ? hs->iters : max_iter;
       if (tridiag_size) *tridiag_size = n_tridiag ? hs->last_tridiag_iter + 1 : 0;
       if (resid_out)
@@ -741,8 +680,6 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
       }
     }
   }
-  cudaEventDestroy(ev[0]);
-  cudaEventDestroy(ev[1]);
   return status;
 }
 

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -94,6 +95,38 @@ struct CgState {
   int nan_flag;
 };
 
+// ---- pinned host scratch (gp_plan::pinned): one fixed byte offset per user ------------------------------------------------
+constexpr size_t PINNED_BYTES = 32768;
+constexpr size_t PIN_DONE_RING = 0;     // int[2]: look-ahead done flags of the mBCG / msMINRES loops (rowpass.cuh)
+constexpr size_t PIN_CG_STATE = 64;     // CgState read back after mBCG (cg.cu)
+constexpr size_t PIN_PC_STATE = 2048;   // PcState read back after the pivoted Cholesky (pivchol.cu)
+constexpr size_t PIN_PRECOND = 3072;    // log det, tail, fail flag of gp_precond_build (pivchol.cu)
+constexpr size_t PIN_SLQ = 3200;        // 64 per-probe log-dets + fail flag (slq.cu)
+constexpr size_t PIN_SCALARS = 4096;    // gp_mll: 64 inv-quad partials (api.cu); gp_lanczos: 2 scalars, then from +64 the k + 1
+                                        // Gram-Schmidt coefficients of step k, which run past the end for num_iter >= 3578
+constexpr size_t PIN_CIQ_TW = 8192;     // tau | w of CIQ, 2 Q <= 64 doubles (minres.cu)
+constexpr size_t PIN_CIQ_OUT = 12288;   // msMINRES read-back: residuals, iterations, flags (minres.cu)
+static_assert(PIN_DONE_RING + 2 * sizeof(int) <= PIN_CG_STATE, "done ring overlaps the CgState slot");
+static_assert(PIN_CG_STATE + sizeof(CgState) <= PIN_PC_STATE, "CgState overflows its pinned slot");
+static_assert(PIN_PRECOND + 2 * sizeof(double) + sizeof(int) <= PIN_SLQ, "gp_precond_build read-back overflows its pinned slot");
+static_assert(PIN_SLQ + 64 * sizeof(double) + sizeof(int) <= PIN_SCALARS, "SLQ read-back overflows its pinned slot");
+static_assert(PIN_SCALARS + 64 * sizeof(double) <= PIN_CIQ_TW, "gp_mll read-back overflows its pinned slot");
+
+// Raises KERNEL's dynamic shared-memory limit to `bytes` on `device` the first time any thread asks for it there (plans are
+// driven from several host threads at once); later calls return the first call's result.
+template <auto KERNEL>
+int opt_in_smem(int device, int bytes) {
+  static std::once_flag once[64];
+  static cudaError_t err[64];
+  const int slot = device & 63;
+  std::call_once(once[slot], [&] { err[slot] = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); });
+  if (err[slot] != cudaSuccess) {
+    set_error("cudaFuncSetAttribute(MaxDynamicSharedMemorySize = %d) -> %s", bytes, cudaGetErrorString(err[slot]));
+    return GP_E_CUDA;
+  }
+  return GP_OK;
+}
+
 }  // namespace gp
 
 // SKI / KISS-GP backend state (ski.cu): grid geometry, compact interpolation data, grid work blocks, Toeplitz factors
@@ -155,7 +188,7 @@ struct gp_plan {
   float* vtiles_ext = nullptr;
   gp::DevBuf part_scale;          // [nparts] outputscale of the term that owns each partial slot
   std::vector<float> part_scale_host;
-  void* pinned = nullptr;  // small pinned host scratch
+  void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
 
 namespace gp {
@@ -176,6 +209,11 @@ int ski_bilinear(gp_plan* p, const float* L16, const float* R16, double* total);
 int sum_pack(gp_plan* p);                                               // sum.cu: geometry / buffers of a kernel-sum plan
 int sum_prepare(gp_plan* p);                                            // refresh the per-slot outputscales (no-op for other plans)
 int sum_kmv_launch(gp_plan* p, const float* V16, const int* done_flag); // one launch per term into the parent's partial slots
+int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,   // cg.cu
+             int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
+             int* tridiag_size, float* resid_out);
+int nccl_allreduce_double(gp_comm* c, double* buf, size_t count, cudaStream_t st);                     // comm.cu
+int nccl_allgather_float(gp_comm* c, float* buf, size_t count_per_rank, cudaStream_t st);
 inline float* partial_ptr(gp_plan* p) { return p->partial_ext ? p->partial_ext : p->partial.as<float>(); }
 inline float* vtiles_ptr(gp_plan* p) { return p->vtiles_ext ? p->vtiles_ext : p->Vtiles.as<float>(); }
 // per-slot scales of the finish kernels: nullptr = one outputscale for all slots

@@ -206,12 +206,7 @@ static int launch_tc_kind(gp_plan* p, const int* done_flag) {
   int ns = 0;
   int smem_bytes = tc_smem_bytes(p->KP, &ns);
   GP_REQUIRE(ns >= 2, GP_E_SHAPE, "tensor-core path: smem ring too small for KP=%d", p->KP);
-  static bool attr_done[64] = {};   // function attributes are per device
-  const int dev_slot = p->device & 63;
-  if (!attr_done[dev_slot]) {
-    GP_CUDA(cudaFuncSetAttribute(kmv_tc_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_done[dev_slot] = true;
-  }
+  GP_CHECK(opt_in_smem<kmv_tc_kernel<KIND>>(p->device, 227 * 1024));
   dim3 grid((unsigned)p->ntile_i, (unsigned)p->nsplit);
   kmv_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
       p->XA.as<float>(), p->XB.as<float>(), vtiles_ptr(p), partial_ptr(p), p->KP, ns, p->ntile_j,

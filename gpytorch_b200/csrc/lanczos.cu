@@ -73,9 +73,6 @@ __global__ void lz_gemv_n_kernel(const float* __restrict__ Qt, int m, int64_t n,
 
 __global__ void lz_sqrt_kernel(double* v) { *v = sqrt(*v); }
 
-int nccl_allreduce_double(gp_comm* c, double* buf, size_t count, cudaStream_t st);   // comm.cu
-int nccl_allgather_float(gp_comm* c, float* buf, size_t count_per_rank, cudaStream_t st);
-
 }  // namespace gp
 
 using namespace gp;
@@ -103,7 +100,7 @@ extern "C" int gp_lanczos(gp_plan* p, const float* INIT, int max_iter, float tol
   double* ds = part + G;            // device scalars: [0] alpha [1] beta / norm
   double* cvec = ds + 8;            // [num_iter]
   std::vector<float> Th((size_t)max_iter * max_iter, 0.f);
-  double* h = reinterpret_cast<double*>(reinterpret_cast<char*>(p->pinned) + 4096);
+  double* h = reinterpret_cast<double*>(static_cast<char*>(p->pinned) + PIN_SCALARS);
 
   auto dot = [&](const float* a, const float* b, double* out, int do_sqrt) {
     lz_dot_kernel<<<G, 256, 0, st>>>(a, b, n, part);

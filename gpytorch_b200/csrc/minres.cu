@@ -39,24 +39,21 @@
 //   sum        beta_{k+1}^2 ; c_{k+1} = U^T v / beta_{k+1}  (re-based on the actual vector every iteration)
 //   update     as above, with x_k in place of q_k in the direction recurrence: the directions and Z are then the F^-T images
 //              of A's, and the tail OUT = K_hat (|b| Z) is the unpreconditioned one unchanged.
-// The preconditioned kernels are overloads of the kernels they replace (same names, so per-kernel resource checks cover both);
-// their row passes walk 64-row chunks, staging the chunk's rows of U [n][k] in shared memory for U c and U^T v.
+// finish, orth and update are one kernel each with a template flag PRE, whose preconditioned instance adds the U / D^-1/2 terms;
+// pre is an overload of ms_scale_kernel.  The kernel names stay those of the unpreconditioned loop, so per-kernel resource
+// checks cover both.  The preconditioned row passes stage each 64-row chunk's rows of U [n][k] in shared memory for U c and U^T v.
 #include <math.h>
 
 #include <algorithm>
 #include <climits>
+#include <cstddef>
 
-#include "gp_common.cuh"
+#include "rowpass.cuh"
 
 namespace gp {
 
-constexpr int MS_THREADS = 256;
-constexpr int MS_ROWS = 64;     // rows per pass of a CTA (4 float4 column groups x 64 row lanes)
 constexpr int MS_QMAX = 32;     // shifts per call
 constexpr int MS_KMAX = 128;    // preconditioner rank (the range of gp_precond_build)
-
-void cg_sum_launch(const float* in, int G, int L, double* out, const int* done, cudaStream_t st);   // cg.cu
-void cg_rhs_sq_launch(const float* RHS, int64_t ldr, int t, int64_t n, float* part, int G, cudaStream_t st);
 
 // scalar state of one run; the per-iteration parts are double-buffered by iteration parity (every CTA of the update kernel
 // reads parity k & 1 while block 0 writes parity (k + 1) & 1)
@@ -74,24 +71,13 @@ struct MsState {
   float resid[MS_QMAX * TP];   // |phibar| per (shift, column) after the last executed iteration
   int iters, nan_flag, all_conv, pad_;
 };
-
-__device__ __forceinline__ void ms_block_reduce(float4 acc, float* red /*[MS_ROWS][TP]*/, float* out /*[TP] global*/) {
-  const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
-  reinterpret_cast<float4*>(red)[rl * 4 + cg] = acc;
-  __syncthreads();
-  for (int s = MS_ROWS / 2; s > 0; s >>= 1) {
-    if (rl < s) {
-      float4 a = reinterpret_cast<float4*>(red)[rl * 4 + cg];
-      float4 b = reinterpret_cast<float4*>(red)[(rl + s) * 4 + cg];
-      reinterpret_cast<float4*>(red)[rl * 4 + cg] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-    }
-    __syncthreads();
-  }
-  if (tid < TP) out[tid] = red[tid];
-}
+constexpr size_t MS_READBACK = sizeof(MsState) - offsetof(MsState, resid);   // resid .. pad_
+static_assert(MS_READBACK == sizeof(float) * MS_QMAX * TP + 4 * sizeof(int), "the read-back is resid, iters, nan_flag, all_conv, pad_");
+static_assert(2 * MS_QMAX * sizeof(double) <= PIN_CIQ_OUT - PIN_CIQ_TW, "tau | w overflows its pinned slot");
+static_assert(PIN_CIQ_OUT + MS_READBACK <= PINNED_BYTES, "the msMINRES read-back overflows the pinned scratch");
 
 // q_1 = b / |b| (zero columns and columns >= t stay 0) ; q_0 = 0 ; Z = 0 ; scalar state of iteration 0
-__global__ void __launch_bounds__(MS_THREADS)
+__global__ void __launch_bounds__(RP_THREADS)
 ms_init_kernel(const float* __restrict__ B, int64_t ldb, int t, int64_t n, const double* __restrict__ sums, int Q,
                const double* __restrict__ tw /*[2][Q] tau | w*/, float* __restrict__ Qcur, float* __restrict__ Qprev,
                float* __restrict__ Z, MsState* __restrict__ st) {
@@ -109,7 +95,7 @@ ms_init_kernel(const float* __restrict__ B, int64_t ldb, int t, int64_t n, const
   }
   __syncthreads();
   if (blockIdx.x == 0) {
-    for (int e = tid; e < MS_QMAX * TP; e += MS_THREADS) {
+    for (int e = tid; e < MS_QMAX * TP; e += RP_THREADS) {
       const int c = e % TP;
       st->c1[0][e] = 1.0; st->s1[0][e] = 0.0; st->c2[0][e] = 1.0; st->s2[0][e] = 0.0;
       const bool live = c < t && (e / TP) < Q && inv_norm[c] != 0.f;   // a zero column starts (and stays) at residual 0
@@ -123,7 +109,7 @@ ms_init_kernel(const float* __restrict__ B, int64_t ldb, int t, int64_t n, const
     if (tid == 0) { st->done = 0; st->done_iter = INT_MAX; st->iters = 0; st->nan_flag = 0; st->all_conv = 0; }
   }
   __syncthreads();
-  for (int64_t r = (int64_t)blockIdx.x * MS_ROWS + rl; r < n; r += (int64_t)gridDim.x * MS_ROWS) {
+  for (int64_t r = (int64_t)blockIdx.x * RP_ROWS + rl; r < n; r += (int64_t)gridDim.x * RP_ROWS) {
     float v[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
@@ -136,83 +122,20 @@ ms_init_kernel(const float* __restrict__ B, int64_t ldb, int t, int64_t n, const
   }
 }
 
-// v = os sum_s partial_s + D q_k - beta_k q_{k-1} ; partials of q_k . v
-__global__ void __launch_bounds__(MS_THREADS)
-ms_finish_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_pad, float os, const float* __restrict__ pscale,
-                 float noise, const float* __restrict__ dvec, const float* __restrict__ Qcur, const float* __restrict__ Qprev,
-                 float* __restrict__ V, int64_t n, const MsState* __restrict__ st, int kk, float* __restrict__ part,
-                 const int* __restrict__ done, const int* __restrict__ xbad) {
-  if (*done) return;
-  __shared__ __align__(16) float red[MS_ROWS * TP];
-  __shared__ __align__(16) float bk[TP];
-  const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
-  if (tid < TP) bk[tid] = (float)st->beta[kk & 1][tid];
-  __syncthreads();
-  const float poison = *xbad ? __int_as_float(0x7fc00000) : 0.f;   // non-finite inputs: K.V is NaN in the reference
-  const float4 b4 = reinterpret_cast<const float4*>(bk)[cg];
-  float4 acc = make_float4(0, 0, 0, 0);
-  for (int64_t r = (int64_t)blockIdx.x * MS_ROWS + rl; r < n; r += (int64_t)gridDim.x * MS_ROWS) {
-    float4 s = make_float4(poison, poison, poison, poison);
-    float osr = os;
-    if (pscale) {   // kernel sum: slot sp belongs to the term with outputscale pscale[sp]
-      for (int sp = 0; sp < nsplit; ++sp) {
-        const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
-        const float w = pscale[sp];
-        s.x = fmaf(w, a.x, s.x); s.y = fmaf(w, a.y, s.y); s.z = fmaf(w, a.z, s.z); s.w = fmaf(w, a.w, s.w);
-      }
-      osr = 1.f;
-    } else {
-      for (int sp = 0; sp < nsplit; ++sp) {
-        const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
-        s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
-      }
-    }
-    const float4 q = reinterpret_cast<const float4*>(Qcur)[r * 4 + cg];
-    const float4 qp = reinterpret_cast<const float4*>(Qprev)[r * 4 + cg];
-    const float d = dvec ? dvec[r] : noise;
-    float4 x = make_float4(fmaf(d, q.x, osr * s.x), fmaf(d, q.y, osr * s.y), fmaf(d, q.z, osr * s.z), fmaf(d, q.w, osr * s.w));
-    x.x = fmaf(-b4.x, qp.x, x.x); x.y = fmaf(-b4.y, qp.y, x.y); x.z = fmaf(-b4.z, qp.z, x.z); x.w = fmaf(-b4.w, qp.w, x.w);
-    reinterpret_cast<float4*>(V)[r * 4 + cg] = x;
-    acc.x = fmaf(q.x, x.x, acc.x); acc.y = fmaf(q.y, x.y, acc.y); acc.z = fmaf(q.z, x.z, acc.z); acc.w = fmaf(q.w, x.w, acc.w);
-  }
-  ms_block_reduce(acc, red, part + (size_t)blockIdx.x * TP);
-}
-
-// v -= alpha_k q_k ; partials of v . v     (sums[0..16) = alpha_k)
-__global__ void __launch_bounds__(MS_THREADS)
-ms_orth_kernel(const double* __restrict__ sums, const float* __restrict__ Qcur, float* __restrict__ V, int64_t n,
-               float* __restrict__ part, const int* __restrict__ done) {
-  if (*done) return;
-  __shared__ __align__(16) float red[MS_ROWS * TP];
-  __shared__ __align__(16) float al[TP];
-  const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
-  if (tid < TP) al[tid] = (float)sums[tid];
-  __syncthreads();
-  const float4 a4 = reinterpret_cast<const float4*>(al)[cg];
-  float4 acc = make_float4(0, 0, 0, 0);
-  for (int64_t r = (int64_t)blockIdx.x * MS_ROWS + rl; r < n; r += (int64_t)gridDim.x * MS_ROWS) {
-    const float4 q = reinterpret_cast<const float4*>(Qcur)[r * 4 + cg];
-    float4 v = reinterpret_cast<float4*>(V)[r * 4 + cg];
-    v.x = fmaf(-a4.x, q.x, v.x); v.y = fmaf(-a4.y, q.y, v.y); v.z = fmaf(-a4.z, q.z, v.z); v.w = fmaf(-a4.w, q.w, v.w);
-    reinterpret_cast<float4*>(V)[r * 4 + cg] = v;
-    acc.x = fmaf(v.x, v.x, acc.x); acc.y = fmaf(v.y, v.y, acc.y); acc.z = fmaf(v.z, v.z, acc.z); acc.w = fmaf(v.w, v.w, acc.w);
-  }
-  ms_block_reduce(acc, red, part + (size_t)blockIdx.x * TP);
-}
-
-// ---- preconditioned row passes ----------------------------------------------------------------------------------------------
-// dynamic shared memory: U rows of one chunk [64][kp] (kp = k | 1: an odd pitch puts the 8 rows a warp reads in 8 banks; the
-// region is at least [64][16] and doubles as the reduction scratch after the last chunk) | X block [64][16] | coefficients [k][16]
+// ---- row passes: finish and orth take PRE = true with a preconditioner ----------------------------------------------------------
+// dynamic shared memory of the preconditioned passes: U rows of one chunk [64][kp] (kp = k | 1: an odd pitch puts the 8 rows a
+// warp reads in 8 banks; the region is at least [64][16] and doubles as the reduction scratch after the last chunk) |
+// X block [64][16] | coefficients [k][16]
 __host__ __device__ inline int ms_upitch(int k) { return k | 1; }
-__host__ __device__ inline int ms_urows(int k) { return MS_ROWS * (ms_upitch(k) > TP ? ms_upitch(k) : TP); }
-inline size_t ms_pre_smem(int k) { return sizeof(float) * ((size_t)ms_urows(k) + MS_ROWS * TP + (size_t)k * TP); }
+__host__ __device__ inline int ms_urows(int k) { return RP_ROWS * (ms_upitch(k) > TP ? ms_upitch(k) : TP); }
+inline size_t ms_pre_smem(int k) { return sizeof(float) * ((size_t)ms_urows(k) + RP_ROWS * TP + (size_t)k * TP); }
 
 // rows [r0, r0 + nr) of U [n][k] (one contiguous block) -> us [nr][kp]
 __device__ __forceinline__ int ms_stage_u(const float* __restrict__ U, int k, int64_t r0, int64_t n, float* __restrict__ us) {
-  const int nr = (int)min((int64_t)MS_ROWS, n - r0);
+  const int nr = (int)min((int64_t)RP_ROWS, n - r0);
   const int kp = ms_upitch(k);
   const float* src = U + r0 * k;
-  for (int e = threadIdx.x; e < nr * k; e += MS_THREADS) {
+  for (int e = threadIdx.x; e < nr * k; e += RP_THREADS) {
     const int r = e / k;
     us[r * kp + (e - r * k)] = src[e];
   }
@@ -259,16 +182,16 @@ __device__ __forceinline__ double ms_pre_alpha(const double* __restrict__ sums, 
 }
 
 // pre: X = D^-1/2 (Q - U c) = F^-T Q   (c = U^T Q, fp64 [k][16])
-__global__ void __launch_bounds__(MS_THREADS)
+__global__ void __launch_bounds__(RP_THREADS)
 ms_scale_kernel(const float* __restrict__ Qin, const double* __restrict__ cvec, const float* __restrict__ U, int k, float noise,
                 const float* __restrict__ dvec, float* __restrict__ X, int64_t n, const int* __restrict__ done) {
   if (done && *done) return;
   extern __shared__ __align__(16) float msh[];
   float* us = msh;
-  float* cs = msh + ms_urows(k) + MS_ROWS * TP;
+  float* cs = msh + ms_urows(k) + RP_ROWS * TP;
   const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
-  for (int e = tid; e < k * TP; e += MS_THREADS) cs[e] = (float)cvec[e];
-  for (int64_t r0 = (int64_t)blockIdx.x * MS_ROWS; r0 < n; r0 += (int64_t)gridDim.x * MS_ROWS) {
+  for (int e = tid; e < k * TP; e += RP_THREADS) cs[e] = (float)cvec[e];
+  for (int64_t r0 = (int64_t)blockIdx.x * RP_ROWS; r0 < n; r0 += (int64_t)gridDim.x * RP_ROWS) {
     ms_stage_u(U, k, r0, n, us);
     __syncthreads();
     const int64_t r = r0 + rl;
@@ -282,50 +205,38 @@ ms_scale_kernel(const float* __restrict__ Qin, const double* __restrict__ cvec, 
   }
 }
 
-// finish: y = D^-1/2 (os sum_s partial_s + D x_k) ; v = y - beta_k q_{k-1} ; partials [ q_k . v | U^T y ]  (row pitch 16 (k + 1))
-__global__ void __launch_bounds__(MS_THREADS)
+// finish: v = K_hat q_k - beta_k q_{k-1} ; partials of q_k . v   (X unused, k = 0)
+// PRE: y = D^-1/2 K_hat x_k ; v = y - beta_k q_{k-1} ; partials [ q_k . v | U^T y ]  (row pitch 16 (k + 1))
+template <bool PRE>
+__global__ void __launch_bounds__(RP_THREADS)
 ms_finish_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_pad, float os, const float* __restrict__ pscale,
                  float noise, const float* __restrict__ dvec, const float* __restrict__ X, const float* __restrict__ Qcur,
                  const float* __restrict__ Qprev, float* __restrict__ V, int64_t n, const MsState* __restrict__ st, int kk,
                  const float* __restrict__ U, int k, float* __restrict__ part, const int* __restrict__ done,
                  const int* __restrict__ xbad) {
   if (*done) return;
-  extern __shared__ __align__(16) float msh[];
+  extern __shared__ __align__(16) float msh[];   // PRE: layout above; else the [64][16] reduction scratch
   float* us = msh;
   float* ys = msh + ms_urows(k);
   __shared__ __align__(16) float bk[TP];
   const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
   if (tid < TP) bk[tid] = (float)st->beta[kk & 1][tid];
   __syncthreads();
-  const float poison = *xbad ? __int_as_float(0x7fc00000) : 0.f;
+  const float poison = *xbad ? __int_as_float(0x7fc00000) : 0.f;   // non-finite inputs: K.V is NaN in the reference
   const float4 b4 = reinterpret_cast<const float4*>(bk)[cg];
   float4 acc = make_float4(0, 0, 0, 0);
   float uacc[MS_KMAX / 16] = {};
-  for (int64_t r0 = (int64_t)blockIdx.x * MS_ROWS; r0 < n; r0 += (int64_t)gridDim.x * MS_ROWS) {
-    const int nr = ms_stage_u(U, k, r0, n, us);
-    const int64_t r = r0 + rl;
+  // PRE: the whole CTA walks every 64-row chunk r0 = r - rl (U staging, U^T reduction); else a thread stops after its last row
+  for (int64_t r = (int64_t)blockIdx.x * RP_ROWS + rl; (PRE ? r - rl : r) < n; r += (int64_t)gridDim.x * RP_ROWS) {
+    int nr = 0;
+    if constexpr (PRE) nr = ms_stage_u(U, k, r - rl, n, us);
     float4 y = make_float4(0, 0, 0, 0);
     if (r < n) {
-      float4 s = make_float4(poison, poison, poison, poison);
-      float osr = os;
-      if (pscale) {
-        for (int sp = 0; sp < nsplit; ++sp) {
-          const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
-          const float w = pscale[sp];
-          s.x = fmaf(w, a.x, s.x); s.y = fmaf(w, a.y, s.y); s.z = fmaf(w, a.z, s.z); s.w = fmaf(w, a.w, s.w);
-        }
-        osr = 1.f;
-      } else {
-        for (int sp = 0; sp < nsplit; ++sp) {
-          const float4 a = reinterpret_cast<const float4*>(kpart)[((int64_t)sp * rows_pad + r) * 4 + cg];
-          s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
-        }
+      y = khat_row(kpart, nsplit, rows_pad, os, pscale, poison, PRE ? X : Qcur, dvec, noise, r, cg);
+      if constexpr (PRE) {
+        const float rs = 1.f / sqrtf(dvec ? dvec[r] : noise);
+        y = make_float4(y.x * rs, y.y * rs, y.z * rs, y.w * rs);
       }
-      const float4 x = reinterpret_cast<const float4*>(X)[r * 4 + cg];
-      const float d = dvec ? dvec[r] : noise;
-      const float rs = 1.f / sqrtf(d);
-      y = make_float4(fmaf(d, x.x, osr * s.x) * rs, fmaf(d, x.y, osr * s.y) * rs, fmaf(d, x.z, osr * s.z) * rs,
-                      fmaf(d, x.w, osr * s.w) * rs);
       const float4 q = reinterpret_cast<const float4*>(Qcur)[r * 4 + cg];
       const float4 qp = reinterpret_cast<const float4*>(Qprev)[r * 4 + cg];
       float4 v;
@@ -333,61 +244,74 @@ ms_finish_kernel(const float* __restrict__ kpart, int nsplit, int64_t rows_pad, 
       reinterpret_cast<float4*>(V)[r * 4 + cg] = v;
       acc.x = fmaf(q.x, v.x, acc.x); acc.y = fmaf(q.y, v.y, acc.y); acc.z = fmaf(q.z, v.z, acc.z); acc.w = fmaf(q.w, v.w, acc.w);
     }
-    reinterpret_cast<float4*>(ys)[rl * 4 + cg] = y;
-    __syncthreads();
-    ms_ut_acc(us, k, ys, nr, uacc);
-    __syncthreads();
+    if constexpr (PRE) {
+      reinterpret_cast<float4*>(ys)[rl * 4 + cg] = y;
+      __syncthreads();
+      ms_ut_acc(us, k, ys, nr, uacc);
+      __syncthreads();
+    }
   }
   float* out = part + (size_t)blockIdx.x * TP * (k + 1);
-  ms_block_reduce(acc, us, out);
-  ms_ut_store(uacc, k, out + TP);
+  block_reduce_cols(acc, msh, out);
+  if constexpr (PRE) ms_ut_store(uacc, k, out + TP);
 }
 
-// orth: v -= U (U^T y) + alpha_k q_k ; partials [ v . v | U^T v ]  (sums = [ q_k . v | U^T y ], cvec = c_k).
-// Without sums (start-up pass) V is only read: partials [ v . v | U^T v ] of the block as it is.
-__global__ void __launch_bounds__(MS_THREADS)
+// orth: v -= alpha_k q_k ; partials of v . v   (sums[0..16) = alpha_k ; cvec, U unused, k = 0)
+// PRE: v -= U (U^T y) + alpha_k q_k ; partials [ v . v | U^T v ]  (sums = [ q_k . v | U^T y ], cvec = c_k).  Without sums
+// (start-up pass) V is only read: partials [ v . v | U^T v ] of the block as it is.
+template <bool PRE>
+__global__ void __launch_bounds__(RP_THREADS)
 ms_orth_kernel(const double* __restrict__ sums, const double* __restrict__ cvec, const float* __restrict__ Qcur,
                float* __restrict__ V, int64_t n, const float* __restrict__ U, int k, float* __restrict__ part,
                const int* __restrict__ done) {
   if (done && *done) return;
-  extern __shared__ __align__(16) float msh[];
+  extern __shared__ __align__(16) float msh[];   // PRE: layout above; else the [64][16] reduction scratch
   float* us = msh;
   float* vs = msh + ms_urows(k);
-  float* cs = vs + MS_ROWS * TP;
+  float* cs = vs + RP_ROWS * TP;
   __shared__ __align__(16) float al[TP];
   const int tid = threadIdx.x, cg = tid & 3, rl = tid >> 2;
-  if (sums) {
-    for (int e = tid; e < k * TP; e += MS_THREADS) cs[e] = (float)sums[TP + e];
-    if (tid < TP) al[tid] = (float)ms_pre_alpha(sums, cvec, k, tid);
+  const bool update = !PRE || sums != nullptr;   // false: the read-only start-up pass
+  if (update) {
+    if constexpr (PRE)
+      for (int e = tid; e < k * TP; e += RP_THREADS) cs[e] = (float)sums[TP + e];
+    if (tid < TP) al[tid] = (float)(PRE ? ms_pre_alpha(sums, cvec, k, tid) : sums[tid]);
   }
   __syncthreads();
   const float4 a4 = reinterpret_cast<const float4*>(al)[cg];
   float4 acc = make_float4(0, 0, 0, 0);
   float uacc[MS_KMAX / 16] = {};
-  for (int64_t r0 = (int64_t)blockIdx.x * MS_ROWS; r0 < n; r0 += (int64_t)gridDim.x * MS_ROWS) {
-    const int nr = ms_stage_u(U, k, r0, n, us);
-    __syncthreads();
-    const int64_t r = r0 + rl;
+  // PRE: the whole CTA walks every 64-row chunk r0 = r - rl (U staging, U^T reduction); else a thread stops after its last row
+  for (int64_t r = (int64_t)blockIdx.x * RP_ROWS + rl; (PRE ? r - rl : r) < n; r += (int64_t)gridDim.x * RP_ROWS) {
+    int nr = 0;
+    if constexpr (PRE) {
+      nr = ms_stage_u(U, k, r - rl, n, us);
+      __syncthreads();
+    }
     float4 v = make_float4(0, 0, 0, 0);
     if (r < n) {
       v = reinterpret_cast<const float4*>(V)[r * 4 + cg];
-      if (sums) {
-        const float4 uc = ms_uc(us, k, cs, rl, cg);
+      if (update) {
+        if constexpr (PRE) {
+          const float4 uc = ms_uc(us, k, cs, rl, cg);
+          v.x -= uc.x; v.y -= uc.y; v.z -= uc.z; v.w -= uc.w;
+        }
         const float4 q = reinterpret_cast<const float4*>(Qcur)[r * 4 + cg];
-        v.x = fmaf(-a4.x, q.x, v.x - uc.x); v.y = fmaf(-a4.y, q.y, v.y - uc.y);
-        v.z = fmaf(-a4.z, q.z, v.z - uc.z); v.w = fmaf(-a4.w, q.w, v.w - uc.w);
+        v.x = fmaf(-a4.x, q.x, v.x); v.y = fmaf(-a4.y, q.y, v.y); v.z = fmaf(-a4.z, q.z, v.z); v.w = fmaf(-a4.w, q.w, v.w);
         reinterpret_cast<float4*>(V)[r * 4 + cg] = v;
       }
       acc.x = fmaf(v.x, v.x, acc.x); acc.y = fmaf(v.y, v.y, acc.y); acc.z = fmaf(v.z, v.z, acc.z); acc.w = fmaf(v.w, v.w, acc.w);
     }
-    reinterpret_cast<float4*>(vs)[rl * 4 + cg] = v;
-    __syncthreads();
-    ms_ut_acc(us, k, vs, nr, uacc);
-    __syncthreads();
+    if constexpr (PRE) {
+      reinterpret_cast<float4*>(vs)[rl * 4 + cg] = v;
+      __syncthreads();
+      ms_ut_acc(us, k, vs, nr, uacc);
+      __syncthreads();
+    }
   }
   float* out = part + (size_t)blockIdx.x * TP * (k + 1);
-  ms_block_reduce(acc, us, out);
-  ms_ut_store(uacc, k, out + TP);
+  block_reduce_cols(acc, msh, out);
+  if constexpr (PRE) ms_ut_store(uacc, k, out + TP);
 }
 
 // rotations + q_{k+1} + direction blocks + Z + stop rule.  sums = [ alpha_k (16) | beta_{k+1}^2 (16) ].
@@ -397,7 +321,7 @@ ms_orth_kernel(const double* __restrict__ sums, const double* __restrict__ cvec,
 // D holds 2 blocks per shift: at iteration kk, d_{k-1} is block 2q + ((kk + 1) & 1) and d_{k-2} is block 2q + (kk & 1); the new
 // direction overwrites d_{k-2}.
 template <bool PRE>
-__global__ void __launch_bounds__(MS_THREADS)
+__global__ void __launch_bounds__(RP_THREADS)
 ms_update_kernel(const double* __restrict__ sums, const double* __restrict__ sums2, const double* __restrict__ cprev,
                  double* __restrict__ cnext, int k, int kk, int Q, int t, float tol, const float* __restrict__ V,
                  const float* __restrict__ Qcur, float* __restrict__ Qnext, float* __restrict__ D, float* __restrict__ Z, int64_t n,
@@ -427,11 +351,11 @@ ms_update_kernel(const double* __restrict__ sums, const double* __restrict__ sum
   }
   __syncthreads();
   if (PRE && writer)
-    for (int e = tid; e < k * TP; e += MS_THREADS) {
+    for (int e = tid; e < k * TP; e += RP_THREADS) {
       const int c = e % TP;
       cnext[e] = (brk_s[c] || st->conv[P][c]) ? 0.0 : sums2[TP + e] / bnext_s[c];
     }
-  for (int e = tid; e < Q * TP; e += MS_THREADS) {
+  for (int e = tid; e < Q * TP; e += RP_THREADS) {
     const int q = e / TP, c = e % TP;
     const double a = alpha_s[c] + st->tau[q];
     const double bk = st->beta[P][c], bn = bnext_s[c];
@@ -459,7 +383,7 @@ ms_update_kernel(const double* __restrict__ sums, const double* __restrict__ sum
   // rows: q_{k+1}, new directions, Z
   const float4 ib = reinterpret_cast<const float4*>(invb)[cg];
   const int64_t blk = n * TP;
-  for (int64_t r = (int64_t)blockIdx.x * MS_ROWS + rl; r < n; r += (int64_t)gridDim.x * MS_ROWS) {
+  for (int64_t r = (int64_t)blockIdx.x * RP_ROWS + rl; r < n; r += (int64_t)gridDim.x * RP_ROWS) {
     const int64_t o = r * 4 + cg;
     const float4 v = reinterpret_cast<const float4*>(V)[o];
     const float4 q = reinterpret_cast<const float4*>(Qcur)[o];
@@ -545,7 +469,7 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
   cudaStream_t st = p->stream;
   const int64_t n = p->n2;
   // the preconditioned row passes hold ~45 KB of shared memory (k = 128): 4 CTAs per SM
-  const int G = (int)std::min<int64_t>(cdiv(n, MS_ROWS), (int64_t)(pre ? 4 : 8) * p->n_sm);
+  const int G = (int)std::min<int64_t>(cdiv(n, RP_ROWS), (int64_t)(pre ? 4 : 8) * p->n_sm);
   const size_t blk = (size_t)n * TP;
   const int L = pre ? TP * (k + 1) : TP;   // partial row: [ dot (16) | U^T block (16 k) ]
   // workspace: q (2 blocks) | v | Z | directions (2 Q blocks) | x (preconditioned) | partials [2][G][L] | sums | tau, w | state
@@ -576,7 +500,7 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
   const int* done = &S->done;
   const float* dvec = p->noise_diag;
 
-  double* h_tw = reinterpret_cast<double*>(reinterpret_cast<char*>(p->pinned) + 8192);
+  double* h_tw = reinterpret_cast<double*>(static_cast<char*>(p->pinned) + PIN_CIQ_TW);
   for (int q = 0; q < Q; ++q) { h_tw[q] = tau[q]; h_tw[Q + q] = w[q]; }
   GP_CUDA(cudaMemcpyAsync(d_tw, h_tw, sizeof(double) * 2 * Q, cudaMemcpyHostToDevice, st));
   GP_CUDA(cudaMemsetAsync(D, 0, sizeof(float) * blk * 2 * Q, st));
@@ -584,21 +508,19 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
   // ---- init ----
   cg_rhs_sq_launch(B, ldb, t, n, part1, G, st);
   cg_sum_launch(part1, G, TP, sums0, nullptr, st);
-  ms_init_kernel<<<G, MS_THREADS, 0, st>>>(B, ldb, t, n, sums0, Q, d_tw, Qb[0], Qb[1], Z, S);
+  ms_init_kernel<<<G, RP_THREADS, 0, st>>>(B, ldb, t, n, sums0, Q, d_tw, Qb[0], Qb[1], Z, S);
   p->launches += 3;
-  const size_t shp = pre ? ms_pre_smem(k) : 0;
+  const size_t shp = pre ? ms_pre_smem(k) : sizeof(float) * RP_ROWS * TP;
   if (pre) {   // c_1 = U^T q_1
-    ms_orth_kernel<<<G, MS_THREADS, shp, st>>>(nullptr, nullptr, nullptr, Qb[0], n, U, k, part2, nullptr);
+    ms_orth_kernel<true><<<G, RP_THREADS, shp, st>>>(nullptr, nullptr, nullptr, Qb[0], n, U, k, part2, nullptr);
     cg_sum_launch(part2, G, L, sumsI, nullptr, st);
     p->launches += 2;
   }
   GP_CUDA(cudaGetLastError());
 
   // ---- iterations ----
-  int* h_done = reinterpret_cast<int*>(p->pinned);   // [0..1] ring of done flags
-  cudaEvent_t ev[2];
-  GP_CUDA(cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming));
-  GP_CUDA(cudaEventCreateWithFlags(&ev[1], cudaEventDisableTiming));
+  SolverLoop loop(p, "msMINRES", done, 0);
+  GP_CHECK(loop.create_events());
   int status = GP_OK;
   bool finished = false;
   for (int kk = 0; kk < max_iter && !finished; ++kk) {
@@ -606,38 +528,28 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
     float* Qoth = Qb[(kk + 1) & 1];   // q_{k-1} on entry, q_{k+1} on exit
     if (pre) {
       const double* ck = cbuf[kk & 1];
-      ms_scale_kernel<<<G, MS_THREADS, shp, st>>>(Qcur, ck, U, k, p->noise, dvec, X, n, done);
+      ms_scale_kernel<<<G, RP_THREADS, shp, st>>>(Qcur, ck, U, k, p->noise, dvec, X, n, done);
       if ((status = kmv_partials(p, X, done)) != GP_OK) break;
-      ms_finish_kernel<<<G, MS_THREADS, shp, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p),
-                                                   p->noise, dvec, X, Qcur, Qoth, V, n, S, kk, U, k, part1, done, p->xbad);
+      ms_finish_kernel<true><<<G, RP_THREADS, shp, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p),
+                                                         p->noise, dvec, X, Qcur, Qoth, V, n, S, kk, U, k, part1, done, p->xbad);
       cg_sum_launch(part1, G, L, sumsA, done, st);
-      ms_orth_kernel<<<G, MS_THREADS, shp, st>>>(sumsA, ck, Qcur, V, n, U, k, part2, done);
+      ms_orth_kernel<true><<<G, RP_THREADS, shp, st>>>(sumsA, ck, Qcur, V, n, U, k, part2, done);
       cg_sum_launch(part2, G, L, sumsB, done, st);
-      ms_update_kernel<true><<<G, MS_THREADS, 0, st>>>(sumsA, sumsB, ck, cbuf[(kk + 1) & 1], k, kk, Q, t, tol, V, X, Qoth, D, Z, n, S);
+      ms_update_kernel<true><<<G, RP_THREADS, 0, st>>>(sumsA, sumsB, ck, cbuf[(kk + 1) & 1], k, kk, Q, t, tol, V, X, Qoth, D, Z, n, S);
       p->launches += 6;
     } else {
       if ((status = kmv_partials(p, Qcur, done)) != GP_OK) break;
-      ms_finish_kernel<<<G, MS_THREADS, 0, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p),
-                                                 p->noise, dvec, Qcur, Qoth, V, n, S, kk, part1, done, p->xbad);
+      ms_finish_kernel<false><<<G, RP_THREADS, shp, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p),
+                                                          p->noise, dvec, nullptr, Qcur, Qoth, V, n, S, kk, nullptr, 0, part1, done, p->xbad);
       cg_sum_launch(part1, G, TP, sums, done, st);
-      ms_orth_kernel<<<G, MS_THREADS, 0, st>>>(sums, Qcur, V, n, part2, done);
+      ms_orth_kernel<false><<<G, RP_THREADS, shp, st>>>(sums, nullptr, Qcur, V, n, nullptr, 0, part2, done);
       cg_sum_launch(part2, G, TP, sums + TP, done, st);
-      ms_update_kernel<false><<<G, MS_THREADS, 0, st>>>(sums, nullptr, nullptr, nullptr, 0, kk, Q, t, tol, V, Qcur, Qoth, D, Z, n, S);
+      ms_update_kernel<false><<<G, RP_THREADS, 0, st>>>(sums, nullptr, nullptr, nullptr, 0, kk, Q, t, tol, V, Qcur, Qoth, D, Z, n, S);
       p->launches += 5;
     }
-    // look-ahead stop check: read the flag of iteration kk after iteration kk + 1 has been enqueued
-    cudaMemcpyAsync(&h_done[kk & 1], &S->done, sizeof(int), cudaMemcpyDeviceToHost, st);
-    cudaEventRecord(ev[kk & 1], st);
-    if (kk > 0) {
-      cudaEventSynchronize(ev[(kk - 1) & 1]);
-      if (h_done[(kk - 1) & 1]) finished = true;
-    }
+    finished = loop.finished(kk);
   }
-  cudaError_t le = cudaGetLastError();
-  if (status == GP_OK && le != cudaSuccess) {
-    set_error("msMINRES launch failed: %s", cudaGetErrorString(le));
-    status = GP_E_CUDA;
-  }
+  status = loop.launch_status(status);
   if (status == GP_OK) {
     // OUT = K_hat (|b| Z)   (preconditioned: Z already holds F^-T sum_q w_q (A + tau_q I)^-1 q_1)
     ms_scale_kernel<<<(unsigned)cdiv((int64_t)blk, 256), 256, 0, st>>>(Z, S, n);
@@ -646,14 +558,10 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
     if (status == GP_OK) status = kmv_finish_user(p, Z, OUT, ldo, t, 1);
   }
   if (status == GP_OK) {
-    float* hs = reinterpret_cast<float*>(reinterpret_cast<char*>(p->pinned) + 12288);
-    const size_t nout = sizeof(float) * MS_QMAX * TP + 4 * sizeof(int);
-    cudaMemcpyAsync(hs, S->resid, nout, cudaMemcpyDeviceToHost, st);
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) {
-      set_error("msMINRES execution failed: %s", cudaGetErrorString(se));
-      status = GP_E_CUDA;
-    } else {
+    float* hs = reinterpret_cast<float*>(static_cast<char*>(p->pinned) + PIN_CIQ_OUT);
+    cudaMemcpyAsync(hs, S->resid, MS_READBACK, cudaMemcpyDeviceToHost, st);
+    status = loop.sync();
+    if (status == GP_OK) {
       const int* hi = reinterpret_cast<const int*>(hs + MS_QMAX * TP);   // iters, nan_flag, all_conv
       if (iters_out) *iters_out = hi[0];
       if (resid_out)
@@ -672,8 +580,6 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
       }
     }
   }
-  cudaEventDestroy(ev[0]);
-  cudaEventDestroy(ev[1]);
   return status;
 }
 

@@ -27,6 +27,7 @@ struct PcState {
   unsigned int counter;  // last-block-done ticket (step-wise path)
   unsigned int bar;      // monotonic grid-barrier counter (persistent path)
 };
+static_assert(PIN_PC_STATE + sizeof(PcState) <= PIN_PRECOND, "PcState overflows its pinned slot");
 
 constexpr int PC_THREADS = 128;
 
@@ -753,7 +754,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   }
   }
   GP_CUDA(cudaGetLastError());
-  PcState* hs = reinterpret_cast<PcState*>(reinterpret_cast<char*>(p->pinned) + 2048);
+  PcState* hs = reinterpret_cast<PcState*>(static_cast<char*>(p->pinned) + PIN_PC_STATE);
   GP_CUDA(cudaMemcpyAsync(hs, S, sizeof(PcState), cudaMemcpyDeviceToHost, st));
   GP_CUDA(cudaStreamSynchronize(st));
   if (rank_out) *rank_out = hs->rank;
@@ -764,6 +765,19 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   return GP_OK;
 }
 
+// launch split of gram_kernel: ntile x ntile output tiles times nz slices of jslice rows, about 2 CTAs per SM
+struct GramSplit {
+  int ntile, nz;
+  int64_t jslice;
+};
+static GramSplit gram_split(const gp_plan* p, int k, int64_t n) {
+  GramSplit g;
+  g.ntile = (int)cdiv(k, GT);
+  g.nz = (int)std::min<int64_t>(64, std::max<int64_t>(1, std::min<int64_t>(n / 1024, (2 * p->n_sm) / (g.ntile * (g.ntile + 1) / 2))));
+  g.jslice = cdiv(cdiv(n, g.nz), 64) * 64;
+  return g;
+}
+
 extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, double* logdet_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_REQUIRE(k >= 1 && k <= 128, GP_E_SHAPE, "preconditioner rank %d not in [1,128]", k);
@@ -771,10 +785,8 @@ extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, do
   GP_REQUIRE(dvec != nullptr || p->noise > 0.f, GP_E_SHAPE, "preconditioner needs noise > 0");
   cudaStream_t st = p->stream;
   const int64_t n = p->n2;
-  const int ntile = (int)cdiv(k, GT);
-  const int nz = (int)std::min<int64_t>(64, std::max<int64_t>(1, std::min<int64_t>(n / 1024, (2 * p->n_sm) / (ntile * (ntile + 1) / 2))));
-  const int64_t jslice = cdiv(cdiv(n, nz), 64) * 64;
-  GP_CHECK(p->gram.ensure(sizeof(double) * (size_t)nz * k * k));
+  const GramSplit g = gram_split(p, k, n);
+  GP_CHECK(p->gram.ensure(sizeof(double) * (size_t)g.nz * k * k));
   GP_CHECK(p->cholC.ensure(sizeof(double) * ((size_t)2 * k * k + 4) + 64));
   double* C = p->cholC.as<double>();
   double* Cinv = C + (size_t)k * k;
@@ -782,8 +794,7 @@ extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, do
   double* d_tail = d_logdet + 1;
   int* d_fail = reinterpret_cast<int*>(d_tail + 1);
   GP_CUDA(cudaMemsetAsync(d_fail, 0, sizeof(int), st));
-  dim3 gg((unsigned)ntile, (unsigned)ntile, (unsigned)nz);
-  gram_kernel<<<gg, 256, 0, st>>>(Lt, k, n, jslice, dvec, p->gram.as<double>());
+  gram_kernel<<<dim3((unsigned)g.ntile, (unsigned)g.ntile, (unsigned)g.nz), 256, 0, st>>>(Lt, k, n, g.jslice, dvec, p->gram.as<double>());
   if (dvec) {
     logsum_kernel<<<1, 256, 0, st>>>(dvec, n, d_tail);
     p->launches++;
@@ -792,13 +803,9 @@ extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, do
     GP_CUDA(cudaMemcpyAsync(d_tail, &tail, sizeof(double), cudaMemcpyHostToDevice, st));   // pageable source: copied before return
   }
   const size_t shc = sizeof(double) * (size_t)k * k;
-  static bool attr_done[64] = {};
-  if (!attr_done[p->device & 63]) {
-    GP_CUDA(cudaFuncSetAttribute(chol_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));   // k <= 128: 128 KB
-    GP_CUDA(cudaFuncSetAttribute(wsolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 168 * 1024));       // 128 KB + 32 KB
-    attr_done[p->device & 63] = true;
-  }
-  chol_small_kernel<<<1, 512, shc, st>>>(p->gram.as<double>(), nz, k, dvec ? 1.0 : (double)p->noise, d_tail, C, d_logdet, d_fail);
+  GP_CHECK(opt_in_smem<chol_small_kernel>(p->device, 160 * 1024));   // k <= 128: 128 KB
+  GP_CHECK(opt_in_smem<wsolve_kernel>(p->device, 168 * 1024));       // 128 KB + 32 KB
+  chol_small_kernel<<<1, 512, shc, st>>>(p->gram.as<double>(), g.nz, k, dvec ? 1.0 : (double)p->noise, d_tail, C, d_logdet, d_fail);
   // W = L C^-T through the explicit inverse (a per-row forward substitution against C in shared memory was tried: 0.52 ms at C2
   // against 0.16 + 0.19 ms for these two kernels -- one 128-thread CTA per SM is latency bound on 5000 dependent steps per row)
   cinv_kernel<<<k, 32, 0, st>>>(C, k, Cinv);
@@ -806,7 +813,7 @@ extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, do
                                                                                                       p->row_count, Cinv, dvec, W);
   p->launches += 4;
   GP_CUDA(cudaGetLastError());
-  double* h = reinterpret_cast<double*>(reinterpret_cast<char*>(p->pinned) + 3072);
+  double* h = reinterpret_cast<double*>(static_cast<char*>(p->pinned) + PIN_PRECOND);
   GP_CUDA(cudaMemcpyAsync(h, d_logdet, sizeof(double) * 2 + sizeof(int), cudaMemcpyDeviceToHost, st));
   GP_CUDA(cudaStreamSynchronize(st));
   if (logdet_out) *logdet_out = h[0];
@@ -827,17 +834,16 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   GP_REQUIRE(dvec != nullptr || p->noise > 0.f, GP_E_SHAPE, "the CIQ preconditioner needs noise > 0");
   cudaStream_t st = p->stream;
   const int64_t n = p->n2;
-  // Gram G = L^T D^-1 L (per-row noise) or L^T L (scalar noise, divided by sigma^2 below): gram_kernel with precond_build's split
-  const int ntile = (int)cdiv(k, GT);
-  const int nz = (int)std::min<int64_t>(64, std::max<int64_t>(1, std::min<int64_t>(n / 1024, (2 * p->n_sm) / (ntile * (ntile + 1) / 2))));
-  const int64_t jslice = cdiv(cdiv(n, nz), 64) * 64;
+  // Gram G = L^T D^-1 L (per-row noise) or L^T L (scalar noise, divided by sigma^2 below)
+  const GramSplit g = gram_split(p, k, n);
+  const int nz = g.nz;
   const int gs = (int)std::max<int64_t>(1, std::min<int64_t>(cdiv((int64_t)k * n, 4096), (int64_t)2 * p->n_sm));
   GP_CHECK(p->gram.ensure(sizeof(double) * ((size_t)nz * k * k + 2 * (size_t)gs)));
   GP_CHECK(p->cholC.ensure(sizeof(double) * ((size_t)2 * k * k + 4) + 64));
   double* gpart = p->gram.as<double>();
   double* spart = gpart + (size_t)nz * k * k;
   double* d_T = p->cholC.as<double>();
-  gram_kernel<<<dim3((unsigned)ntile, (unsigned)ntile, (unsigned)nz), 256, 0, st>>>(Lt, k, n, jslice, dvec, gpart);
+  gram_kernel<<<dim3((unsigned)g.ntile, (unsigned)g.ntile, (unsigned)nz), 256, 0, st>>>(Lt, k, n, g.jslice, dvec, gpart);
   ciq_stats_kernel<<<gs, 256, 0, st>>>(Lt, (int64_t)k * n, dvec, n, spart);
   p->launches += 2;
   GP_CUDA(cudaGetLastError());
@@ -870,11 +876,7 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   }
   GP_CUDA(cudaMemcpyAsync(d_T, T.data(), sizeof(double) * k * k, cudaMemcpyHostToDevice, st));   // pageable: copied before return
   const size_t shu = sizeof(double) * ((size_t)k * k + (size_t)k * 32);
-  static bool attr_done[64] = {};
-  if (!attr_done[p->device & 63]) {
-    GP_CUDA(cudaFuncSetAttribute(usolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 168 * 1024));   // 128 KB + 32 KB
-    attr_done[p->device & 63] = true;
-  }
+  GP_CHECK(opt_in_smem<usolve_kernel>(p->device, 168 * 1024));   // 128 KB + 32 KB
   usolve_kernel<<<(unsigned)cdiv(n, 32 * WS_BLOCKS), 128, shu, st>>>(Lt, k, n, d_T, dvec, 1.0 / sqrt((double)p->noise), U);
   p->launches += 1;
   GP_CUDA(cudaGetLastError());

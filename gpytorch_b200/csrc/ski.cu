@@ -746,11 +746,7 @@ static int ski_bilinear_d(gp_plan* p, const float* L16, const float* R16, double
 }
 
 int ski_bilinear(gp_plan* p, const float* L16, const float* R16, double* total) {
-  static bool attr_done[64] = {};
-  if (!attr_done[p->device & 63]) {
-    GP_CUDA(cudaFuncSetAttribute(ski_mode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    attr_done[p->device & 63] = true;
-  }
+  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
   switch (p->d) {
     case 1: return ski_bilinear_d<1>(p, L16, R16, total);
     case 2: return ski_bilinear_d<2>(p, L16, R16, total);
@@ -764,11 +760,7 @@ int ski_bilinear(gp_plan* p, const float* L16, const float* R16, double* total) 
 // partial[0][r][:] = (W K_uu W^T V16)[r][:]   (outputscale / noise are applied by the finish kernels)
 int ski_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   (void)done_flag;   // the products of a finished mBCG are cheap no-ops for the dense kernels; here they simply run
-  static bool attr_done[64] = {};
-  if (!attr_done[p->device & 63]) {
-    GP_CUDA(cudaFuncSetAttribute(ski_mode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    attr_done[p->device & 63] = true;
-  }
+  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
   switch (p->d) {
     case 1: return ski_matmul_d<1>(p, V16, TP, p->partial.as<float>());
     case 2: return ski_matmul_d<2>(p, V16, TP, p->partial.as<float>());

@@ -85,7 +85,7 @@ extern "C" int gp_slq_logdet(gp_plan* p, const float* TMAT, int n_tridiag, int l
   slq_kernel<<<1, 64, 0, p->stream>>>(TMAT, n_tridiag, ldt, J, (double)n / (double)n_tridiag, d_out, d_fail);
   p->launches++;
   GP_CUDA(cudaGetLastError());
-  double* h = reinterpret_cast<double*>(reinterpret_cast<char*>(p->pinned) + 3200);
+  double* h = reinterpret_cast<double*>(static_cast<char*>(p->pinned) + PIN_SLQ);
   GP_CUDA(cudaMemcpyAsync(h, d_out, sizeof(double) * 64 + sizeof(int), cudaMemcpyDeviceToHost, p->stream));
   GP_CUDA(cudaStreamSynchronize(p->stream));
   double s = 0.0;
