@@ -6,23 +6,34 @@
 //   dense K @ V inside linear_cg         lazy/lazy_evaluated_kernel_tensor.py:245-276 (chunked form)
 // The N x N matrix K never exists in HBM: per 64 x 64 tile it lives in the registers of one warpgroup.
 //
-// One CTA (two warpgroups, two CTAs resident per SM) owns one work unit = (128-row tile of K) x (a contiguous range of
-// 64-column tiles).  Warpgroup w owns rows [64 w, +64) of the tile; both share one B / V stream.  Per column tile:
+// One CTA per SM owns one work unit = (128-row tile of K) x (a contiguous range of 64-column tiles).  Per column tile j
+// each consumer warpgroup computes, for its 64 rows:
 //   GEMM1  S  = A_i . B_j^T     wgmma m64n64k8 tf32, both operands in shared memory (3xTF32 split operands packed by
 //                               pack.cu so that S_ij = -0.5|z_i - z_j|^2 directly); S lands in 32 fp32 registers per thread
 //   EPI    P  = cov(S)          ex2 / sqrt on the MUFU, in registers; P = P_hi + P_lo, both tf32 (P_hi: P with the low 13
-//                               bits cleared, P_lo: the exact fp32 residual)
+//                               bits cleared, P_lo: the exact fp32 residual), each in its own 32 registers
 //   GEMM2  O  = P_hi [V_hi;V_lo] (m64n32k8) + P_lo V_hi (m64n16k8), A operand from registers, B = V^T tiles in shared memory;
 //          a fresh accumulator per tile, folded into fp32 registers after every tile
-// The accumulator of GEMM1 is used directly as the register A operand of GEMM2.  That works because pack.cu stores the
-// columns of every 8-column group of XB in the order 0 4 1 5 2 6 3 7: a thread's accumulator pair (2t, 2t+1) then holds
+// P_hi / P_lo are the register A operand of GEMM2 in the layout of the GEMM1 accumulator.  That works because pack.cu stores
+// the columns of every 8-column group of XB in the order 0 4 1 5 2 6 3 7: a thread's accumulator pair (2t, 2t+1) then holds
 // the columns (t, t+4) the tf32 A fragment expects, and the V tiles keep their natural row order.
-// Operands arrive by bulk TMA (cp.async.bulk, mbarrier complete_tx) from tiles pre-packed in HBM in the wgmma K-major
-// no-swizzle layout, through an NS-deep shared-memory ring that thread 0 refills: a stage is reloaded at the start of the
-// tile after the one that used it, once both warpgroups have released it.  There is no separate producer warp: 8 warps
-// per CTA leave 128 registers per thread at two CTAs per SM (a ninth warp puts five warps on one SM sub-partition and
-// caps them at 96, where the wgmma chain spills and is serialised).  The two CTAs per SM keep the tensor core busy while
-// the other CTA's warpgroups are in their MUFU-bound epilogue.
+//
+// Warp specialisation (384 threads):
+//   warpgroup 0   producer: one thread issues the bulk copies (cp.async.bulk, mbarrier complete_tx) of the A tile and of
+//                 the B / V tiles, pre-packed in HBM in the wgmma K-major no-swizzle layout, into an NS-deep shared-memory
+//                 ring; it refills a stage once both consumers have released it.
+//   warpgroups 1-2 consumers, rows [64 c, +64) of the tile for consumer c.  In its turn on the tensor core a consumer runs
+//                 GEMM2 of tile j - 1 (two chains, one wait), then issues GEMM1 of tile j (one chain) and hands the tensor
+//                 core to the other consumer (named barriers 1 and 2) before it waits for S and runs the MUFU-bound epilogue.
+//                 So one consumer's epilogue overlaps the other's 21+ wgmmas.
+// Every wgmma chain is issued back to back (no per-instruction wait) at <= 128 registers per thread: each chain starts
+// with a write-only wgmma, so no accumulator is kept live across tiles; P and P_hi are stored in the A-fragment order, so
+// P_lo is formed in P's registers (S's) once the P_hi chain has been issued.  ptxas checks the register need of the
+// wgmma pipeline against the kernel's launch count (128), not against a warpgroup's setmaxnreg count: a consumer that
+// keeps P_lo in 32 registers of its own, so that GEMM2 of tile j - 1 and GEMM1 of tile j go out as one batch with one
+// wait, needs 153 registers; with a setmaxnreg 40 / 168 split under the 128 launch count ptxas serialises it (C7512) and
+// it runs 1.7-2.3x slower than this kernel; compiled at 168 registers per thread it is no faster (H100: level with this
+// kernel for RBF and C2 Matern-3/2, 2-10 % slower for the other Matern cases).
 #include "gp_common.cuh"
 #include "tc_ptx.cuh"
 
@@ -30,10 +41,11 @@ namespace gp {
 
 using namespace ptx;
 
-constexpr int TC_THREADS = 256;                     // 2 warpgroups
+constexpr int TC_THREADS = 384;                     // producer warpgroup + 2 consumer warpgroups
 constexpr int V_TF32_BYTES = 2 * TILE_J * TP * 4;   // [64/4][32 rows: V_hi(16) | V_lo(16)][4 tf32] = 8192
 constexpr int V_TILE_BYTES = V_TF32_BYTES + TILE_J * TP * 2;   // pitch of the packed V tiles in HBM (pack.cu)
-constexpr int MAX_NS = 8;
+constexpr int MAX_NS = 12;
+constexpr uint32_t TURN_BAR0 = 1;                   // named barriers 1, 2: consumer 0's / 1's turn on the tensor core
 
 struct TcBars {
   uint64_t a_full;
@@ -50,7 +62,7 @@ __device__ __forceinline__ float cov_tc(float a) {
 }
 
 template <int KIND>
-__global__ void __launch_bounds__(TC_THREADS, 2)
+__global__ void __maxnreg__(128)
 kmv_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const float* __restrict__ Vt,
               float* __restrict__ partial, int KP, int NS, int64_t ntile_j, int64_t tiles_per_split,
               int64_t rows_pad, int same, int64_t row_begin, const int* __restrict__ done_flag) {
@@ -79,104 +91,164 @@ kmv_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const 
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  __syncthreads();   // the last CTA-wide barrier: the roles below never meet all 384 threads again
   if (T == 0) return;
 
-  // load tile u into ring stage u % NS (thread 0 only)
-  auto load_stage = [&](int u) {
-    const uint32_t full = smem_u32(&bars->b_full[u % NS]);
-    uint8_t* st = sStage + (size_t)(u % NS) * stage_bytes;
-    const int64_t jt = jt0 + u;
-    mbar_arrive_expect_tx(full, stage_bytes);
-    bulk_g2s(smem_u32(st), XB + jt * (int64_t)TILE_J * KP, b_bytes, full);
-    // only the tf32 part of the packed V tile: the products run in tf32 (P_lo is multiplied by V_hi)
-    bulk_g2s(smem_u32(st + b_bytes), reinterpret_cast<const uint8_t*>(Vt) + jt * (int64_t)V_TILE_BYTES, V_TF32_BYTES, full);
-  };
-  if (threadIdx.x == 0) {
-    mbar_arrive_expect_tx(smem_u32(&bars->a_full), a_bytes);
-    bulk_g2s(smem_u32(sA), XA + it * (int64_t)TILE_I * KP, a_bytes, smem_u32(&bars->a_full));
-    for (int u = 0; u < NS && u < T; ++u) load_stage(u);
+  if (warp < 4) {
+    // ---- producer ----
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(smem_u32(&bars->a_full), a_bytes);
+      bulk_g2s(smem_u32(sA), XA + it * (int64_t)TILE_I * KP, a_bytes, smem_u32(&bars->a_full));
+      int s = 0;
+      uint32_t par = 0;   // phase of b_empty[s] the consumers complete when they release the stage's previous tile
+      for (int u = 0; u < T; ++u) {
+        if (u >= NS) mbar_wait(smem_u32(&bars->b_empty[s]), par);
+        const uint32_t full = smem_u32(&bars->b_full[s]);
+        uint8_t* st = sStage + (size_t)s * stage_bytes;
+        const int64_t jt = jt0 + u;
+        mbar_arrive_expect_tx(full, stage_bytes);
+        bulk_g2s(smem_u32(st), XB + jt * (int64_t)TILE_J * KP, b_bytes, full);
+        // only the tf32 part of the packed V tile: the products run in tf32 (P_lo is multiplied by V_hi)
+        bulk_g2s(smem_u32(st + b_bytes), reinterpret_cast<const uint8_t*>(Vt) + jt * (int64_t)V_TILE_BYTES, V_TF32_BYTES, full);
+        if (++s == NS) {
+          s = 0;
+          if (u >= NS) par ^= 1;
+        }
+      }
+    }
+    return;
   }
 
+  // ---- consumers ----
   // accumulator fragment of wgmma m64nN (fp32): register i of thread (warp wq of the warpgroup, lane = 4 g + t) holds row
   // 16 wq + g + 8 ((i >> 1) & 1) and column position 8 (i >> 2) + 2 t + (i & 1); with the XB column order of pack.cu the
   // position 2 t + e of an 8-column group is column t + 4 e of the tile.
-  const int wg = warp >> 2;
+  const int wg = (warp >> 2) - 1;   // consumer 0 / 1
   const int wq = warp & 3;
   const int g = lane >> 2, t = lane & 3;
   const int64_t rloc0 = it * TILE_I + wg * 64 + wq * 16 + g;   // local (padded) rows rloc0 and rloc0 + 8 of this thread
-  const int64_t gi0 = row_begin + rloc0;
+  const int64_t diag_off = row_begin + it * TILE_I + wg * 64 - jt0 * TILE_J;   // first global row of this warpgroup - jt0 * 64
   const uint64_t a_desc0 = gmma_desc(smem_u32(sA) + (uint32_t)wg * 8 * 128, TILE_I * 16, 128);
   constexpr uint64_t A_KSTEP = (2 * TILE_I * 16) >> 4, B_KSTEP = (2 * TILE_J * 16) >> 4, V_KSTEP = (2 * 2 * TP * 16) >> 4;
   const int ksteps1 = KP / 8;
+  const uint32_t my_turn = TURN_BAR0 + wg, other_turn = TURN_BAR0 + (wg ^ 1);
 
   float acc[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) acc[c] = 0.f;
-  mbar_wait(smem_u32(&bars->a_full), 0);
-  int sb = 0;
-  uint32_t par = 0;
+  float s[32], o1[16], o2[8];   // s: S of the current tile, then P, then P_lo
+  uint32_t hi[32];
+
+  auto stage_addr = [&](int sb) { return smem_u32(sStage + (size_t)sb * stage_bytes); };
+  // GEMM1 of the tile in stage sb into s
+  auto issue_gemm1 = [&](int sb) {
+    const uint64_t b_desc0 = gmma_desc(stage_addr(sb), TILE_J * 16, 128);
+    wgmma_m64n64k8_ss_first(s, a_desc0, b_desc0);
 #pragma unroll 1
-  for (int u = 0; u < T; ++u) {
-    if (threadIdx.x == 0 && u >= 1 && u - 1 + NS < T) {
-      // stage (u - 1) % NS: released by both warpgroups after tile u - 1 (phase (u - 1) / NS of its empty barrier)
-      mbar_wait(smem_u32(&bars->b_empty[(u - 1) % NS]), (uint32_t)(((u - 1) / NS) & 1));
-      load_stage(u - 1 + NS);
-    }
-    mbar_wait(smem_u32(&bars->b_full[sb]), par);
-    const uint32_t st = smem_u32(sStage + (size_t)sb * stage_bytes);
-    const uint64_t b_desc0 = gmma_desc(st, TILE_J * 16, 128);
-    const uint64_t v_desc0 = gmma_desc(st + b_bytes, 2 * TP * 16, 128);   // rows 0-15 V_hi, 16-31 V_lo
-    float s[32];
-    fence_regs(s);
+    for (int ks = 1; ks < ksteps1; ++ks) wgmma_m64n64k8_ss(s, a_desc0 + ks * A_KSTEP, b_desc0 + ks * B_KSTEP, 1u);
+  };
+  // GEMM2 of the tile in stage sb into a fresh o1 / o2, as two chains: P_hi [V_hi;V_lo] (P_hi in hi), then P_lo V_hi with
+  // P_lo = P - P_hi formed in place of P (in s) once the first chain has read P_hi.  Two chains keep P, P_hi, P_lo and O
+  // within the register budget of 384-thread CTAs.
+  auto run_gemm2 = [&](int sb) {
+    const uint64_t v_desc0 = gmma_desc(stage_addr(sb) + b_bytes, 2 * TP * 16, 128);   // rows 0-15 V_hi, 16-31 V_lo
+    fence_regs(o1);
     wgmma_fence();
-#pragma unroll 1
-    for (int ks = 0; ks < ksteps1; ++ks)
-      wgmma_m64n64k8_ss(s, a_desc0 + ks * A_KSTEP, b_desc0 + ks * B_KSTEP, ks > 0 ? 1u : 0u);
+    wgmma_m64n32k8_rs_first(o1, hi[0], hi[1], hi[2], hi[3], v_desc0);
+#pragma unroll
+    for (int jb = 1; jb < TILE_J / 8; ++jb)
+      wgmma_m64n32k8_rs(o1, hi[4 * jb], hi[4 * jb + 1], hi[4 * jb + 2], hi[4 * jb + 3], v_desc0 + jb * V_KSTEP, 1u);
+    wgmma_commit();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = s[i] - __uint_as_float(hi[i]);
+    fence_regs(s);
+    fence_regs(o2);
+    wgmma_fence();
+    wgmma_m64n16k8_rs_first(o2, __float_as_uint(s[0]), __float_as_uint(s[1]), __float_as_uint(s[2]), __float_as_uint(s[3]), v_desc0);
+#pragma unroll
+    for (int jb = 1; jb < TILE_J / 8; ++jb)
+      wgmma_m64n16k8_rs(o2, __float_as_uint(s[4 * jb]), __float_as_uint(s[4 * jb + 1]), __float_as_uint(s[4 * jb + 2]),
+                        __float_as_uint(s[4 * jb + 3]), v_desc0 + jb * V_KSTEP, 1u);
     wgmma_commit();
     wgmma_wait_all();
     fence_regs(s);
-
-    const int64_t jbase = (jt0 + u) * TILE_J;
-    const bool diag_tile = same && (gi0 - wq * 16 - g < jbase + TILE_J) && (jbase < gi0 - wq * 16 - g + 64);
-    if (diag_tile) {
+    fence_regs(o1);
+    fence_regs(o2);
+  };
+  // covariance P of tile u (S in s) and its tf32 part P_hi (the fp32 residual P_lo is formed in run_gemm2)
+  auto epilogue = [&](int u) {
+    const int64_t d = diag_off - (int64_t)u * TILE_J;   // first row of this warpgroup - first column of the tile
+    if (same && d > -64 && d < TILE_J) {
+      const int dr = (int)d + wq * 16 + g - t;           // global row of register 0 - global column of register 0
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int64_t gi = gi0 + 8 * ((i >> 1) & 1);
-        const int64_t gj = jbase + 8 * (i >> 2) + t + 4 * (i & 1);
-        if (gi == gj) s[i] = 0.f;   // a_ii = 0 exactly (kernel.py:44-45 fills the diagonal with 0)
+      for (int i = 0; i < 32; ++i)   // a_ii = 0 exactly (kernel.py:44-45 fills the diagonal with 0)
+        if (dr + 8 * ((i >> 1) & 1) - 8 * (i >> 2) - 4 * (i & 1) == 0) s[i] = 0.f;
+    }
+    // P goes back into s, P_hi into hi, both in the tf32 A-fragment order (registers 4 jb + {0, 2, 1, 3} of the accumulator)
+#pragma unroll
+    for (int jb = 0; jb < TILE_J / 8; ++jb) {
+      float pv[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) pv[k] = cov_tc<KIND>(s[4 * jb + k]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        s[4 * jb + k] = pv[(k >> 1) | ((k & 1) << 1)];   // k = 0 1 2 3 <- accumulator register 0 2 1 3
+        hi[4 * jb + k] = __float_as_uint(s[4 * jb + k]) & 0xFFFFE000u;
       }
     }
-    // P = cov(S) split into tf32 P_hi (in hi) and the fp32 residual P_lo (in place of S)
-    uint32_t hi[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const float pv = cov_tc<KIND>(s[i]);
-      hi[i] = __float_as_uint(pv) & 0xFFFFE000u;
-      s[i] = pv - __uint_as_float(hi[i]);
-    }
-    float o1[16], o2[8];
-    fence_regs(s);
-    fence_regs(o1);
-    fence_regs(o2);
-    wgmma_fence();
-#pragma unroll
-    for (int jb = 0; jb < TILE_J / 8; ++jb)
-      wgmma_m64n32k8_rs(o1, hi[4 * jb], hi[4 * jb + 2], hi[4 * jb + 1], hi[4 * jb + 3], v_desc0 + jb * V_KSTEP, jb > 0 ? 1u : 0u);
-#pragma unroll
-    for (int jb = 0; jb < TILE_J / 8; ++jb)
-      wgmma_m64n16k8_rs(o2, __float_as_uint(s[4 * jb]), __float_as_uint(s[4 * jb + 2]), __float_as_uint(s[4 * jb + 1]),
-                        __float_as_uint(s[4 * jb + 3]), v_desc0 + jb * V_KSTEP, jb > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait_all();
-    fence_regs(o1);
-    fence_regs(o2);
+  };
+  // O of the previous tile (stage sb): release the stage, fold into acc.  Long accumulation chains inside the tensor core
+  // drift, hence a fresh GEMM2 accumulator per tile.
+  auto fold = [&](int sb) {
     mbar_arrive(smem_u32(&bars->b_empty[sb]));   // this thread's share of the stage has been read
-    if (++sb == NS) { sb = 0; par ^= 1; }
-    // O is folded into fp32 registers after every tile: long accumulation chains inside the tensor core drift
 #pragma unroll
     for (int c = 0; c < 8; ++c) acc[c] += o1[c] + o1[c + 8] + o2[c];
+  };
+  auto issue_gemm1_batch = [&](int sb) {
+    fence_regs(s);
+    wgmma_fence();
+    issue_gemm1(sb);
+    wgmma_commit();
+  };
+  auto wait_gemm1 = [&]() {
+    wgmma_wait_all();
+    fence_regs(s);
+  };
+
+  mbar_wait(smem_u32(&bars->a_full), 0);
+  if (wg == 1) named_bar_arrive(TURN_BAR0, 256);   // consumer 0 takes the first turn
+
+  // turn 0: GEMM1 of tile 0
+  mbar_wait(smem_u32(&bars->b_full[0]), 0);
+  named_bar_sync(my_turn, 256);
+  issue_gemm1_batch(0);
+  named_bar_arrive(other_turn, 256);
+  wait_gemm1();
+  epilogue(0);
+
+  // turns 1 .. T - 1: GEMM2 of tile u - 1, then GEMM1 of tile u
+  int sb_prev = 0, sb = 1;   // NS >= 2 (launch_tc_kind)
+  uint32_t par = 0;
+#pragma unroll 1
+  for (int u = 1; u < T; ++u) {
+    mbar_wait(smem_u32(&bars->b_full[sb]), par);
+    named_bar_sync(my_turn, 256);
+    run_gemm2(sb_prev);
+    fold(sb_prev);
+    issue_gemm1_batch(sb);
+    named_bar_arrive(other_turn, 256);
+    wait_gemm1();
+    epilogue(u);
+    sb_prev = sb;
+    if (++sb == NS) { sb = 0; par ^= 1; }
   }
+
+  // last turn: GEMM2 of tile T - 1; consumer 1 has no one to hand the tensor core to
+  named_bar_sync(my_turn, 256);
+  run_gemm2(sb_prev);
+  if (wg == 0) named_bar_arrive(other_turn, 256);
+  fold(sb_prev);
+
   // columns 2 t, 2 t + 1 (c even) and 8 + 2 t, 9 + 2 t of rows rloc0 (c & 2 == 0) and rloc0 + 8
 #pragma unroll
   for (int c = 0; c < 8; c += 2) {
@@ -189,13 +261,9 @@ kmv_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const 
 static int tc_smem_bytes(int KP, int* ns_out) {
   const int a_bytes = KP * TILE_I * 4;
   const int stage = KP * TILE_J * 4 + V_TF32_BYTES;
-  // preferred: two CTAs per SM (<= ~113 KB each of the 228 KB); wide feature vectors fall back to one CTA per SM
-  int budget = 112 * 1024 - a_bytes - (int)sizeof(TcBars) - 1024;
+  // one CTA per SM: the whole 227 KB opt-in shared memory
+  const int budget = 226 * 1024 - a_bytes - (int)sizeof(TcBars);
   int ns = budget / stage;
-  if (ns < 3) {
-    budget = 226 * 1024 - a_bytes - (int)sizeof(TcBars) - 1024;
-    ns = budget / stage;
-  }
   if (ns > MAX_NS) ns = MAX_NS;
   *ns_out = ns;
   return a_bytes + ns * stage + (int)sizeof(TcBars);

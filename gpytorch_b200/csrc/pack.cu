@@ -165,7 +165,10 @@ int choose_geometry(gp_plan* p) {
     int64_t per = cdiv(ntj, s);
     if (s > 1 && per < 8) break;  // keep units long enough to amortise the prologue
     int64_t units = nti * s;
-    const int64_t slots = (int64_t)p->n_sm * (p->backend == GP_BACKEND_TCGEN05 ? 2 : 1);  // resident CTAs
+    // 2 slots per SM on the tensor-core path: the K.V kernel now runs one 384-thread CTA per SM, but the factor is kept so
+    // that the work units -- and with them the split of every row sum into partials, hence the results bit for bit -- stay
+    // what they were
+    const int64_t slots = (int64_t)p->n_sm * (p->backend == GP_BACKEND_TCGEN05 ? 2 : 1);
     int64_t waves = cdiv(units, slots);
     double eff = (double)(nti * ntj) / (double)(waves * slots * per);
     if (eff > best_eff + 0.02) { best_eff = eff; best = s; }

@@ -40,6 +40,16 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// ---- named barriers (ids 1..15; 0 is __syncthreads) ---------------------------------------------------------------
+// bar.sync waits until `count` threads have arrived (its own warps included); bar.arrive counts towards the barrier
+// without waiting.  count is a multiple of 32.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // ---- bulk TMA: contiguous global -> shared, completion on an mbarrier (SASS: UBLKCP) -------
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src_gmem, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
@@ -81,6 +91,37 @@ __device__ __forceinline__ void wgmma_m64n64k8_ss(float (&d)[32], uint64_t a_des
         "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
         "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+// The *_first forms start a chain: D = A * B^T with D write-only (scale-d 0).  Unlike the (+)= forms with accumulate = 0
+// they do not read D, so D's previous values need not stay live in D's registers until the chain starts -- registers that
+// held an accumulator can be reused freely (and vice versa) without copies that serialise the wgmma pipeline.
+__device__ __forceinline__ void wgmma_m64n64k8_ss_first(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 0, 1, 1;"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]),
+        "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]),
+        "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]),
+        "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31])
+      : "l"(a_desc), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_m64n32k8_rs_first(float (&d)[16], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                        uint64_t b_desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 0, 1, 1;"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]),
+        "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_m64n16k8_rs_first(float (&d)[8], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                        uint64_t b_desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 0, 1, 1;"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc));
 }
 // D[64 x 32] (+)= A[registers, 64 x 8 tf32] * B[smem desc, 32 x 8 tf32]^T   (D: 16 registers per thread)
 __device__ __forceinline__ void wgmma_m64n32k8_rs(float (&d)[16], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc,
