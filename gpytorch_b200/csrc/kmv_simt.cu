@@ -7,6 +7,7 @@
 // Reference semantics: LazyEvaluatedKernelTensor._matmul (lazy/lazy_evaluated_kernel_tensor.py:245-276),
 // _getitem (:136-243), _diagonal (:107-133), _bilinear_derivative (:69-105).
 #include "gp_common.cuh"
+#include "ski_rows.cuh"
 
 namespace gp {
 
@@ -336,10 +337,10 @@ using namespace gp;
 
 extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "row extraction is not available for the SKI backend");
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "row extraction of a kernel sum: call gp_krows on every term and add");
   GP_REQUIRE(m >= 0 && ldo >= p->n2, GP_E_SHAPE, "bad krows shape");
   if (m == 0) return GP_OK;
+  if (p->backend == GP_BACKEND_SKI) return ski_krows(p, idx, m, OUT, ldo);   // separable entries (ski_rows.cuh)
   const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
   dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
   size_t sh = sizeof(float) * p->DP;
@@ -356,8 +357,8 @@ extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, i
 
 extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "the diagonal is not available for the SKI backend");
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "diagonal of a kernel sum: call gp_kdiag on every term and add");
+  if (p->backend == GP_BACKEND_SKI) return ski_kdiag(p, OUT);   // not constant: w_i^T K_uu w_i (ski_rows.cuh)
   if (p->same) {
     // stationary kernels: k(x,x) = outputscale (lazy_evaluated_kernel_tensor.py:107-133 evaluates kernel(diag=True))
     fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, p->outputscale);

@@ -13,6 +13,7 @@
 #include <cmath>
 
 #include "gp_common.cuh"
+#include "ski_rows.cuh"
 
 namespace gp {
 
@@ -185,6 +186,9 @@ constexpr int PCP_RED = 512;
 // Arithmetic and tie-breaking (earliest position) per entry are those of pc_step_kernel: bit-identical pivots.
 // kernel sums (GP_BACKEND_SUM): K[pivot, j] = sum_t os_t k_t(|z_t,pivot - z_t,j|^2), every term with its own packed inputs
 constexpr int PC_KIND_SUM = 64;
+// SKI (GP_BACKEND_SKI): K[pivot, j] = s prod_k w_jk^T u_k[f_jk : f_jk + 4] with u of the pivot staged where the pivot row of Z sits
+// (ski_rows.cuh); DP = sum_k G_k
+constexpr int PC_KIND_SKI = 65;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -209,7 +213,7 @@ struct PcPart {
 template <int KIND>
 __global__ void __launch_bounds__(PCP_THREADS)
 pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, int64_t n, int max_rank, float tol,
-                      float* diag, int* pos, PcState* st, int64_t* piv_out, PcPart* part, const PcTerms tt) {
+                      float* diag, int* pos, PcState* st, int64_t* piv_out, PcPart* part, const PcTerms tt, const SkiRows sk) {
   extern __shared__ float sh[];
   float* zp = sh;
   float* lp = sh + DP;
@@ -240,6 +244,8 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
         for (int c = tid; c < tt.DP[t]; c += PCP_THREADS) zp[off + c] = tt.Z[t][(int64_t)pi * tt.DP[t] + c];
         off += tt.DP[t];
       }
+    } else if (KIND == PC_KIND_SKI) {
+      ski_stage_u(sk, pi, zp, tid, PCP_THREADS);
     } else {
       for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[(int64_t)pi * DP + c];
     }
@@ -276,13 +282,15 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             v = fmaf(tt.os[t], pc_cov_rt(tt.kind[t], -0.5f * s), v);
             off += tt.DP[t];
           }
+        } else if (KIND == PC_KIND_SKI) {
+          v = ski_entry(sk, zp, j);
         } else {
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
             float df = zp[c] - Z[j * DP + c];
             s = fmaf(df, df, s);
           }
-          v = os * cov_from_arg<(KIND == PC_KIND_SUM ? GP_RBF : KIND)>(-0.5f * s);
+          v = os * cov_from_arg<(KIND >= PC_KIND_SUM ? GP_RBF : KIND)>(-0.5f * s);
         }
         {
           float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -387,6 +395,51 @@ __global__ void pc_init_kernel(float* __restrict__ diag, int* __restrict__ perm,
   diag[j] = os;  // _approx_diagonal of a stationary kernel
   perm[j] = (int)j;
   pos[j] = (int)j;
+}
+
+// SKI: the initial diagonal is not constant.  diag[j] = K_ski(j, j), identity permutation; then pc_first_pivot_kernel
+__global__ void pc_init_ski_kernel(const SkiRows sk, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos, int64_t n) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  diag[j] = ski_diag_entry(sk, j);
+  perm[j] = (int)j;
+  pos[j] = (int)j;
+}
+
+// one CTA: first pivot = argmax of the diagonal, earliest index among equal maxima (torch.max over the whole diagonal), moved
+// to position 0; orig_err = that maximum (oracle/linalg.pivoted_cholesky).  A NaN or a non-positive maximum stops at once.
+constexpr int PC_FIRST_THREADS = 1024;
+__global__ void __launch_bounds__(PC_FIRST_THREADS)
+pc_first_pivot_kernel(const float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos, int64_t n, PcState* __restrict__ st,
+                      int64_t* __restrict__ piv_out) {
+  __shared__ float s_val[PC_FIRST_THREADS];
+  __shared__ int s_idx[PC_FIRST_THREADS];
+  const int tid = threadIdx.x;
+  float best = -INFINITY;
+  int bi = 0x7fffffff;
+  for (int64_t j = tid; j < n; j += PC_FIRST_THREADS) {   // ascending j per thread: strict > keeps the earliest
+    const float v = diag[j];
+    const float cv = (v != v) ? INFINITY : v;           // NaN wins and is reported below
+    if (cv > best) { best = cv; bi = (int)j; }
+  }
+  s_val[tid] = best; s_idx[tid] = bi;
+  __syncthreads();
+  for (int s = PC_FIRST_THREADS / 2; s > 0; s >>= 1) {
+    if (tid < s) {
+      const float v2 = s_val[tid + s]; const int i2 = s_idx[tid + s];
+      if (v2 > s_val[tid] || (v2 == s_val[tid] && i2 < s_idx[tid])) { s_val[tid] = v2; s_idx[tid] = i2; }
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    const int im = s_idx[0];
+    const float mx = diag[im];
+    st->done = 0; st->rank = 0; st->pivot = im; st->nan_flag = (mx > 0.f && mx < INFINITY) ? 0 : 1; st->dpiv = sqrtf(mx);
+    st->orig_err = mx; st->err = 0.f; st->counter = 0u; st->bar = 0u;
+    piv_out[0] = im;
+    perm[0] = im; perm[im] = 0;   // the swap of step 0 (im == 0: no-op)
+    pos[0] = im; pos[im] = 0;
+  }
 }
 
 // ---- preconditioner factor ---------------------------------------------------------------------
@@ -672,7 +725,6 @@ using namespace gp;
 extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float* Lt, int64_t* piv, int* rank_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_REQUIRE(p->same, GP_E_SHAPE, "pivoted Cholesky needs a square operator");
-  GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "pivoted Cholesky is not available for the SKI backend");
   GP_CHECK(sum_prepare(p));
   const int64_t n = p->n2;
   GP_REQUIRE(n < (int64_t)1 << 31, GP_E_SHAPE, "n too large");
@@ -694,8 +746,11 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_CUDA(cudaMemsetAsync(Lt, 0, sizeof(float) * (size_t)rank * n, st));
   GP_CUDA(cudaMemsetAsync(piv, 0, sizeof(int64_t) * rank, st));
   const bool sum = p->backend == GP_BACKEND_SUM;
+  const bool ski = p->backend == GP_BACKEND_SKI;
   PcTerms tt;
   memset(&tt, 0, sizeof(tt));
+  SkiRows sk;
+  memset(&sk, 0, sizeof(sk));
   float os_total = p->outputscale;
   int dp_total = p->DP;
   if (sum) {
@@ -709,21 +764,31 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       dp_total += q->DP;
     }
   }
-  pc_init_kernel<<<gb, PC_THREADS, 0, st>>>(diag, perm, pos, n, os_total, S, piv);   // stationary terms: constant initial diagonal
-  p->launches += 1;
-  const float* Z = sum ? nullptr : p->Z2.as<float>();
+  if (ski) {
+    GP_CHECK(ski_rows_args(p, &sk));
+    dp_total = sk.usum;   // the pivot's u_k take the place of its packed inputs in shared memory
+    pc_init_ski_kernel<<<gb, PC_THREADS, 0, st>>>(sk, diag, perm, pos, n);
+    pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
+    p->launches += 2;
+  } else {
+    pc_init_kernel<<<gb, PC_THREADS, 0, st>>>(diag, perm, pos, n, os_total, S, piv);   // stationary terms: constant initial diagonal
+    p->launches += 1;
+  }
+  const float* Z = (sum || ski) ? nullptr : p->Z2.as<float>();
   const bool stepwise = getenv("GP_PC_STEPWISE") != nullptr;   // debugging / A-B switch: one launch per step
   int coop = 0;
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, p->device);
   GP_REQUIRE(!sum || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a kernel sum needs the cooperative kernel");
+  GP_REQUIRE(!ski || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a SKI operator needs the cooperative kernel");
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : p->kind) {
+    switch (sum ? PC_KIND_SUM : ski ? PC_KIND_SKI : p->kind) {
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
       case GP_MATERN12: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN12>; break;
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
       case PC_KIND_SUM: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SUM>; break;
+      case PC_KIND_SKI: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SKI>; break;
       default: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN52>; break;
     }
     GP_CUDA(cudaFuncSetAttribute(fn1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
@@ -736,7 +801,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     int DPv = dp_total, rk = rank;
     float osv = os_total, tolv = error_tol;
     int64_t nn = n;
-    void* args[] = {(void*)&Z, &DPv, &osv, &Lt, &nn, &rk, &tolv, &diag, &pos, &S, &piv, &part, &tt};
+    void* args[] = {(void*)&Z, &DPv, &osv, &Lt, &nn, &rk, &tolv, &diag, &pos, &S, &piv, &part, &tt, &sk};
     GP_CUDA(cudaLaunchCooperativeKernel(fn1, dim3(grid1), dim3(PCP_THREADS), args, sh, st));
     p->launches += 1;
   } else {
@@ -827,7 +892,6 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   GP_REQUIRE(k >= 1 && k <= 128, GP_E_SHAPE, "preconditioner rank %d not in [1,128]", k);
   GP_REQUIRE(Lt != nullptr && U != nullptr, GP_E_SHAPE, "Lt / U missing");
   GP_REQUIRE(p->same, GP_E_SHAPE, "the CIQ preconditioner needs a square operator");
-  GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "the CIQ preconditioner is not available for the SKI backend");
   GP_REQUIRE(!(p->comm && p->comm->world > 1) && p->row_begin == 0 && p->row_count == p->n2, GP_E_SHAPE,
              "gp_ciq_precond_build is not supported on row-sharded plans");
   const float* dvec = p->noise_diag;
@@ -880,13 +944,17 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   usolve_kernel<<<(unsigned)cdiv(n, 32 * WS_BLOCKS), 128, shu, st>>>(Lt, k, n, d_T, dvec, 1.0 / sqrt((double)p->noise), U);
   p->launches += 1;
   GP_CUDA(cudaGetLastError());
-  // tr(K - L L^T): the diagonal of a stationary kernel (sum) is its (summed) outputscale, as gp_kdiag fills it
-  double os_total = p->outputscale;
+  // tr(K - L L^T): the diagonal of a stationary kernel (sum) is its (summed) outputscale, as gp_kdiag fills it; the SKI diagonal
+  // w_i^T K_uu w_i varies from row to row and is summed in fp64
+  double tr_k = (double)n * p->outputscale;
   if (p->backend == GP_BACKEND_SUM) {
-    os_total = 0.0;
+    double os_total = 0.0;
     for (const gp_plan* q : p->terms) os_total += q->outputscale;
+    tr_k = (double)n * os_total;
+  } else if (p->backend == GP_BACKEND_SKI) {
+    GP_CHECK(ski_diag_sum(p, &tr_k));
   }
-  if (trace_resid_out) *trace_resid_out = (double)n * os_total - lsq;
+  if (trace_resid_out) *trace_resid_out = tr_k - lsq;
   GP_CUDA(cudaStreamSynchronize(st));
   return GP_OK;
 }

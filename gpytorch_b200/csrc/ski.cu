@@ -24,6 +24,7 @@
 #include <algorithm>
 
 #include "gp_common.cuh"
+#include "ski_rows.cuh"
 
 namespace gp {
 
@@ -769,6 +770,93 @@ int ski_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   }
   set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
   return GP_E_SHAPE;
+}
+
+// ---- single entries (ski_rows.cuh): the diagonal, requested rows and the pivoted Cholesky (pivchol.cu) ----------------------------
+int ski_rows_args(const gp_plan* p, SkiRows* s) {
+  const gp_ski_state* k = p->ski;
+  GP_REQUIRE(k != nullptr && k->T.p != nullptr, GP_E_STATE, "SKI grid not packed");
+  s->d = p->d;
+  int toff = 0, uoff = 0;
+  for (int i = 0; i < 4; ++i) {
+    const bool live = i < p->d;
+    s->G[i] = live ? k->G[i] : 0;
+    s->toff[i] = toff;
+    s->uoff[i] = uoff;
+    if (live) { toff += k->G[i] * k->G[i]; uoff += k->G[i]; }
+  }
+  s->usum = uoff;
+  s->os = p->outputscale;
+  s->T = k->T.as<float>();
+  s->first = k->first.as<int>();
+  s->wts = k->wts.as<float>();
+  return GP_OK;
+}
+
+__global__ void ski_kdiag_kernel(const SkiRows s, int64_t n, float* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = ski_diag_entry(s, i);
+}
+
+// OUT[r][j] = K_ski(idx[r], j): blockIdx.y = r, u of row idx[r] staged by every CTA of the row
+__global__ void __launch_bounds__(256)
+ski_krows_kernel(const SkiRows s, const int64_t* __restrict__ idx, int64_t n, float* __restrict__ out, int64_t ldo) {
+  __shared__ float u[SKI_U_MAX];
+  const int64_t i = idx[blockIdx.y];
+  ski_stage_u(s, i, u, threadIdx.x, 256);
+  __syncthreads();
+  const int64_t j = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (j < n) out[(int64_t)blockIdx.y * ldo + j] = ski_entry(s, u, j);
+}
+
+// per-CTA fp64 partial sums of the diagonal (fixed order in the CTA and on the host: reproducible)
+__global__ void __launch_bounds__(256) ski_diag_sum_kernel(const SkiRows s, int64_t n, double* __restrict__ part) {
+  __shared__ double sh[256];
+  double acc = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) acc += (double)ski_diag_entry(s, i);
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) part[blockIdx.x] = sh[0];
+}
+
+int ski_kdiag(gp_plan* p, float* OUT) {
+  SkiRows s;
+  GP_CHECK(ski_rows_args(p, &s));
+  ski_kdiag_kernel<<<(unsigned)cdiv(p->n1, 256), 256, 0, p->stream>>>(s, p->n1, OUT);
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
+int ski_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
+  GP_REQUIRE(m <= 65535, GP_E_SHAPE, "SKI row extraction takes at most 65535 rows per call (got %lld)", (long long)m);
+  SkiRows s;
+  GP_CHECK(ski_rows_args(p, &s));
+  ski_krows_kernel<<<dim3((unsigned)cdiv(p->n1, 256), (unsigned)m), 256, 0, p->stream>>>(s, idx, p->n1, OUT, ldo);
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
+int ski_diag_sum(gp_plan* p, double* out) {
+  SkiRows s;
+  GP_CHECK(ski_rows_args(p, &s));
+  const int gs = (int)std::max<int64_t>(1, std::min<int64_t>(cdiv(p->n1, 256), 2 * (int64_t)p->n_sm));
+  GP_CHECK(p->misc.ensure(sizeof(double) * gs));
+  ski_diag_sum_kernel<<<gs, 256, 0, p->stream>>>(s, p->n1, p->misc.as<double>());
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  std::vector<double> h(gs);
+  GP_CUDA(cudaMemcpyAsync(h.data(), p->misc.p, sizeof(double) * gs, cudaMemcpyDeviceToHost, p->stream));
+  GP_CUDA(cudaStreamSynchronize(p->stream));
+  double acc = 0.0;
+  for (int b = 0; b < gs; ++b) acc += h[b];
+  *out = acc;
+  return GP_OK;
 }
 
 }  // namespace gp

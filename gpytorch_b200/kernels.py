@@ -172,7 +172,8 @@ class ScaleKernel(Kernel):
         os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
         from .operators import SKIKernelLinearOperator
         if isinstance(base, SKIKernelLinearOperator):
-            return SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
+            op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
+            return op.diagonal() if diag else op
         op = KernelLinearOperator(base.x1, base.x2, base.kind, base.lengthscale, os_)
         return op.diagonal() if diag else op
 
@@ -260,6 +261,4 @@ class GridInterpolationKernel(Kernel):
         ls = self.base_kernel.lengthscale.reshape(-1)
         ls = ls[0] if ls.numel() == 1 else ls
         op = SKIKernelLinearOperator(x1, self.base_kernel.kind, ls, None, self.grid_sizes, lo, step)
-        if diag:
-            raise NotImplementedError("diag=True for the SKI operator")
-        return op
+        return op.diagonal() if diag else op

@@ -547,7 +547,10 @@ class SKIKernelLinearOperator(KernelLinearOperator):
         return torch.cat([self.plan().kmv(eye[:, c0:c0 + 16].contiguous()) for c0 in range(0, n, 16)], -1)
 
     def diagonal(self, dim1=-2, dim2=-1):
-        raise NotImplementedError("diagonal of the SKI operator")
+        """s w_i^T K_uu w_i per row (gp_kdiag on the SKI plan): not constant, unlike a stationary kernel's."""
+        return self.plan().diag()
+
+    _diagonal = diagonal
 
     def __getitem__(self, index):
         """Rows / columns of the interpolated operator: K[r, c] = W[r] K_uu W[c]^T (the reference slices the interpolation
@@ -791,8 +794,10 @@ class AddedDiagLinearOperator(_SamplingMixin):
         n = self.shape[0]
         if settings.max_preconditioner_size.value() == 0 or n < settings.min_preconditioning_size.value():
             return None, None, 0.0
-        if isinstance(self.kernel_op, SKIKernelLinearOperator):
-            return None, None, 0.0      # the reference's interpolated operator has no pivoted-Cholesky preconditioner either
+        if isinstance(self.kernel_op, SKIKernelLinearOperator) and settings.ski_preconditioner.off():
+            # Off by default so that existing SKI results do not change; whether the reference preconditions interpolated
+            # operators (linear_operator, absent here) is not established.  settings.ski_preconditioner documents the choice.
+            return None, None, 0.0
         if self._precond_cache is None:
             p = self._plan()
             lt, piv, st = p.pivoted_cholesky(settings.max_preconditioner_size.value(), settings.preconditioner_tolerance.value())

@@ -120,7 +120,8 @@ class ciq_preconditioner(_feature_flag):
     msMINRES then needs about sqrt(kappa(A)) instead of sqrt(kappa(K_hat)) iterations.  The draw has the same distribution
     N(0, K_hat) but is a different root applied to the same xi: off, samples are K_hat^{1/2} xi, continuous in the
     hyper-parameters (common random numbers across a sweep); on, they jump where the pivot order changes.  No effect where the
-    solves have no preconditioner (SKI, no noise, n < min_preconditioning_size, max_preconditioner_size(0), a failed build)."""
+    solves have no preconditioner (SKI without ski_preconditioner, no noise, n < min_preconditioning_size,
+    max_preconditioner_size(0), a failed build)."""
     _default = False
 
 
@@ -223,6 +224,17 @@ class fast_computations:
 class backend(_value_context):
     """'auto' | 'tcgen05' | 'simt': which fused K.V kernel the engine runs."""
     _global_value = "auto"
+
+
+class ski_preconditioner(_feature_flag):
+    """Precondition solves of a SKI / KISS-GP operator (GridInterpolationKernel) with the pivoted-Cholesky preconditioner of the
+    dense kernels (same knobs: max_preconditioner_size, min_preconditioning_size, preconditioner_tolerance).  The pivoted
+    Cholesky reads exact entries of K_ski = s W K_uu W^T from its separable form (csrc/ski_rows.cuh); the N(0, P) probes, mBCG
+    with the preconditioner, the prediction mean cache and, with ciq_preconditioner, the split-preconditioned CIQ sampler then
+    pick it up as they do for dense kernels.  Off by default because turning it on changes results of existing SKI runs: the
+    probe distribution and the log-det estimator of the MLL, and the root that preconditioned CIQ applies to xi.  Whether the
+    reference preconditions interpolated operators by default is not established here."""
+    _default = False
 
 
 class probe_seed(_value_context):

@@ -87,7 +87,8 @@ int gp_plan_set_noise_diag(gp_plan* plan, const float* diag, int64_t n);
  * the plan's operator becomes K_ski = W (T_0 x ... x T_{d-1}) W^T with cubic interpolation onto a regular grid; grid_lo[i] /
  * grid_step[i] are the first node and the spacing of dimension i (utils/grid.py:142-180), grid_sizes[i] in [4, 128], d <= 4.
  * Call after gp_plan_set_data (square operator); products, mBCG, SLQ, gp_mll (without preconditioner) and gp_lanczos then run
- * on the interpolated operator.  Out-of-bounds inputs fail like the reference ("Received data that was out of bounds ..."). */
+ * on the interpolated operator, and gp_kdiag, gp_krows, gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg with W,
+ * gp_ciq_precond_build and gp_ciq_sqrt_matmul_precond accept it (a preconditioned SKI MLL combines these primitives).  Out-of-bounds inputs fail like the reference ("Received data that was out of bounds ..."). */
 int gp_plan_set_ski(gp_plan* plan, const int* grid_sizes, const float* grid_lo, const float* grid_step, int d);
 
 /* Kernel sums (AdditiveKernel, kernels/kernel.py:592-621: k = k_1 + ... + k_m, each term with its own covariance function,
@@ -108,10 +109,10 @@ int gp_plan_set_sum(gp_plan* plan, gp_plan* const* terms, int n_terms);
 int gp_kmv(gp_plan* plan, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo, int add_noise);
 
 /* OUT[m, n2] = K(X1[idx], X2): row extraction, LazyEvaluatedKernelTensor._getitem (:136-243);
- * idx is a DEVICE int64 array. */
+ * idx is a DEVICE int64 array.  SKI plans: exact entries s prod_k w_ik^T T_k w_jk from the separable form, m <= 65535. */
 int gp_krows(gp_plan* plan, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
 
-/* OUT[n1] = diag K(X1,X1): LazyEvaluatedKernelTensor._diagonal (:107-133). */
+/* OUT[n1] = diag K(X1,X1): LazyEvaluatedKernelTensor._diagonal (:107-133).  SKI plans: s prod_k w_ik^T T_k w_ik (not constant). */
 int gp_kdiag(gp_plan* plan, float* OUT);
 
 /* d/d(theta) sum_ij sum_s Lf[i,s] K_theta(x_i,x_j) Rt[j,s]: LazyEvaluatedKernelTensor.
@@ -125,7 +126,9 @@ int gp_bilinear_grad(gp_plan* plan, const float* Lf, int64_t ldl, const float* R
 
 /* Greedy pivoted partial Cholesky of K(X1,X1) (outputscale included, no noise):
  * linear_operator.functions._pivoted_cholesky, surfaced at gpytorch/__init__.py:146-173.
- * Lt [rank, n] row-major (= L^T), piv int64[rank] (device), *rank_out <= rank. */
+ * Lt [rank, n] row-major (= L^T), piv int64[rank] (device), *rank_out <= rank.  Dense, kernel-sum and SKI plans; for SKI the
+ * initial diagonal is not constant: the first pivot is its argmax (earliest index on ties) and the error is sum|diag| / max diag.
+ * Kernel sums and SKI need the cooperative (persistent) kernel. */
 int gp_pivoted_cholesky(gp_plan* plan, int rank, float error_tol, float* Lt, int64_t* piv,
                         int* rank_out);
 
@@ -172,7 +175,8 @@ int gp_ciq_sqrt_matmul(gp_plan* plan, const float* B, int64_t ldb, int t, const 
 
 /* Split factor of the pivoted-Cholesky preconditioner P = L L^T + D for the CIQ sampler, from Lt [k, n] (1 <= k <= 128):
  * U [n, k] with F^-1 = (I - U U^T) D^-1/2 for F = D^1/2 (I + M M^T)^1/2, M = D^-1/2 L (eigh of L^T D^-1 L in fp64 on the host);
- * *trace_resid_out = tr(K - L L^T) in fp64.  Needs noise > 0 (all d > 0); square, unsharded, non-SKI plans.
+ * *trace_resid_out = tr(K - L L^T) in fp64 (SKI plans: the fp64 sum of the SKI diagonal).  Needs noise > 0 (all d > 0); square,
+ * unsharded plans.
  * A non-finite Gram returns GP_W_PIVCHOL_NAN (the caller drops the preconditioner). */
 int gp_ciq_precond_build(gp_plan* plan, const float* Lt, int k, float* U, double* trace_resid_out);
 

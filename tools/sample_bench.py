@@ -13,8 +13,7 @@ fixed 10- and 30-iteration runs next to the fused K.V launch alone (gp_time_kmv_
 the same two runs.  At c2 it also times dense fp32 Cholesky sampling of the same xi and reports the largest difference.
 --precond-rank takes a comma-separated list of ranks k (default 0: the unpreconditioned run only).  For k > 0 the run uses the
 split preconditioner of settings.ciq_preconditioner (gp_ciq_sqrt_matmul_precond) and also reports k, the build time (pivoted
-Cholesky + gp_ciq_precond_build, CUDA events) and the trace interval [m, M]; c5 (SKI) has no pivoted-Cholesky preconditioner and
-is reported as skipped.
+Cholesky + gp_ciq_precond_build, CUDA events) and the trace interval [m, M]; c5 (SKI) runs with settings.ski_preconditioner on.
 """
 from __future__ import annotations
 
@@ -78,6 +77,11 @@ def _timed(fn, flush, reps):
 
 
 def run(name, cfg, reps, dev, rank=0):
+    with settings.ski_preconditioner("grid" in cfg and rank > 0):
+        return _run(name, cfg, reps, dev, rank)
+
+
+def _run(name, cfg, reps, dev, rank):
     gen = torch.Generator().manual_seed(0)
     op = _operator(cfg, dev, gen)
     n, s, Q, tol = cfg["n"], 16, 15, 1e-4
@@ -156,10 +160,7 @@ def main():
             continue
         for rank in ranks:
             key = name if rank == 0 else f"{name}_k{rank}"
-            if rank > 0 and "grid" in cfg:
-                result["workloads"][key] = {"skipped": "SKI has no pivoted-Cholesky preconditioner"}
-            else:
-                result["workloads"][key] = run(name, cfg, a.reps, dev, rank)
+            result["workloads"][key] = run(name, cfg, a.reps, dev, rank)
             print(key, json.dumps(result["workloads"][key]), flush=True)
     with open(a.out, "w") as f:
         json.dump(result, f, indent=1)
