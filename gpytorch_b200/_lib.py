@@ -74,6 +74,7 @@ PROTOTYPES = {
     "gp_plan_set_noise_diag": (_I, [_P, _P, _L]),
     "gp_plan_set_ski": (_I, [_P, C.POINTER(_I), C.POINTER(_F), C.POINTER(_F), _I]),
     "gp_plan_set_sum": (_I, [_P, C.POINTER(_P), _I]),
+    "gp_plan_set_lowrank": (_I, [_P, _P, _L, _I]),
     "gp_kmv": (_I, [_P, _P, _L, _I, _P, _L, _I]),
     "gp_krows": (_I, [_P, _P, _L, _P, _L]),
     "gp_kdiag": (_I, [_P, _P]),

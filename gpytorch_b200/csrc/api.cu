@@ -100,7 +100,7 @@ extern "C" int gp_plan_destroy(gp_plan* p) {
   gp::DevBuf* bufs[] = {&p->mean, &p->scale, &p->Z1, &p->Z2, &p->XA, &p->XB, &p->V16, &p->Vtiles, &p->partial, &p->out16,
                         &p->cgU, &p->cgR, &p->cgZ, &p->cgP, &p->cgV, &p->cgPfull, &p->red, &p->sums, &p->qtr, &p->state,
                         &p->tmat_tmp, &p->misc, &p->misc2, &p->misc3, &p->pcdiag, &p->pcperm, &p->pcpos, &p->pcstate,
-                        &p->pcpart, &p->gram, &p->cholC, &p->part_scale, &p->msw};
+                        &p->pcpart, &p->gram, &p->cholC, &p->part_scale, &p->msw, &p->lrw};
   for (auto* b : bufs) b->release();
   if (p->ski) {
     gp::DevBuf* sb[] = {&p->ski->first, &p->ski->wts, &p->ski->gridA, &p->ski->gridB, &p->ski->gridC, &p->ski->gridD, &p->ski->T, &p->ski->dT, &p->ski->flag,
@@ -259,7 +259,8 @@ extern "C" int gp_mll(gp_plan* p, const float* y_minus_mean, const float* eps1, 
   int k = 0;
   double logdet_p = 0.0;
   const float* W = nullptr;
-  const bool want_precond = o->precond_rank > 0 && N >= o->min_precond_size && p->backend != GP_BACKEND_SKI;
+  // SKI and low-rank-corrected plans run unpreconditioned (no pivoted Cholesky of a downdated operator, lowrank.cu)
+  const bool want_precond = o->precond_rank > 0 && N >= o->min_precond_size && p->backend != GP_BACKEND_SKI && p->lr_U == nullptr;
   float* Lt = nullptr;
   if (want_precond) {
     int rank = (int)std::min<int64_t>(o->precond_rank, N);

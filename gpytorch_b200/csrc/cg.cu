@@ -542,6 +542,7 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   GP_REQUIRE(max_tridiag_iter <= max_iter, GP_E_SHAPE,
              "Getting a tridiagonalization larger than the number of CG iterations run is not possible!");
   GP_REQUIRE(W == nullptr || (k >= 1 && k <= KMAX), GP_E_SHAPE, "preconditioner rank %d not in [1,%d]", k, KMAX);
+  if (W != nullptr) GP_REFUSE_LOWRANK(p, "gp_mbcg with a preconditioner");
   cudaStream_t st = p->stream;
   const int64_t n = p->row_count;       // local rows
   const int64_t N = p->n2;              // global size
@@ -607,7 +608,10 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   const int64_t nchunk_pack = fuse_pack ? p->ntile_j * (TILE_J / 4) : 0;
   const int Gd = (int)std::min<int64_t>(cdiv(std::max<int64_t>(nchunk_pack, cdiv(n, (int64_t)4)) * 4, (int64_t)RP_THREADS), 4 * p->n_sm);
   auto kmv = [&]() -> int {
-    if (fuse_pack) return kmv_tc_launch(p, done);
+    if (fuse_pack) {   // the direction block's fp32 rows (Pfull) feed the low-rank slot
+      GP_CHECK(kmv_tc_launch(p, done));
+      return lowrank_partials(p, Pfull, done);
+    }
     if (sharded) GP_CHECK(nccl_allgather_float(p->comm, Pfull, (size_t)n * TP, st));
     return kmv_partials(p, Pfull, done);
   };
@@ -642,7 +646,7 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   bool finished = false;
   for (int kk = 0; kk < max_iter && !finished; ++kk) {
     if ((status = kmv()) != GP_OK) break;
-    cg_finishv_wtv_kernel<true><<<G, RP_THREADS, sh_b, st>>>(p->partial.as<float>(), p->nparts, p->rows_pad, p->outputscale, part_scale_ptr(p), p->noise, dvec, P, V,
+    cg_finishv_wtv_kernel<true><<<G, RP_THREADS, sh_b, st>>>(p->partial.as<float>(), nslots(p), p->rows_pad, p->outputscale, part_scale_ptr(p), p->noise, dvec, P, V,
                                                           nullptr, W, k, wp, n, red1, L1, done, p->xbad);
     cg_sum_launch(red1, G, L1, sums1, done, st);
     if ((status = allreduce(p, sums1, L1)) != GP_OK) break;

@@ -186,8 +186,14 @@ struct gp_plan {
   bool sum_any_tc = false;        // at least one term reads the packed V tiles
   float* partial_ext = nullptr;   // set on a TERM for the duration of one launch by its parent
   float* vtiles_ext = nullptr;
-  gp::DevBuf part_scale;          // [nparts] outputscale of the term that owns each partial slot
+  gp::DevBuf part_scale;          // [nslots] scale of each partial slot: the owning term's outputscale, 1 for the low-rank slot
   std::vector<float> part_scale_host;
+  // low-rank correction (lowrank.cu): the operator is  s K - U U^T ; U [n2, lr_r] (leading dimension lr_ld) is caller-owned
+  const float* lr_U = nullptr;
+  int64_t lr_ld = 0;
+  int64_t lr_n = 0;               // rows of U: the operator size when the correction was set (re-checked at every use)
+  int lr_r = 0;
+  gp::DevBuf lrw;                 // U^T V partials [G][16 r] | c = U^T V [r][16] fp64
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
 
@@ -207,8 +213,12 @@ int ski_pack(gp_plan* p);                                               // ski.c
 int ski_kmv_partials(gp_plan* p, const float* V16, const int* done_flag);
 int ski_bilinear(gp_plan* p, const float* L16, const float* R16, double* total);   // total[0] += <A, K_uu B>, total[1 + i] += <A, (l_i dK_uu/dl_i) B>
 int sum_pack(gp_plan* p);                                               // sum.cu: geometry / buffers of a kernel-sum plan
-int sum_prepare(gp_plan* p);                                            // refresh the per-slot outputscales (no-op for other plans)
+int slot_scales_prepare(gp_plan* p);                                    // refresh the per-slot scales (sum / low-rank plans only)
 int sum_kmv_launch(gp_plan* p, const float* V16, const int* done_flag); // one launch per term into the parent's partial slots
+int lowrank_partials(gp_plan* p, const float* V16, const int* done_flag);   // lowrank.cu: -U U^T V into the last slot (no-op without U)
+int lowrank_kdiag(gp_plan* p, float* OUT);                              // OUT[i] -= sum_j U_ij^2
+int lowrank_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);   // OUT[r] -= U[idx_r] U^T
+int sum_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);       // rows of a kernel sum (terms added in order)
 int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,   // cg.cu
              int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
              int* tridiag_size, float* resid_out);
@@ -216,8 +226,14 @@ int nccl_allreduce_double(gp_comm* c, double* buf, size_t count, cudaStream_t st
 int nccl_allgather_float(gp_comm* c, float* buf, size_t count_per_rank, cudaStream_t st);
 inline float* partial_ptr(gp_plan* p) { return p->partial_ext ? p->partial_ext : p->partial.as<float>(); }
 inline float* vtiles_ptr(gp_plan* p) { return p->vtiles_ext ? p->vtiles_ext : p->Vtiles.as<float>(); }
+// partial slots the finish kernels sum: the backend's nparts, plus the low-rank slot
+inline int nslots(const gp_plan* p) { return p->nparts + (p->lr_U ? 1 : 0); }
 // per-slot scales of the finish kernels: nullptr = one outputscale for all slots
-inline const float* part_scale_ptr(gp_plan* p) { return p->backend == GP_BACKEND_SUM ? p->part_scale.as<float>() : nullptr; }
+inline const float* part_scale_ptr(gp_plan* p) {
+  return (p->backend == GP_BACKEND_SUM || p->lr_U) ? p->part_scale.as<float>() : nullptr;
+}
+#define GP_REFUSE_LOWRANK(p, what) \
+  GP_REQUIRE((p)->lr_U == nullptr, GP_E_STATE, "%s is not available on a plan with a low-rank correction (gp_plan_set_lowrank)", what)
 inline bool plan_is_tc(const gp_plan* p) { return p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_tc); }
 
 __host__ __device__ inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }

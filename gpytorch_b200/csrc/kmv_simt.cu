@@ -105,7 +105,7 @@ int kmv_simt_launch(gp_plan* p, const float* V16, const int* done_flag) {
   return GP_E_SHAPE;
 }
 
-int kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
+static int kmv_partials_base(gp_plan* p, const float* V16, const int* done_flag) {
   if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, V16, done_flag);
   if (p->backend == GP_BACKEND_SUM) {
     if (p->sum_any_tc) GP_CHECK(pack_v_tiles(p, V16));
@@ -116,6 +116,12 @@ int kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
     return kmv_tc_launch(p, done_flag);
   }
   return kmv_simt_launch(p, V16, done_flag);
+}
+
+// the backend's slots, then the low-rank slot (lowrank.cu) when the plan has one
+int kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
+  GP_CHECK(kmv_partials_base(p, V16, done_flag));
+  return lowrank_partials(p, V16, done_flag);
 }
 
 // OUT[r, c] = os * sum_s partial[s][r][c] + noise * V16[row_begin + r][c]
@@ -146,7 +152,7 @@ int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t
   int64_t tot = p->row_count * TP;
   float na = (add_noise && p->same) ? p->noise : 0.f;
   const float* dv = (add_noise && p->same) ? p->noise_diag : nullptr;
-  kmv_finish_user_kernel<<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(p->partial.as<float>(), p->nparts, p->row_count,
+  kmv_finish_user_kernel<<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(p->partial.as<float>(), nslots(p), p->row_count,
                                                                           rows_pad, p->outputscale, part_scale_ptr(p), na, dv, V16, p->row_begin,
                                                                           OUT, ldo, t, p->xbad);
   p->launches++;
@@ -335,11 +341,21 @@ static int launch_bilinear(gp_plan* p, const float* L16, const float* R16, doubl
 
 using namespace gp;
 
+static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
+
 extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "row extraction of a kernel sum: call gp_krows on every term and add");
+  GP_REQUIRE(p->backend != GP_BACKEND_SUM || p->lr_U, GP_E_SHAPE, "row extraction of a kernel sum: call gp_krows on every term and add");
   GP_REQUIRE(m >= 0 && ldo >= p->n2, GP_E_SHAPE, "bad krows shape");
   if (m == 0) return GP_OK;
+  if (p->lr_U) {   // rows of the operator the plan multiplies: s K - U U^T
+    GP_CHECK(p->backend == GP_BACKEND_SUM ? sum_krows(p, idx, m, OUT, ldo) : krows_base(p, idx, m, OUT, ldo));
+    return lowrank_krows(p, idx, m, OUT, ldo);
+  }
+  return krows_base(p, idx, m, OUT, ldo);
+}
+
+static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   if (p->backend == GP_BACKEND_SKI) return ski_krows(p, idx, m, OUT, ldo);   // separable entries (ski_rows.cuh)
   const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
   dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
@@ -355,9 +371,27 @@ extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, i
   return GP_OK;
 }
 
+static int kdiag_base(gp_plan* p, float* OUT);
+
 extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "diagonal of a kernel sum: call gp_kdiag on every term and add");
+  GP_REQUIRE(p->backend != GP_BACKEND_SUM || p->lr_U, GP_E_SHAPE, "diagonal of a kernel sum: call gp_kdiag on every term and add");
+  if (p->lr_U) {   // diag(s K) - sum_j U_ij^2
+    if (p->backend == GP_BACKEND_SUM) {
+      // a low-rank plan is square: every stationary term contributes its constant outputscale, added in term order
+      float os = 0.f;
+      for (gp_plan* t : p->terms) os += t->outputscale;
+      fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, os);
+      p->launches++;
+    } else {
+      GP_CHECK(kdiag_base(p, OUT));
+    }
+    return lowrank_kdiag(p, OUT);
+  }
+  return kdiag_base(p, OUT);
+}
+
+static int kdiag_base(gp_plan* p, float* OUT) {
   if (p->backend == GP_BACKEND_SKI) return ski_kdiag(p, OUT);   // not constant: w_i^T K_uu w_i (ski_rows.cuh)
   if (p->same) {
     // stationary kernels: k(x,x) = outputscale (lazy_evaluated_kernel_tensor.py:107-133 evaluates kernel(diag=True))
@@ -383,6 +417,7 @@ extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
 extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float* Rt, int64_t ldr, int s,
                                 double* grad_ls, double* grad_os) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  GP_REFUSE_LOWRANK(p, "gp_bilinear_grad");
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "gradients of a kernel sum: call gp_bilinear_grad on every term");
   GP_REQUIRE(s >= 1, GP_E_SHAPE, "s must be >= 1");
   const bool ard = p->ls.size() > 1;

@@ -229,7 +229,7 @@ int pack_inputs(gp_plan* p) {
     GP_CHECK(p->Vtiles.ensure(sizeof(float) * p->ntile_j * (2 * TILE_J * TP + TILE_J * TP / 2)));
   }
   p->nparts = p->nsplit;
-  GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)p->nparts * p->rows_pad * TP));
+  GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)nslots(p) * p->rows_pad * TP));
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }

@@ -724,8 +724,9 @@ using namespace gp;
 
 extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float* Lt, int64_t* piv, int* rank_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  GP_REFUSE_LOWRANK(p, "gp_pivoted_cholesky");
   GP_REQUIRE(p->same, GP_E_SHAPE, "pivoted Cholesky needs a square operator");
-  GP_CHECK(sum_prepare(p));
+  GP_CHECK(slot_scales_prepare(p));
   const int64_t n = p->n2;
   GP_REQUIRE(n < (int64_t)1 << 31, GP_E_SHAPE, "n too large");
   rank = (int)std::min<int64_t>(rank, n);
@@ -845,6 +846,7 @@ static GramSplit gram_split(const gp_plan* p, int k, int64_t n) {
 
 extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, double* logdet_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  GP_REFUSE_LOWRANK(p, "gp_precond_build");
   GP_REQUIRE(k >= 1 && k <= 128, GP_E_SHAPE, "preconditioner rank %d not in [1,128]", k);
   const float* dvec = p->noise_diag;
   GP_REQUIRE(dvec != nullptr || p->noise > 0.f, GP_E_SHAPE, "preconditioner needs noise > 0");
@@ -889,6 +891,7 @@ extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, do
 
 extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U, double* trace_resid_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  GP_REFUSE_LOWRANK(p, "gp_ciq_precond_build");
   GP_REQUIRE(k >= 1 && k <= 128, GP_E_SHAPE, "preconditioner rank %d not in [1,128]", k);
   GP_REQUIRE(Lt != nullptr && U != nullptr, GP_E_SHAPE, "Lt / U missing");
   GP_REQUIRE(p->same, GP_E_SHAPE, "the CIQ preconditioner needs a square operator");
@@ -961,6 +964,7 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
 
 extern "C" int gp_precond_probes(gp_plan* p, const float* Lt, int k, const float* eps1, const float* eps2, int tp, float* Z) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  GP_REFUSE_LOWRANK(p, "gp_precond_probes");
   GP_REQUIRE(k >= 1 && tp >= 1 && (size_t)k * tp * 4 <= 40 * 1024, GP_E_SHAPE, "bad probe shape k=%d tp=%d", k, tp);
   int64_t tot = p->row_count * tp;
   probes_kernel<<<(unsigned)cdiv(tot, 256), 256, sizeof(float) * k * tp, p->stream>>>(Lt, k, p->n2, p->row_begin, p->row_count,

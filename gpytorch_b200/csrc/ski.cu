@@ -636,7 +636,7 @@ int ski_pack(gp_plan* p) {
   p->nsplit = 1;
   p->nparts = 1;
   p->rows_pad = cdiv(p->row_count, 2 * TILE_I) * 2 * TILE_I;
-  GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)p->rows_pad * TP));
+  GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)nslots(p) * p->rows_pad * TP));
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
@@ -803,6 +803,11 @@ __global__ void __launch_bounds__(256)
 ski_krows_kernel(const SkiRows s, const int64_t* __restrict__ idx, int64_t n, float* __restrict__ out, int64_t ldo) {
   __shared__ float u[SKI_U_MAX];
   const int64_t i = idx[blockIdx.y];
+  if (i < 0 || i >= n) {   // out-of-range row index (CTA-uniform): NaN row, as the dense row extraction, instead of an out-of-bounds read
+    const int64_t jj = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (jj < n) out[(int64_t)blockIdx.y * ldo + jj] = __int_as_float(0x7fc00000);
+    return;
+  }
   ski_stage_u(s, i, u, threadIdx.x, 256);
   __syncthreads();
   const int64_t j = (int64_t)blockIdx.x * 256 + threadIdx.x;

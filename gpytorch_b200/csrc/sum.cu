@@ -40,21 +40,32 @@ int sum_pack(gp_plan* p) {
   p->nparts = np;
   p->nsplit = np;
   p->xbad = p->terms[0]->xbad;   // the terms see the same rows: one non-finite flag serves all
-  GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)np * p->rows_pad * TP));
+  GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)nslots(p) * p->rows_pad * TP));
   if (any_tc) GP_CHECK(p->Vtiles.ensure(sizeof(float) * p->ntile_j * (2 * TILE_J * TP + TILE_J * TP / 2)));
-  GP_CHECK(p->part_scale.ensure(sizeof(float) * 64));
   p->part_scale_host.clear();
-  return sum_prepare(p);
+  return slot_scales_prepare(p);
 }
 
-// per-slot outputscales: refreshed whenever a term was re-packed with a new outputscale (cheap host compare per call)
-int sum_prepare(gp_plan* p) {
-  if (p->backend != GP_BACKEND_SUM) return GP_OK;
+// per-slot scales: a kernel sum scales each slot by the outputscale of the term that owns it, a low-rank plan scales the backend's
+// slots by its outputscale and its own last slot by 1.  Refreshed whenever a term was re-packed or the hyper-parameters changed
+// (cheap host compare per call); other plans keep one outputscale for all slots (part_scale_ptr = nullptr).
+int slot_scales_prepare(gp_plan* p) {
+  const bool sum = p->backend == GP_BACKEND_SUM;
+  if (!sum && !p->lr_U) return GP_OK;
   std::vector<float> sc;
-  for (gp_plan* t : p->terms)
-    for (int s = 0; s < t->nsplit; ++s) sc.push_back(t->outputscale);
-  GP_REQUIRE((int)sc.size() == p->nparts, GP_E_STATE, "kernel sum: a term changed its geometry (%d slots, expected %d); call gp_plan_set_sum again",
-             (int)sc.size(), p->nparts);
+  if (sum) {
+    for (gp_plan* t : p->terms)
+      for (int s = 0; s < t->nsplit; ++s) sc.push_back(t->outputscale);
+    GP_REQUIRE((int)sc.size() == p->nparts, GP_E_STATE, "kernel sum: a term changed its geometry (%d slots, expected %d); call gp_plan_set_sum again",
+               (int)sc.size(), p->nparts);
+  } else {
+    sc.assign(p->nparts, p->outputscale);
+  }
+  if (p->lr_U) sc.push_back(1.f);
+  if (sizeof(float) * sc.size() > p->part_scale.cap) {
+    GP_CHECK(p->part_scale.ensure(sizeof(float) * std::max<size_t>(64, sc.size())));
+    p->part_scale_host.clear();
+  }
   if (sc != p->part_scale_host) {
     p->part_scale_host = sc;
     // pageable source: staged by the runtime before the call returns
@@ -64,7 +75,7 @@ int sum_prepare(gp_plan* p) {
 }
 
 int sum_kmv_launch(gp_plan* p, const float* V16, const int* done_flag) {
-  GP_CHECK(sum_prepare(p));
+  GP_CHECK(slot_scales_prepare(p));
   int off = 0;
   for (gp_plan* t : p->terms) {
     GP_REQUIRE(t->backend == GP_BACKEND_TCGEN05 || V16 != nullptr, GP_E_STATE, "kernel sum: fp32 rows of V needed for a CUDA-core term");
@@ -77,6 +88,25 @@ int sum_kmv_launch(gp_plan* p, const float* V16, const int* done_flag) {
     p->launches++;
     off += t->nsplit;
   }
+  return GP_OK;
+}
+
+// rows of the sum: term 0 writes OUT, every later term writes scratch rows that are added in term order
+__global__ void add_rows_kernel(const float* __restrict__ src, int64_t m, int64_t n, float* __restrict__ OUT, int64_t ldo) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n) OUT[blockIdx.y * ldo + j] += src[blockIdx.y * n + j];
+}
+
+int sum_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
+  GP_REQUIRE(m <= 65535, GP_E_SHAPE, "rows of a kernel sum: at most 65535 rows per call (m=%lld)", (long long)m);
+  GP_CHECK(gp_krows(p->terms[0], idx, m, OUT, ldo));
+  if (p->terms.size() > 1) GP_CHECK(p->misc.ensure(sizeof(float) * (size_t)m * p->n2));
+  for (size_t t = 1; t < p->terms.size(); ++t) {
+    GP_CHECK(gp_krows(p->terms[t], idx, m, p->misc.as<float>(), p->n2));
+    add_rows_kernel<<<dim3((unsigned)cdiv(p->n2, 256), (unsigned)m), 256, 0, p->stream>>>(p->misc.as<float>(), m, p->n2, OUT, ldo);
+    p->launches++;
+  }
+  GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
 

@@ -135,6 +135,24 @@ class Plan:
         check(self.lib.gp_plan_set_noise_diag(self._h, _ptr(self._noise_diag), self._noise_diag.numel()))
         return self
 
+    def set_lowrank(self, u: torch.Tensor | None):
+        """Low-rank correction: the operator becomes s K - U U^T (+ noise).  u [n, r], 1 <= r <= 128; None clears it."""
+        if u is None or u.size(-1) == 0:
+            self._lowrank = None
+            check(self.lib.gp_plan_set_lowrank(self._h, _ptr(None), 0, 0))
+            return self
+        _require_cuda_f32(u, "low-rank factor")
+        if u.device != self.device:
+            raise RuntimeError(f"low-rank factor lives on {u.device}, the plan on {self.device}")
+        if u.dim() != 2 or u.size(0) != self.n2:
+            raise RuntimeError(f"low-rank factor must be [{self.n2}, r] (got {tuple(u.shape)})")
+        if u.stride(-1) != 1:
+            u = u.contiguous()
+        self._lowrank = u                         # keep it alive: the engine holds the raw pointer
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_lowrank(self._h, _ptr(u), u.stride(0), u.size(1)))
+        return self
+
     def info(self):
         b, s, k, m = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         check(self.lib.gp_plan_info(self._h, C.byref(b), C.byref(s), C.byref(k), C.byref(m)))

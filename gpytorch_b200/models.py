@@ -6,6 +6,18 @@ from . import settings
 from .distributions import MultivariateNormal
 from .likelihoods import _GaussianLikelihoodBase
 from .module import Module
+from .operators import LOWRANK_MAX_RANK, LowRankUpdatedKernelLinearOperator
+
+
+def _posterior_covar_mode(k_ss) -> str:
+    """Which posterior covariance an exact GP returns: 'skip' (zeros), 'lazy_love' (K** - U U^T as an engine operator: with
+    settings.fast_pred_samples, which turns LOVE on by itself as in exact_prediction_strategies.py:787-826, when K** is a
+    plan-backed non-SKI operator without batch dimension on an unsharded plan), 'love' (dense LOVE) or 'exact'."""
+    if settings.skip_posterior_variances.on():
+        return "skip"
+    if settings.fast_pred_samples.on():
+        return "lazy_love" if LowRankUpdatedKernelLinearOperator.supports(k_ss) else "love"
+    return "love" if settings.fast_pred_var.on() else "exact"
 
 
 class ExactGP(Module):
@@ -56,9 +68,10 @@ class ExactGP(Module):
             test_mean = full_mean[..., n:] + k_star.matmul(self._mean_cache)  # :396
             m = test_x.size(-2)
             dense = lambda a: a if torch.is_tensor(a) else a.to_dense()  # noqa: E731
-            if settings.skip_posterior_variances.on():       # exact_prediction_strategies.py:432-433
+            mode = _posterior_covar_mode(k_ss)
+            if mode == "skip":                               # exact_prediction_strategies.py:432-433
                 covar = torch.zeros(m, m, device=test_x.device)
-            elif settings.fast_pred_var.on():                # LOVE: :268-272 (cache), :464-478 (use)
+            elif mode in ("love", "lazy_love"):              # LOVE: :268-272 (cache), :464-478 (use)
                 if self._covar_cache is None:
                     init = None
                     if settings.probe_seed.value() is not None:
@@ -66,7 +79,10 @@ class ExactGP(Module):
                         init = torch.randn(n, generator=g).to(train_x.device)
                     self._covar_cache = khat.root_inv_decomposition(init).detach()   # [n, J], R R^T ~= K_hat^{-1}
                 root = k_star.matmul(self._covar_cache)      # covar_inv_quad_form_root, [m, J]
-                covar = dense(k_ss) - root @ root.transpose(-1, -2)
+                if mode == "lazy_love" and root.size(-1) <= LOWRANK_MAX_RANK:
+                    covar = LowRankUpdatedKernelLinearOperator(k_ss, root.detach())
+                else:
+                    covar = dense(k_ss) - root @ root.transpose(-1, -2)
             else:
                 rhs = dense(full_covar[:n, n:])          # K(train, test) [n, m]
                 corr = k_star.matmul(khat.solve(rhs))    # exact predictive covariance, :435-462

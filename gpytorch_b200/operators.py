@@ -459,7 +459,7 @@ class SumKernelLinearOperator(KernelLinearOperator):
         terms = [o.plan(0.0) for o in self.ops]
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
         with _PLAN_LOCK:
-            key = ("sum", tuple(id(t) for t in terms))
+            key = ("sum", tuple(id(t) for t in terms), getattr(self, "_plan_slot", 0))
             parent = _SUM_PLANS.pop(key, None)
             if parent is None:
                 parent = Plan(self.x1, None if self.same else self.x2, backend="auto", row_begin=self._row_begin,
@@ -619,6 +619,177 @@ class _SKISliceOperator:
 
     def to_dense(self):
         return self.matmul(torch.eye(self.cols.numel(), device=self.device))
+
+
+_LOWRANK_SLOT = 8   # plan-cache slot of low-rank operators (kernel-sum terms use 1..4): a plain operator never sees their U
+LOWRANK_MAX_RANK = 128
+
+
+class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
+    """K** - U U^T kept lazy: the LOVE posterior covariance K** - K*x R R^T Kx* with U = K*x R [m, J] (the reference's
+    `test_test_covar + MatmulLinearOperator(root, -root^T)`, models/exact_prediction_strategies.py:464-478).  Every product,
+    diagonal and row runs on the engine plan of K** with the correction as one more partial slot (csrc/lowrank.cu), so nothing
+    m x m exists unless to_dense() is asked for.
+
+    `base` is a plan-backed square KernelLinearOperator or SumKernelLinearOperator (not SKI, not row-sharded), 1 <= J <= 128.  The
+    operator has its own plan-cache slot and sets U on that plan whenever U's storage or version changes.  It is detached: it
+    exposes no hyper-parameter tensors (gradients still reach the posterior mean and the right-hand side of log_prob).  No
+    preconditioner is built for it (AddedDiagLinearOperator._preconditioner returns none).
+
+    Sampling is _SamplingMixin's: CIQ with settings.ciq_samples, the dense psd-safe Cholesky up to max_cholesky_size, else a device
+    Lanczos root.  For the observed posterior K** - U U^T + sigma^2 I the CIQ interval starts at the noise floor sigma^2 (min d_i
+    for a per-row diagonal).  That floor is valid because the LOVE posterior dominates the exact one: R R^T = Q (Q^T K_hat Q)^-1 Q^T
+    <= K_hat^-1 for the Lanczos basis Q of K_hat = K_xx + D, hence K** - K*x R R^T Kx* >= K** - K*x K_hat^-1 Kx* >= 0.  The
+    noise-free latent posterior has no floor and falls back to the Ritz interval."""
+
+    def __init__(self, base, U: torch.Tensor):
+        if not self.supports(base):
+            raise RuntimeError("LowRankUpdatedKernelLinearOperator needs a square, unsharded, plan-backed kernel operator or "
+                               "kernel sum (not SKI)")
+        if U.dim() != 2 or U.size(0) != base.shape[0] or not 1 <= U.size(1) <= LOWRANK_MAX_RANK:
+            raise RuntimeError(f"low-rank factor must be [{base.shape[0]}, r] with 1 <= r <= {LOWRANK_MAX_RANK} (got {tuple(U.shape)})")
+        self.base = base.detach()
+        self.base._plan_slot = _LOWRANK_SLOT
+        self.U = U.detach().float().contiguous()
+
+    @staticmethod
+    def supports(base) -> bool:
+        """A plan-backed non-SKI kernel operator (or kernel sum) without batch dimension on an unsharded square plan."""
+        return (isinstance(base, KernelLinearOperator) and not isinstance(base, SKIKernelLinearOperator) and base.same
+                and base._comm is None and base._row_begin == 0 and base._row_count in (0, base.shape[0]))
+
+    def plan(self, noise=0.0) -> Plan:
+        p = self.base.plan(noise)
+        cur = getattr(p, "_lowrank", None)
+        if cur is None or cur.data_ptr() != self.U.data_ptr() or cur.shape != self.U.shape or p._lowrank_version != self.U._version:
+            p.set_lowrank(self.U)
+            p._lowrank_version = self.U._version
+        return p
+
+    def _sampling_plan(self) -> Plan:
+        """The plan of K** - U U^T alone: no noise, no per-row diagonal left over from an earlier + D."""
+        p = self.plan(0.0)
+        if getattr(p, "_noise_diag", None) is not None:
+            p.set_noise_diag(None)
+        return p
+
+    def _any_plan(self) -> Plan:
+        return self.plan(getattr(self, "_last_noise", 0.0))   # products / rows / diagonal ignore the plan's noise
+
+    @property
+    def shape(self):
+        return self.base.shape
+
+    def size(self, dim=None):
+        return self.shape if dim is None else self.shape[dim]
+
+    @property
+    def dtype(self):
+        return self.base.dtype
+
+    @property
+    def device(self):
+        return self.base.device
+
+    @property
+    def batch_shape(self):
+        return torch.Size([])
+
+    @property
+    def matrix_shape(self):
+        return self.shape
+
+    def _size(self):
+        return self.shape
+
+    def dim(self):
+        return 2
+
+    ndimension = dim
+
+    def numel(self):
+        return self.shape[0] * self.shape[1]
+
+    @property
+    def requires_grad(self):
+        return False
+
+    def evaluate_kernel(self):
+        return self
+
+    def representation(self):
+        return (self.U,)
+
+    def hyper_tensors(self):
+        return []
+
+    def _bilinear_derivative_list(self, left, right):
+        return []
+
+    def transpose(self, dim1, dim2):
+        return self          # symmetric
+
+    def t(self):
+        return self
+
+    _transpose_nonbatch = t
+
+    @property
+    def mT(self):
+        return self
+
+    def detach(self):
+        return self
+
+    def matmul(self, rhs):
+        return _LowRankMatmul.apply(self, rhs)
+
+    __matmul__ = matmul
+    _matmul = matmul
+
+    def diagonal(self, dim1=-2, dim2=-1):
+        """diag(K**) - sum_j U_ij^2 (gp_kdiag on the low-rank plan)."""
+        return self._any_plan().diag()
+
+    _diagonal = diagonal
+
+    def to_dense(self):
+        """Rows of K** - U U^T (gp_krows on the low-rank plan): the m x m matrix, for the dense branch only."""
+        p = self._any_plan()
+        return p.rows(torch.arange(self.shape[0], device=self.device))
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("LowRankUpdatedKernelLinearOperator only adds a (Constant)DiagLinearOperator")
+
+    def _with_zero_diag(self):
+        return AddedDiagLinearOperator(self, ConstantDiagLinearOperator(torch.zeros((), device=self.device), self.shape[0]))
+
+    def inv_quad_logdet(self, inv_quad_rhs=None, logdet=False, reduce_inv_quad=True):
+        """log_prob of the latent (noise-free) posterior: the solves of K** - U U^T itself -- the dense Cholesky up to
+        max_cholesky_size, else unpreconditioned mBCG + SLQ -- as a dense posterior covariance gets them from its Cholesky
+        factor.  The latent posterior can be close to singular; likelihood(post) adds the noise."""
+        return self._with_zero_diag().inv_quad_logdet(inv_quad_rhs, logdet=logdet, reduce_inv_quad=reduce_inv_quad)
+
+    def solve(self, rhs, lhs=None):
+        return self._with_zero_diag().solve(rhs, lhs)
+
+    def add_jitter(self, jitter_val=1e-3):
+        return AddedDiagLinearOperator(self, ConstantDiagLinearOperator(torch.tensor(jitter_val, device=self.device), self.shape[0]))
+
+
+class _LowRankMatmul(torch.autograd.Function):
+    """(K** - U U^T) rhs; the operator is symmetric and detached, so only the right-hand side gets a gradient."""
+
+    @staticmethod
+    def forward(ctx, op, rhs):
+        ctx.op = op
+        return op._any_plan().kmv(rhs.detach().float())
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        return None, ctx.op._any_plan().kmv(grad_out.contiguous())
 
 
 class _KernelMatmul(torch.autograd.Function):
@@ -794,6 +965,8 @@ class AddedDiagLinearOperator(_SamplingMixin):
         n = self.shape[0]
         if settings.max_preconditioner_size.value() == 0 or n < settings.min_preconditioning_size.value():
             return None, None, 0.0
+        if isinstance(self.kernel_op, LowRankUpdatedKernelLinearOperator):
+            return None, None, 0.0           # no pivoted Cholesky of a downdated operator (the engine refuses it)
         if isinstance(self.kernel_op, SKIKernelLinearOperator) and settings.ski_preconditioner.off():
             # Off by default so that existing SKI results do not change; whether the reference preconditions interpolated
             # operators (linear_operator, absent here) is not established.  settings.ski_preconditioner documents the choice.

@@ -145,6 +145,22 @@ class fast_pred_var(_feature_flag):
     _default = False
 
 
+class fast_pred_samples(_feature_flag):
+    """Fast predictive samples using Lanczos Variance Estimates (LOVE).
+    Use this for improved performance when sampling from a predictive posterior matrix.
+
+    As described in the paper: `Constant-Time Predictive Distributions for Gaussian Processes`_.
+
+    (settings.py:225-243.)  Here: an exact GP's posterior in eval mode keeps its LOVE covariance K** - K*x R R^T Kx* lazy
+    (operators.LowRankUpdatedKernelLinearOperator), so that variances, CIQ samples and log_prob at m test points never build an
+    m x m matrix.  Off by default.
+
+    .. _`Constant-Time Predictive Distributions for Gaussian Processes`:
+        https://arxiv.org/abs/1803.06058
+    """
+    _default = False
+
+
 class skip_posterior_variances(_feature_flag):
     """Return a zero predictive covariance (models/exact_prediction_strategies.py:432-433)."""
     _default = False

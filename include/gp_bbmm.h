@@ -101,6 +101,19 @@ int gp_plan_set_ski(gp_plan* plan, const int* grid_sizes, const float* grid_lo, 
  * Hyper-parameter gradients: gp_bilinear_grad on each term plan. */
 int gp_plan_set_sum(gp_plan* plan, gp_plan* const* terms, int n_terms);
 
+/* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
+ * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
+ * (+ its noise / per-row diagonal where a call adds it).  U: device [n, r] fp32, leading dimension ldu, caller-owned, must outlive
+ * the plan's use of it; 1 <= r <= 128.  U = NULL or r = 0 clears it.  Square, unsharded plans of every backend (tensor-core,
+ * SIMT, kernel sum, SKI); GP_E_SHAPE otherwise.  The correction is one more partial slot of every product (U^T V reduced in a
+ * fixed order: repeated products are bit-identical), so gp_kmv, gp_mbcg without W, gp_lanczos, gp_slq_logdet, gp_ciq_sqrt_matmul
+ * and gp_mll (unpreconditioned) run on it; gp_kdiag returns diag(s K) - sum_j U_ij^2 and gp_krows the rows of s K - U U^T (also
+ * for kernel sums).  gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond,
+ * gp_bilinear_grad and gp_mbcg with W return GP_E_STATE while a correction is set; gp_mll skips its preconditioner.  A later
+ * gp_plan_set_data / gp_plan_set_comm that changes the size or shards the plan makes every call that applies the correction
+ * return GP_E_STATE until gp_plan_set_lowrank is called again. */
+int gp_plan_set_lowrank(gp_plan* plan, const float* U, int64_t ldu, int r);
+
 /* ---- kernel seam (LazyEvaluatedKernelTensor, lazy/lazy_evaluated_kernel_tensor.py) --- */
 
 /* OUT[n1_local, t] = K(X1,X2) V [+ noise * V when add_noise and X2 == X1].
@@ -109,7 +122,8 @@ int gp_plan_set_sum(gp_plan* plan, gp_plan* const* terms, int n_terms);
 int gp_kmv(gp_plan* plan, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo, int add_noise);
 
 /* OUT[m, n2] = K(X1[idx], X2): row extraction, LazyEvaluatedKernelTensor._getitem (:136-243);
- * idx is a DEVICE int64 array.  SKI plans: exact entries s prod_k w_ik^T T_k w_jk from the separable form, m <= 65535. */
+ * idx is a DEVICE int64 array; an index outside [0, n1) gives a row of NaN (every backend).  SKI plans: exact entries
+ * s prod_k w_ik^T T_k w_jk from the separable form, m <= 65535. */
 int gp_krows(gp_plan* plan, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
 
 /* OUT[n1] = diag K(X1,X1): LazyEvaluatedKernelTensor._diagonal (:107-133).  SKI plans: s prod_k w_ik^T T_k w_ik (not constant). */
