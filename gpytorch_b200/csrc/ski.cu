@@ -18,6 +18,9 @@
 //   gather   out = W U'           per tile: node block staged in shared memory, 4^d reads per (row, column group) from there,
 //                                 written as the K.V partial block the mBCG finish kernels read (outputscale / noise applied there)
 // and the bilinear derivative (hyper-parameter gradients) is d + 1 sweeps of the mode products between two scatters and a dot.
+// Prediction on the grid (gp_ski_grid_matmul / gp_ski_interp_matmul, the reference's InterpolatedPredictionStrategy) reuses the
+// scatter and the mode products to build grid caches s K_uu W^T V, and interpolates a user grid matrix C [M][t] to the points
+// with ski_interp_tiled_kernel, the gather generalised to any t.
 // HBM/L2-bound: algorithmic bytes per product (SURVEY.md section 8f) = N 4^d (4 + 8) B as the reference stores W explicitly.
 #include <math.h>
 
@@ -642,16 +645,20 @@ int ski_pack(gp_plan* p) {
 }
 
 template <int D>
-static int ski_matmul_d(gp_plan* p, const float* V16, int t, float* OUT16) {
-  gp_ski_state* s = p->ski;
-  cudaStream_t st = p->stream;
-  const int64_t n = p->n1;
+static SkiGeom ski_geom(const gp_ski_state* s) {
   SkiGeom g;
   g.d = D;
   g.M = 1;
   for (int i = D - 1; i >= 0; --i) { g.G[i] = s->G[i]; g.lo[i] = s->lo[i]; g.step[i] = s->step[i]; g.stride[i] = g.M; g.M *= s->G[i]; }
-  (void)t;
-  (void)n;
+  return g;
+}
+
+// scatter + d mode products: *grid_out = (T_0 x ... x T_{d-1}) W^T V16, a [M][16] block (gridA or gridB)
+template <int D>
+static int ski_grid_apply_d(gp_plan* p, const float* V16, float** grid_out) {
+  gp_ski_state* s = p->ski;
+  cudaStream_t st = p->stream;
+  const SkiGeom g = ski_geom<D>(s);
   float* A = s->gridA.as<float>();
   float* B = s->gridB.as<float>();
   const SkiTiles tl = ski_tiles_of(s, D);
@@ -676,8 +683,24 @@ static int ski_matmul_d(gp_plan* p, const float* V16, int t, float* OUT16) {
     toff += (size_t)G * G;
     std::swap(cur, nxt);
   }
-  ski_gather_tiled_kernel<D><<<tgrid, 256, tsm, st>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, cur, OUT16);
-  p->launches += 2 + D;
+  p->launches += 1 + D;
+  GP_CUDA(cudaGetLastError());
+  *grid_out = cur;
+  return GP_OK;
+}
+
+template <int D>
+static int ski_matmul_d(gp_plan* p, const float* V16, float* OUT16) {
+  gp_ski_state* s = p->ski;
+  const SkiGeom g = ski_geom<D>(s);
+  float* cur = nullptr;
+  GP_CHECK(ski_grid_apply_d<D>(p, V16, &cur));
+  const SkiTiles tl = ski_tiles_of(s, D);
+  const int parts = ski_tile_parts(p);
+  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
+  ski_gather_tiled_kernel<D><<<tgrid, 256, ski_tile_smem(s, D), p->stream>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(),
+                                                                            s->tile_off.as<int>(), g, tl, parts, cur, OUT16);
+  p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
@@ -763,10 +786,10 @@ int ski_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   (void)done_flag;   // the products of a finished mBCG are cheap no-ops for the dense kernels; here they simply run
   GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
   switch (p->d) {
-    case 1: return ski_matmul_d<1>(p, V16, TP, p->partial.as<float>());
-    case 2: return ski_matmul_d<2>(p, V16, TP, p->partial.as<float>());
-    case 3: return ski_matmul_d<3>(p, V16, TP, p->partial.as<float>());
-    case 4: return ski_matmul_d<4>(p, V16, TP, p->partial.as<float>());
+    case 1: return ski_matmul_d<1>(p, V16, p->partial.as<float>());
+    case 2: return ski_matmul_d<2>(p, V16, p->partial.as<float>());
+    case 3: return ski_matmul_d<3>(p, V16, p->partial.as<float>());
+    case 4: return ski_matmul_d<4>(p, V16, p->partial.as<float>());
   }
   set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
   return GP_E_SHAPE;
@@ -864,6 +887,156 @@ int ski_diag_sum(gp_plan* p, double* out) {
   return GP_OK;
 }
 
+// ---- prediction on the grid (gp_ski_grid_matmul / gp_ski_interp_matmul) ----------------------------------------------------------
+// The reference's InterpolatedPredictionStrategy (models/exact_prediction_strategies.py:481-827) keeps its mean and LOVE caches on
+// the grid, c = s K_uu W^T alpha and C = s K_uu W^T R, and predicts with one interpolation W* c / W* C per call: O(4^d t) per test
+// point, independent of the training-set size.
+
+// OUT[r][c] = s U[r][c] for c < tc: the [M][16] grid block of one column chunk into the caller's [M][ldo] matrix
+__global__ void ski_grid_export_kernel(const float* __restrict__ U, int64_t M, int tc, float s, float* __restrict__ out, int64_t ldo) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= M * tc) return;
+  const int64_t r = e / tc;
+  const int c = (int)(e - r * tc);
+  out[r * ldo + c] = s * U[r * TP + c];
+}
+
+// sum_q w_q C[node_q] for one point and column in the fixed separable order  sum_a w_0[a] (sum_b w_1[b] (... C[...])):
+// b points at the point's first node, pitch[k] is the distance of neighbouring nodes of dimension k (in floats)
+template <int D, int K>
+struct SkiInterpSum {
+  static __device__ __forceinline__ float run(const float* b, const float4 (&w)[D], const int (&pitch)[D]) {
+    float s = w[K].x * SkiInterpSum<D, K + 1>::run(b, w, pitch);
+    s = fmaf(w[K].y, SkiInterpSum<D, K + 1>::run(b + pitch[K], w, pitch), s);
+    s = fmaf(w[K].z, SkiInterpSum<D, K + 1>::run(b + 2 * pitch[K], w, pitch), s);
+    s = fmaf(w[K].w, SkiInterpSum<D, K + 1>::run(b + 3 * pitch[K], w, pitch), s);
+    return s;
+  }
+};
+template <int D>
+struct SkiInterpSum<D, D> {
+  static __device__ __forceinline__ float run(const float* b, const float4 (&)[D], const int (&)[D]) { return *b; }
+};
+
+// OUT[perm[p]][c] = sum_q w_q C[node_q][c] for the tc <= 32 columns of one chunk (C and OUT offset to the chunk by the caller).
+// One CTA per (tile, part), as the gather: the tile's (E + 3)^D node block of the chunk is staged in shared memory as [node][LP],
+// LP = tc rounded up to a power of two (44 KB at d = 3, LP = 32), then every lane owns one (point, column) pair: LP lanes per point
+// read consecutive columns of a node, 32 / LP points per warp -- so a single column (the mean) keeps all 32 lanes busy on 32
+// points.  The point's 4 D weights sit in registers; no atomics and no cross-lane sums, so repeated calls are bit-identical
+// whatever ldc / ldo.  Staged with float4 loads when the chunk is full and 16-byte aligned (vec).
+constexpr int SKI_IP_THREADS = 256;
+constexpr int SKI_IP_CW = 32;   // columns per chunk
+template <int D>
+__global__ void __launch_bounds__(SKI_IP_THREADS)
+ski_interp_tiled_kernel(const int* __restrict__ first_s, const float* __restrict__ wts_s, const int* __restrict__ perm,
+                        const int* __restrict__ off, SkiGeom g, SkiTiles tl, int parts, const float* __restrict__ C, int64_t ldc,
+                        int tc, int lp_log2, int vec, float* __restrict__ out, int64_t ldo) {
+  extern __shared__ __align__(16) float blk[];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int col = lane & ((1 << lp_log2) - 1);
+  const int slot = (tid >> lp_log2);                    // this lane's point slot in the CTA
+  const int nslot = SKI_IP_THREADS >> lp_log2;
+  const int gshift = vec ? lp_log2 - 2 : lp_log2;        // log2 of the staged column groups per node (float4 or float)
+  for (int64_t wk = blockIdx.x; wk < (int64_t)tl.ntiles * parts; wk += gridDim.x) {
+    const int tile = (int)(wk / parts), part = (int)(wk % parts);
+    const int t0 = off[tile], tn = off[tile + 1] - t0;
+    const int p0 = t0 + (int)((int64_t)tn * part / parts), p1 = t0 + (int)((int64_t)tn * (part + 1) / parts);
+    if (p0 == p1) continue;
+    const SkiBlock<D> b = ski_block_of<D>(tile, g, tl);
+    __syncthreads();
+    // staging, row by row as ski_block_rows: a row fixes dimensions 0 .. D-2, the lanes cover (last-dimension node, column group)
+    const int last = b.ext[D - 1];
+    const int nrows = b.nodes / last;
+    for (int row = warp; row < nrows; row += SKI_IP_THREADS / 32) {
+      int rem = row, node0 = 0;
+      int64_t idx0 = (int64_t)b.base[D - 1] * g.stride[D - 1];
+#pragma unroll
+      for (int i = D - 2; i >= 0; --i) {
+        const int c = rem % b.ext[i];
+        rem /= b.ext[i];
+        node0 += c * b.pitch[i];
+        idx0 += (int64_t)(b.base[i] + c) * g.stride[i];
+      }
+      for (int e = lane; e < (last << gshift); e += 32) {
+        const int c = e >> gshift, q = e & ((1 << gshift) - 1);
+        const float* src = C + (idx0 + (int64_t)c * g.stride[D - 1]) * ldc;
+        float* dst = blk + ((size_t)(node0 + c) << lp_log2);
+        if (vec) reinterpret_cast<float4*>(dst)[q] = __ldg(reinterpret_cast<const float4*>(src) + q);
+        else dst[q] = (q < tc) ? __ldg(src + q) : 0.f;
+      }
+    }
+    __syncthreads();
+    if (col < tc) {
+      int pitch[D];
+#pragma unroll
+      for (int i = 0; i < D; ++i) pitch[i] = b.pitch[i] << lp_log2;
+      for (int p = p0 + slot; p < p1; p += nslot) {
+        float4 w[D];
+        int node = 0;
+#pragma unroll
+        for (int i = 0; i < D; ++i) {
+          node += (first_s[(int64_t)p * D + i] - b.base[i]) * b.pitch[i];
+          w[i] = reinterpret_cast<const float4*>(wts_s)[(int64_t)p * D + i];
+        }
+        const float v = SkiInterpSum<D, 0>::run(blk + ((size_t)node << lp_log2) + col, w, pitch);
+        out[(int64_t)perm[p] * ldo + col] = v;
+      }
+    }
+  }
+}
+
+template <int D>
+static int ski_grid_matmul_d(gp_plan* p, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo) {
+  const int64_t M = ski_geom<D>(p->ski).M;
+  GP_CHECK(p->V16.ensure(sizeof(float) * p->n1 * TP));
+  for (int c0 = 0; c0 < t; c0 += TP) {
+    const int tc = std::min(TP, t - c0);
+    GP_CHECK(to_v16(p, V + c0, ldv, tc, p->n1, p->V16.as<float>()));
+    float* cur = nullptr;
+    GP_CHECK(ski_grid_apply_d<D>(p, p->V16.as<float>(), &cur));
+    ski_grid_export_kernel<<<(unsigned)cdiv(M * tc, 256), 256, 0, p->stream>>>(cur, M, tc, p->outputscale, OUT + c0, ldo);
+    p->launches++;
+  }
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
+template <int D>
+static int ski_interp_matmul_d(gp_plan* p, const float* C, int64_t ldc, int t, float* OUT, int64_t ldo) {
+  const gp_ski_state* s = p->ski;
+  const SkiGeom g = ski_geom<D>(s);
+  const SkiTiles tl = ski_tiles_of(s, D);
+  GP_CHECK(opt_in_smem<ski_interp_tiled_kernel<D>>(p->device, SKI_TILE_SMEM));
+  const int parts = ski_tile_parts(p);
+  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
+  const size_t nodes = ski_tile_smem(s, D) / (TP * sizeof(float));
+  for (int c0 = 0; c0 < t; c0 += SKI_IP_CW) {
+    const int tc = std::min(SKI_IP_CW, t - c0);
+    int lg = 0;
+    while ((1 << lg) < tc) ++lg;
+    const int vec = tc == (1 << lg) && tc >= 4 && ldc % 4 == 0 && (reinterpret_cast<uintptr_t>(C + c0) & 15) == 0;
+    ski_interp_tiled_kernel<D><<<tgrid, SKI_IP_THREADS, nodes * (sizeof(float) << lg), p->stream>>>(
+        s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, C + c0, ldc, tc, lg, vec,
+        OUT + c0, ldo);
+    p->launches++;
+  }
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
+// the arguments both calls share: a packed, unsharded SKI plan; t >= 1 columns, leading dimensions >= t
+static int ski_predict_check(gp_plan* p, int t, int64_t ld_in, int64_t ld_out, const char* what) {
+  GP_REQUIRE(p != nullptr && p->data_set && p->hypers_set, GP_E_STATE, "%s: plan not ready (set_data + set_ski + set_hypers)", what);
+  GP_REQUIRE(p->backend == GP_BACKEND_SKI && p->ski != nullptr, GP_E_STATE, "%s needs a SKI plan (gp_plan_set_ski)", what);
+  GP_REQUIRE(!(p->comm && p->comm->world > 1) && p->row_begin == 0 && p->row_count == p->n1, GP_E_SHAPE,
+             "%s is not available on row-sharded plans", what);
+  GP_REQUIRE(t >= 1 && ld_in >= t && ld_out >= t, GP_E_SHAPE, "%s: bad shape t=%d, leading dimensions %lld / %lld", what, t,
+             (long long)ld_in, (long long)ld_out);
+  GP_REQUIRE(p->ski->T.p != nullptr && p->ski->perm.p != nullptr, GP_E_STATE, "%s: SKI grid not packed", what);
+  GP_CUDA(cudaSetDevice(p->device));
+  return GP_OK;
+}
+
 }  // namespace gp
 
 using namespace gp;
@@ -881,4 +1054,29 @@ extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* g
   p->backend = GP_BACKEND_SKI;
   if (p->hypers_set) return pack_inputs(p);
   return GP_OK;
+}
+
+extern "C" int gp_ski_grid_matmul(gp_plan* p, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo) {
+  GP_CHECK(ski_predict_check(p, t, ldv, ldo, "gp_ski_grid_matmul"));
+  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
+  switch (p->d) {
+    case 1: return ski_grid_matmul_d<1>(p, V, ldv, t, OUT, ldo);
+    case 2: return ski_grid_matmul_d<2>(p, V, ldv, t, OUT, ldo);
+    case 3: return ski_grid_matmul_d<3>(p, V, ldv, t, OUT, ldo);
+    case 4: return ski_grid_matmul_d<4>(p, V, ldv, t, OUT, ldo);
+  }
+  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
+  return GP_E_SHAPE;
+}
+
+extern "C" int gp_ski_interp_matmul(gp_plan* p, const float* C, int64_t ldc, int t, float* OUT, int64_t ldo) {
+  GP_CHECK(ski_predict_check(p, t, ldc, ldo, "gp_ski_interp_matmul"));
+  switch (p->d) {
+    case 1: return ski_interp_matmul_d<1>(p, C, ldc, t, OUT, ldo);
+    case 2: return ski_interp_matmul_d<2>(p, C, ldc, t, OUT, ldo);
+    case 3: return ski_interp_matmul_d<3>(p, C, ldc, t, OUT, ldo);
+    case 4: return ski_interp_matmul_d<4>(p, C, ldc, t, OUT, ldo);
+  }
+  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
+  return GP_E_SHAPE;
 }

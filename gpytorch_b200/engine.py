@@ -111,7 +111,43 @@ class Plan:
         st = (C.c_float * d)(*[float(v) for v in grid_step])
         with torch.cuda.device(self.device):
             check(self.lib.gp_plan_set_ski(self._h, gs, lo, st, d))
+        self.grid_points = 1
+        for v in grid_sizes:
+            self.grid_points *= int(v)
         return self
+
+    def _ski_block(self, a: torch.Tensor, grid_rows: bool, name: str):
+        """a as a 2-D block with unit column stride, checked against the plan: [M, t] (grid_rows) or [n, t]."""
+        _require_cuda_f32(a, name)
+        if a.device != self.device:
+            raise RuntimeError(f"{name} lives on {a.device}, the plan on {self.device}")
+        if getattr(self, "grid_points", None) is None:
+            raise RuntimeError("the plan has no SKI grid (set_ski)")
+        rows = self.grid_points if grid_rows else self.n1
+        vec = a.dim() == 1
+        a2 = a.unsqueeze(-1) if vec else a
+        if a2.dim() != 2 or a2.size(0) != rows:
+            raise RuntimeError(f"{name} must be [{rows}] or [{rows}, t] (got {tuple(a.shape)})")
+        if a2.stride(-1) != 1:
+            a2 = a2.contiguous()
+        return a2, vec
+
+    def ski_grid_matmul(self, v: torch.Tensor) -> torch.Tensor:
+        """s K_uu W^T v on the SKI grid: v [n] or [n, t] over the plan's points -> [M] or [M, t], M = prod(grid_sizes), rows in
+        the reference's flat grid order (dimension 0 slowest)."""
+        v2, vec = self._ski_block(v, False, "rhs")
+        out = torch.empty(self.grid_points, v2.size(1), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_ski_grid_matmul(self._h, _ptr(v2), v2.stride(0), v2.size(1), _ptr(out), out.stride(0)))
+        return out.squeeze(-1) if vec else out
+
+    def ski_interp_matmul(self, c: torch.Tensor) -> torch.Tensor:
+        """W c: grid values c [M] or [M, t] interpolated to the plan's points -> [n] or [n, t] in the caller's row order."""
+        c2, vec = self._ski_block(c, True, "grid matrix")
+        out = torch.empty(self.n1, c2.size(1), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_ski_interp_matmul(self._h, _ptr(c2), c2.stride(0), c2.size(1), _ptr(out), out.stride(0)))
+        return out.squeeze(-1) if vec else out
 
     def set_sum(self, terms):
         """Kernel sum (AdditiveKernel): this plan's operator becomes sum_t K_t (+ its own noise).  `terms` are ready plans over

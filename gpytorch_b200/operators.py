@@ -521,7 +521,7 @@ class SKIKernelLinearOperator(KernelLinearOperator):
     def plan(self, noise=0.0) -> Plan:
         if self._plan is None:
             key = "ski:" + repr((self.grid_sizes, self.grid_lo, self.grid_step))
-            self._plan = _get_plan(self.x1, None, key, 0, 0, None)
+            self._plan = _get_plan(self.x1, None, key, 0, 0, None, getattr(self, "_plan_slot", 0))
             if getattr(self._plan, "_ski_key", None) != key:
                 self._plan.set_ski(self.grid_sizes, self.grid_lo, self.grid_step)
                 self._plan._ski_key = key
@@ -551,6 +551,26 @@ class SKIKernelLinearOperator(KernelLinearOperator):
         return self.plan().diag()
 
     _diagonal = diagonal
+
+    def same_grid(self, other) -> bool:
+        """other is a SKI operator on the same grid with the same kind and hyper-parameter values: its points interpolate the
+        same K_uu, so the grid caches of one operator serve the other (models._ski_grid_mode)."""
+        if type(other) is not type(self):
+            return False
+        if (self.grid_sizes, self.grid_lo, self.grid_step, self.kind) != (other.grid_sizes, other.grid_lo, other.grid_step, other.kind):
+            return False
+        return (self.lengthscale.shape == other.lengthscale.shape and bool(torch.equal(self.lengthscale.detach(), other.lengthscale.detach()))
+                and bool(torch.equal(self.outputscale.detach().reshape(-1), other.outputscale.detach().reshape(-1))))
+
+    def grid_matmul(self, rhs):
+        """s K_uu W^T rhs: rhs [n] or [n, t] over this operator's points -> [M] or [M, t] on the grid (gp_ski_grid_matmul; the
+        caches c = s K_uu W^T alpha and C = s K_uu W^T R of the reference's InterpolatedPredictionStrategy).  Detached."""
+        return self.plan().ski_grid_matmul(rhs.detach().float())
+
+    def interp_matmul(self, grid):
+        """W grid: grid values [M] or [M, t] interpolated to this operator's points (gp_ski_interp_matmul; the reference's
+        left_interp).  Detached."""
+        return self.plan().ski_interp_matmul(grid.detach().float())
 
     def __getitem__(self, index):
         """Rows / columns of the interpolated operator: K[r, c] = W[r] K_uu W[c]^T (the reference slices the interpolation
@@ -646,11 +666,25 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
         if not self.supports(base):
             raise RuntimeError("LowRankUpdatedKernelLinearOperator needs a square, unsharded, plan-backed kernel operator or "
                                "kernel sum (not SKI)")
+        self._setup(base, U)
+
+    def _setup(self, base, U):
         if U.dim() != 2 or U.size(0) != base.shape[0] or not 1 <= U.size(1) <= LOWRANK_MAX_RANK:
             raise RuntimeError(f"low-rank factor must be [{base.shape[0]}, r] with 1 <= r <= {LOWRANK_MAX_RANK} (got {tuple(U.shape)})")
         self.base = base.detach()
         self.base._plan_slot = _LOWRANK_SLOT
         self.U = U.detach().float().contiguous()
+
+    @classmethod
+    def on_ski(cls, base, U: torch.Tensor):
+        """K**_test - U U^T on a standalone SKI operator, i.e. one whose plan is over the test points only (the KISS-GP grid
+        prediction of models.ExactGP, settings.ski_grid_prediction).  The SKI plan takes the correction like any other backend.
+        Kept out of supports() / the default constructor: the joint path's SKI blocks are slices of a train + test operator."""
+        if type(base) is not SKIKernelLinearOperator:
+            raise RuntimeError("LowRankUpdatedKernelLinearOperator.on_ski needs a standalone SKIKernelLinearOperator")
+        op = cls.__new__(cls)
+        op._setup(base, U)
+        return op
 
     @staticmethod
     def supports(base) -> bool:

@@ -253,6 +253,19 @@ class ski_preconditioner(_feature_flag):
     _default = False
 
 
+class ski_grid_prediction(_feature_flag):
+    """Predict from a KISS-GP model (ScaleKernel(GridInterpolationKernel(...))) with caches kept on the grid, as the reference's
+    InterpolatedPredictionStrategy does (models/exact_prediction_strategies.py:481-827): the mean is mu* + W* c with
+    c = s K_uu W^T alpha, the LOVE covariance K**_test - U U^T with U = W* C, C = s K_uu W^T R.  The cost per test point is
+    O(4^d J) and does not depend on the training-set size; the test prior is forward(test_x) alone, never the joint train + test
+    operator (models._ski_grid_mode lists when it applies and what it falls back to).
+
+    Off by default because a feature may not change existing results: with the flag off, SKI predictions keep the joint path bit
+    for bit.  tools/ski_predict_bench.py measures both paths, so that a follow-up can make this path the default and delete the
+    SKI branch of the joint path."""
+    _default = False
+
+
 class probe_seed(_value_context):
     """Seed of the base samples for the SLQ probes (None = draw from torch's global CUDA generator)."""
     _global_value = None

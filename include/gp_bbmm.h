@@ -91,6 +91,18 @@ int gp_plan_set_noise_diag(gp_plan* plan, const float* diag, int64_t n);
  * gp_ciq_precond_build and gp_ciq_sqrt_matmul_precond accept it (a preconditioned SKI MLL combines these primitives).  Out-of-bounds inputs fail like the reference ("Received data that was out of bounds ..."). */
 int gp_plan_set_ski(gp_plan* plan, const int* grid_sizes, const float* grid_lo, const float* grid_step, int d);
 
+/* KISS-GP prediction on the grid (InterpolatedPredictionStrategy, models/exact_prediction_strategies.py:481-827: mean_cache,
+ * covar_cache, exact_predictive_mean / exact_predictive_covar).  Both take a packed SKI plan (gp_plan_set_ski + gp_plan_set_hypers)
+ * over n points; grid matrices are row-major [M][t] (M = prod G_i) in the reference's flat grid order, dimension 0 slowest
+ * (utils/interpolation.py:157-163).  t >= 1 is arbitrary, ld >= t.  GP_E_STATE on a non-SKI plan, GP_E_SHAPE for t < 1, ld < t
+ * or a row-sharded plan.
+ *  gp_ski_grid_matmul:   OUT[M, t] = s K_uu W^T V for V [n, t] over the plan's points (the grid caches c = s K_uu W^T alpha and
+ *                        C = s K_uu W^T R);
+ *  gp_ski_interp_matmul: OUT[n, t] = W C for C [M, t] (the reference's left_interp; W is never expanded, every call with the same
+ *                        C returns bit-identical results). */
+int gp_ski_grid_matmul(gp_plan* plan, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo);
+int gp_ski_interp_matmul(gp_plan* plan, const float* C, int64_t ldc, int t, float* OUT, int64_t ldo);
+
 /* Kernel sums (AdditiveKernel, kernels/kernel.py:592-621: k = k_1 + ... + k_m, each term with its own covariance function,
  * lengthscale(s), outputscale and active dimensions): `plan` becomes the operator  sum_t K_t  (+ its own noise), where every
  * K_t is a ready plan over the same rows (same n1 / n2 / row shard / stream; the data pointers may differ: active_dims).
