@@ -81,6 +81,8 @@ PROTOTYPES = {
     "gp_krows": (_I, [_P, _P, _L, _P, _L]),
     "gp_kdiag": (_I, [_P, _P]),
     "gp_bilinear_grad": (_I, [_P, _P, _L, _P, _L, _I, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "gp_kmv_input_grad": (_I, [_P, _P, _L, _P, _L, _I, _P, _L, _P, _L]),
+    "gp_kdense_input_grad": (_I, [_P, _P, _L, _P, _L, _P, _L]),
     "gp_pivoted_cholesky": (_I, [_P, _I, _F, _P, _P, C.POINTER(_I)]),
     "gp_precond_build": (_I, [_P, _P, _I, _P, C.POINTER(C.c_double)]),
     "gp_precond_probes": (_I, [_P, _P, _I, _P, _P, _I, _P]),

@@ -299,6 +299,22 @@ __device__ __forceinline__ float dcov_from_arg(float a, float* kout) {
     return (rho + 1.f) * m * 0.33333334f * e;
   }
 }
+// input-derivative factor q = dk/da of the same covariance (xgrad.cu): dk/dz_i = -q (z_i - z_j) in the packed units.
+//   RBF: ln2 2^a ; M12: e / (2 rho) ; M32: e / 2 ; M52: (1 + rho) e / 6      (e = exp(-rho), rho^2 = -a)
+// q is the h of the raw-unit form  dk/dx_i = -h (x_i - x_j) / l^2  times l^2 / C (C = log2 e, 2, 6, 10 as in pack.cu).  A pair at
+// distance 0 contributes 0 (its direction is 0; Matern-1/2's q is unbounded there): the caller masks a == 0.
+template <int KIND>
+__device__ __forceinline__ float hcov_from_arg(float a) {
+  if (KIND == GP_RBF) {
+    return 0.69314718f * ex2_approx(fminf(a, 0.f));
+  } else {
+    float rho = sqrt_approx(fmaxf(-a, 0.f));
+    float e = ex2_approx(-LOG2E * rho);
+    if (KIND == GP_MATERN12) return 0.5f * e / rho;
+    if (KIND == GP_MATERN32) return 0.5f * e;
+    return (rho + 1.f) * e * 0.16666667f;
+  }
+}
 #endif
 
 }  // namespace gp

@@ -14,6 +14,12 @@ def _ptr(t: torch.Tensor | None):
     return C.c_void_p(0) if t is None else C.c_void_p(t.data_ptr())
 
 
+def _ld(t: torch.Tensor) -> int:
+    """Leading dimension of a row-major block with unit column stride: a single row may carry any row stride (torch calls an
+    expanded [1, t] tensor contiguous), so it gets t."""
+    return t.stride(0) if t.size(0) > 1 else t.size(1)
+
+
 def _require_cuda_f32(t: torch.Tensor, name: str):
     if not t.is_cuda:
         raise RuntimeError(f"{name} must live on a CUDA device: gpytorch_b200 has no CPU path")
@@ -213,7 +219,7 @@ class Plan:
         if v2.size(0) != self.n2:
             raise RuntimeError(f"Size mismatch: operator has {self.n2} columns, rhs has {v2.size(0)} rows")
         out = torch.empty(self.row_count, v2.size(1), device=self.device, dtype=torch.float32)
-        check(self.lib.gp_kmv(self._h, _ptr(v2), v2.stride(0), v2.size(1), _ptr(out), out.stride(0), int(add_noise)))
+        check(self.lib.gp_kmv(self._h, _ptr(v2), _ld(v2), v2.size(1), _ptr(out), out.stride(0), int(add_noise)))
         return out.squeeze(-1) if vec else out
 
     def rows(self, idx: torch.Tensor) -> torch.Tensor:
@@ -236,6 +242,41 @@ class Plan:
         go = C.c_double()
         check(self.lib.gp_bilinear_grad(self._h, _ptr(left), left.stride(0), _ptr(right), right.stride(0), s, gl, C.byref(go)))
         return [gl[i] for i in range(nls)], go.value
+
+    def _grad_outputs(self, dx1: bool, dx2: bool):
+        """The output blocks of an input gradient: on a square plan DX1 receives the total and DX2 is None."""
+        o1 = torch.empty(self.n1, self.d, device=self.device, dtype=torch.float32) if dx1 else None
+        o2 = torch.empty(self.n2, self.d, device=self.device, dtype=torch.float32) if (dx2 and not self.same) else None
+        return o1, o2
+
+    def kmv_input_grad(self, g: torch.Tensor, v: torch.Tensor, dx1: bool = True, dx2: bool = True):
+        """(dF/dx1 [n1, d], dF/dx2 [n2, d]) of F = sum(g * (K @ v)) in raw input units (outputscale folded in, noise excluded);
+        g [n1] or [n1, t], v [n2] or [n2, t].  On a square plan the first entry is the total gradient and the second is None;
+        an entry not asked for is None."""
+        _require_cuda_f32(g, "g")
+        _require_cuda_f32(v, "v")
+        g2 = g.unsqueeze(-1) if g.dim() == 1 else g
+        v2 = v.unsqueeze(-1) if v.dim() == 1 else v
+        if g2.dim() != 2 or v2.dim() != 2 or g2.shape != (self.row_count, v2.size(1)) or v2.size(0) != self.n2:
+            raise RuntimeError(f"kmv_input_grad: g must be [{self.row_count}, t] and v [{self.n2}, t] (got {tuple(g.shape)}, {tuple(v.shape)})")
+        g2 = g2 if g2.stride(-1) == 1 else g2.contiguous()
+        v2 = v2 if v2.stride(-1) == 1 else v2.contiguous()
+        o1, o2 = self._grad_outputs(dx1, dx2)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_kmv_input_grad(self._h, _ptr(g2), _ld(g2), _ptr(v2), _ld(v2), v2.size(1),
+                                             _ptr(o1), self.d, _ptr(o2), self.d))
+        return o1, o2
+
+    def dense_input_grad(self, w: torch.Tensor, dx1: bool = True, dx2: bool = True):
+        """(dF/dx1, dF/dx2) of F = sum(w * K) for w [n1, n2]: the input gradient of the block rows() returns (see kmv_input_grad)."""
+        _require_cuda_f32(w, "w")
+        if w.dim() != 2 or tuple(w.shape) != (self.row_count, self.n2):
+            raise RuntimeError(f"dense_input_grad: w must be [{self.row_count}, {self.n2}] (got {tuple(w.shape)})")
+        w = w if w.stride(-1) == 1 else w.contiguous()
+        o1, o2 = self._grad_outputs(dx1, dx2)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_kdense_input_grad(self._h, _ptr(w), _ld(w), _ptr(o1), self.d, _ptr(o2), self.d))
+        return o1, o2
 
     # ---- solver seam -------------------------------------------------------------------------
     def pivoted_cholesky(self, rank: int, error_tol: float = 1e-3):

@@ -308,9 +308,28 @@ class KernelLinearOperator(_SamplingMixin):
         gradients (the autograd functions below take them as explicit inputs)."""
         return [self.lengthscale, self.outputscale]
 
+    def input_tensors(self):
+        """The inputs K is differentiated in by the product and dense-block autograd functions below, which take them after
+        the hyper-parameters: [x1] for a square operator (both arguments are the same points), [x1, x2] for a cross-covariance."""
+        return [self.x1] if self.same else [self.x1, self.x2]
+
     def _bilinear_derivative_list(self, left, right):
         gl, go = self._bilinear_derivative(left, right)
         return [gl.reshape(self.lengthscale.shape), go.reshape(self.outputscale.shape)]
+
+    def _input_grad_list(self, left, right, needs):
+        """Gradients of sum(left * (K @ right)) w.r.t. input_tensors(), None where `needs` is False (gp_kmv_input_grad)."""
+        if not any(needs):
+            return [None] * len(needs)
+        d1, d2 = self.plan(getattr(self, "_last_noise", 0.0)).kmv_input_grad(left, right, needs[0], len(needs) > 1 and needs[1])
+        return [d1, d2][: len(needs)]
+
+    def _dense_input_grad_list(self, w, needs):
+        """Gradients of sum(w * K) w.r.t. input_tensors(), None where `needs` is False (gp_kdense_input_grad)."""
+        if not any(needs):
+            return [None] * len(needs)
+        d1, d2 = self.plan().dense_input_grad(w, needs[0], len(needs) > 1 and needs[1])
+        return [d1, d2][: len(needs)]
 
     # -- LinearOperator protocol: shape helpers / transpose (lazy_evaluated_kernel_tensor.py:277-341) --
     def _size(self):
@@ -345,19 +364,18 @@ class KernelLinearOperator(_SamplingMixin):
         return self._transpose_nonbatch()
 
     def detach(self):
-        return KernelLinearOperator(self.x1, self.x2, self.kind, self.lengthscale.detach(), self.outputscale.detach())
+        return KernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.kind, self.lengthscale.detach(),
+                                    self.outputscale.detach())
 
     # -- products --
     def matmul(self, rhs):
-        return _KernelMatmul.apply(self, rhs, *self.hyper_tensors())
+        return _KernelMatmul.apply(self, rhs, *self.hyper_tensors(), *self.input_tensors())
 
     __matmul__ = matmul
     _matmul = matmul
 
     def to_dense(self):
-        p = self.plan()
-        idx = torch.arange(p.row_count, device=self.device)   # local rows of a row-sharded plan
-        return p.rows(idx)
+        return _KernelDense.apply(self, *self.input_tensors())
 
     def diagonal(self, dim1=-2, dim2=-1):
         """kernel(x1, x2, diag=True) (lazy_evaluated_kernel_tensor.py:107-133): the constant outputscale for x2 == x1,
@@ -440,6 +458,18 @@ class SumKernelLinearOperator(KernelLinearOperator):
 
     def hyper_tensors(self):
         return [t for o in self.ops for t in o.hyper_tensors()]
+
+    def input_tensors(self):
+        return [t for o in self.ops for t in o.input_tensors()]
+
+    def _input_grad_list(self, left, right, needs):
+        """One gp_kmv_input_grad call per term (the engine refuses a kernel-sum plan)."""
+        out, k = [], 0
+        for o in self.ops:
+            m = len(o.input_tensors())
+            out.extend(o._input_grad_list(left, right, needs[k:k + m]))
+            k += m
+        return out
 
     def _bilinear_derivative_list(self, left, right):
         out = []
@@ -536,6 +566,10 @@ class SKIKernelLinearOperator(KernelLinearOperator):
             self._plan.set_hypers(self.kind, ls, os_, nz)
             self._plan._hyp_key = hk
         return self._plan
+
+    def input_tensors(self):
+        """No inputs: SKI input gradients are not implemented, so the interpolated operator stays detached from its inputs."""
+        return []
 
     def detach(self):
         return SKIKernelLinearOperator(self.x1, self.kind, self.lengthscale.detach(), self.outputscale.detach(), self.grid_sizes,
@@ -827,9 +861,14 @@ class _LowRankMatmul(torch.autograd.Function):
 
 
 class _KernelMatmul(torch.autograd.Function):
+    """K @ rhs.  Takes the operator's hyper_tensors() and then its input_tensors(): the backward returns the hyper-parameter
+    gradients (gp_bilinear_grad) and the input gradients (gp_kmv_input_grad, one call per term of a kernel sum) only for the
+    tensors whose gradient autograd asks for."""
+
     @staticmethod
-    def forward(ctx, op, rhs, *hypers):
+    def forward(ctx, op, rhs, *tensors):
         ctx.op = op
+        ctx.nh = len(op.hyper_tensors())
         out = op.plan(getattr(op, "_last_noise", 0.0)).kmv(rhs.detach())
         ctx.save_for_backward(rhs.detach())
         return out
@@ -843,18 +882,35 @@ class _KernelMatmul(torch.autograd.Function):
         g2 = g.unsqueeze(-1) if vec else g
         r2 = rhs.unsqueeze(-1) if vec else rhs
         grad_rhs = None
-        nh = len(ctx.needs_input_grad) - 2
+        nh = ctx.nh
         grads = [None] * nh
+        need_h, need_x = ctx.needs_input_grad[2:2 + nh], ctx.needs_input_grad[2 + nh:]
         if ctx.needs_input_grad[1]:
             # K^T g: for x1 == x2 the operator is symmetric
             if not op.same:
                 grad_rhs = op._transpose_nonbatch().plan().kmv(g)
             else:
                 grad_rhs = op.plan(getattr(op, "_last_noise", 0.0)).kmv(g)
-        if any(ctx.needs_input_grad[2:]):
+        if any(need_h):
             gs = op._bilinear_derivative_list(g2, r2)
-            grads = [gi if need else None for gi, need in zip(gs, ctx.needs_input_grad[2:])]
-        return (None, grad_rhs, *grads)
+            grads = [gi if need else None for gi, need in zip(gs, need_h)]
+        return (None, grad_rhs, *grads, *op._input_grad_list(g2, r2, need_x))
+
+
+class _KernelDense(torch.autograd.Function):
+    """K(x1, x2) as a dense block (gp_krows; the local rows of a row-sharded plan) whose backward reaches the input tensors
+    (gp_kdense_input_grad).  Hyper-parameter gradients through to_dense() are not implemented: the block is detached from the
+    lengthscale and outputscale, as it always was."""
+
+    @staticmethod
+    def forward(ctx, op, *inputs):
+        ctx.op = op
+        p = op.plan()
+        return p.rows(torch.arange(p.row_count, device=op.device))
+
+    @staticmethod
+    def backward(ctx, grad):
+        return (None, *ctx.op._dense_input_grad_list(grad.contiguous(), ctx.needs_input_grad[1:]))
 
 
 class AddedDiagLinearOperator(_SamplingMixin):

@@ -148,6 +148,18 @@ int gp_kdiag(gp_plan* plan, float* OUT);
 int gp_bilinear_grad(gp_plan* plan, const float* Lf, int64_t ldl, const float* Rt, int64_t ldr,
                      int s, double* grad_ls, double* grad_os);
 
+/* Input gradients (the autograd of RBFKernel.forward / MaternKernel.forward's slow branch, kernels/rbf_kernel.py:68-85,
+ * kernels/matern_kernel.py:86-107, w.r.t. x1 / x2): DX1 = dF/dX1 [n1][d] (ld1), DX2 = dF/dX2 [n2][d] (ld2), in raw input units
+ * with the outputscale folded in and the noise excluded, for F = sum_ic G_ic (K V)_ic; G [n1, t] ldg, V [n2, t] ldv, any t >= 1.
+ * Either output may be NULL; on a square plan (X2 == X1) DX1 gets the total gradient and DX2 must be NULL.  A pair at distance 0
+ * contributes 0; a non-finite input gives NaN outputs.  Repeated calls give identical bits (no atomics).
+ * GP_E_SHAPE on SKI, kernel-sum (call on every term) and row-sharded plans, for bad shapes, t < 1 or d > 64; GP_E_STATE on a
+ * plan with a low-rank correction. */
+int gp_kmv_input_grad(gp_plan* plan, const float* G, int64_t ldg, const float* V, int64_t ldv, int t,
+                      float* DX1, int64_t ld1, float* DX2, int64_t ld2);
+/* the same for F = sum_ij W_ij K_ij, W [n1][n2] (ldw >= n2): the input gradient of the dense block gp_krows returns */
+int gp_kdense_input_grad(gp_plan* plan, const float* W, int64_t ldw, float* DX1, int64_t ld1, float* DX2, int64_t ld2);
+
 /* ---- solver seam (linear_operator) --------------------------------------------------- */
 
 /* Greedy pivoted partial Cholesky of K(X1,X1) (outputscale included, no noise):
