@@ -77,6 +77,7 @@ PROTOTYPES = {
     "gp_plan_set_lowrank": (_I, [_P, _P, _L, _I]),
     "gp_ski_grid_matmul": (_I, [_P, _P, _L, _I, _P, _L]),
     "gp_ski_interp_matmul": (_I, [_P, _P, _L, _I, _P, _L]),
+    "gp_ski_input_grad": (_I, [_P, _P, _L, _P, _L, _I, _P, _L]),
     "gp_kmv": (_I, [_P, _P, _L, _I, _P, _L, _I]),
     "gp_krows": (_I, [_P, _P, _L, _P, _L]),
     "gp_kdiag": (_I, [_P, _P]),

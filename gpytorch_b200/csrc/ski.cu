@@ -49,6 +49,52 @@ __device__ __forceinline__ float cubic_w(float s) {
   return (u < 1.f) ? nearv : farv;     // u in [0, 2]: 1 - clamp(floor(u), 0, 1) selects the branch
 }
 
+// its derivative dw/ds = sign(s) (4.5 u^2 - 5 u) for u = |s| < 1, sign(s) (-1.5 u^2 + 5 u - 4) for 1 <= u < 2 (what autograd gives
+// through the reference's expression; 0 at s = 0)
+__device__ __forceinline__ float cubic_dw(float s) {
+  const float u = fabsf(s);
+  const float nearv = (4.5f * u - 5.f) * u;
+  const float farv = (-1.5f * u + 5.f) * u - 4.f;
+  const float v = (u < 1.f) ? nearv : farv;
+  return (s < 0.f) ? -v : v;
+}
+
+// Interpolation data of coordinate x on one grid axis (first node lo, spacing step, G nodes): returns the first of the 4 nodes
+// and their weights w; with DERIV also dw = dw/dx (1 / step per unit of distance; exactly 0 in the one-hot first / last cells,
+// as the reference's autograd gives).  ski_interp_kernel and ski_input_grad_tiled_kernel both call this, so they pick the same cell.
+template <bool DERIV>
+__device__ __forceinline__ int ski_axis_weights(float x, float lo, float step, int G, float (&w)[4], float (&dw)[4]) {
+  const float h = fmaxf(step, 1e-10f);
+  const float t = (x - lo) / h;
+  const float cell = floorf(t);
+  const float frac = t - cell;
+  int f = (int)cell - 1;                       // left-most of the 4 nodes
+#pragma unroll
+  for (int j = 0; j < 4; ++j) w[j] = cubic_w(frac + (float)(1 - j));   // distances f+1, f, f-1, f-2
+  if (DERIV) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) dw[j] = cubic_dw(frac + (float)(1 - j)) / h;
+  }
+  if (f < 0 || f > G - 4) {
+    // first / last cell: the nearest of the first / last 4 nodes gets weight 1 (interpolation.py:84-131)
+    const int base = (f < 0) ? 0 : G - 4;
+    int best = 0;
+    float bd = 3.4e38f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float dj = fabsf(lo + step * (float)(base + j) - x);
+      if (dj < bd) { bd = dj; best = j; }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      w[j] = (j == best) ? 1.f : 0.f;
+      if (DERIV) dw[j] = 0.f;
+    }
+    f = base;
+  }
+  return f;
+}
+
 // per row and dimension: first node index and the 4 weights
 __global__ void ski_interp_kernel(const float* __restrict__ X, int64_t n, int64_t ldx, SkiGeom g, int* __restrict__ first,
                                   float* __restrict__ wts, int* __restrict__ oob) {
@@ -58,27 +104,8 @@ __global__ void ski_interp_kernel(const float* __restrict__ X, int64_t n, int64_
     const float x = X[r * ldx + i];
     const float hi = g.lo[i] + g.step[i] * (float)(g.G[i] - 1);
     if (!(x - g.lo[i] >= -1e-7f) || !(x - hi <= 1e-7f)) *oob = 1;   // "Received data that was out of bounds for the specified grid."
-    const float t = (x - g.lo[i]) / fmaxf(g.step[i], 1e-10f);
-    const float cell = floorf(t);
-    const float frac = t - cell;
-    int f = (int)cell - 1;                       // left-most of the 4 nodes
-    float w[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) w[j] = cubic_w(frac + (float)(1 - j));   // distances f+1, f, f-1, f-2
-    if (f < 0 || f > g.G[i] - 4) {
-      // first / last cell: the nearest of the first / last 4 nodes gets weight 1 (interpolation.py:84-131)
-      const int base = (f < 0) ? 0 : g.G[i] - 4;
-      int best = 0;
-      float bd = 3.4e38f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float dj = fabsf(g.lo[i] + g.step[i] * (float)(base + j) - x);
-        if (dj < bd) { bd = dj; best = j; }
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) w[j] = (j == best) ? 1.f : 0.f;
-      f = base;
-    }
+    float w[4], unused[4];
+    const int f = ski_axis_weights<false>(x, g.lo[i], g.step[i], g.G[i], w, unused);
     first[r * g.d + i] = f;
 #pragma unroll
     for (int j = 0; j < 4; ++j) wts[(r * g.d + i) * 4 + j] = w[j];
@@ -1024,6 +1051,140 @@ static int ski_interp_matmul_d(gp_plan* p, const float* C, int64_t ldc, int t, f
   return GP_OK;
 }
 
+// ---- input gradient (gp_ski_input_grad: deep kernel learning through a KISS-GP operator) -------------------------------------------
+// F = sum_i L_i . (K_ski R)_i with K_ski = s W K_uu W^T.  Row i of W depends on x_i alone, so
+//   dF/dx_ik = sum_c [ L_ic (d_k W_i . B_R)_c + R_ic (d_k W_i . B_L)_c ],   B_R = s K_uu W^T R,  B_L = s K_uu W^T L   ([M][t] grid blocks)
+// where d_k W_i is row i's 4^D tensor-product weights with the dimension-k factor replaced by dw_k (ski_axis_weights<true>).
+// One CTA per (tile, part), as ski_interp_tiled_kernel: the tile's node block of one column chunk [B_R | B_L] (2 tc <= 32 columns,
+// padded to LP = a power of two) is staged in shared memory; a lane owns one (point, column) pair, forms the D derivative-weighted
+// sums in the fixed separable order and multiplies each by its paired coefficient (L_ic for a B_R column, R_ic for a B_L column).
+// The LP lanes of a point reduce with a fixed xor-shuffle tree; chunk c0 > 0 adds to what the previous chunk wrote (same stream,
+// fixed order).  The pass has no atomics; B_R / B_L come from the product's scatter, whose per-tile red.add order varies, so
+// repeated calls agree to the rounding of those sums.  The plan keeps no cell fractions, so the weights and
+// their derivatives are recomputed from the plan's inputs X by the helper that packed them.
+template <int D>
+__global__ void __launch_bounds__(SKI_IP_THREADS)
+ski_input_grad_tiled_kernel(const int* __restrict__ first_s, const int* __restrict__ perm, const int* __restrict__ off, SkiGeom g,
+                            SkiTiles tl, int parts, const float* __restrict__ X, int64_t ldx, const float* __restrict__ BR,
+                            const float* __restrict__ BL, int tc, int lp_log2, const float* __restrict__ L, int64_t ldl,
+                            const float* __restrict__ R, int64_t ldr, int accumulate, float* __restrict__ DX, int64_t lddx) {
+  extern __shared__ __align__(16) float blk[];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int lp = 1 << lp_log2;
+  const int col = lane & (lp - 1);
+  const int ppw = 32 >> lp_log2;                          // points per warp and step
+  const int pstep = (SKI_IP_THREADS / 32) * ppw;
+  for (int64_t wk = blockIdx.x; wk < (int64_t)tl.ntiles * parts; wk += gridDim.x) {
+    const int tile = (int)(wk / parts), part = (int)(wk % parts);
+    const int t0 = off[tile], tn = off[tile + 1] - t0;
+    const int p0 = t0 + (int)((int64_t)tn * part / parts), p1 = t0 + (int)((int64_t)tn * (part + 1) / parts);
+    if (p0 == p1) continue;
+    const SkiBlock<D> b = ski_block_of<D>(tile, g, tl);
+    __syncthreads();
+    const int last = b.ext[D - 1];
+    const int nrows = b.nodes / last;
+    for (int row = warp; row < nrows; row += SKI_IP_THREADS / 32) {
+      int rem = row, node0 = 0;
+      int64_t idx0 = (int64_t)b.base[D - 1] * g.stride[D - 1];
+#pragma unroll
+      for (int i = D - 2; i >= 0; --i) {
+        const int c = rem % b.ext[i];
+        rem /= b.ext[i];
+        node0 += c * b.pitch[i];
+        idx0 += (int64_t)(b.base[i] + c) * g.stride[i];
+      }
+      for (int e = lane; e < (last << lp_log2); e += 32) {
+        const int c = e >> lp_log2, q = e & (lp - 1);
+        const int64_t gi = (idx0 + (int64_t)c * g.stride[D - 1]) * TP;
+        blk[((size_t)(node0 + c) << lp_log2) + q] = (q < tc) ? __ldg(BR + gi + q) : (q < 2 * tc ? __ldg(BL + gi + q - tc) : 0.f);
+      }
+    }
+    __syncthreads();
+    int pitch[D];
+#pragma unroll
+    for (int i = 0; i < D; ++i) pitch[i] = b.pitch[i] << lp_log2;
+    // warp-uniform trip count: the reduction shuffles need every lane
+    for (int pb = p0 + warp * ppw; pb < p1; pb += pstep) {
+      const int p = pb + (lane >> lp_log2);
+      const bool live = p < p1;
+      float gk[D];
+#pragma unroll
+      for (int k = 0; k < D; ++k) gk[k] = 0.f;
+      int row = 0;
+      if (live) {
+        row = perm[p];
+        float4 w[D], dw[D];
+        int node = 0;
+#pragma unroll
+        for (int i = 0; i < D; ++i) {
+          float a[4], da[4];
+          ski_axis_weights<true>(X[(int64_t)row * ldx + i], g.lo[i], g.step[i], g.G[i], a, da);
+          w[i] = make_float4(a[0], a[1], a[2], a[3]);
+          dw[i] = make_float4(da[0], da[1], da[2], da[3]);
+          node += (first_s[(int64_t)p * D + i] - b.base[i]) * b.pitch[i];
+        }
+        if (col < 2 * tc) {
+          const float coef = (col < tc) ? L[(int64_t)row * ldl + col] : R[(int64_t)row * ldr + (col - tc)];
+          const float* base = blk + ((size_t)node << lp_log2) + col;
+#pragma unroll
+          for (int k = 0; k < D; ++k) {
+            float4 wk[D];
+#pragma unroll
+            for (int i = 0; i < D; ++i) wk[i] = (i == k) ? dw[i] : w[i];
+            gk[k] = coef * SkiInterpSum<D, 0>::run(base, wk, pitch);
+          }
+        }
+      }
+      for (int o = 1; o < lp; o <<= 1) {
+#pragma unroll
+        for (int k = 0; k < D; ++k) gk[k] += __shfl_xor_sync(0xffffffffu, gk[k], o);
+      }
+      if (live && col == 0) {
+        float* dst = DX + (int64_t)row * lddx;
+#pragma unroll
+        for (int k = 0; k < D; ++k) dst[k] = accumulate ? dst[k] + gk[k] : gk[k];
+      }
+    }
+  }
+}
+
+template <int D>
+static int ski_input_grad_d(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, float* DX, int64_t lddx) {
+  gp_ski_state* s = p->ski;
+  cudaStream_t st = p->stream;
+  const SkiGeom g = ski_geom<D>(s);
+  const SkiTiles tl = ski_tiles_of(s, D);
+  GP_CHECK(opt_in_smem<ski_input_grad_tiled_kernel<D>>(p->device, SKI_TILE_SMEM));
+  const int parts = ski_tile_parts(p);
+  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
+  const size_t nodes = ski_tile_smem(s, D) / (TP * sizeof(float));
+  // B_R / B_L of one 16-column chunk live in the bilinear derivative's grid blocks (allocated by the hyper-parameter backward)
+  GP_CHECK(p->V16.ensure(sizeof(float) * p->n1 * TP));
+  GP_CHECK(s->gridC.ensure(sizeof(float) * g.M * TP));
+  GP_CHECK(s->gridD.ensure(sizeof(float) * g.M * TP));
+  float* BR = s->gridC.as<float>();
+  float* BL = s->gridD.as<float>();
+  const unsigned eg = (unsigned)cdiv(g.M * TP, 256);
+  for (int c0 = 0; c0 < t; c0 += TP) {
+    const int tc = std::min(TP, t - c0);
+    float* cur = nullptr;
+    GP_CHECK(to_v16(p, R + c0, ldr, tc, p->n1, p->V16.as<float>()));
+    GP_CHECK(ski_grid_apply_d<D>(p, p->V16.as<float>(), &cur));
+    ski_grid_export_kernel<<<eg, 256, 0, st>>>(cur, g.M, TP, p->outputscale, BR, TP);
+    GP_CHECK(to_v16(p, L + c0, ldl, tc, p->n1, p->V16.as<float>()));
+    GP_CHECK(ski_grid_apply_d<D>(p, p->V16.as<float>(), &cur));
+    ski_grid_export_kernel<<<eg, 256, 0, st>>>(cur, g.M, TP, p->outputscale, BL, TP);
+    int lg = 1;
+    while ((1 << lg) < 2 * tc) ++lg;
+    ski_input_grad_tiled_kernel<D><<<tgrid, SKI_IP_THREADS, nodes * (sizeof(float) << lg), st>>>(
+        s->first_s.as<int>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, p->X1, p->ld1, BR, BL, tc, lg, L + c0, ldl,
+        R + c0, ldr, c0 > 0, DX, lddx);
+    p->launches += 3;
+  }
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
 // the arguments both calls share: a packed, unsharded SKI plan; t >= 1 columns, leading dimensions >= t
 static int ski_predict_check(gp_plan* p, int t, int64_t ld_in, int64_t ld_out, const char* what) {
   GP_REQUIRE(p != nullptr && p->data_set && p->hypers_set, GP_E_STATE, "%s: plan not ready (set_data + set_ski + set_hypers)", what);
@@ -1064,6 +1225,21 @@ extern "C" int gp_ski_grid_matmul(gp_plan* p, const float* V, int64_t ldv, int t
     case 2: return ski_grid_matmul_d<2>(p, V, ldv, t, OUT, ldo);
     case 3: return ski_grid_matmul_d<3>(p, V, ldv, t, OUT, ldo);
     case 4: return ski_grid_matmul_d<4>(p, V, ldv, t, OUT, ldo);
+  }
+  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
+  return GP_E_SHAPE;
+}
+
+extern "C" int gp_ski_input_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, float* DX, int64_t lddx) {
+  GP_CHECK(ski_predict_check(p, t, ldl, ldr, "gp_ski_input_grad"));
+  GP_REFUSE_LOWRANK(p, "gp_ski_input_grad");
+  GP_REQUIRE(L && R && DX && lddx >= p->d, GP_E_SHAPE, "gp_ski_input_grad: bad output (leading dimension %lld, d=%d)", (long long)lddx, p->d);
+  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
+  switch (p->d) {
+    case 1: return ski_input_grad_d<1>(p, L, ldl, R, ldr, t, DX, lddx);
+    case 2: return ski_input_grad_d<2>(p, L, ldl, R, ldr, t, DX, lddx);
+    case 3: return ski_input_grad_d<3>(p, L, ldl, R, ldr, t, DX, lddx);
+    case 4: return ski_input_grad_d<4>(p, L, ldl, R, ldr, t, DX, lddx);
   }
   set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
   return GP_E_SHAPE;

@@ -155,6 +155,18 @@ class Plan:
             check(self.lib.gp_ski_interp_matmul(self._h, _ptr(c2), c2.stride(0), c2.size(1), _ptr(out), out.stride(0)))
         return out.squeeze(-1) if vec else out
 
+    def ski_input_grad(self, left: torch.Tensor, right: torch.Tensor) -> torch.Tensor:
+        """dF/dx [n, d] of F = sum(left * (K_ski @ right)) for left, right [n] or [n, t] over the plan's points: the input gradient
+        of the interpolated operator (outputscale folded in, noise excluded; the grid covariance does not move with x)."""
+        l2, _ = self._ski_block(left, False, "left")
+        r2, _ = self._ski_block(right, False, "right")
+        if l2.size(1) != r2.size(1):
+            raise RuntimeError(f"ski_input_grad: left and right need the same columns (got {tuple(left.shape)}, {tuple(right.shape)})")
+        out = torch.empty(self.n1, self.d, device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_ski_input_grad(self._h, _ptr(l2), _ld(l2), _ptr(r2), _ld(r2), r2.size(1), _ptr(out), out.stride(0)))
+        return out
+
     def set_sum(self, terms):
         """Kernel sum (AdditiveKernel): this plan's operator becomes sum_t K_t (+ its own noise).  `terms` are ready plans over
         the same rows (their own kind / lengthscales / outputscale / active dimensions); they must outlive this plan.  Call after

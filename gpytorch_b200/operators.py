@@ -14,6 +14,8 @@ All arithmetic runs in libgpbbmm (CUDA); torch supplies memory, streams and the 
 """
 from __future__ import annotations
 
+import weakref
+
 import torch
 
 from . import settings
@@ -34,29 +36,42 @@ _PLAN_CACHE_MAX = 64          # a batch of 16 independent operators (+ their cro
 _PLAN_LOCK = __import__("threading").RLock()   # BatchLinearOperator drives the cache from worker threads
 
 
-def _get_plan(x1, x2, backend, row_begin, row_count, comm, slot=0) -> Plan:
+def _get_plan(x1, x2, backend, row_begin, row_count, comm, slot=0, owner=None) -> Plan:
     if not x1.is_cuda:
         raise RuntimeError("x1 must live on a CUDA device: gpytorch_b200 has no CPU path")
     with _PLAN_LOCK:
-        return _get_plan_locked(x1, x2, backend, row_begin, row_count, comm, slot)
+        return _get_plan_locked(x1, x2, backend, row_begin, row_count, comm, slot, owner)
 
 
-def _get_plan_locked(x1, x2, backend, row_begin, row_count, comm, slot=0) -> Plan:
+def _get_plan_locked(x1, x2, backend, row_begin, row_count, comm, slot=0, owner=None) -> Plan:
     # a plan enqueues on the stream that was current when it was created: the stream is part of the identity; so is the slot:
     # the terms of a kernel sum over the SAME inputs need one plan each (each holds its own packed lengthscales)
-    key = (x1.data_ptr(), tuple(x1.shape), x1.stride(0), None if x2 is None else (x2.data_ptr(), tuple(x2.shape), x2.stride(0)),
-           backend, str(x1.device), row_begin, row_count, id(comm), torch.cuda.current_stream(x1.device).cuda_stream, slot)
+    role = (tuple(x1.shape), x1.stride(0), None if x2 is None else (tuple(x2.shape), x2.stride(0)), backend, str(x1.device),
+            row_begin, row_count, id(comm), torch.cuda.current_stream(x1.device).cuda_stream, slot)
+    key = (x1.data_ptr(), None if x2 is None else x2.data_ptr(), role)
     plan = _PLAN_CACHE.pop(key, None)
     src_versions = (x1._version, None if x2 is None else x2._version)
+    if plan is None:
+        # New buffers in a known role: deep kernel learning computes new features every step, and the plan holds the old ones, so
+        # their address never comes back.  Re-point a plan of the same role whose operators are all gone instead of growing a
+        # new one (with its workspaces) per step; a plan that a live operator uses is never taken.
+        for k, cand in _PLAN_CACHE.items():
+            if k[2] == role and not cand._owners:
+                plan = _PLAN_CACHE.pop(k)
+                plan._src_versions = None
+                break
     if plan is not None and plan._src_versions != src_versions:
-        # same buffers, new contents (x.copy_(new), an optimiser step on the inputs, ...): the packed tiles are stale.
-        # torch bumps a tensor's version counter on every in-place write, so this is exact, not a heuristic.
+        # same buffers, new contents (x.copy_(new), an optimiser step on the inputs, ...) or a re-pointed plan: the packed tiles
+        # are stale.  torch bumps a tensor's version counter on every in-place write, so this is exact, not a heuristic.
         plan.x1 = x1.contiguous()
         plan.x2 = plan.x1 if x2 is None else x2.contiguous()
         plan.refresh_data()
     if plan is None:
         plan = Plan(x1, x2, backend="auto" if backend.startswith("ski:") else backend, row_begin=row_begin, row_count=row_count, comm=comm)
         plan._hyp_key = None
+        plan._owners = weakref.WeakSet()
+    if owner is not None:
+        plan._owners.add(owner)
     plan._src_versions = src_versions
     _PLAN_CACHE[key] = plan  # most recently used last
     while len(_PLAN_CACHE) > _PLAN_CACHE_MAX:
@@ -260,7 +275,7 @@ class KernelLinearOperator(_SamplingMixin):
         fresh = False
         if self._plan is None:
             self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(),
-                                   self._row_begin, self._row_count, self._comm, getattr(self, "_plan_slot", 0))
+                                   self._row_begin, self._row_count, self._comm, getattr(self, "_plan_slot", 0), owner=self)
             fresh = True
         if torch.is_tensor(noise):
             ls, os_, nz, _ = self._host_hypers(noise)
@@ -312,6 +327,11 @@ class KernelLinearOperator(_SamplingMixin):
         """The inputs K is differentiated in by the product and dense-block autograd functions below, which take them after
         the hyper-parameters: [x1] for a square operator (both arguments are the same points), [x1, x2] for a cross-covariance."""
         return [self.x1] if self.same else [self.x1, self.x2]
+
+    def solve_input_tensors(self):
+        """The inputs _InvQuadLogdet and _Solve differentiate K in, after the hyper-parameters: input_tensors() for an exact
+        operator or a kernel sum; a SKI operator adds its points there only (deep kernel learning trains through the MLL)."""
+        return self.input_tensors()
 
     def _bilinear_derivative_list(self, left, right):
         gl, go = self._bilinear_derivative(left, right)
@@ -471,6 +491,15 @@ class SumKernelLinearOperator(KernelLinearOperator):
             k += m
         return out
 
+    def _dense_input_grad_list(self, w, needs):
+        """One gp_kdense_input_grad call per term."""
+        out, k = [], 0
+        for o in self.ops:
+            m = len(o.input_tensors())
+            out.extend(o._dense_input_grad_list(w, needs[k:k + m]))
+            k += m
+        return out
+
     def _bilinear_derivative_list(self, left, right):
         out = []
         for o in self.ops:
@@ -495,6 +524,11 @@ class SumKernelLinearOperator(KernelLinearOperator):
                 parent = Plan(self.x1, None if self.same else self.x2, backend="auto", row_begin=self._row_begin,
                               row_count=self._row_count, comm=self._comm)
                 parent._hyp_key = None
+            elif parent.x1.data_ptr() != self.x1.data_ptr():
+                # the term plans were re-pointed to new inputs (_get_plan_locked): follow them
+                parent.x1 = self.x1.contiguous()
+                parent.x2 = parent.x1 if self.same else self.x2.contiguous()
+                parent.refresh_data()
             _SUM_PLANS[key] = parent
             while len(_SUM_PLANS) > 16:
                 _SUM_PLANS.pop(next(iter(_SUM_PLANS))).close()
@@ -551,7 +585,7 @@ class SKIKernelLinearOperator(KernelLinearOperator):
     def plan(self, noise=0.0) -> Plan:
         if self._plan is None:
             key = "ski:" + repr((self.grid_sizes, self.grid_lo, self.grid_step))
-            self._plan = _get_plan(self.x1, None, key, 0, 0, None, getattr(self, "_plan_slot", 0))
+            self._plan = _get_plan(self.x1, None, key, 0, 0, None, getattr(self, "_plan_slot", 0), owner=self)
             if getattr(self._plan, "_ski_key", None) != key:
                 self._plan.set_ski(self.grid_sizes, self.grid_lo, self.grid_step)
                 self._plan._ski_key = key
@@ -568,8 +602,25 @@ class SKIKernelLinearOperator(KernelLinearOperator):
         return self._plan
 
     def input_tensors(self):
-        """No inputs: SKI input gradients are not implemented, so the interpolated operator stays detached from its inputs."""
+        """No inputs: products, slices and the posterior paths of the interpolated operator stay detached from its inputs."""
         return []
+
+    def solve_input_tensors(self):
+        """[x1]: the MLL and solves reach the points through gp_ski_input_grad (deep kernel learning on KISS-GP)."""
+        return [self.x1]
+
+    def _input_grad_list(self, left, right, needs):
+        """[dF/dx1] of F = sum(left * (K_ski @ right)) (gp_ski_input_grad), [None] when not needed."""
+        if not any(needs):
+            return [None] * len(needs)
+        return [self.plan(getattr(self, "_last_noise", 0.0)).ski_input_grad(left, right)]
+
+    def _dense_input_grad_list(self, w, needs):
+        """[dF/dx1] of F = sum(w * K_ski): the product form with the identity, n columns.  Only the Cholesky branch of the solves
+        (n <= max_cholesky_size) asks for it; the engine has no dense SKI block."""
+        if not any(needs):
+            return [None] * len(needs)
+        return self._input_grad_list(w, torch.eye(w.size(0), device=w.device, dtype=w.dtype), needs)
 
     def detach(self):
         return SKIKernelLinearOperator(self.x1, self.kind, self.lengthscale.detach(), self.outputscale.detach(), self.grid_sizes,
@@ -789,6 +840,9 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
         return (self.U,)
 
     def hyper_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
         return []
 
     def _bilinear_derivative_list(self, left, right):
@@ -1108,7 +1162,7 @@ class AddedDiagLinearOperator(_SamplingMixin):
 
     def solve(self, rhs, lhs=None):
         """K_hat^{-1} rhs by preconditioned CG (LinearOperator.solve -> linear_cg, n_tridiag = 0)."""
-        out = _Solve.apply(self, rhs, self._noise_param, *self.kernel_op.hyper_tensors())
+        out = _Solve.apply(self, rhs, self._noise_param, *self.kernel_op.hyper_tensors(), *self.kernel_op.solve_input_tensors())
         return out if lhs is None else lhs @ out
 
     def inv_quad_logdet(self, inv_quad_rhs=None, logdet=False, reduce_inv_quad=True):
@@ -1120,7 +1174,8 @@ class AddedDiagLinearOperator(_SamplingMixin):
         rhs = inv_quad_rhs
         if rhs is not None and rhs.dim() == 1:
             rhs = rhs.unsqueeze(-1)
-        iq, ld = _InvQuadLogdet.apply(self, rhs, bool(logdet), self._noise_param, *self.kernel_op.hyper_tensors())
+        iq, ld = _InvQuadLogdet.apply(self, rhs, bool(logdet), self._noise_param, *self.kernel_op.hyper_tensors(),
+                                      *self.kernel_op.solve_input_tensors())
         if rhs is None:
             iq = torch.empty(0, device=self.device)
         elif reduce_inv_quad:
@@ -1312,8 +1367,12 @@ def _dense_branch(n: int, fast_flag) -> bool:
 
 
 class _Solve(torch.autograd.Function):
+    """K_hat^{-1} rhs.  Takes the kernel operator's hyper_tensors() and then its solve_input_tensors(); the backward asks the
+    engine for the input gradients autograd needs with the factors of the hyper-parameter backward, (-K_hat^-1 g, solve)."""
+
     @staticmethod
-    def forward(ctx, op, rhs, noise, *hypers):
+    def forward(ctx, op, rhs, noise, *tensors):
+        ctx.nh = len(op.kernel_op.hyper_tensors())
         vec = rhs.dim() == 1
         r2 = (rhs.unsqueeze(-1) if vec else rhs).detach().float().contiguous()
         n = op.shape[0]
@@ -1340,21 +1399,26 @@ class _Solve(torch.autograd.Function):
             gsol, _, _ = _run_cg(op, g, 0, w)
         grad_rhs = (gsol.squeeze(-1) if ctx.vec else gsol) if ctx.needs_input_grad[1] else None
         gn = None
-        grads = [None] * (len(ctx.needs_input_grad) - 3)
-        if any(ctx.needs_input_grad[2:]):
-            if any(ctx.needs_input_grad[3:]):
+        need_h, need_x = ctx.needs_input_grad[3:3 + ctx.nh], ctx.needs_input_grad[3 + ctx.nh:]
+        grads = [None] * ctx.nh
+        if any(ctx.needs_input_grad[2:3 + ctx.nh]):
+            if any(need_h):
                 gs = op.kernel_op._bilinear_derivative_list(-gsol, sol)
-                grads = [gi if need else None for gi, need in zip(gs, ctx.needs_input_grad[3:])]
+                grads = [gi if need else None for gi, need in zip(gs, need_h)]
             if ctx.needs_input_grad[2]:
                 gn = (-(gsol * sol).sum(-1)) if op.per_row else (-(gsol * sol).sum()).reshape(op.diag.diag_value.shape)
-        return (None, grad_rhs, gn, *grads)
+        xgrads = op.kernel_op._input_grad_list((-gsol).contiguous(), sol, need_x) if any(need_x) else [None] * len(need_x)
+        return (None, grad_rhs, gn, *grads, *xgrads)
 
 
 class _InvQuadLogdet(torch.autograd.Function):
-    """linear_operator.functions._inv_quad_logdet.InvQuadLogdet (SURVEY.md Appendix A.5)."""
+    """linear_operator.functions._inv_quad_logdet.InvQuadLogdet (SURVEY.md Appendix A.5).  Takes the kernel operator's
+    hyper_tensors() and then its solve_input_tensors().  The input gradients use the left / right factors of the hyper-parameter
+    backward on the CG branch, and the dense weight W = -sol diag(grad_iq) sol^T + grad_ld K_hat^-1 on the Cholesky branch."""
 
     @staticmethod
-    def forward(ctx, op, rhs, want_logdet, noise, *hypers):
+    def forward(ctx, op, rhs, want_logdet, noise, *tensors):
+        ctx.nh = len(op.kernel_op.hyper_tensors())
         n = op.shape[0]
         dev = op.device
         ctx.op, ctx.want_logdet, ctx.has_rhs = op, want_logdet, rhs is not None
@@ -1398,8 +1462,11 @@ class _InvQuadLogdet(torch.autograd.Function):
     def backward(ctx, grad_iq, grad_ld):
         op = ctx.op
         gn = grad_rhs = None
-        grads = [None] * (len(ctx.needs_input_grad) - 4)
-        need_k = any(ctx.needs_input_grad[3:])
+        nh = ctx.nh
+        grads = [None] * nh
+        need_h, need_x = ctx.needs_input_grad[4:4 + nh], ctx.needs_input_grad[4 + nh:]
+        xgrads = [None] * len(need_x)
+        need_k = any(ctx.needs_input_grad[3:4 + nh])
         if ctx.mode == "chol":
             chol, sol = ctx.saved_tensors
             n = op.shape[0]
@@ -1409,16 +1476,22 @@ class _InvQuadLogdet(torch.autograd.Function):
                 left_cols.append(-sol * grad_iq.reshape(1, -1)); right_cols.append(sol)
                 if ctx.needs_input_grad[1]:
                     grad_rhs = 2 * sol * grad_iq.reshape(1, -1)
+            kinv = torch.cholesky_inverse(chol) if (ctx.want_logdet and (need_k or any(need_x))) else None
             if need_k:
                 if ctx.want_logdet:
-                    kinv = torch.cholesky_inverse(chol)
                     left_cols.append(kinv * grad_ld); right_cols.append(torch.eye(n, device=op.device))
                 left = torch.cat(left_cols, -1).contiguous(); right = torch.cat(right_cols, -1).contiguous()
+            if any(need_x):
+                w = torch.zeros(n, n, device=op.device, dtype=torch.float32)
+                if ctx.has_rhs:
+                    w = w - (sol * grad_iq.reshape(1, -1)) @ sol.t()
+                if kinv is not None:
+                    w = w + grad_ld * kinv
         else:
             solves, probes, w = ctx.saved_tensors
             tp = ctx.tp
             left_cols, right_cols = [], []
-            if ctx.want_logdet and tp and need_k:
+            if ctx.want_logdet and tp and (need_k or any(need_x)):
                 coef = 1.0 / tp
                 norms = probes.norm(2, dim=-2, keepdim=True)
                 pv_solves = solves[:, :tp] * coef * norms * grad_ld   # (1/tp) K^-1 z_i
@@ -1435,12 +1508,16 @@ class _InvQuadLogdet(torch.autograd.Function):
                 left_cols.append(neg); right_cols.append(iq_solves)
                 if ctx.needs_input_grad[1]:
                     grad_rhs = -2 * neg
-            if need_k and left_cols:
+            if (need_k or any(need_x)) and left_cols:
                 left = torch.cat(left_cols, -1).contiguous(); right = torch.cat(right_cols, -1).contiguous()
         if need_k and left_cols:
-            if any(ctx.needs_input_grad[4:]):
+            if any(need_h):
                 gs = op.kernel_op._bilinear_derivative_list(left, right)
-                grads = [gi if need else None for gi, need in zip(gs, ctx.needs_input_grad[4:])]
+                grads = [gi if need else None for gi, need in zip(gs, need_h)]
             if ctx.needs_input_grad[3]:
                 gn = (left * right).sum(-1) if op.per_row else (left * right).sum().reshape(op.diag.diag_value.shape)
-        return (None, grad_rhs, None, gn, *grads)
+        if any(need_x) and ctx.mode == "chol":
+            xgrads = op.kernel_op._dense_input_grad_list(w.contiguous(), need_x)
+        elif any(need_x) and left_cols:
+            xgrads = op.kernel_op._input_grad_list(left, right, need_x)
+        return (None, grad_rhs, None, gn, *grads, *xgrads)

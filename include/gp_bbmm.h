@@ -103,6 +103,15 @@ int gp_plan_set_ski(gp_plan* plan, const int* grid_sizes, const float* grid_lo, 
 int gp_ski_grid_matmul(gp_plan* plan, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo);
 int gp_ski_interp_matmul(gp_plan* plan, const float* C, int64_t ldc, int t, float* OUT, int64_t ldo);
 
+/* Input gradient of a SKI operator (deep kernel learning through KISS-GP): DX[n, d] (lddx >= d) = dF/dX of
+ * F = sum_ic L_ic (K_ski R)_ic, K_ski = s W K_uu W^T, L and R [n, t] over the plan's points (ldl, ldr >= t, any t >= 1), in raw input
+ * units.  Only W depends on X: the derivative of the Keys cubic weights, exactly 0 in the one-hot first / last grid cells, as the
+ * reference's autograd through Interpolation.interpolate gives.  The gradient pass has no atomics; its grid blocks come from the
+ * SKI scatter (per-tile atomic adds), so repeated calls agree to fp32 rounding.  A non-finite L
+ * or R gives NaN.  GP_E_STATE on a non-SKI plan or one with a low-rank correction; GP_E_SHAPE for a row-sharded plan, t < 1 or
+ * bad leading dimensions. */
+int gp_ski_input_grad(gp_plan* plan, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, float* DX, int64_t lddx);
+
 /* Kernel sums (AdditiveKernel, kernels/kernel.py:592-621: k = k_1 + ... + k_m, each term with its own covariance function,
  * lengthscale(s), outputscale and active dimensions): `plan` becomes the operator  sum_t K_t  (+ its own noise), where every
  * K_t is a ready plan over the same rows (same n1 / n2 / row shard / stream; the data pointers may differ: active_dims).
