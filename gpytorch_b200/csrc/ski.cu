@@ -25,6 +25,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "gp_common.cuh"
 #include "ski_rows.cuh"
@@ -206,23 +207,43 @@ __device__ __forceinline__ SkiBlock<D> ski_block_of(int tile, const SkiGeom& g, 
   b.nodes = pch;
   return b;
 }
-// Row-wise traversal of a tile's node block for the exchanges with the global grid block: a "row" fixes the coordinates of
-// dimensions 0 .. D-2 (one division chain per row instead of one per element), the lanes cover (last-dimension node, column
-// group) pairs, 8 nodes x 4 groups per pass.  fn(local node, global flat index, column group).
+// Work item wk = (tile, part) of a tiled pass: crowded tiles (few tiles, many points: small grids in low dimension) are shared by
+// `parts` CTAs, part taking the sorted points [p0, p1) of its tile.  False when that range is empty.
+__device__ __forceinline__ bool ski_work_range(int64_t wk, int parts, const int* __restrict__ off, int& tile, int& p0, int& p1) {
+  tile = (int)(wk / parts);
+  const int part = (int)(wk % parts);
+  const int t0 = off[tile], tn = off[tile + 1] - t0;
+  p0 = t0 + (int)((int64_t)tn * part / parts);
+  p1 = t0 + (int)((int64_t)tn * (part + 1) / parts);
+  return p0 != p1;
+}
+// A "row" of a tile's node block fixes the coordinates of dimensions 0 .. D-2: block-local node and global flat index of its
+// first node (one division chain per row instead of one per element)
+struct SkiRowOrigin {
+  int node0;
+  int64_t idx0;
+};
+template <int D>
+__device__ __forceinline__ SkiRowOrigin ski_row_origin(const SkiBlock<D>& b, const SkiGeom& g, int row) {
+  int rem = row, node0 = 0;
+  int64_t idx0 = (int64_t)b.base[D - 1] * g.stride[D - 1];
+#pragma unroll
+  for (int i = D - 2; i >= 0; --i) {
+    const int c = rem % b.ext[i];
+    rem /= b.ext[i];
+    node0 += c * b.pitch[i];
+    idx0 += (int64_t)(b.base[i] + c) * g.stride[i];
+  }
+  return {node0, idx0};
+}
+// Row-wise traversal of a tile's node block for the exchanges with the global grid block: the lanes cover (last-dimension node,
+// column group) pairs of a row, 8 nodes x 4 groups per pass.  fn(local node, global flat index, column group).
 template <int D, typename F>
 __device__ __forceinline__ void ski_block_rows(const SkiBlock<D>& b, const SkiGeom& g, int warp, int nwarps, int lane, F fn) {
   const int last = b.ext[D - 1];
   const int nrows = b.nodes / last;
   for (int row = warp; row < nrows; row += nwarps) {
-    int rem = row, node0 = 0;
-    int64_t idx0 = (int64_t)b.base[D - 1] * g.stride[D - 1];
-#pragma unroll
-    for (int i = D - 2; i >= 0; --i) {
-      const int c = rem % b.ext[i];
-      rem /= b.ext[i];
-      node0 += c * b.pitch[i];
-      idx0 += (int64_t)(b.base[i] + c) * g.stride[i];
-    }
+    const auto [node0, idx0] = ski_row_origin<D>(b, g, row);
     for (int c = lane >> 2; c < last; c += 8) fn(node0 + c, idx0 + (int64_t)c * g.stride[D - 1], lane & 3);
   }
 }
@@ -278,12 +299,9 @@ ski_scatter_tiled_kernel(const int* __restrict__ first_s, const float* __restric
   extern __shared__ __align__(16) float blk[];   // [4 column groups][nodes][4]: a warp's 32 lanes (32 nodes, one column group) then
                                                  // spread over all banks; with [nodes][16] they hit 4 banks (16-way conflicts, 1.3 ms)
   const int tid = threadIdx.x, lane = tid & 31, cg = tid >> 5;
-  // work item = (tile, part): crowded tiles (few tiles, many points: small grids in low dimension) are shared by `parts` CTAs
   for (int64_t wk = blockIdx.x; wk < (int64_t)tl.ntiles * parts; wk += gridDim.x) {
-    const int tile = (int)(wk / parts), part = (int)(wk % parts);
-    const int t0 = off[tile], tn = off[tile + 1] - t0;
-    const int p0 = t0 + (int)((int64_t)tn * part / parts), p1 = t0 + (int)((int64_t)tn * (part + 1) / parts);
-    if (p0 == p1) continue;
+    int tile, p0, p1;
+    if (!ski_work_range(wk, parts, off, tile, p0, p1)) continue;
     const SkiBlock<D> b = ski_block_of<D>(tile, g, tl);
     __syncthreads();
     for (int e = tid; e < b.nodes * 4; e += SKI_SC_THREADS) reinterpret_cast<float4*>(blk)[e] = make_float4(0, 0, 0, 0);
@@ -344,10 +362,8 @@ ski_gather_tiled_kernel(const int* __restrict__ first_s, const float* __restrict
   extern __shared__ __align__(16) float blk[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, cg = lane & 3;
   for (int64_t wk = blockIdx.x; wk < (int64_t)tl.ntiles * parts; wk += gridDim.x) {
-    const int tile = (int)(wk / parts), part = (int)(wk % parts);
-    const int t0 = off[tile], tn = off[tile + 1] - t0;
-    const int p0 = t0 + (int)((int64_t)tn * part / parts), p1 = t0 + (int)((int64_t)tn * (part + 1) / parts);
-    if (p0 == p1) continue;
+    int tile, p0, p1;
+    if (!ski_work_range(wk, parts, off, tile, p0, p1)) continue;
     const SkiBlock<D> b = ski_block_of<D>(tile, g, tl);
     __syncthreads();
     ski_block_rows<D>(b, g, warp, 8, lane, [&](int node, int64_t idx, int q4) {
@@ -545,6 +561,27 @@ static size_t ski_mode_smem(int G) {
   return sizeof(float) * (GM * (GK + 4) + 2 * GK * SKI_BP);
 }
 
+// fn(std::integral_constant<int, D>()) for D = d: the passes are compiled once per dimension 1 .. SKI_MAXD
+template <typename F>
+static int ski_with_d(int d, F&& fn) {
+  switch (d) {
+    case 1: return fn(std::integral_constant<int, 1>());
+    case 2: return fn(std::integral_constant<int, 2>());
+    case 3: return fn(std::integral_constant<int, 3>());
+    case 4: return fn(std::integral_constant<int, 4>());
+  }
+  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", d);
+  return GP_E_SHAPE;
+}
+
+static SkiGeom ski_geom(const gp_ski_state* s, int d) {
+  SkiGeom g;
+  g.d = d;
+  g.M = 1;
+  for (int i = d - 1; i >= 0; --i) { g.G[i] = s->G[i]; g.lo[i] = s->lo[i]; g.step[i] = s->step[i]; g.stride[i] = g.M; g.M *= s->G[i]; }
+  return g;
+}
+
 static SkiTiles ski_tiles_of(const gp_ski_state* s, int d) {
   SkiTiles tl;
   tl.ntiles = s->ntiles;
@@ -580,46 +617,48 @@ static int ski_bucket_points(gp_plan* p, const SkiGeom& g) {
   const unsigned gb = (unsigned)cdiv(n, 256);
   int* cnt = s->tile_cnt.as<int>();
   int* off = s->tile_off.as<int>();
-#define GP_SKI_BUCKET(DD)                                                                                                   \
-  case DD:                                                                                                                  \
-    ski_tile_count_kernel<DD><<<gb, 256, 0, st>>>(s->first.as<int>(), n, tl, cnt);                                          \
-    ski_tile_scan_kernel<<<1, 1024, 0, st>>>(cnt, (int)nt, off);                                                            \
-    ski_tile_fill_kernel<DD><<<gb, 256, 0, st>>>(s->first.as<int>(), s->wts.as<float>(), n, tl, off, cnt, s->perm.as<int>(), \
-                                                 s->first_s.as<int>(), s->wts_s.as<float>());                               \
-    break;
-  switch (d) {
-    GP_SKI_BUCKET(1)
-    GP_SKI_BUCKET(2)
-    GP_SKI_BUCKET(3)
-    GP_SKI_BUCKET(4)
-  }
-#undef GP_SKI_BUCKET
+  GP_CHECK(ski_with_d(d, [&](auto D) {
+    ski_tile_count_kernel<D><<<gb, 256, 0, st>>>(s->first.as<int>(), n, tl, cnt);
+    ski_tile_scan_kernel<<<1, 1024, 0, st>>>(cnt, (int)nt, off);
+    ski_tile_fill_kernel<D><<<gb, 256, 0, st>>>(s->first.as<int>(), s->wts.as<float>(), n, tl, off, cnt, s->perm.as<int>(),
+                                                s->first_s.as<int>(), s->wts_s.as<float>());
+    return GP_OK;
+  }));
   p->launches += 3;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
 
-constexpr int SKI_TILE_SMEM = 96 * 1024;
+constexpr int SKI_TILE_SMEM = 96 * 1024;   // dynamic shared memory the tiled kernels opt in to
+constexpr int SKI_IP_CW = 32;              // columns per chunk of the interpolation and input-gradient passes
+
+// Launch shape of the tiled passes (scatter, gather, interpolation, input gradient): one CTA per (tile, part) work item, parts =
+// CTAs per tile at ~256 points each on average (no host read-back of the real counts: the split only balances load), at most 16
+// CTAs per SM striding over the work items; a CTA stages the nodes of its tile's block in shared memory.
+struct SkiPass {
+  SkiGeom g;
+  SkiTiles tl;
+  int parts;
+  unsigned grid;
+  size_t nodes;   // nodes of the largest tile block
+};
 template <int D>
-static int ski_tiled_attrs(gp_plan* p) {
-  static bool done[64] = {};
-  if (!done[p->device & 63]) {
-    GP_CUDA(cudaFuncSetAttribute(ski_scatter_tiled_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, SKI_TILE_SMEM));
-    GP_CUDA(cudaFuncSetAttribute(ski_gather_tiled_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, SKI_TILE_SMEM));
-    done[p->device & 63] = true;
-  }
+static int ski_tiled_pass(gp_plan* p, SkiPass* ps) {
+  const gp_ski_state* s = p->ski;
+  ps->g = ski_geom(s, D);
+  ps->tl = ski_tiles_of(s, D);
+  const int64_t avg = p->n1 / std::max(1, s->ntiles);
+  ps->parts = (int)std::min<int64_t>(1024, std::max<int64_t>(1, cdiv(avg, 256)));
+  ps->grid = (unsigned)std::min<int64_t>((int64_t)ps->tl.ntiles * ps->parts, 16 * (int64_t)p->n_sm);
+  ps->nodes = 1;
+  for (int i = 0; i < D; ++i) ps->nodes *= (size_t)std::min(s->tile_edge[i] + 3, s->G[i]);
+  // the widest staging: SKI_IP_CW floats per node (the scatter and gather stage TP)
+  GP_REQUIRE(ps->nodes * SKI_IP_CW * sizeof(float) <= (size_t)SKI_TILE_SMEM, GP_E_SHAPE,
+             "SKI: tile block of %zu nodes does not fit in shared memory", ps->nodes);
+  // the interpolation and input-gradient kernels (below) opt in where they are launched
+  GP_CHECK(opt_in_smem<ski_scatter_tiled_kernel<D>>(p->device, SKI_TILE_SMEM));
+  GP_CHECK(opt_in_smem<ski_gather_tiled_kernel<D>>(p->device, SKI_TILE_SMEM));
   return GP_OK;
-}
-// CTAs per tile: ~256 points each on average (no host read-back of the real counts: the split only balances load)
-static int ski_tile_parts(const gp_plan* p) {
-  const int64_t avg = p->n1 / std::max(1, p->ski->ntiles);
-  return (int)std::min<int64_t>(1024, std::max<int64_t>(1, cdiv(avg, 256)));
-}
-// shared memory of one tile's node block
-static size_t ski_tile_smem(const gp_ski_state* s, int d) {
-  size_t nodes = 1;
-  for (int i = 0; i < d; ++i) nodes *= (size_t)std::min(s->tile_edge[i] + 3, s->G[i]);
-  return nodes * TP * sizeof(float);
 }
 
 int ski_pack(gp_plan* p) {
@@ -629,10 +668,7 @@ int ski_pack(gp_plan* p) {
   cudaStream_t st = p->stream;
   const int d = p->d;
   const int64_t n = p->n1;
-  SkiGeom g;
-  g.d = d;
-  g.M = 1;
-  for (int i = d - 1; i >= 0; --i) { g.G[i] = s->G[i]; g.lo[i] = s->lo[i]; g.step[i] = s->step[i]; g.stride[i] = g.M; g.M *= s->G[i]; }
+  const SkiGeom g = ski_geom(s, d);
   s->M = g.M;
   GP_CHECK(s->first.ensure(sizeof(int) * n * d));
   GP_CHECK(s->wts.ensure(sizeof(float) * n * d * 4));
@@ -671,62 +707,53 @@ int ski_pack(gp_plan* p) {
   return GP_OK;
 }
 
-template <int D>
-static SkiGeom ski_geom(const gp_ski_state* s) {
-  SkiGeom g;
-  g.d = D;
-  g.M = 1;
-  for (int i = D - 1; i >= 0; --i) { g.G[i] = s->G[i]; g.lo[i] = s->lo[i]; g.step[i] = s->step[i]; g.stride[i] = g.M; g.M *= s->G[i]; }
-  return g;
+// d mode products  *out = (F_0 x ... x F_{d-1}) in,  F_i = dT_i for i == dt_dim and T_i otherwise (dt_dim = -1: K_uu).  Product i
+// writes bufs[i & 1]; `in` may be buf1 (overwritten after the first product), and *out is the buffer of the last product.
+static int ski_mode_products(gp_plan* p, const SkiGeom& g, const float* in, float* buf0, float* buf1, int dt_dim, float** out) {
+  const gp_ski_state* s = p->ski;
+  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
+  float* bufs[2] = {buf0, buf1};
+  const float* cur = in;
+  size_t toff = 0;
+  for (int i = 0; i < g.d; ++i) {
+    const int G = g.G[i];
+    const int64_t inner = g.stride[i] * TP;                // elements after mode i (incl. the 16 columns)
+    const int64_t total = g.M / G * TP;                    // positions of the flattened (outer, inner) space
+    const int64_t nslab = cdiv(total, SKI_MT);
+    const float* F = (i == dt_dim ? s->dT : s->T).as<float>() + toff;
+    GP_REQUIRE(total < ((int64_t)1 << 31), GP_E_SHAPE, "SKI: grid block too large");
+    ski_mode_kernel<<<(unsigned)std::min<int64_t>(nslab, 2 * p->n_sm), 256, ski_mode_smem(G), p->stream>>>(F, G, cur, bufs[i & 1], inner, total, nslab);
+    cur = bufs[i & 1];
+    toff += (size_t)G * G;
+  }
+  p->launches += g.d;
+  *out = bufs[(g.d - 1) & 1];
+  return GP_OK;
 }
 
 // scatter + d mode products: *grid_out = (T_0 x ... x T_{d-1}) W^T V16, a [M][16] block (gridA or gridB)
 template <int D>
-static int ski_grid_apply_d(gp_plan* p, const float* V16, float** grid_out) {
+static int ski_grid_apply(gp_plan* p, const SkiPass& ps, const float* V16, float** grid_out) {
   gp_ski_state* s = p->ski;
-  cudaStream_t st = p->stream;
-  const SkiGeom g = ski_geom<D>(s);
   float* A = s->gridA.as<float>();
-  float* B = s->gridB.as<float>();
-  const SkiTiles tl = ski_tiles_of(s, D);
-  const size_t tsm = ski_tile_smem(s, D);
-  GP_REQUIRE(tsm <= (size_t)SKI_TILE_SMEM, GP_E_SHAPE, "SKI: tile block of %zu bytes does not fit in shared memory", tsm);
-  GP_CHECK(ski_tiled_attrs<D>(p));
-  const int parts = ski_tile_parts(p);
-  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
-  GP_CUDA(cudaMemsetAsync(A, 0, sizeof(float) * g.M * TP, st));
-  ski_scatter_tiled_kernel<D><<<tgrid, SKI_SC_THREADS, tsm, st>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, V16, A);
-  size_t toff = 0;
-  float* cur = A;
-  float* nxt = B;
-  for (int i = 0; i < D; ++i) {
-    const int G = s->G[i];
-    const int64_t inner = g.stride[i] * TP;                // elements after mode i (incl. the 16 columns)
-    const int64_t total = g.M / G * TP;                    // positions of the flattened (outer, inner) space
-    const int64_t nslab = cdiv(total, SKI_MT);
-    const size_t sh = ski_mode_smem(G);
-    GP_REQUIRE(total < ((int64_t)1 << 31), GP_E_SHAPE, "SKI: grid block too large");
-    ski_mode_kernel<<<(unsigned)std::min<int64_t>(nslab, 2 * p->n_sm), 256, sh, st>>>(s->T.as<float>() + toff, G, cur, nxt, inner, total, nslab);
-    toff += (size_t)G * G;
-    std::swap(cur, nxt);
-  }
-  p->launches += 1 + D;
+  GP_CUDA(cudaMemsetAsync(A, 0, sizeof(float) * ps.g.M * TP, p->stream));
+  ski_scatter_tiled_kernel<D><<<ps.grid, SKI_SC_THREADS, ps.nodes * TP * sizeof(float), p->stream>>>(
+      s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), ps.g, ps.tl, ps.parts, V16, A);
+  p->launches++;
+  GP_CHECK(ski_mode_products(p, ps.g, A, s->gridB.as<float>(), A, -1, grid_out));
   GP_CUDA(cudaGetLastError());
-  *grid_out = cur;
   return GP_OK;
 }
 
 template <int D>
 static int ski_matmul_d(gp_plan* p, const float* V16, float* OUT16) {
   gp_ski_state* s = p->ski;
-  const SkiGeom g = ski_geom<D>(s);
+  SkiPass ps;
+  GP_CHECK(ski_tiled_pass<D>(p, &ps));
   float* cur = nullptr;
-  GP_CHECK(ski_grid_apply_d<D>(p, V16, &cur));
-  const SkiTiles tl = ski_tiles_of(s, D);
-  const int parts = ski_tile_parts(p);
-  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
-  ski_gather_tiled_kernel<D><<<tgrid, 256, ski_tile_smem(s, D), p->stream>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(),
-                                                                            s->tile_off.as<int>(), g, tl, parts, cur, OUT16);
+  GP_CHECK(ski_grid_apply<D>(p, ps, V16, &cur));
+  ski_gather_tiled_kernel<D><<<ps.grid, 256, ps.nodes * TP * sizeof(float), p->stream>>>(
+      s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), ps.g, ps.tl, ps.parts, cur, OUT16);
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -741,18 +768,11 @@ template <int D>
 static int ski_bilinear_d(gp_plan* p, const float* L16, const float* R16, double* total) {
   gp_ski_state* s = p->ski;
   cudaStream_t st = p->stream;
-  const int64_t n = p->n1;
-  SkiGeom g;
-  g.d = D;
-  g.M = 1;
-  for (int i = D - 1; i >= 0; --i) { g.G[i] = s->G[i]; g.lo[i] = s->lo[i]; g.step[i] = s->step[i]; g.stride[i] = g.M; g.M *= s->G[i]; }
-  (void)n;
   constexpr int DOT_BLOCKS = 296;
-  const SkiTiles tl = ski_tiles_of(s, D);
-  const size_t tsm = ski_tile_smem(s, D);
-  GP_CHECK(ski_tiled_attrs<D>(p));
-  const int parts = ski_tile_parts(p);
-  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
+  SkiPass ps;
+  GP_CHECK(ski_tiled_pass<D>(p, &ps));
+  const SkiGeom& g = ps.g;
+  const size_t tsm = ps.nodes * TP * sizeof(float);
   GP_CHECK(s->gridC.ensure(sizeof(float) * g.M * TP));
   GP_CHECK(s->gridD.ensure(sizeof(float) * g.M * TP));
   GP_CHECK(p->misc.ensure(sizeof(double) * DOT_BLOCKS * (D + 1)));
@@ -761,28 +781,14 @@ static int ski_bilinear_d(gp_plan* p, const float* L16, const float* R16, double
   double* part = p->misc.as<double>();
   GP_CUDA(cudaMemsetAsync(A, 0, sizeof(float) * g.M * TP, st));
   GP_CUDA(cudaMemsetAsync(B, 0, sizeof(float) * g.M * TP, st));
-  ski_scatter_tiled_kernel<D><<<tgrid, SKI_SC_THREADS, tsm, st>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, L16, A);
-  ski_scatter_tiled_kernel<D><<<tgrid, SKI_SC_THREADS, tsm, st>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, R16, B);
+  ski_scatter_tiled_kernel<D><<<ps.grid, SKI_SC_THREADS, tsm, st>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, ps.tl, ps.parts, L16, A);
+  ski_scatter_tiled_kernel<D><<<ps.grid, SKI_SC_THREADS, tsm, st>>>(s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, ps.tl, ps.parts, R16, B);
   p->launches += 2;
   for (int term = 0; term <= D; ++term) {          // term 0: K_uu ; term 1 + i: derivative factor in dimension i
-    size_t toff = 0;
-    const float* cur = B;
-    float* bufs[2] = {s->gridA.as<float>(), s->gridB.as<float>()};
-    for (int i = 0; i < D; ++i) {
-      const int G = s->G[i];
-      const int64_t inner = g.stride[i] * TP;
-      const int64_t tot = g.M / G * TP;
-      const int64_t nslab = cdiv(tot, SKI_MT);
-      const size_t sh = ski_mode_smem(G);
-      const float* Tm = ((term == 1 + i) ? s->dT.as<float>() : s->T.as<float>()) + toff;
-      float* out = bufs[i & 1];
-      GP_REQUIRE(tot < ((int64_t)1 << 31), GP_E_SHAPE, "SKI: grid block too large");
-      ski_mode_kernel<<<(unsigned)std::min<int64_t>(nslab, 2 * p->n_sm), 256, sh, st>>>(Tm, G, cur, out, inner, tot, nslab);
-      cur = out;
-      toff += (size_t)G * G;
-    }
+    float* cur = nullptr;
+    GP_CHECK(ski_mode_products(p, g, B, s->gridA.as<float>(), s->gridB.as<float>(), term - 1, &cur));
     ski_dot_kernel<<<DOT_BLOCKS, 256, 0, st>>>(A, cur, g.M * TP / 4, part + (size_t)term * DOT_BLOCKS);
-    p->launches += D + 1;
+    p->launches++;
   }
   GP_CUDA(cudaGetLastError());
   std::vector<double> h((size_t)DOT_BLOCKS * (D + 1));
@@ -797,29 +803,13 @@ static int ski_bilinear_d(gp_plan* p, const float* L16, const float* R16, double
 }
 
 int ski_bilinear(gp_plan* p, const float* L16, const float* R16, double* total) {
-  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
-  switch (p->d) {
-    case 1: return ski_bilinear_d<1>(p, L16, R16, total);
-    case 2: return ski_bilinear_d<2>(p, L16, R16, total);
-    case 3: return ski_bilinear_d<3>(p, L16, R16, total);
-    case 4: return ski_bilinear_d<4>(p, L16, R16, total);
-  }
-  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
-  return GP_E_SHAPE;
+  return ski_with_d(p->d, [&](auto D) { return ski_bilinear_d<D>(p, L16, R16, total); });
 }
 
 // partial[0][r][:] = (W K_uu W^T V16)[r][:]   (outputscale / noise are applied by the finish kernels)
 int ski_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   (void)done_flag;   // the products of a finished mBCG are cheap no-ops for the dense kernels; here they simply run
-  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
-  switch (p->d) {
-    case 1: return ski_matmul_d<1>(p, V16, p->partial.as<float>());
-    case 2: return ski_matmul_d<2>(p, V16, p->partial.as<float>());
-    case 3: return ski_matmul_d<3>(p, V16, p->partial.as<float>());
-    case 4: return ski_matmul_d<4>(p, V16, p->partial.as<float>());
-  }
-  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
-  return GP_E_SHAPE;
+  return ski_with_d(p->d, [&](auto D) { return ski_matmul_d<D>(p, V16, p->partial.as<float>()); });
 }
 
 // ---- single entries (ski_rows.cuh): the diagonal, requested rows and the pivoted Cholesky (pivchol.cu) ----------------------------
@@ -928,6 +918,18 @@ __global__ void ski_grid_export_kernel(const float* __restrict__ U, int64_t M, i
   out[r * ldo + c] = s * U[r * TP + c];
 }
 
+// OUT[:, 0:tc] = s K_uu W^T V[:, 0:tc] for one chunk of tc <= 16 columns (staged in p->V16), OUT a [M][ldo] grid matrix
+template <int D>
+static int ski_grid_block(gp_plan* p, const SkiPass& ps, const float* V, int64_t ldv, int tc, float* OUT, int64_t ldo) {
+  float* cur = nullptr;
+  GP_CHECK(to_v16(p, V, ldv, tc, p->n1, p->V16.as<float>()));
+  GP_CHECK(ski_grid_apply<D>(p, ps, p->V16.as<float>(), &cur));
+  ski_grid_export_kernel<<<(unsigned)cdiv(ps.g.M * tc, 256), 256, 0, p->stream>>>(cur, ps.g.M, tc, p->outputscale, OUT, ldo);
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
 // sum_q w_q C[node_q] for one point and column in the fixed separable order  sum_a w_0[a] (sum_b w_1[b] (... C[...])):
 // b points at the point's first node, pitch[k] is the distance of neighbouring nodes of dimension k (in floats)
 template <int D, int K>
@@ -952,7 +954,6 @@ struct SkiInterpSum<D, D> {
 // points.  The point's 4 D weights sit in registers; no atomics and no cross-lane sums, so repeated calls are bit-identical
 // whatever ldc / ldo.  Staged with float4 loads when the chunk is full and 16-byte aligned (vec).
 constexpr int SKI_IP_THREADS = 256;
-constexpr int SKI_IP_CW = 32;   // columns per chunk
 template <int D>
 __global__ void __launch_bounds__(SKI_IP_THREADS)
 ski_interp_tiled_kernel(const int* __restrict__ first_s, const float* __restrict__ wts_s, const int* __restrict__ perm,
@@ -965,25 +966,15 @@ ski_interp_tiled_kernel(const int* __restrict__ first_s, const float* __restrict
   const int nslot = SKI_IP_THREADS >> lp_log2;
   const int gshift = vec ? lp_log2 - 2 : lp_log2;        // log2 of the staged column groups per node (float4 or float)
   for (int64_t wk = blockIdx.x; wk < (int64_t)tl.ntiles * parts; wk += gridDim.x) {
-    const int tile = (int)(wk / parts), part = (int)(wk % parts);
-    const int t0 = off[tile], tn = off[tile + 1] - t0;
-    const int p0 = t0 + (int)((int64_t)tn * part / parts), p1 = t0 + (int)((int64_t)tn * (part + 1) / parts);
-    if (p0 == p1) continue;
+    int tile, p0, p1;
+    if (!ski_work_range(wk, parts, off, tile, p0, p1)) continue;
     const SkiBlock<D> b = ski_block_of<D>(tile, g, tl);
     __syncthreads();
-    // staging, row by row as ski_block_rows: a row fixes dimensions 0 .. D-2, the lanes cover (last-dimension node, column group)
+    // staging, row by row as ski_block_rows: the lanes cover (last-dimension node, column group) pairs of a row
     const int last = b.ext[D - 1];
     const int nrows = b.nodes / last;
     for (int row = warp; row < nrows; row += SKI_IP_THREADS / 32) {
-      int rem = row, node0 = 0;
-      int64_t idx0 = (int64_t)b.base[D - 1] * g.stride[D - 1];
-#pragma unroll
-      for (int i = D - 2; i >= 0; --i) {
-        const int c = rem % b.ext[i];
-        rem /= b.ext[i];
-        node0 += c * b.pitch[i];
-        idx0 += (int64_t)(b.base[i] + c) * g.stride[i];
-      }
+      const auto [node0, idx0] = ski_row_origin<D>(b, g, row);
       for (int e = lane; e < (last << gshift); e += 32) {
         const int c = e >> gshift, q = e & ((1 << gshift) - 1);
         const float* src = C + (idx0 + (int64_t)c * g.stride[D - 1]) * ldc;
@@ -1014,37 +1005,27 @@ ski_interp_tiled_kernel(const int* __restrict__ first_s, const float* __restrict
 
 template <int D>
 static int ski_grid_matmul_d(gp_plan* p, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo) {
-  const int64_t M = ski_geom<D>(p->ski).M;
+  SkiPass ps;
+  GP_CHECK(ski_tiled_pass<D>(p, &ps));
   GP_CHECK(p->V16.ensure(sizeof(float) * p->n1 * TP));
-  for (int c0 = 0; c0 < t; c0 += TP) {
-    const int tc = std::min(TP, t - c0);
-    GP_CHECK(to_v16(p, V + c0, ldv, tc, p->n1, p->V16.as<float>()));
-    float* cur = nullptr;
-    GP_CHECK(ski_grid_apply_d<D>(p, p->V16.as<float>(), &cur));
-    ski_grid_export_kernel<<<(unsigned)cdiv(M * tc, 256), 256, 0, p->stream>>>(cur, M, tc, p->outputscale, OUT + c0, ldo);
-    p->launches++;
-  }
-  GP_CUDA(cudaGetLastError());
+  for (int c0 = 0; c0 < t; c0 += TP) GP_CHECK(ski_grid_block<D>(p, ps, V + c0, ldv, std::min(TP, t - c0), OUT + c0, ldo));
   return GP_OK;
 }
 
 template <int D>
 static int ski_interp_matmul_d(gp_plan* p, const float* C, int64_t ldc, int t, float* OUT, int64_t ldo) {
   const gp_ski_state* s = p->ski;
-  const SkiGeom g = ski_geom<D>(s);
-  const SkiTiles tl = ski_tiles_of(s, D);
+  SkiPass ps;
+  GP_CHECK(ski_tiled_pass<D>(p, &ps));
   GP_CHECK(opt_in_smem<ski_interp_tiled_kernel<D>>(p->device, SKI_TILE_SMEM));
-  const int parts = ski_tile_parts(p);
-  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
-  const size_t nodes = ski_tile_smem(s, D) / (TP * sizeof(float));
   for (int c0 = 0; c0 < t; c0 += SKI_IP_CW) {
     const int tc = std::min(SKI_IP_CW, t - c0);
     int lg = 0;
     while ((1 << lg) < tc) ++lg;
     const int vec = tc == (1 << lg) && tc >= 4 && ldc % 4 == 0 && (reinterpret_cast<uintptr_t>(C + c0) & 15) == 0;
-    ski_interp_tiled_kernel<D><<<tgrid, SKI_IP_THREADS, nodes * (sizeof(float) << lg), p->stream>>>(
-        s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, C + c0, ldc, tc, lg, vec,
-        OUT + c0, ldo);
+    ski_interp_tiled_kernel<D><<<ps.grid, SKI_IP_THREADS, ps.nodes * (sizeof(float) << lg), p->stream>>>(
+        s->first_s.as<int>(), s->wts_s.as<float>(), s->perm.as<int>(), s->tile_off.as<int>(), ps.g, ps.tl, ps.parts, C + c0, ldc, tc,
+        lg, vec, OUT + c0, ldo);
     p->launches++;
   }
   GP_CUDA(cudaGetLastError());
@@ -1075,24 +1056,14 @@ ski_input_grad_tiled_kernel(const int* __restrict__ first_s, const int* __restri
   const int ppw = 32 >> lp_log2;                          // points per warp and step
   const int pstep = (SKI_IP_THREADS / 32) * ppw;
   for (int64_t wk = blockIdx.x; wk < (int64_t)tl.ntiles * parts; wk += gridDim.x) {
-    const int tile = (int)(wk / parts), part = (int)(wk % parts);
-    const int t0 = off[tile], tn = off[tile + 1] - t0;
-    const int p0 = t0 + (int)((int64_t)tn * part / parts), p1 = t0 + (int)((int64_t)tn * (part + 1) / parts);
-    if (p0 == p1) continue;
+    int tile, p0, p1;
+    if (!ski_work_range(wk, parts, off, tile, p0, p1)) continue;
     const SkiBlock<D> b = ski_block_of<D>(tile, g, tl);
     __syncthreads();
     const int last = b.ext[D - 1];
     const int nrows = b.nodes / last;
     for (int row = warp; row < nrows; row += SKI_IP_THREADS / 32) {
-      int rem = row, node0 = 0;
-      int64_t idx0 = (int64_t)b.base[D - 1] * g.stride[D - 1];
-#pragma unroll
-      for (int i = D - 2; i >= 0; --i) {
-        const int c = rem % b.ext[i];
-        rem /= b.ext[i];
-        node0 += c * b.pitch[i];
-        idx0 += (int64_t)(b.base[i] + c) * g.stride[i];
-      }
+      const auto [node0, idx0] = ski_row_origin<D>(b, g, row);
       for (int e = lane; e < (last << lp_log2); e += 32) {
         const int c = e >> lp_log2, q = e & (lp - 1);
         const int64_t gi = (idx0 + (int64_t)c * g.stride[D - 1]) * TP;
@@ -1151,35 +1122,25 @@ ski_input_grad_tiled_kernel(const int* __restrict__ first_s, const int* __restri
 template <int D>
 static int ski_input_grad_d(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, float* DX, int64_t lddx) {
   gp_ski_state* s = p->ski;
-  cudaStream_t st = p->stream;
-  const SkiGeom g = ski_geom<D>(s);
-  const SkiTiles tl = ski_tiles_of(s, D);
+  SkiPass ps;
+  GP_CHECK(ski_tiled_pass<D>(p, &ps));
   GP_CHECK(opt_in_smem<ski_input_grad_tiled_kernel<D>>(p->device, SKI_TILE_SMEM));
-  const int parts = ski_tile_parts(p);
-  const unsigned tgrid = (unsigned)std::min<int64_t>((int64_t)tl.ntiles * parts, 16 * (int64_t)p->n_sm);
-  const size_t nodes = ski_tile_smem(s, D) / (TP * sizeof(float));
   // B_R / B_L of one 16-column chunk live in the bilinear derivative's grid blocks (allocated by the hyper-parameter backward)
   GP_CHECK(p->V16.ensure(sizeof(float) * p->n1 * TP));
-  GP_CHECK(s->gridC.ensure(sizeof(float) * g.M * TP));
-  GP_CHECK(s->gridD.ensure(sizeof(float) * g.M * TP));
+  GP_CHECK(s->gridC.ensure(sizeof(float) * ps.g.M * TP));
+  GP_CHECK(s->gridD.ensure(sizeof(float) * ps.g.M * TP));
   float* BR = s->gridC.as<float>();
   float* BL = s->gridD.as<float>();
-  const unsigned eg = (unsigned)cdiv(g.M * TP, 256);
   for (int c0 = 0; c0 < t; c0 += TP) {
     const int tc = std::min(TP, t - c0);
-    float* cur = nullptr;
-    GP_CHECK(to_v16(p, R + c0, ldr, tc, p->n1, p->V16.as<float>()));
-    GP_CHECK(ski_grid_apply_d<D>(p, p->V16.as<float>(), &cur));
-    ski_grid_export_kernel<<<eg, 256, 0, st>>>(cur, g.M, TP, p->outputscale, BR, TP);
-    GP_CHECK(to_v16(p, L + c0, ldl, tc, p->n1, p->V16.as<float>()));
-    GP_CHECK(ski_grid_apply_d<D>(p, p->V16.as<float>(), &cur));
-    ski_grid_export_kernel<<<eg, 256, 0, st>>>(cur, g.M, TP, p->outputscale, BL, TP);
+    GP_CHECK(ski_grid_block<D>(p, ps, R + c0, ldr, tc, BR, TP));
+    GP_CHECK(ski_grid_block<D>(p, ps, L + c0, ldl, tc, BL, TP));
     int lg = 1;
     while ((1 << lg) < 2 * tc) ++lg;
-    ski_input_grad_tiled_kernel<D><<<tgrid, SKI_IP_THREADS, nodes * (sizeof(float) << lg), st>>>(
-        s->first_s.as<int>(), s->perm.as<int>(), s->tile_off.as<int>(), g, tl, parts, p->X1, p->ld1, BR, BL, tc, lg, L + c0, ldl,
-        R + c0, ldr, c0 > 0, DX, lddx);
-    p->launches += 3;
+    ski_input_grad_tiled_kernel<D><<<ps.grid, SKI_IP_THREADS, ps.nodes * (sizeof(float) << lg), p->stream>>>(
+        s->first_s.as<int>(), s->perm.as<int>(), s->tile_off.as<int>(), ps.g, ps.tl, ps.parts, p->X1, p->ld1, BR, BL, tc, lg,
+        L + c0, ldl, R + c0, ldr, c0 > 0, DX, lddx);
+    p->launches++;
   }
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -1219,40 +1180,17 @@ extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* g
 
 extern "C" int gp_ski_grid_matmul(gp_plan* p, const float* V, int64_t ldv, int t, float* OUT, int64_t ldo) {
   GP_CHECK(ski_predict_check(p, t, ldv, ldo, "gp_ski_grid_matmul"));
-  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
-  switch (p->d) {
-    case 1: return ski_grid_matmul_d<1>(p, V, ldv, t, OUT, ldo);
-    case 2: return ski_grid_matmul_d<2>(p, V, ldv, t, OUT, ldo);
-    case 3: return ski_grid_matmul_d<3>(p, V, ldv, t, OUT, ldo);
-    case 4: return ski_grid_matmul_d<4>(p, V, ldv, t, OUT, ldo);
-  }
-  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
-  return GP_E_SHAPE;
+  return ski_with_d(p->d, [&](auto D) { return ski_grid_matmul_d<D>(p, V, ldv, t, OUT, ldo); });
 }
 
 extern "C" int gp_ski_input_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, float* DX, int64_t lddx) {
   GP_CHECK(ski_predict_check(p, t, ldl, ldr, "gp_ski_input_grad"));
   GP_REFUSE_LOWRANK(p, "gp_ski_input_grad");
   GP_REQUIRE(L && R && DX && lddx >= p->d, GP_E_SHAPE, "gp_ski_input_grad: bad output (leading dimension %lld, d=%d)", (long long)lddx, p->d);
-  GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
-  switch (p->d) {
-    case 1: return ski_input_grad_d<1>(p, L, ldl, R, ldr, t, DX, lddx);
-    case 2: return ski_input_grad_d<2>(p, L, ldl, R, ldr, t, DX, lddx);
-    case 3: return ski_input_grad_d<3>(p, L, ldl, R, ldr, t, DX, lddx);
-    case 4: return ski_input_grad_d<4>(p, L, ldl, R, ldr, t, DX, lddx);
-  }
-  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
-  return GP_E_SHAPE;
+  return ski_with_d(p->d, [&](auto D) { return ski_input_grad_d<D>(p, L, ldl, R, ldr, t, DX, lddx); });
 }
 
 extern "C" int gp_ski_interp_matmul(gp_plan* p, const float* C, int64_t ldc, int t, float* OUT, int64_t ldo) {
   GP_CHECK(ski_predict_check(p, t, ldc, ldo, "gp_ski_interp_matmul"));
-  switch (p->d) {
-    case 1: return ski_interp_matmul_d<1>(p, C, ldc, t, OUT, ldo);
-    case 2: return ski_interp_matmul_d<2>(p, C, ldc, t, OUT, ldo);
-    case 3: return ski_interp_matmul_d<3>(p, C, ldc, t, OUT, ldo);
-    case 4: return ski_interp_matmul_d<4>(p, C, ldc, t, OUT, ldo);
-  }
-  set_error("SKI backend supports 1 <= d <= 4 (d=%d)", p->d);
-  return GP_E_SHAPE;
+  return ski_with_d(p->d, [&](auto D) { return ski_interp_matmul_d<D>(p, C, ldc, t, OUT, ldo); });
 }
