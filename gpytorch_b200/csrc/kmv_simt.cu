@@ -164,11 +164,13 @@ int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t
 template <int KIND>
 __global__ void krows_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP,
                              const int64_t* __restrict__ idx, int64_t n1_local, int64_t n2, float os, int same,
-                             int64_t row_begin, float* __restrict__ OUT, int64_t ldo) {
+                             int64_t row_begin, float* __restrict__ OUT, int64_t ldo, const int* __restrict__ xbad) {
   extern __shared__ float zi[];
   const int64_t r = blockIdx.y;
   const int64_t i = idx[r];
-  if (i < 0 || i >= n1_local) {   // out-of-range row index (CTA-uniform): NaN row instead of an out-of-bounds read
+  // out-of-range row index (CTA-uniform): NaN row instead of an out-of-bounds read.  Non-finite inputs: every entry is NaN in
+  // the reference (mean-centring spreads it), while cov_from_arg's clamps would turn it into the constant outputscale
+  if (i < 0 || i >= n1_local || *xbad) {
     int64_t jj = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (jj < n2) OUT[r * ldo + jj] = __int_as_float(0x7fc00000);
     return;
@@ -288,13 +290,15 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
   }
 }
 
+// xbad: non-finite inputs make every gradient NaN, as in the reference (the covariance clamps would otherwise treat every pair
+// as distance 0 and return finite sums)
 __global__ void sum_partials_double_kernel(const double* __restrict__ in, int64_t nblk, int stride, int nout,
-                                           double* __restrict__ out) {
+                                           double* __restrict__ out, const int* __restrict__ xbad) {
   int o = blockIdx.x * blockDim.x + threadIdx.x;
   if (o >= nout) return;
   double s = 0.0;
   for (int64_t b = 0; b < nblk; ++b) s += in[b * stride + o];
-  out[o] = s;
+  out[o] = *xbad ? __longlong_as_double(0x7ff8000000000000LL) : s;
 }
 
 // tensor-core path of the bilinear derivative: gout[block][o] = sum_{r,c} L16[r][c] * sum_split partial[split][r][c]
@@ -325,11 +329,8 @@ static int launch_bilinear(gp_plan* p, const float* L16, const float* R16, doubl
     bilinear_kernel<KIND, D, ARD><<<grid, SIMT_TI, 0, p->stream>>>(Z1, Z2, L16, R16, p->row_count, p->n2, cps,     \
                                                                    p->same ? 1 : 0, p->row_begin, p->d, gout, gstride); \
     break;
-  switch (p->DP) {
+  switch (p->DP) {   // DP <= 64: gp_bilinear_grad refuses wider plans before any launch
     GP_BL_CASE(4) GP_BL_CASE(8) GP_BL_CASE(12) GP_BL_CASE(16) GP_BL_CASE(24) GP_BL_CASE(32) GP_BL_CASE(48) GP_BL_CASE(64)
-    default:
-      set_error("bilinear gradient supports d <= 64 (DP=%d)", p->DP);
-      return GP_E_SHAPE;
   }
 #undef GP_BL_CASE
   p->launches++;
@@ -361,10 +362,10 @@ static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int
   dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
   size_t sh = sizeof(float) * p->DP;
   switch (p->kind) {
-    case GP_RBF: krows_kernel<GP_RBF><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo); break;
-    case GP_MATERN12: krows_kernel<GP_MATERN12><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo); break;
-    case GP_MATERN32: krows_kernel<GP_MATERN32><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo); break;
-    default: krows_kernel<GP_MATERN52><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo); break;
+    case GP_RBF: krows_kernel<GP_RBF><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
+    case GP_MATERN12: krows_kernel<GP_MATERN12><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
+    case GP_MATERN32: krows_kernel<GP_MATERN32><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
+    default: krows_kernel<GP_MATERN52><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
   }
   p->launches++;
   GP_CUDA(cudaGetLastError());
@@ -420,6 +421,12 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   GP_REFUSE_LOWRANK(p, "gp_bilinear_grad");
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "gradients of a kernel sum: call gp_bilinear_grad on every term");
   GP_REQUIRE(s >= 1, GP_E_SHAPE, "s must be >= 1");
+  GP_REQUIRE(Lf && Rt, GP_E_SHAPE, "gp_bilinear_grad: null factor");
+  // a single row is read at offset 0 only, so it may carry any row stride
+  GP_REQUIRE((ldl >= s || p->row_count == 1) && (ldr >= s || p->n2 == 1), GP_E_SHAPE,
+             "gp_bilinear_grad: leading dimensions must be >= s (ldl=%lld, ldr=%lld, s=%d)", (long long)ldl, (long long)ldr, s);
+  // before any launch: the SIMT derivative kernel is instantiated up to DP = 64
+  GP_REQUIRE(p->backend == GP_BACKEND_SKI || p->DP <= 64, GP_E_SHAPE, "bilinear gradient supports d <= 64 (d=%d)", p->d);
   const bool ard = p->ls.size() > 1;
   if (p->backend == GP_BACKEND_SKI) {
     // interpolated operator: everything happens on the grid (ski.cu); one sweep per 16 columns
@@ -474,7 +481,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
         p->launches++;
       }
       GP_CUDA(cudaGetLastError());
-      sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, dot_blocks, nout, nout, gsum);
+      sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, dot_blocks, nout, nout, gsum, p->xbad);
       p->launches++;
       std::vector<double> h(nout);
       GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
@@ -494,7 +501,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
     }
 #undef GP_BL_KIND
     GP_CHECK(st);
-    sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, nblk, nout, nout, gsum);
+    sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, nblk, nout, nout, gsum, p->xbad);
     p->launches++;
     std::vector<double> h(nout);
     GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));

@@ -20,6 +20,12 @@ def _ld(t: torch.Tensor) -> int:
     return t.stride(0) if t.size(0) > 1 else t.size(1)
 
 
+def _row_block(t: torch.Tensor) -> torch.Tensor:
+    """t itself when the engine can walk its rows with one leading dimension >= t.size(1) (unit column stride; a single row may
+    carry any row stride), else a contiguous copy, e.g. of an expanded [n, s] block with row stride 0."""
+    return t if t.stride(-1) == 1 and (t.size(0) == 1 or t.stride(0) >= t.size(1)) else t.contiguous()
+
+
 def _require_cuda_f32(t: torch.Tensor, name: str):
     if not t.is_cuda:
         raise RuntimeError(f"{name} must live on a CUDA device: gpytorch_b200 has no CPU path")
@@ -246,13 +252,23 @@ class Plan:
         return out
 
     def bilinear_grad(self, left: torch.Tensor, right: torch.Tensor):
-        """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right))."""
-        left = left.contiguous(); right = right.contiguous()
+        """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right)) for left [row_count, s], right [n2, s]."""
+        if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.row_count or right.size(0) != self.n2 \
+                or left.size(1) != right.size(1) or left.size(1) < 1:
+            raise RuntimeError(f"bilinear_grad: left must be [{self.row_count}, s] and right [{self.n2}, s] with s >= 1 "
+                               f"(got {tuple(left.shape)}, {tuple(right.shape)})")
+        _require_cuda_f32(left, "left")
+        _require_cuda_f32(right, "right")
+        for t, name in ((left, "left"), (right, "right")):
+            if t.device != self.device:
+                raise RuntimeError(f"{name} lives on {t.device}, the plan on {self.device}")
+        left, right = _row_block(left), _row_block(right)
         s = left.size(1)
         nls = len(self.lengthscale)
         gl = (C.c_double * nls)()
         go = C.c_double()
-        check(self.lib.gp_bilinear_grad(self._h, _ptr(left), left.stride(0), _ptr(right), right.stride(0), s, gl, C.byref(go)))
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_bilinear_grad(self._h, _ptr(left), _ld(left), _ptr(right), _ld(right), s, gl, C.byref(go)))
         return [gl[i] for i in range(nls)], go.value
 
     def _grad_outputs(self, dx1: bool, dx2: bool):
