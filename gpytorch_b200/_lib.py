@@ -75,6 +75,9 @@ PROTOTYPES = {
     "gp_plan_set_ski": (_I, [_P, C.POINTER(_I), C.POINTER(_F), C.POINTER(_F), _I]),
     "gp_plan_set_sum": (_I, [_P, C.POINTER(_P), _I]),
     "gp_plan_set_lowrank": (_I, [_P, _P, _L, _I]),
+    "gp_plan_set_tasks": (_I, [_P, _P, _P, _I]),
+    "gp_plan_set_task_covar": (_I, [_P, C.POINTER(_F), _I]),
+    "gp_task_covar_grad": (_I, [_P, _P, _L, _P, _L, _I, C.POINTER(C.c_double)]),
     "gp_ski_grid_matmul": (_I, [_P, _P, _L, _I, _P, _L]),
     "gp_ski_interp_matmul": (_I, [_P, _P, _L, _I, _P, _L]),
     "gp_ski_input_grad": (_I, [_P, _P, _L, _P, _L, _I, _P, _L]),

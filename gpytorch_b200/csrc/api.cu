@@ -108,6 +108,10 @@ extern "C" int gp_plan_destroy(gp_plan* p) {
     for (auto* b : sb) b->release();
     delete p->ski;
   }
+  if (p->tasks) {
+    p->data_set = false;   // release only, no re-pack
+    gp_plan_set_tasks(p, nullptr, nullptr, 0);
+  }
   if (p->pinned) cudaFreeHost(p->pinned);
   delete p;
   return GP_OK;
@@ -128,6 +132,11 @@ extern "C" int gp_plan_set_data(gp_plan* p, const float* X1, int64_t n1, int64_t
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(X1 != nullptr && n1 >= 1 && d >= 1 && ld1 >= d, GP_E_SHAPE, "bad X1 shape n1=%lld d=%d ld1=%lld", (long long)n1, d, (long long)ld1);
   GP_CUDA(cudaSetDevice(p->device));
+  // task indices belong to the rows they were set for: new data drops them (gp_plan_set_tasks again)
+  if (p->tasks) {
+    p->data_set = false;   // no re-pack of the old layout on the way out
+    GP_CHECK(gp_plan_set_tasks(p, nullptr, nullptr, 0));
+  }
   p->X1 = X1; p->n1 = n1; p->ld1 = ld1; p->d = d;
   p->same = (X2 == nullptr) || (X2 == X1 && n2 == n1 && ld2 == ld1);
   if (p->same) { p->X2 = X1; p->n2 = n1; p->ld2 = ld1; }
@@ -190,6 +199,7 @@ extern "C" int gp_kmv(gp_plan* p, const float* V, int64_t ldv, int t, float* OUT
 
 extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  GP_REQUIRE(!(p->tasks && comm && comm->world > 1), GP_E_SHAPE, "task indices are not available on a row-sharded plan");
   p->comm = comm;
   return GP_OK;
 }
@@ -211,8 +221,10 @@ extern "C" int gp_time_kmv_kernel(gp_plan* p, const float* V, int64_t ldv, int t
   GP_CUDA(cudaSetDevice(p->device));
   GP_CHECK(p->V16.ensure(sizeof(float) * p->n2 * TP));
   GP_CHECK(to_v16(p, V, ldv, t, p->n2, p->V16.as<float>()));
-  if (p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_any_tc)) GP_CHECK(pack_v_tiles(p, p->V16.as<float>()));
+  if (!p->tasks && (p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_any_tc))) GP_CHECK(pack_v_tiles(p, p->V16.as<float>()));
   auto launch = [&]() -> int {
+    // a multitask plan: the whole product (gather, V tiles, one launch per column task, combine)
+    if (p->tasks) return tasks_kmv_partials(p, p->V16.as<float>(), p->kind, nullptr);
     if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, p->V16.as<float>(), nullptr);
     return p->backend == GP_BACKEND_TCGEN05 ? kmv_tc_launch(p, nullptr) : kmv_simt_launch(p, p->V16.as<float>(), nullptr);

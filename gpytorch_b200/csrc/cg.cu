@@ -603,7 +603,7 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   // the direction block is written straight into the packed K.V tiles when this rank owns all rows and the tensor-core
   // kernel runs; sharded runs all-gather the fp32 rows first and pack the gathered block (pack.cu)
   const bool tc = plan_is_tc(p);
-  const bool fuse_pack = tc && !sharded;
+  const bool fuse_pack = tc && !sharded && !p->tasks;   // a multitask product packs its own task-ordered tiles (tasks.cu)
   float* Vt = fuse_pack ? p->Vtiles.as<float>() : nullptr;
   const int64_t nchunk_pack = fuse_pack ? p->ntile_j * (TILE_J / 4) : 0;
   const int Gd = (int)std::min<int64_t>(cdiv(std::max<int64_t>(nchunk_pack, cdiv(n, (int64_t)4)) * 4, (int64_t)RP_THREADS), 4 * p->n_sm);

@@ -24,6 +24,8 @@ constexpr int TILE_J = 64;     // columns of K per pipeline step (wgmma N of GEM
 constexpr int KP_MAX = 128;    // max padded augmented feature width of the tensor-core path (3d+4 <= 128)
 constexpr int SIMT_TI = 128;   // rows per CTA in the SIMT kernel
 constexpr int SIMT_TJ = 64;    // staged columns per step in the SIMT kernel
+// one packed 64-row tile of V (pack.cu): [64/4][32][4] tf32 (V_hi | V_lo) + [64/8][16][8] bf16
+constexpr int V_TILE_FLOATS = (2 * TILE_J * TP * 4 + TILE_J * TP * 2) / 4;   // 2560
 constexpr float LOG2E = 1.4426950408889634f;
 
 // ---- error plumbing -----------------------------------------------------------------------
@@ -139,6 +141,35 @@ struct gp_ski_state {
   gp::DevBuf perm, tile_off, tile_cnt, first_s, wts_s;                        // points sorted by tile + the permutation back
 };
 
+// Hadamard multitask state (tasks.cu): the operator is s K o B[t, t'].  Rows are sorted by task (stable), the columns of task b
+// form one segment of the packed column layout (on the tensor-core path every segment starts at a 64-column tile), and one K.V
+// is one launch of the plain fused kernel per column task into its own partial slots, combined with B row by row.
+struct gp_task_state {
+  int T = 0;
+  std::vector<int> t1, t2;                 // host copies of the task ids (user order)
+  std::vector<int64_t> off1, off2;         // [T + 1] start of every task in the sorted row / column order
+  std::vector<int> perm1, perm2;           // sorted position -> user index
+  // column layout of the packed inputs (backend dependent, tasks_pack): segment b = positions [seg[b], seg[b] + cnt_b)
+  std::vector<int64_t> seg;                // [T + 1]
+  int64_t ncol_layout = 0;
+  std::vector<int64_t> tps;                // per column task: tiles (tensor cores) / columns (SIMT) per split
+  std::vector<int> nsplit, slot0;          // per column task: splits and first partial slot (slot0[T] = all slots)
+  bool lay_ok = false, lay_tc = false;     // the column layout above is current for this backend
+  std::vector<float> B;                    // host T x T task covariance, row-major
+  bool b_set = false;
+  gp::DevBuf ids;                          // perm1 [n1] | ts1 [n1] (sorted row tasks) | t1 [n1] | t2 [n2] (user order)
+  gp::DevBuf lay;                          // map2 [ncol_layout] (layout position -> user column, -1 = padding) | slot_task | slot0
+  gp::DevBuf Bd;                           // B on the device
+  gp::DevBuf Zs1, Zs2, Vs, Ls, tpart, red;
+  int* d_perm1 = nullptr;
+  int* d_ts1 = nullptr;
+  int* d_t1 = nullptr;
+  int* d_t2 = nullptr;
+  int* d_map2 = nullptr;
+  int* d_slot_task = nullptr;
+  int* d_slot0 = nullptr;
+};
+
 struct gp_comm {
   void* nccl_comm = nullptr;
   int rank = 0, world = 1;
@@ -194,6 +225,7 @@ struct gp_plan {
   int64_t lr_n = 0;               // rows of U: the operator size when the correction was set (re-checked at every use)
   int lr_r = 0;
   gp::DevBuf lrw;                 // U^T V partials [G][16 r] | c = U^T V [r][16] fp64
+  gp_task_state* tasks = nullptr; // non-null: Hadamard multitask operator s K o B[t, t'] (gp_plan_set_tasks)
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
 
@@ -219,6 +251,24 @@ int lowrank_partials(gp_plan* p, const float* V16, const int* done_flag);   // l
 int lowrank_kdiag(gp_plan* p, float* OUT);                              // OUT[i] -= sum_j U_ij^2
 int lowrank_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);   // OUT[r] -= U[idx_r] U^T
 int sum_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);       // rows of a kernel sum (terms added in order)
+// one launch of the fused kernels over an explicit column block (Hadamard plans): columns [0, ntile_j) tiles of XB / Vt (tensor
+// cores) or [0, n2) rows of Z2 / V16 (SIMT), partial slots from `partial`, diag_row_begin = row_begin of the exact-diagonal test
+int kmv_tc_launch_cols(gp_plan* p, int kind, const float* XA, const float* XB, const float* Vt, float* partial, int64_t ntile_j,
+                       int64_t tiles_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag);
+int kmv_simt_launch_cols(gp_plan* p, int kind, const float* Z1, const float* Z2, const float* V16, float* partial, int64_t n2,
+                         int64_t cols_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag);
+int64_t bilinear_blocks(const gp_plan* p, int64_t n2);                      // CTAs of one SIMT derivative launch over n2 columns
+int bilinear_launch_cols(gp_plan* p, bool ard, const float* Z1, const float* Z2, const float* L16, const float* R16, int64_t n2,
+                         int64_t diag_row_begin, double* gout, int gstride, int64_t* nblk_out);
+int pack_v_tiles_rows(gp_plan* p, const float* V16, int64_t nrows, int64_t ntiles, float* Vt);
+int pack_tc_rows(gp_plan* p, const float* Z, int64_t nvalid, int64_t npad, bool is_a, float* out);
+int tasks_pack(gp_plan* p);                                                  // tasks.cu
+int tasks_kmv_partials(gp_plan* p, const float* V16, int kind, const int* done_flag);   // K o B V into partial slot 0
+int tasks_kdiag_scale(gp_plan* p, float* OUT);                               // OUT[i] *= B[t1_i, t2_i]
+int tasks_krows_scale(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
+int tasks_bilinear(gp_plan* p, const float* L16, const float* R16, bool ard, std::vector<double>& total);
+#define GP_REFUSE_TASKS(p, what) \
+  GP_REQUIRE((p)->tasks == nullptr, GP_E_STATE, "%s is not available on a plan with task indices (gp_plan_set_tasks)", what)
 int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,   // cg.cu
              int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
              int* tridiag_size, float* resid_out);

@@ -68,18 +68,24 @@ kmv_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
   }
 }
 
+struct SimtLaunch {
+  const float* Z1;
+  const float* Z2;
+  const float* V16;
+  float* partial;
+  int64_t n2, cps, row_begin;
+  int nsplit;
+};
+
 template <int KIND>
-static int launch_simt_kind(gp_plan* p, const float* V16, const int* done_flag) {
-  const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
-  const float* Z2 = p->Z2.as<float>();
+static int launch_simt_kind(gp_plan* p, const SimtLaunch& a, const int* done_flag) {
   int64_t rows_pad = p->rows_pad;
-  dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)p->nsplit);
-  int64_t cps = p->tiles_per_split * SIMT_TJ;
+  dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)a.nsplit);
 #define GP_SIMT_CASE(D)                                                                                          \
   case D:                                                                                                        \
-    kmv_simt_kernel<KIND, D><<<grid, SIMT_TI, 0, p->stream>>>(Z1, Z2, V16, partial_ptr(p), p->row_count, \
-                                                              p->n2, rows_pad, cps, p->same ? 1 : 0,             \
-                                                              p->row_begin, done_flag);                          \
+    kmv_simt_kernel<KIND, D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count,        \
+                                                              a.n2, rows_pad, a.cps, p->same ? 1 : 0,            \
+                                                              a.row_begin, done_flag);                           \
     break;
   switch (p->DP) {
     GP_SIMT_CASE(4) GP_SIMT_CASE(8) GP_SIMT_CASE(12) GP_SIMT_CASE(16) GP_SIMT_CASE(24) GP_SIMT_CASE(32)
@@ -94,18 +100,31 @@ static int launch_simt_kind(gp_plan* p, const float* V16, const int* done_flag) 
   return GP_OK;
 }
 
-int kmv_simt_launch(gp_plan* p, const float* V16, const int* done_flag) {
-  switch (p->kind) {
-    case GP_RBF: return launch_simt_kind<GP_RBF>(p, V16, done_flag);
-    case GP_MATERN12: return launch_simt_kind<GP_MATERN12>(p, V16, done_flag);
-    case GP_MATERN32: return launch_simt_kind<GP_MATERN32>(p, V16, done_flag);
-    case GP_MATERN52: return launch_simt_kind<GP_MATERN52>(p, V16, done_flag);
+static int launch_simt_any(gp_plan* p, int kind, const SimtLaunch& a, const int* done_flag) {
+  switch (kind) {
+    case GP_RBF: return launch_simt_kind<GP_RBF>(p, a, done_flag);
+    case GP_MATERN12: return launch_simt_kind<GP_MATERN12>(p, a, done_flag);
+    case GP_MATERN32: return launch_simt_kind<GP_MATERN32>(p, a, done_flag);
+    case GP_MATERN52: return launch_simt_kind<GP_MATERN52>(p, a, done_flag);
   }
-  set_error("bad kernel kind %d", p->kind);
+  set_error("bad kernel kind %d", kind);
   return GP_E_SHAPE;
 }
 
+int kmv_simt_launch(gp_plan* p, const float* V16, const int* done_flag) {
+  const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
+  const SimtLaunch a{Z1, p->Z2.as<float>(), V16, partial_ptr(p), p->n2, p->tiles_per_split * SIMT_TJ, p->row_begin, p->nsplit};
+  return launch_simt_any(p, p->kind, a, done_flag);
+}
+
+int kmv_simt_launch_cols(gp_plan* p, int kind, const float* Z1, const float* Z2, const float* V16, float* partial, int64_t n2,
+                         int64_t cols_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag) {
+  const SimtLaunch a{Z1, Z2, V16, partial, n2, cols_per_split, diag_row_begin, nsplit};
+  return launch_simt_any(p, kind, a, done_flag);
+}
+
 static int kmv_partials_base(gp_plan* p, const float* V16, const int* done_flag) {
+  if (p->tasks) return tasks_kmv_partials(p, V16, p->kind, done_flag);
   if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, V16, done_flag);
   if (p->backend == GP_BACKEND_SUM) {
     if (p->sum_any_tc) GP_CHECK(pack_v_tiles(p, V16));
@@ -320,14 +339,19 @@ __global__ void bilin_dot_kernel(const float* __restrict__ partial, int nsplit, 
   if (threadIdx.x == 0) gout[(int64_t)blockIdx.x * gstride + o] = red[0];
 }
 
+struct BilinLaunch {
+  const float* Z1;
+  const float* Z2;
+  int64_t n2, row_begin;
+};
+
 template <int KIND, bool ARD>
-static int launch_bilinear(gp_plan* p, const float* L16, const float* R16, double* gout, int gstride, dim3 grid, int64_t cps) {
-  const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
-  const float* Z2 = p->Z2.as<float>();
+static int launch_bilinear(gp_plan* p, const BilinLaunch& a, const float* L16, const float* R16, double* gout, int gstride, dim3 grid,
+                           int64_t cps) {
 #define GP_BL_CASE(D)                                                                                              \
   case D:                                                                                                          \
-    bilinear_kernel<KIND, D, ARD><<<grid, SIMT_TI, 0, p->stream>>>(Z1, Z2, L16, R16, p->row_count, p->n2, cps,     \
-                                                                   p->same ? 1 : 0, p->row_begin, p->d, gout, gstride); \
+    bilinear_kernel<KIND, D, ARD><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, L16, R16, p->row_count, a.n2, cps,  \
+                                                                   p->same ? 1 : 0, a.row_begin, p->d, gout, gstride); \
     break;
   switch (p->DP) {   // DP <= 64: gp_bilinear_grad refuses wider plans before any launch
     GP_BL_CASE(4) GP_BL_CASE(8) GP_BL_CASE(12) GP_BL_CASE(16) GP_BL_CASE(24) GP_BL_CASE(32) GP_BL_CASE(48) GP_BL_CASE(64)
@@ -336,6 +360,44 @@ static int launch_bilinear(gp_plan* p, const float* L16, const float* R16, doubl
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
+}
+
+// the SIMT derivative launch split of gp_bilinear_grad over n2 columns
+static void bilinear_split(const gp_plan* p, int64_t n2, dim3* grid, int64_t* cps) {
+  int64_t ntj = cdiv(n2, SIMT_TJ);
+  int nsp = (int)std::min<int64_t>(ntj, std::max<int64_t>(1, (2 * p->n_sm) / std::max<int64_t>(1, cdiv(p->row_count, SIMT_TI))));
+  *cps = cdiv(ntj, nsp) * SIMT_TJ;
+  nsp = (int)cdiv(n2, *cps);
+  *grid = dim3((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)nsp);
+}
+
+template <bool ARD>
+static int launch_bilinear_any(gp_plan* p, const BilinLaunch& a, const float* L16, const float* R16, double* gout, int gstride,
+                               dim3 grid, int64_t cps) {
+  switch (p->kind) {
+    case GP_RBF: return launch_bilinear<GP_RBF, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
+    case GP_MATERN12: return launch_bilinear<GP_MATERN12, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
+    case GP_MATERN32: return launch_bilinear<GP_MATERN32, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
+    default: return launch_bilinear<GP_MATERN52, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
+  }
+}
+
+int64_t bilinear_blocks(const gp_plan* p, int64_t n2) {
+  dim3 grid;
+  int64_t cps;
+  bilinear_split(p, n2, &grid, &cps);
+  return (int64_t)grid.x * grid.y;
+}
+
+int bilinear_launch_cols(gp_plan* p, bool ard, const float* Z1, const float* Z2, const float* L16, const float* R16, int64_t n2,
+                         int64_t diag_row_begin, double* gout, int gstride, int64_t* nblk_out) {
+  dim3 grid;
+  int64_t cps;
+  bilinear_split(p, n2, &grid, &cps);
+  *nblk_out = (int64_t)grid.x * grid.y;
+  const BilinLaunch a{Z1, Z2, n2, diag_row_begin};
+  return ard ? launch_bilinear_any<true>(p, a, L16, R16, gout, gstride, grid, cps)
+             : launch_bilinear_any<false>(p, a, L16, R16, gout, gstride, grid, cps);
 }
 
 }  // namespace gp
@@ -353,7 +415,8 @@ extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, i
     GP_CHECK(p->backend == GP_BACKEND_SUM ? sum_krows(p, idx, m, OUT, ldo) : krows_base(p, idx, m, OUT, ldo));
     return lowrank_krows(p, idx, m, OUT, ldo);
   }
-  return krows_base(p, idx, m, OUT, ldo);
+  GP_CHECK(krows_base(p, idx, m, OUT, ldo));
+  return p->tasks ? tasks_krows_scale(p, idx, m, OUT, ldo) : GP_OK;
 }
 
 static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
@@ -389,7 +452,8 @@ extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
     }
     return lowrank_kdiag(p, OUT);
   }
-  return kdiag_base(p, OUT);
+  GP_CHECK(kdiag_base(p, OUT));
+  return p->tasks ? tasks_kdiag_scale(p, OUT) : GP_OK;
 }
 
 static int kdiag_base(gp_plan* p, float* OUT) {
@@ -451,62 +515,65 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   }
   const int nout = 1 + (ard ? p->d : 1);
   std::vector<double> total(nout, 0.0);
-  int64_t ntj = cdiv(p->n2, SIMT_TJ);
-  int nsp = (int)std::min<int64_t>(ntj, std::max<int64_t>(1, (2 * p->n_sm) / std::max<int64_t>(1, cdiv(p->row_count, SIMT_TI))));
-  int64_t cps = cdiv(ntj, nsp) * SIMT_TJ;
-  nsp = (int)cdiv(p->n2, cps);
-  dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)nsp);
-  int64_t nblk = (int64_t)grid.x * grid.y;
-  GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-  double* gout = p->misc.as<double>();
-  double* gsum = gout + nblk * nout;
-  // scalar lengthscale on the tensor-core backend: sum_ij (L_i . R_j) f_ij = sum_i L_i . (F R)_i, i.e. two launches of
-  // the fused K.V kernel (f = k, then f = g = l dk/dl through the derivative kinds) + a dot product with L.  ARD needs d
-  // weighted sums per pair and stays on the SIMT kernel.
-  const bool use_tc = !ard && p->backend == GP_BACKEND_TCGEN05;
-  const int64_t rows_pad = p->rows_pad;
-  const int dot_blocks = (int)std::min<int64_t>(nblk, 2 * p->n_sm);
-  for (int c0 = 0; c0 < s; c0 += TP) {
-    int tc = std::min(TP, s - c0);
-    GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-    if (use_tc) {
-      GP_CHECK(pack_v_tiles(p, p->misc3.as<float>()));
-      for (int pass = 0; pass < 2; ++pass) {
-        GP_CHECK(kmv_tc_launch_kind(p, pass == 0 ? p->kind : GP_DERIV + p->kind, nullptr));
-        bilin_dot_kernel<<<dot_blocks, 256, 0, p->stream>>>(p->partial.as<float>(), p->nparts, p->row_count, rows_pad,
-                                                            p->misc2.as<float>(), gout, nout, pass);
+  if (p->tasks && (ard || p->backend != GP_BACKEND_TCGEN05)) {
+    // K o B on the SIMT derivative kernel: one pass per column task with B folded into the rows (tasks.cu)
+    GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
+    GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
+    for (int c0 = 0; c0 < s; c0 += TP) {
+      const int tc = std::min(TP, s - c0);
+      GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
+      GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
+      GP_CHECK(tasks_bilinear(p, p->misc2.as<float>(), p->misc3.as<float>(), ard, total));
+    }
+  } else {
+    dim3 grid;
+    int64_t cps;
+    bilinear_split(p, p->n2, &grid, &cps);
+    int64_t nblk = (int64_t)grid.x * grid.y;
+    GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
+    GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
+    GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
+    double* gout = p->misc.as<double>();
+    double* gsum = gout + nblk * nout;
+    // scalar lengthscale on the tensor-core backend: sum_ij (L_i . R_j) f_ij = sum_i L_i . (F R)_i, i.e. two launches of
+    // the fused K.V kernel (f = k, then f = g = l dk/dl through the derivative kinds) + a dot product with L.  ARD needs d
+    // weighted sums per pair and stays on the SIMT kernel.
+    const bool use_tc = !ard && p->backend == GP_BACKEND_TCGEN05;
+    const int64_t rows_pad = p->rows_pad;
+    const int dot_blocks = (int)std::min<int64_t>(nblk, 2 * p->n_sm);
+    for (int c0 = 0; c0 < s; c0 += TP) {
+      int tc = std::min(TP, s - c0);
+      GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
+      GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
+      if (use_tc) {
+        if (!p->tasks) GP_CHECK(pack_v_tiles(p, p->misc3.as<float>()));
+        for (int pass = 0; pass < 2; ++pass) {
+          const int kind = pass == 0 ? p->kind : GP_DERIV + p->kind;
+          // a multitask plan runs both passes on K o B (tasks.cu), combined into slot 0 in user row order
+          GP_CHECK(p->tasks ? tasks_kmv_partials(p, p->misc3.as<float>(), kind, nullptr) : kmv_tc_launch_kind(p, kind, nullptr));
+          bilin_dot_kernel<<<dot_blocks, 256, 0, p->stream>>>(p->partial.as<float>(), p->nparts, p->row_count, rows_pad,
+                                                              p->misc2.as<float>(), gout, nout, pass);
+          p->launches++;
+        }
+        GP_CUDA(cudaGetLastError());
+        sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, dot_blocks, nout, nout, gsum, p->xbad);
         p->launches++;
+        std::vector<double> h(nout);
+        GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
+        GP_CUDA(cudaStreamSynchronize(p->stream));
+        for (int o = 0; o < nout; ++o) total[o] += h[o];
+        continue;
       }
-      GP_CUDA(cudaGetLastError());
-      sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, dot_blocks, nout, nout, gsum, p->xbad);
+      const BilinLaunch a{p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>(), p->Z2.as<float>(), p->n2, p->row_begin};
+      GP_CHECK(ard ? launch_bilinear_any<true>(p, a, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout, grid, cps)
+                   : launch_bilinear_any<false>(p, a, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout, grid, cps));
+      sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, nblk, nout, nout, gsum, p->xbad);
       p->launches++;
       std::vector<double> h(nout);
       GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
       GP_CUDA(cudaStreamSynchronize(p->stream));
       for (int o = 0; o < nout; ++o) total[o] += h[o];
-      continue;
     }
-    int st;
-#define GP_BL_KIND(KK)                                                                                         \
-  st = ard ? launch_bilinear<KK, true>(p, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout, grid, cps)   \
-           : launch_bilinear<KK, false>(p, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout, grid, cps);
-    switch (p->kind) {
-      case GP_RBF: GP_BL_KIND(GP_RBF) break;
-      case GP_MATERN12: GP_BL_KIND(GP_MATERN12) break;
-      case GP_MATERN32: GP_BL_KIND(GP_MATERN32) break;
-      default: GP_BL_KIND(GP_MATERN52) break;
-    }
-#undef GP_BL_KIND
-    GP_CHECK(st);
-    sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, nblk, nout, nout, gsum, p->xbad);
-    p->launches++;
-    std::vector<double> h(nout);
-    GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-    GP_CUDA(cudaStreamSynchronize(p->stream));
-    for (int o = 0; o < nout; ++o) total[o] += h[o];
   }
   // d/d outputscale of os*k = k ; d/dl: scalar -> sum w g / l ; ARD -> sum w g dz_c^2/s / l_c ; both times os
   *grad_os = total[0];

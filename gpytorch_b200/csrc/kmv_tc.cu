@@ -43,7 +43,8 @@ using namespace ptx;
 
 constexpr int TC_THREADS = 384;                     // producer warpgroup + 2 consumer warpgroups
 constexpr int V_TF32_BYTES = 2 * TILE_J * TP * 4;   // [64/4][32 rows: V_hi(16) | V_lo(16)][4 tf32] = 8192
-constexpr int V_TILE_BYTES = V_TF32_BYTES + TILE_J * TP * 2;   // pitch of the packed V tiles in HBM (pack.cu)
+constexpr int V_TILE_BYTES = V_TILE_FLOATS * 4;                 // pitch of the packed V tiles in HBM (pack.cu)
+static_assert(V_TILE_BYTES == V_TF32_BYTES + TILE_J * TP * 2, "packed V tile layout");
 constexpr int MAX_NS = 12;
 constexpr uint32_t TURN_BAR0 = 1;                   // named barriers 1, 2: consumer 0's / 1's turn on the tensor core
 
@@ -269,34 +270,54 @@ static int tc_smem_bytes(int KP, int* ns_out) {
   return a_bytes + ns * stage + (int)sizeof(TcBars);
 }
 
+struct TcLaunch {
+  const float* XA;
+  const float* XB;
+  const float* Vt;
+  float* partial;
+  int64_t ntile_j, tiles_per_split, row_begin;
+  int nsplit;
+};
+
 template <int KIND>
-static int launch_tc_kind(gp_plan* p, const int* done_flag) {
+static int launch_tc_kind(gp_plan* p, const TcLaunch& a, const int* done_flag) {
   int ns = 0;
   int smem_bytes = tc_smem_bytes(p->KP, &ns);
   GP_REQUIRE(ns >= 2, GP_E_SHAPE, "tensor-core path: smem ring too small for KP=%d", p->KP);
   GP_CHECK(opt_in_smem<kmv_tc_kernel<KIND>>(p->device, 227 * 1024));
-  dim3 grid((unsigned)p->ntile_i, (unsigned)p->nsplit);
+  dim3 grid((unsigned)p->ntile_i, (unsigned)a.nsplit);
   kmv_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
-      p->XA.as<float>(), p->XB.as<float>(), vtiles_ptr(p), partial_ptr(p), p->KP, ns, p->ntile_j,
-      p->tiles_per_split, p->rows_pad, p->same ? 1 : 0, p->row_begin, done_flag);
+      a.XA, a.XB, a.Vt, a.partial, p->KP, ns, a.ntile_j, a.tiles_per_split, p->rows_pad, p->same ? 1 : 0, a.row_begin, done_flag);
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
 
-int kmv_tc_launch_kind(gp_plan* p, int kind, const int* done_flag) {
+static int launch_tc_any(gp_plan* p, int kind, const TcLaunch& a, const int* done_flag) {
   switch (kind) {
-    case GP_RBF: return launch_tc_kind<GP_RBF>(p, done_flag);
-    case GP_MATERN12: return launch_tc_kind<GP_MATERN12>(p, done_flag);
-    case GP_MATERN32: return launch_tc_kind<GP_MATERN32>(p, done_flag);
-    case GP_MATERN52: return launch_tc_kind<GP_MATERN52>(p, done_flag);
-    case GP_DERIV + GP_RBF: return launch_tc_kind<GP_DERIV + GP_RBF>(p, done_flag);
-    case GP_DERIV + GP_MATERN12: return launch_tc_kind<GP_DERIV + GP_MATERN12>(p, done_flag);
-    case GP_DERIV + GP_MATERN32: return launch_tc_kind<GP_DERIV + GP_MATERN32>(p, done_flag);
-    case GP_DERIV + GP_MATERN52: return launch_tc_kind<GP_DERIV + GP_MATERN52>(p, done_flag);
+    case GP_RBF: return launch_tc_kind<GP_RBF>(p, a, done_flag);
+    case GP_MATERN12: return launch_tc_kind<GP_MATERN12>(p, a, done_flag);
+    case GP_MATERN32: return launch_tc_kind<GP_MATERN32>(p, a, done_flag);
+    case GP_MATERN52: return launch_tc_kind<GP_MATERN52>(p, a, done_flag);
+    case GP_DERIV + GP_RBF: return launch_tc_kind<GP_DERIV + GP_RBF>(p, a, done_flag);
+    case GP_DERIV + GP_MATERN12: return launch_tc_kind<GP_DERIV + GP_MATERN12>(p, a, done_flag);
+    case GP_DERIV + GP_MATERN32: return launch_tc_kind<GP_DERIV + GP_MATERN32>(p, a, done_flag);
+    case GP_DERIV + GP_MATERN52: return launch_tc_kind<GP_DERIV + GP_MATERN52>(p, a, done_flag);
   }
   set_error("bad kernel kind %d", kind);
   return GP_E_SHAPE;
+}
+
+int kmv_tc_launch_kind(gp_plan* p, int kind, const int* done_flag) {
+  const TcLaunch a{p->XA.as<float>(), p->XB.as<float>(), vtiles_ptr(p), partial_ptr(p), p->ntile_j, p->tiles_per_split,
+                   p->row_begin, p->nsplit};
+  return launch_tc_any(p, kind, a, done_flag);
+}
+
+int kmv_tc_launch_cols(gp_plan* p, int kind, const float* XA, const float* XB, const float* Vt, float* partial, int64_t ntile_j,
+                       int64_t tiles_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag) {
+  const TcLaunch a{XA, XB, Vt, partial, ntile_j, tiles_per_split, diag_row_begin, nsplit};
+  return launch_tc_any(p, kind, a, done_flag);
 }
 int kmv_tc_launch(gp_plan* p, const int* done_flag) {
   if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, nullptr, done_flag);   // all terms on tensor cores (plan_is_tc)

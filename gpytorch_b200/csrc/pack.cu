@@ -105,7 +105,6 @@ __global__ void to_v16_kernel(const float* __restrict__ V, int64_t ldv, int t, i
 // thread per (4-row chunk, column): V16 [n2][16] -> Vt tiles.  Per 64-row tile (10240 B):
 //   [0, 8192)      tf32 tile  [64/4][32 rows][4]: rows 0-15 = hi, rows 16-31 = lo of the 16 columns
 //   [8192, 10240)  bf16 tile  [64/8][16 rows][8]: bf16(v), the B operand of the P_lo pass
-constexpr int V_TILE_FLOATS = (2 * TILE_J * TP * 4 + TILE_J * TP * 2) / 4;  // 2560
 __global__ void pack_v_tiles_kernel(const float* __restrict__ V16, int64_t n2, int64_t ntile_j, float* __restrict__ Vt) {
   int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   int64_t nchunk = ntile_j * (TILE_J / 4);
@@ -216,7 +215,9 @@ int pack_inputs(gp_plan* p) {
                                                               p->mean.as<float>(), p->scale.as<float>(), p->Z1.as<float>(), p->xbad);
     p->launches++;
   }
-  if (p->backend == GP_BACKEND_TCGEN05) {
+  if (p->tasks) {
+    GP_CHECK(tasks_pack(p));   // task-sorted packing and the per-task column segments (tasks.cu)
+  } else if (p->backend == GP_BACKEND_TCGEN05) {
     const int KP = p->KP;
     int64_t padA = p->rows_pad, padB = p->ntile_j * TILE_J;
     GP_CHECK(p->XA.ensure(sizeof(float) * padA * KP));
@@ -228,7 +229,7 @@ int pack_inputs(gp_plan* p) {
     p->launches += 2;
     GP_CHECK(p->Vtiles.ensure(sizeof(float) * p->ntile_j * (2 * TILE_J * TP + TILE_J * TP / 2)));
   }
-  p->nparts = p->nsplit;
+  p->nparts = p->tasks ? 1 : p->nsplit;   // a Hadamard product is combined into one slot in user row order
   GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)nslots(p) * p->rows_pad * TP));
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -242,9 +243,22 @@ int to_v16(gp_plan* p, const float* V, int64_t ldv, int t, int64_t n, float* V16
   return GP_OK;
 }
 
+// tensor-core operand tiles of rows [0, npad) of Z (rows >= nvalid zero): the A side (XA layout) or the B side (XB layout)
+int pack_tc_rows(gp_plan* p, const float* Z, int64_t nvalid, int64_t npad, bool is_a, float* out) {
+  if (is_a) pack_tc_kernel<true><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, p->d, p->DP, p->KP, TILE_I, out);
+  else pack_tc_kernel<false><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, p->d, p->DP, p->KP, TILE_J, out);
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
 int pack_v_tiles(gp_plan* p, const float* V16) {
-  int64_t tot = p->ntile_j * (TILE_J / 4) * TP;
-  pack_v_tiles_kernel<<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(V16, p->n2, p->ntile_j, p->Vtiles.as<float>());
+  return pack_v_tiles_rows(p, V16, p->n2, p->ntile_j, p->Vtiles.as<float>());
+}
+
+int pack_v_tiles_rows(gp_plan* p, const float* V16, int64_t nrows, int64_t ntiles, float* Vt) {
+  int64_t tot = ntiles * (TILE_J / 4) * TP;
+  pack_v_tiles_kernel<<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(V16, nrows, ntiles, Vt);
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;

@@ -189,11 +189,16 @@ constexpr int PC_KIND_SUM = 64;
 // SKI (GP_BACKEND_SKI): K[pivot, j] = s prod_k w_jk^T u_k[f_jk : f_jk + 4] with u of the pivot staged where the pivot row of Z sits
 // (ski_rows.cuh); DP = sum_k G_k
 constexpr int PC_KIND_SKI = 65;
+// Hadamard multitask (tasks.cu): K[pivot, j] = s B[t_pivot, t_j] k(|z_pivot - z_j|^2), covariance kind kind[0]
+constexpr int PC_KIND_TASK = 66;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
   float os[4];
   const float* Z[4];
+  const int* task;   // PC_KIND_TASK: task ids (user order) and B [T][T]
+  const float* B;
+  int T;
 };
 __device__ __forceinline__ float pc_cov_rt(int kind, float a) {
   switch (kind) {
@@ -284,6 +289,13 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
           }
         } else if (KIND == PC_KIND_SKI) {
           v = ski_entry(sk, zp, j);
+        } else if (KIND == PC_KIND_TASK) {
+          float s = 0.f;
+          for (int c = 0; c < DP; ++c) {
+            float df = zp[c] - Z[j * DP + c];
+            s = fmaf(df, df, s);
+          }
+          v = os * tt.B[tt.task[pi] * tt.T + tt.task[j]] * pc_cov_rt(tt.kind[0], -0.5f * s);
         } else {
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
@@ -402,6 +414,16 @@ __global__ void pc_init_ski_kernel(const SkiRows sk, float* __restrict__ diag, i
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   diag[j] = ski_diag_entry(sk, j);
+  perm[j] = (int)j;
+  pos[j] = (int)j;
+}
+
+// Hadamard multitask: diag[j] = s B[t_j, t_j] (not constant across tasks), identity permutation; then pc_first_pivot_kernel
+__global__ void pc_init_task_kernel(const int* __restrict__ task, const float* __restrict__ B, int T, float os, float* __restrict__ diag,
+                                    int* __restrict__ perm, int* __restrict__ pos, int64_t n) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  diag[j] = os * B[task[j] * T + task[j]];
   perm[j] = (int)j;
   pos[j] = (int)j;
 }
@@ -765,7 +787,14 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       dp_total += q->DP;
     }
   }
-  if (ski) {
+  const bool tasks = p->tasks != nullptr;
+  if (tasks) {
+    GP_REQUIRE(p->tasks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
+    tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T;
+    pc_init_task_kernel<<<gb, PC_THREADS, 0, st>>>(tt.task, tt.B, tt.T, p->outputscale, diag, perm, pos, n);
+    pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
+    p->launches += 2;
+  } else if (ski) {
     GP_CHECK(ski_rows_args(p, &sk));
     dp_total = sk.usum;   // the pivot's u_k take the place of its packed inputs in shared memory
     pc_init_ski_kernel<<<gb, PC_THREADS, 0, st>>>(sk, diag, perm, pos, n);
@@ -781,10 +810,12 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, p->device);
   GP_REQUIRE(!sum || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a kernel sum needs the cooperative kernel");
   GP_REQUIRE(!ski || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a SKI operator needs the cooperative kernel");
+  GP_REQUIRE(!tasks || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a multitask operator needs the cooperative kernel");
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : ski ? PC_KIND_SKI : p->kind) {
+    switch (sum ? PC_KIND_SUM : ski ? PC_KIND_SKI : tasks ? PC_KIND_TASK : p->kind) {
+      case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
       case GP_MATERN12: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN12>; break;
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
@@ -956,6 +987,11 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
     tr_k = (double)n * os_total;
   } else if (p->backend == GP_BACKEND_SKI) {
     GP_CHECK(ski_diag_sum(p, &tr_k));
+  } else if (p->tasks) {   // s sum_i B[t_i, t_i]
+    const gp_task_state* ts = p->tasks;
+    double bt = 0.0;
+    for (int a = 0; a < ts->T; ++a) bt += (double)(ts->off1[a + 1] - ts->off1[a]) * (double)ts->B[(size_t)a * ts->T + a];
+    tr_k = (double)p->outputscale * bt;
   }
   if (trace_resid_out) *trace_resid_out = tr_k - lsq;
   GP_CUDA(cudaStreamSynchronize(st));

@@ -92,6 +92,12 @@ class Plan:
                 self._h, _ptr(self.x1), self.n1, self.x1.stride(0),
                 _ptr(None if self.same else self.x2), self.n2, self.x2.stride(0), self.d,
                 self.row_begin, self.row_count if self.row_count != self.n1 else 0))
+            tasks = getattr(self, "_tasks", None)
+            if tasks is not None:   # new data drops the engine's task layout: put it back
+                check(self.lib.gp_plan_set_tasks(self._h, _ptr(tasks[0]), _ptr(tasks[1]), tasks[2]))
+                if getattr(self, "_task_covar", None) is not None:
+                    bh = self._task_covar
+                    check(self.lib.gp_plan_set_task_covar(self._h, (C.c_float * bh.numel())(*bh.reshape(-1).tolist()), tasks[2]))
         return self
 
     def close(self):
@@ -212,6 +218,63 @@ class Plan:
         with torch.cuda.device(self.device):
             check(self.lib.gp_plan_set_lowrank(self._h, _ptr(u), u.stride(0), u.size(1)))
         return self
+
+    def set_tasks(self, task1: torch.Tensor | None, task2: torch.Tensor | None = None, num_tasks: int | None = None):
+        """Hadamard multitask: the operator becomes s K(x, x') o B[t, t'] once set_task_covar supplies B.  task1 [n1] (task2 [n2] on
+        a cross plan, None on a square one) integer task ids in [0, num_tasks); None clears them.  The engine copies the ids and
+        sorts its packed rows and columns by task; refresh_data (new inputs) re-applies them."""
+        if task1 is None:
+            self._tasks = None
+            with torch.cuda.device(self.device):
+                check(self.lib.gp_plan_set_tasks(self._h, _ptr(None), _ptr(None), 0))
+            return self
+        t1 = task1.reshape(-1).to(device=self.device, dtype=torch.int32).contiguous()
+        if t1.numel() != self.n1:
+            raise RuntimeError(f"task1 must have {self.n1} entries (got {t1.numel()})")
+        t2 = None
+        if not self.same:
+            if task2 is None:
+                raise RuntimeError("a cross plan needs the task ids of both inputs")
+            t2 = task2.reshape(-1).to(device=self.device, dtype=torch.int32).contiguous()
+            if t2.numel() != self.n2:
+                raise RuntimeError(f"task2 must have {self.n2} entries (got {t2.numel()})")
+        T = int(num_tasks) if num_tasks is not None else int(max(t1.max().item(), -1 if t2 is None else t2.max().item())) + 1
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_tasks(self._h, _ptr(t1), _ptr(t2), T))
+        self._tasks = (t1, t2, T)
+        self.num_tasks = T
+        return self
+
+    def set_task_covar(self, b: torch.Tensor):
+        """B [T, T] of the Hadamard operator (any device; copied to the host).  Call again whenever it changes."""
+        T = getattr(self, "num_tasks", None)
+        if getattr(self, "_tasks", None) is None or T is None:
+            raise RuntimeError("set_task_covar: the plan has no task ids (set_tasks)")
+        bh = b.detach().to(device="cpu", dtype=torch.float32).contiguous()
+        if tuple(bh.shape) != (T, T):
+            raise RuntimeError(f"task covariance must be [{T}, {T}] (got {tuple(b.shape)})")
+        arr = (C.c_float * (T * T))(*bh.reshape(-1).tolist())
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_task_covar(self._h, arr, T))
+        self._task_covar = bh
+        return self
+
+    def task_covar_grad(self, left: torch.Tensor, right: torch.Tensor) -> torch.Tensor:
+        """d/dB [T, T] (float64, CPU) of sum(left * ((s K o B) @ right)) for left [n1, s], right [n2, s]."""
+        T = getattr(self, "num_tasks", None)
+        if getattr(self, "_tasks", None) is None or T is None:
+            raise RuntimeError("task_covar_grad: the plan has no task ids (set_tasks)")
+        if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.n1 or right.size(0) != self.n2 \
+                or left.size(1) != right.size(1) or left.size(1) < 1:
+            raise RuntimeError(f"task_covar_grad: left must be [{self.n1}, s] and right [{self.n2}, s] "
+                               f"(got {tuple(left.shape)}, {tuple(right.shape)})")
+        _require_cuda_f32(left, "left")
+        _require_cuda_f32(right, "right")
+        left, right = _row_block(left), _row_block(right)
+        out = (C.c_double * (T * T))()
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_task_covar_grad(self._h, _ptr(left), _ld(left), _ptr(right), _ld(right), left.size(1), out))
+        return torch.tensor([out[i] for i in range(T * T)], dtype=torch.float64).reshape(T, T)
 
     def info(self):
         b, s, k, m = C.c_int(), C.c_int(), C.c_int(), C.c_int()

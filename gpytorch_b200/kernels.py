@@ -216,6 +216,56 @@ class AdditiveKernel(Kernel):
         return terms[0] if len(terms) == 1 else SumKernelLinearOperator(terms)
 
 
+class IndexKernel(Module):
+    """Task covariance B = F F^T + diag(v) over task indices (kernels/index_kernel.py:18-117): parameters `covar_factor` [T, rank]
+    and `raw_var` [T] with the reference's names and initialisation.  Calling it on task ids returns a lazy IndexLinearOperator
+    that a data kernel's operator multiplies in (`covar_x.mul(covar_i)`): the Hadamard multitask model.  Unbatched, no prior."""
+
+    def __init__(self, num_tasks, rank=1, batch_shape=None, prior=None, var_constraint=None, **kwargs):
+        if rank > num_tasks:
+            raise RuntimeError("Cannot create a task covariance matrix larger than the number of tasks")
+        super().__init__()
+        self.batch_shape = torch.Size(batch_shape) if batch_shape is not None else torch.Size()
+        if len(self.batch_shape):
+            raise NotImplementedError("a batched IndexKernel is not available on the accelerated path")
+        if prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        if num_tasks > 32:
+            raise NotImplementedError("the accelerated path supports up to 32 tasks")
+        self.num_tasks = num_tasks
+        self.register_parameter("covar_factor", torch.nn.Parameter(torch.randn(*self.batch_shape, num_tasks, rank)))
+        self.register_parameter("raw_var", torch.nn.Parameter(torch.randn(*self.batch_shape, num_tasks)))
+        self.register_constraint("raw_var", var_constraint or Positive())
+
+    @property
+    def var(self):
+        return self.raw_var_constraint.transform(self.raw_var)
+
+    @var.setter
+    def var(self, value):
+        self._set_var(value)
+
+    def _set_var(self, value):
+        self._set_constrained("raw_var", value)
+
+    def _eval_covar_matrix(self):
+        cf = self.covar_factor
+        return cf @ cf.transpose(-1, -2) + torch.diag_embed(self.var)
+
+    @property
+    def covar_matrix(self):
+        """B as a dense [T, T] tensor (the reference returns it as PsdSumLinearOperator(RootLinearOperator(F), DiagLinearOperator(v)))."""
+        return self._eval_covar_matrix()
+
+    def __call__(self, i1, i2=None, **params):
+        from .operators import IndexLinearOperator
+        i1 = i1.long().reshape(-1)
+        i2 = i1 if i2 is None else i2.long().reshape(-1)
+        return IndexLinearOperator(i1, i2, self._eval_covar_matrix())
+
+    forward = __call__
+
+
 class GridInterpolationKernel(Kernel):
     """SKI / KISS-GP (kernels/grid_interpolation_kernel.py:14-213): base_kernel(x, x') ~= w_x^T K_grid w_x' with cubic interpolation
     onto a regular grid; K_grid is a Kronecker product of per-dimension Toeplitz matrices (kernels/grid_kernel.py:107-177).

@@ -118,6 +118,70 @@ class GaussianLikelihood(_GaussianLikelihoodBase):
         self.noise_covar.initialize(raw_noise=value)
 
 
+class MultitaskHomoskedasticNoise(HomoskedasticNoise):
+    """noise_models.py:102-106: one learned sigma^2 per task, raw_noise [*batch_shape, num_tasks]."""
+
+    def __init__(self, num_tasks, noise_prior=None, noise_constraint=None, batch_shape=torch.Size()):
+        super().__init__(noise_prior=noise_prior, noise_constraint=noise_constraint, batch_shape=batch_shape, num_tasks=num_tasks)
+
+
+class HadamardGaussianLikelihood(_GaussianLikelihoodBase):
+    """Task-wise noise sigma^2_{t_i} for the Hadamard multitask model (likelihoods/hadamard_gaussian_likelihood.py): the noise
+    covariance is the per-row diagonal noise[t] (gp_plan_set_noise_diag on the engine).  The task ids come as the first extra
+    argument: a tensor of ids [n] / [n, 1], or the model's inputs (a tuple / list), where the integer-valued tensor is taken, or
+    column `task_feature_index` of a single input that carries the task as a feature."""
+
+    def __init__(self, num_tasks, noise_prior=None, noise_constraint=None, batch_shape=torch.Size(), task_feature_index=None,
+                 **kwargs):
+        super().__init__()
+        if noise_prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        if len(torch.Size(batch_shape)):
+            raise NotImplementedError("a batched HadamardGaussianLikelihood is not available on the accelerated path")
+        self.noise_covar = MultitaskHomoskedasticNoise(num_tasks=num_tasks, noise_constraint=noise_constraint,
+                                                       batch_shape=torch.Size(batch_shape))
+        self.num_tasks = num_tasks
+        self.task_feature_index = task_feature_index
+
+    @property
+    def noise(self):
+        return self.noise_covar.noise
+
+    @noise.setter
+    def noise(self, value):
+        self.noise_covar._set_noise(value)
+
+    @property
+    def raw_noise(self):
+        return self.noise_covar.raw_noise
+
+    @raw_noise.setter
+    def raw_noise(self, value):
+        self.noise_covar.initialize(raw_noise=value)
+
+    def _task_ids(self, params):
+        if len(params) == 0 or params[0] is None or (not torch.is_tensor(params[0]) and len(params[0]) == 0):
+            raise ValueError("Task indices must be provided.")
+        p = params[0]
+        if not torch.is_tensor(p):
+            ints = [a for a in p if torch.is_tensor(a) and not a.is_floating_point()]
+            p = ints[-1] if ints else p[0]
+        if p.dim() > 1 and p.shape[-1] > 1:
+            if self.task_feature_index is None:
+                raise ValueError("Task indices must be a single dimension if task_feature_index is not provided.")
+            p = p[..., self.task_feature_index]
+        t = p.reshape(-1)
+        if t.is_floating_point() and not torch.equal(t, t.round()):
+            raise ValueError("Expected task indexes with integer values.")
+        return t.long()
+
+    def _shaped_noise_covar(self, base_shape, *params, **kwargs):
+        t = self._task_ids(params)
+        if t.numel() != base_shape[-1]:
+            raise ValueError(f"Expected {base_shape[-1]} task indexes, got {t.numel()}.")
+        return DiagLinearOperator(self.noise.reshape(-1)[t])
+
+
 class FixedNoiseGaussianLikelihood(_GaussianLikelihoodBase):
     """Known heteroscedastic observation noise (+ optionally a learned homoskedastic term): gaussian_likelihood.py:245-363."""
 

@@ -110,16 +110,27 @@ class ExactGP(Module):
         # (lazy_evaluated_kernel_tensor.py:136-243 re-indexes x1 / x2; nothing is materialised).
         train_x, test_x = self.train_inputs[0], inputs[0]
         n = train_x.size(-2)
-        train_out = self.forward(train_x)
-        if settings.ski_grid_prediction.on():
-            test_out = self.forward(test_x)
-            mode = _ski_grid_mode(train_out.lazy_covariance_matrix, test_out.lazy_covariance_matrix)
-            if mode is not None:
-                return self._ski_grid_posterior(train_x, test_x, train_out, test_out, mode)
-        full_out = self.forward(torch.cat([train_x, test_x], dim=-2))
+        multi = len(self.train_inputs) > 1
+        if multi:
+            # several inputs (e.g. x and the task index of a Hadamard multitask model): every input is concatenated, train then
+            # test, for the joint forward, and the likelihood sees the train inputs (exact_prediction_strategies.py passes them)
+            if len(inputs) != len(self.train_inputs):
+                raise RuntimeError(f"the model was trained on {len(self.train_inputs)} inputs, got {len(inputs)}")
+            train_out = self.forward(*self.train_inputs)
+            full_out = self.forward(*[torch.cat([a, b], dim=-2) for a, b in zip(self.train_inputs, inputs)])
+            lik_params = (self.train_inputs,)
+        else:
+            train_out = self.forward(train_x)
+            if settings.ski_grid_prediction.on():
+                test_out = self.forward(test_x)
+                mode = _ski_grid_mode(train_out.lazy_covariance_matrix, test_out.lazy_covariance_matrix)
+                if mode is not None:
+                    return self._ski_grid_posterior(train_x, test_x, train_out, test_out, mode)
+            full_out = self.forward(torch.cat([train_x, test_x], dim=-2))
+            lik_params = ()
         full_mean, full_covar = full_out.mean, full_out.lazy_covariance_matrix
         with settings._use_eval_tolerance(True):
-            khat = self.likelihood(train_out).lazy_covariance_matrix
+            khat = self.likelihood(train_out, *lik_params).lazy_covariance_matrix
             if self._mean_cache is None:
                 resid = (self.train_targets - train_out.mean).unsqueeze(-1)
                 self._mean_cache = khat.solve(resid).squeeze(-1)  # exact_prediction_strategies.py:286

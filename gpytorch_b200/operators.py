@@ -431,6 +431,19 @@ class KernelLinearOperator(_SamplingMixin):
     def add_jitter(self, jitter_val=1e-3):
         return AddedDiagLinearOperator(self, ConstantDiagLinearOperator(torch.tensor(jitter_val, device=self.device), self.shape[0]))
 
+    def mul(self, other):
+        """K o B[t, t'] with an IndexKernel's operator (the Hadamard multitask model, covar_x.mul(covar_i)): one engine operator
+        (gp_plan_set_tasks).  RBF / Matern operators, optionally scaled, only."""
+        if not isinstance(other, IndexLinearOperator) or type(self) is not KernelLinearOperator:
+            raise NotImplementedError("the accelerated path multiplies an RBF / Matern kernel operator (optionally scaled) by an "
+                                      "IndexKernel operator only")
+        if tuple(other.shape) != tuple(self.shape):
+            raise RuntimeError(f"mul: operator shapes {tuple(self.shape)} and {tuple(other.shape)} differ")
+        return HadamardKernelLinearOperator(self.x1, None if self.same else self.x2, self.kind, self.lengthscale, self.outputscale,
+                                            other.i1, other.i2, other.B)
+
+    __mul__ = mul
+
     def _sampling_plan(self) -> Plan:
         """The plan of K alone: no noise, no per-row diagonal left over from an earlier K + D."""
         if not self.same:
@@ -444,6 +457,143 @@ class KernelLinearOperator(_SamplingMixin):
         """(d/d lengthscale, d/d outputscale) of sum(left * (K @ right)); lazy_evaluated_kernel_tensor.py:69-105."""
         gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
         return torch.tensor(gl, device=self.device, dtype=self.dtype), torch.tensor(go, device=self.device, dtype=self.dtype)
+
+
+class IndexLinearOperator:
+    """B[i1, i2] of an IndexKernel (kernels/index_kernel.py:101-117 returns it as an InterpolatedLinearOperator): lazy, it only
+    carries the task ids and B until a kernel operator multiplies it in (KernelLinearOperator.mul)."""
+
+    def __init__(self, i1: torch.Tensor, i2: torch.Tensor, B: torch.Tensor):
+        self.i1, self.i2, self.B = i1, i2, B
+
+    @property
+    def shape(self):
+        return torch.Size([self.i1.numel(), self.i2.numel()])
+
+    def size(self, dim=None):
+        return self.shape if dim is None else self.shape[dim]
+
+    @property
+    def device(self):
+        return self.B.device
+
+    def to_dense(self):
+        return self.B[self.i1][:, self.i2]
+
+    def diagonal(self, dim1=-2, dim2=-1):
+        return self.B[self.i1, self.i2]
+
+    def mul(self, other):
+        if isinstance(other, KernelLinearOperator):
+            return other.mul(self)
+        raise NotImplementedError("an IndexKernel operator multiplies an RBF / Matern kernel operator only")
+
+    __mul__ = mul
+
+
+_TASK_SLOT = 16   # plan-cache slot of Hadamard operators: a plain operator over the same inputs never sees their task ids
+
+
+class HadamardKernelLinearOperator(KernelLinearOperator):
+    """s K(x1, x2) o B[t1, t2] (the Hadamard multitask model, examples/03_Multitask_Exact_GPs/Hadamard_Multitask_GP_Regression.ipynb):
+    one engine operator whose plan carries the task ids (gp_plan_set_tasks) and B (gp_plan_set_task_covar).  The hyper-parameters
+    are lengthscale, outputscale and B; B's gradient comes from gp_task_covar_grad and autograd carries it to the IndexKernel's
+    covar_factor / raw_var.  Input gradients are not available: inputs that require grad are refused."""
+
+    def __init__(self, x1, x2, kind, lengthscale, outputscale, t1, t2, B):
+        if x1.requires_grad or (x2 is not None and x2.requires_grad):
+            raise RuntimeError("gradients with respect to the inputs of a Hadamard multitask operator (K o B) are not implemented: "
+                               "pass inputs that do not require grad")
+        super().__init__(x1, x2, kind, lengthscale, outputscale)
+        self.t1 = t1.reshape(-1)
+        if self.same and t2 is not None and t2 is not t1 and not torch.equal(t2.reshape(-1), self.t1):
+            raise NotImplementedError("a square kernel operator takes one set of task ids (x2 == x1 needs t2 == t1)")
+        self.t2 = self.t1 if self.same else t2.reshape(-1)
+        if self.t1.numel() != self.shape[0] or self.t2.numel() != self.shape[1]:
+            raise RuntimeError(f"task ids of sizes {self.t1.numel()}, {self.t2.numel()} do not match the operator {tuple(self.shape)}")
+        self.B = B
+        self._plan_slot = _TASK_SLOT
+
+    def plan(self, noise=0.0) -> Plan:
+        p = super().plan(noise)
+        T = int(self.B.shape[-1])
+        src = getattr(p, "_task_src", None)
+        # the plan keeps the id tensors it was given alive, so an identity + version match cannot be a recycled buffer
+        if src is None or src[0] is not self.t1 or src[1] is not self.t2 or src[2] != (self.t1._version, self.t2._version) \
+                or src[3] != T or getattr(p, "_tasks", None) is None:
+            p.set_tasks(self.t1, None if self.same else self.t2, T)
+            p._task_src = (self.t1, self.t2, (self.t1._version, self.t2._version), T)
+            p._b_key = None
+        bh = getattr(self, "_b_host", None)
+        if bh is None:
+            bh = self._b_host = self.B.detach().float().cpu()
+        if getattr(p, "_b_key", None) is None or not torch.equal(p._b_key, bh):
+            p.set_task_covar(bh)
+            p._b_key = bh
+        return p
+
+    @property
+    def requires_grad(self):
+        return bool(super().requires_grad or self.B.requires_grad)
+
+    def representation(self):
+        return (self.x1, self.x2, self.lengthscale, self.outputscale, self.B)
+
+    def hyper_tensors(self):
+        return [self.lengthscale, self.outputscale, self.B]
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    def _bilinear_derivative_list(self, left, right):
+        p = self.plan(getattr(self, "_last_noise", 0.0))
+        gl, go = p.bilinear_grad(left, right)
+        dB = p.task_covar_grad(left, right)
+        return [torch.tensor(gl, device=self.device, dtype=self.dtype).reshape(self.lengthscale.shape),
+                torch.tensor(go, device=self.device, dtype=self.dtype).reshape(self.outputscale.shape),
+                dB.to(device=self.device, dtype=self.B.dtype)]
+
+    def _bilinear_derivative(self, left, right):
+        gl, go, _ = self._bilinear_derivative_list(left, right)
+        return gl, go
+
+    def _transpose_nonbatch(self):
+        if self.same:
+            return self
+        return HadamardKernelLinearOperator(self.x2, self.x1, self.kind, self.lengthscale, self.outputscale, self.t2, self.t1,
+                                            self.B.transpose(-1, -2))
+
+    def detach(self):
+        return HadamardKernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.kind,
+                                            self.lengthscale.detach(), self.outputscale.detach(), self.t1,
+                                            None if self.same else self.t2, self.B.detach())
+
+    def to_dense(self):
+        return _KernelDense.apply(self)
+
+    def __getitem__(self, index):
+        """Slices re-index the task ids together with x1 / x2 (prediction slices the joint operator)."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        x2 = self.x1 if self.same else self.x2
+        return HadamardKernelLinearOperator(self.x1[ri], x2[ci], self.kind, self.lengthscale, self.outputscale, self.t1[ri],
+                                            self.t2[ci], self.B)
+
+    def mul(self, other):
+        raise NotImplementedError("a Hadamard multitask operator takes one IndexKernel factor")
+
+    __mul__ = mul
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("a Hadamard multitask operator adds a (Constant)DiagLinearOperator only")
 
 
 class SumKernelLinearOperator(KernelLinearOperator):
@@ -774,7 +924,8 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
     @staticmethod
     def supports(base) -> bool:
         """A plan-backed non-SKI kernel operator (or kernel sum) without batch dimension on an unsharded square plan."""
-        return (isinstance(base, KernelLinearOperator) and not isinstance(base, SKIKernelLinearOperator) and base.same
+        return (isinstance(base, KernelLinearOperator) and not isinstance(base, (SKIKernelLinearOperator, HadamardKernelLinearOperator))
+                and base.same
                 and base._comm is None and base._row_begin == 0 and base._row_count in (0, base.shape[0]))
 
     def plan(self, noise=0.0) -> Plan:

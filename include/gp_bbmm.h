@@ -135,6 +135,28 @@ int gp_plan_set_sum(gp_plan* plan, gp_plan* const* terms, int n_terms);
  * return GP_E_STATE until gp_plan_set_lowrank is called again. */
 int gp_plan_set_lowrank(gp_plan* plan, const float* U, int64_t ldu, int r);
 
+/* Hadamard multitask GPs (IndexKernel, kernels/index_kernel.py:18-117, multiplied into the data kernel as in
+ * examples/03_Multitask_Exact_GPs/Hadamard_Multitask_GP_Regression.ipynb): with task ids set, the plan's operator becomes
+ *     s K(x_i, x'_j) B[t_i, t'_j]   (+ its noise / per-row diagonal where a call adds it).
+ * gp_plan_set_tasks: device int32 task ids, task1 [n1] and task2 [n2] (task2 = NULL on a square plan), 1 <= T <= 32; ids outside
+ *   [0, T) return GP_E_SHAPE.  Call after gp_plan_set_data (new data drops the tasks); task1 = NULL clears them.  The ids are copied:
+ *   the caller's arrays need not outlive the call.  GP_E_STATE on SKI, kernel-sum and low-rank-corrected plans, GP_E_SHAPE on a
+ *   row-sharded plan.
+ * gp_plan_set_task_covar: B as a host array, row-major T x T (need not be symmetric or PSD: not checked); call again whenever it
+ *   changes, like gp_plan_set_hypers.  Every call that applies the operator returns GP_E_STATE until it has been set.
+ * Tensor-core and SIMT plans, square and cross: gp_kmv, gp_krows, gp_kdiag (s B[t_i, t_i]: not constant), gp_pivoted_cholesky
+ * (first pivot = argmax of that diagonal, as for SKI), gp_precond_build / gp_precond_probes, gp_mbcg, gp_slq_logdet, gp_mll,
+ * gp_lanczos, gp_ciq_* and gp_bilinear_grad (lengthscale(s) and outputscale of s K o B).  The input gradients (gp_kmv_input_grad,
+ * gp_kdense_input_grad, gp_ski_input_grad) return GP_E_STATE.  One K.V is one launch of the plain fused kernel per column task over
+ * that task's columns (rows and columns packed in task order), then B is applied row by row: no atomics, repeated calls agree bit
+ * for bit.
+ * gp_task_covar_grad: dB [T][T] (host, row-major) with dB[a][b] = s sum_{i: t_i = a} sum_{j: t'_j = b} (L_i . R_j) k(x_i, x'_j),
+ * L [n1, t] (ldl), R [n2, t] (ldr), any t >= 1: the gradient of sum_ic L_ic ((s K o B) R)_ic with respect to B, at the cost of one
+ * K.V per 16 columns.  Non-finite inputs give NaN. */
+int gp_plan_set_tasks(gp_plan* plan, const int32_t* task1, const int32_t* task2, int T);
+int gp_plan_set_task_covar(gp_plan* plan, const float* B, int T);
+int gp_task_covar_grad(gp_plan* plan, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB);
+
 /* ---- kernel seam (LazyEvaluatedKernelTensor, lazy/lazy_evaluated_kernel_tensor.py) --- */
 
 /* OUT[n1_local, t] = K(X1,X2) V [+ noise * V when add_noise and X2 == X1].
@@ -267,7 +289,8 @@ int gp_plan_set_comm(gp_plan* plan, gp_comm* comm);      /* NULL = single GPU */
 int64_t gp_kernel_launches(gp_plan* plan);               /* kernels launched by this plan so far */
 int gp_plan_info(gp_plan* plan, int* backend, int* nsplit, int* kpad, int* n_sm);
 /* Times `reps` back-to-back launches of the fused K.V kernel ALONE (after `warmup` untimed ones) with CUDA
- * events on the plan's stream; V [n2, t].  *ms_per_launch is the average device time of one launch. */
+ * events on the plan's stream; V [n2, t].  *ms_per_launch is the average device time of one launch.  On a plan with task ids a
+ * "launch" is the whole K o B product (V gather and tiles, one launch per column task, combine). */
 int gp_time_kmv_kernel(gp_plan* plan, const float* V, int64_t ldv, int t, int warmup, int reps, float* ms_per_launch);
 
 #ifdef __cplusplus
