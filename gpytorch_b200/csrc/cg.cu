@@ -536,6 +536,7 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
              int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
              int* tridiag_size, float* resid_out) {
   GP_REQUIRE(p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  KronColsScope kcols(p, t);   // the direction block's columns >= t stay zero
   GP_REQUIRE(p->same, GP_E_SHAPE, "mBCG needs a square operator (X2 == X1)");
   GP_REQUIRE(t >= 1 && t <= TP, GP_E_SHAPE, "mBCG handles 1..%d right-hand sides per call (t=%d)", TP, t);
   GP_REQUIRE(n_tridiag >= 0 && n_tridiag <= t, GP_E_SHAPE, "n_tridiag=%d out of range", n_tridiag);
@@ -603,7 +604,8 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   // the direction block is written straight into the packed K.V tiles when this rank owns all rows and the tensor-core
   // kernel runs; sharded runs all-gather the fp32 rows first and pack the gathered block (pack.cu)
   const bool tc = plan_is_tc(p);
-  const bool fuse_pack = tc && !sharded && !p->tasks;   // a multitask product packs its own task-ordered tiles (tasks.cu)
+  // a multitask product packs its own task-ordered tiles (tasks.cu); a Kronecker product packs its B-mixed chunks (kron.cu)
+  const bool fuse_pack = tc && !sharded && !p->tasks && !p->kron;
   float* Vt = fuse_pack ? p->Vtiles.as<float>() : nullptr;
   const int64_t nchunk_pack = fuse_pack ? p->ntile_j * (TILE_J / 4) : 0;
   const int Gd = (int)std::min<int64_t>(cdiv(std::max<int64_t>(nchunk_pack, cdiv(n, (int64_t)4)) * 4, (int64_t)RP_THREADS), 4 * p->n_sm);

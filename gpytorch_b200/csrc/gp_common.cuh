@@ -170,6 +170,20 @@ struct gp_task_state {
   int* d_slot0 = nullptr;
 };
 
+// Kronecker multitask state (kron.cu): the operator is (s K_data) (x) B over interleaved rows i T + a.  One K.V mixes the block by
+// B into ceil(T t / 16) zero-padded [N2, 16] column chunks, runs the data plan's fused kernel once per chunk into its own partial
+// slots, and scatters the chunks back to rows i T + a of partial slot 0.
+struct gp_kron_state {
+  gp_plan* data = nullptr;                 // caller-owned plain plan of K_data
+  int T = 0;
+  std::vector<float> B;                    // host T x T task covariance, row-major
+  bool b_set = false;
+  bool b_bad = false;                      // B has a non-finite entry: every product and gradient is NaN
+  gp::DevBuf Bd;                           // B on the device
+  gp::DevBuf W, Vt, part;                  // mixed chunks [nchunk][npad][16] | their packed V tiles | data's slots per chunk
+  gp::DevBuf Lw, red, idx, rows;           // gradient / row-extraction scratch
+};
+
 struct gp_comm {
   void* nccl_comm = nullptr;
   int rank = 0, world = 1;
@@ -226,7 +240,18 @@ struct gp_plan {
   int lr_r = 0;
   gp::DevBuf lrw;                 // U^T V partials [G][16 r] | c = U^T V [r][16] fp64
   gp_task_state* tasks = nullptr; // non-null: Hadamard multitask operator s K o B[t, t'] (gp_plan_set_tasks)
+  gp_kron_state* kron = nullptr;  // non-null: Kronecker multitask operator (s K_data) (x) B (gp_plan_set_kron)
+  int kron_cols = 16;             // columns of V16 a Kronecker product mixes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
+};
+
+// A solver loop that applies a Kronecker operator to blocks of t < 16 live columns narrows the mix to those columns for its
+// lifetime: ceil(T t / 16) data-kernel launches per product instead of T.  Other plans ignore it.
+struct KronColsScope {
+  gp_plan* p;
+  int old;
+  KronColsScope(gp_plan* plan, int t) : p(plan), old(plan->kron_cols) { p->kron_cols = t < 1 ? 1 : (t > 16 ? 16 : t); }
+  ~KronColsScope() { p->kron_cols = old; }
 };
 
 namespace gp {
@@ -269,6 +294,16 @@ int tasks_krows_scale(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int
 int tasks_bilinear(gp_plan* p, const float* L16, const float* R16, bool ard, std::vector<double>& total);
 #define GP_REFUSE_TASKS(p, what) \
   GP_REQUIRE((p)->tasks == nullptr, GP_E_STATE, "%s is not available on a plan with task indices (gp_plan_set_tasks)", what)
+int kron_pack(gp_plan* p);                                                   // kron.cu
+int kron_kmv_partials(gp_plan* p, const float* V16, const int* done_flag);   // (s K) (x) B V into partial slot 0 (unscaled)
+int kron_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
+int kron_kdiag(gp_plan* p, float* OUT);
+int kron_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+int kron_refresh(gp_plan* p);                                                // re-check the data plan, take its scale / kind / flag
+int kron_set_task_covar(gp_plan* p, const float* B, int T);                  // gp_plan_set_task_covar on a Kronecker plan
+int kron_task_covar_grad_checked(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB);
+#define GP_REFUSE_KRON(p, what) \
+  GP_REQUIRE((p)->kron == nullptr, GP_E_STATE, "%s is not available on a Kronecker multitask plan (gp_plan_set_kron)", what)
 int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,   // cg.cu
              int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
              int* tridiag_size, float* resid_out);

@@ -81,6 +81,7 @@ extern "C" int gp_lanczos(gp_plan* p, const float* INIT, int max_iter, float tol
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_REQUIRE(p->same, GP_E_SHAPE, "Lanczos needs a square operator");
   GP_REQUIRE(max_iter >= 1, GP_E_SHAPE, "max_iter must be >= 1");
+  KronColsScope kcols(p, 1);   // one Lanczos vector per product
   cudaStream_t st = p->stream;
   // row-sharded runs (one process per GPU): every vector (INIT, the basis rows of Qt, r) holds this rank's rows only; the
   // products all-gather the current basis vector, the dots / Gram-Schmidt coefficients are all-reduced (fp64)

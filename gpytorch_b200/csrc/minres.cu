@@ -447,6 +447,7 @@ __global__ void ms_scale_kernel(float* __restrict__ Z, const MsState* __restrict
 int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int k, const double* tau, const double* w, int Q,
             float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out, float* resid_out) {
   GP_REQUIRE(p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  KronColsScope kcols(p, t);   // the Lanczos blocks' columns >= t stay zero
   const bool pre = U != nullptr || k != 0;
   if (pre) {
     GP_REQUIRE(U != nullptr && k >= 1 && k <= MS_KMAX, GP_E_SHAPE, "preconditioner factor U [n, k] with k in [1,%d] (k=%d, U %s)",

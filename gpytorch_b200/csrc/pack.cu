@@ -181,6 +181,7 @@ int pack_inputs(gp_plan* p) {
   GP_REQUIRE(p->data_set && p->hypers_set, GP_E_STATE, "set_data and set_hypers must both be called");
   if (p->backend == GP_BACKEND_SKI) return ski_pack(p);
   if (p->backend_req == GP_BACKEND_SUM) return sum_pack(p);
+  if (p->backend_req == GP_BACKEND_KRON) return kron_pack(p);
   GP_CHECK(choose_geometry(p));
   cudaStream_t st = p->stream;
   const int d = p->d, DP = p->DP;

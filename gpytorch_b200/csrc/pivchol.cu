@@ -189,17 +189,20 @@ constexpr int PC_KIND_SUM = 64;
 // SKI (GP_BACKEND_SKI): K[pivot, j] = s prod_k w_jk^T u_k[f_jk : f_jk + 4] with u of the pivot staged where the pivot row of Z sits
 // (ski_rows.cuh); DP = sum_k G_k
 constexpr int PC_KIND_SKI = 65;
-// Hadamard multitask (tasks.cu): K[pivot, j] = s B[t_pivot, t_j] k(|z_pivot - z_j|^2), covariance kind kind[0]
+// multitask (tasks.cu, kron.cu): K[r, r'] = s B[task(r), task(r')] k(|z_point(r) - z_point(r')|^2), covariance kind kind[0]; row r is
+// point r / rep, task task[r] (Hadamard: rep = 1, task ids) or point r / T, task r mod T (Kronecker: rep = T, task = nullptr)
 constexpr int PC_KIND_TASK = 66;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
   float os[4];
   const float* Z[4];
-  const int* task;   // PC_KIND_TASK: task ids (user order) and B [T][T]
+  const int* task;   // PC_KIND_TASK: task ids (user order; nullptr: r mod rep) and B [T][T]
   const float* B;
   int T;
+  int rep;           // PC_KIND_TASK: rows per point
 };
+__device__ __forceinline__ int pc_task_of(const PcTerms& tt, int r) { return tt.task ? tt.task[r] : r % tt.rep; }
 __device__ __forceinline__ float pc_cov_rt(int kind, float a) {
   switch (kind) {
     case GP_RBF: return cov_from_arg<GP_RBF>(a);
@@ -252,7 +255,8 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
     } else if (KIND == PC_KIND_SKI) {
       ski_stage_u(sk, pi, zp, tid, PCP_THREADS);
     } else {
-      for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[(int64_t)pi * DP + c];
+      const int64_t zr = KIND == PC_KIND_TASK ? pi / tt.rep : pi;
+      for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[zr * DP + c];
     }
     for (int q = tid; q < m; q += PCP_THREADS) lp[q] = __ldcg(Lt + (int64_t)q * n + pi);   // written by another SM, before the last barrier
     __syncthreads();
@@ -290,12 +294,13 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
         } else if (KIND == PC_KIND_SKI) {
           v = ski_entry(sk, zp, j);
         } else if (KIND == PC_KIND_TASK) {
+          const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
-            float df = zp[c] - Z[j * DP + c];
+            float df = zp[c] - zj[c];
             s = fmaf(df, df, s);
           }
-          v = os * tt.B[tt.task[pi] * tt.T + tt.task[j]] * pc_cov_rt(tt.kind[0], -0.5f * s);
+          v = os * tt.B[pc_task_of(tt, pi) * tt.T + pc_task_of(tt, (int)j)] * pc_cov_rt(tt.kind[0], -0.5f * s);
         } else {
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
@@ -418,12 +423,13 @@ __global__ void pc_init_ski_kernel(const SkiRows sk, float* __restrict__ diag, i
   pos[j] = (int)j;
 }
 
-// Hadamard multitask: diag[j] = s B[t_j, t_j] (not constant across tasks), identity permutation; then pc_first_pivot_kernel
-__global__ void pc_init_task_kernel(const int* __restrict__ task, const float* __restrict__ B, int T, float os, float* __restrict__ diag,
-                                    int* __restrict__ perm, int* __restrict__ pos, int64_t n) {
+// multitask: diag[j] = s B[t_j, t_j] (not constant across tasks), identity permutation; then pc_first_pivot_kernel
+__global__ void pc_init_task_kernel(const PcTerms tt, float os, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos,
+                                    int64_t n) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
-  diag[j] = os * B[task[j] * T + task[j]];
+  const int a = pc_task_of(tt, (int)j);
+  diag[j] = os * tt.B[a * tt.T + a];
   perm[j] = (int)j;
   pos[j] = (int)j;
 }
@@ -787,11 +793,23 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       dp_total += q->DP;
     }
   }
-  const bool tasks = p->tasks != nullptr;
-  if (tasks) {
+  const bool kron = p->kron != nullptr;
+  const bool tasks = p->tasks != nullptr || kron;
+  const float* Zsrc = p->Z2.as<float>();
+  if (kron) {   // entries of (s K_data) (x) B from the data plan's packed rows
+    GP_REQUIRE(p->kron->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
+    GP_CHECK(kron_refresh(p));
+    const gp_plan* q = p->kron->data;
+    tt.kind[0] = q->kind; tt.task = nullptr; tt.B = p->kron->Bd.as<float>(); tt.T = p->kron->T; tt.rep = p->kron->T;
+    Zsrc = q->Z2.as<float>();
+    dp_total = q->DP;
+    os_total = q->outputscale;
+  } else if (tasks) {
     GP_REQUIRE(p->tasks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
-    tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T;
-    pc_init_task_kernel<<<gb, PC_THREADS, 0, st>>>(tt.task, tt.B, tt.T, p->outputscale, diag, perm, pos, n);
+    tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T; tt.rep = 1;
+  }
+  if (tasks) {
+    pc_init_task_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;
   } else if (ski) {
@@ -804,7 +822,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     pc_init_kernel<<<gb, PC_THREADS, 0, st>>>(diag, perm, pos, n, os_total, S, piv);   // stationary terms: constant initial diagonal
     p->launches += 1;
   }
-  const float* Z = (sum || ski) ? nullptr : p->Z2.as<float>();
+  const float* Z = (sum || ski) ? nullptr : Zsrc;
   const bool stepwise = getenv("GP_PC_STEPWISE") != nullptr;   // debugging / A-B switch: one launch per step
   int coop = 0;
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, p->device);
@@ -987,6 +1005,11 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
     tr_k = (double)n * os_total;
   } else if (p->backend == GP_BACKEND_SKI) {
     GP_CHECK(ski_diag_sum(p, &tr_k));
+  } else if (p->kron) {     // s N sum_a B[a, a]
+    const gp_kron_state* ks = p->kron;
+    double bt = 0.0;
+    for (int a = 0; a < ks->T; ++a) bt += (double)ks->B[(size_t)a * ks->T + a];
+    tr_k = (double)ks->data->outputscale * (double)ks->data->n2 * bt;
   } else if (p->tasks) {   // s sum_i B[t_i, t_i]
     const gp_task_state* ts = p->tasks;
     double bt = 0.0;

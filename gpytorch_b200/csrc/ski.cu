@@ -1168,6 +1168,7 @@ using namespace gp;
 extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* grid_lo, const float* grid_step, int d) {
   GP_REQUIRE(p != nullptr && p->data_set, GP_E_STATE, "set_data must precede set_ski");
   GP_REFUSE_TASKS(p, "gp_plan_set_ski");
+  GP_REFUSE_KRON(p, "gp_plan_set_ski");
   GP_REQUIRE(d == p->d && d >= 1 && d <= SKI_MAXD, GP_E_SHAPE, "SKI: grid dimension %d does not match the data (d=%d, max %d)", d, p->d, SKI_MAXD);
   for (int i = 0; i < d; ++i)
     GP_REQUIRE(grid_sizes[i] >= 4 && grid_sizes[i] <= 128 && grid_step[i] > 0.f, GP_E_SHAPE, "SKI: grid size %d (dim %d) must be in [4, 128]", grid_sizes[i], i);
@@ -1188,6 +1189,7 @@ extern "C" int gp_ski_input_grad(gp_plan* p, const float* L, int64_t ldl, const 
   GP_CHECK(ski_predict_check(p, t, ldl, ldr, "gp_ski_input_grad"));
   GP_REFUSE_LOWRANK(p, "gp_ski_input_grad");
   GP_REFUSE_TASKS(p, "gp_ski_input_grad");
+  GP_REFUSE_KRON(p, "gp_ski_input_grad");
   GP_REQUIRE(L && R && DX && lddx >= p->d, GP_E_SHAPE, "gp_ski_input_grad: bad output (leading dimension %lld, d=%d)", (long long)lddx, p->d);
   return ski_with_d(p->d, [&](auto D) { return ski_input_grad_d<D>(p, L, ldl, R, ldr, t, DX, lddx); });
 }

@@ -120,6 +120,7 @@ extern "C" int gp_plan_set_sum(gp_plan* p, gp_plan* const* terms, int n_terms) {
   GP_REQUIRE(terms != nullptr && n_terms >= 1 && n_terms <= 4, GP_E_SHAPE, "a kernel sum takes 1 to 4 terms (got %d)", n_terms);
   GP_REQUIRE(p->ski == nullptr, GP_E_STATE, "a SKI plan cannot become a kernel sum");
   GP_REFUSE_TASKS(p, "gp_plan_set_sum");
+  GP_REFUSE_KRON(p, "gp_plan_set_sum");
   GP_CUDA(cudaSetDevice(p->device));
   p->terms.assign(terms, terms + n_terms);
   p->backend_req = GP_BACKEND_SUM;

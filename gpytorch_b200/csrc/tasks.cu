@@ -312,6 +312,7 @@ extern "C" int gp_plan_set_tasks(gp_plan* p, const int32_t* task1, const int32_t
     }
     return GP_OK;
   }
+  GP_REFUSE_KRON(p, "gp_plan_set_tasks");
   GP_REQUIRE(p->data_set, GP_E_STATE, "gp_plan_set_tasks: call gp_plan_set_data first");
   GP_REQUIRE(T >= 1 && T <= 32, GP_E_SHAPE, "number of tasks T=%d not in [1, 32]", T);
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "task indices are not available on a SKI plan");
@@ -373,6 +374,7 @@ extern "C" int gp_plan_set_tasks(gp_plan* p, const int32_t* task1, const int32_t
 
 extern "C" int gp_plan_set_task_covar(gp_plan* p, const float* B, int T) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  if (p->kron) return kron_set_task_covar(p, B, T);   // the B of (s K) (x) B (kron.cu)
   GP_REQUIRE(p->tasks != nullptr, GP_E_STATE, "gp_plan_set_task_covar: no task indices (gp_plan_set_tasks)");
   GP_REQUIRE(B != nullptr && T == p->tasks->T, GP_E_SHAPE, "task covariance must be %d x %d (got T=%d)", p->tasks->T, p->tasks->T, T);
   GP_CUDA(cudaSetDevice(p->device));
@@ -387,6 +389,7 @@ extern "C" int gp_plan_set_task_covar(gp_plan* p, const float* B, int T) {
 
 extern "C" int gp_task_covar_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  if (p->kron) return kron_task_covar_grad_checked(p, L, ldl, R, ldr, t, dB);   // dB of (s K) (x) B (kron.cu)
   GP_REQUIRE(p->tasks != nullptr, GP_E_STATE, "gp_task_covar_grad: no task indices (gp_plan_set_tasks)");
   GP_REQUIRE(t >= 1 && L && R && dB, GP_E_SHAPE, "gp_task_covar_grad: bad arguments");
   GP_REQUIRE((ldl >= t || p->n1 == 1) && (ldr >= t || p->n2 == 1), GP_E_SHAPE,

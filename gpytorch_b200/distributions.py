@@ -91,3 +91,46 @@ class MultivariateNormal:
         """rsample without gradients (multivariate_normal.py:322-337)."""
         with torch.no_grad():
             return self.rsample(sample_shape=sample_shape, base_samples=base_samples)
+
+
+class MultitaskMultivariateNormal(MultivariateNormal):
+    """distributions/multitask_multivariate_normal.py:34-281 with interleaved=True: mean [n, T], covariance over the interleaved
+    vector vec(mean) (row i T + a = point i, task a).  event_shape is (n, T), so ExactMarginalLogLikelihood divides by n T; log_prob,
+    samples and the variance flatten / reshape row-major."""
+
+    def __init__(self, mean, covariance_matrix, validate_args=False, interleaved=True):
+        if not interleaved:
+            raise NotImplementedError("a non-interleaved MultitaskMultivariateNormal is not available on the accelerated path")
+        if not torch.is_tensor(mean) or mean.dim() != 2:
+            raise RuntimeError("MultitaskMultivariateNormal takes a mean of shape [n, num_tasks] on the accelerated path")
+        n, T = mean.shape
+        if covariance_matrix.shape[-1] != n * T or covariance_matrix.shape[-2] != n * T:
+            raise RuntimeError(f"mean shape {tuple(mean.shape)} is incompatible with covariance shape {tuple(covariance_matrix.shape)}")
+        self._output_shape = mean.shape
+        self._interleaved = True
+        super().__init__(mean.reshape(-1), covariance_matrix)
+
+    @property
+    def num_tasks(self):
+        return self._output_shape[-1]
+
+    @property
+    def mean(self):
+        return self.loc.reshape(self._output_shape)
+
+    @property
+    def variance(self):
+        return super().variance.reshape(self._output_shape)
+
+    @property
+    def event_shape(self):
+        return self._output_shape
+
+    def log_prob(self, value):
+        return super().log_prob(value.reshape(-1))
+
+    def rsample(self, sample_shape=torch.Size(), base_samples=None):
+        if base_samples is not None:
+            base_samples = base_samples.reshape(*base_samples.shape[:-2], -1)
+        res = super().rsample(sample_shape=sample_shape, base_samples=base_samples)
+        return res.reshape(*res.shape[:-1], *self._output_shape)

@@ -248,8 +248,8 @@ class Plan:
     def set_task_covar(self, b: torch.Tensor):
         """B [T, T] of the Hadamard operator (any device; copied to the host).  Call again whenever it changes."""
         T = getattr(self, "num_tasks", None)
-        if getattr(self, "_tasks", None) is None or T is None:
-            raise RuntimeError("set_task_covar: the plan has no task ids (set_tasks)")
+        if (getattr(self, "_tasks", None) is None and getattr(self, "data", None) is None) or T is None:
+            raise RuntimeError("set_task_covar: the plan has no task ids (set_tasks) and is no Kronecker plan")
         bh = b.detach().to(device="cpu", dtype=torch.float32).contiguous()
         if tuple(bh.shape) != (T, T):
             raise RuntimeError(f"task covariance must be [{T}, {T}] (got {tuple(b.shape)})")
@@ -262,8 +262,8 @@ class Plan:
     def task_covar_grad(self, left: torch.Tensor, right: torch.Tensor) -> torch.Tensor:
         """d/dB [T, T] (float64, CPU) of sum(left * ((s K o B) @ right)) for left [n1, s], right [n2, s]."""
         T = getattr(self, "num_tasks", None)
-        if getattr(self, "_tasks", None) is None or T is None:
-            raise RuntimeError("task_covar_grad: the plan has no task ids (set_tasks)")
+        if (getattr(self, "_tasks", None) is None and getattr(self, "data", None) is None) or T is None:
+            raise RuntimeError("task_covar_grad: the plan has no task ids (set_tasks) and is no Kronecker plan")
         if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.n1 or right.size(0) != self.n2 \
                 or left.size(1) != right.size(1) or left.size(1) < 1:
             raise RuntimeError(f"task_covar_grad: left must be [{self.n1}, s] and right [{self.n2}, s] "
@@ -279,7 +279,7 @@ class Plan:
     def info(self):
         b, s, k, m = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         check(self.lib.gp_plan_info(self._h, C.byref(b), C.byref(s), C.byref(k), C.byref(m)))
-        return {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum"}.get(b.value, "?"), "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
+        return {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum", 5: "kron"}.get(b.value, "?"), "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
 
     def time_kmv_kernel(self, v: torch.Tensor, warmup: int = 3, reps: int = 20) -> float:
         """Average device time (ms) of ONE launch of the fused K.V kernel alone (CUDA events on the plan stream)."""
@@ -487,3 +487,47 @@ class Plan:
             import warnings
             warnings.warn(_lib.last_error(), _lib.NumericalWarning)
         return res, solve
+
+
+class KronPlan(Plan):
+    """The Kronecker multitask operator (s K_data) (x) B over interleaved rows i T + a (gp_plan_set_kron): N1 T x N2 T, built on a
+    ready data Plan (kept alive here).  set_noise supplies the noise; set_task_covar / task_covar_grad take B and its gradient,
+    bilinear_grad returns the data kernel's (lengthscale, outputscale) gradients.  Every product, solve and sample call of Plan
+    works on it."""
+
+    def __init__(self, data: Plan, num_tasks: int):
+        self.lib = data.lib
+        self.device = data.device
+        self._h = C.c_void_p()
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(self.lib.gp_plan_create(C.byref(self._h), self.device.index or 0, C.c_void_p(stream)))
+        self.comm = None
+        self.noise, self.outputscale = 0.0, 1.0
+        self.attach(data, num_tasks)
+
+    def attach(self, data: Plan, num_tasks: int):
+        """(Re-)attach the data plan: validation and geometry only; a B of the same size stays set."""
+        T = int(num_tasks)
+        self.data, self.num_tasks = data, T
+        self.same, self.d = data.same, data.d
+        self.n1, self.n2 = data.n1 * T, data.n2 * T
+        self.row_begin, self.row_count = 0, self.n1
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_kron(self._h, data._h, T))
+        return self
+
+    def refresh_data(self):
+        return self.attach(self.data, self.num_tasks)
+
+    def set_hypers(self, kind=None, lengthscale=None, outputscale: float = 1.0, noise: float = 0.0):
+        """Only the noise is this plan's own: kind and lengthscales are the data plan's."""
+        return self.set_noise(noise)
+
+    def set_noise(self, noise: float):
+        ls = list(self.data.lengthscale)
+        arr = (C.c_float * len(ls))(*ls)
+        self.kind, self.lengthscale, self.noise = self.data.kind, ls, float(noise)
+        self.outputscale = self.data.outputscale
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_hypers(self._h, KIND[self.kind], arr, len(ls), float(self.outputscale), float(noise)))
+        return self

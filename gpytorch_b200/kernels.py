@@ -266,6 +266,43 @@ class IndexKernel(Module):
     forward = __call__
 
 
+class MultitaskKernel(Kernel):
+    """Kronecker multitask kernel (kernels/multitask_kernel.py:13-61): K = K_data(x1, x2) (x) B over interleaved rows i T + a, B from
+    `task_covar_module` (an IndexKernel with the reference's covar_factor / raw_var).  `data_covar_module` is an RBFKernel /
+    MaternKernel, optionally inside a ScaleKernel; forward returns one engine KroneckerKernelLinearOperator (gp_plan_set_kron).
+    Unbatched, no prior."""
+
+    def __init__(self, data_covar_module, num_tasks, rank=1, task_covar_prior=None, **kwargs):
+        super().__init__(**kwargs)
+        if len(self.batch_shape):
+            raise NotImplementedError("a batched MultitaskKernel is not available on the accelerated path")
+        if task_covar_prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        self.task_covar_module = IndexKernel(num_tasks=num_tasks, batch_shape=self.batch_shape, rank=rank, prior=task_covar_prior)
+        self.data_covar_module = data_covar_module
+        self.num_tasks = num_tasks
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, last_dim_is_batch=False, **params):
+        if last_dim_is_batch:
+            raise RuntimeError("MultitaskKernel does not accept the last_dim_is_batch argument.")
+        if _batch_index is not None:
+            raise NotImplementedError("a batched MultitaskKernel is not available on the accelerated path")
+        dm = self.data_covar_module
+        base = dm.base_kernel if isinstance(dm, ScaleKernel) else dm
+        if not isinstance(base, _StationaryKernel) or len(dm.batch_shape):
+            raise NotImplementedError("the accelerated MultitaskKernel takes an RBFKernel / MaternKernel data kernel, optionally "
+                                      "inside a ScaleKernel")
+        covar_x = dm(x1, None if _same else x2)
+        from .operators import KroneckerKernelLinearOperator
+        op = KroneckerKernelLinearOperator(covar_x.x1, None if covar_x.same else covar_x.x2, covar_x.kind, covar_x.lengthscale,
+                                           covar_x.outputscale, self.task_covar_module.covar_matrix)
+        return op.diagonal() if diag else op
+
+    def num_outputs_per_input(self, x1, x2):
+        """An n x m data covariance becomes an (n T) x (m T) multitask covariance."""
+        return self.num_tasks
+
+
 class GridInterpolationKernel(Kernel):
     """SKI / KISS-GP (kernels/grid_interpolation_kernel.py:14-213): base_kernel(x, x') ~= w_x^T K_grid w_x' with cubic interpolation
     onto a regular grid; K_grid is a Kronecker product of per-dimension Toeplitz matrices (kernels/grid_kernel.py:107-177).

@@ -6,7 +6,7 @@ import warnings
 import torch
 
 from .constraints import GreaterThan
-from .distributions import MultivariateNormal
+from .distributions import MultitaskMultivariateNormal, MultivariateNormal
 from .module import Module
 from .operators import ConstantDiagLinearOperator, DiagLinearOperator
 
@@ -222,3 +222,73 @@ class FixedNoiseGaussianLikelihood(_GaussianLikelihoodBase):
             warnings.warn("You have passed data through a FixedNoiseGaussianLikelihood that did not match the size "
                           "of the fixed noise, *and* you did not specify noise. This is treated as a no-op.")
         return res
+
+
+class MultitaskGaussianLikelihood(_GaussianLikelihoodBase):
+    """likelihoods/multitask_gaussian_likelihood.py:162-301 with rank = 0: noise sigma^2 + sigma^2_a on row i T + a of the interleaved
+    covariance (:118-154), added through the per-row noise path (gp_plan_set_noise_diag).  `raw_task_noises` [T] and `raw_noise` [1]
+    with GreaterThan(1e-4), the reference's names and initialisation."""
+
+    def __init__(self, num_tasks, rank=0, batch_shape=torch.Size(), task_prior=None, noise_prior=None, noise_constraint=None,
+                 has_global_noise=True, has_task_noise=True, **kwargs):
+        super().__init__()
+        if noise_constraint is None:
+            noise_constraint = GreaterThan(1e-4)
+        if not has_task_noise and not has_global_noise:
+            raise ValueError("At least one of has_task_noise or has_global_noise must be specified. "
+                             "Attempting to specify a likelihood that has no noise terms.")
+        if rank != 0:
+            raise NotImplementedError("a task noise covariance of rank > 0 is not available on the accelerated path")
+        if noise_prior is not None or task_prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        if len(torch.Size(batch_shape)):
+            raise NotImplementedError("a batched MultitaskGaussianLikelihood is not available on the accelerated path")
+        if has_task_noise:
+            self.register_parameter("raw_task_noises", torch.nn.Parameter(torch.zeros(num_tasks)))
+            self.register_constraint("raw_task_noises", noise_constraint)
+        if has_global_noise:
+            self.register_parameter("raw_noise", torch.nn.Parameter(torch.zeros(1)))
+            self.register_constraint("raw_noise", noise_constraint)
+        self.num_tasks = num_tasks
+        self.rank = rank
+        self.has_global_noise = has_global_noise
+        self.has_task_noise = has_task_noise
+
+    @property
+    def noise(self):
+        return self.raw_noise_constraint.transform(self.raw_noise) if self.has_global_noise else None
+
+    @noise.setter
+    def noise(self, value):
+        self._set_constrained("raw_noise", value)
+
+    @property
+    def task_noises(self):
+        return self.raw_task_noises_constraint.transform(self.raw_task_noises) if self.has_task_noise else None
+
+    @task_noises.setter
+    def task_noises(self, value):
+        self._set_constrained("raw_task_noises", value)
+
+    def _task_noise_diag(self, n):
+        """[n T]: sigma^2 + sigma^2_a at row i T + a."""
+        per_task = None
+        if self.has_task_noise:
+            per_task = self.task_noises
+        if self.has_global_noise:
+            per_task = self.noise.expand(self.num_tasks) if per_task is None else per_task + self.noise
+        return per_task.repeat(n)
+
+    def _shaped_noise_covar(self, base_shape, *params, **kwargs):
+        n, T = base_shape[-2], base_shape[-1]
+        if T != self.num_tasks:
+            raise RuntimeError(f"the likelihood has {self.num_tasks} tasks, the function has {T}")
+        return DiagLinearOperator(self._task_noise_diag(n))
+
+    def marginal(self, function_dist, *params, **kwargs):
+        if not isinstance(function_dist, MultitaskMultivariateNormal):
+            raise RuntimeError("MultitaskGaussianLikelihood needs a MultitaskMultivariateNormal")
+        mean, covar = function_dist.mean, function_dist.lazy_covariance_matrix
+        noise_covar = self._shaped_noise_covar(mean.shape, *params, **kwargs)
+        full = covar + noise_covar.to_dense() if torch.is_tensor(covar) else covar + noise_covar
+        return MultitaskMultivariateNormal(mean, full)

@@ -1,5 +1,7 @@
 """Mean functions (gpytorch/means/constant_mean.py:33-113, zero_mean.py).  Parameter names and shapes follow the
 reference (`raw_constant` of shape batch_shape) so that state dicts are interchangeable."""
+from copy import deepcopy
+
 import torch
 
 from .module import Module
@@ -50,3 +52,24 @@ class ConstantMean(Module):
 
     def __call__(self, x):
         return self.forward(x)
+
+
+class MultitaskMean(Module):
+    """means/multitask_mean.py:20-45: one mean per task (a single mean is deep-copied T times); forward returns [n, T]."""
+
+    def __init__(self, base_means, num_tasks):
+        super().__init__()
+        if isinstance(base_means, Module):
+            base_means = [base_means]
+        if not isinstance(base_means, list) or (len(base_means) != 1 and len(base_means) != num_tasks):
+            raise RuntimeError("base_means should be a list of means of length either 1 or num_tasks")
+        if len(base_means) == 1:
+            base_means = base_means + [deepcopy(base_means[0]) for _ in range(num_tasks - 1)]
+        self.base_means = torch.nn.ModuleList(base_means)
+        self.num_tasks = num_tasks
+
+    def forward(self, input):
+        return torch.cat([sub_mean(input).unsqueeze(-1) for sub_mean in self.base_means], dim=-1)
+
+    def __call__(self, input):
+        return self.forward(input)

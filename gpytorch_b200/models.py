@@ -4,7 +4,7 @@ grid caches of InterpolatedPredictionStrategy (:481-827) behind settings.ski_gri
 import torch
 
 from . import settings
-from .distributions import MultivariateNormal
+from .distributions import MultitaskMultivariateNormal, MultivariateNormal
 from .likelihoods import _GaussianLikelihoodBase
 from .module import Module
 from .operators import LOWRANK_MAX_RANK, LowRankUpdatedKernelLinearOperator, SKIKernelLinearOperator
@@ -89,7 +89,7 @@ class ExactGP(Module):
             init = None
             if settings.probe_seed.value() is not None:
                 g = torch.Generator(device="cpu").manual_seed(int(settings.probe_seed.value()))
-                init = torch.randn(train_x.size(-2), generator=g).to(train_x.device)
+                init = torch.randn(khat.shape[-1], generator=g).to(train_x.device)   # n (n T rows for a multitask model)
             self._covar_cache = khat.root_inv_decomposition(init).detach()
         return self._covar_cache
 
@@ -129,15 +129,30 @@ class ExactGP(Module):
             full_out = self.forward(torch.cat([train_x, test_x], dim=-2))
             lik_params = ()
         full_mean, full_covar = full_out.mean, full_out.lazy_covariance_matrix
+        # a Kronecker multitask model (MultitaskMultivariateNormal): every covariance block is over the interleaved rows i T + a,
+        # so the joint operator is sliced at n T and the means are [n, T] (flattened row-major for the solves)
+        multitask = isinstance(train_out, MultitaskMultivariateNormal)
         with settings._use_eval_tolerance(True):
             khat = self.likelihood(train_out, *lik_params).lazy_covariance_matrix
-            if self._mean_cache is None:
-                resid = (self.train_targets - train_out.mean).unsqueeze(-1)
-                self._mean_cache = khat.solve(resid).squeeze(-1)  # exact_prediction_strategies.py:286
-            k_star = full_covar[n:, :n]                           # K(test, train)
-            k_ss = full_covar[n:, n:]
-            test_mean = full_mean[..., n:] + k_star.matmul(self._mean_cache)  # :396
-            m = test_x.size(-2)
+            if multitask:
+                T = train_out.num_tasks
+                n_rows = n * T
+                if self._mean_cache is None:
+                    resid = (self.train_targets - train_out.mean).reshape(-1, 1)
+                    self._mean_cache = khat.solve(resid).squeeze(-1)
+                k_star = full_covar[n_rows:, :n_rows]
+                k_ss = full_covar[n_rows:, n_rows:]
+                test_mean = (full_mean[n:].reshape(-1) + k_star.matmul(self._mean_cache)).reshape(-1, T)
+                m = test_x.size(-2) * T
+            else:
+                n_rows = n
+                if self._mean_cache is None:
+                    resid = (self.train_targets - train_out.mean).unsqueeze(-1)
+                    self._mean_cache = khat.solve(resid).squeeze(-1)  # exact_prediction_strategies.py:286
+                k_star = full_covar[n:, :n]                           # K(test, train)
+                k_ss = full_covar[n:, n:]
+                test_mean = full_mean[..., n:] + k_star.matmul(self._mean_cache)  # :396
+                m = test_x.size(-2)
             mode = _posterior_covar_mode(k_ss)
             if mode == "skip":                               # exact_prediction_strategies.py:432-433
                 covar = torch.zeros(m, m, device=test_x.device)
@@ -148,9 +163,11 @@ class ExactGP(Module):
                 else:
                     covar = _dense(k_ss) - root @ root.transpose(-1, -2)
             else:
-                rhs = _dense(full_covar[:n, n:])         # K(train, test) [n, m]
-                corr = k_star.matmul(khat.solve(rhs))    # exact predictive covariance, :435-462
+                rhs = _dense(full_covar[:n_rows, n_rows:])   # K(train, test) [n, m]
+                corr = k_star.matmul(khat.solve(rhs))        # exact predictive covariance, :435-462
                 covar = _dense(k_ss) - corr
+        if multitask:
+            return MultitaskMultivariateNormal(test_mean, covar)
         return MultivariateNormal(test_mean, covar)
 
     def _ski_grid_posterior(self, train_x, test_x, train_out, test_out, mode):

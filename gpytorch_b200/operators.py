@@ -20,7 +20,7 @@ import torch
 
 from . import settings
 from ._lib import NanError
-from .engine import Plan
+from .engine import KronPlan, Plan
 from .sampling import contour_quadrature, psd_safe_cholesky
 
 
@@ -83,6 +83,8 @@ def clear_plan_cache():
     with _PLAN_LOCK:
         while _SUM_PLANS:
             _SUM_PLANS.popitem()[1].close()
+        while _KRON_PLANS:
+            _KRON_PLANS.popitem()[1].close()
         while _PLAN_CACHE:
             _PLAN_CACHE.popitem()[1].close()
 
@@ -596,6 +598,150 @@ class HadamardKernelLinearOperator(KernelLinearOperator):
         raise NotImplementedError("a Hadamard multitask operator adds a (Constant)DiagLinearOperator only")
 
 
+_KRON_SLOT = 24   # plan-cache slot of the data plans of Kronecker operators
+
+
+def _aligned(ix, T: int, n: int):
+    """The point slice of a row / column slice of a Kronecker operator that starts and stops on multiples of T (None otherwise)."""
+    if not isinstance(ix, slice) or ix.step not in (None, 1):
+        return None
+    a, b, _ = ix.indices(n * T)
+    if a % T or b % T or b < a:
+        return None
+    return slice(a // T, b // T)
+
+
+class KroneckerKernelLinearOperator(KernelLinearOperator):
+    """(s K(x1, x2)) (x) B over interleaved rows i T + a (MultitaskKernel, kernels/multitask_kernel.py:13-61; the reference returns
+    KroneckerProductLinearOperator(covar_x, covar_i)): ONE engine operator (gp_plan_set_kron) on the plan of the data kernel.  The
+    hyper-parameters are lengthscale, outputscale and B; B's gradient comes from gp_task_covar_grad and autograd carries it to the
+    IndexKernel's covar_factor / raw_var.  Input gradients are not available: inputs that require grad are refused."""
+
+    def __init__(self, x1, x2, kind, lengthscale, outputscale, B):
+        if x1.requires_grad or (x2 is not None and x2.requires_grad):
+            raise RuntimeError("gradients with respect to the inputs of a Kronecker multitask operator (K (x) B) are not implemented: "
+                               "pass inputs that do not require grad")
+        super().__init__(x1, x2, kind, lengthscale, outputscale)
+        if B.dim() != 2 or B.shape[0] != B.shape[1] or not 1 <= B.shape[0] <= 32:
+            raise RuntimeError(f"the task covariance must be [T, T] with 1 <= T <= 32 (got {tuple(B.shape)})")
+        self.B = B
+        self.num_tasks = int(B.shape[-1])
+        self._data_op = KernelLinearOperator(x1, x2, kind, lengthscale, outputscale)
+        self._data_op._plan_slot = _KRON_SLOT
+
+    @property
+    def shape(self):
+        n2 = self.x1.size(0) if self.same else self.x2.size(0)
+        return torch.Size([self.x1.size(0) * self.num_tasks, n2 * self.num_tasks])
+
+    def plan(self, noise=0.0) -> Plan:
+        data = self._data_op.plan(0.0)
+        if getattr(data, "_noise_diag", None) is not None:
+            data.set_noise_diag(None)
+        nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
+        T = self.num_tasks
+        with _PLAN_LOCK:
+            key = (id(data), T)
+            parent = _KRON_PLANS.pop(key, None)
+            if parent is None:
+                parent = KronPlan(data, T)
+                parent._hyp_key = None
+                parent._b_key = None
+            _KRON_PLANS[key] = parent
+            while len(_KRON_PLANS) > 16:
+                _KRON_PLANS.pop(next(iter(_KRON_PLANS))).close()
+        # the data plan may have been re-packed or re-pointed since the last use: re-attach it (validation, no allocation)
+        parent.attach(data, T)
+        hk = (nz, data.kind, tuple(data.lengthscale), data.outputscale)
+        if parent._hyp_key != hk:
+            parent.set_noise(nz)
+            parent._hyp_key = hk
+        bh = getattr(self, "_b_host", None)
+        if bh is None:
+            bh = self._b_host = self.B.detach().float().cpu()
+        if parent._b_key is None or not torch.equal(parent._b_key, bh):
+            parent.set_task_covar(bh)
+            parent._b_key = bh
+        self._plan = parent
+        return parent
+
+    @property
+    def requires_grad(self):
+        return bool(super().requires_grad or self.B.requires_grad)
+
+    def representation(self):
+        return (self.x1, self.x2, self.lengthscale, self.outputscale, self.B)
+
+    def hyper_tensors(self):
+        return [self.lengthscale, self.outputscale, self.B]
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    def _bilinear_derivative_list(self, left, right):
+        p = self.plan(getattr(self, "_last_noise", 0.0))
+        gl, go = p.bilinear_grad(left, right)
+        dB = p.task_covar_grad(left, right)
+        return [torch.tensor(gl, device=self.device, dtype=self.dtype).reshape(self.lengthscale.shape),
+                torch.tensor(go, device=self.device, dtype=self.dtype).reshape(self.outputscale.shape),
+                dB.to(device=self.device, dtype=self.B.dtype)]
+
+    def _bilinear_derivative(self, left, right):
+        gl, go, _ = self._bilinear_derivative_list(left, right)
+        return gl, go
+
+    def _transpose_nonbatch(self):
+        if self.same:
+            return self
+        return KroneckerKernelLinearOperator(self.x2, self.x1, self.kind, self.lengthscale, self.outputscale, self.B.transpose(-1, -2))
+
+    def detach(self):
+        return KroneckerKernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.kind,
+                                             self.lengthscale.detach(), self.outputscale.detach(), self.B.detach())
+
+    def to_dense(self):
+        return _KernelDense.apply(self)
+
+    def diagonal(self, dim1=-2, dim2=-1):
+        """s k(x1_i, x2_i) B[a, a] at row i T + a."""
+        if self.shape[0] != self.shape[1]:
+            raise RuntimeError(f"diagonal of a non-square operator {tuple(self.shape)} is undefined")
+        return self.plan().diag()
+
+    _diagonal = diagonal
+
+    def __getitem__(self, index):
+        """Slices that start and stop on multiples of T re-index x1 / x2 (prediction slices the joint operator at n T)."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        T = self.num_tasks
+        x2 = self.x1 if self.same else self.x2
+        rs, cs = _aligned(ri, T, self.x1.size(0)), _aligned(ci, T, x2.size(0))
+        if rs is None or cs is None:
+            raise NotImplementedError("a Kronecker multitask operator takes row / column slices that start and stop on multiples of "
+                                      "the number of tasks")
+        return KroneckerKernelLinearOperator(self.x1[rs], x2[cs], self.kind, self.lengthscale, self.outputscale, self.B)
+
+    def mul(self, other):
+        raise NotImplementedError("a Kronecker multitask operator takes one task covariance")
+
+    __mul__ = mul
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("a Kronecker multitask operator adds a (Constant)DiagLinearOperator only")
+
+
+_KRON_PLANS: "dict[tuple, Plan]" = {}
+
+
 class SumKernelLinearOperator(KernelLinearOperator):
     """K_1 + ... + K_m over the same inputs (AdditiveKernel, kernels/kernel.py:592-621).  The reference evaluates every term
     densely and adds the matrices; here the sum is ONE engine operator (gp_plan_set_sum): a product launches the fused kernel of
@@ -924,7 +1070,8 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
     @staticmethod
     def supports(base) -> bool:
         """A plan-backed non-SKI kernel operator (or kernel sum) without batch dimension on an unsharded square plan."""
-        return (isinstance(base, KernelLinearOperator) and not isinstance(base, (SKIKernelLinearOperator, HadamardKernelLinearOperator))
+        return (isinstance(base, KernelLinearOperator) and not isinstance(base, (SKIKernelLinearOperator, HadamardKernelLinearOperator,
+                                                                                          KroneckerKernelLinearOperator))
                 and base.same
                 and base._comm is None and base._row_begin == 0 and base._row_count in (0, base.shape[0]))
 

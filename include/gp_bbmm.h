@@ -47,7 +47,7 @@ enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3 };
  * (the name is historical),
  * GP_BACKEND_SIMT = fp32 CUDA-core kernel (bring-up / cross-check / d > 41). */
 enum { GP_BACKEND_AUTO = 0, GP_BACKEND_TCGEN05 = 1, GP_BACKEND_SIMT = 2, GP_BACKEND_SKI = 3 /* set by gp_plan_set_ski */,
-       GP_BACKEND_SUM = 4 /* set by gp_plan_set_sum */ };
+       GP_BACKEND_SUM = 4 /* set by gp_plan_set_sum */, GP_BACKEND_KRON = 5 /* set by gp_plan_set_kron */ };
 
 typedef struct gp_plan gp_plan;   /* opaque: repacked X, workspaces, stream, comm */
 typedef struct gp_comm gp_comm;   /* opaque: NCCL communicator for row-sharded runs */
@@ -156,6 +156,21 @@ int gp_plan_set_lowrank(gp_plan* plan, const float* U, int64_t ldu, int r);
 int gp_plan_set_tasks(gp_plan* plan, const int32_t* task1, const int32_t* task2, int T);
 int gp_plan_set_task_covar(gp_plan* plan, const float* B, int T);
 int gp_task_covar_grad(gp_plan* plan, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB);
+
+/* Kronecker multitask GPs (MultitaskKernel, kernels/multitask_kernel.py:13-61, with every input observed for every task as in
+ * examples/03_Multitask_Exact_GPs/Multitask_GP_Regression.ipynb): `plan` becomes the N1 T x N2 T operator
+ *     (s K_data) (x) B   over interleaved rows i T + a (point i, task a)   (+ its noise / per-row diagonal where a call adds it),
+ * where K_data is `data`'s operator.  `data` is a ready plain plan (tensor-core or SIMT, any kind, scalar or ARD lengthscale,
+ * square or cross) on the same device and stream, caller-owned, and must outlive `plan`; re-packing it (gp_plan_set_hypers) is
+ * picked up by the next call on `plan`.  data = NULL clears the operator.  1 <= T <= 32.  gp_plan_set_hypers on `plan` supplies the
+ * noise only (as on a kernel sum); gp_plan_set_noise_diag takes N T entries.  B comes through gp_plan_set_task_covar(plan, B, T)
+ * and its gradient through gp_task_covar_grad; gp_bilinear_grad on `plan` returns the gradients of data's lengthscale(s) and
+ * outputscale.  One K.V of [N T, t] columns is ceil(T t / 16) launches of data's fused kernel on the B-mixed blocks
+ * W[j, a t + c] = sum_b B[a, b] V[j T + b, c]: no atomics, repeated calls agree bit for bit.  gp_kmv, gp_krows, gp_kdiag,
+ * gp_pivoted_cholesky, the preconditioner calls, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos and gp_ciq_* run on it.
+ * GP_E_STATE / GP_E_SHAPE: a SKI, kernel-sum, multitask, low-rank-corrected or row-sharded data plan; gp_plan_set_comm with more
+ * than one rank, gp_plan_set_lowrank, gp_plan_set_tasks and the input gradients on `plan`. */
+int gp_plan_set_kron(gp_plan* plan, gp_plan* data, int T);
 
 /* ---- kernel seam (LazyEvaluatedKernelTensor, lazy/lazy_evaluated_kernel_tensor.py) --- */
 
