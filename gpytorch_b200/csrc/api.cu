@@ -104,7 +104,8 @@ extern "C" int gp_plan_destroy(gp_plan* p) {
   for (auto* b : bufs) b->release();
   if (p->ski) {
     gp::DevBuf* sb[] = {&p->ski->first, &p->ski->wts, &p->ski->gridA, &p->ski->gridB, &p->ski->gridC, &p->ski->gridD, &p->ski->T, &p->ski->dT, &p->ski->flag,
-                        &p->ski->perm, &p->ski->tile_off, &p->ski->tile_cnt, &p->ski->first_s, &p->ski->wts_s};
+                        &p->ski->perm, &p->ski->tile_off, &p->ski->tile_cnt, &p->ski->first_s, &p->ski->wts_s,
+                        &p->ski->tcol, &p->ski->dtcol, &p->ski->band};
     for (auto* b : sb) b->release();
     delete p->ski;
   }

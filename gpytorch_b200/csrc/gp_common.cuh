@@ -139,6 +139,7 @@ struct gp_ski_state {
   int tile_edge[4] = {0, 0, 0, 0}, tile_num[4] = {0, 0, 0, 0}, ntiles = 0;   // spatial buckets of the points (ski.cu)
   gp::DevBuf first, wts, gridA, gridB, gridC, gridD, T, dT, flag;
   gp::DevBuf perm, tile_off, tile_cnt, first_s, wts_s;                        // points sorted by tile + the permutation back
+  gp::DevBuf tcol, dtcol, band;   // generating columns t_i, l dt_i/dl (sum_i G_i floats each) and their band ends (8 ints)
 };
 
 // Hadamard multitask state (tasks.cu): the operator is s K o B[t, t'].  Rows are sorted by task (stable), the columns of task b

@@ -187,7 +187,7 @@ constexpr int PCP_RED = 512;
 // kernel sums (GP_BACKEND_SUM): K[pivot, j] = sum_t os_t k_t(|z_t,pivot - z_t,j|^2), every term with its own packed inputs
 constexpr int PC_KIND_SUM = 64;
 // SKI (GP_BACKEND_SKI): K[pivot, j] = s prod_k w_jk^T u_k[f_jk : f_jk + 4] with u of the pivot staged where the pivot row of Z sits
-// (ski_rows.cuh); DP = sum_k G_k
+// (ski_rows.cuh); DP = sum_k G_k (0 on grids too large to stage u: the entries form it from the pivot's interpolation data)
 constexpr int PC_KIND_SKI = 65;
 // multitask (tasks.cu, kron.cu): K[r, r'] = s B[task(r), task(r')] k(|z_point(r) - z_point(r')|^2), covariance kind kind[0]; row r is
 // point r / rep, task task[r] (Hadamard: rep = 1, task ids) or point r / T, task r mod T (Kronecker: rep = T, task = nullptr)
@@ -292,7 +292,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             off += tt.DP[t];
           }
         } else if (KIND == PC_KIND_SKI) {
-          v = ski_entry(sk, zp, j);
+          v = ski_entry(sk, zp, pi, j);
         } else if (KIND == PC_KIND_TASK) {
           const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
           float s = 0.f;
@@ -814,7 +814,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     p->launches += 2;
   } else if (ski) {
     GP_CHECK(ski_rows_args(p, &sk));
-    dp_total = sk.usum;   // the pivot's u_k take the place of its packed inputs in shared memory
+    dp_total = sk.staged ? sk.usum : 0;   // the pivot's u_k take the place of its packed inputs in shared memory (staged grids)
     pc_init_ski_kernel<<<gb, PC_THREADS, 0, st>>>(sk, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;

@@ -13,8 +13,10 @@
 // node, so that a CTA works on the (E + 3)^d grid nodes of one tile in shared memory.  A product is three passes:
 //   scatter  U  = W^T V           per tile: shared-memory accumulation, then one red.global.add.v4.f32 per touched node into the
 //                                 [M][16] grid block (M = prod G_i; 64 MB at 100^3)
-//   modes    U' = (T_0 x ... x T_{d-1}) U   one dense [G x G] product per dimension (the Toeplitz structure saves nothing at
-//                                 G = 100: an FFT of length 2G-2 costs as many flops as the direct product)
+//   modes    U' = (T_0 x ... x T_{d-1}) U   one [G x G] product per dimension on the tensor cores: from the dense factor at
+//                                 G <= 128 (the Toeplitz structure saves nothing at G = 100: an FFT of length 2G-2 costs as many
+//                                 flops as the direct product), from the factor's generating column t[|a - b|] above, skipping the
+//                                 k-chunks where t is exactly zero (O(G band) instead of O(G^2))
 //   gather   out = W U'           per tile: node block staged in shared memory, 4^d reads per (row, column group) from there,
 //                                 written as the K.V partial block the mBCG finish kernels read (outputscale / noise applied there)
 // and the bilinear derivative (hyper-parameter gradients) is d + 1 sweeps of the mode products between two scatters and a dot.
@@ -33,6 +35,8 @@
 namespace gp {
 
 constexpr int SKI_MAXD = 4;
+constexpr int SKI_DENSE_G = 128;       // largest grid dimension whose mode product stages its dense factor (ski_mode_kernel)
+constexpr int SKI_MAX_G = 131072;      // largest grid dimension (ski_mode_banded_kernel above SKI_DENSE_G)
 
 struct SkiGeom {
   int d;
@@ -517,13 +521,134 @@ ski_mode_kernel(const float* __restrict__ T, int G, const float* __restrict__ in
   }
 }
 
+// Mode product for G > 128 (ski_mode_kernel stages the whole G x G factor, which stops fitting in shared memory there), same
+// contract and the same 3xTF32 split on mma.sync.m16n8k8.  T is Toeplitz, T[i][k] = t[|i - k|], and is never stored: a work item
+// is (64-position slab, block of SKI_BR output rows), and it loops over the k rows of the mode in chunks of SKI_KC.  Per chunk the
+// CTA stages the slab's SKI_KC input rows (split into tf32 hi / lo, as the dense kernel) and the generating window
+// w[e] = t[|r0 - k0 - (SKI_KC - 1) + e|], e < SKI_BR + SKI_KC - 1, that holds every entry of the (rows, chunk) tile:
+// T[r0 + a][k0 + c] = w[a - c + SKI_KC - 1].  Shared memory is 20 KB whatever G.  Chunks where the tile's entries are all exactly
+// 0.0f are skipped: entries at |i - k| >= band are zero (ski_toeplitz_col_kernel writes band on the device), so only chunks that
+// meet [r0 - band + 1, r1 + band - 1) run, and a product costs O(G band) per position instead of O(G^2).  Dropping exact zeros
+// changes only which zero terms enter the fp32 accumulation.  The next chunk's input rows are loaded into registers while the
+// tensor cores work on the current one.
+constexpr int SKI_BR = 128;                 // output rows per work item: 4 warp pairs x 32 rows
+constexpr int SKI_KC = 32;                  // k rows per chunk: 4 k-steps of 8
+constexpr int SKI_WIN = SKI_BR + SKI_KC;    // staged generating window (SKI_BR + SKI_KC - 1 entries used)
+__global__ void __launch_bounds__(256, 2)
+ski_mode_banded_kernel(const float* __restrict__ t, const int* __restrict__ band, int G, const float* __restrict__ in,
+                       float* __restrict__ out, int64_t inner, int64_t total, int64_t nslab) {
+  __shared__ __align__(16) uint32_t Bh[SKI_KC * SKI_BP];
+  __shared__ __align__(16) uint32_t Bl[SKI_KC * SKI_BP];
+  __shared__ uint32_t Wh[SKI_WIN], Wl[SKI_WIN];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int gr = lane >> 2, gc = lane & 3;      // fragment coordinates
+  const int nh = warp & 1, mp = warp >> 1;      // warp tile: half nh of the slab's 64 positions, rows mp * 32 .. + 32 of the block
+  const int j4 = tid & 15, kst = tid >> 4;      // staging: this thread's float4 column of the slab, k rows kst and kst + 16
+  const uint32_t inner32 = (uint32_t)inner, total32 = (uint32_t)total;   // the host checks total < 2^31
+  const int bw = *band;
+  const int nrb = (G + SKI_BR - 1) / SKI_BR;
+  for (int64_t wk = blockIdx.x; wk < nslab * nrb; wk += gridDim.x) {
+    const int64_t slab = wk / nrb;               // the row blocks of one slab are neighbours: they share input rows in L2
+    const int r0 = (int)(wk - slab * nrb) * SKI_BR;
+    const int r1 = min(G, r0 + SKI_BR);
+    const uint32_t q0 = (uint32_t)slab * SKI_MT;
+    const int klo = max(0, r0 - bw + 1), khi = bw > 0 ? min(G, r1 + bw - 1) : 0;   // empty when t is all zero
+    // 4 consecutive positions share o (inner is a multiple of 16): one division per thread and work item
+    const uint32_t qs = q0 + (uint32_t)j4 * 4;
+    const bool live = qs < total32;
+    const uint32_t os = live ? qs / inner32 : 0u, xs = live ? qs - os * inner32 : 0u;
+    const float* src = in + ((size_t)os * G) * inner + xs;
+    auto load = [&](int k0, float4 (&v)[2]) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int k = k0 + kst + 16 * h;
+        v[h] = (live && k < G) ? *reinterpret_cast<const float4*>(src + (size_t)k * inner) : make_float4(0, 0, 0, 0);
+      }
+    };
+    // warp-uniform: this warp's positions or rows lie entirely outside the operand (d = 1 has 16 positions; the last row block)
+    const bool work = q0 + (uint32_t)nh * 32 < total32 && r0 + mp * 32 < G;
+    float acc[2][4][4];
+#pragma unroll
+    for (int m = 0; m < 2; ++m)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[m][nt][j] = 0.f;
+    const int kfirst = klo / SKI_KC * SKI_KC;
+    float4 pf[2];
+    if (kfirst < khi) load(kfirst, pf);
+    for (int k0 = kfirst; k0 < khi; k0 += SKI_KC) {
+      __syncthreads();                           // the previous chunk's fragments have been read
+      for (int e = tid; e < SKI_WIN - 1; e += 256) {
+        const int dl = abs(r0 - k0 - (SKI_KC - 1) + e);
+        const float v = dl < G ? t[dl] : 0.f;    // dl >= G only pairs a padding row with a padding k (B rows k >= G are zero)
+        const uint32_t h = tf32_rna(v);
+        Wh[e] = h;
+        Wl[e] = tf32_rna(v - __uint_as_float(h));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float4 v = pf[h];
+        uint4 hi, lo;
+        hi.x = tf32_rna(v.x); hi.y = tf32_rna(v.y); hi.z = tf32_rna(v.z); hi.w = tf32_rna(v.w);
+        lo.x = tf32_rna(v.x - __uint_as_float(hi.x)); lo.y = tf32_rna(v.y - __uint_as_float(hi.y));
+        lo.z = tf32_rna(v.z - __uint_as_float(hi.z)); lo.w = tf32_rna(v.w - __uint_as_float(hi.w));
+        *reinterpret_cast<uint4*>(&Bh[(kst + 16 * h) * SKI_BP + j4 * 4]) = hi;
+        *reinterpret_cast<uint4*>(&Bl[(kst + 16 * h) * SKI_BP + j4 * 4]) = lo;
+      }
+      __syncthreads();
+      if (k0 + SKI_KC < khi) load(k0 + SKI_KC, pf);   // in flight during the MMAs below
+      if (!work) continue;
+#pragma unroll
+      for (int ks = 0; ks < SKI_KC / 8; ++ks) {
+        uint32_t ah[2][4], al[2][4];
+#pragma unroll
+        for (int m = 0; m < 2; ++m) {
+          // A fragment (rows gr, gr + 8; columns gc, gc + 4 of the 16 x 8 tile) from the window: lanes read 11 consecutive words
+          const int e = mp * 32 + m * 16 + gr - ks * 8 - gc + SKI_KC - 1;
+          const int ei[4] = {e, e + 8, e - 4, e + 4};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) { ah[m][j] = Wh[ei[j]]; al[m][j] = Wl[ei[j]]; }
+        }
+        const uint32_t* bh = Bh + (size_t)(ks * 8 + gc) * SKI_BP + nh * 32 + gr;
+        const uint32_t* bl = Bl + (size_t)(ks * 8 + gc) * SKI_BP + nh * 32 + gr;
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          if (q0 + (uint32_t)(nh * 32 + nt * 8) < total32) {   // warp-uniform: position tiles past the operand are left out
+            const uint32_t bh0 = bh[nt * 8], bh1 = bh[nt * 8 + 4 * SKI_BP], bl0 = bl[nt * 8], bl1 = bl[nt * 8 + 4 * SKI_BP];
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {
+              mma_tf32_16x8x8(acc[m][nt], al[m], bh0, bh1);   // small terms first
+              mma_tf32_16x8x8(acc[m][nt], ah[m], bl0, bl1);
+              mma_tf32_16x8x8(acc[m][nt], ah[m], bh0, bh1);
+            }
+          }
+        }
+      }
+    }
+    // every row of the block is written, those whose chunks were all skipped with 0
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt) {
+        const uint32_t q = q0 + (uint32_t)(nh * 32 + nt * 8 + 2 * gc);
+        if (q < total32) {
+          const uint32_t o = q / inner32, x = q - o * inner32;
+          const int r = r0 + mp * 32 + m * 16 + gr;
+          float* dst = out + ((size_t)o * G + r) * inner + x;
+          if (r < G) *reinterpret_cast<float2*>(dst) = make_float2(acc[m][nt][0], acc[m][nt][1]);
+          if (r + 8 < G) *reinterpret_cast<float2*>(dst + 8 * (size_t)inner) = make_float2(acc[m][nt][2], acc[m][nt][3]);
+        }
+      }
+    }
+  }
+}
+
 // T_i[a][b] = k_1d(|a - b| step_i / l_i): per-dimension factor of the grid covariance (grid_kernel.py:138-157 evaluates the base
-// kernel on every dimension separately, last_dim_is_batch=True)
-__global__ void ski_toeplitz_kernel(float* __restrict__ T, int G, float step, float inv_ls, int kind, int deriv) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= G * G) return;
-  const int a = e / G, b = e % G;
-  const float r = fabsf((float)(a - b)) * step * inv_ls;   // |dx| / l
+// kernel on every dimension separately, last_dim_is_batch=True).  The dense factor (G <= 128, read by ski_mode_kernel) and the
+// generating column (every G) evaluate this one expression, so t[k] == T[a][b] bit for bit for |a - b| = k.
+__device__ __forceinline__ float ski_toeplitz_entry(int diff, float step, float inv_ls, int kind, int deriv) {
+  const float r = fabsf((float)diff) * step * inv_ls;      // |dx| / l
   float v;
   if (kind == GP_RBF) {
     v = expf(-0.5f * r * r);
@@ -535,7 +660,36 @@ __global__ void ski_toeplitz_kernel(float* __restrict__ T, int G, float step, fl
     if (!deriv) v = (kind == GP_MATERN12) ? ex : (kind == GP_MATERN32 ? (1.f + rho) * ex : (1.f + rho + rho * rho * (1.f / 3.f)) * ex);
     else        v = (kind == GP_MATERN12) ? rho * ex : (kind == GP_MATERN32 ? rho * rho * ex : (1.f + rho) * rho * rho * (1.f / 3.f) * ex);
   }                                                        // l dk/dl = -rho dk/drho  (functions/matern_covariance.py:27-56)
-  T[e] = v;
+  return v;
+}
+
+__global__ void ski_toeplitz_kernel(float* __restrict__ T, int G, float step, float inv_ls, int kind, int deriv) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= G * G) return;
+  const int a = e / G, b = e % G;
+  T[e] = ski_toeplitz_entry(a - b, step, inv_ls, kind, deriv);
+}
+
+// Generating columns t[k] = T[k][0] and dt[k] = l dT[k][0]/dl, k < G, and their band ends: band[0] = 1 + the last k with t[k] != 0
+// (0 if none; a NaN counts as non-zero), band[1] the same for dt.  Every entry of T at |a - b| >= band[0] is exactly 0.0f, which
+// is what lets ski_mode_banded_kernel skip its k-chunks.  band must be zero before the launch (atomicMax of a fixed set of
+// values: the result does not depend on the order).
+__global__ void __launch_bounds__(256)
+ski_toeplitz_col_kernel(float* __restrict__ t, float* __restrict__ dt, int G, float step, float inv_ls, int kind, int* __restrict__ band) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  float v = 0.f, dv = 0.f;
+  if (k < G) {
+    v = ski_toeplitz_entry(k, step, inv_ls, kind, 0);
+    dv = ski_toeplitz_entry(k, step, inv_ls, kind, 1);
+    t[k] = v;
+    dt[k] = dv;
+  }
+  const unsigned e0 = __reduce_max_sync(0xffffffffu, (k < G && !(v == 0.f)) ? (unsigned)k + 1u : 0u);
+  const unsigned e1 = __reduce_max_sync(0xffffffffu, (k < G && !(dv == 0.f)) ? (unsigned)k + 1u : 0u);
+  if ((threadIdx.x & 31) == 0) {
+    if (e0) atomicMax(band, (int)e0);
+    if (e1) atomicMax(band + 1, (int)e1);
+  }
 }
 
 // <a, b> over n floats -> one fp64 partial per CTA (fixed order inside the CTA and on the host: reproducible)
@@ -682,17 +836,32 @@ int ski_pack(gp_plan* p) {
   ski_interp_kernel<<<(unsigned)cdiv(n, 256), 256, 0, st>>>(p->X1, n, p->ld1, g, s->first.as<int>(), s->wts.as<float>(), s->flag.as<int>());
   p->launches++;
   GP_CHECK(ski_bucket_points(p, g));
-  size_t toff = 0;
-  for (int i = 0; i < d; ++i) toff += (size_t)s->G[i] * s->G[i];
+  // dense factors for the dimensions ski_mode_kernel runs (G <= SKI_DENSE_G), generating columns and band ends for every dimension
+  size_t toff = 0, coff = 0;
+  for (int i = 0; i < d; ++i) {
+    if (s->G[i] <= SKI_DENSE_G) toff += (size_t)s->G[i] * s->G[i];
+    coff += (size_t)s->G[i];
+  }
   GP_CHECK(s->T.ensure(sizeof(float) * toff));
   GP_CHECK(s->dT.ensure(sizeof(float) * toff));   // l_i dT_i/dl_i: the factors of the hyper-parameter gradients
+  GP_CHECK(s->tcol.ensure(sizeof(float) * coff));
+  GP_CHECK(s->dtcol.ensure(sizeof(float) * coff));
+  GP_CHECK(s->band.ensure(sizeof(int) * 2 * SKI_MAXD));
+  GP_CUDA(cudaMemsetAsync(s->band.p, 0, sizeof(int) * 2 * SKI_MAXD, st));
   toff = 0;
+  coff = 0;
   for (int i = 0; i < d; ++i) {
     const float l = (p->ls.size() == 1) ? p->ls[0] : p->ls[i];
-    ski_toeplitz_kernel<<<(unsigned)cdiv((int64_t)s->G[i] * s->G[i], 256), 256, 0, st>>>(s->T.as<float>() + toff, s->G[i], s->step[i], 1.f / l, p->kind, 0);
-    ski_toeplitz_kernel<<<(unsigned)cdiv((int64_t)s->G[i] * s->G[i], 256), 256, 0, st>>>(s->dT.as<float>() + toff, s->G[i], s->step[i], 1.f / l, p->kind, 1);
-    p->launches += 2;
-    toff += (size_t)s->G[i] * s->G[i];
+    if (s->G[i] <= SKI_DENSE_G) {
+      ski_toeplitz_kernel<<<(unsigned)cdiv((int64_t)s->G[i] * s->G[i], 256), 256, 0, st>>>(s->T.as<float>() + toff, s->G[i], s->step[i], 1.f / l, p->kind, 0);
+      ski_toeplitz_kernel<<<(unsigned)cdiv((int64_t)s->G[i] * s->G[i], 256), 256, 0, st>>>(s->dT.as<float>() + toff, s->G[i], s->step[i], 1.f / l, p->kind, 1);
+      p->launches += 2;
+      toff += (size_t)s->G[i] * s->G[i];
+    }
+    ski_toeplitz_col_kernel<<<(unsigned)cdiv(s->G[i], 256), 256, 0, st>>>(s->tcol.as<float>() + coff, s->dtcol.as<float>() + coff, s->G[i],
+                                                                         s->step[i], 1.f / l, p->kind, s->band.as<int>() + 2 * i);
+    p->launches++;
+    coff += (size_t)s->G[i];
   }
   int h_oob = 0;
   GP_CUDA(cudaMemcpyAsync(&h_oob, s->flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -709,22 +878,32 @@ int ski_pack(gp_plan* p) {
 
 // d mode products  *out = (F_0 x ... x F_{d-1}) in,  F_i = dT_i for i == dt_dim and T_i otherwise (dt_dim = -1: K_uu).  Product i
 // writes bufs[i & 1]; `in` may be buf1 (overwritten after the first product), and *out is the buffer of the last product.
+// A dimension with G <= SKI_DENSE_G runs ski_mode_kernel on its dense factor, a larger one ski_mode_banded_kernel on its
+// generating column.
 static int ski_mode_products(gp_plan* p, const SkiGeom& g, const float* in, float* buf0, float* buf1, int dt_dim, float** out) {
   const gp_ski_state* s = p->ski;
   GP_CHECK(opt_in_smem<ski_mode_kernel>(p->device, 160 * 1024));
   float* bufs[2] = {buf0, buf1};
   const float* cur = in;
-  size_t toff = 0;
+  size_t toff = 0, coff = 0;
   for (int i = 0; i < g.d; ++i) {
     const int G = g.G[i];
     const int64_t inner = g.stride[i] * TP;                // elements after mode i (incl. the 16 columns)
     const int64_t total = g.M / G * TP;                    // positions of the flattened (outer, inner) space
     const int64_t nslab = cdiv(total, SKI_MT);
-    const float* F = (i == dt_dim ? s->dT : s->T).as<float>() + toff;
     GP_REQUIRE(total < ((int64_t)1 << 31), GP_E_SHAPE, "SKI: grid block too large");
-    ski_mode_kernel<<<(unsigned)std::min<int64_t>(nslab, 2 * p->n_sm), 256, ski_mode_smem(G), p->stream>>>(F, G, cur, bufs[i & 1], inner, total, nslab);
+    if (G <= SKI_DENSE_G) {
+      const float* F = (i == dt_dim ? s->dT : s->T).as<float>() + toff;
+      ski_mode_kernel<<<(unsigned)std::min<int64_t>(nslab, 2 * p->n_sm), 256, ski_mode_smem(G), p->stream>>>(F, G, cur, bufs[i & 1], inner, total, nslab);
+      toff += (size_t)G * G;
+    } else {
+      const float* F = (i == dt_dim ? s->dtcol : s->tcol).as<float>() + coff;
+      const int* band = s->band.as<int>() + 2 * i + (i == dt_dim ? 1 : 0);
+      const int64_t items = nslab * cdiv(G, SKI_BR);
+      ski_mode_banded_kernel<<<(unsigned)std::min<int64_t>(items, 4 * p->n_sm), 256, 0, p->stream>>>(F, band, G, cur, bufs[i & 1], inner, total, nslab);
+    }
     cur = bufs[i & 1];
-    toff += (size_t)G * G;
+    coff += (size_t)G;
   }
   p->launches += g.d;
   *out = bufs[(g.d - 1) & 1];
@@ -815,19 +994,20 @@ int ski_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
 // ---- single entries (ski_rows.cuh): the diagonal, requested rows and the pivoted Cholesky (pivchol.cu) ----------------------------
 int ski_rows_args(const gp_plan* p, SkiRows* s) {
   const gp_ski_state* k = p->ski;
-  GP_REQUIRE(k != nullptr && k->T.p != nullptr, GP_E_STATE, "SKI grid not packed");
+  GP_REQUIRE(k != nullptr && k->tcol.p != nullptr, GP_E_STATE, "SKI grid not packed");
   s->d = p->d;
-  int toff = 0, uoff = 0;
+  int off = 0;
   for (int i = 0; i < 4; ++i) {
     const bool live = i < p->d;
     s->G[i] = live ? k->G[i] : 0;
-    s->toff[i] = toff;
-    s->uoff[i] = uoff;
-    if (live) { toff += k->G[i] * k->G[i]; uoff += k->G[i]; }
+    s->coff[i] = off;
+    s->uoff[i] = off;
+    if (live) off += k->G[i];
   }
-  s->usum = uoff;
+  s->usum = off;
+  s->staged = off <= SKI_U_MAX;
   s->os = p->outputscale;
-  s->T = k->T.as<float>();
+  s->tc = k->tcol.as<float>();
   s->first = k->first.as<int>();
   s->wts = k->wts.as<float>();
   return GP_OK;
@@ -851,7 +1031,7 @@ ski_krows_kernel(const SkiRows s, const int64_t* __restrict__ idx, int64_t n, fl
   ski_stage_u(s, i, u, threadIdx.x, 256);
   __syncthreads();
   const int64_t j = (int64_t)blockIdx.x * 256 + threadIdx.x;
-  if (j < n) out[(int64_t)blockIdx.y * ldo + j] = ski_entry(s, u, j);
+  if (j < n) out[(int64_t)blockIdx.y * ldo + j] = ski_entry(s, u, i, j);
 }
 
 // per-CTA fp64 partial sums of the diagonal (fixed order in the CTA and on the host: reproducible)
@@ -1154,7 +1334,7 @@ static int ski_predict_check(gp_plan* p, int t, int64_t ld_in, int64_t ld_out, c
              "%s is not available on row-sharded plans", what);
   GP_REQUIRE(t >= 1 && ld_in >= t && ld_out >= t, GP_E_SHAPE, "%s: bad shape t=%d, leading dimensions %lld / %lld", what, t,
              (long long)ld_in, (long long)ld_out);
-  GP_REQUIRE(p->ski->T.p != nullptr && p->ski->perm.p != nullptr, GP_E_STATE, "%s: SKI grid not packed", what);
+  GP_REQUIRE(p->ski->tcol.p != nullptr && p->ski->perm.p != nullptr, GP_E_STATE, "%s: SKI grid not packed", what);
   GP_CUDA(cudaSetDevice(p->device));
   return GP_OK;
 }
@@ -1170,8 +1350,18 @@ extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* g
   GP_REFUSE_TASKS(p, "gp_plan_set_ski");
   GP_REFUSE_KRON(p, "gp_plan_set_ski");
   GP_REQUIRE(d == p->d && d >= 1 && d <= SKI_MAXD, GP_E_SHAPE, "SKI: grid dimension %d does not match the data (d=%d, max %d)", d, p->d, SKI_MAXD);
-  for (int i = 0; i < d; ++i)
-    GP_REQUIRE(grid_sizes[i] >= 4 && grid_sizes[i] <= 128 && grid_step[i] > 0.f, GP_E_SHAPE, "SKI: grid size %d (dim %d) must be in [4, 128]", grid_sizes[i], i);
+  int64_t M = 1;
+  bool large = false;
+  for (int i = 0; i < d; ++i) {
+    GP_REQUIRE(grid_sizes[i] >= 4 && grid_sizes[i] <= SKI_MAX_G && grid_step[i] > 0.f, GP_E_SHAPE,
+               "SKI: grid size %d (dim %d) must be in [4, %d]", grid_sizes[i], i, SKI_MAX_G);
+    M = std::min<int64_t>(M * grid_sizes[i], (int64_t)1 << 40);   // saturated: 4 dimensions of 2^17 would overflow
+    large |= grid_sizes[i] > SKI_DENSE_G;
+  }
+  // the mode kernels index the [M][16] grid block's positions in 32 bits; grids within [4, 128]^d keep the limits they always had
+  // (the per-mode check in ski_mode_products)
+  GP_REQUIRE(!large || M * TP < ((int64_t)1 << 31), GP_E_SHAPE, "SKI: grid of %lld nodes too large (M * 16 must be below 2^31)",
+             (long long)M);
   if (!p->ski) p->ski = new gp_ski_state();
   for (int i = 0; i < d; ++i) { p->ski->G[i] = grid_sizes[i]; p->ski->lo[i] = grid_lo[i]; p->ski->step[i] = grid_step[i]; }
   p->backend_req = GP_BACKEND_SKI;

@@ -1,4 +1,7 @@
-"""gpytorch.utils.grid.ScaleToBounds (utils/grid.py:11-54 of the reference): keeps learned features inside a fixed KISS-GP grid."""
+"""gpytorch.utils.grid subset of the reference (utils/grid.py): ScaleToBounds (lines 11-54) keeps learned features inside a fixed
+KISS-GP grid, choose_grid_size (lines 80-100) sizes a grid from the training set."""
+import math
+
 import torch
 
 
@@ -27,3 +30,14 @@ class ScaleToBounds(torch.nn.Module):
             x = x.clamp(lo, hi)
         span = 0.95 * (self.upper_bound - self.lower_bound)
         return (x - lo) * (span / (hi - lo)) + 0.95 * self.lower_bound
+
+
+def choose_grid_size(train_inputs, ratio=1.0, kronecker_structure=True):
+    """utils/grid.py:80-100 of the reference: a KISS-GP grid size for training inputs x ([n] or [..., n, d]).  With Kronecker
+    structure (the default) every dimension gets int(ratio * n^(1/d)) nodes, so that the grid has about ratio * n nodes in all;
+    without it, ratio * n.  The SKI backend accepts 4 to 131072 nodes per dimension."""
+    num_data = train_inputs.numel() if train_inputs.dim() == 1 else train_inputs.size(-2)
+    num_dim = 1 if train_inputs.dim() == 1 else train_inputs.size(-1)
+    if kronecker_structure:
+        return int(ratio * math.pow(num_data, 1.0 / num_dim))
+    return ratio * num_data

@@ -85,7 +85,9 @@ int gp_plan_set_noise_diag(gp_plan* plan, const float* diag, int64_t n);
 
 /* SKI / KISS-GP (kernels/grid_interpolation_kernel.py:132-213, kernels/grid_kernel.py:107-177, utils/interpolation.py:15-167):
  * the plan's operator becomes K_ski = W (T_0 x ... x T_{d-1}) W^T with cubic interpolation onto a regular grid; grid_lo[i] /
- * grid_step[i] are the first node and the spacing of dimension i (utils/grid.py:142-180), grid_sizes[i] in [4, 128], d <= 4.
+ * grid_step[i] are the first node and the spacing of dimension i (utils/grid.py:142-180), grid_sizes[i] in [4, 131072], d <= 4;
+ * a grid with a dimension over 128 also needs prod_i grid_sizes[i] * 16 < 2^31 (GP_E_SHAPE otherwise).  Dimensions up to 128
+ * nodes multiply by their dense Toeplitz factor, larger ones by its generating column, skipping the exactly-zero far band.
  * Call after gp_plan_set_data (square operator); products, mBCG, SLQ, gp_mll (without preconditioner) and gp_lanczos then run
  * on the interpolated operator, and gp_kdiag, gp_krows, gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg with W,
  * gp_ciq_precond_build and gp_ciq_sqrt_matmul_precond accept it (a preconditioned SKI MLL combines these primitives).  Out-of-bounds inputs fail like the reference ("Received data that was out of bounds ..."). */
