@@ -114,6 +114,7 @@ extern "C" int gp_plan_destroy(gp_plan* p) {
     gp_plan_set_tasks(p, nullptr, nullptr, 0);
   }
   if (p->kron) gp_plan_set_kron(p, nullptr, 0);   // the data plan stays the caller's
+  if (p->deriv) gp_plan_set_deriv(p, nullptr);
   if (p->pinned) cudaFreeHost(p->pinned);
   delete p;
   return GP_OK;
@@ -125,6 +126,7 @@ extern "C" int gp_plan_set_backend(gp_plan* p, int backend) {
   GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_STATE, "the SKI backend is selected by gp_plan_set_ski");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel sum runs the backends of its terms");
   GP_REQUIRE(p->kron == nullptr, GP_E_STATE, "a Kronecker plan runs the backend of its data plan");
+  GP_REFUSE_DERIV(p, "gp_plan_set_backend");
   p->backend_req = backend;
   if (p->data_set && p->hypers_set) return pack_inputs(p);
   return GP_OK;
@@ -134,6 +136,7 @@ extern "C" int gp_plan_set_data(gp_plan* p, const float* X1, int64_t n1, int64_t
                                 int64_t ld2, int d, int64_t row_begin, int64_t row_count) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(p->kron == nullptr, GP_E_STATE, "a Kronecker plan takes its rows from its data plan (gp_plan_set_kron)");
+  GP_REQUIRE(p->deriv == nullptr, GP_E_STATE, "a derivative plan takes its rows from its data plan (gp_plan_set_deriv)");
   GP_REQUIRE(X1 != nullptr && n1 >= 1 && d >= 1 && ld1 >= d, GP_E_SHAPE, "bad X1 shape n1=%lld d=%d ld1=%lld", (long long)n1, d, (long long)ld1);
   GP_CUDA(cudaSetDevice(p->device));
   // task indices belong to the rows they were set for: new data drops them (gp_plan_set_tasks again)
@@ -206,6 +209,7 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(!(p->tasks && comm && comm->world > 1), GP_E_SHAPE, "task indices are not available on a row-sharded plan");
   GP_REQUIRE(!(p->kron && comm && comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
+  GP_REQUIRE(!(p->deriv && comm && comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   p->comm = comm;
   return GP_OK;
 }
@@ -228,12 +232,14 @@ extern "C" int gp_time_kmv_kernel(gp_plan* p, const float* V, int64_t ldv, int t
   GP_CHECK(p->V16.ensure(sizeof(float) * p->n2 * TP));
   GP_CHECK(to_v16(p, V, ldv, t, p->n2, p->V16.as<float>()));
   KronColsScope kcols(p, t);
-  if (!p->tasks && (p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_any_tc))) GP_CHECK(pack_v_tiles(p, p->V16.as<float>()));
+  if (!p->tasks && !p->deriv && (p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_any_tc))) GP_CHECK(pack_v_tiles(p, p->V16.as<float>()));
   auto launch = [&]() -> int {
     // a multitask plan: the whole product (gather, V tiles, one launch per column task, combine)
     if (p->tasks) return tasks_kmv_partials(p, p->V16.as<float>(), p->kind, nullptr);
     // a Kronecker plan: the whole product (B mix, V tiles, one data-kernel launch per chunk, scatter)
     if (p->kron) return kron_kmv_partials(p, p->V16.as<float>(), nullptr);
+    // a derivative plan: the derivative kernel over the live column chunks and the split sum
+    if (p->deriv) return deriv_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, p->V16.as<float>(), nullptr);
     return p->backend == GP_BACKEND_TCGEN05 ? kmv_tc_launch(p, nullptr) : kmv_simt_launch(p, p->V16.as<float>(), nullptr);

@@ -185,6 +185,23 @@ struct gp_kron_state {
   gp::DevBuf Lw, red, idx, rows;           // gradient / row-extraction scratch
 };
 
+// Derivative-observation state (deriv.cu): the RBF value / gradient operator over interleaved rows i (d+1) + a on a plain RBF data
+// plan.  Per dimension c < d: w[c] = 1 / (sqrt(log2 e) l_c) turns a packed difference into u_c = D_c / l_c^2, il2[c] = 1 / l_c^2;
+// both are 0 for c >= d.
+constexpr int DERIV_DMAX = 16;   // d + 1 rows per point stay within the engine's 32-task limit; the kernels are built for DP <= 16
+struct DerivHyp {
+  float w[DERIV_DMAX];
+  float il2[DERIV_DMAX];
+};
+struct gp_deriv_state {
+  gp_plan* data = nullptr;                 // caller-owned plain RBF plan
+  DerivHyp hyp;                            // from data's lengthscales at the last refresh (kernel parameter)
+  bool hyp_set = false;
+  int nsplit = 1;                          // column splits of the derivative kernels (deriv_geometry)
+  int64_t cps = 0;                         // points of the other side per split
+  gp::DevBuf part, gout, hypd;             // split partials [nsplit][N1 (d+1)][16] | gradient CTA partials | hyp on the device
+};
+
 struct gp_comm {
   void* nccl_comm = nullptr;
   int rank = 0, world = 1;
@@ -242,7 +259,8 @@ struct gp_plan {
   gp::DevBuf lrw;                 // U^T V partials [G][16 r] | c = U^T V [r][16] fp64
   gp_task_state* tasks = nullptr; // non-null: Hadamard multitask operator s K o B[t, t'] (gp_plan_set_tasks)
   gp_kron_state* kron = nullptr;  // non-null: Kronecker multitask operator (s K_data) (x) B (gp_plan_set_kron)
-  int kron_cols = 16;             // columns of V16 a Kronecker product mixes (KronColsScope); the rest must be zero or unused
+  gp_deriv_state* deriv = nullptr;   // non-null: derivative-observation operator over a plain RBF plan (gp_plan_set_deriv)
+  int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
 
@@ -305,6 +323,15 @@ int kron_set_task_covar(gp_plan* p, const float* B, int T);                  // 
 int kron_task_covar_grad_checked(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB);
 #define GP_REFUSE_KRON(p, what) \
   GP_REQUIRE((p)->kron == nullptr, GP_E_STATE, "%s is not available on a Kronecker multitask plan (gp_plan_set_kron)", what)
+int deriv_pack(gp_plan* p);                                                  // deriv.cu
+int deriv_kmv_partials(gp_plan* p, const float* V16, const int* done_flag);  // K_grad V into partial slot 0 (unscaled)
+int deriv_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
+int deriv_kdiag(gp_plan* p, float* OUT);
+int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+int deriv_refresh(gp_plan* p);                                               // re-check the data plan, take its scale / lengthscales / flag
+double deriv_trace(const gp_plan* p);                                        // s N (1 + sum_c 1 / l_c^2) in fp64
+#define GP_REFUSE_DERIV(p, what) \
+  GP_REQUIRE((p)->deriv == nullptr, GP_E_STATE, "%s is not available on a derivative-observation plan (gp_plan_set_deriv)", what)
 int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,   // cg.cu
              int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
              int* tridiag_size, float* resid_out);

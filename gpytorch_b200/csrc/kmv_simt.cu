@@ -125,6 +125,7 @@ int kmv_simt_launch_cols(gp_plan* p, int kind, const float* Z1, const float* Z2,
 
 static int kmv_partials_base(gp_plan* p, const float* V16, const int* done_flag) {
   if (p->kron) return kron_kmv_partials(p, V16, done_flag);
+  if (p->deriv) return deriv_kmv_partials(p, V16, done_flag);
   if (p->tasks) return tasks_kmv_partials(p, V16, p->kind, done_flag);
   if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, V16, done_flag);
   if (p->backend == GP_BACKEND_SUM) {
@@ -413,6 +414,7 @@ extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, i
   GP_REQUIRE(m >= 0 && ldo >= p->n2, GP_E_SHAPE, "bad krows shape");
   if (m == 0) return GP_OK;
   if (p->kron) return kron_krows(p, idx, m, OUT, ldo);
+  if (p->deriv) return deriv_krows(p, idx, m, OUT, ldo);
   if (p->lr_U) {   // rows of the operator the plan multiplies: s K - U U^T
     GP_CHECK(p->backend == GP_BACKEND_SUM ? sum_krows(p, idx, m, OUT, ldo) : krows_base(p, idx, m, OUT, ldo));
     return lowrank_krows(p, idx, m, OUT, ldo);
@@ -443,6 +445,7 @@ extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_REQUIRE(p->backend != GP_BACKEND_SUM || p->lr_U, GP_E_SHAPE, "diagonal of a kernel sum: call gp_kdiag on every term and add");
   if (p->kron) return kron_kdiag(p, OUT);
+  if (p->deriv) return deriv_kdiag(p, OUT);
   if (p->lr_U) {   // diag(s K) - sum_j U_ij^2
     if (p->backend == GP_BACKEND_SUM) {
       // a low-rank plan is square: every stationary term contributes its constant outputscale, added in term order
@@ -493,6 +496,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   GP_REQUIRE((ldl >= s || p->row_count == 1) && (ldr >= s || p->n2 == 1), GP_E_SHAPE,
              "gp_bilinear_grad: leading dimensions must be >= s (ldl=%lld, ldr=%lld, s=%d)", (long long)ldl, (long long)ldr, s);
   if (p->kron) return kron_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
+  if (p->deriv) return deriv_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   // before any launch: the SIMT derivative kernel is instantiated up to DP = 64
   GP_REQUIRE(p->backend == GP_BACKEND_SKI || p->DP <= 64, GP_E_SHAPE, "bilinear gradient supports d <= 64 (d=%d)", p->d);
   const bool ard = p->ls.size() > 1;

@@ -363,6 +363,7 @@ extern "C" int gp_plan_set_kron(gp_plan* p, gp_plan* data, int T) {
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a Kronecker plan");
   GP_REFUSE_TASKS(p, "gp_plan_set_kron");
   GP_REFUSE_LOWRANK(p, "gp_plan_set_kron");
+  GP_REFUSE_DERIV(p, "gp_plan_set_kron");
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   gp_kron_state* ks = p->kron ? p->kron : new gp_kron_state();
   const bool keep_b = p->kron && ks->T == T && ks->b_set;

@@ -192,6 +192,9 @@ constexpr int PC_KIND_SKI = 65;
 // multitask (tasks.cu, kron.cu): K[r, r'] = s B[task(r), task(r')] k(|z_point(r) - z_point(r')|^2), covariance kind kind[0]; row r is
 // point r / rep, task task[r] (Hadamard: rep = 1, task ids) or point r / T, task r mod T (Kronecker: rep = T, task = nullptr)
 constexpr int PC_KIND_TASK = 66;
+// derivative observations (deriv.cu): row r is point r / rep, component r mod rep (rep = d + 1); the entry of rows (a, b) is the
+// RBF value / gradient block entry with u_c = dz_c w[c] and 1 / l_c^2 = il2[c] from dh (a DerivHyp on the device)
+constexpr int PC_KIND_DERIV = 67;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -200,7 +203,8 @@ struct PcTerms {
   const int* task;   // PC_KIND_TASK: task ids (user order; nullptr: r mod rep) and B [T][T]
   const float* B;
   int T;
-  int rep;           // PC_KIND_TASK: rows per point
+  int rep;           // PC_KIND_TASK / PC_KIND_DERIV: rows per point
+  const DerivHyp* dh;   // PC_KIND_DERIV
 };
 __device__ __forceinline__ int pc_task_of(const PcTerms& tt, int r) { return tt.task ? tt.task[r] : r % tt.rep; }
 __device__ __forceinline__ float pc_cov_rt(int kind, float a) {
@@ -255,7 +259,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
     } else if (KIND == PC_KIND_SKI) {
       ski_stage_u(sk, pi, zp, tid, PCP_THREADS);
     } else {
-      const int64_t zr = KIND == PC_KIND_TASK ? pi / tt.rep : pi;
+      const int64_t zr = (KIND == PC_KIND_TASK || KIND == PC_KIND_DERIV) ? pi / tt.rep : pi;
       for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[zr * DP + c];
     }
     for (int q = tid; q < m; q += PCP_THREADS) lp[q] = __ldcg(Lt + (int64_t)q * n + pi);   // written by another SM, before the last barrier
@@ -301,6 +305,18 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             s = fmaf(df, df, s);
           }
           v = os * tt.B[pc_task_of(tt, pi) * tt.T + pc_task_of(tt, (int)j)] * pc_cov_rt(tt.kind[0], -0.5f * s);
+        } else if (KIND == PC_KIND_DERIV) {
+          const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
+          float s = 0.f;
+          for (int c = 0; c < DP; ++c) {
+            float df = zp[c] - zj[c];
+            s = fmaf(df, df, s);
+          }
+          const float k = os * cov_from_arg<GP_RBF>(-0.5f * s);
+          const int a = pi % tt.rep, b = (int)j % tt.rep;
+          const float ua = a ? (zp[a - 1] - zj[a - 1]) * tt.dh->w[a - 1] : 0.f;
+          const float ub = b ? (zp[b - 1] - zj[b - 1]) * tt.dh->w[b - 1] : 0.f;
+          v = a == 0 ? (b == 0 ? k : k * ub) : (b == 0 ? -k * ua : k * ((a == b ? tt.dh->il2[a - 1] : 0.f) - ua * ub));
         } else {
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
@@ -430,6 +446,17 @@ __global__ void pc_init_task_kernel(const PcTerms tt, float os, float* __restric
   if (j >= n) return;
   const int a = pc_task_of(tt, (int)j);
   diag[j] = os * tt.B[a * tt.T + a];
+  perm[j] = (int)j;
+  pos[j] = (int)j;
+}
+
+// derivative observations: diag[j] = s (value rows), s / l_b^2 (derivative rows b); then pc_first_pivot_kernel
+__global__ void pc_init_deriv_kernel(const PcTerms tt, float os, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos,
+                                     int64_t n) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int b = (int)(j % tt.rep);
+  diag[j] = b ? os * tt.dh->il2[b - 1] : os;
   perm[j] = (int)j;
   pos[j] = (int)j;
 }
@@ -795,8 +822,16 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   }
   const bool kron = p->kron != nullptr;
   const bool tasks = p->tasks != nullptr || kron;
+  const bool deriv = p->deriv != nullptr;
   const float* Zsrc = p->Z2.as<float>();
-  if (kron) {   // entries of (s K_data) (x) B from the data plan's packed rows
+  if (deriv) {   // entries of the value / gradient operator from the data plan's packed rows
+    GP_CHECK(deriv_refresh(p));
+    const gp_plan* q = p->deriv->data;
+    tt.rep = q->d + 1; tt.dh = p->deriv->hypd.as<DerivHyp>();
+    Zsrc = q->Z2.as<float>();
+    dp_total = q->DP;
+    os_total = q->outputscale;
+  } else if (kron) {   // entries of (s K_data) (x) B from the data plan's packed rows
     GP_REQUIRE(p->kron->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
     GP_CHECK(kron_refresh(p));
     const gp_plan* q = p->kron->data;
@@ -808,7 +843,11 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     GP_REQUIRE(p->tasks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
     tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T; tt.rep = 1;
   }
-  if (tasks) {
+  if (deriv) {
+    pc_init_deriv_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, diag, perm, pos, n);
+    pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
+    p->launches += 2;
+  } else if (tasks) {
     pc_init_task_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;
@@ -829,11 +868,13 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_REQUIRE(!sum || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a kernel sum needs the cooperative kernel");
   GP_REQUIRE(!ski || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a SKI operator needs the cooperative kernel");
   GP_REQUIRE(!tasks || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a multitask operator needs the cooperative kernel");
+  GP_REQUIRE(!deriv || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a derivative operator needs the cooperative kernel");
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : ski ? PC_KIND_SKI : tasks ? PC_KIND_TASK : p->kind) {
+    switch (sum ? PC_KIND_SUM : ski ? PC_KIND_SKI : deriv ? PC_KIND_DERIV : tasks ? PC_KIND_TASK : p->kind) {
       case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
+      case PC_KIND_DERIV: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_DERIV>; break;
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
       case GP_MATERN12: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN12>; break;
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
@@ -1005,6 +1046,9 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
     tr_k = (double)n * os_total;
   } else if (p->backend == GP_BACKEND_SKI) {
     GP_CHECK(ski_diag_sum(p, &tr_k));
+  } else if (p->deriv) {    // s N (1 + sum_c 1 / l_c^2)
+    GP_CHECK(deriv_refresh(p));
+    tr_k = deriv_trace(p);
   } else if (p->kron) {     // s N sum_a B[a, a]
     const gp_kron_state* ks = p->kron;
     double bt = 0.0;

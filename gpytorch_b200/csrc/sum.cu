@@ -121,6 +121,7 @@ extern "C" int gp_plan_set_sum(gp_plan* p, gp_plan* const* terms, int n_terms) {
   GP_REQUIRE(p->ski == nullptr, GP_E_STATE, "a SKI plan cannot become a kernel sum");
   GP_REFUSE_TASKS(p, "gp_plan_set_sum");
   GP_REFUSE_KRON(p, "gp_plan_set_sum");
+  GP_REFUSE_DERIV(p, "gp_plan_set_sum");
   GP_CUDA(cudaSetDevice(p->device));
   p->terms.assign(terms, terms + n_terms);
   p->backend_req = GP_BACKEND_SUM;

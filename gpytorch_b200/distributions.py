@@ -32,6 +32,16 @@ class MultivariateNormal:
         return c.diagonal(dim1=-2, dim2=-1) if torch.is_tensor(c) else c.diagonal()
 
     @property
+    def stddev(self):
+        return self.variance.clamp_min(0).sqrt()
+
+    def confidence_region(self):
+        """(mean - 2 stddev, mean + 2 stddev) (multivariate_normal.py confidence_region)."""
+        std2 = self.stddev.mul(2)
+        mean = self.mean
+        return mean.sub(std2), mean.add(std2)
+
+    @property
     def event_shape(self):
         return self.loc.shape[-1:]
 

@@ -279,7 +279,7 @@ class Plan:
     def info(self):
         b, s, k, m = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         check(self.lib.gp_plan_info(self._h, C.byref(b), C.byref(s), C.byref(k), C.byref(m)))
-        return {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum", 5: "kron"}.get(b.value, "?"), "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
+        return {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum", 5: "kron", 6: "deriv"}.get(b.value, "?"), "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
 
     def time_kmv_kernel(self, v: torch.Tensor, warmup: int = 3, reps: int = 20) -> float:
         """Average device time (ms) of ONE launch of the fused K.V kernel alone (CUDA events on the plan stream)."""
@@ -489,13 +489,11 @@ class Plan:
         return res, solve
 
 
-class KronPlan(Plan):
-    """The Kronecker multitask operator (s K_data) (x) B over interleaved rows i T + a (gp_plan_set_kron): N1 T x N2 T, built on a
-    ready data Plan (kept alive here).  set_noise supplies the noise; set_task_covar / task_covar_grad take B and its gradient,
-    bilinear_grad returns the data kernel's (lengthscale, outputscale) gradients.  Every product, solve and sample call of Plan
-    works on it."""
+class _DataPlanOperator(Plan):
+    """A plan whose operator is built on a ready data Plan (kept alive here): the engine reads the data plan's packed rows and
+    hyper-parameters, and only the noise is this plan's own.  Subclasses attach the data plan through their C call."""
 
-    def __init__(self, data: Plan, num_tasks: int):
+    def __init__(self, data: Plan, *args):
         self.lib = data.lib
         self.device = data.device
         self._h = C.c_void_p()
@@ -503,7 +501,30 @@ class KronPlan(Plan):
         check(self.lib.gp_plan_create(C.byref(self._h), self.device.index or 0, C.c_void_p(stream)))
         self.comm = None
         self.noise, self.outputscale = 0.0, 1.0
-        self.attach(data, num_tasks)
+        self.attach(data, *args)
+
+    def set_hypers(self, kind=None, lengthscale=None, outputscale: float = 1.0, noise: float = 0.0):
+        """Only the noise is this plan's own: kind and lengthscales are the data plan's."""
+        return self.set_noise(noise)
+
+    def set_noise(self, noise: float):
+        ls = list(self.data.lengthscale)
+        arr = (C.c_float * len(ls))(*ls)
+        self.kind, self.lengthscale, self.noise = self.data.kind, ls, float(noise)
+        self.outputscale = self.data.outputscale
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_hypers(self._h, KIND[self.kind], arr, len(ls), float(self.outputscale), float(noise)))
+        return self
+
+
+class KronPlan(_DataPlanOperator):
+    """The Kronecker multitask operator (s K_data) (x) B over interleaved rows i T + a (gp_plan_set_kron): N1 T x N2 T, built on a
+    ready data Plan (kept alive here).  set_noise supplies the noise; set_task_covar / task_covar_grad take B and its gradient,
+    bilinear_grad returns the data kernel's (lengthscale, outputscale) gradients.  Every product, solve and sample call of Plan
+    works on it."""
+
+    def __init__(self, data: Plan, num_tasks: int):
+        super().__init__(data, num_tasks)
 
     def attach(self, data: Plan, num_tasks: int):
         """(Re-)attach the data plan: validation and geometry only; a B of the same size stays set."""
@@ -519,15 +540,31 @@ class KronPlan(Plan):
     def refresh_data(self):
         return self.attach(self.data, self.num_tasks)
 
-    def set_hypers(self, kind=None, lengthscale=None, outputscale: float = 1.0, noise: float = 0.0):
-        """Only the noise is this plan's own: kind and lengthscales are the data plan's."""
-        return self.set_noise(noise)
 
-    def set_noise(self, noise: float):
-        ls = list(self.data.lengthscale)
-        arr = (C.c_float * len(ls))(*ls)
-        self.kind, self.lengthscale, self.noise = self.data.kind, ls, float(noise)
-        self.outputscale = self.data.outputscale
+class DerivPlan(_DataPlanOperator):
+    """The RBF value / gradient operator over interleaved rows i (d+1) + a (gp_plan_set_deriv): N1 (d+1) x N2 (d+1), built on a
+    ready plain RBF data Plan (kept alive here).  set_noise supplies the noise; bilinear_grad returns the data kernel's (lengthscale,
+    outputscale) gradients.  Every product, solve and sample call of Plan works on it; it has no task covariance."""
+
+    def __init__(self, data: Plan):
+        super().__init__(data)
+
+    def attach(self, data: Plan):
+        """(Re-)attach the data plan: validation and geometry only."""
+        rw = data.d + 1
+        self.data, self.num_outputs = data, rw
+        self.same, self.d = data.same, data.d
+        self.n1, self.n2 = data.n1 * rw, data.n2 * rw
+        self.row_begin, self.row_count = 0, self.n1
         with torch.cuda.device(self.device):
-            check(self.lib.gp_plan_set_hypers(self._h, KIND[self.kind], arr, len(ls), float(self.outputscale), float(noise)))
+            check(self.lib.gp_plan_set_deriv(self._h, data._h))
         return self
+
+    def refresh_data(self):
+        return self.attach(self.data)
+
+    def set_task_covar(self, b):
+        raise RuntimeError("a derivative-observation plan has no task covariance (its d + 1 outputs per point are fixed by the kernel)")
+
+    def task_covar_grad(self, left, right):
+        raise RuntimeError("a derivative-observation plan has no task covariance (its d + 1 outputs per point are fixed by the kernel)")

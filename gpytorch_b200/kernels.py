@@ -1,4 +1,5 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, MaternKernel, ScaleKernel, AdditiveKernel, GridInterpolationKernel} for the accelerated path.
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, ScaleKernel, AdditiveKernel, GridInterpolationKernel} for the
+accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
 rbf_kernel.py:68-85; matern_kernel.py:79-110; scale_kernel.py:64-118), but `forward` returns an
@@ -59,6 +60,10 @@ class Kernel(Module):
     def _batch_size(self):
         return self.batch_shape[0] if len(self.batch_shape) else None
 
+    def _batchable(self):
+        """Whether batched inputs or a batch_shape can run (one independent operator per batch entry)."""
+        return True
+
     def __call__(self, x1, x2=None, diag=False, **params):
         # kernels/kernel.py:454-534: active dims, 1-D -> 2-D, x2=None -> x1, size check
         if self.active_dims is not None:
@@ -78,6 +83,9 @@ class Kernel(Module):
                                f"(based on the ard_num_dims argument). Got {x1.size(-1)}.")
         same = x2 is None
         nb = self._batch_size()
+        if (x1.dim() == 3 or nb is not None) and not self._batchable():
+            raise NotImplementedError("a batched RBFKernelGrad (batched inputs or a batch_shape) is not available on the "
+                                      "accelerated path")
         if x1.dim() == 3 or nb is not None:
             # one leading batch dimension (kernels/kernel.py:119-121 broadcasts every op over it): B independent operators, each
             # with its own inputs and hyper-parameters; the solver runs them concurrently (operators.BatchLinearOperator)
@@ -113,6 +121,30 @@ class _StationaryKernel(Kernel):
 class RBFKernel(_StationaryKernel):
     """k = exp(-0.5 |x1 - x2|^2 / l^2)  (kernels/rbf_kernel.py)."""
     kind = "rbf"
+
+
+class RBFKernelGrad(RBFKernel):
+    """Covariance of values and partial derivatives of an RBF GP (kernels/rbf_kernel_grad.py): an n x m input pair gives an
+    n (d+1) x m (d+1) operator over interleaved rows i (d+1) + a (a = 0: f(x_i), a = 1..d: df/dx_a at x_i), as the reference returns
+    after its perfect shuffle.  forward returns one engine DerivKernelLinearOperator (gp_plan_set_deriv); d <= 16, unbatched.
+    diag=True gives 1 at value rows and 1 / l_a^2 at derivative rows (times the outputscale inside a ScaleKernel)."""
+
+    def _batchable(self):
+        return False
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, **params):
+        if _batch_index is not None or len(self.batch_shape) or x1.dim() != 2:
+            raise NotImplementedError("a batched RBFKernelGrad is not available on the accelerated path")
+        from .operators import DerivKernelLinearOperator
+        if diag and not (_same or (x1.shape == x2.shape and torch.equal(x1, x2))):
+            raise RuntimeError("diag=True only works when x1 == x2")
+        ls = self.lengthscale.reshape(-1)
+        ls = ls[0] if ls.numel() == 1 else ls
+        op = DerivKernelLinearOperator(x1, None if _same else x2, ls)
+        return op.diagonal() if diag else op
+
+    def num_outputs_per_input(self, x1, x2):
+        return x1.size(-1) + 1
 
 
 class MaternKernel(_StationaryKernel):
@@ -170,12 +202,18 @@ class ScaleKernel(Kernel):
         else:
             base = self.base_kernel.forward(x1, x2, diag=False, _same=_same, _batch_index=bi, **params)
         os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
-        from .operators import SKIKernelLinearOperator
+        from .operators import DerivKernelLinearOperator, SKIKernelLinearOperator
+        if isinstance(base, DerivKernelLinearOperator):   # s folded into the same value / gradient operator
+            op = DerivKernelLinearOperator(base.x1, None if base.same else base.x2, base.lengthscale, os_)
+            return op.diagonal() if diag else op
         if isinstance(base, SKIKernelLinearOperator):
             op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
             return op.diagonal() if diag else op
         op = KernelLinearOperator(base.x1, base.x2, base.kind, base.lengthscale, os_)
         return op.diagonal() if diag else op
+
+    def _batchable(self):
+        return self.base_kernel._batchable()
 
     def __call__(self, x1, x2=None, diag=False, **params):
         self.active_dims = None  # selection happens once, here (base active_dims were lifted in __init__)

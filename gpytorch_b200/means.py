@@ -54,6 +54,26 @@ class ConstantMean(Module):
         return self.forward(x)
 
 
+class ConstantMeanGrad(Module):
+    """means/constant_mean_grad.py: a constant mean for the value and zero for the d partial derivatives.  The parameter is named
+    `constant` with shape [*batch_shape, 1], as in the reference, so state dicts interchange; forward returns [*batch, n, d + 1]."""
+
+    def __init__(self, prior=None, batch_shape=torch.Size(), **kwargs):
+        super().__init__()
+        if prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        self.batch_shape = torch.Size(batch_shape)
+        self.register_parameter("constant", torch.nn.Parameter(torch.zeros(*self.batch_shape, 1)))
+
+    def forward(self, input):
+        shape = torch.broadcast_shapes(self.batch_shape, input.shape[:-2]) + input.shape[-2:-1]
+        value = self.constant.unsqueeze(-2).expand(*shape, 1)                        # [*batch, n, 1]
+        return torch.cat([value, value.new_zeros(*shape, input.size(-1))], dim=-1)   # zero mean for the d derivatives
+
+    def __call__(self, input):
+        return self.forward(input)
+
+
 class MultitaskMean(Module):
     """means/multitask_mean.py:20-45: one mean per task (a single mean is deep-copied T times); forward returns [n, T]."""
 

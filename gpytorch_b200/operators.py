@@ -20,7 +20,7 @@ import torch
 
 from . import settings
 from ._lib import NanError
-from .engine import KronPlan, Plan
+from .engine import DerivPlan, KronPlan, Plan
 from .sampling import contour_quadrature, psd_safe_cholesky
 
 
@@ -85,6 +85,8 @@ def clear_plan_cache():
             _SUM_PLANS.popitem()[1].close()
         while _KRON_PLANS:
             _KRON_PLANS.popitem()[1].close()
+        while _DERIV_PLANS:
+            _DERIV_PLANS.popitem()[1].close()
         while _PLAN_CACHE:
             _PLAN_CACHE.popitem()[1].close()
 
@@ -741,6 +743,109 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
 
 _KRON_PLANS: "dict[tuple, Plan]" = {}
 
+_DERIV_SLOT = 28   # plan-cache slot of the data plans of derivative operators
+
+
+class DerivKernelLinearOperator(KernelLinearOperator):
+    """The RBF covariance of values and gradients over interleaved rows i (d+1) + a (RBFKernelGrad, kernels/rbf_kernel_grad.py:60-104,
+    after its perfect shuffle): ONE engine operator (gp_plan_set_deriv) on the plan of the plain RBF kernel; no N (d+1) x N (d+1)
+    matrix is stored.  The hyper-parameters are lengthscale (scalar or ARD) and outputscale.  Input gradients are not available:
+    inputs that require grad are refused."""
+
+    def __init__(self, x1, x2, lengthscale, outputscale=None):
+        if x1.requires_grad or (x2 is not None and x2.requires_grad):
+            raise RuntimeError("gradients with respect to the inputs of a derivative operator (RBFKernelGrad) are not implemented: "
+                               "pass inputs that do not require grad")
+        d = x1.size(-1)
+        if d > 16:
+            raise RuntimeError(f"RBFKernelGrad on the accelerated path supports d <= 16 input dimensions (got d={d})")
+        super().__init__(x1, x2, "rbf", lengthscale, outputscale)
+        self.num_outputs = d + 1
+        self._data_op = KernelLinearOperator(x1, x2, "rbf", lengthscale, self.outputscale)
+        self._data_op._plan_slot = _DERIV_SLOT
+
+    @property
+    def shape(self):
+        n2 = self.x1.size(0) if self.same else self.x2.size(0)
+        return torch.Size([self.x1.size(0) * self.num_outputs, n2 * self.num_outputs])
+
+    def plan(self, noise=0.0) -> Plan:
+        data = self._data_op.plan(0.0)
+        if getattr(data, "_noise_diag", None) is not None:
+            data.set_noise_diag(None)
+        nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
+        with _PLAN_LOCK:
+            key = id(data)
+            parent = _DERIV_PLANS.pop(key, None)
+            if parent is None:
+                parent = DerivPlan(data)
+                parent._hyp_key = None
+            _DERIV_PLANS[key] = parent
+            while len(_DERIV_PLANS) > 16:
+                _DERIV_PLANS.pop(next(iter(_DERIV_PLANS))).close()
+        # the data plan may have been re-packed or re-pointed since the last use: re-attach it (validation, no allocation)
+        parent.attach(data)
+        hk = (nz, tuple(data.lengthscale), data.outputscale)
+        if parent._hyp_key != hk:
+            parent.set_noise(nz)
+            parent._hyp_key = hk
+        self._plan = parent
+        return parent
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    def _transpose_nonbatch(self):
+        """K(x1, x2)^T = K(x2, x1): the value / gradient blocks swap with D -> -D."""
+        if self.same:
+            return self
+        return DerivKernelLinearOperator(self.x2, self.x1, self.lengthscale, self.outputscale)
+
+    def detach(self):
+        return DerivKernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.lengthscale.detach(),
+                                         self.outputscale.detach())
+
+    def to_dense(self):
+        return _KernelDense.apply(self)
+
+    def diagonal(self, dim1=-2, dim2=-1):
+        """s at value rows, s / l_a^2 at derivative rows (rbf_kernel_grad.py:106-115) for x2 == x1."""
+        if self.shape[0] != self.shape[1]:
+            raise RuntimeError(f"diagonal of a non-square operator {tuple(self.shape)} is undefined")
+        return self.plan().diag()
+
+    _diagonal = diagonal
+
+    def __getitem__(self, index):
+        """Slices that start and stop on multiples of d + 1 re-index x1 / x2 (prediction slices the joint operator at n (d+1))."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        R = self.num_outputs
+        x2 = self.x1 if self.same else self.x2
+        rs, cs = _aligned(ri, R, self.x1.size(0)), _aligned(ci, R, x2.size(0))
+        if rs is None or cs is None:
+            raise NotImplementedError("a derivative operator takes row / column slices that start and stop on multiples of d + 1")
+        return DerivKernelLinearOperator(self.x1[rs], x2[cs], self.lengthscale, self.outputscale)
+
+    def mul(self, other):
+        raise NotImplementedError("a derivative operator (RBFKernelGrad) does not multiply by a task covariance")
+
+    __mul__ = mul
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("a derivative operator adds a (Constant)DiagLinearOperator only")
+
+
+_DERIV_PLANS: "dict[int, Plan]" = {}
+
 
 class SumKernelLinearOperator(KernelLinearOperator):
     """K_1 + ... + K_m over the same inputs (AdditiveKernel, kernels/kernel.py:592-621).  The reference evaluates every term
@@ -1071,7 +1176,8 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
     def supports(base) -> bool:
         """A plan-backed non-SKI kernel operator (or kernel sum) without batch dimension on an unsharded square plan."""
         return (isinstance(base, KernelLinearOperator) and not isinstance(base, (SKIKernelLinearOperator, HadamardKernelLinearOperator,
-                                                                                          KroneckerKernelLinearOperator))
+                                                                                          KroneckerKernelLinearOperator,
+                                                                                          DerivKernelLinearOperator))
                 and base.same
                 and base._comm is None and base._row_begin == 0 and base._row_count in (0, base.shape[0]))
 

@@ -47,7 +47,8 @@ enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3 };
  * (the name is historical),
  * GP_BACKEND_SIMT = fp32 CUDA-core kernel (bring-up / cross-check / d > 41). */
 enum { GP_BACKEND_AUTO = 0, GP_BACKEND_TCGEN05 = 1, GP_BACKEND_SIMT = 2, GP_BACKEND_SKI = 3 /* set by gp_plan_set_ski */,
-       GP_BACKEND_SUM = 4 /* set by gp_plan_set_sum */, GP_BACKEND_KRON = 5 /* set by gp_plan_set_kron */ };
+       GP_BACKEND_SUM = 4 /* set by gp_plan_set_sum */, GP_BACKEND_KRON = 5 /* set by gp_plan_set_kron */,
+       GP_BACKEND_DERIV = 6 /* set by gp_plan_set_deriv */ };
 
 typedef struct gp_plan gp_plan;   /* opaque: repacked X, workspaces, stream, comm */
 typedef struct gp_comm gp_comm;   /* opaque: NCCL communicator for row-sharded runs */
@@ -173,6 +174,25 @@ int gp_task_covar_grad(gp_plan* plan, const float* L, int64_t ldl, const float* 
  * GP_E_STATE / GP_E_SHAPE: a SKI, kernel-sum, multitask, low-rank-corrected or row-sharded data plan; gp_plan_set_comm with more
  * than one rank, gp_plan_set_lowrank, gp_plan_set_tasks and the input gradients on `plan`. */
 int gp_plan_set_kron(gp_plan* plan, gp_plan* data, int T);
+
+/* GPs with derivative observations (RBFKernelGrad, kernels/rbf_kernel_grad.py:60-115, with the perfect shuffle of :99-102, as in
+ * examples/08_Advanced_Usage/Simple_GP_Regression_Derivative_Information_{1d,2d}.ipynb): `plan` becomes the N1 (d+1) x N2 (d+1)
+ * operator over interleaved rows i (d+1) + a (a = 0: f(x_i); a = 1..d: df/dx_a at x_i) with, for D = x_i - x'_j,
+ * u_a = D_a / l_a^2 and k = s exp(-|D / l|^2 / 2),
+ *     [value, value] = k,  [value, d/dx'_b] = k u_b,  [d/dx_a, value] = -k u_a,  [d/dx_a, d/dx'_b] = k (delta_ab / l_a^2 - u_a u_b)
+ * (+ its noise / per-row diagonal where a call adds it).  `data` is a ready plain RBF plan (tensor-core or SIMT, scalar or ARD
+ * lengthscale, square or cross, 1 <= d <= 16) on the same device and stream, caller-owned, and must outlive `plan`; the derivative
+ * kernels read its packed inputs and hyper-parameters and never call its fused kernel.  Re-packing it (gp_plan_set_hypers) is
+ * picked up by the next call on `plan`.  data = NULL clears the operator.  gp_plan_set_hypers on `plan` supplies the noise only (as
+ * on a kernel sum); gp_plan_set_noise_diag takes N (d+1) entries.  One K.V is one launch of an fp32 SIMT kernel per 4 columns
+ * (16 for d <= 4) and a fixed-order sum of its column-split partials: no atomics, repeated calls agree bit for bit.
+ * gp_kmv, gp_krows, gp_kdiag (s, s / l_a^2 on a square plan), gp_pivoted_cholesky (first pivot = argmax of that diagonal), the
+ * preconditioner calls, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos and gp_ciq_* run on it; gp_bilinear_grad returns the gradients of
+ * data's lengthscale(s) and outputscale.  A non-finite input makes products, rows, the diagonal and gradients NaN.
+ * GP_E_STATE / GP_E_SHAPE: a non-RBF, SKI, kernel-sum, multitask, Kronecker, derivative, low-rank-corrected or row-sharded data
+ * plan, d > 16; gp_plan_set_comm with more than one rank, gp_plan_set_lowrank, gp_plan_set_tasks, gp_plan_set_kron and the input
+ * gradients on `plan`. */
+int gp_plan_set_deriv(gp_plan* plan, gp_plan* data);
 
 /* ---- kernel seam (LazyEvaluatedKernelTensor, lazy/lazy_evaluated_kernel_tensor.py) --- */
 
