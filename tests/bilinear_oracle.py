@@ -134,6 +134,32 @@ def simt_cps(rows, n2, n_sm):
     return min(cdiv(ntj, nsp) * 64, n2)
 
 
+def pair_arg(zr, zc, nr, path, DP, KP):
+    """The per-pair part of the bound below for packed rows zr [r, d] against packed columns zc [c, d] (nr = |zc|^2 per column):
+    (dz, Ec, sq, S, m, da) with dz_c = z_ic - z_jc, Ec the packing error of dz_c, sq = dz^2, S = sum sq, m = S / 2 and da the
+    bound on the engine's error in a = -m on `path` ("simt": direct differences, "tc": the 3xTF32 GEMM).  Shared with the K.V
+    bound of tests/kmv_oracle.py."""
+    d = zr.size(1)
+    dz = [zr[:, c, None] - zc[None, :, c] for c in range(d)]
+    Ec = [2 * U32 * (zr[:, c, None].abs() + zc[None, :, c].abs()) for c in range(d)]
+    sq = [v * v for v in dz]
+    S = sum(sq)
+    E2 = sum(e * e for e in Ec)
+    m = 0.5 * S
+    da = E2.sqrt() * S.sqrt() + 0.5 * E2
+    if path == "simt":
+        da = da + (DP + 4) * U32 * m
+    else:
+        da = da + (1 + KP / 4) * 2.0 ** -21 * ((zr * zr).sum(1)[:, None] + nr[None, :]) + 4 * U32 * m
+    return dz, Ec, sq, S, m, da
+
+
+def pair_rel(m, eps_sum=0.0):
+    """eps_sum plus the relative error of one covariance value at m beyond the interval of a (_dev): ex2.approx 2^-21 of the
+    value, sqrt.approx, the fp32 product log2(e) rho and the Matern polynomial."""
+    return eps_sum + 2.0 ** -21 + 2 * U32 * (1 + m.sqrt()) + 6 * U32
+
+
 def bound(kind, x1, x2, lengthscale, outputscale, L, R, path, same=False, row_begin=0, n_sm=132, block=256):
     """(bound on |engine - closed_form| for dF/dl [1 or d], same for dF/ds) of gp_bilinear_grad on the same fp32 inputs.
     path: "simt" (bilinear_kernel; every ARD plan) or "tc" (scalar lengthscale on the tensor-core backend).
@@ -177,17 +203,7 @@ def bound(kind, x1, x2, lengthscale, outputscale, L, R, path, same=False, row_be
     nr = (zc * zc).sum(1)
     for b in _blocks(xr.size(0), block):
         Wabs = Labs[b] @ Rabs.t()
-        dz = [zr[b, c, None] - zc[None, :, c] for c in range(d)]
-        Ec = [2 * U32 * (zr[b, c, None].abs() + zc[None, :, c].abs()) for c in range(d)]
-        sq = [v * v for v in dz]
-        S = sum(sq)
-        E2 = sum(e * e for e in Ec)
-        m = 0.5 * S
-        da = E2.sqrt() * S.sqrt() + 0.5 * E2
-        if path == "simt":
-            da = da + (DP + 4) * U32 * m
-        else:
-            da = da + (1 + KP / 4) * 2.0 ** -21 * ((zr[b] * zr[b]).sum(1)[:, None] + nr[None, :]) + 4 * U32 * m
+        dz, Ec, sq, S, m, da = pair_arg(zr[b], zc, nr, path, DP, KP)
         if same:   # exact diagonal: a = 0 on both paths
             rows = torch.arange(b.start, b.stop, device=xr.device)
             cols = rows + row_begin
@@ -195,7 +211,7 @@ def bound(kind, x1, x2, lengthscale, outputscale, L, R, path, same=False, row_be
             da[rows - b.start, cols] = 0.0
         k, g = _kg(kind, m)
         dk, dg = _dev(kind, m, da)
-        rel = eps_sum + 2.0 ** -21 + 2 * U32 * (1 + m.sqrt()) + 6 * U32
+        rel = pair_rel(m, eps_sum)
         bk += (Wabs * (k * rel + dk)).sum()
         eg = g * rel + dg
         if not ard:
