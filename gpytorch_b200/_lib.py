@@ -15,7 +15,7 @@ LIB_PATH = os.environ.get("GPBBMM_LIB") or os.path.join(_HERE, "lib", "libgpbbmm
 
 GP_OK, GP_E_SHAPE, GP_E_CUDA, GP_E_NAN_MVM, GP_W_NOT_CONVERGED, GP_W_PIVCHOL_NAN, GP_E_NCCL, GP_E_STATE, GP_W_EIG_NOT_CONVERGED = range(9)
 GP_RBF, GP_MATERN12, GP_MATERN32, GP_MATERN52 = range(4)
-GP_BACKEND_AUTO, GP_BACKEND_TCGEN05, GP_BACKEND_SIMT, GP_BACKEND_SKI, GP_BACKEND_SUM, GP_BACKEND_KRON, GP_BACKEND_DERIV = range(7)
+GP_BACKEND_AUTO, GP_BACKEND_TCGEN05, GP_BACKEND_SIMT, GP_BACKEND_SKI, GP_BACKEND_SUM, GP_BACKEND_KRON, GP_BACKEND_DERIV, GP_BACKEND_PRODUCT = range(8)
 KIND = {"rbf": GP_RBF, "matern12": GP_MATERN12, "matern32": GP_MATERN32, "matern52": GP_MATERN52}
 BACKEND = {"auto": GP_BACKEND_AUTO, "tcgen05": GP_BACKEND_TCGEN05, "simt": GP_BACKEND_SIMT}
 
@@ -74,6 +74,7 @@ PROTOTYPES = {
     "gp_plan_set_noise_diag": (_I, [_P, _P, _L]),
     "gp_plan_set_ski": (_I, [_P, C.POINTER(_I), C.POINTER(_F), C.POINTER(_F), _I]),
     "gp_plan_set_sum": (_I, [_P, C.POINTER(_P), _I]),
+    "gp_plan_set_product": (_I, [_P, C.POINTER(_P), _I]),
     "gp_plan_set_lowrank": (_I, [_P, _P, _L, _I]),
     "gp_plan_set_tasks": (_I, [_P, _P, _P, _I]),
     "gp_plan_set_task_covar": (_I, [_P, C.POINTER(_F), _I]),

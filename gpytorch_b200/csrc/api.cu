@@ -127,6 +127,7 @@ extern "C" int gp_plan_set_backend(gp_plan* p, int backend) {
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel sum runs the backends of its terms");
   GP_REQUIRE(p->kron == nullptr, GP_E_STATE, "a Kronecker plan runs the backend of its data plan");
   GP_REFUSE_DERIV(p, "gp_plan_set_backend");
+  GP_REFUSE_PRODUCT(p, "gp_plan_set_backend");
   p->backend_req = backend;
   if (p->data_set && p->hypers_set) return pack_inputs(p);
   return GP_OK;
@@ -210,6 +211,8 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
   GP_REQUIRE(!(p->tasks && comm && comm->world > 1), GP_E_SHAPE, "task indices are not available on a row-sharded plan");
   GP_REQUIRE(!(p->kron && comm && comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   GP_REQUIRE(!(p->deriv && comm && comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
+  GP_REQUIRE(!(p->backend_req == GP_BACKEND_PRODUCT && comm && comm->world > 1), GP_E_STATE,
+             "gp_plan_set_comm with more than one rank is not available on a kernel-product plan (gp_plan_set_product)");
   p->comm = comm;
   return GP_OK;
 }
@@ -232,7 +235,8 @@ extern "C" int gp_time_kmv_kernel(gp_plan* p, const float* V, int64_t ldv, int t
   GP_CHECK(p->V16.ensure(sizeof(float) * p->n2 * TP));
   GP_CHECK(to_v16(p, V, ldv, t, p->n2, p->V16.as<float>()));
   KronColsScope kcols(p, t);
-  if (!p->tasks && !p->deriv && (p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_any_tc))) GP_CHECK(pack_v_tiles(p, p->V16.as<float>()));
+  if (p->backend == GP_BACKEND_PRODUCT) GP_CHECK(product_refresh(p));
+  if (!p->tasks && !p->deriv && (p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_any_tc) || (p->backend == GP_BACKEND_PRODUCT && p->prod_tc))) GP_CHECK(pack_v_tiles(p, p->V16.as<float>()));
   auto launch = [&]() -> int {
     // a multitask plan: the whole product (gather, V tiles, one launch per column task, combine)
     if (p->tasks) return tasks_kmv_partials(p, p->V16.as<float>(), p->kind, nullptr);
@@ -242,6 +246,7 @@ extern "C" int gp_time_kmv_kernel(gp_plan* p, const float* V, int64_t ldv, int t
     if (p->deriv) return deriv_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, p->V16.as<float>(), nullptr);
+    if (p->backend == GP_BACKEND_PRODUCT) return product_kmv_launch(p, p->V16.as<float>(), nullptr);
     return p->backend == GP_BACKEND_TCGEN05 ? kmv_tc_launch(p, nullptr) : kmv_simt_launch(p, p->V16.as<float>(), nullptr);
   };
   for (int i = 0; i < warmup; ++i) GP_CHECK(launch());

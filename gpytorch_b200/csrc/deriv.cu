@@ -499,6 +499,8 @@ extern "C" int gp_plan_set_deriv(gp_plan* p, gp_plan* data) {
   GP_REFUSE_TASKS(p, "gp_plan_set_deriv");
   GP_REFUSE_LOWRANK(p, "gp_plan_set_deriv");
   GP_REFUSE_KRON(p, "gp_plan_set_deriv");
+  GP_REFUSE_PRODUCT(p, "gp_plan_set_deriv");
+  if (data) GP_REFUSE_PRODUCT(data, "gp_plan_set_deriv (as the data plan)");
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   gp_deriv_state* ds = p->deriv ? p->deriv : new gp_deriv_state();
   gp_plan* old = ds->data;

@@ -260,6 +260,12 @@ struct gp_plan {
   gp_task_state* tasks = nullptr; // non-null: Hadamard multitask operator s K o B[t, t'] (gp_plan_set_tasks)
   gp_kron_state* kron = nullptr;  // non-null: Kronecker multitask operator (s K_data) (x) B (gp_plan_set_kron)
   gp_deriv_state* deriv = nullptr;   // non-null: derivative-observation operator over a plain RBF plan (gp_plan_set_deriv)
+  // kernel products (GP_BACKEND_PRODUCT, product.cu): the factors (caller-owned plain plans over the same rows); the plan's
+  // outputscale is the product of theirs, its xbad flag the OR of theirs
+  std::vector<gp_plan*> factors;
+  bool prod_tc = false;           // two tensor-core factors with KP_a + KP_b <= 128: product_tc_kernel, else product_simt_kernel
+  uint64_t pack_gen = 0;          // bumped by every re-pack of a plain plan
+  uint64_t fac_gen[4] = {0, 0, 0, 0};   // the factors' pack_gen at the last product_pack
   int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
@@ -285,12 +291,21 @@ int kmv_simt_launch(gp_plan* p, const float* V16, const int* done_flag);
 int kmv_tc_launch(gp_plan* p, const int* done_flag);
 int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t, int add_noise);
 int choose_geometry(gp_plan* p);
+void choose_splits(gp_plan* p, bool tc);                                // column splits of the K.V work from ntile_i / ntile_j / n_sm
 int ski_pack(gp_plan* p);                                               // ski.cu
 int ski_kmv_partials(gp_plan* p, const float* V16, const int* done_flag);
 int ski_bilinear(gp_plan* p, const float* L16, const float* R16, double* total);   // total[0] += <A, K_uu B>, total[1 + i] += <A, (l_i dK_uu/dl_i) B>
 int sum_pack(gp_plan* p);                                               // sum.cu: geometry / buffers of a kernel-sum plan
 int slot_scales_prepare(gp_plan* p);                                    // refresh the per-slot scales (sum / low-rank plans only)
 int sum_kmv_launch(gp_plan* p, const float* V16, const int* done_flag); // one launch per term into the parent's partial slots
+int product_pack(gp_plan* p);                                           // product.cu: validation / geometry / scale of a kernel product
+int product_refresh(gp_plan* p);                                        // re-pack when a factor was re-packed since (host compare)
+int product_kmv_launch(gp_plan* p, const float* V16, const int* done_flag);   // one launch: prod_f k_f V into the plan's partial slots
+int product_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);   // the factors' rows multiplied in order
+int product_kdiag_cross(gp_plan* p, float* OUT);                        // diagonal of a cross product: the factors' diagonals multiplied
+int product_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+#define GP_REFUSE_PRODUCT(p, what) \
+  GP_REQUIRE((p)->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "%s is not available on a kernel-product plan (gp_plan_set_product)", what)
 int lowrank_partials(gp_plan* p, const float* V16, const int* done_flag);   // lowrank.cu: -U U^T V into the last slot (no-op without U)
 int lowrank_kdiag(gp_plan* p, float* OUT);                              // OUT[i] -= sum_j U_ij^2
 int lowrank_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);   // OUT[r] -= U[idx_r] U^T
@@ -301,6 +316,7 @@ int kmv_tc_launch_cols(gp_plan* p, int kind, const float* XA, const float* XB, c
                        int64_t tiles_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag);
 int kmv_simt_launch_cols(gp_plan* p, int kind, const float* Z1, const float* Z2, const float* V16, float* partial, int64_t n2,
                          int64_t cols_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag);
+int sum_partials_double(gp_plan* p, const double* in, int64_t nblk, int stride, int nout, double* out);   // out[o] = sum_b in[b][o], NaN when xbad
 int64_t bilinear_blocks(const gp_plan* p, int64_t n2);                      // CTAs of one SIMT derivative launch over n2 columns
 int bilinear_launch_cols(gp_plan* p, bool ard, const float* Z1, const float* Z2, const float* L16, const float* R16, int64_t n2,
                          int64_t diag_row_begin, double* gout, int gstride, int64_t* nblk_out);
@@ -347,7 +363,9 @@ inline const float* part_scale_ptr(gp_plan* p) {
 }
 #define GP_REFUSE_LOWRANK(p, what) \
   GP_REQUIRE((p)->lr_U == nullptr, GP_E_STATE, "%s is not available on a plan with a low-rank correction (gp_plan_set_lowrank)", what)
-inline bool plan_is_tc(const gp_plan* p) { return p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_tc); }
+inline bool plan_is_tc(const gp_plan* p) {
+  return p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_tc) || (p->backend == GP_BACKEND_PRODUCT && p->prod_tc);
+}
 
 __host__ __device__ inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
@@ -410,6 +428,43 @@ __device__ __forceinline__ float dcov_from_arg(float a, float* kout) {
     if (KIND == GP_MATERN32) { *kout = fmaf(rho, e, e); return m * e; }
     *kout = fmaf(fmaf(rho, 0.33333334f, 1.f), rho, 1.f) * e;
     return (rho + 1.f) * m * 0.33333334f * e;
+  }
+}
+// Product form of the same covariances, for kernel products (product.cu).  In the packed units every kind is poly(rho) 2^e:
+//   RBF     poly = 1, e = a;     Matern   rho = sqrt(-a), e = -log2e rho, poly = 1 + c1 rho + c2 rho^2
+// with (c1, c2) = (0, 0) nu = 1/2, (1, 0) nu = 3/2, (1, 1/3) nu = 5/2, so  prod_f k_f = (prod_f poly_f) ex2(sum_f e_f): one ex2
+// per pair whatever the number of factors, plus one sqrt per Matern factor.  l dk/dl has the same shape, gpoly(rho) 2^e with
+//   RBF  gpoly = -2 a / log2e;   Matern  gpoly = rho (poly - poly') = rho ((1 - c1) + (c1 - 2 c2) rho + c2 rho^2)
+// (dcov_from_arg's rho, rho^2, (1 + rho) rho^2 / 3).  CLAMP = false leaves an RBF argument unclamped, as cov_tc does.
+struct CovPoly {
+  float c1, c2;
+};
+__host__ __device__ inline CovPoly cov_poly_of(int kind) {
+  return kind == GP_MATERN32 ? CovPoly{1.f, 0.f} : kind == GP_MATERN52 ? CovPoly{1.f, 0.33333334f} : CovPoly{0.f, 0.f};
+}
+template <bool CLAMP>
+__device__ __forceinline__ void cov_poly_exp(bool rbf, CovPoly c, float a, float* poly, float* e) {
+  if (rbf) {
+    *poly = 1.f;
+    *e = CLAMP ? fminf(a, 0.f) : a;
+  } else {
+    const float rho = sqrt_approx(fmaxf(-a, 0.f));
+    *poly = fmaf(fmaf(c.c2, rho, c.c1), rho, 1.f);
+    *e = -LOG2E * rho;
+  }
+}
+// the same with the derivative polynomial gpoly (l dk/dl = gpoly 2^e for a scalar lengthscale)
+__device__ __forceinline__ void dcov_poly_exp(bool rbf, CovPoly c, float a, float* poly, float* gpoly, float* e) {
+  if (rbf) {
+    const float am = fminf(a, 0.f);
+    *poly = 1.f;
+    *gpoly = (-2.f / LOG2E) * am;
+    *e = am;
+  } else {
+    const float rho = sqrt_approx(fmaxf(-a, 0.f));
+    *poly = fmaf(fmaf(c.c2, rho, c.c1), rho, 1.f);
+    *gpoly = rho * fmaf(fmaf(c.c2, rho, c.c1 - 2.f * c.c2), rho, 1.f - c.c1);
+    *e = -LOG2E * rho;
   }
 }
 // input-derivative factor q = dk/da of the same covariance (xgrad.cu): dk/dz_i = -q (z_i - z_j) in the packed units.

@@ -128,6 +128,11 @@ static int kmv_partials_base(gp_plan* p, const float* V16, const int* done_flag)
   if (p->deriv) return deriv_kmv_partials(p, V16, done_flag);
   if (p->tasks) return tasks_kmv_partials(p, V16, p->kind, done_flag);
   if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, V16, done_flag);
+  if (p->backend == GP_BACKEND_PRODUCT) {
+    GP_CHECK(product_refresh(p));   // before the V tiles are packed: a re-packed factor can change the backend
+    if (p->prod_tc) GP_CHECK(pack_v_tiles(p, V16));
+    return product_kmv_launch(p, V16, done_flag);
+  }
   if (p->backend == GP_BACKEND_SUM) {
     if (p->sum_any_tc) GP_CHECK(pack_v_tiles(p, V16));
     return sum_kmv_launch(p, V16, done_flag);
@@ -341,6 +346,13 @@ __global__ void bilin_dot_kernel(const float* __restrict__ partial, int nsplit, 
   if (threadIdx.x == 0) gout[(int64_t)blockIdx.x * gstride + o] = red[0];
 }
 
+int sum_partials_double(gp_plan* p, const double* in, int64_t nblk, int stride, int nout, double* out) {
+  sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(in, nblk, stride, nout, out, p->xbad);
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
 struct BilinLaunch {
   const float* Z1;
   const float* Z2;
@@ -413,6 +425,7 @@ extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, i
   GP_REQUIRE(p->backend != GP_BACKEND_SUM || p->lr_U, GP_E_SHAPE, "row extraction of a kernel sum: call gp_krows on every term and add");
   GP_REQUIRE(m >= 0 && ldo >= p->n2, GP_E_SHAPE, "bad krows shape");
   if (m == 0) return GP_OK;
+  if (p->backend == GP_BACKEND_PRODUCT) return product_krows(p, idx, m, OUT, ldo);
   if (p->kron) return kron_krows(p, idx, m, OUT, ldo);
   if (p->deriv) return deriv_krows(p, idx, m, OUT, ldo);
   if (p->lr_U) {   // rows of the operator the plan multiplies: s K - U U^T
@@ -444,6 +457,10 @@ static int kdiag_base(gp_plan* p, float* OUT);
 extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_REQUIRE(p->backend != GP_BACKEND_SUM || p->lr_U, GP_E_SHAPE, "diagonal of a kernel sum: call gp_kdiag on every term and add");
+  if (p->backend == GP_BACKEND_PRODUCT) {   // square: the constant S = prod_f s_f (kdiag_base); cross: the factors' diagonals
+    GP_CHECK(product_refresh(p));
+    if (!p->same) return product_kdiag_cross(p, OUT);
+  }
   if (p->kron) return kron_kdiag(p, OUT);
   if (p->deriv) return deriv_kdiag(p, OUT);
   if (p->lr_U) {   // diag(s K) - sum_j U_ij^2
@@ -495,6 +512,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   // a single row is read at offset 0 only, so it may carry any row stride
   GP_REQUIRE((ldl >= s || p->row_count == 1) && (ldr >= s || p->n2 == 1), GP_E_SHAPE,
              "gp_bilinear_grad: leading dimensions must be >= s (ldl=%lld, ldr=%lld, s=%d)", (long long)ldl, (long long)ldr, s);
+  if (p->backend == GP_BACKEND_PRODUCT) return product_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->kron) return kron_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->deriv) return deriv_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   // before any launch: the SIMT derivative kernel is instantiated up to DP = 64

@@ -322,6 +322,7 @@ int kmv_tc_launch_cols(gp_plan* p, int kind, const float* XA, const float* XB, c
 }
 int kmv_tc_launch(gp_plan* p, const int* done_flag) {
   if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, nullptr, done_flag);   // all terms on tensor cores (plan_is_tc)
+  if (p->backend == GP_BACKEND_PRODUCT) return product_kmv_launch(p, nullptr, done_flag);   // two tensor-core factors (plan_is_tc)
   return kmv_tc_launch_kind(p, p->kind, done_flag);
 }
 

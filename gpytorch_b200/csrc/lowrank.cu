@@ -182,6 +182,7 @@ extern "C" int gp_plan_set_lowrank(gp_plan* p, const float* U, int64_t ldu, int 
   GP_REFUSE_TASKS(p, "gp_plan_set_lowrank");
   GP_REFUSE_KRON(p, "gp_plan_set_lowrank");
   GP_REFUSE_DERIV(p, "gp_plan_set_lowrank");
+  GP_REFUSE_PRODUCT(p, "gp_plan_set_lowrank");
   GP_REQUIRE(r >= 1 && r <= LR_RMAX, GP_E_SHAPE, "low-rank correction of rank %d: 1 <= r <= %d", r, LR_RMAX);
   GP_REQUIRE(ldu >= r, GP_E_SHAPE, "low-rank correction: ldu=%lld < r=%d", (long long)ldu, r);
   GP_REQUIRE(p->same, GP_E_SHAPE, "a low-rank correction needs a square operator (X2 == X1)");

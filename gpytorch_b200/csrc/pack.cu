@@ -154,9 +154,14 @@ int choose_geometry(gp_plan* p) {
   p->rows_pad = cdiv(p->row_count, 2 * TILE_I) * 2 * TILE_I;
   p->ntile_i = p->rows_pad / TILE_I;
   p->ntile_j = cdiv(p->n2, TILE_J);
-  // column splits: pick the smallest nsplit whose unit count fills the SMs best
-  int64_t nti = (p->backend == GP_BACKEND_TCGEN05) ? p->ntile_i : cdiv(p->row_count, SIMT_TI);
-  int64_t ntj = (p->backend == GP_BACKEND_TCGEN05) ? p->ntile_j : cdiv(p->n2, SIMT_TJ);
+  choose_splits(p, p->backend == GP_BACKEND_TCGEN05);
+  return GP_OK;
+}
+
+// column splits: pick the smallest nsplit whose unit count fills the SMs best
+void choose_splits(gp_plan* p, bool tc) {
+  int64_t nti = tc ? p->ntile_i : cdiv(p->row_count, SIMT_TI);
+  int64_t ntj = tc ? p->ntile_j : cdiv(p->n2, SIMT_TJ);
   int best = 1;
   double best_eff = -1.0;
   for (int s = 1; s <= 16; ++s) {
@@ -167,14 +172,13 @@ int choose_geometry(gp_plan* p) {
     // 2 slots per SM on the tensor-core path: the K.V kernel now runs one 384-thread CTA per SM, but the factor is kept so
     // that the work units -- and with them the split of every row sum into partials, hence the results bit for bit -- stay
     // what they were
-    const int64_t slots = (int64_t)p->n_sm * (p->backend == GP_BACKEND_TCGEN05 ? 2 : 1);
+    const int64_t slots = (int64_t)p->n_sm * (tc ? 2 : 1);
     int64_t waves = cdiv(units, slots);
     double eff = (double)(nti * ntj) / (double)(waves * slots * per);
     if (eff > best_eff + 0.02) { best_eff = eff; best = s; }
   }
   p->tiles_per_split = cdiv(ntj, best);
   p->nsplit = (int)cdiv(ntj, p->tiles_per_split);  // no empty splits
-  return GP_OK;
 }
 
 int pack_inputs(gp_plan* p) {
@@ -183,6 +187,8 @@ int pack_inputs(gp_plan* p) {
   if (p->backend_req == GP_BACKEND_SUM) return sum_pack(p);
   if (p->backend_req == GP_BACKEND_KRON) return kron_pack(p);
   if (p->backend_req == GP_BACKEND_DERIV) return deriv_pack(p);
+  if (p->backend_req == GP_BACKEND_PRODUCT) return product_pack(p);
+  p->pack_gen++;   // a kernel product over this plan re-reads its scale, geometry and flag (product.cu)
   GP_CHECK(choose_geometry(p));
   cudaStream_t st = p->stream;
   const int d = p->d, DP = p->DP;

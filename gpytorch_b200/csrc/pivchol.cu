@@ -195,6 +195,8 @@ constexpr int PC_KIND_TASK = 66;
 // derivative observations (deriv.cu): row r is point r / rep, component r mod rep (rep = d + 1); the entry of rows (a, b) is the
 // RBF value / gradient block entry with u_c = dz_c w[c] and 1 / l_c^2 = il2[c] from dh (a DerivHyp on the device)
 constexpr int PC_KIND_DERIV = 67;
+// kernel products (GP_BACKEND_PRODUCT): K[pivot, j] = S prod_f k_f(|z_f,pivot - z_f,j|^2), the sum's staging and loop with a multiply
+constexpr int PC_KIND_PRODUCT = 68;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -250,7 +252,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
   auto better = [](float v2, int p2, float v1, int p1) { return v2 > v1 || (v2 == v1 && p2 < p1); };
   for (int m = 0; m < max_rank; ++m) {
     if (tid == 0) s_old = -1;
-    if (KIND == PC_KIND_SUM) {   // DP = sum of the terms' widths: the pivot rows of all terms back to back
+    if (KIND == PC_KIND_SUM || KIND == PC_KIND_PRODUCT) {   // DP = sum of the terms' widths: the pivot rows of all terms back to back
       int off = 0;
       for (int t = 0; t < tt.n; ++t) {
         for (int c = tid; c < tt.DP[t]; c += PCP_THREADS) zp[off + c] = tt.Z[t][(int64_t)pi * tt.DP[t] + c];
@@ -293,6 +295,19 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
               s = fmaf(df, df, s);
             }
             v = fmaf(tt.os[t], pc_cov_rt(tt.kind[t], -0.5f * s), v);
+            off += tt.DP[t];
+          }
+        } else if (KIND == PC_KIND_PRODUCT) {
+          v = os;
+          int off = 0;
+          for (int t = 0; t < tt.n; ++t) {
+            const float* zj = tt.Z[t] + j * tt.DP[t];
+            float s = 0.f;
+            for (int c = 0; c < tt.DP[t]; ++c) {
+              float df = zp[off + c] - zj[c];
+              s = fmaf(df, df, s);
+            }
+            v *= pc_cov_rt(tt.kind[t], -0.5f * s);
             off += tt.DP[t];
           }
         } else if (KIND == PC_KIND_SKI) {
@@ -782,6 +797,8 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_REFUSE_LOWRANK(p, "gp_pivoted_cholesky");
   GP_REQUIRE(p->same, GP_E_SHAPE, "pivoted Cholesky needs a square operator");
   GP_CHECK(slot_scales_prepare(p));
+  const bool prod = p->backend == GP_BACKEND_PRODUCT;
+  if (prod) GP_CHECK(product_refresh(p));   // S = prod_f s_f into p->outputscale
   const int64_t n = p->n2;
   GP_REQUIRE(n < (int64_t)1 << 31, GP_E_SHAPE, "n too large");
   rank = (int)std::min<int64_t>(rank, n);
@@ -818,6 +835,12 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       tt.kind[t] = q->kind; tt.DP[t] = q->DP; tt.os[t] = q->outputscale; tt.Z[t] = q->Z2.as<float>();
       os_total += q->outputscale;
       dp_total += q->DP;
+    }
+  } else if (prod) {   // os_total = S, dp_total = the factors' widths back to back (product_pack)
+    tt.n = (int)p->factors.size();
+    for (int t = 0; t < tt.n; ++t) {
+      const gp_plan* q = p->factors[t];
+      tt.kind[t] = q->kind; tt.DP[t] = q->DP; tt.Z[t] = q->Z2.as<float>();
     }
   }
   const bool kron = p->kron != nullptr;
@@ -861,24 +884,26 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     pc_init_kernel<<<gb, PC_THREADS, 0, st>>>(diag, perm, pos, n, os_total, S, piv);   // stationary terms: constant initial diagonal
     p->launches += 1;
   }
-  const float* Z = (sum || ski) ? nullptr : Zsrc;
+  const float* Z = (sum || ski || prod) ? nullptr : Zsrc;
   const bool stepwise = getenv("GP_PC_STEPWISE") != nullptr;   // debugging / A-B switch: one launch per step
   int coop = 0;
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, p->device);
   GP_REQUIRE(!sum || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a kernel sum needs the cooperative kernel");
+  GP_REQUIRE(!prod || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a kernel product needs the cooperative kernel");
   GP_REQUIRE(!ski || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a SKI operator needs the cooperative kernel");
   GP_REQUIRE(!tasks || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a multitask operator needs the cooperative kernel");
   GP_REQUIRE(!deriv || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a derivative operator needs the cooperative kernel");
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : ski ? PC_KIND_SKI : deriv ? PC_KIND_DERIV : tasks ? PC_KIND_TASK : p->kind) {
+    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? PC_KIND_DERIV : tasks ? PC_KIND_TASK : p->kind) {
       case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
       case PC_KIND_DERIV: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_DERIV>; break;
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
       case GP_MATERN12: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN12>; break;
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
       case PC_KIND_SUM: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SUM>; break;
+      case PC_KIND_PRODUCT: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_PRODUCT>; break;
       case PC_KIND_SKI: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SKI>; break;
       default: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN52>; break;
     }
@@ -1039,6 +1064,7 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   GP_CUDA(cudaGetLastError());
   // tr(K - L L^T): the diagonal of a stationary kernel (sum) is its (summed) outputscale, as gp_kdiag fills it; the SKI diagonal
   // w_i^T K_uu w_i varies from row to row and is summed in fp64
+  if (p->backend == GP_BACKEND_PRODUCT) GP_CHECK(product_refresh(p));   // the constant diagonal S = prod_f s_f
   double tr_k = (double)n * p->outputscale;
   if (p->backend == GP_BACKEND_SUM) {
     double os_total = 0.0;

@@ -1350,6 +1350,7 @@ extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* g
   GP_REFUSE_TASKS(p, "gp_plan_set_ski");
   GP_REFUSE_KRON(p, "gp_plan_set_ski");
   GP_REFUSE_DERIV(p, "gp_plan_set_ski");
+  GP_REFUSE_PRODUCT(p, "gp_plan_set_ski");
   GP_REQUIRE(d == p->d && d >= 1 && d <= SKI_MAXD, GP_E_SHAPE, "SKI: grid dimension %d does not match the data (d=%d, max %d)", d, p->d, SKI_MAXD);
   int64_t M = 1;
   bool large = false;
@@ -1382,6 +1383,7 @@ extern "C" int gp_ski_input_grad(gp_plan* p, const float* L, int64_t ldl, const 
   GP_REFUSE_TASKS(p, "gp_ski_input_grad");
   GP_REFUSE_KRON(p, "gp_ski_input_grad");
   GP_REFUSE_DERIV(p, "gp_ski_input_grad");
+  GP_REFUSE_PRODUCT(p, "gp_ski_input_grad");
   GP_REQUIRE(L && R && DX && lddx >= p->d, GP_E_SHAPE, "gp_ski_input_grad: bad output (leading dimension %lld, d=%d)", (long long)lddx, p->d);
   return ski_with_d(p->d, [&](auto D) { return ski_input_grad_d<D>(p, L, ldl, R, ldr, t, DX, lddx); });
 }

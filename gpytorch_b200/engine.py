@@ -190,6 +190,17 @@ class Plan:
             check(self.lib.gp_plan_set_sum(self._h, arr, len(terms)))
         return self
 
+    def set_product(self, factors):
+        """Kernel product (ProductKernel): this plan's operator becomes S prod_f K_f (+ its own noise), S the product of the
+        factors' outputscales.  `factors` are 2 to 4 ready plain plans over the same rows (their own kind / lengthscales /
+        outputscale / active dimensions); they must outlive this plan.  set_hypers on this plan supplies the noise only."""
+        factors = list(factors)
+        arr = (C.c_void_p * max(len(factors), 1))(*[f._h.value for f in factors])
+        self._factors = factors                   # keep them alive
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_product(self._h, arr, len(factors)))
+        return self
+
     def set_noise_diag(self, diag: torch.Tensor | None):
         """Per-row noise variances (FixedNoiseGaussianLikelihood): K_hat = K + diag(d).  None restores the scalar noise."""
         if diag is None:
@@ -279,7 +290,7 @@ class Plan:
     def info(self):
         b, s, k, m = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         check(self.lib.gp_plan_info(self._h, C.byref(b), C.byref(s), C.byref(k), C.byref(m)))
-        return {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum", 5: "kron", 6: "deriv"}.get(b.value, "?"), "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
+        return {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum", 5: "kron", 6: "deriv", 7: "product"}.get(b.value, "?"), "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
 
     def time_kmv_kernel(self, v: torch.Tensor, warmup: int = 3, reps: int = 20) -> float:
         """Average device time (ms) of ONE launch of the fused K.V kernel alone (CUDA events on the plan stream)."""
@@ -315,7 +326,8 @@ class Plan:
         return out
 
     def bilinear_grad(self, left: torch.Tensor, right: torch.Tensor):
-        """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right)) for left [row_count, s], right [n2, s]."""
+        """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right)) for left [row_count, s], right [n2, s].  On a kernel
+        product: the factors' lengthscale gradients one after the other, and the gradient of the combined scale S."""
         if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.row_count or right.size(0) != self.n2 \
                 or left.size(1) != right.size(1) or left.size(1) < 1:
             raise RuntimeError(f"bilinear_grad: left must be [{self.row_count}, s] and right [{self.n2}, s] with s >= 1 "
@@ -327,7 +339,8 @@ class Plan:
                 raise RuntimeError(f"{name} lives on {t.device}, the plan on {self.device}")
         left, right = _row_block(left), _row_block(right)
         s = left.size(1)
-        nls = len(self.lengthscale)
+        factors = getattr(self, "_factors", None)
+        nls = sum(len(f.lengthscale) for f in factors) if factors else len(self.lengthscale)
         gl = (C.c_double * nls)()
         go = C.c_double()
         with torch.cuda.device(self.device):

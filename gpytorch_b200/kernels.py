@@ -1,5 +1,5 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, ScaleKernel, AdditiveKernel, GridInterpolationKernel} for the
-accelerated path.
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, ScaleKernel, AdditiveKernel, ProductKernel,
+GridInterpolationKernel} for the accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
 rbf_kernel.py:68-85; matern_kernel.py:79-110; scale_kernel.py:64-118), but `forward` returns an
@@ -56,6 +56,13 @@ class Kernel(Module):
         for k in (self, other):
             parts.extend(k.kernels if isinstance(k, AdditiveKernel) else (k,))
         return AdditiveKernel(*parts)
+
+    def __mul__(self, other):
+        # k1 * k2 -> ProductKernel with nested products flattened (kernels/kernel.py:547-551)
+        parts = []
+        for k in (self, other):
+            parts.extend(k.kernels if isinstance(k, ProductKernel) else (k,))
+        return ProductKernel(*parts)
 
     def _batch_size(self):
         return self.batch_shape[0] if len(self.batch_shape) else None
@@ -197,6 +204,15 @@ class ScaleKernel(Kernel):
             scaled = [KernelLinearOperator(t.x1, t.x2, t.kind, t.lengthscale, self.outputscale * t.outputscale) for t in terms]
             op = scaled[0] if len(scaled) == 1 else SumKernelLinearOperator(scaled)
             return op.diagonal() if diag else op
+        if isinstance(self.base_kernel, ProductKernel):
+            # s (k_1 ... k_m): the scale is folded into the first factor's outputscale (autograd sees the product)
+            from .operators import ProductKernelLinearOperator
+            if _batch_index is not None:
+                raise NotImplementedError("batched ScaleKernel over a ProductKernel")
+            f = self.base_kernel(x1, None if _same else x2).ops
+            first = KernelLinearOperator(f[0].x1, f[0].x2, f[0].kind, f[0].lengthscale, self.outputscale * f[0].outputscale)
+            op = ProductKernelLinearOperator([first, *f[1:]])
+            return op.diagonal() if diag else op
         if isinstance(self.base_kernel, GridInterpolationKernel):
             base = self.base_kernel.forward(x1, x2, diag=False, _same=_same, **params)
         else:
@@ -236,6 +252,8 @@ class AdditiveKernel(Kernel):
                 raise RuntimeError("AdditiveKernel components must be kernels")
             if len(k.batch_shape):
                 raise NotImplementedError("batched components of an AdditiveKernel")
+            if isinstance(k, ProductKernel) or isinstance(getattr(k, "base_kernel", None), ProductKernel):
+                raise NotImplementedError("sums that contain a ProductKernel are not available on the accelerated path")
         self.kernels = torch.nn.ModuleList(kernels)
 
     def forward(self, x1, x2, diag=False, **params):
@@ -252,6 +270,43 @@ class AdditiveKernel(Kernel):
         if any(isinstance(t, SKIKernelLinearOperator) or not isinstance(t, KernelLinearOperator) for t in terms):
             raise NotImplementedError("AdditiveKernel components must be RBF / Matern kernels (optionally scaled) on the accelerated path")
         return terms[0] if len(terms) == 1 else SumKernelLinearOperator(terms)
+
+
+class ProductKernel(Kernel):
+    """k = k_1 * ... * k_m (kernels/kernel.py:634-690).  Every factor is called on the full inputs (so its own active_dims apply, as
+    in the reference) and must be an RBFKernel / MaternKernel, optionally inside a ScaleKernel; the product is ONE
+    ProductKernelLinearOperator whose products / solves run natively (gp_plan_set_product), not a dense multiplication.  2 to 4
+    unbatched factors."""
+
+    def __init__(self, *kernels):
+        super().__init__()
+        if len(kernels) > 4:
+            raise NotImplementedError(f"a ProductKernel takes up to 4 factors on the accelerated path (got {len(kernels)})")
+        for k in kernels:
+            if not isinstance(k, Kernel):
+                raise RuntimeError("ProductKernel factors must be kernels")
+            base = k.base_kernel if isinstance(k, ScaleKernel) else k
+            if not isinstance(base, _StationaryKernel) or isinstance(base, RBFKernelGrad):
+                raise NotImplementedError("ProductKernel factors must be RBF / Matern kernels (optionally scaled) on the accelerated "
+                                          "path: sums, SKI, multitask and derivative kernels inside a product are not available")
+            if len(k.batch_shape):
+                raise NotImplementedError("batched factors of a ProductKernel")
+        self.kernels = torch.nn.ModuleList(kernels)
+
+    def forward(self, x1, x2, diag=False, **params):
+        raise NotImplementedError("ProductKernel dispatches to its factors in __call__")
+
+    def __call__(self, x1, x2=None, diag=False, **params):
+        from .operators import ProductKernelLinearOperator
+        if x1.dim() == 3 or (x2 is not None and x2.dim() == 3):
+            raise NotImplementedError("batched inputs of a ProductKernel")
+        factors = [k(x1, x2, diag=diag, **params) for k in self.kernels]
+        if diag:
+            out = factors[0]
+            for t in factors[1:]:
+                out = out * t
+            return out
+        return factors[0] if len(factors) == 1 else ProductKernelLinearOperator(factors)
 
 
 class IndexKernel(Module):

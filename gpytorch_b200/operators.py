@@ -83,6 +83,8 @@ def clear_plan_cache():
     with _PLAN_LOCK:
         while _SUM_PLANS:
             _SUM_PLANS.popitem()[1].close()
+        while _PRODUCT_PLANS:
+            _PRODUCT_PLANS.popitem()[1].close()
         while _KRON_PLANS:
             _KRON_PLANS.popitem()[1].close()
         while _DERIV_PLANS:
@@ -427,7 +429,7 @@ class KernelLinearOperator(_SamplingMixin):
     def __add__(self, other):
         if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
             return AddedDiagLinearOperator(self, other)
-        if isinstance(other, KernelLinearOperator) and not isinstance(other, SKIKernelLinearOperator) \
+        if isinstance(other, KernelLinearOperator) and not isinstance(other, (SKIKernelLinearOperator, ProductKernelLinearOperator)) \
                 and not isinstance(self, SKIKernelLinearOperator):
             return SumKernelLinearOperator([self, other])     # K_1 + K_2 stays lazy: one engine operator (csrc/sum.cu)
         raise NotImplementedError("a kernel operator adds a (Constant)DiagLinearOperator or another kernel operator")
@@ -437,7 +439,11 @@ class KernelLinearOperator(_SamplingMixin):
 
     def mul(self, other):
         """K o B[t, t'] with an IndexKernel's operator (the Hadamard multitask model, covar_x.mul(covar_i)): one engine operator
-        (gp_plan_set_tasks).  RBF / Matern operators, optionally scaled, only."""
+        (gp_plan_set_tasks).  RBF / Matern operators, optionally scaled, only.  With another RBF / Matern kernel operator (or a
+        product of them) of the same shape: the elementwise product K_1 o K_2 as one engine operator (gp_plan_set_product)."""
+        plain = (KernelLinearOperator, ProductKernelLinearOperator)
+        if type(self) in plain and type(other) in plain:
+            return ProductKernelLinearOperator([self, other])
         if not isinstance(other, IndexLinearOperator) or type(self) is not KernelLinearOperator:
             raise NotImplementedError("the accelerated path multiplies an RBF / Matern kernel operator (optionally scaled) by an "
                                       "IndexKernel operator only")
@@ -975,6 +981,135 @@ class SumKernelLinearOperator(KernelLinearOperator):
 _SUM_PLANS: "dict[tuple, Plan]" = {}
 
 
+class ProductKernelLinearOperator(KernelLinearOperator):
+    """K_1 o ... o K_m over the same inputs (ProductKernel, kernels/kernel.py:634-690).  The reference evaluates every factor
+    densely and multiplies the matrices; here the product is ONE engine operator (gp_plan_set_product): a product with a block of
+    vectors is one fused kernel launch that forms prod_f k_f per pair in registers, the solves / preconditioner / SLQ run on it, and
+    one engine call returns every factor's hyper-parameter gradients.  2 to 4 RBF / Matern factors; gradients with respect to the
+    inputs are not available through a product."""
+
+    def __init__(self, ops):
+        flat = []
+        for o in ops:
+            flat.extend(o.ops if isinstance(o, ProductKernelLinearOperator) else [o])
+        if not 2 <= len(flat) <= 4:
+            raise NotImplementedError(f"a kernel product takes 2 to 4 factors on the accelerated path (got {len(flat)})")
+        first = flat[0]
+        for o in flat:
+            if type(o) is not KernelLinearOperator:
+                raise NotImplementedError("the factors of a kernel product must be RBF / Matern kernel operators (optionally scaled) "
+                                          "on the accelerated path")
+            if o.shape != first.shape or o.same != first.same:
+                raise RuntimeError(f"cannot multiply kernels of shapes {tuple(first.shape)} and {tuple(o.shape)}")
+            if o._comm is not None or o._row_begin != 0 or o._row_count not in (0, o.shape[0]):
+                raise NotImplementedError("a row-sharded kernel product is not available on the accelerated path")
+            if o.x1.requires_grad or (not o.same and o.x2.requires_grad):
+                raise NotImplementedError("gradients with respect to the inputs of a kernel product (deep kernel learning, test-input "
+                                          "gradients) are not available on the accelerated path")
+        # one engine plan per factor even when the factors see the same inputs: re-wrap and give each its own plan-cache slot
+        self.ops = []
+        for i, o in enumerate(flat):
+            t = KernelLinearOperator(o.x1, o.x2, o.kind, o.lengthscale, o.outputscale)
+            t._plan_slot = 5 + i
+            self.ops.append(t)
+        self.x1, self.x2, self.same = first.x1, first.x2, first.same
+        self.kind = "product"
+        self.lengthscale, self.outputscale = first.lengthscale, first.outputscale   # representative only (device / dtype)
+        self._comm, self._row_begin, self._row_count = None, 0, 0
+        self._plan = None
+
+    def hyper_tensors(self):
+        return [t for o in self.ops for t in o.hyper_tensors()]
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    @staticmethod
+    def _split_grads(gl, go, n_ls, scales):
+        """The engine's flat result (the factors' lengthscale gradients one after the other, dF/dS of the combined scale
+        S = prod_f s_f) as per-factor pairs: (lengthscale gradient [n_ls_f], dF/ds_f = S / s_f dF/dS)."""
+        S = 1.0
+        for s in scales:
+            S *= s
+        out, k = [], 0
+        for n, s in zip(n_ls, scales):
+            out.append((gl[k:k + n], go * S / s))
+            k += n
+        return out
+
+    def _bilinear_derivative_list(self, left, right):
+        gl, go = self.plan(0.0).bilinear_grad(left, right)
+        parts = self._split_grads(gl, go, [o.lengthscale.numel() for o in self.ops], [o._host_hypers()[1] for o in self.ops])
+        out = []
+        for o, (g, gs) in zip(self.ops, parts):
+            out.append(torch.tensor(g, device=self.device, dtype=self.dtype).reshape(o.lengthscale.shape))
+            out.append(torch.tensor(gs, device=self.device, dtype=self.dtype).reshape(o.outputscale.shape))
+        return out
+
+    def _bilinear_derivative(self, left, right):
+        raise NotImplementedError("a kernel product has one (lengthscale, outputscale) pair per factor: use _bilinear_derivative_list")
+
+    @property
+    def requires_grad(self):
+        return any(o.requires_grad for o in self.ops)
+
+    def representation(self):
+        return tuple(t for o in self.ops for t in o.representation())
+
+    def plan(self, noise=0.0) -> Plan:
+        factors = [o.plan(0.0) for o in self.ops]
+        nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
+        with _PLAN_LOCK:
+            key = ("product", tuple(id(f) for f in factors))
+            parent = _PRODUCT_PLANS.pop(key, None)
+            if parent is None:
+                parent = Plan(self.x1, None if self.same else self.x2, backend="auto")
+                parent._hyp_key = None
+            elif parent.x1.data_ptr() != self.x1.data_ptr():
+                # the factor plans were re-pointed to new inputs (_get_plan_locked): follow them
+                parent.x1 = self.x1.contiguous()
+                parent.x2 = parent.x1 if self.same else self.x2.contiguous()
+                parent.refresh_data()
+            _PRODUCT_PLANS[key] = parent
+            while len(_PRODUCT_PLANS) > 16:
+                _PRODUCT_PLANS.pop(next(iter(_PRODUCT_PLANS))).close()
+        # the factors may have been re-created / re-packed since the last use: (re-)attach them every time (validation only),
+        # then set the noise of the product
+        parent.set_product(factors)
+        if parent._hyp_key != nz:
+            parent.set_hypers("rbf", [1.0], 1.0, nz)
+            parent._hyp_key = nz
+        self._plan = parent
+        return parent
+
+    def _transpose_nonbatch(self):
+        return self if self.same else ProductKernelLinearOperator([o._transpose_nonbatch() for o in self.ops])
+
+    def detach(self):
+        return ProductKernelLinearOperator([o.detach() for o in self.ops])
+
+    def __getitem__(self, index):
+        parts = [o[index] for o in self.ops]
+        if torch.is_tensor(parts[0]):
+            out = parts[0]
+            for t in parts[1:]:
+                out = out * t
+            return out
+        return ProductKernelLinearOperator(parts)
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("a kernel product adds a (Constant)DiagLinearOperator only: sums that contain products are not "
+                                  "available on the accelerated path")
+
+
+_PRODUCT_PLANS: "dict[tuple, Plan]" = {}
+
+
 class SKIKernelLinearOperator(KernelLinearOperator):
     """K_ski = s W (T_0 x ... x T_{d-1}) W^T (kernels/grid_interpolation_kernel.py:132-213): the engine's SKI backend -- cubic
     interpolation weights kept in compact per-dimension form, Kronecker / Toeplitz grid covariance applied mode by mode."""
@@ -1177,7 +1312,8 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
         """A plan-backed non-SKI kernel operator (or kernel sum) without batch dimension on an unsharded square plan."""
         return (isinstance(base, KernelLinearOperator) and not isinstance(base, (SKIKernelLinearOperator, HadamardKernelLinearOperator,
                                                                                           KroneckerKernelLinearOperator,
-                                                                                          DerivKernelLinearOperator))
+                                                                                          DerivKernelLinearOperator,
+                                                                                          ProductKernelLinearOperator))
                 and base.same
                 and base._comm is None and base._row_begin == 0 and base._row_count in (0, base.shape[0]))
 

@@ -48,7 +48,7 @@ enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3 };
  * GP_BACKEND_SIMT = fp32 CUDA-core kernel (bring-up / cross-check / d > 41). */
 enum { GP_BACKEND_AUTO = 0, GP_BACKEND_TCGEN05 = 1, GP_BACKEND_SIMT = 2, GP_BACKEND_SKI = 3 /* set by gp_plan_set_ski */,
        GP_BACKEND_SUM = 4 /* set by gp_plan_set_sum */, GP_BACKEND_KRON = 5 /* set by gp_plan_set_kron */,
-       GP_BACKEND_DERIV = 6 /* set by gp_plan_set_deriv */ };
+       GP_BACKEND_DERIV = 6 /* set by gp_plan_set_deriv */, GP_BACKEND_PRODUCT = 7 /* set by gp_plan_set_product */ };
 
 typedef struct gp_plan gp_plan;   /* opaque: repacked X, workspaces, stream, comm */
 typedef struct gp_comm gp_comm;   /* opaque: NCCL communicator for row-sharded runs */
@@ -124,6 +124,25 @@ int gp_ski_input_grad(gp_plan* plan, const float* L, int64_t ldl, const float* R
  * reduced by the same finish kernels; gp_pivoted_cholesky evaluates rows of the sum.  n_terms in [1, 4].
  * Hyper-parameter gradients: gp_bilinear_grad on each term plan. */
 int gp_plan_set_sum(gp_plan* plan, gp_plan* const* terms, int n_terms);
+
+/* Kernel products (ProductKernel, kernels/kernel.py:547-551, :634-690: k = k_1 * ... * k_m, each factor with its own covariance
+ * function, lengthscale(s), outputscale and active dimensions; the reference multiplies the dense N x N matrices): `plan` becomes
+ * the operator  S prod_f k_f  (+ its own noise / per-row diagonal where a call adds it), S = prod_f s_f, where every factor is a
+ * ready plain plan (tensor-core or SIMT backend, any kind, scalar or ARD lengthscale) over the same rows, device and stream (the
+ * data pointers may differ: active_dims).  Call after gp_plan_set_data on `plan`; gp_plan_set_hypers on `plan` (before or after)
+ * supplies the noise only.  The factors stay owned by the caller and must outlive `plan`; re-packing a factor (gp_plan_set_hypers
+ * on it) is picked up by the next call on `plan`.  n_factors in [2, 4]; NULL / 0 clears.  One K.V is ONE launch that forms
+ * prod_f k_f per pair in registers with one ex2: two tensor-core factors with KP_a + KP_b <= 128 run the wgmma kernel
+ * (gp_plan_info reports kpad = KP_a + KP_b), everything else with a total padded width <= 128 the CUDA-core kernel.
+ * gp_kmv, gp_krows, gp_kdiag (square and cross), gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg, gp_slq_logdet,
+ * gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond, gp_plan_set_noise_diag and
+ * gp_time_kmv_kernel run on it.  gp_bilinear_grad returns, factor after factor, the gradients of that factor's lengthscale(s)
+ * (1 or d_f entries, sum_f n_ls_f in all; total padded width <= 64) and in grad_os dF/dS of the combined scale (dF/ds_f = S / s_f
+ * dF/dS).  A factor that is SKI, a sum, a product, multitask, derivative, low-rank-corrected or row-sharded is refused
+ * (GP_E_SHAPE / GP_E_STATE); on a product plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv, gp_plan_set_sum,
+ * gp_plan_set_ski, gp_plan_set_lowrank, gp_plan_set_backend, gp_plan_set_comm with more than one rank and the input-gradient
+ * calls return GP_E_STATE. */
+int gp_plan_set_product(gp_plan* plan, gp_plan* const* factors, int n_factors);
 
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
  * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
