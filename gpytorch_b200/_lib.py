@@ -81,6 +81,7 @@ PROTOTYPES = {
     "gp_task_covar_grad": (_I, [_P, _P, _L, _P, _L, _I, C.POINTER(C.c_double)]),
     "gp_plan_set_kron": (_I, [_P, _P, _I]),
     "gp_plan_set_deriv": (_I, [_P, _P]),
+    "gp_plan_set_deriv_kind": (_I, [_P, _P, _I]),
     "gp_ski_grid_matmul": (_I, [_P, _P, _L, _I, _P, _L]),
     "gp_ski_interp_matmul": (_I, [_P, _P, _L, _I, _P, _L]),
     "gp_ski_input_grad": (_I, [_P, _P, _L, _P, _L, _I, _P, _L]),

@@ -18,6 +18,9 @@
 //     l_c d/dl_c = s sum k [ (dz_c^2 / log2 e) F - 2 u_c (g r_c - l_c h) - 2 l_c r_c / l_c^2 ].
 // deriv_grad_kernel evaluates these per thread in fp32 over its columns and reduces every CTA in fp64; the host adds the CTA
 // partials in a fixed order.
+//
+// A plan built by gp_plan_set_deriv_kind(..., GP_MATERN52) shares this file's geometry, refresh, split sum and host reductions;
+// its entries, products, rows, diagonal and gradient come from the Matern-5/2 table of m52grad.cu.
 #include <math.h>
 #include <string.h>
 
@@ -28,8 +31,6 @@
 
 namespace gp {
 
-constexpr int DV_TI = 128;   // points per CTA, one per thread
-constexpr int DV_TJ = 64;    // staged points of the other side per step
 constexpr float DV_LN2 = 0.69314718f;   // 1 / log2 e: dz_c^2 / log2 e = D_c^2 / l_c^2
 
 // columns per CTA: (DP + 1) x TW accumulators per thread in the product (DP = 8 with 8 columns takes 201 registers and ran d = 5
@@ -273,7 +274,10 @@ static int deriv_check_data(const gp_plan* p, const gp_plan* q) {
   GP_REQUIRE(q->data_set && q->hypers_set, GP_E_STATE, "derivative plan: the data plan needs set_data + set_hypers");
   GP_REQUIRE(q->backend == GP_BACKEND_TCGEN05 || q->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
              "derivative plan: the data plan must be a plain kernel plan (not SKI, not a kernel sum, not Kronecker or derivative)");
-  GP_REQUIRE(q->kind == GP_RBF, GP_E_SHAPE, "derivative observations are available for the RBF kernel only (kind=%d)", q->kind);
+  if (p->deriv->kind == GP_MATERN52)
+    GP_REQUIRE(q->kind == GP_MATERN52, GP_E_SHAPE, "Matern-5/2 derivative plan: the data plan must be a Matern-5/2 plan (kind=%d)", q->kind);
+  else
+    GP_REQUIRE(q->kind == GP_RBF, GP_E_SHAPE, "derivative observations are available for the RBF kernel only (kind=%d)", q->kind);
   GP_REQUIRE(q->tasks == nullptr, GP_E_STATE, "derivative plan: a data plan with task indices is not available");
   GP_REQUIRE(q->lr_U == nullptr, GP_E_STATE, "derivative plan: a data plan with a low-rank correction is not available");
   GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
@@ -324,7 +328,7 @@ int deriv_refresh(gp_plan* p) {
   p->xbad = q->xbad;
   DerivHyp h;
   memset(&h, 0, sizeof(h));
-  const double rc = sqrt(1.4426950408889634);
+  const double rc = sqrt(ds->kind == GP_MATERN52 ? 10.0 : 1.4426950408889634);   // the packing constant of pack.cu
   for (int c = 0; c < q->d; ++c) {
     const double l = q->ls.size() == 1 ? q->ls[0] : q->ls[c];
     h.w[c] = (float)(1.0 / (rc * l));
@@ -348,7 +352,16 @@ int deriv_pack(gp_plan* p) {
   return GP_OK;
 }
 
-static const float* deriv_z1(const gp_plan* q) { return q->same ? q->Z2.as<float>() : q->Z1.as<float>(); }
+// the split partials of the first ncols columns, summed in order into the parent's partial slot 0
+int deriv_finish_launch(gp_plan* p, int ncols, const int* done_flag) {
+  gp_deriv_state* ds = p->deriv;
+  const int64_t rows = p->n1;
+  deriv_finish_kernel<<<(unsigned)cdiv(rows * TP, 256), 256, 0, p->stream>>>(ds->part.as<float>(), ds->nsplit, rows, ncols,
+                                                                            p->partial.as<float>(), done_flag);
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
 
 template <int DP>
 static int deriv_kmv_launch(gp_plan* p, const float* V16, int ncols, const int* done_flag) {
@@ -361,34 +374,22 @@ static int deriv_kmv_launch(gp_plan* p, const float* V16, int ncols, const int* 
   dim3 grid((unsigned)cdiv(q->n1, DV_TI), (unsigned)ds->nsplit, (unsigned)nchunk);
   deriv_kmv_kernel<DP, TW><<<grid, DV_TI, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), V16, ds->part.as<float>(), q->n1, q->n2, q->d,
                                                           ds->cps, rows, ds->hyp, done_flag);
-  deriv_finish_kernel<<<(unsigned)cdiv(rows * TP, 256), 256, 0, p->stream>>>(ds->part.as<float>(), ds->nsplit, rows, nchunk * TW,
-                                                                            p->partial.as<float>(), done_flag);
-  p->launches += 2;
+  p->launches++;
   GP_CUDA(cudaGetLastError());
-  return GP_OK;
-}
-
-template <class F>
-static int deriv_with_dp(int DP, F&& f) {
-  switch (DP) {
-    case 4: return f(std::integral_constant<int, 4>{});
-    case 8: return f(std::integral_constant<int, 8>{});
-    case 12: return f(std::integral_constant<int, 12>{});
-    case 16: return f(std::integral_constant<int, 16>{});
-  }
-  set_error("derivative plan: unsupported padded width DP=%d", DP);
-  return GP_E_SHAPE;
+  return deriv_finish_launch(p, nchunk * TW, done_flag);
 }
 
 int deriv_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   GP_CHECK(deriv_refresh(p));
   const int ncols = p->kron_cols;
+  if (p->deriv->kind == GP_MATERN52) return m52g_kmv_partials(p, V16, ncols, done_flag);
   return deriv_with_dp(p->DP, [&](auto D) { return deriv_kmv_launch<decltype(D)::value>(p, V16, ncols, done_flag); });
 }
 
 int deriv_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   GP_REQUIRE(m <= 65535, GP_E_SHAPE, "rows of a derivative plan: at most 65535 rows per call (m=%lld)", (long long)m);
   GP_CHECK(deriv_refresh(p));
+  if (p->deriv->kind == GP_MATERN52) return m52g_krows(p, idx, m, OUT, ldo);
   gp_deriv_state* ds = p->deriv;
   const gp_plan* q = ds->data;
   dim3 grid((unsigned)cdiv(q->n2, 256), (unsigned)m);
@@ -404,6 +405,7 @@ int deriv_kdiag(gp_plan* p, float* OUT) {
   gp_deriv_state* ds = p->deriv;
   const gp_plan* q = ds->data;
   GP_REQUIRE(q->same || q->n1 == q->n2, GP_E_SHAPE, "diagonal of a %lld x %lld cross-covariance is undefined", (long long)p->n1, (long long)p->n2);
+  if (ds->kind == GP_MATERN52) return m52g_kdiag(p, OUT);
   deriv_kdiag_kernel<<<(unsigned)cdiv(p->n1, 256), 256, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), q->DP, q->d, q->n1, q->outputscale,
                                                                        ds->hyp, OUT, q->xbad);
   p->launches++;
@@ -425,8 +427,12 @@ static int deriv_grad_launch(gp_plan* p, const float* L16, const float* R16, int
                                                            ds->gout.as<double>());
   p->launches++;
   GP_CUDA(cudaGetLastError());
+  return deriv_sum_gout(p, nblk, nout, tot);
+}
+
+int deriv_sum_gout(gp_plan* p, size_t nblk, int nout, std::vector<double>& tot) {
   std::vector<double> h(nblk * nout);
-  GP_CUDA(cudaMemcpyAsync(h.data(), ds->gout.p, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, p->stream));
+  GP_CUDA(cudaMemcpyAsync(h.data(), p->deriv->gout.p, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, p->stream));
   GP_CUDA(cudaStreamSynchronize(p->stream));
   for (size_t b = 0; b < nblk; ++b)
     for (int o = 0; o < nout; ++o) tot[o] += h[b * nout + o];
@@ -444,7 +450,10 @@ int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R,
     const int tc = std::min(TP, s - c0);
     GP_CHECK(to_v16(p, L + c0, ldl, tc, p->n1, p->misc2.as<float>()));
     GP_CHECK(to_v16(p, R + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-    GP_CHECK(deriv_with_dp(p->DP, [&](auto D) { return deriv_grad_launch<decltype(D)::value>(p, p->misc2.as<float>(), p->misc3.as<float>(), tc, tot); }));
+    if (p->deriv->kind == GP_MATERN52)
+      GP_CHECK(m52g_grad(p, p->misc2.as<float>(), p->misc3.as<float>(), tc, tot));
+    else
+      GP_CHECK(deriv_with_dp(p->DP, [&](auto D) { return deriv_grad_launch<decltype(D)::value>(p, p->misc2.as<float>(), p->misc3.as<float>(), tc, tot); }));
   }
   int bad = 0;
   GP_CUDA(cudaMemcpyAsync(&bad, q->xbad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
@@ -463,8 +472,10 @@ int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R,
 
 double deriv_trace(const gp_plan* p) {
   const gp_deriv_state* ds = p->deriv;
+  // the derivative rows' diagonal is s / l_c^2 (RBF) or (5/3) s / l_c^2 (Matern-5/2, m52grad.cu)
+  const double f = ds->kind == GP_MATERN52 ? 5.0 / 3.0 : 1.0;
   double t = 1.0;
-  for (int c = 0; c < ds->data->d; ++c) t += (double)ds->hyp.il2[c];
+  for (int c = 0; c < ds->data->d; ++c) t += f * (double)ds->hyp.il2[c];
   return (double)ds->data->outputscale * (double)ds->data->n2 * t;
 }
 
@@ -476,12 +487,8 @@ static void deriv_release(gp_plan* p) {
   p->deriv = nullptr;
 }
 
-}  // namespace gp
-
-using namespace gp;
-
-extern "C" int gp_plan_set_deriv(gp_plan* p, gp_plan* data) {
-  GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+// gp_plan_set_deriv (RBF) and gp_plan_set_deriv_kind: `what` names the C call in the refusals
+static int deriv_set(gp_plan* p, gp_plan* data, int kind, const char* what) {
   GP_CUDA(cudaSetDevice(p->device));
   if (data == nullptr) {
     if (p->deriv) {
@@ -496,19 +503,21 @@ extern "C" int gp_plan_set_deriv(gp_plan* p, gp_plan* data) {
   GP_REQUIRE(data != p, GP_E_STATE, "a derivative plan cannot be its own data plan");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a derivative plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a derivative plan");
-  GP_REFUSE_TASKS(p, "gp_plan_set_deriv");
-  GP_REFUSE_LOWRANK(p, "gp_plan_set_deriv");
-  GP_REFUSE_KRON(p, "gp_plan_set_deriv");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_deriv");
-  if (data) GP_REFUSE_PRODUCT(data, "gp_plan_set_deriv (as the data plan)");
+  GP_REFUSE_TASKS(p, what);
+  GP_REFUSE_LOWRANK(p, what);
+  GP_REFUSE_KRON(p, what);
+  GP_REFUSE_PRODUCT(p, what);
+  if (data) GP_REQUIRE(data->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "%s (as the data plan) is not available on a kernel-product plan (gp_plan_set_product)", what);
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   gp_deriv_state* ds = p->deriv ? p->deriv : new gp_deriv_state();
   gp_plan* old = ds->data;
+  const int old_kind = ds->kind;
   ds->data = data;
+  ds->kind = kind;
   p->deriv = ds;
   const int st = deriv_check_data(p, data);
   if (st != GP_OK) {
-    if (old) ds->data = old;
+    if (old) { ds->data = old; ds->kind = old_kind; }
     else deriv_release(p);
     return st;
   }
@@ -516,4 +525,20 @@ extern "C" int gp_plan_set_deriv(gp_plan* p, gp_plan* data) {
   deriv_geometry(p);
   p->data_set = true;
   return p->hypers_set ? deriv_pack(p) : GP_OK;   // without the noise yet: packed by gp_plan_set_hypers
+}
+
+}  // namespace gp
+
+using namespace gp;
+
+extern "C" int gp_plan_set_deriv(gp_plan* p, gp_plan* data) {
+  GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  return deriv_set(p, data, GP_RBF, "gp_plan_set_deriv");
+}
+
+extern "C" int gp_plan_set_deriv_kind(gp_plan* p, gp_plan* data, int kind) {
+  GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  GP_REQUIRE(kind == GP_RBF || kind == GP_MATERN52, GP_E_SHAPE,
+             "derivative observations are available for the RBF and Matern-5/2 kernels (kind=%d)", kind);
+  return deriv_set(p, data, kind, "gp_plan_set_deriv_kind");
 }

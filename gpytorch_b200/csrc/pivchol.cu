@@ -197,6 +197,8 @@ constexpr int PC_KIND_TASK = 66;
 constexpr int PC_KIND_DERIV = 67;
 // kernel products (GP_BACKEND_PRODUCT): K[pivot, j] = S prod_f k_f(|z_f,pivot - z_f,j|^2), the sum's staging and loop with a multiply
 constexpr int PC_KIND_PRODUCT = 68;
+// Matern-5/2 derivative observations (m52grad.cu): rows as PC_KIND_DERIV, entries from the Matern-5/2 value / gradient table
+constexpr int PC_KIND_M52GRAD = 69;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -205,8 +207,8 @@ struct PcTerms {
   const int* task;   // PC_KIND_TASK: task ids (user order; nullptr: r mod rep) and B [T][T]
   const float* B;
   int T;
-  int rep;           // PC_KIND_TASK / PC_KIND_DERIV: rows per point
-  const DerivHyp* dh;   // PC_KIND_DERIV
+  int rep;           // PC_KIND_TASK / PC_KIND_DERIV / PC_KIND_M52GRAD: rows per point
+  const DerivHyp* dh;   // PC_KIND_DERIV / PC_KIND_M52GRAD
 };
 __device__ __forceinline__ int pc_task_of(const PcTerms& tt, int r) { return tt.task ? tt.task[r] : r % tt.rep; }
 __device__ __forceinline__ float pc_cov_rt(int kind, float a) {
@@ -261,7 +263,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
     } else if (KIND == PC_KIND_SKI) {
       ski_stage_u(sk, pi, zp, tid, PCP_THREADS);
     } else {
-      const int64_t zr = (KIND == PC_KIND_TASK || KIND == PC_KIND_DERIV) ? pi / tt.rep : pi;
+      const int64_t zr = (KIND == PC_KIND_TASK || KIND == PC_KIND_DERIV || KIND == PC_KIND_M52GRAD) ? pi / tt.rep : pi;
       for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[zr * DP + c];
     }
     for (int q = tid; q < m; q += PCP_THREADS) lp[q] = __ldcg(Lt + (int64_t)q * n + pi);   // written by another SM, before the last barrier
@@ -332,6 +334,21 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
           const float ua = a ? (zp[a - 1] - zj[a - 1]) * tt.dh->w[a - 1] : 0.f;
           const float ub = b ? (zp[b - 1] - zj[b - 1]) * tt.dh->w[b - 1] : 0.f;
           v = a == 0 ? (b == 0 ? k : k * ub) : (b == 0 ? -k * ua : k * ((a == b ? tt.dh->il2[a - 1] : 0.f) - ua * ub));
+        } else if (KIND == PC_KIND_M52GRAD) {   // [0,0] = k0, [0,b] = A u_b, [a,0] = -A u_a, [a,b] = A delta_ab / l_a^2 - B u_a u_b
+          const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
+          float s = 0.f;
+          for (int c = 0; c < DP; ++c) {
+            float df = zp[c] - zj[c];
+            s = fmaf(df, df, s);
+          }
+          const float rho = sqrt_approx(0.5f * s);
+          const float e = ex2_approx(-LOG2E * rho);
+          const float A = os * 1.6666666f * fmaf(rho, e, e), B = os * 8.3333333f * e;
+          const int a = pi % tt.rep, b = (int)j % tt.rep;
+          const float ua = a ? (zp[a - 1] - zj[a - 1]) * tt.dh->w[a - 1] : 0.f;
+          const float ub = b ? (zp[b - 1] - zj[b - 1]) * tt.dh->w[b - 1] : 0.f;
+          v = a == 0 ? (b == 0 ? os * fmaf(fmaf(rho, 0.33333334f, 1.f), rho, 1.f) * e : A * ub)
+                     : (b == 0 ? -A * ua : fmaf(-B * ua, ub, a == b ? A * tt.dh->il2[a - 1] : 0.f));
         } else {
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
@@ -465,13 +482,14 @@ __global__ void pc_init_task_kernel(const PcTerms tt, float os, float* __restric
   pos[j] = (int)j;
 }
 
-// derivative observations: diag[j] = s (value rows), s / l_b^2 (derivative rows b); then pc_first_pivot_kernel
-__global__ void pc_init_deriv_kernel(const PcTerms tt, float os, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos,
-                                     int64_t n) {
+// derivative observations: diag[j] = s (value rows), c s / l_b^2 (derivative rows b; c = 1 RBF, 5/3 Matern-5/2); then
+// pc_first_pivot_kernel
+__global__ void pc_init_deriv_kernel(const PcTerms tt, float os, float c, float* __restrict__ diag, int* __restrict__ perm,
+                                     int* __restrict__ pos, int64_t n) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   const int b = (int)(j % tt.rep);
-  diag[j] = b ? os * tt.dh->il2[b - 1] : os;
+  diag[j] = b ? os * (c * tt.dh->il2[b - 1]) : os;
   perm[j] = (int)j;
   pos[j] = (int)j;
 }
@@ -867,7 +885,8 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T; tt.rep = 1;
   }
   if (deriv) {
-    pc_init_deriv_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, diag, perm, pos, n);
+    const float c = p->deriv->kind == GP_MATERN52 ? 5.f / 3.f : 1.f;
+    pc_init_deriv_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, c, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;
   } else if (tasks) {
@@ -896,9 +915,10 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? PC_KIND_DERIV : tasks ? PC_KIND_TASK : p->kind) {
+    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : tasks ? PC_KIND_TASK : p->kind) {
       case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
       case PC_KIND_DERIV: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_DERIV>; break;
+      case PC_KIND_M52GRAD: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_M52GRAD>; break;
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
       case GP_MATERN12: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN12>; break;
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
@@ -1072,7 +1092,7 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
     tr_k = (double)n * os_total;
   } else if (p->backend == GP_BACKEND_SKI) {
     GP_CHECK(ski_diag_sum(p, &tr_k));
-  } else if (p->deriv) {    // s N (1 + sum_c 1 / l_c^2)
+  } else if (p->deriv) {    // s N (1 + c sum_c 1 / l_c^2), c = 1 RBF, 5/3 Matern-5/2
     GP_CHECK(deriv_refresh(p));
     tr_k = deriv_trace(p);
   } else if (p->kron) {     // s N sum_a B[a, a]

@@ -555,26 +555,32 @@ class KronPlan(_DataPlanOperator):
 
 
 class DerivPlan(_DataPlanOperator):
-    """The RBF value / gradient operator over interleaved rows i (d+1) + a (gp_plan_set_deriv): N1 (d+1) x N2 (d+1), built on a
-    ready plain RBF data Plan (kept alive here).  set_noise supplies the noise; bilinear_grad returns the data kernel's (lengthscale,
-    outputscale) gradients.  Every product, solve and sample call of Plan works on it; it has no task covariance."""
+    """The value / gradient operator over interleaved rows i (d+1) + a: N1 (d+1) x N2 (d+1), built on a ready plain data Plan of
+    covariance `kind` (kept alive here): "rbf" (gp_plan_set_deriv, RBFKernelGrad) or "matern52" (gp_plan_set_deriv_kind,
+    Matern52KernelGrad).  set_noise supplies the noise; bilinear_grad returns the data kernel's (lengthscale, outputscale)
+    gradients.  Every product, solve and sample call of Plan works on it; it has no task covariance."""
 
-    def __init__(self, data: Plan):
-        super().__init__(data)
+    def __init__(self, data: Plan, kind: str = "rbf"):
+        if kind not in ("rbf", "matern52"):
+            raise ValueError(f"derivative observations are available for the 'rbf' and 'matern52' kernels (got {kind!r})")
+        super().__init__(data, kind)
 
-    def attach(self, data: Plan):
-        """(Re-)attach the data plan: validation and geometry only."""
+    def attach(self, data: Plan, kind: str = "rbf"):
+        """(Re-)attach the data plan: validation and geometry only.  A refused data plan leaves the operator as it was."""
+        with torch.cuda.device(self.device):
+            if kind == "rbf":
+                check(self.lib.gp_plan_set_deriv(self._h, data._h))
+            else:
+                check(self.lib.gp_plan_set_deriv_kind(self._h, data._h, KIND[kind]))
         rw = data.d + 1
-        self.data, self.num_outputs = data, rw
+        self.data, self.num_outputs, self.deriv_kind = data, rw, kind
         self.same, self.d = data.same, data.d
         self.n1, self.n2 = data.n1 * rw, data.n2 * rw
         self.row_begin, self.row_count = 0, self.n1
-        with torch.cuda.device(self.device):
-            check(self.lib.gp_plan_set_deriv(self._h, data._h))
         return self
 
     def refresh_data(self):
-        return self.attach(self.data)
+        return self.attach(self.data, self.deriv_kind)
 
     def set_task_covar(self, b):
         raise RuntimeError("a derivative-observation plan has no task covariance (its d + 1 outputs per point are fixed by the kernel)")

@@ -1,4 +1,4 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, ScaleKernel, AdditiveKernel, ProductKernel,
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, ScaleKernel, AdditiveKernel, ProductKernel,
 GridInterpolationKernel} for the accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
@@ -71,6 +71,10 @@ class Kernel(Module):
         """Whether batched inputs or a batch_shape can run (one independent operator per batch entry)."""
         return True
 
+    def _unbatched_name(self):
+        """The kernel named when batched inputs or a batch_shape are refused (_batchable() is False)."""
+        return "RBFKernelGrad"
+
     def __call__(self, x1, x2=None, diag=False, **params):
         # kernels/kernel.py:454-534: active dims, 1-D -> 2-D, x2=None -> x1, size check
         if self.active_dims is not None:
@@ -91,8 +95,8 @@ class Kernel(Module):
         same = x2 is None
         nb = self._batch_size()
         if (x1.dim() == 3 or nb is not None) and not self._batchable():
-            raise NotImplementedError("a batched RBFKernelGrad (batched inputs or a batch_shape) is not available on the "
-                                      "accelerated path")
+            raise NotImplementedError(f"a batched {self._unbatched_name()} (batched inputs or a batch_shape) is not available "
+                                      "on the accelerated path")
         if x1.dim() == 3 or nb is not None:
             # one leading batch dimension (kernels/kernel.py:119-121 broadcasts every op over it): B independent operators, each
             # with its own inputs and hyper-parameters; the solver runs them concurrently (operators.BatchLinearOperator)
@@ -168,6 +172,44 @@ class MaternKernel(_StationaryKernel):
         return {0.5: "matern12", 1.5: "matern32", 2.5: "matern52"}[self.nu]
 
 
+class Matern52KernelGrad(MaternKernel):
+    """Covariance of values and partial derivatives of a Matern-5/2 GP (kernels/matern52_kernel_grad.py): an n x m input pair gives
+    an n (d+1) x m (d+1) operator over interleaved rows i (d+1) + a (a = 0: f(x_i), a = 1..d: df/dx_a at x_i), as the reference
+    returns after its perfect shuffle.  `nu` is dropped and fixed to 2.5, as in the reference.  forward returns one engine
+    DerivKernelLinearOperator of kind "matern52" (gp_plan_set_deriv_kind); d <= 16, unbatched.  diag=True gives 1 at value rows and
+    (5/3) / l_a^2 at derivative rows (times the outputscale inside a ScaleKernel).  Sums, products, multitask and SKI kernels do not
+    take it."""
+
+    def __init__(self, **kwargs):
+        kwargs.pop("nu", None)
+        super().__init__(nu=2.5, **kwargs)
+
+    def _batchable(self):
+        return False
+
+    def _unbatched_name(self):
+        return "Matern52KernelGrad"
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, **params):
+        if _batch_index is not None or len(self.batch_shape) or x1.dim() != 2:
+            raise NotImplementedError("a batched Matern52KernelGrad is not available on the accelerated path")
+        from .operators import DerivKernelLinearOperator
+        if diag and not (_same or (x1.shape == x2.shape and torch.equal(x1, x2))):
+            raise RuntimeError("diag=True only works when x1 == x2")
+        ls = self.lengthscale.reshape(-1)
+        ls = ls[0] if ls.numel() == 1 else ls
+        op = DerivKernelLinearOperator(x1, None if _same else x2, ls, kind="matern52")
+        return op.diagonal() if diag else op
+
+    def num_outputs_per_input(self, x1, x2):
+        return x1.size(-1) + 1
+
+
+def _is_m52_grad(k):
+    """k is a Matern52KernelGrad, or a ScaleKernel around one."""
+    return isinstance(k, Matern52KernelGrad) or isinstance(getattr(k, "base_kernel", None), Matern52KernelGrad)
+
+
 class ScaleKernel(Kernel):
     """K <- outputscale * base(K)  (kernels/scale_kernel.py:64-118); the scale is folded into the fused kernel."""
 
@@ -220,7 +262,7 @@ class ScaleKernel(Kernel):
         os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
         from .operators import DerivKernelLinearOperator, SKIKernelLinearOperator
         if isinstance(base, DerivKernelLinearOperator):   # s folded into the same value / gradient operator
-            op = DerivKernelLinearOperator(base.x1, None if base.same else base.x2, base.lengthscale, os_)
+            op = DerivKernelLinearOperator(base.x1, None if base.same else base.x2, base.lengthscale, os_, base.kind)
             return op.diagonal() if diag else op
         if isinstance(base, SKIKernelLinearOperator):
             op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
@@ -230,6 +272,9 @@ class ScaleKernel(Kernel):
 
     def _batchable(self):
         return self.base_kernel._batchable()
+
+    def _unbatched_name(self):
+        return self.base_kernel._unbatched_name()
 
     def __call__(self, x1, x2=None, diag=False, **params):
         self.active_dims = None  # selection happens once, here (base active_dims were lifted in __init__)
@@ -254,6 +299,8 @@ class AdditiveKernel(Kernel):
                 raise NotImplementedError("batched components of an AdditiveKernel")
             if isinstance(k, ProductKernel) or isinstance(getattr(k, "base_kernel", None), ProductKernel):
                 raise NotImplementedError("sums that contain a ProductKernel are not available on the accelerated path")
+            if _is_m52_grad(k):
+                raise NotImplementedError("sums that contain a Matern52KernelGrad are not available on the accelerated path")
         self.kernels = torch.nn.ModuleList(kernels)
 
     def forward(self, x1, x2, diag=False, **params):
@@ -286,7 +333,7 @@ class ProductKernel(Kernel):
             if not isinstance(k, Kernel):
                 raise RuntimeError("ProductKernel factors must be kernels")
             base = k.base_kernel if isinstance(k, ScaleKernel) else k
-            if not isinstance(base, _StationaryKernel) or isinstance(base, RBFKernelGrad):
+            if not isinstance(base, _StationaryKernel) or isinstance(base, (RBFKernelGrad, Matern52KernelGrad)):
                 raise NotImplementedError("ProductKernel factors must be RBF / Matern kernels (optionally scaled) on the accelerated "
                                           "path: sums, SKI, multitask and derivative kernels inside a product are not available")
             if len(k.batch_shape):
@@ -385,6 +432,8 @@ class MultitaskKernel(Kernel):
         if not isinstance(base, _StationaryKernel) or len(dm.batch_shape):
             raise NotImplementedError("the accelerated MultitaskKernel takes an RBFKernel / MaternKernel data kernel, optionally "
                                       "inside a ScaleKernel")
+        if isinstance(base, Matern52KernelGrad):
+            raise NotImplementedError("a Matern52KernelGrad data kernel of a MultitaskKernel is not available on the accelerated path")
         covar_x = dm(x1, None if _same else x2)
         from .operators import KroneckerKernelLinearOperator
         op = KroneckerKernelLinearOperator(covar_x.x1, None if covar_x.same else covar_x.x2, covar_x.kind, covar_x.lengthscale,
@@ -407,6 +456,9 @@ class GridInterpolationKernel(Kernel):
         super().__init__(active_dims=active_dims)
         if not isinstance(base_kernel, _StationaryKernel):
             raise RuntimeError("GridInterpolationKernel needs an RBFKernel or MaternKernel base kernel on the accelerated path")
+        if isinstance(base_kernel, Matern52KernelGrad):
+            raise NotImplementedError("a Matern52KernelGrad base kernel of a GridInterpolationKernel is not available on the "
+                                      "accelerated path")
         if num_dims is None:
             raise RuntimeError("num_dims must be supplied")
         self.base_kernel = base_kernel

@@ -752,22 +752,29 @@ _KRON_PLANS: "dict[tuple, Plan]" = {}
 _DERIV_SLOT = 28   # plan-cache slot of the data plans of derivative operators
 
 
-class DerivKernelLinearOperator(KernelLinearOperator):
-    """The RBF covariance of values and gradients over interleaved rows i (d+1) + a (RBFKernelGrad, kernels/rbf_kernel_grad.py:60-104,
-    after its perfect shuffle): ONE engine operator (gp_plan_set_deriv) on the plan of the plain RBF kernel; no N (d+1) x N (d+1)
-    matrix is stored.  The hyper-parameters are lengthscale (scalar or ARD) and outputscale.  Input gradients are not available:
-    inputs that require grad are refused."""
+_DERIV_NAMES = {"rbf": "RBFKernelGrad", "matern52": "Matern52KernelGrad"}
 
-    def __init__(self, x1, x2, lengthscale, outputscale=None):
+
+class DerivKernelLinearOperator(KernelLinearOperator):
+    """The covariance of values and gradients over interleaved rows i (d+1) + a, kind "rbf" (RBFKernelGrad,
+    kernels/rbf_kernel_grad.py:60-104) or "matern52" (Matern52KernelGrad, kernels/matern52_kernel_grad.py), after the reference's
+    perfect shuffle: ONE engine operator (gp_plan_set_deriv / gp_plan_set_deriv_kind) on the plan of the plain kernel of that kind;
+    no N (d+1) x N (d+1) matrix is stored.  The hyper-parameters are lengthscale (scalar or ARD) and outputscale.  Input gradients
+    are not available: inputs that require grad are refused."""
+
+    def __init__(self, x1, x2, lengthscale, outputscale=None, kind="rbf"):
+        if kind not in _DERIV_NAMES:
+            raise ValueError(f"derivative observations are available for the 'rbf' and 'matern52' kernels (got {kind!r})")
+        name = _DERIV_NAMES[kind]
         if x1.requires_grad or (x2 is not None and x2.requires_grad):
-            raise RuntimeError("gradients with respect to the inputs of a derivative operator (RBFKernelGrad) are not implemented: "
+            raise RuntimeError(f"gradients with respect to the inputs of a derivative operator ({name}) are not implemented: "
                                "pass inputs that do not require grad")
         d = x1.size(-1)
         if d > 16:
-            raise RuntimeError(f"RBFKernelGrad on the accelerated path supports d <= 16 input dimensions (got d={d})")
-        super().__init__(x1, x2, "rbf", lengthscale, outputscale)
+            raise RuntimeError(f"{name} on the accelerated path supports d <= 16 input dimensions (got d={d})")
+        super().__init__(x1, x2, kind, lengthscale, outputscale)
         self.num_outputs = d + 1
-        self._data_op = KernelLinearOperator(x1, x2, "rbf", lengthscale, self.outputscale)
+        self._data_op = KernelLinearOperator(x1, x2, kind, lengthscale, self.outputscale)
         self._data_op._plan_slot = _DERIV_SLOT
 
     @property
@@ -781,16 +788,16 @@ class DerivKernelLinearOperator(KernelLinearOperator):
             data.set_noise_diag(None)
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
         with _PLAN_LOCK:
-            key = id(data)
+            key = (id(data), self.kind)   # one parent per (data plan, kind): never re-attached to a data plan of another kind
             parent = _DERIV_PLANS.pop(key, None)
             if parent is None:
-                parent = DerivPlan(data)
+                parent = DerivPlan(data, self.kind)
                 parent._hyp_key = None
             _DERIV_PLANS[key] = parent
             while len(_DERIV_PLANS) > 16:
                 _DERIV_PLANS.pop(next(iter(_DERIV_PLANS))).close()
         # the data plan may have been re-packed or re-pointed since the last use: re-attach it (validation, no allocation)
-        parent.attach(data)
+        parent.attach(data, self.kind)
         hk = (nz, tuple(data.lengthscale), data.outputscale)
         if parent._hyp_key != hk:
             parent.set_noise(nz)
@@ -808,17 +815,18 @@ class DerivKernelLinearOperator(KernelLinearOperator):
         """K(x1, x2)^T = K(x2, x1): the value / gradient blocks swap with D -> -D."""
         if self.same:
             return self
-        return DerivKernelLinearOperator(self.x2, self.x1, self.lengthscale, self.outputscale)
+        return DerivKernelLinearOperator(self.x2, self.x1, self.lengthscale, self.outputscale, self.kind)
 
     def detach(self):
         return DerivKernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.lengthscale.detach(),
-                                         self.outputscale.detach())
+                                         self.outputscale.detach(), self.kind)
 
     def to_dense(self):
         return _KernelDense.apply(self)
 
     def diagonal(self, dim1=-2, dim2=-1):
-        """s at value rows, s / l_a^2 at derivative rows (rbf_kernel_grad.py:106-115) for x2 == x1."""
+        """s at value rows, s / l_a^2 (RBF, rbf_kernel_grad.py:106-115) or (5/3) s / l_a^2 (Matern-5/2) at derivative rows for
+        x2 == x1."""
         if self.shape[0] != self.shape[1]:
             raise RuntimeError(f"diagonal of a non-square operator {tuple(self.shape)} is undefined")
         return self.plan().diag()
@@ -837,10 +845,10 @@ class DerivKernelLinearOperator(KernelLinearOperator):
         rs, cs = _aligned(ri, R, self.x1.size(0)), _aligned(ci, R, x2.size(0))
         if rs is None or cs is None:
             raise NotImplementedError("a derivative operator takes row / column slices that start and stop on multiples of d + 1")
-        return DerivKernelLinearOperator(self.x1[rs], x2[cs], self.lengthscale, self.outputscale)
+        return DerivKernelLinearOperator(self.x1[rs], x2[cs], self.lengthscale, self.outputscale, self.kind)
 
     def mul(self, other):
-        raise NotImplementedError("a derivative operator (RBFKernelGrad) does not multiply by a task covariance")
+        raise NotImplementedError(f"a derivative operator ({_DERIV_NAMES[self.kind]}) does not multiply by a task covariance")
 
     __mul__ = mul
 
@@ -850,7 +858,7 @@ class DerivKernelLinearOperator(KernelLinearOperator):
         raise NotImplementedError("a derivative operator adds a (Constant)DiagLinearOperator only")
 
 
-_DERIV_PLANS: "dict[int, Plan]" = {}
+_DERIV_PLANS: "dict[tuple, Plan]" = {}
 
 
 class SumKernelLinearOperator(KernelLinearOperator):

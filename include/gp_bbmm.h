@@ -213,6 +213,14 @@ int gp_plan_set_kron(gp_plan* plan, gp_plan* data, int T);
  * gradients on `plan`. */
 int gp_plan_set_deriv(gp_plan* plan, gp_plan* data);
 
+/* The same value / gradient operator for another covariance (kernels/matern52_kernel_grad.py): kind = GP_RBF is
+ * gp_plan_set_deriv; kind = GP_MATERN52 takes a ready plain Matern-5/2 data plan and gives, with D = x_i - x'_j, u_a = D_a / l_a^2,
+ * rho = sqrt(5 |D / l|^2), e = exp(-rho), A = (5/3) (1 + rho) e, B = (25/3) e and the data plan's outputscale s,
+ *     [0, 0] = s (1 + rho + rho^2 / 3) e,  [0, b] = s A u_b,  [a, 0] = -s A u_a,  [a, b] = s (A delta_ab / l_a^2 - B u_a u_b);
+ * gp_kdiag returns s and (5/3) s / l_a^2 on a square plan.  Every call and refusal of gp_plan_set_deriv applies.  The plan
+ * remembers `kind`: a data plan whose covariance later differs is refused by the next call (GP_E_SHAPE).  Another kind: GP_E_SHAPE. */
+int gp_plan_set_deriv_kind(gp_plan* plan, gp_plan* data, int kind);
+
 /* ---- kernel seam (LazyEvaluatedKernelTensor, lazy/lazy_evaluated_kernel_tensor.py) --- */
 
 /* OUT[n1_local, t] = K(X1,X2) V [+ noise * V when add_noise and X2 == X1].
