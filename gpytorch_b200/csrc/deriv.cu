@@ -19,8 +19,30 @@
 // deriv_grad_kernel evaluates these per thread in fp32 over its columns and reduces every CTA in fp64; the host adds the CTA
 // partials in a fixed order.
 //
-// A plan built by gp_plan_set_deriv_kind(..., GP_MATERN52) shares this file's geometry, refresh, split sum and host reductions;
-// its entries, products, rows, diagonal and gradient come from the Matern-5/2 table of m52grad.cu.
+// Matern-5/2 (gp_plan_set_deriv_kind(..., GP_MATERN52)): the value / gradient operator of Matern52KernelGrad
+// (kernels/matern52_kernel_grad.py) over the same interleaved rows, on a plain Matern-5/2 data plan.
+//
+// Entries.  With D = x_i - x'_j, u_a = D_a / l_a^2, rho = sqrt(5) r (r^2 = sum_c D_c^2 / l_c^2), e = exp(-rho),
+// A = (5/3) (1 + rho) e and B = (25/3) e (times the outputscale s):
+//     [0, 0] = (1 + rho + rho^2 / 3) e,   [0, b] = A u_b,   [a, 0] = -A u_a,   [a, b] = A delta_ab / l_a^2 - B u_a u_b.
+// The data plan packs z = (x - mean) sqrt(10) / l (pack.cu), so rho = sqrt(|dz|^2 / 2) and u_c = dz_c / (sqrt(10) l_c) = dz_c w[c].
+// D = 0 gives s and (5/3) s / l_a^2 on the diagonal exactly.
+//
+// Products.  With h = sum_b u_b v^b per column:  out0 += [0,0] v0 + A h,  out^a += A v^a / l_a^2 - u_a (A v0 + B h): 3 d + 4 FMAs
+// per pair and column, one sqrt and one ex2 per pair.
+//
+// Gradients (DESIGN 4.16).  For one pair and column, with P = l0 r0, h = sum u_b r^b, g = sum u_a l^a, q = sum l^a r^a / l_a^2:
+//     F = sum_ab l_a E_ab r_b = [0,0] P + A (l0 h - g r0 + q) - B g h           (d/ds = sum F)
+// and with q_c = (D_c / l_c)^2 = dz_c^2 / 10:  l_c d[0,0]/dl_c = A q_c,  l_c dA/dl_c = B q_c,  l_c dB/dl_c = 5 B q_c / rho,
+// l_c du_a/dl_c = -2 delta_ac u_a,  l_c d(1 / l_a^2)/dl_c = -2 delta_ac / l_a^2, so
+//     l_c dF/dl_c = q_c [A P + B (l0 h - g r0 + q) - (5 B / rho) g h] - 2 A [u_c (l0 r^c - l^c r0) + r^c l^c / l_c^2]
+//                   + 2 B u_c (l^c h + r^c g).
+// q_c / rho <= rho / 5 is bounded but 0 / 0 at coincident points (and where |dz|^2 flushes to zero): 5 B / rho is taken as 0 at
+// rho = 0, where every q_c is 0 as well.
+//
+// One kernel per job serves both kinds: deriv_kmv_kernel, deriv_grad_kernel, deriv_krows_kernel and deriv_kdiag_kernel stage,
+// index and reduce; the kind's DerivTable (deriv_table.cuh) supplies the pair coefficients, the entry, the product's per-column
+// and the gradient's per-pair update.
 #include <math.h>
 #include <string.h>
 
@@ -28,22 +50,15 @@
 #include <cmath>
 
 #include "gp_common.cuh"
+#include "deriv_table.cuh"
 
 namespace gp {
 
-constexpr float DV_LN2 = 0.69314718f;   // 1 / log2 e: dz_c^2 / log2 e = D_c^2 / l_c^2
-
-// columns per CTA: (DP + 1) x TW accumulators per thread in the product (DP = 8 with 8 columns takes 201 registers and ran d = 5
-// at 6.7 TFLOP/s, with 4 columns 127 registers and 14.5 TFLOP/s, DESIGN 4.14); the gradient holds (DP + 1) x TW of L instead, and
-// half the columns keep it out of local memory
-template <int DP>
-struct DerivTW { static constexpr int value = DP <= 4 ? 16 : 4; };
-template <int DP>
-struct DerivGradTW { static constexpr int value = DP <= 4 ? 8 : (DP <= 8 ? 4 : 2); };
+static const float* deriv_z1(const gp_plan* q) { return q->same ? q->Z2.as<float>() : q->Z1.as<float>(); }
 
 // out rows i (d+1) + a of the split's partial, columns [c0, c0 + TW)
-template <int DP, int TW>
-__global__ void __launch_bounds__(DV_TI)
+template <class K, int DP, int TW>
+__global__ void __launch_bounds__(DV_TI, K::min_blocks(DP))
 deriv_kmv_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ V16, float* __restrict__ part,
                  int64_t n1, int64_t n2, int d, int64_t cols_per_split, int64_t slot_rows, const __grid_constant__ DerivHyp hy,
                  const int* __restrict__ done_flag) {
@@ -77,9 +92,9 @@ deriv_kmv_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, con
       (&vj[0][0][0])[e] = (jj < nj && b < rw) ? V16[((j0 + jj) * rw + b) * TP + c0 + t] : 0.f;
     }
     __syncthreads();
-#pragma unroll 2
-    for (int jj = 0; jj < DV_TJ; ++jj) {
-      float u[DP], kl[DP];
+#pragma unroll (K::unroll(DP))
+    for (int jj = 0; jj < DV_TJ; ++jj) {   // staged padding points carry V = 0: they add 0
+      float u[DP];
       float s = 0.f;
 #pragma unroll
       for (int c = 0; c < DP; ++c) {
@@ -87,19 +102,12 @@ deriv_kmv_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, con
         s = fmaf(df, df, s);
         u[c] = df * hy.w[c];
       }
-      const float k = ex2_approx(fminf(-0.5f * s, 0.f));
+      const auto p = K::pair(s);
+      float kl[DP];
 #pragma unroll
-      for (int c = 0; c < DP; ++c) kl[c] = k * hy.il2[c];
+      for (int c = 0; c < DP; ++c) kl[c] = K::delta_coef(p) * hy.il2[c];
 #pragma unroll
-      for (int t = 0; t < TW; ++t) {
-        float h = vj[jj][0][t];
-#pragma unroll
-        for (int c = 0; c < DP; ++c) h = fmaf(u[c], vj[jj][1 + c][t], h);
-        const float kh = k * h;
-        acc[0][t] += kh;
-#pragma unroll
-        for (int c = 0; c < DP; ++c) acc[1 + c][t] = fmaf(kl[c], vj[jj][1 + c][t], fmaf(-u[c], kh, acc[1 + c][t]));
-      }
+      for (int t = 0; t < TW; ++t) K::template kmv_column<DP, TW>(p, u, kl, vj[jj], t, acc);
     }
   }
   if (!rv) return;
@@ -126,8 +134,8 @@ __global__ void deriv_finish_kernel(const float* __restrict__ part, int nsplit, 
   out[idx] = s;
 }
 
-// gout[blk][0] = sum k F ; gout[blk][1 + c] = sum k [ (dz_c^2 / log2 e) F - 2 u_c (g r_c - l_c h) - 2 il2_c l_c r_c ]  (c < d)
-template <int DP, int TW>
+// gout[blk][0] = sum_pairs d/ds, gout[blk][1 + c] = sum_pairs l_c d/dl_c / s (c < d): the kind's grad_pair per pair
+template <class K, int DP, int TW>
 __global__ void __launch_bounds__(DV_TI)
 deriv_grad_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ L16, const float* __restrict__ R16,
                   int64_t n1, int64_t n2, int d, int64_t cols_per_split, const __grid_constant__ DerivHyp hy, double* __restrict__ gout) {
@@ -171,29 +179,7 @@ deriv_grad_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, co
         s += dz2[c];
         u[c] = df * hy.w[c];
       }
-      const float k = ex2_approx(fminf(-0.5f * s, 0.f));
-      float fs = 0.f, hc[DP];
-#pragma unroll
-      for (int c = 0; c < DP; ++c) hc[c] = 0.f;
-#pragma unroll
-      for (int t = 0; t < TW; ++t) {
-        float h = rj[jj][0][t], g = li[0][t], q = 0.f;
-#pragma unroll
-        for (int c = 0; c < DP; ++c) {
-          h = fmaf(u[c], rj[jj][1 + c][t], h);
-          g = fmaf(-u[c], li[1 + c][t], g);
-          q = fmaf(hy.il2[c] * li[1 + c][t], rj[jj][1 + c][t], q);
-        }
-        fs += fmaf(g, h, q);
-#pragma unroll
-        for (int c = 0; c < DP; ++c) {
-          const float lr = li[1 + c][t] * rj[jj][1 + c][t];
-          hc[c] = fmaf(-2.f * u[c], fmaf(g, rj[jj][1 + c][t], -li[1 + c][t] * h), fmaf(-2.f * hy.il2[c], lr, hc[c]));
-        }
-      }
-      gk = fmaf(k, fs, gk);
-#pragma unroll
-      for (int c = 0; c < DP; ++c) gc[c] = fmaf(k, fmaf(DV_LN2 * dz2[c], fs, hc[c]), gc[c]);
+      K::template grad_pair<DP, TW>(K::pair(s), u, dz2, li, rj[jj], hy, gk, gc);
     }
   }
   const int nout = 1 + d;
@@ -214,6 +200,7 @@ deriv_grad_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, co
 }
 
 // OUT[r][j (d+1) + b] = s E(i a, j b) for row idx[r] = i (d+1) + a; a NaN row for an index outside [0, n1 (d+1)) or non-finite inputs
+template <class K>
 __global__ void deriv_krows_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP, int d, const int64_t* __restrict__ idx,
                                    int64_t nrows, int64_t n2, float os, const __grid_constant__ DerivHyp hy, float* __restrict__ OUT,
                                    int64_t ldo, const int* __restrict__ xbad) {
@@ -238,17 +225,15 @@ __global__ void deriv_krows_kernel(const float* __restrict__ Z1, const float* __
     const float df = zs[c] - zj[c];
     s = fmaf(df, df, s);
   }
-  const float k = os * ex2_approx(fminf(-0.5f * s, 0.f));
+  const auto pr = K::pair(s).scaled(os);
   const float ua = a ? (zs[a - 1] - zj[a - 1]) * hy.w[a - 1] : 0.f;
   float* out = OUT + r * ldo + j * rw;
-  out[0] = a ? -k * ua : k;
-  for (int b = 1; b < rw; ++b) {
-    const float ub = (zs[b - 1] - zj[b - 1]) * hy.w[b - 1];
-    out[b] = a ? k * ((a == b ? hy.il2[a - 1] : 0.f) - ua * ub) : k * ub;
-  }
+  out[0] = K::entry(pr, a, 0, ua, 0.f, hy);
+  for (int b = 1; b < rw; ++b) out[b] = K::entry(pr, a, b, ua, (zs[b - 1] - zj[b - 1]) * hy.w[b - 1], hy);
 }
 
-// OUT[i (d+1) + a] = s E(i a, i a): s and s / l_a^2 on a square plan (D = 0), k (1 / l_a^2 - u_a^2) for a cross plan of equal sizes
+// OUT[i (d+1) + a] = s E(i a, i a): s and DIAG s / l_a^2 on a square plan (D = 0), the full entry for a cross plan of equal sizes
+template <class K>
 __global__ void deriv_kdiag_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP, int d, int64_t n, float os,
                                    const __grid_constant__ DerivHyp hy, float* __restrict__ OUT, const int* __restrict__ xbad) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -261,13 +246,8 @@ __global__ void deriv_kdiag_kernel(const float* __restrict__ Z1, const float* __
     const float df = Z1[i * DP + c] - Z2[i * DP + c];
     s = fmaf(df, df, s);
   }
-  const float k = os * ex2_approx(fminf(-0.5f * s, 0.f));
-  float o = k;
-  if (a) {
-    const float ua = (Z1[i * DP + a - 1] - Z2[i * DP + a - 1]) * hy.w[a - 1];
-    o = k * (hy.il2[a - 1] - ua * ua);
-  }
-  OUT[e] = *xbad ? __int_as_float(0x7fc00000) : o;
+  const float ua = a ? (Z1[i * DP + a - 1] - Z2[i * DP + a - 1]) * hy.w[a - 1] : 0.f;
+  OUT[e] = *xbad ? __int_as_float(0x7fc00000) : K::entry(K::pair(s).scaled(os), a, a, ua, ua, hy);
 }
 
 static int deriv_check_data(const gp_plan* p, const gp_plan* q) {
@@ -328,7 +308,7 @@ int deriv_refresh(gp_plan* p) {
   p->xbad = q->xbad;
   DerivHyp h;
   memset(&h, 0, sizeof(h));
-  const double rc = sqrt(ds->kind == GP_MATERN52 ? 10.0 : 1.4426950408889634);   // the packing constant of pack.cu
+  const double rc = sqrt(deriv_with_kind(ds->kind, [](auto K) { return decltype(K)::PACK; }));
   for (int c = 0; c < q->d; ++c) {
     const double l = q->ls.size() == 1 ? q->ls[0] : q->ls[c];
     h.w[c] = (float)(1.0 / (rc * l));
@@ -353,7 +333,7 @@ int deriv_pack(gp_plan* p) {
 }
 
 // the split partials of the first ncols columns, summed in order into the parent's partial slot 0
-int deriv_finish_launch(gp_plan* p, int ncols, const int* done_flag) {
+static int deriv_finish_launch(gp_plan* p, int ncols, const int* done_flag) {
   gp_deriv_state* ds = p->deriv;
   const int64_t rows = p->n1;
   deriv_finish_kernel<<<(unsigned)cdiv(rows * TP, 256), 256, 0, p->stream>>>(ds->part.as<float>(), ds->nsplit, rows, ncols,
@@ -363,17 +343,40 @@ int deriv_finish_launch(gp_plan* p, int ncols, const int* done_flag) {
   return GP_OK;
 }
 
-template <int DP>
+// tot[o] += the CTA partials of ds->gout, in order
+static int deriv_sum_gout(gp_plan* p, size_t nblk, int nout, std::vector<double>& tot) {
+  std::vector<double> h(nblk * nout);
+  GP_CUDA(cudaMemcpyAsync(h.data(), p->deriv->gout.p, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, p->stream));
+  GP_CUDA(cudaStreamSynchronize(p->stream));
+  for (size_t b = 0; b < nblk; ++b)
+    for (int o = 0; o < nout; ++o) tot[o] += h[b * nout + o];
+  return GP_OK;
+}
+
+// f(integral_constant<DP>) for the padded widths the product and gradient kernels are built for
+template <class F>
+static int deriv_with_dp(int DP, F&& f) {
+  switch (DP) {
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    case 12: return f(std::integral_constant<int, 12>{});
+    case 16: return f(std::integral_constant<int, 16>{});
+  }
+  set_error("derivative plan: unsupported padded width DP=%d", DP);
+  return GP_E_SHAPE;
+}
+
+template <class K, int DP>
 static int deriv_kmv_launch(gp_plan* p, const float* V16, int ncols, const int* done_flag) {
-  constexpr int TW = DerivTW<DP>::value;
+  constexpr int TW = K::kmv_tw(DP);
   gp_deriv_state* ds = p->deriv;
   const gp_plan* q = ds->data;
   const int nchunk = (int)cdiv(ncols, TW);
   const int64_t rows = p->n1;
   GP_CHECK(ds->part.ensure(sizeof(float) * (size_t)ds->nsplit * rows * TP));
   dim3 grid((unsigned)cdiv(q->n1, DV_TI), (unsigned)ds->nsplit, (unsigned)nchunk);
-  deriv_kmv_kernel<DP, TW><<<grid, DV_TI, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), V16, ds->part.as<float>(), q->n1, q->n2, q->d,
-                                                          ds->cps, rows, ds->hyp, done_flag);
+  deriv_kmv_kernel<K, DP, TW><<<grid, DV_TI, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), V16, ds->part.as<float>(), q->n1, q->n2,
+                                                             q->d, ds->cps, rows, ds->hyp, done_flag);
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return deriv_finish_launch(p, nchunk * TW, done_flag);
@@ -382,19 +385,21 @@ static int deriv_kmv_launch(gp_plan* p, const float* V16, int ncols, const int* 
 int deriv_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   GP_CHECK(deriv_refresh(p));
   const int ncols = p->kron_cols;
-  if (p->deriv->kind == GP_MATERN52) return m52g_kmv_partials(p, V16, ncols, done_flag);
-  return deriv_with_dp(p->DP, [&](auto D) { return deriv_kmv_launch<decltype(D)::value>(p, V16, ncols, done_flag); });
+  return deriv_with_kind(p->deriv->kind, [&](auto K) {
+    return deriv_with_dp(p->DP, [&](auto D) { return deriv_kmv_launch<decltype(K), decltype(D)::value>(p, V16, ncols, done_flag); });
+  });
 }
 
 int deriv_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   GP_REQUIRE(m <= 65535, GP_E_SHAPE, "rows of a derivative plan: at most 65535 rows per call (m=%lld)", (long long)m);
   GP_CHECK(deriv_refresh(p));
-  if (p->deriv->kind == GP_MATERN52) return m52g_krows(p, idx, m, OUT, ldo);
   gp_deriv_state* ds = p->deriv;
   const gp_plan* q = ds->data;
   dim3 grid((unsigned)cdiv(q->n2, 256), (unsigned)m);
-  deriv_krows_kernel<<<grid, 256, sizeof(float) * q->DP, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), q->DP, q->d, idx, p->n1, q->n2,
-                                                                      q->outputscale, ds->hyp, OUT, ldo, q->xbad);
+  deriv_with_kind(ds->kind, [&](auto K) {
+    deriv_krows_kernel<decltype(K)><<<grid, 256, sizeof(float) * q->DP, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), q->DP, q->d, idx,
+                                                                                    p->n1, q->n2, q->outputscale, ds->hyp, OUT, ldo, q->xbad);
+  });
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -405,17 +410,18 @@ int deriv_kdiag(gp_plan* p, float* OUT) {
   gp_deriv_state* ds = p->deriv;
   const gp_plan* q = ds->data;
   GP_REQUIRE(q->same || q->n1 == q->n2, GP_E_SHAPE, "diagonal of a %lld x %lld cross-covariance is undefined", (long long)p->n1, (long long)p->n2);
-  if (ds->kind == GP_MATERN52) return m52g_kdiag(p, OUT);
-  deriv_kdiag_kernel<<<(unsigned)cdiv(p->n1, 256), 256, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), q->DP, q->d, q->n1, q->outputscale,
-                                                                       ds->hyp, OUT, q->xbad);
+  deriv_with_kind(ds->kind, [&](auto K) {
+    deriv_kdiag_kernel<decltype(K)><<<(unsigned)cdiv(p->n1, 256), 256, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), q->DP, q->d, q->n1,
+                                                                                       q->outputscale, ds->hyp, OUT, q->xbad);
+  });
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
 
-template <int DP>
+template <class K, int DP>
 static int deriv_grad_launch(gp_plan* p, const float* L16, const float* R16, int ncols, std::vector<double>& tot) {
-  constexpr int TW = DerivGradTW<DP>::value;
+  constexpr int TW = K::grad_tw(DP);
   gp_deriv_state* ds = p->deriv;
   const gp_plan* q = ds->data;
   const int nout = 1 + q->d;
@@ -423,20 +429,11 @@ static int deriv_grad_launch(gp_plan* p, const float* L16, const float* R16, int
   dim3 grid((unsigned)cdiv(q->n1, DV_TI), (unsigned)ds->nsplit, (unsigned)nchunk);
   const size_t nblk = (size_t)grid.x * grid.y * grid.z;
   GP_CHECK(ds->gout.ensure(sizeof(double) * nblk * nout));
-  deriv_grad_kernel<DP, TW><<<grid, DV_TI, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), L16, R16, q->n1, q->n2, q->d, ds->cps, ds->hyp,
-                                                           ds->gout.as<double>());
+  deriv_grad_kernel<K, DP, TW><<<grid, DV_TI, 0, p->stream>>>(deriv_z1(q), q->Z2.as<float>(), L16, R16, q->n1, q->n2, q->d, ds->cps,
+                                                              ds->hyp, ds->gout.as<double>());
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return deriv_sum_gout(p, nblk, nout, tot);
-}
-
-int deriv_sum_gout(gp_plan* p, size_t nblk, int nout, std::vector<double>& tot) {
-  std::vector<double> h(nblk * nout);
-  GP_CUDA(cudaMemcpyAsync(h.data(), p->deriv->gout.p, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, p->stream));
-  GP_CUDA(cudaStreamSynchronize(p->stream));
-  for (size_t b = 0; b < nblk; ++b)
-    for (int o = 0; o < nout; ++o) tot[o] += h[b * nout + o];
-  return GP_OK;
 }
 
 int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os) {
@@ -450,10 +447,11 @@ int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R,
     const int tc = std::min(TP, s - c0);
     GP_CHECK(to_v16(p, L + c0, ldl, tc, p->n1, p->misc2.as<float>()));
     GP_CHECK(to_v16(p, R + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-    if (p->deriv->kind == GP_MATERN52)
-      GP_CHECK(m52g_grad(p, p->misc2.as<float>(), p->misc3.as<float>(), tc, tot));
-    else
-      GP_CHECK(deriv_with_dp(p->DP, [&](auto D) { return deriv_grad_launch<decltype(D)::value>(p, p->misc2.as<float>(), p->misc3.as<float>(), tc, tot); }));
+    GP_CHECK(deriv_with_kind(p->deriv->kind, [&](auto K) {
+      return deriv_with_dp(p->DP, [&](auto D) {
+        return deriv_grad_launch<decltype(K), decltype(D)::value>(p, p->misc2.as<float>(), p->misc3.as<float>(), tc, tot);
+      });
+    }));
   }
   int bad = 0;
   GP_CUDA(cudaMemcpyAsync(&bad, q->xbad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
@@ -472,8 +470,7 @@ int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R,
 
 double deriv_trace(const gp_plan* p) {
   const gp_deriv_state* ds = p->deriv;
-  // the derivative rows' diagonal is s / l_c^2 (RBF) or (5/3) s / l_c^2 (Matern-5/2, m52grad.cu)
-  const double f = ds->kind == GP_MATERN52 ? 5.0 / 3.0 : 1.0;
+  const double f = deriv_with_kind(ds->kind, [](auto K) { return decltype(K)::DIAG; });   // the derivative rows' diagonal is f s / l_c^2
   double t = 1.0;
   for (int c = 0; c < ds->data->d; ++c) t += f * (double)ds->hyp.il2[c];
   return (double)ds->data->outputscale * (double)ds->data->n2 * t;

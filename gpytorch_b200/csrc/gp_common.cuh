@@ -186,7 +186,7 @@ struct gp_kron_state {
   gp::DevBuf Lw, red, idx, rows;           // gradient / row-extraction scratch
 };
 
-// Derivative-observation state (deriv.cu, m52grad.cu): the RBF or Matern-5/2 value / gradient operator over interleaved rows
+// Derivative-observation state (deriv.cu, deriv_table.cuh): the RBF or Matern-5/2 value / gradient operator over interleaved rows
 // i (d+1) + a on a plain data plan of the same kind.  Per dimension c < d: w[c] = 1 / (sqrt(C) l_c) turns a packed difference
 // (z = (x - mean) sqrt(C) / l, C = log2 e for RBF, 10 for Matern-5/2, pack.cu) into u_c = D_c / l_c^2, il2[c] = 1 / l_c^2; both
 // are 0 for c >= d.
@@ -351,24 +351,6 @@ int deriv_kdiag(gp_plan* p, float* OUT);
 int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
 int deriv_refresh(gp_plan* p);                                               // re-check the data plan, take its scale / lengthscales / flag
 double deriv_trace(const gp_plan* p);                                        // s N (1 + c sum_c 1 / l_c^2) in fp64, c = 1 or 5/3
-int deriv_finish_launch(gp_plan* p, int ncols, const int* done_flag);        // split partials -> parent slot 0 (fixed order)
-int deriv_sum_gout(gp_plan* p, size_t nblk, int nout, std::vector<double>& tot);   // tot[o] += CTA partials of ds->gout in order
-int m52g_kmv_partials(gp_plan* p, const float* V16, int ncols, const int* done_flag);   // m52grad.cu: the Matern-5/2 table
-int m52g_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
-int m52g_kdiag(gp_plan* p, float* OUT);
-int m52g_grad(gp_plan* p, const float* L16, const float* R16, int ncols, std::vector<double>& tot);
-inline const float* deriv_z1(const gp_plan* q) { return q->same ? q->Z2.as<float>() : q->Z1.as<float>(); }
-template <class F>
-inline int deriv_with_dp(int DP, F&& f) {
-  switch (DP) {
-    case 4: return f(std::integral_constant<int, 4>{});
-    case 8: return f(std::integral_constant<int, 8>{});
-    case 12: return f(std::integral_constant<int, 12>{});
-    case 16: return f(std::integral_constant<int, 16>{});
-  }
-  set_error("derivative plan: unsupported padded width DP=%d", DP);
-  return GP_E_SHAPE;
-}
 #define GP_REFUSE_DERIV(p, what) \
   GP_REQUIRE((p)->deriv == nullptr, GP_E_STATE, "%s is not available on a derivative-observation plan (gp_plan_set_deriv)", what)
 int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,   // cg.cu

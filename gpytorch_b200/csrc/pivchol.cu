@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <cmath>
 
+#include "deriv_table.cuh"
 #include "gp_common.cuh"
 #include "ski_rows.cuh"
 
@@ -193,11 +194,11 @@ constexpr int PC_KIND_SKI = 65;
 // point r / rep, task task[r] (Hadamard: rep = 1, task ids) or point r / T, task r mod T (Kronecker: rep = T, task = nullptr)
 constexpr int PC_KIND_TASK = 66;
 // derivative observations (deriv.cu): row r is point r / rep, component r mod rep (rep = d + 1); the entry of rows (a, b) is the
-// RBF value / gradient block entry with u_c = dz_c w[c] and 1 / l_c^2 = il2[c] from dh (a DerivHyp on the device)
+// RBF table's block entry (deriv_table.cuh) with u_c = dz_c w[c] and 1 / l_c^2 = il2[c] from dh (a DerivHyp on the device)
 constexpr int PC_KIND_DERIV = 67;
 // kernel products (GP_BACKEND_PRODUCT): K[pivot, j] = S prod_f k_f(|z_f,pivot - z_f,j|^2), the sum's staging and loop with a multiply
 constexpr int PC_KIND_PRODUCT = 68;
-// Matern-5/2 derivative observations (m52grad.cu): rows as PC_KIND_DERIV, entries from the Matern-5/2 value / gradient table
+// Matern-5/2 derivative observations: rows as PC_KIND_DERIV, entries from the Matern-5/2 table
 constexpr int PC_KIND_M52GRAD = 69;
 struct PcTerms {
   int n;
@@ -322,33 +323,18 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             s = fmaf(df, df, s);
           }
           v = os * tt.B[pc_task_of(tt, pi) * tt.T + pc_task_of(tt, (int)j)] * pc_cov_rt(tt.kind[0], -0.5f * s);
-        } else if (KIND == PC_KIND_DERIV) {
+        } else if (KIND == PC_KIND_DERIV || KIND == PC_KIND_M52GRAD) {
+          using K = DerivTable<KIND == PC_KIND_M52GRAD ? GP_MATERN52 : GP_RBF>;
           const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
             float df = zp[c] - zj[c];
             s = fmaf(df, df, s);
           }
-          const float k = os * cov_from_arg<GP_RBF>(-0.5f * s);
           const int a = pi % tt.rep, b = (int)j % tt.rep;
           const float ua = a ? (zp[a - 1] - zj[a - 1]) * tt.dh->w[a - 1] : 0.f;
           const float ub = b ? (zp[b - 1] - zj[b - 1]) * tt.dh->w[b - 1] : 0.f;
-          v = a == 0 ? (b == 0 ? k : k * ub) : (b == 0 ? -k * ua : k * ((a == b ? tt.dh->il2[a - 1] : 0.f) - ua * ub));
-        } else if (KIND == PC_KIND_M52GRAD) {   // [0,0] = k0, [0,b] = A u_b, [a,0] = -A u_a, [a,b] = A delta_ab / l_a^2 - B u_a u_b
-          const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
-          float s = 0.f;
-          for (int c = 0; c < DP; ++c) {
-            float df = zp[c] - zj[c];
-            s = fmaf(df, df, s);
-          }
-          const float rho = sqrt_approx(0.5f * s);
-          const float e = ex2_approx(-LOG2E * rho);
-          const float A = os * 1.6666666f * fmaf(rho, e, e), B = os * 8.3333333f * e;
-          const int a = pi % tt.rep, b = (int)j % tt.rep;
-          const float ua = a ? (zp[a - 1] - zj[a - 1]) * tt.dh->w[a - 1] : 0.f;
-          const float ub = b ? (zp[b - 1] - zj[b - 1]) * tt.dh->w[b - 1] : 0.f;
-          v = a == 0 ? (b == 0 ? os * fmaf(fmaf(rho, 0.33333334f, 1.f), rho, 1.f) * e : A * ub)
-                     : (b == 0 ? -A * ua : fmaf(-B * ua, ub, a == b ? A * tt.dh->il2[a - 1] : 0.f));
+          v = K::entry(K::pair(s).scaled(os), a, b, ua, ub, *tt.dh);
         } else {
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
@@ -482,7 +468,7 @@ __global__ void pc_init_task_kernel(const PcTerms tt, float os, float* __restric
   pos[j] = (int)j;
 }
 
-// derivative observations: diag[j] = s (value rows), c s / l_b^2 (derivative rows b; c = 1 RBF, 5/3 Matern-5/2); then
+// derivative observations: diag[j] = s (value rows), c s / l_b^2 (derivative rows b; c = the table's DIAG); then
 // pc_first_pivot_kernel
 __global__ void pc_init_deriv_kernel(const PcTerms tt, float os, float c, float* __restrict__ diag, int* __restrict__ perm,
                                      int* __restrict__ pos, int64_t n) {
@@ -885,7 +871,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T; tt.rep = 1;
   }
   if (deriv) {
-    const float c = p->deriv->kind == GP_MATERN52 ? 5.f / 3.f : 1.f;
+    const float c = (float)deriv_with_kind(p->deriv->kind, [](auto K) { return decltype(K)::DIAG; });
     pc_init_deriv_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, c, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;

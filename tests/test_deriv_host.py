@@ -157,14 +157,23 @@ _SIMT_REGS = {(0, 4): 60, (0, 8): 70, (0, 12): 66, (0, 16): 72, (0, 24): 80, (0,
               (3, 48): 106, (3, 64): 128, (3, 96): 167, (3, 128): 204}
 
 
-def test_deriv_kernels_have_no_local_memory_and_fused_kernels_keep_their_registers():
+# registers of the RBF derivative product and gradient kernels, {(job, DP): REG}, as built before their Matern-5/2 siblings were
+# folded into the same kernels over a per-kind table (CUDA 12.9, -O3, sm_90a)
+_DERIV_REGS = {("kmv", 4): 168, ("kmv", 8): 127, ("kmv", 12): 168, ("kmv", 16): 230,
+               ("grad", 4): 160, ("grad", 8): 216, ("grad", 12): 204, ("grad", 16): 255}
+
+
+def test_rbf_table_kernels_have_no_local_memory_and_fused_kernels_keep_their_registers():
     res = _res_usage()
-    deriv = {k: v for k, v in res.items() if "deriv_" in k or "pc_persistent1_kernelILi67E" in k}
+    deriv = {k: v for k, v in res.items() if ("deriv_" in k and "DerivTableILi3E" not in k) or "pc_persistent1_kernelILi67E" in k}
     # the product and gradient kernels for DP = 4, 8, 12, 16 (every d <= 16), rows, diagonal, split sum, pivoted-Cholesky source + init
     assert sum("deriv_kmv_kernel" in k for k in deriv) == 4 and sum("deriv_grad_kernel" in k for k in deriv) == 4, sorted(deriv)
     assert len(deriv) == 4 + 4 + 3 + 2, sorted(deriv)   # + pc_init_deriv_kernel
     for k, (_, stack, local) in deriv.items():
         assert stack == 0 and local == 0, (k, stack, local)
+    regs = {(m.group(1), int(m.group(2))): v[0] for k, v in deriv.items()
+            for m in [re.search(r"deriv_(kmv|grad)_kernelINS_10DerivTableILi0EEELi(\d+)E", k)] if m}
+    assert regs == _DERIV_REGS
     tc = {int(re.search(r"kmv_tc_kernelILi(\d+)E", k).group(1)): v[0] for k, v in res.items() if "kmv_tc_kernel" in k}
     simt = {(int(m.group(1)), int(m.group(2))): v[0] for k, v in res.items()
             for m in [re.search(r"kmv_simt_kernelILi(\d+)ELi(\d+)E", k)] if m}

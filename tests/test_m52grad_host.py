@@ -1,7 +1,7 @@
 """CPU checks of the Matern-5/2 derivative-observation layer (Matern52KernelGrad): the fp64 oracle against the reference's own
 Matern52KernelGrad.forward and its known answer (tests/golden/m52grad_golden.npz) and against autograd second derivatives of the
-Matern-5/2; the kernel class (parameters, diag, the refusals that need no device); and the machine code of m52grad.cu (no stack or
-local memory in any instantiation serving d <= 16) next to the unchanged RBF derivative kernels and fused K.V register counts."""
+Matern-5/2; the kernel class (parameters, diag, the refusals that need no device); and the machine code of its kernels in deriv.cu (no
+stack or local memory in any instantiation serving d <= 16) next to the unchanged RBF derivative kernels and fused K.V register counts."""
 import math
 import os
 import re
@@ -173,16 +173,23 @@ def _res_usage():
 # registers of the fused K.V kernels (CUDA 12.9, -O3, sm_90a), as pinned by tests/test_deriv_host.py: the Matern-5/2 derivative
 # operator adds no code to them
 _TC_REGS = {k: (126 if k == 0 else 124) for k in range(8)}
+# registers of the Matern-5/2 derivative product and gradient kernels, {(job, DP): REG}, as built before they were folded into the
+# RBF kernels over a per-kind table (CUDA 12.9, -O3, sm_90a)
+_M52_REGS = {("kmv", 4): 168, ("kmv", 8): 126, ("kmv", 12): 168, ("kmv", 16): 236,
+             ("grad", 4): 168, ("grad", 8): 224, ("grad", 12): 168, ("grad", 16): 254}
 
 
-def test_m52grad_kernels_have_no_local_memory_and_the_rbf_kernels_stay():
+def test_matern52_table_kernels_have_no_local_memory_and_the_rbf_kernels_stay():
     res = _res_usage()
-    m52 = {k: v for k, v in res.items() if "m52g_" in k or "pc_persistent1_kernelILi69E" in k}
-    assert sum("m52g_kmv_kernel" in k for k in m52) == 4 and sum("m52g_grad_kernel" in k for k in m52) == 4, sorted(m52)
+    m52 = {k: v for k, v in res.items() if "DerivTableILi3E" in k or "pc_persistent1_kernelILi69E" in k}
+    assert sum("deriv_kmv_kernel" in k for k in m52) == 4 and sum("deriv_grad_kernel" in k for k in m52) == 4, sorted(m52)
     assert len(m52) == 4 + 4 + 2 + 1, sorted(m52)   # + rows, diagonal, pivoted-Cholesky source
     for k, (_, stack, local) in m52.items():
         assert stack == 0 and local == 0, (k, stack, local)
-    deriv = {k for k in res if "deriv_" in k or "pc_persistent1_kernelILi67E" in k}
+    regs = {(m.group(1), int(m.group(2))): v[0] for k, v in m52.items()
+            for m in [re.search(r"deriv_(kmv|grad)_kernelINS_10DerivTableILi3EEELi(\d+)E", k)] if m}
+    assert regs == _M52_REGS
+    deriv = {k for k in res if ("deriv_" in k and "DerivTableILi3E" not in k) or "pc_persistent1_kernelILi67E" in k}
     assert len(deriv) == 13 and sum("deriv_kmv_kernel" in k for k in deriv) == 4, sorted(deriv)
     tc = {int(re.search(r"kmv_tc_kernelILi(\d+)E", k).group(1)): v[0] for k, v in res.items() if "kmv_tc_kernel" in k}
     assert tc == _TC_REGS
