@@ -292,6 +292,7 @@ int to_v16(gp_plan* p, const float* V, int64_t ldv, int t, int64_t n, float* V16
 int pack_v_tiles(gp_plan* p, const float* V16);                         // pack.cu (tensor-core B operand of GEMM2)
 int kmv_partials(gp_plan* p, const float* V16, const int* done_flag);   // dispatch simt / tensor cores
 int kmv_tc_launch_kind(gp_plan* p, int kind, const int* done_flag);     // kind may be GP_DERIV + kind
+int product_tc_launch(gp_plan* p, const int* done_flag);                // kmv_tc.cu: the two tensor-core factors of a product plan
 int kmv_simt_launch(gp_plan* p, const float* V16, const int* done_flag);
 int kmv_tc_launch(gp_plan* p, const int* done_flag);
 int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t, int add_noise);
@@ -323,6 +324,7 @@ int kmv_simt_launch_cols(gp_plan* p, int kind, const float* Z1, const float* Z2,
                          int64_t cols_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag);
 int sum_partials_double(gp_plan* p, const double* in, int64_t nblk, int stride, int nout, double* out);   // out[o] = sum_b in[b][o], NaN when xbad
 int64_t bilinear_blocks(const gp_plan* p, int64_t n2);                      // CTAs of one SIMT derivative launch over n2 columns
+void bilinear_split(const gp_plan* p, int64_t n2, dim3* grid, int64_t* cps);  // its grid and columns per split (kmv_simt.cu)
 int bilinear_launch_cols(gp_plan* p, bool ard, const float* Z1, const float* Z2, const float* L16, const float* R16, int64_t n2,
                          int64_t diag_row_begin, double* gout, int gstride, int64_t* nblk_out);
 int pack_v_tiles_rows(gp_plan* p, const float* V16, int64_t nrows, int64_t ntiles, float* Vt);

@@ -377,7 +377,7 @@ static int launch_bilinear(gp_plan* p, const BilinLaunch& a, const float* L16, c
 }
 
 // the SIMT derivative launch split of gp_bilinear_grad over n2 columns
-static void bilinear_split(const gp_plan* p, int64_t n2, dim3* grid, int64_t* cps) {
+void bilinear_split(const gp_plan* p, int64_t n2, dim3* grid, int64_t* cps) {
   int64_t ntj = cdiv(n2, SIMT_TJ);
   int nsp = (int)std::min<int64_t>(ntj, std::max<int64_t>(1, (2 * p->n_sm) / std::max<int64_t>(1, cdiv(p->row_count, SIMT_TI))));
   *cps = cdiv(ntj, nsp) * SIMT_TJ;

@@ -10,12 +10,9 @@
 // One exponential per pair: in the packed units every covariance is poly(rho) 2^e (cov_poly_exp, gp_common.cuh), so
 // prod_f k_f = (prod_f poly_f) ex2(sum_f e_f) costs one ex2 whatever the number of factors, plus one sqrt per Matern factor.
 //
-//   product_tc_kernel    two tensor-core factors, KP_a + KP_b <= 128: the warp-specialised wgmma pipeline of kmv_tc.cu (producer
-//                        warpgroup with a bulk-TMA mbarrier ring, two ping-pong consumers, GEMM2 = P_hi [V_hi; V_lo] + P_lo V_hi)
-//                        with TWO GEMM1 chains per column tile: S_a into s[32] and S_b into the 32 registers that hold P_hi
-//                        afterwards.  Both are dead once GEMM2 of the previous tile has returned, so the live set (s, hi, o1, o2,
-//                        acc) is that of kmv_tc_kernel.  A stage holds the B tile of factor a, the B tile of factor b and the V
-//                        tile; the A tiles of both factors sit side by side.
+//   product_tc_kernel    two tensor-core factors, KP_a + KP_b <= 128: the one warp-specialised wgmma pipeline of kmv_tc.cu, run
+//                        with a second GEMM1 operand (the factors' own packed tiles; S_a into s, S_b into the registers that
+//                        hold P_hi afterwards) and the product covariance in the epilogue.  It and its launcher live in kmv_tc.cu.
 //   product_simt_kernel  2 to 4 factors of a total padded width <= 128 on CUDA cores: the structure of kmv_simt_kernel with the
 //                        factors' packed rows staged back to back, direct differences per factor, exact a_f = 0 on the diagonal.
 //   product_bilinear_kernel  one pass over the pairs for every factor's lengthscale gradient and dF/dS (fp32, fp64 block partials).
@@ -24,11 +21,8 @@
 #include <algorithm>
 
 #include "gp_common.cuh"
-#include "tc_ptx.cuh"
 
 namespace gp {
-
-using namespace ptx;
 
 // ---- the factors as a kernel argument (indexed with compile-time constants only) ------------------------------------------
 struct ProdFactors {
@@ -248,229 +242,6 @@ product_bilinear_kernel(const ProdFactors pf, const float* __restrict__ L16, con
   }
 }
 
-// ---- (b) tensor-core product kernel for two factors ------------------------------------------------------------------------
-constexpr int PTC_THREADS = 384;                    // producer warpgroup + 2 consumer warpgroups
-constexpr int PV_TF32_BYTES = 2 * TILE_J * TP * 4;  // the tf32 part of a packed V tile (pack.cu)
-constexpr int PV_TILE_BYTES = V_TILE_FLOATS * 4;
-constexpr int PTC_MAX_NS = 12;
-constexpr uint32_t PTC_TURN_BAR0 = 1;               // named barriers 1, 2: consumer 0's / 1's turn on the tensor core
-
-struct ProdBars {
-  uint64_t a_full;
-  uint64_t b_full[PTC_MAX_NS];
-  uint64_t b_empty[PTC_MAX_NS];   // 256 arrivals: every consumer thread, after its warpgroup's GEMM2 has read the stage
-};
-
-// XA_f / XB_f: the factors' own packed operand tiles (pack.cu), widths KPa / KPb; the roles, barriers and turn order are those of
-// kmv_tc_kernel (see its header comment), the differences are marked "product".
-template <bool RBF_A, bool RBF_B>
-__global__ void __maxnreg__(128)
-product_tc_kernel(const float* __restrict__ XAa, const float* __restrict__ XAb, const float* __restrict__ XBa,
-                  const float* __restrict__ XBb, const float* __restrict__ Vt, float* __restrict__ partial, int KPa, int KPb, int NS,
-                  int64_t ntile_j, int64_t tiles_per_split, int64_t rows_pad, int same, int64_t row_begin, CovPoly ca, CovPoly cb,
-                  const int* __restrict__ done_flag) {
-  if (done_flag && *done_flag) return;  // CTA-uniform, before any barrier exists
-  extern __shared__ __align__(128) uint8_t smem[];
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int64_t it = blockIdx.x;
-  const int split = blockIdx.y;
-  const int64_t jt0 = (int64_t)split * tiles_per_split;
-  const int64_t jt1 = min(ntile_j, jt0 + tiles_per_split);
-  const int T = (int)max((int64_t)0, jt1 - jt0);
-
-  // product: [A_a | A_b | NS x (B_a | B_b | V) | barriers]
-  const uint32_t aa_bytes = (uint32_t)KPa * TILE_I * 4, ab_bytes = (uint32_t)KPb * TILE_I * 4;
-  const uint32_t ba_bytes = (uint32_t)KPa * TILE_J * 4, bb_bytes = (uint32_t)KPb * TILE_J * 4;
-  const uint32_t b_bytes = ba_bytes + bb_bytes;
-  const uint32_t stage_bytes = b_bytes + PV_TF32_BYTES;
-  uint8_t* sA = smem;
-  uint8_t* sStage = smem + aa_bytes + ab_bytes;
-  ProdBars* bars = reinterpret_cast<ProdBars*>(sStage + (size_t)NS * stage_bytes);
-
-  if (threadIdx.x == 0) {
-    mbar_init(smem_u32(&bars->a_full), 1);
-    for (int s = 0; s < PTC_MAX_NS; ++s) {
-      mbar_init(smem_u32(&bars->b_full[s]), 1);
-      mbar_init(smem_u32(&bars->b_empty[s]), 256);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();   // the last CTA-wide barrier: the roles below never meet all 384 threads again
-  if (T == 0) return;
-
-  if (warp < 4) {
-    // ---- producer ----
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(smem_u32(&bars->a_full), aa_bytes + ab_bytes);
-      bulk_g2s(smem_u32(sA), XAa + it * (int64_t)TILE_I * KPa, aa_bytes, smem_u32(&bars->a_full));
-      bulk_g2s(smem_u32(sA + aa_bytes), XAb + it * (int64_t)TILE_I * KPb, ab_bytes, smem_u32(&bars->a_full));
-      int s = 0;
-      uint32_t par = 0;   // phase of b_empty[s] the consumers complete when they release the stage's previous tile
-      for (int u = 0; u < T; ++u) {
-        if (u >= NS) mbar_wait(smem_u32(&bars->b_empty[s]), par);
-        const uint32_t full = smem_u32(&bars->b_full[s]);
-        uint8_t* st = sStage + (size_t)s * stage_bytes;
-        const int64_t jt = jt0 + u;
-        mbar_arrive_expect_tx(full, stage_bytes);
-        bulk_g2s(smem_u32(st), XBa + jt * (int64_t)TILE_J * KPa, ba_bytes, full);
-        bulk_g2s(smem_u32(st + ba_bytes), XBb + jt * (int64_t)TILE_J * KPb, bb_bytes, full);
-        bulk_g2s(smem_u32(st + b_bytes), reinterpret_cast<const uint8_t*>(Vt) + jt * (int64_t)PV_TILE_BYTES, PV_TF32_BYTES, full);
-        if (++s == NS) {
-          s = 0;
-          if (u >= NS) par ^= 1;
-        }
-      }
-    }
-    return;
-  }
-
-  // ---- consumers (accumulator fragment layout: kmv_tc_kernel) ----
-  const int wg = (warp >> 2) - 1;   // consumer 0 / 1
-  const int wq = warp & 3;
-  const int g = lane >> 2, t = lane & 3;
-  const int64_t rloc0 = it * TILE_I + wg * 64 + wq * 16 + g;
-  const int64_t diag_off = row_begin + it * TILE_I + wg * 64 - jt0 * TILE_J;
-  const uint64_t aa_desc0 = gmma_desc(smem_u32(sA) + (uint32_t)wg * 8 * 128, TILE_I * 16, 128);
-  const uint64_t ab_desc0 = gmma_desc(smem_u32(sA + aa_bytes) + (uint32_t)wg * 8 * 128, TILE_I * 16, 128);
-  constexpr uint64_t A_KSTEP = (2 * TILE_I * 16) >> 4, B_KSTEP = (2 * TILE_J * 16) >> 4, V_KSTEP = (2 * 2 * TP * 16) >> 4;
-  const int ksteps_a = KPa / 8, ksteps_b = KPb / 8;
-  const uint32_t my_turn = PTC_TURN_BAR0 + wg, other_turn = PTC_TURN_BAR0 + (wg ^ 1);
-
-  float acc[8];
-#pragma unroll
-  for (int c = 0; c < 8; ++c) acc[c] = 0.f;
-  float s[32], o1[16], o2[8];   // s: S_a of the current tile, then P, then P_lo
-  float hi[32];                 // product: S_b of the current tile, then P_hi (tf32 bit pattern)
-
-  auto stage_addr = [&](int sb) { return smem_u32(sStage + (size_t)sb * stage_bytes); };
-  // product: GEMM1 of both factors for the tile in stage sb, S_a into s and S_b into hi, two chains in one batch
-  auto issue_gemm1 = [&](int sb) {
-    const uint64_t ba_desc0 = gmma_desc(stage_addr(sb), TILE_J * 16, 128);
-    const uint64_t bb_desc0 = gmma_desc(stage_addr(sb) + ba_bytes, TILE_J * 16, 128);
-    wgmma_m64n64k8_ss_first(s, aa_desc0, ba_desc0);
-#pragma unroll 1
-    for (int ks = 1; ks < ksteps_a; ++ks) wgmma_m64n64k8_ss(s, aa_desc0 + ks * A_KSTEP, ba_desc0 + ks * B_KSTEP, 1u);
-    wgmma_m64n64k8_ss_first(hi, ab_desc0, bb_desc0);
-#pragma unroll 1
-    for (int ks = 1; ks < ksteps_b; ++ks) wgmma_m64n64k8_ss(hi, ab_desc0 + ks * A_KSTEP, bb_desc0 + ks * B_KSTEP, 1u);
-  };
-  auto run_gemm2 = [&](int sb) {
-    const uint64_t v_desc0 = gmma_desc(stage_addr(sb) + b_bytes, 2 * TP * 16, 128);   // rows 0-15 V_hi, 16-31 V_lo
-    fence_regs(o1);
-    wgmma_fence();
-    wgmma_m64n32k8_rs_first(o1, __float_as_uint(hi[0]), __float_as_uint(hi[1]), __float_as_uint(hi[2]), __float_as_uint(hi[3]), v_desc0);
-#pragma unroll
-    for (int jb = 1; jb < TILE_J / 8; ++jb)
-      wgmma_m64n32k8_rs(o1, __float_as_uint(hi[4 * jb]), __float_as_uint(hi[4 * jb + 1]), __float_as_uint(hi[4 * jb + 2]),
-                        __float_as_uint(hi[4 * jb + 3]), v_desc0 + jb * V_KSTEP, 1u);
-    wgmma_commit();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) s[i] = s[i] - hi[i];
-    fence_regs(s);
-    fence_regs(o2);
-    wgmma_fence();
-    wgmma_m64n16k8_rs_first(o2, __float_as_uint(s[0]), __float_as_uint(s[1]), __float_as_uint(s[2]), __float_as_uint(s[3]), v_desc0);
-#pragma unroll
-    for (int jb = 1; jb < TILE_J / 8; ++jb)
-      wgmma_m64n16k8_rs(o2, __float_as_uint(s[4 * jb]), __float_as_uint(s[4 * jb + 1]), __float_as_uint(s[4 * jb + 2]),
-                        __float_as_uint(s[4 * jb + 3]), v_desc0 + jb * V_KSTEP, 1u);
-    wgmma_commit();
-    wgmma_wait_all();
-    fence_regs(s);
-    fence_regs(hi);
-    fence_regs(o1);
-    fence_regs(o2);
-  };
-  // product: P = poly_a poly_b ex2(e_a + e_b) of tile u (arguments in s and hi) and its tf32 part P_hi
-  auto epilogue = [&](int u) {
-    const int64_t d = diag_off - (int64_t)u * TILE_J;
-    if (same && d > -64 && d < TILE_J) {
-      const int dr = (int)d + wq * 16 + g - t;
-#pragma unroll
-      for (int i = 0; i < 32; ++i)   // both arguments are exactly 0 on the diagonal
-        if (dr + 8 * ((i >> 1) & 1) - 8 * (i >> 2) - 4 * (i & 1) == 0) {
-          s[i] = 0.f;
-          hi[i] = 0.f;
-        }
-    }
-#pragma unroll
-    for (int jb = 0; jb < TILE_J / 8; ++jb) {
-      float pv[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        float pa, ea, pb, eb;
-        cov_poly_exp<false>(RBF_A, ca, s[4 * jb + k], &pa, &ea);
-        cov_poly_exp<false>(RBF_B, cb, hi[4 * jb + k], &pb, &eb);
-        pv[k] = (pa * pb) * ex2_approx(ea + eb);
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        s[4 * jb + k] = pv[(k >> 1) | ((k & 1) << 1)];   // k = 0 1 2 3 <- accumulator register 0 2 1 3
-        hi[4 * jb + k] = __uint_as_float(__float_as_uint(s[4 * jb + k]) & 0xFFFFE000u);
-      }
-    }
-  };
-  auto fold = [&](int sb) {
-    mbar_arrive(smem_u32(&bars->b_empty[sb]));   // this thread's share of the stage has been read
-#pragma unroll
-    for (int c = 0; c < 8; ++c) acc[c] += o1[c] + o1[c + 8] + o2[c];
-  };
-  auto issue_gemm1_batch = [&](int sb) {
-    fence_regs(s);
-    fence_regs(hi);
-    wgmma_fence();
-    issue_gemm1(sb);
-    wgmma_commit();
-  };
-  auto wait_gemm1 = [&]() {
-    wgmma_wait_all();
-    fence_regs(s);
-    fence_regs(hi);
-  };
-
-  mbar_wait(smem_u32(&bars->a_full), 0);
-  if (wg == 1) named_bar_arrive(PTC_TURN_BAR0, 256);   // consumer 0 takes the first turn
-
-  // turn 0: GEMM1 of tile 0
-  mbar_wait(smem_u32(&bars->b_full[0]), 0);
-  named_bar_sync(my_turn, 256);
-  issue_gemm1_batch(0);
-  named_bar_arrive(other_turn, 256);
-  wait_gemm1();
-  epilogue(0);
-
-  // turns 1 .. T - 1: GEMM2 of tile u - 1, then GEMM1 of tile u
-  int sb_prev = 0, sb = 1;   // NS >= 2 (product_tc_launch)
-  uint32_t par = 0;
-#pragma unroll 1
-  for (int u = 1; u < T; ++u) {
-    mbar_wait(smem_u32(&bars->b_full[sb]), par);
-    named_bar_sync(my_turn, 256);
-    run_gemm2(sb_prev);
-    fold(sb_prev);
-    issue_gemm1_batch(sb);
-    named_bar_arrive(other_turn, 256);
-    wait_gemm1();
-    epilogue(u);
-    sb_prev = sb;
-    if (++sb == NS) { sb = 0; par ^= 1; }
-  }
-
-  // last turn: GEMM2 of tile T - 1; consumer 1 has no one to hand the tensor core to
-  named_bar_sync(my_turn, 256);
-  run_gemm2(sb_prev);
-  if (wg == 0) named_bar_arrive(other_turn, 256);
-  fold(sb_prev);
-
-#pragma unroll
-  for (int c = 0; c < 8; c += 2) {
-    const int64_t row = rloc0 + 8 * ((c >> 1) & 1);
-    float2* dst = reinterpret_cast<float2*>(partial + ((int64_t)split * rows_pad + row) * TP + 8 * (c >> 2) + 2 * t);
-    *dst = make_float2(acc[c], acc[c + 1]);
-  }
-}
-
 // ---- small kernels ---------------------------------------------------------------------------------------------------------------
 __global__ void product_or_flags_kernel(const int* f0, const int* f1, const int* f2, const int* f3, int* out) {
   *out = (*f0 | *f1 | (f2 ? *f2 : 0) | (f3 ? *f3 : 0)) ? 1 : 0;
@@ -561,46 +332,24 @@ int product_refresh(gp_plan* p) {
   return GP_OK;
 }
 
-template <bool RA, bool RB>
-static int product_tc_launch_kind(gp_plan* p, const int* done_flag) {
-  const gp_plan* a = p->factors[0];
-  const gp_plan* b = p->factors[1];
-  const int a_bytes = p->KP * TILE_I * 4, stage = p->KP * TILE_J * 4 + PV_TF32_BYTES;
-  // one CTA per SM: the whole 227 KB opt-in shared memory
-  const int ns = std::min(PTC_MAX_NS, (226 * 1024 - a_bytes - (int)sizeof(ProdBars)) / stage);
-  GP_REQUIRE(ns >= 2, GP_E_SHAPE, "kernel product: smem ring too small for KP=%d", p->KP);
-  GP_CHECK((opt_in_smem<product_tc_kernel<RA, RB>>(p->device, 227 * 1024)));
-  dim3 grid((unsigned)p->ntile_i, (unsigned)p->nsplit);
-  product_tc_kernel<RA, RB><<<grid, PTC_THREADS, a_bytes + ns * stage + (int)sizeof(ProdBars), p->stream>>>(
-      a->XA.as<float>(), b->XA.as<float>(), a->XB.as<float>(), b->XB.as<float>(), p->Vtiles.as<float>(), p->partial.as<float>(), a->KP,
-      b->KP, ns, p->ntile_j, p->tiles_per_split, p->rows_pad, p->same ? 1 : 0, p->row_begin, cov_poly_of(a->kind), cov_poly_of(b->kind),
-      done_flag);
-  return GP_OK;
-}
-
 // the tensor-core kernel reads the plan's packed V tiles (pack_v_tiles by the caller), the CUDA-core kernel the fp32 rows V16
 int product_kmv_launch(gp_plan* p, const float* V16, const int* done_flag) {
   GP_CHECK(product_refresh(p));
-  if (p->prod_tc) {
-    const bool ra = p->factors[0]->kind == GP_RBF, rb = p->factors[1]->kind == GP_RBF;
-    GP_CHECK(ra ? (rb ? product_tc_launch_kind<true, true>(p, done_flag) : product_tc_launch_kind<true, false>(p, done_flag))
-                : (rb ? product_tc_launch_kind<false, true>(p, done_flag) : product_tc_launch_kind<false, false>(p, done_flag)));
-  } else {
-    GP_REQUIRE(V16 != nullptr, GP_E_STATE, "kernel product: fp32 rows of V needed for the CUDA-core kernel");
-    const ProdFactors pf = prod_factors(p);
-    dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)p->nsplit);
-    const int64_t cps = p->tiles_per_split * SIMT_TJ;
+  if (p->prod_tc) return product_tc_launch(p, done_flag);
+  GP_REQUIRE(V16 != nullptr, GP_E_STATE, "kernel product: fp32 rows of V needed for the CUDA-core kernel");
+  const ProdFactors pf = prod_factors(p);
+  dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)p->nsplit);
+  const int64_t cps = p->tiles_per_split * SIMT_TJ;
 #define GP_PROD_SIMT_CASE(D)                                                                                                      \
   case D:                                                                                                                         \
     product_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(pf, V16, p->partial.as<float>(), p->row_count, p->n2, p->rows_pad, cps, \
                                                             p->same ? 1 : 0, p->row_begin, done_flag);                            \
     break;
-    switch (round_dpt(p->DP)) {
-      GP_PROD_SIMT_CASE(8) GP_PROD_SIMT_CASE(12) GP_PROD_SIMT_CASE(16) GP_PROD_SIMT_CASE(24) GP_PROD_SIMT_CASE(32)
-      GP_PROD_SIMT_CASE(48) GP_PROD_SIMT_CASE(64) GP_PROD_SIMT_CASE(96) GP_PROD_SIMT_CASE(128)
-    }
-#undef GP_PROD_SIMT_CASE
+  switch (round_dpt(p->DP)) {
+    GP_PROD_SIMT_CASE(8) GP_PROD_SIMT_CASE(12) GP_PROD_SIMT_CASE(16) GP_PROD_SIMT_CASE(24) GP_PROD_SIMT_CASE(32)
+    GP_PROD_SIMT_CASE(48) GP_PROD_SIMT_CASE(64) GP_PROD_SIMT_CASE(96) GP_PROD_SIMT_CASE(128)
   }
+#undef GP_PROD_SIMT_CASE
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -639,13 +388,10 @@ int product_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float*
   GP_REQUIRE(p->DP <= 64, GP_E_SHAPE, "bilinear gradient of a kernel product supports a total padded input width <= 64 (got %d)", p->DP);
   const int DPT = round_dpt(p->DP), nout = 1 + DPT;
   const ProdFactors pf = prod_factors(p);
-  // the launch split of the plain SIMT derivative kernel (kmv_simt.cu)
-  const int64_t ntj = cdiv(p->n2, SIMT_TJ), nbi = cdiv(p->row_count, SIMT_TI);
-  int nsp = (int)std::min<int64_t>(ntj, std::max<int64_t>(1, (2 * p->n_sm) / std::max<int64_t>(1, nbi)));
-  const int64_t cps = cdiv(ntj, nsp) * SIMT_TJ;
-  nsp = (int)cdiv(p->n2, cps);
-  const dim3 grid((unsigned)nbi, (unsigned)nsp);
-  const int64_t nblk = nbi * nsp;
+  dim3 grid;
+  int64_t cps;
+  bilinear_split(p, p->n2, &grid, &cps);
+  const int64_t nblk = (int64_t)grid.x * grid.y;
   GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
   GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
   GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
