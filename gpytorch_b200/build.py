@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
-SOURCES = ["api.cu", "pack.cu", "kmv_simt.cu", "kmv_tc.cu", "cg.cu", "pivchol.cu", "slq.cu", "lanczos.cu", "comm.cu", "ski.cu", "sum.cu", "minres.cu", "lowrank.cu", "xgrad.cu", "tasks.cu", "kron.cu", "deriv.cu", "product.cu"]
+SOURCES = ["api.cu", "pack.cu", "kmv_simt.cu", "kmv_tc.cu", "cg.cu", "pivchol.cu", "slq.cu", "lanczos.cu", "comm.cu", "ski.cu", "sum.cu", "minres.cu", "lowrank.cu", "xgrad.cu", "tasks.cu", "kron.cu", "deriv.cu", "product.cu", "additive.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 LIB = os.path.join(LIBDIR, "libgpbbmm.so")

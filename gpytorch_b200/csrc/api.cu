@@ -128,6 +128,7 @@ extern "C" int gp_plan_set_backend(gp_plan* p, int backend) {
   GP_REQUIRE(p->kron == nullptr, GP_E_STATE, "a Kronecker plan runs the backend of its data plan");
   GP_REFUSE_DERIV(p, "gp_plan_set_backend");
   GP_REFUSE_PRODUCT(p, "gp_plan_set_backend");
+  GP_REFUSE_ADDITIVE(p, "gp_plan_set_backend");
   p->backend_req = backend;
   if (p->data_set && p->hypers_set) return pack_inputs(p);
   return GP_OK;
@@ -213,6 +214,8 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
   GP_REQUIRE(!(p->deriv && comm && comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   GP_REQUIRE(!(p->backend_req == GP_BACKEND_PRODUCT && comm && comm->world > 1), GP_E_STATE,
              "gp_plan_set_comm with more than one rank is not available on a kernel-product plan (gp_plan_set_product)");
+  GP_REQUIRE(!(p->add_M && comm && comm->world > 1), GP_E_STATE,
+             "gp_plan_set_comm with more than one rank is not available on an additive plan (gp_plan_set_additive)");
   p->comm = comm;
   return GP_OK;
 }
@@ -247,6 +250,7 @@ extern "C" int gp_time_kmv_kernel(gp_plan* p, const float* V, int64_t ldv, int t
     if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_PRODUCT) return product_kmv_launch(p, p->V16.as<float>(), nullptr);
+    if (p->add_M) return additive_kmv_launch(p, p->V16.as<float>(), nullptr);
     return p->backend == GP_BACKEND_TCGEN05 ? kmv_tc_launch(p, nullptr) : kmv_simt_launch(p, p->V16.as<float>(), nullptr);
   };
   for (int i = 0; i < warmup; ++i) GP_CHECK(launch());

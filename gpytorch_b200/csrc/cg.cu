@@ -648,7 +648,7 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   bool finished = false;
   for (int kk = 0; kk < max_iter && !finished; ++kk) {
     if ((status = kmv()) != GP_OK) break;
-    cg_finishv_wtv_kernel<true><<<G, RP_THREADS, sh_b, st>>>(p->partial.as<float>(), nslots(p), p->rows_pad, p->outputscale, part_scale_ptr(p), p->noise, dvec, P, V,
+    cg_finishv_wtv_kernel<true><<<G, RP_THREADS, sh_b, st>>>(p->partial.as<float>(), nslots(p), p->rows_pad, kernel_scale(p), part_scale_ptr(p), p->noise, dvec, P, V,
                                                           nullptr, W, k, wp, n, red1, L1, done, p->xbad);
     cg_sum_launch(red1, G, L1, sums1, done, st);
     if ((status = allreduce(p, sums1, L1)) != GP_OK) break;

@@ -505,6 +505,8 @@ static int deriv_set(gp_plan* p, gp_plan* data, int kind, const char* what) {
   GP_REFUSE_KRON(p, what);
   GP_REFUSE_PRODUCT(p, what);
   if (data) GP_REQUIRE(data->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "%s (as the data plan) is not available on a kernel-product plan (gp_plan_set_product)", what);
+  GP_REFUSE_ADDITIVE(p, what);
+  if (data) GP_REQUIRE(data->add_M == 0, GP_E_STATE, "%s (as the data plan) is not available on an additive plan (gp_plan_set_additive)", what);
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   gp_deriv_state* ds = p->deriv ? p->deriv : new gp_deriv_state();
   gp_plan* old = ds->data;

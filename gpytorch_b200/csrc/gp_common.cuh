@@ -271,6 +271,11 @@ struct gp_plan {
   bool prod_tc = false;           // two tensor-core factors with KP_a + KP_b <= 128: product_tc_kernel, else product_simt_kernel
   uint64_t pack_gen = 0;          // bumped by every re-pack of a plain plan
   uint64_t fac_gen[4] = {0, 0, 0, 0};   // the factors' pack_gen at the last product_pack
+  // additive GPs (additive.cu): sum_{m=1}^{add_M} e_m(c_1 .. c_D), c_i = add_s[i] k(x_i, x'_i) over the D = d columns of a plain
+  // SIMT plan with D ARD lengthscales; add_M = 0 is a plain plan.  The plan's outputscale is not applied (kernel_scale)
+  int add_M = 0;
+  std::vector<float> add_s;       // the D component scales
+  double add_diag = 0.0;          // sum_{m=1}^{M} e_m(s_1 .. s_D): the constant diagonal of a square operator
   int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
@@ -370,6 +375,17 @@ inline const float* part_scale_ptr(gp_plan* p) {
 }
 #define GP_REFUSE_LOWRANK(p, what) \
   GP_REQUIRE((p)->lr_U == nullptr, GP_E_STATE, "%s is not available on a plan with a low-rank correction (gp_plan_set_lowrank)", what)
+// the scale the finish kernels apply to the backend's slots: the outputscale, or 1 on an additive plan (whose components carry
+// their own scales)
+inline float kernel_scale(const gp_plan* p) { return p->add_M ? 1.f : p->outputscale; }
+// additive.cu
+int additive_pack(gp_plan* p);                                          // checks the plan against its components, forms add_diag
+int additive_kmv_launch(gp_plan* p, const float* V16, const int* done_flag);
+int additive_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
+int additive_kdiag(gp_plan* p, float* OUT);
+int additive_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+#define GP_REFUSE_ADDITIVE(p, what) \
+  GP_REQUIRE((p)->add_M == 0, GP_E_STATE, "%s is not available on an additive plan (gp_plan_set_additive)", what)
 inline bool plan_is_tc(const gp_plan* p) {
   return p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_tc) || (p->backend == GP_BACKEND_PRODUCT && p->prod_tc);
 }
@@ -474,6 +490,52 @@ __device__ __forceinline__ void dcov_poly_exp(bool rbf, CovPoly c, float a, floa
     *e = -LOG2E * rho;
   }
 }
+// Additive GPs (additive.cu): components c_i = s_i k_i(z_i - z'_i) over one packed column each, combined by the positive
+// recurrence e_m <- e_m + c_i e_{m-1} (m = M .. 1) into K = sum_{m=1}^{M} e_m(c_1 .. c_D).  No alternating signs: nothing cancels.
+constexpr int ADD_DMAX = 32;   // components
+constexpr int ADD_MMAX = 8;    // interaction degree
+struct AddHyp {
+  float s[ADD_DMAX];   // component scales (0 beyond D)
+  int D, M;
+  int rbf;             // kind RBF (else Matern with polynomial cp)
+  CovPoly cp;
+};
+// e[0 .. MT] <- the recurrence with one more component c (degrees above M untouched; MT = M folds the test away)
+template <int MT, class T>
+__device__ __forceinline__ void esym_push(T (&e)[MT + 1], T c, int M) {
+#pragma unroll
+  for (int m = MT; m >= 1; --m)
+    if (m <= M) e[m] = fma(c, e[m - 1], e[m]);
+}
+template <int MT, class T>
+__device__ __forceinline__ T esym_total(const T (&e)[MT + 1], int M) {
+  T k = e[1];
+#pragma unroll
+  for (int m = 2; m <= MT; ++m)
+    if (m <= M) k += e[m];
+  return k;
+}
+// k_i of one component from its packed difference df (RBF: poly = 1 folds away)
+template <bool RBF>
+__device__ __forceinline__ float add_comp(CovPoly cp, float df) {
+  float pl, ex;
+  cov_poly_exp<true>(RBF, cp, -0.5f * (df * df), &pl, &ex);
+  return pl * ex2_approx(ex);
+}
+// one entry K(a, b) from two packed rows (rows, diagonal, pivoted Cholesky)
+template <bool RBF>
+__device__ __forceinline__ float add_pair(const AddHyp& h, const float* za, const float* zb) {
+  float e[ADD_MMAX + 1];
+  e[0] = 1.f;
+#pragma unroll
+  for (int m = 1; m <= ADD_MMAX; ++m) e[m] = 0.f;
+  for (int c = 0; c < h.D; ++c) esym_push<ADD_MMAX>(e, h.s[c] * add_comp<RBF>(h.cp, za[c] - zb[c]), h.M);
+  return esym_total<ADD_MMAX>(e, h.M);
+}
+__device__ __forceinline__ float add_pair_rt(const AddHyp& h, const float* za, const float* zb) {
+  return h.rbf ? add_pair<true>(h, za, zb) : add_pair<false>(h, za, zb);
+}
+AddHyp additive_hyp(const gp_plan* p);   // additive.cu: the kernel argument of an additive plan
 // input-derivative factor q = dk/da of the same covariance (xgrad.cu): dk/dz_i = -q (z_i - z_j) in the packed units.
 //   RBF: ln2 2^a ; M12: e / (2 rho) ; M32: e / 2 ; M52: (1 + rho) e / 6      (e = exp(-rho), rho^2 = -a)
 // q is the h of the raw-unit form  dk/dx_i = -h (x_i - x_j) / l^2  times l^2 / C (C = log2 e, 2, 6, 10 as in pack.cu).  A pair at

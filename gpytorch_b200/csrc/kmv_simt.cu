@@ -141,6 +141,7 @@ static int kmv_partials_base(gp_plan* p, const float* V16, const int* done_flag)
     GP_CHECK(pack_v_tiles(p, V16));
     return kmv_tc_launch(p, done_flag);
   }
+  if (p->add_M) return additive_kmv_launch(p, V16, done_flag);
   return kmv_simt_launch(p, V16, done_flag);
 }
 
@@ -179,7 +180,7 @@ int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t
   float na = (add_noise && p->same) ? p->noise : 0.f;
   const float* dv = (add_noise && p->same) ? p->noise_diag : nullptr;
   kmv_finish_user_kernel<<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(p->partial.as<float>(), nslots(p), p->row_count,
-                                                                          rows_pad, p->outputscale, part_scale_ptr(p), na, dv, V16, p->row_begin,
+                                                                          rows_pad, kernel_scale(p), part_scale_ptr(p), na, dv, V16, p->row_begin,
                                                                           OUT, ldo, t, p->xbad);
   p->launches++;
   GP_CUDA(cudaGetLastError());
@@ -438,6 +439,7 @@ extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, i
 
 static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   if (p->backend == GP_BACKEND_SKI) return ski_krows(p, idx, m, OUT, ldo);   // separable entries (ski_rows.cuh)
+  if (p->add_M) return additive_krows(p, idx, m, OUT, ldo);
   const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
   dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
   size_t sh = sizeof(float) * p->DP;
@@ -481,6 +483,7 @@ extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
 
 static int kdiag_base(gp_plan* p, float* OUT) {
   if (p->backend == GP_BACKEND_SKI) return ski_kdiag(p, OUT);   // not constant: w_i^T K_uu w_i (ski_rows.cuh)
+  if (p->add_M) return additive_kdiag(p, OUT);   // square: the constant sum_m e_m(s); cross: per pair
   if (p->same) {
     // stationary kernels: k(x,x) = outputscale (lazy_evaluated_kernel_tensor.py:107-133 evaluates kernel(diag=True))
     fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, p->outputscale);
@@ -515,6 +518,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   if (p->backend == GP_BACKEND_PRODUCT) return product_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->kron) return kron_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->deriv) return deriv_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
+  if (p->add_M) return additive_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   // before any launch: the SIMT derivative kernel is instantiated up to DP = 64
   GP_REQUIRE(p->backend == GP_BACKEND_SKI || p->DP <= 64, GP_E_SHAPE, "bilinear gradient supports d <= 64 (d=%d)", p->d);
   const bool ard = p->ls.size() > 1;

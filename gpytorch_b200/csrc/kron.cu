@@ -366,6 +366,8 @@ extern "C" int gp_plan_set_kron(gp_plan* p, gp_plan* data, int T) {
   GP_REFUSE_DERIV(p, "gp_plan_set_kron");
   GP_REFUSE_PRODUCT(p, "gp_plan_set_kron");
   if (data) GP_REFUSE_PRODUCT(data, "gp_plan_set_kron (as the data plan)");
+  GP_REFUSE_ADDITIVE(p, "gp_plan_set_kron");
+  if (data) GP_REFUSE_ADDITIVE(data, "gp_plan_set_kron (as the data plan)");
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   gp_kron_state* ks = p->kron ? p->kron : new gp_kron_state();
   const bool keep_b = p->kron && ks->T == T && ks->b_set;

@@ -531,7 +531,7 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
       const double* ck = cbuf[kk & 1];
       ms_scale_kernel<<<G, RP_THREADS, shp, st>>>(Qcur, ck, U, k, p->noise, dvec, X, n, done);
       if ((status = kmv_partials(p, X, done)) != GP_OK) break;
-      ms_finish_kernel<true><<<G, RP_THREADS, shp, st>>>(p->partial.as<float>(), nslots(p), p->rows_pad, p->outputscale, part_scale_ptr(p),
+      ms_finish_kernel<true><<<G, RP_THREADS, shp, st>>>(p->partial.as<float>(), nslots(p), p->rows_pad, kernel_scale(p), part_scale_ptr(p),
                                                          p->noise, dvec, X, Qcur, Qoth, V, n, S, kk, U, k, part1, done, p->xbad);
       cg_sum_launch(part1, G, L, sumsA, done, st);
       ms_orth_kernel<true><<<G, RP_THREADS, shp, st>>>(sumsA, ck, Qcur, V, n, U, k, part2, done);
@@ -540,7 +540,7 @@ int ciq_run(gp_plan* p, const float* B, int64_t ldb, int t, const float* U, int 
       p->launches += 6;
     } else {
       if ((status = kmv_partials(p, Qcur, done)) != GP_OK) break;
-      ms_finish_kernel<false><<<G, RP_THREADS, shp, st>>>(p->partial.as<float>(), nslots(p), p->rows_pad, p->outputscale, part_scale_ptr(p),
+      ms_finish_kernel<false><<<G, RP_THREADS, shp, st>>>(p->partial.as<float>(), nslots(p), p->rows_pad, kernel_scale(p), part_scale_ptr(p),
                                                           p->noise, dvec, nullptr, Qcur, Qoth, V, n, S, kk, nullptr, 0, part1, done, p->xbad);
       cg_sum_launch(part1, G, TP, sums, done, st);
       ms_orth_kernel<false><<<G, RP_THREADS, shp, st>>>(sums, nullptr, Qcur, V, n, nullptr, 0, part2, done);

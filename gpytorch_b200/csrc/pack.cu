@@ -148,6 +148,7 @@ int choose_geometry(gp_plan* p) {
   p->KP = ((kp + 7) / 8) * 8;
   int want = p->backend_req;
   if (want == GP_BACKEND_AUTO) want = (p->KP <= KP_MAX) ? GP_BACKEND_TCGEN05 : GP_BACKEND_SIMT;
+  if (p->add_M) want = GP_BACKEND_SIMT;   // additive plans run their own CUDA-core kernels on Z (additive.cu)
   GP_REQUIRE(!(want == GP_BACKEND_TCGEN05 && p->KP > KP_MAX), GP_E_SHAPE,
              "tcgen05 (tensor-core) backend needs 3d+4 <= %d (d=%d)", KP_MAX, p->d);
   p->backend = want;
@@ -238,6 +239,7 @@ int pack_inputs(gp_plan* p) {
     GP_CHECK(p->Vtiles.ensure(sizeof(float) * p->ntile_j * (2 * TILE_J * TP + TILE_J * TP / 2)));
   }
   p->nparts = p->tasks ? 1 : p->nsplit;   // a Hadamard product is combined into one slot in user row order
+  if (p->add_M) GP_CHECK(additive_pack(p));
   GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)nslots(p) * p->rows_pad * TP));
   GP_CUDA(cudaGetLastError());
   return GP_OK;

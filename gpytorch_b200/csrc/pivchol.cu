@@ -200,6 +200,8 @@ constexpr int PC_KIND_DERIV = 67;
 constexpr int PC_KIND_PRODUCT = 68;
 // Matern-5/2 derivative observations: rows as PC_KIND_DERIV, entries from the Matern-5/2 table
 constexpr int PC_KIND_M52GRAD = 69;
+// additive GPs (additive.cu): K[pivot, j] = sum_{m=1}^{M} e_m(s_i k_i(z_pivot,i - z_j,i)) from the plan's packed rows
+constexpr int PC_KIND_ADDITIVE = 70;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -210,6 +212,7 @@ struct PcTerms {
   int T;
   int rep;           // PC_KIND_TASK / PC_KIND_DERIV / PC_KIND_M52GRAD: rows per point
   const DerivHyp* dh;   // PC_KIND_DERIV / PC_KIND_M52GRAD
+  AddHyp ah;            // PC_KIND_ADDITIVE
 };
 __device__ __forceinline__ int pc_task_of(const PcTerms& tt, int r) { return tt.task ? tt.task[r] : r % tt.rep; }
 __device__ __forceinline__ float pc_cov_rt(int kind, float a) {
@@ -315,6 +318,8 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
           }
         } else if (KIND == PC_KIND_SKI) {
           v = ski_entry(sk, zp, pi, j);
+        } else if (KIND == PC_KIND_ADDITIVE) {
+          v = add_pair_rt(tt.ah, zp, Z + j * DP);
         } else if (KIND == PC_KIND_TASK) {
           const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
           float s = 0.f;
@@ -824,6 +829,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_CUDA(cudaMemsetAsync(piv, 0, sizeof(int64_t) * rank, st));
   const bool sum = p->backend == GP_BACKEND_SUM;
   const bool ski = p->backend == GP_BACKEND_SKI;
+  const bool add = p->add_M > 0;
   PcTerms tt;
   memset(&tt, 0, sizeof(tt));
   SkiRows sk;
@@ -869,6 +875,9 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   } else if (tasks) {
     GP_REQUIRE(p->tasks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
     tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T; tt.rep = 1;
+  } else if (add) {   // the constant initial diagonal sum_m e_m(s), entries from the packed rows
+    tt.ah = additive_hyp(p);
+    os_total = (float)p->add_diag;
   }
   if (deriv) {
     const float c = (float)deriv_with_kind(p->deriv->kind, [](auto K) { return decltype(K)::DIAG; });
@@ -898,10 +907,12 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_REQUIRE(!ski || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a SKI operator needs the cooperative kernel");
   GP_REQUIRE(!tasks || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a multitask operator needs the cooperative kernel");
   GP_REQUIRE(!deriv || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a derivative operator needs the cooperative kernel");
+  GP_REQUIRE(!add || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of an additive operator needs the cooperative kernel");
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : tasks ? PC_KIND_TASK : p->kind) {
+    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : p->kind) {
+      case PC_KIND_ADDITIVE: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_ADDITIVE>; break;
       case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
       case PC_KIND_DERIV: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_DERIV>; break;
       case PC_KIND_M52GRAD: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_M52GRAD>; break;
@@ -1091,6 +1102,8 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
     double bt = 0.0;
     for (int a = 0; a < ts->T; ++a) bt += (double)(ts->off1[a + 1] - ts->off1[a]) * (double)ts->B[(size_t)a * ts->T + a];
     tr_k = (double)p->outputscale * bt;
+  } else if (p->add_M) {   // N sum_m e_m(s)
+    tr_k = (double)n * p->add_diag;
   }
   if (trace_resid_out) *trace_resid_out = tr_k - lsq;
   GP_CUDA(cudaStreamSynchronize(st));

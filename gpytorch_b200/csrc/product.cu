@@ -444,6 +444,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   GP_REFUSE_KRON(p, "gp_plan_set_product");
   GP_REFUSE_DERIV(p, "gp_plan_set_product");
   GP_REFUSE_LOWRANK(p, "gp_plan_set_product");
+  GP_REFUSE_ADDITIVE(p, "gp_plan_set_product");
   GP_CUDA(cudaSetDevice(p->device));
   if (factors == nullptr || n_factors == 0) {   // back to a plain plan
     if (p->backend_req != GP_BACKEND_PRODUCT) return GP_OK;
@@ -457,6 +458,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   for (int f = 0; f < n_factors; ++f) {
     GP_REQUIRE(factors[f] != nullptr && factors[f] != p, GP_E_STATE, "kernel product: factor %d is null or the product itself", f);
     GP_REQUIRE(factors[f]->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "kernel product: a factor that is itself a kernel product is not available");
+    GP_REQUIRE(factors[f]->add_M == 0, GP_E_STATE, "gp_plan_set_product: an additive plan as a factor is not available (gp_plan_set_additive)");
   }
   p->factors.assign(factors, factors + n_factors);
   p->backend_req = GP_BACKEND_PRODUCT;

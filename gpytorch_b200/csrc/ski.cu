@@ -1351,6 +1351,7 @@ extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* g
   GP_REFUSE_KRON(p, "gp_plan_set_ski");
   GP_REFUSE_DERIV(p, "gp_plan_set_ski");
   GP_REFUSE_PRODUCT(p, "gp_plan_set_ski");
+  GP_REFUSE_ADDITIVE(p, "gp_plan_set_ski");
   GP_REQUIRE(d == p->d && d >= 1 && d <= SKI_MAXD, GP_E_SHAPE, "SKI: grid dimension %d does not match the data (d=%d, max %d)", d, p->d, SKI_MAXD);
   int64_t M = 1;
   bool large = false;

@@ -60,7 +60,7 @@ int slot_scales_prepare(gp_plan* p) {
     GP_REQUIRE((int)sc.size() == p->nparts, GP_E_STATE, "kernel sum: a term changed its geometry (%d slots, expected %d); call gp_plan_set_sum again",
                (int)sc.size(), p->nparts);
   } else {
-    sc.assign(p->nparts, p->outputscale);
+    sc.assign(p->nparts, kernel_scale(p));
   }
   if (p->lr_U) sc.push_back(1.f);
   if (sizeof(float) * sc.size() > p->part_scale.cap) {
@@ -123,9 +123,13 @@ extern "C" int gp_plan_set_sum(gp_plan* p, gp_plan* const* terms, int n_terms) {
   GP_REFUSE_KRON(p, "gp_plan_set_sum");
   GP_REFUSE_DERIV(p, "gp_plan_set_sum");
   GP_REFUSE_PRODUCT(p, "gp_plan_set_sum");
+  GP_REFUSE_ADDITIVE(p, "gp_plan_set_sum");
   for (int t = 0; t < n_terms; ++t)
     GP_REQUIRE(terms[t] == nullptr || terms[t]->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE,
                "gp_plan_set_sum: a kernel product as a term is not available (gp_plan_set_product)");
+  for (int t = 0; t < n_terms; ++t)
+    GP_REQUIRE(terms[t] == nullptr || terms[t]->add_M == 0, GP_E_STATE,
+               "gp_plan_set_sum: an additive plan as a term is not available (gp_plan_set_additive)");
   GP_CUDA(cudaSetDevice(p->device));
   p->terms.assign(terms, terms + n_terms);
   p->backend_req = GP_BACKEND_SUM;

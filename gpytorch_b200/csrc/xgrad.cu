@@ -211,6 +211,7 @@ static int xgrad_check(gp_plan* p, const char* what, float* DX1, int64_t ld1, fl
   GP_REFUSE_KRON(p, what);
   GP_REFUSE_DERIV(p, what);
   GP_REFUSE_PRODUCT(p, what);
+  GP_REFUSE_ADDITIVE(p, what);
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "%s of a kernel sum: call it on every term", what);
   GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "%s is not available on a SKI plan", what);
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,

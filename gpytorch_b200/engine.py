@@ -201,6 +201,23 @@ class Plan:
             check(self.lib.gp_plan_set_product(self._h, arr, len(factors)))
         return self
 
+    def set_additive(self, max_degree: int | None, comp_scale=None):
+        """Additive GP: this plan's operator becomes sum_{m=1}^{M} e_m(c_1 .. c_D), c_i = comp_scale[i] k(x_i, x'_i) over the D = d
+        columns (e_m the elementary symmetric polynomials, M = min(max_degree, D)).  set_hypers gives D lengthscales; its
+        outputscale is ignored.  max_degree None (or comp_scale None) clears it.  bilinear_grad then returns the D lengthscale
+        gradients and the list of D component-scale gradients."""
+        if max_degree is None or comp_scale is None:
+            self._additive = None
+            with torch.cuda.device(self.device):
+                check(self.lib.gp_plan_set_additive(self._h, 0, None, 0))
+            return self
+        sc = [float(v) for v in comp_scale]
+        arr = (C.c_float * len(sc))(*sc)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_additive(self._h, int(max_degree), arr, len(sc)))
+        self._additive = (int(max_degree), sc)
+        return self
+
     def set_noise_diag(self, diag: torch.Tensor | None):
         """Per-row noise variances (FixedNoiseGaussianLikelihood): K_hat = K + diag(d).  None restores the scalar noise."""
         if diag is None:
@@ -327,7 +344,8 @@ class Plan:
 
     def bilinear_grad(self, left: torch.Tensor, right: torch.Tensor):
         """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right)) for left [row_count, s], right [n2, s].  On a kernel
-        product: the factors' lengthscale gradients one after the other, and the gradient of the combined scale S."""
+        product: the factors' lengthscale gradients one after the other, and the gradient of the combined scale S.  On an additive
+        plan: the D lengthscale gradients and the list of the D component-scale gradients."""
         if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.row_count or right.size(0) != self.n2 \
                 or left.size(1) != right.size(1) or left.size(1) < 1:
             raise RuntimeError(f"bilinear_grad: left must be [{self.row_count}, s] and right [{self.n2}, s] with s >= 1 "
@@ -342,6 +360,11 @@ class Plan:
         factors = getattr(self, "_factors", None)
         nls = sum(len(f.lengthscale) for f in factors) if factors else len(self.lengthscale)
         gl = (C.c_double * nls)()
+        if getattr(self, "_additive", None) is not None:   # D component-scale gradients
+            go = (C.c_double * len(self._additive[1]))()
+            with torch.cuda.device(self.device):
+                check(self.lib.gp_bilinear_grad(self._h, _ptr(left), _ld(left), _ptr(right), _ld(right), s, gl, go))
+            return [gl[i] for i in range(nls)], list(go)
         go = C.c_double()
         with torch.cuda.device(self.device):
             check(self.lib.gp_bilinear_grad(self._h, _ptr(left), _ld(left), _ptr(right), _ld(right), s, gl, C.byref(go)))

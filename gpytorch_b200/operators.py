@@ -14,6 +14,7 @@ All arithmetic runs in libgpbbmm (CUDA); torch supplies memory, streams and the 
 """
 from __future__ import annotations
 
+import collections
 import weakref
 
 import torch
@@ -91,6 +92,7 @@ def clear_plan_cache():
             _DERIV_PLANS.popitem()[1].close()
         while _PLAN_CACHE:
             _PLAN_CACHE.popitem()[1].close()
+        _ADDITIVE_X.clear()
 
 
 class ConstantDiagLinearOperator:
@@ -429,6 +431,8 @@ class KernelLinearOperator(_SamplingMixin):
     def __add__(self, other):
         if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
             return AddedDiagLinearOperator(self, other)
+        if isinstance(other, AdditiveKernelLinearOperator):
+            raise NotImplementedError("sums that contain additive operators are not available on the accelerated path")
         if isinstance(other, KernelLinearOperator) and not isinstance(other, (SKIKernelLinearOperator, ProductKernelLinearOperator)) \
                 and not isinstance(self, SKIKernelLinearOperator):
             return SumKernelLinearOperator([self, other])     # K_1 + K_2 stays lazy: one engine operator (csrc/sum.cu)
@@ -874,6 +878,9 @@ class SumKernelLinearOperator(KernelLinearOperator):
             flat.extend(o.ops if isinstance(o, SumKernelLinearOperator) else [o])
         if not 1 <= len(flat) <= 4:
             raise RuntimeError(f"a kernel sum takes 1 to 4 terms (got {len(flat)})")
+        if any(isinstance(o, AdditiveKernelLinearOperator) for o in flat):
+            # a term is re-wrapped from its inputs, kind and (single) hyper-parameters below, which an additive operator does not have
+            raise NotImplementedError("sums that contain additive operators are not available on the accelerated path")
         first = flat[0]
         for o in flat[1:]:
             if o.shape != first.shape or o.same != first.same:
@@ -1116,6 +1123,193 @@ class ProductKernelLinearOperator(KernelLinearOperator):
 
 
 _PRODUCT_PLANS: "dict[tuple, Plan]" = {}
+
+
+ADDITIVE_MAX_COMPONENTS = 32
+ADDITIVE_MAX_DEGREE = 8
+_ADDITIVE_SLOT = 16        # plan-cache slot of additive operators (sum terms 1..4, product factors 5..8, low-rank 8)
+_ADDITIVE_KINDS = ("rbf", "matern12", "matern32", "matern52")
+_ADDITIVE_X: "collections.OrderedDict[tuple, list]" = collections.OrderedDict()
+_ADDITIVE_X_ROLES = 8      # stacked inputs kept: the most recently used roles (shape, side, device), two buffers each
+
+
+def _stable_stack(cols, role):
+    """torch.cat(cols, -1), or the tensor an earlier operator stacked from the same values: the kernels of an additive model are
+    called on fresh [n, 1] slices every forward, and the engine plan is keyed on its input buffer, so equal inputs keep one buffer
+    and their plan is neither re-pointed nor re-packed."""
+    x = torch.cat([c.detach() for c in cols], -1)
+    with _PLAN_LOCK:
+        seen = _ADDITIVE_X.pop(role, [])
+        _ADDITIVE_X[role] = seen   # most recently used last
+        found = next((old for old in seen if torch.equal(old, x)), None)   # one device comparison per kept buffer of this role
+        if found is None:
+            seen.append(x)
+            del seen[:-2]
+        while len(_ADDITIVE_X) > _ADDITIVE_X_ROLES:
+            _ADDITIVE_X.popitem(last=False)
+    return x if found is None else found
+
+
+def _additive_components(ops, what):
+    """The D one-dimensional RBF / Matern operators of an additive model, checked; raises NotImplementedError naming what it refuses."""
+    ops = list(ops)
+    if not 1 <= len(ops) <= ADDITIVE_MAX_COMPONENTS:
+        raise NotImplementedError(f"{what}: an additive operator takes 1 to {ADDITIVE_MAX_COMPONENTS} components on the accelerated "
+                                  f"path (got {len(ops)})")
+    first = ops[0]
+    for o in ops:
+        if type(o) is not KernelLinearOperator:
+            raise NotImplementedError(f"{what}: every component must be a plain RBF / Matern kernel operator (optionally scaled) on "
+                                      f"the accelerated path, not {type(o).__name__}")
+        if o.kind not in _ADDITIVE_KINDS or o.kind != first.kind:
+            raise NotImplementedError(f"{what}: the components must share one RBF / Matern kind (got {o.kind!r} and {first.kind!r})")
+        if o.x1.dim() != 2 or o.x1.size(-1) != 1:
+            raise NotImplementedError(f"{what}: every component must act on one input dimension ([n, 1] inputs), got "
+                                      f"{tuple(o.x1.shape)}")
+        if o.lengthscale.numel() != 1 or o.outputscale.numel() != 1:
+            raise NotImplementedError(f"{what}: every component needs one lengthscale and one outputscale")
+        if o.shape != first.shape or o.same != first.same:
+            raise RuntimeError(f"{what}: component shapes {tuple(first.shape)} and {tuple(o.shape)} differ")
+        if o._comm is not None or o._row_begin != 0 or o._row_count not in (0, o.shape[0]):
+            raise NotImplementedError(f"{what}: a row-sharded additive operator is not available on the accelerated path")
+        if o.x1.requires_grad or (not o.same and o.x2.requires_grad):
+            raise NotImplementedError(f"{what}: gradients with respect to the inputs of an additive operator (deep kernel learning, "
+                                      "test-input gradients) are not available on the accelerated path")
+    return ops
+
+
+class AdditiveKernelLinearOperator(KernelLinearOperator):
+    """sum_{m=1}^{M} e_m(K_1, .., K_D) over D one-dimensional kernel operators K_i = s_i k_i(x_i, x'_i), e_m the elementary symmetric
+    polynomial of degree m taken entry by entry (Duvenaud et al.'s additive GPs): M = 1 is `.sum(dim=-3)` of the batch of
+    components, M >= 2 `sum_interaction_terms(..., max_degree=M)`.  The reference evaluates the D components densely and combines
+    them by Newton-Girard; here the operator is ONE engine plan (gp_plan_set_additive) whose kernels form the positive recurrence
+    e_m += c_i e_{m-1} per pair, so products, solves, the preconditioner and SLQ never hold an N x N matrix.  The components' [n, 1]
+    inputs are stacked into one [n, D] block; a component's lengthscale and scale stay its own tensors (hyper_tensors), so autograd
+    reaches batched [D, 1, 1] / [D] parameters and sums the gradients of a shared one.  1 <= D <= 32, M <= 8 after clamping to D;
+    gradients with respect to the inputs are not available."""
+
+    def __init__(self, ops, max_degree=1):
+        self.ops = _additive_components(ops, "AdditiveKernelLinearOperator")
+        D = len(self.ops)
+        if int(max_degree) < 1:
+            raise ValueError(f"max_degree must be >= 1 (got {max_degree})")
+        self.max_degree = min(int(max_degree), D)     # e_m = 0 for m > D
+        if self.max_degree > ADDITIVE_MAX_DEGREE:
+            raise NotImplementedError(f"an additive operator takes interaction terms up to degree {ADDITIVE_MAX_DEGREE} on the "
+                                      f"accelerated path (got max_degree={max_degree} with {D} components)")
+        first = self.ops[0]
+        self.same = first.same
+        n1 = first.shape[0]
+        self.x1 = _stable_stack([o.x1 for o in self.ops], ("x1", n1, D, str(first.x1.device)))
+        self.x2 = self.x1 if self.same else _stable_stack([o.x2 for o in self.ops], ("x2", first.shape[1], D, str(first.x1.device)))
+        self.kind = first.kind
+        self.lengthscale, self.outputscale = first.lengthscale, first.outputscale   # representative only (device / dtype)
+        self._comm, self._row_begin, self._row_count = None, 0, 0
+        self._plan = None
+
+    def hyper_tensors(self):
+        return [t for o in self.ops for t in o.hyper_tensors()]
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    def _host_hypers(self, noise_t=None):
+        """([l_1 .. l_D], [s_1 .. s_D], noise) with one device -> host read."""
+        cached = getattr(self, "_hyp_host", None)
+        if cached is None or (noise_t is not None and cached[3] is not noise_t):
+            parts = [o.lengthscale.detach().reshape(1).float() for o in self.ops]
+            parts += [o.outputscale.detach().reshape(1).float().to(o.lengthscale.device) for o in self.ops]
+            if noise_t is not None:
+                parts.append(noise_t.detach().reshape(-1)[:1].float())
+            vals = torch.cat(parts).tolist()
+            D = len(self.ops)
+            cached = (vals[:D], vals[D:2 * D], vals[2 * D] if noise_t is not None else None, noise_t)
+            self._hyp_host = cached
+        return cached
+
+    def plan(self, noise=0.0) -> Plan:
+        fresh = False
+        if self._plan is None:
+            self._plan = _get_plan(self.x1, None if self.same else self.x2, "auto", 0, 0, None,
+                                   getattr(self, "_plan_slot", _ADDITIVE_SLOT), owner=self)
+            fresh = True
+        if torch.is_tensor(noise):
+            ls, sc, nz, _ = self._host_hypers(noise)
+        else:
+            ls, sc, _, _ = self._host_hypers(None)
+            nz = float(noise)
+        p = self._plan
+        akey = (self.max_degree, tuple(sc))
+        if fresh or getattr(p, "_add_key", None) != akey:
+            p.set_additive(self.max_degree, sc)
+            p._add_key = akey
+        key = (self.kind, tuple(ls), 1.0, nz)
+        if fresh or getattr(p, "_hyp_key", None) != key:
+            p.set_hypers(self.kind, ls, 1.0, nz)
+            p._hyp_key = key
+        return p
+
+    def _bilinear_derivative_list(self, left, right):
+        gl, gs = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
+        vals = torch.tensor(list(gl) + list(gs), device=self.device, dtype=self.dtype)
+        D = len(self.ops)
+        out = []
+        for i, o in enumerate(self.ops):
+            out.append(vals[i].reshape(o.lengthscale.shape))
+            out.append(vals[D + i].reshape(o.outputscale.shape))
+        return out
+
+    def _bilinear_derivative(self, left, right):
+        raise NotImplementedError("an additive operator has one (lengthscale, scale) pair per component: use _bilinear_derivative_list")
+
+    def _input_grad_list(self, left, right, needs):
+        raise NotImplementedError("gradients with respect to the inputs of an additive operator are not available on the accelerated path")
+
+    _dense_input_grad_list = _input_grad_list
+
+    @property
+    def requires_grad(self):
+        return any(o.requires_grad for o in self.ops)
+
+    def representation(self):
+        return tuple(t for o in self.ops for t in o.representation())
+
+    def _transpose_nonbatch(self):
+        return self if self.same else AdditiveKernelLinearOperator([o._transpose_nonbatch() for o in self.ops], self.max_degree)
+
+    def detach(self):
+        return AdditiveKernelLinearOperator([o.detach() for o in self.ops], self.max_degree)
+
+    def diagonal(self, dim1=-2, dim2=-1):
+        """The constant sum_m e_m(s_1 .. s_D) for x2 == x1, K(x1_i, x2_i) for a cross operator of equal sizes."""
+        if not self.same and self.ops[0].x1.size(0) != self.ops[0].x2.size(0):
+            raise RuntimeError(f"diagonal of a non-square operator {tuple(self.shape)} is undefined")
+        return self.plan().diag()
+
+    _diagonal = diagonal
+
+    def __getitem__(self, index):
+        """Row / column blocks (the train / test blocks of prediction) re-index every component: a cross plan for x1 != x2."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        return AdditiveKernelLinearOperator([o[ri, ci] for o in self.ops], self.max_degree)
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("an additive operator adds a (Constant)DiagLinearOperator only: sums that contain additive "
+                                  "operators are not available on the accelerated path")
+
+    def mul(self, other):
+        raise NotImplementedError("products that contain an additive operator are not available on the accelerated path")
+
+    __mul__ = mul
 
 
 class SKIKernelLinearOperator(KernelLinearOperator):
@@ -1854,6 +2048,14 @@ class BatchLinearOperator:
 
     def to_dense(self):
         return torch.stack([op.to_dense() for op in self.ops])
+
+    def sum(self, dim=-3):
+        """sum_b K_b over the batch dimension as ONE engine operator: the additive GP of D one-dimensional RBF / Matern components
+        (AdditiveKernelLinearOperator with max_degree 1).  Only the batch dimension (-3 or 0) is summed."""
+        if dim not in (-3, 0):
+            raise NotImplementedError(f"BatchLinearOperator.sum(dim={dim}): only the batch dimension (-3 or 0) is summed on the "
+                                      "accelerated path")
+        return AdditiveKernelLinearOperator(_additive_components(self.ops, "BatchLinearOperator.sum"), 1)
 
     def solve(self, rhs, lhs=None):
         return torch.stack(self._map(lambda b, op: op.solve(rhs[b] if rhs.dim() >= 2 and rhs.size(0) == len(self.ops) else rhs)))

@@ -144,6 +144,26 @@ int gp_plan_set_sum(gp_plan* plan, gp_plan* const* terms, int n_terms);
  * calls return GP_E_STATE. */
 int gp_plan_set_product(gp_plan* plan, gp_plan* const* factors, int n_factors);
 
+/* Additive GPs (the reference's ScaleKernel(RBFKernel(batch_shape=[D], ard_num_dims=1)) over X.mT.unsqueeze(-1), then .sum(dim=-3)
+ * or utils/sum_interaction_terms.py, both dense): `plan` becomes the operator
+ *   K(x, x') = sum_{m=1}^{M} e_m(c_1, .., c_D),   c_i = comp_scale[i] k(x_i, x'_i)   (+ its noise / per-row diagonal where a call adds it)
+ * with e_m the elementary symmetric polynomial of degree m and k the plan's kind (RBF or Matern) over column i alone, with
+ * lengthscale l_i.  M = min(max_degree, D): M = 1 is the sum of the components, M >= 2 adds every interaction term up to degree M.
+ * The plan is a plain plan whose data has d = n_comp = D columns (1 <= D <= 32) and whose gp_plan_set_hypers gives D lengthscales
+ * (before or after this call); its outputscale is ignored, its noise kept.  max_degree in [1, 8]; comp_scale: host [D], > 0.
+ * comp_scale = NULL or n_comp = 0 clears the setting.  Square and cross plans; the plan runs its own CUDA-core kernels, which form e
+ * per pair in registers by the positive recurrence e_m += c_i e_{m-1} (no cancellation).
+ * gp_kmv, gp_krows, gp_kdiag (square: the constant sum_m e_m(comp_scale); cross: per pair), gp_pivoted_cholesky, gp_precond_build,
+ * gp_precond_probes, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build,
+ * gp_ciq_sqrt_matmul_precond, gp_plan_set_noise_diag, gp_plan_set_lowrank and gp_time_kmv_kernel run on it.  gp_bilinear_grad returns
+ * the D lengthscale gradients dF/dl_i in grad_ls and the D component-scale gradients dF/ds_i in grad_os, which must hold D doubles.
+ * A non-finite input makes products, rows, the diagonal and gradients NaN.  On an additive plan gp_plan_set_tasks, gp_plan_set_kron,
+ * gp_plan_set_deriv, gp_plan_set_deriv_kind, gp_plan_set_sum, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_backend,
+ * gp_plan_set_comm with more than one rank, gp_kmv_input_grad and gp_kdense_input_grad return GP_E_STATE with a message naming the
+ * call; an additive plan as a term of gp_plan_set_sum, a factor of gp_plan_set_product or the data plan of gp_plan_set_kron /
+ * gp_plan_set_deriv is refused the same way.  A SKI, sum, product, multitask, derivative or row-sharded plan cannot become additive. */
+int gp_plan_set_additive(gp_plan* plan, int max_degree, const float* comp_scale, int n_comp);
+
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
  * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
  * (+ its noise / per-row diagonal where a call adds it).  U: device [n, r] fp32, leading dimension ldu, caller-owned, must outlive
