@@ -129,6 +129,7 @@ extern "C" int gp_plan_set_backend(gp_plan* p, int backend) {
   GP_REFUSE_DERIV(p, "gp_plan_set_backend");
   GP_REFUSE_PRODUCT(p, "gp_plan_set_backend");
   GP_REFUSE_ADDITIVE(p, "gp_plan_set_backend");
+  GP_REFUSE_SPECTRAL(p, "gp_plan_set_backend");
   p->backend_req = backend;
   if (p->data_set && p->hypers_set) return pack_inputs(p);
   return GP_OK;
@@ -216,6 +217,8 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
              "gp_plan_set_comm with more than one rank is not available on a kernel-product plan (gp_plan_set_product)");
   GP_REQUIRE(!(p->add_M && comm && comm->world > 1), GP_E_STATE,
              "gp_plan_set_comm with more than one rank is not available on an additive plan (gp_plan_set_additive)");
+  GP_REQUIRE(!(p->sm_Q && comm && comm->world > 1), GP_E_STATE,
+             "gp_plan_set_comm with more than one rank is not available on a spectral mixture plan (gp_plan_set_spectral)");
   p->comm = comm;
   return GP_OK;
 }
@@ -251,6 +254,7 @@ extern "C" int gp_time_kmv_kernel(gp_plan* p, const float* V, int64_t ldv, int t
     if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_PRODUCT) return product_kmv_launch(p, p->V16.as<float>(), nullptr);
     if (p->add_M) return additive_kmv_launch(p, p->V16.as<float>(), nullptr);
+    if (p->sm_Q) return spectral_kmv_launch(p, p->V16.as<float>(), nullptr);
     return p->backend == GP_BACKEND_TCGEN05 ? kmv_tc_launch(p, nullptr) : kmv_simt_launch(p, p->V16.as<float>(), nullptr);
   };
   for (int i = 0; i < warmup; ++i) GP_CHECK(launch());

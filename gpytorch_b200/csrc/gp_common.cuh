@@ -276,6 +276,11 @@ struct gp_plan {
   int add_M = 0;
   std::vector<float> add_s;       // the D component scales
   double add_diag = 0.0;          // sum_{m=1}^{M} e_m(s_1 .. s_D): the constant diagonal of a square operator
+  // spectral mixture kernels (spectral.cu): S prod_d sum_q w_q exp(-2 pi^2 v_qd^2 tau_d^2) cos(2 pi mu_qd tau_d) on a plain SIMT
+  // plan whose Z1 / Z2 hold the packed rows [x | reduced phases] of DP = pad4(d + Q d) floats; sm_Q = 0 is a plain plan
+  int sm_Q = 0;
+  std::vector<float> sm_w, sm_mu, sm_v;   // weights [Q], means and scales [Q][d]
+  double sm_diag = 0.0;           // S (sum_q w_q)^d: the constant diagonal of a square operator
   int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
@@ -386,6 +391,14 @@ int additive_kdiag(gp_plan* p, float* OUT);
 int additive_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
 #define GP_REFUSE_ADDITIVE(p, what) \
   GP_REQUIRE((p)->add_M == 0, GP_E_STATE, "%s is not available on an additive plan (gp_plan_set_additive)", what)
+// spectral.cu
+int spectral_pack(gp_plan* p);                                          // packs [x | reduced phases] into Z1 / Z2, forms sm_diag
+int spectral_kmv_launch(gp_plan* p, const float* V16, const int* done_flag);
+int spectral_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
+int spectral_kdiag(gp_plan* p, float* OUT);
+int spectral_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+#define GP_REFUSE_SPECTRAL(p, what) \
+  GP_REQUIRE((p)->sm_Q == 0, GP_E_STATE, "%s is not available on a spectral mixture plan (gp_plan_set_spectral)", what)
 inline bool plan_is_tc(const gp_plan* p) {
   return p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_tc) || (p->backend == GP_BACKEND_PRODUCT && p->prod_tc);
 }
@@ -536,6 +549,34 @@ __device__ __forceinline__ float add_pair_rt(const AddHyp& h, const float* za, c
   return h.rbf ? add_pair<true>(h, za, zb) : add_pair<false>(h, za, zb);
 }
 AddHyp additive_hyp(const gp_plan* p);   // additive.cu: the kernel argument of an additive plan
+// Spectral mixture kernels (spectral.cu): the weights and the exponent coefficients beta_qc = -2 pi^2 v_qc^2 log2 e are uniform
+// across threads and travel in the kernel argument; a packed row is [x_0 .. x_{d-1} | p_qc at d + q d + c] (reduced phases).
+constexpr int SM_QMAX = 16;    // components
+constexpr int SM_DMAX = 8;     // input dimensions
+constexpr int SM_QDMAX = 32;   // Q d
+constexpr int SM_WMAX = 40;    // packed row width: pad4(d + Q d) <= 40
+struct SmHyp {
+  float w[SM_QMAX];
+  float beta[SM_QDMAX];
+  int Q, d;
+  float S;             // outputscale: rows, diagonals and pivoted-Cholesky entries (the K.V finish kernels apply it there)
+};
+// one entry S prod_c sum_q w_q 2^{beta_qc tau_c^2} cos(2 pi (p_qc - p'_qc)) from two packed rows (rows, diagonal, pivoted Cholesky)
+__device__ __forceinline__ float sm_pair(const SmHyp& h, const float* za, const float* zb) {
+  float k = h.S;
+  for (int c = 0; c < h.d; ++c) {
+    const float t = za[c] - zb[c];
+    const float t2 = t * t;
+    float s = 0.f;
+    for (int q = 0; q < h.Q; ++q) {
+      const int o = q * h.d + c;
+      s = fmaf(h.w[q], ex2_approx(h.beta[o] * t2) * __cosf(6.2831853071795865f * (za[h.d + o] - zb[h.d + o])), s);
+    }
+    k *= s;
+  }
+  return k;
+}
+SmHyp spectral_hyp(const gp_plan* p);   // spectral.cu: the kernel argument of a spectral plan
 // input-derivative factor q = dk/da of the same covariance (xgrad.cu): dk/dz_i = -q (z_i - z_j) in the packed units.
 //   RBF: ln2 2^a ; M12: e / (2 rho) ; M32: e / 2 ; M52: (1 + rho) e / 6      (e = exp(-rho), rho^2 = -a)
 // q is the h of the raw-unit form  dk/dx_i = -h (x_i - x_j) / l^2  times l^2 / C (C = log2 e, 2, 6, 10 as in pack.cu).  A pair at

@@ -142,6 +142,7 @@ static int kmv_partials_base(gp_plan* p, const float* V16, const int* done_flag)
     return kmv_tc_launch(p, done_flag);
   }
   if (p->add_M) return additive_kmv_launch(p, V16, done_flag);
+  if (p->sm_Q) return spectral_kmv_launch(p, V16, done_flag);
   return kmv_simt_launch(p, V16, done_flag);
 }
 
@@ -440,6 +441,7 @@ extern "C" int gp_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, i
 static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   if (p->backend == GP_BACKEND_SKI) return ski_krows(p, idx, m, OUT, ldo);   // separable entries (ski_rows.cuh)
   if (p->add_M) return additive_krows(p, idx, m, OUT, ldo);
+  if (p->sm_Q) return spectral_krows(p, idx, m, OUT, ldo);
   const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
   dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
   size_t sh = sizeof(float) * p->DP;
@@ -484,6 +486,7 @@ extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
 static int kdiag_base(gp_plan* p, float* OUT) {
   if (p->backend == GP_BACKEND_SKI) return ski_kdiag(p, OUT);   // not constant: w_i^T K_uu w_i (ski_rows.cuh)
   if (p->add_M) return additive_kdiag(p, OUT);   // square: the constant sum_m e_m(s); cross: per pair
+  if (p->sm_Q) return spectral_kdiag(p, OUT);    // square: the constant S (sum_q w_q)^d; cross: per pair
   if (p->same) {
     // stationary kernels: k(x,x) = outputscale (lazy_evaluated_kernel_tensor.py:107-133 evaluates kernel(diag=True))
     fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, p->outputscale);
@@ -519,6 +522,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   if (p->kron) return kron_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->deriv) return deriv_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->add_M) return additive_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
+  if (p->sm_Q) return spectral_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   // before any launch: the SIMT derivative kernel is instantiated up to DP = 64
   GP_REQUIRE(p->backend == GP_BACKEND_SKI || p->DP <= 64, GP_E_SHAPE, "bilinear gradient supports d <= 64 (d=%d)", p->d);
   const bool ard = p->ls.size() > 1;

@@ -149,6 +149,7 @@ int choose_geometry(gp_plan* p) {
   int want = p->backend_req;
   if (want == GP_BACKEND_AUTO) want = (p->KP <= KP_MAX) ? GP_BACKEND_TCGEN05 : GP_BACKEND_SIMT;
   if (p->add_M) want = GP_BACKEND_SIMT;   // additive plans run their own CUDA-core kernels on Z (additive.cu)
+  if (p->sm_Q) want = GP_BACKEND_SIMT;    // so do spectral plans, on their own packed rows (spectral.cu)
   GP_REQUIRE(!(want == GP_BACKEND_TCGEN05 && p->KP > KP_MAX), GP_E_SHAPE,
              "tcgen05 (tensor-core) backend needs 3d+4 <= %d (d=%d)", KP_MAX, p->d);
   p->backend = want;
@@ -191,6 +192,7 @@ int pack_inputs(gp_plan* p) {
   if (p->backend_req == GP_BACKEND_PRODUCT) return product_pack(p);
   p->pack_gen++;   // a kernel product over this plan re-reads its scale, geometry and flag (product.cu)
   GP_CHECK(choose_geometry(p));
+  if (p->sm_Q) return spectral_pack(p);
   cudaStream_t st = p->stream;
   const int d = p->d, DP = p->DP;
   GP_CHECK(p->mean.ensure(sizeof(float) * (d + 4)));

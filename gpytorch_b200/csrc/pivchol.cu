@@ -202,6 +202,8 @@ constexpr int PC_KIND_PRODUCT = 68;
 constexpr int PC_KIND_M52GRAD = 69;
 // additive GPs (additive.cu): K[pivot, j] = sum_{m=1}^{M} e_m(s_i k_i(z_pivot,i - z_j,i)) from the plan's packed rows
 constexpr int PC_KIND_ADDITIVE = 70;
+// spectral mixture kernels (spectral.cu): K[pivot, j] = S prod_d sum_q w_q e_qd cos_qd from the plan's packed rows
+constexpr int PC_KIND_SPECTRAL = 71;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -213,6 +215,7 @@ struct PcTerms {
   int rep;           // PC_KIND_TASK / PC_KIND_DERIV / PC_KIND_M52GRAD: rows per point
   const DerivHyp* dh;   // PC_KIND_DERIV / PC_KIND_M52GRAD
   AddHyp ah;            // PC_KIND_ADDITIVE
+  SmHyp sh;             // PC_KIND_SPECTRAL
 };
 __device__ __forceinline__ int pc_task_of(const PcTerms& tt, int r) { return tt.task ? tt.task[r] : r % tt.rep; }
 __device__ __forceinline__ float pc_cov_rt(int kind, float a) {
@@ -320,6 +323,8 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
           v = ski_entry(sk, zp, pi, j);
         } else if (KIND == PC_KIND_ADDITIVE) {
           v = add_pair_rt(tt.ah, zp, Z + j * DP);
+        } else if (KIND == PC_KIND_SPECTRAL) {
+          v = sm_pair(tt.sh, zp, Z + j * DP);
         } else if (KIND == PC_KIND_TASK) {
           const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
           float s = 0.f;
@@ -830,6 +835,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   const bool sum = p->backend == GP_BACKEND_SUM;
   const bool ski = p->backend == GP_BACKEND_SKI;
   const bool add = p->add_M > 0;
+  const bool spec = p->sm_Q > 0;
   PcTerms tt;
   memset(&tt, 0, sizeof(tt));
   SkiRows sk;
@@ -878,6 +884,9 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   } else if (add) {   // the constant initial diagonal sum_m e_m(s), entries from the packed rows
     tt.ah = additive_hyp(p);
     os_total = (float)p->add_diag;
+  } else if (spec) {   // the constant initial diagonal S (sum_q w_q)^d, entries from the packed rows
+    tt.sh = spectral_hyp(p);
+    os_total = (float)p->sm_diag;
   }
   if (deriv) {
     const float c = (float)deriv_with_kind(p->deriv->kind, [](auto K) { return decltype(K)::DIAG; });
@@ -908,11 +917,13 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_REQUIRE(!tasks || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a multitask operator needs the cooperative kernel");
   GP_REQUIRE(!deriv || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a derivative operator needs the cooperative kernel");
   GP_REQUIRE(!add || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of an additive operator needs the cooperative kernel");
+  GP_REQUIRE(!spec || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a spectral mixture operator needs the cooperative kernel");
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : p->kind) {
+    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : spec ? PC_KIND_SPECTRAL : p->kind) {
       case PC_KIND_ADDITIVE: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_ADDITIVE>; break;
+      case PC_KIND_SPECTRAL: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SPECTRAL>; break;
       case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
       case PC_KIND_DERIV: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_DERIV>; break;
       case PC_KIND_M52GRAD: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_M52GRAD>; break;
@@ -1104,6 +1115,8 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
     tr_k = (double)p->outputscale * bt;
   } else if (p->add_M) {   // N sum_m e_m(s)
     tr_k = (double)n * p->add_diag;
+  } else if (p->sm_Q) {   // N S (sum_q w_q)^d
+    tr_k = (double)n * p->sm_diag;
   }
   if (trace_resid_out) *trace_resid_out = tr_k - lsq;
   GP_CUDA(cudaStreamSynchronize(st));

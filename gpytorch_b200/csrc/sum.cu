@@ -124,12 +124,16 @@ extern "C" int gp_plan_set_sum(gp_plan* p, gp_plan* const* terms, int n_terms) {
   GP_REFUSE_DERIV(p, "gp_plan_set_sum");
   GP_REFUSE_PRODUCT(p, "gp_plan_set_sum");
   GP_REFUSE_ADDITIVE(p, "gp_plan_set_sum");
+  GP_REFUSE_SPECTRAL(p, "gp_plan_set_sum");
   for (int t = 0; t < n_terms; ++t)
     GP_REQUIRE(terms[t] == nullptr || terms[t]->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE,
                "gp_plan_set_sum: a kernel product as a term is not available (gp_plan_set_product)");
   for (int t = 0; t < n_terms; ++t)
     GP_REQUIRE(terms[t] == nullptr || terms[t]->add_M == 0, GP_E_STATE,
                "gp_plan_set_sum: an additive plan as a term is not available (gp_plan_set_additive)");
+  for (int t = 0; t < n_terms; ++t)
+    GP_REQUIRE(terms[t] == nullptr || terms[t]->sm_Q == 0, GP_E_STATE,
+               "gp_plan_set_sum: a spectral mixture plan as a term is not available (gp_plan_set_spectral)");
   GP_CUDA(cudaSetDevice(p->device));
   p->terms.assign(terms, terms + n_terms);
   p->backend_req = GP_BACKEND_SUM;

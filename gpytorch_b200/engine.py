@@ -218,6 +218,26 @@ class Plan:
         self._additive = (int(max_degree), sc)
         return self
 
+    def set_spectral(self, weights=None, means=None, scales=None):
+        """Spectral mixture kernel: this plan's operator becomes S prod_d sum_q w_q exp(-2 pi^2 v_qd^2 tau_d^2) cos(2 pi mu_qd tau_d)
+        over tau = x - x' (S the outputscale of set_hypers, whose kind and lengthscale are ignored).  weights [Q], means and scales
+        [Q, d] (host sequences or tensors); weights None clears it.  bilinear_grad then returns the Q (1 + 2d) gradients
+        [dw | dmu (row-major) | dv (row-major)] and dF/dS."""
+        if weights is None:
+            self._spectral = None
+            with torch.cuda.device(self.device):
+                check(self.lib.gp_plan_set_spectral(self._h, 0, None, None, None, 0))
+            return self
+        w = [float(v) for v in (weights.reshape(-1).tolist() if torch.is_tensor(weights) else weights)]
+        mu = torch.as_tensor(means, dtype=torch.float64).reshape(len(w), -1)
+        sc = torch.as_tensor(scales, dtype=torch.float64).reshape(len(w), -1)
+        Q, d = mu.shape
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_spectral(self._h, Q, (C.c_float * Q)(*w), (C.c_float * (Q * d))(*mu.reshape(-1).tolist()),
+                                                (C.c_float * (Q * d))(*sc.reshape(-1).tolist()), d))
+        self._spectral = (Q, d)
+        return self
+
     def set_noise_diag(self, diag: torch.Tensor | None):
         """Per-row noise variances (FixedNoiseGaussianLikelihood): K_hat = K + diag(d).  None restores the scalar noise."""
         if diag is None:
@@ -345,7 +365,8 @@ class Plan:
     def bilinear_grad(self, left: torch.Tensor, right: torch.Tensor):
         """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right)) for left [row_count, s], right [n2, s].  On a kernel
         product: the factors' lengthscale gradients one after the other, and the gradient of the combined scale S.  On an additive
-        plan: the D lengthscale gradients and the list of the D component-scale gradients."""
+        plan: the D lengthscale gradients and the list of the D component-scale gradients.  On a spectral plan: the Q (1 + 2d)
+        gradients [dw | dmu | dv] and dF/dS."""
         if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.row_count or right.size(0) != self.n2 \
                 or left.size(1) != right.size(1) or left.size(1) < 1:
             raise RuntimeError(f"bilinear_grad: left must be [{self.row_count}, s] and right [{self.n2}, s] with s >= 1 "
@@ -360,6 +381,10 @@ class Plan:
         factors = getattr(self, "_factors", None)
         nls = sum(len(f.lengthscale) for f in factors) if factors else len(self.lengthscale)
         gl = (C.c_double * nls)()
+        if getattr(self, "_spectral", None) is not None:   # [dw | dmu | dv] and dF/dS
+            Q, d = self._spectral
+            nls = Q * (1 + 2 * d)
+            gl = (C.c_double * nls)()
         if getattr(self, "_additive", None) is not None:   # D component-scale gradients
             go = (C.c_double * len(self._additive[1]))()
             with torch.cuda.device(self.device):

@@ -1,5 +1,5 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, ScaleKernel, AdditiveKernel, ProductKernel,
-GridInterpolationKernel} for the accelerated path.
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, SpectralMixtureKernel, ScaleKernel,
+AdditiveKernel, ProductKernel, GridInterpolationKernel} for the accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
 rbf_kernel.py:68-85; matern_kernel.py:79-110; scale_kernel.py:64-118), but `forward` returns an
@@ -7,6 +7,8 @@ engine-backed KernelLinearOperator (the KeOps plug-in pattern, kernels/keops/rbf
 instead of a dense tensor: K is never materialised.
 """
 from __future__ import annotations
+
+import logging
 
 import torch
 
@@ -205,6 +207,147 @@ class Matern52KernelGrad(MaternKernel):
         return x1.size(-1) + 1
 
 
+class SpectralMixtureKernel(Kernel):
+    """k(x, x') = prod_d sum_q w_q exp(-2 pi^2 v_qd^2 tau_d^2) cos(2 pi mu_qd tau_d), tau = x - x' (Wilson & Adams 2013;
+    kernels/spectral_mixture_kernel.py, whose forward sums the components of each dimension and multiplies over the dimensions).
+    Parameters as in the reference: raw_mixture_weights [*B, Q], raw_mixture_means / raw_mixture_scales [*B, Q, 1, d], each with a
+    Positive() constraint unless one is given.  forward returns one engine SpectralMixtureKernelLinearOperator (gp_plan_set_spectral);
+    inside a ScaleKernel the outputscale S multiplies it.  1 <= num_mixtures <= 16, 1 <= d <= 8, num_mixtures * d <= 32, one batch
+    dimension at most.  Sums, products, SKI, multitask and derivative kernels do not take it, and the inputs get no gradient."""
+
+    is_stationary = True
+
+    def __init__(self, num_mixtures=None, ard_num_dims=1, batch_shape=None, mixture_scales_prior=None, mixture_scales_constraint=None,
+                 mixture_means_prior=None, mixture_means_constraint=None, mixture_weights_prior=None, mixture_weights_constraint=None,
+                 **kwargs):
+        if num_mixtures is None:
+            raise RuntimeError("num_mixtures is a required argument")
+        if mixture_means_prior is not None or mixture_scales_prior is not None or mixture_weights_prior is not None:
+            logging.getLogger().warning("Priors not implemented for SpectralMixtureKernel")
+        super().__init__(ard_num_dims=ard_num_dims, batch_shape=batch_shape, **kwargs)
+        self.num_mixtures = int(num_mixtures)
+        shape = torch.Size([*self.batch_shape, self.num_mixtures, 1, self.ard_num_dims])
+        self.register_parameter("raw_mixture_weights", torch.nn.Parameter(torch.zeros(*self.batch_shape, self.num_mixtures)))
+        self.register_parameter("raw_mixture_means", torch.nn.Parameter(torch.zeros(shape)))
+        self.register_parameter("raw_mixture_scales", torch.nn.Parameter(torch.zeros(shape)))
+        self.register_constraint("raw_mixture_scales", mixture_scales_constraint or Positive())
+        self.register_constraint("raw_mixture_means", mixture_means_constraint or Positive())
+        self.register_constraint("raw_mixture_weights", mixture_weights_constraint or Positive())
+
+    @property
+    def mixture_scales(self):
+        return self.raw_mixture_scales_constraint.transform(self.raw_mixture_scales)
+
+    @mixture_scales.setter
+    def mixture_scales(self, value):
+        self._set_mixture_scales(value)
+
+    def _set_mixture_scales(self, value):
+        self._set_constrained("raw_mixture_scales", value)
+
+    @property
+    def mixture_means(self):
+        return self.raw_mixture_means_constraint.transform(self.raw_mixture_means)
+
+    @mixture_means.setter
+    def mixture_means(self, value):
+        self._set_mixture_means(value)
+
+    def _set_mixture_means(self, value):
+        self._set_constrained("raw_mixture_means", value)
+
+    @property
+    def mixture_weights(self):
+        return self.raw_mixture_weights_constraint.transform(self.raw_mixture_weights)
+
+    @mixture_weights.setter
+    def mixture_weights(self, value):
+        self._set_mixture_weights(value)
+
+    def _set_mixture_weights(self, value):
+        self._set_constrained("raw_mixture_weights", value)
+
+    def _training_inputs(self, train_x, train_y):
+        if not torch.is_tensor(train_x) or not torch.is_tensor(train_y):
+            raise RuntimeError("train_x and train_y should be tensors")
+        if train_x.dim() == 1:
+            train_x = train_x.unsqueeze(-1)
+        if self.active_dims is not None:
+            train_x = train_x[..., self.active_dims.to(train_x.device)]
+        return train_x
+
+    def initialize_from_data(self, train_x, train_y, **kwargs):
+        """Scales from the data's extent, means from its finest spacing and weights from std(y) (the reference's statistics, with
+        the same torch random draws: one randn_like of the scales, then one rand_like of the means).  For irregular samples."""
+        with torch.no_grad():
+            x = self._training_inputs(train_x, train_y)
+            xs = x.sort(dim=-2)[0]
+            span = xs[..., -1, :] - xs[..., 0, :]                                  # [*, d]
+            gaps = xs[..., 1:, :] - xs[..., :-1, :]
+            gaps = torch.where(gaps == 0, torch.full_like(gaps, 1.0e10), gaps)    # repeated points do not set the finest spacing
+            finest = gaps.min(dim=-2)[0]                                           # [*, d]
+            # one value per parameter slot: reduce the leading data dimensions the parameters do not carry
+            extra = finest.dim() - 1 - len(self.batch_shape)
+            for _ in range(max(extra, 0)):
+                finest, span = finest.min(dim=0)[0], span.max(dim=0)[0]
+            finest = finest.unsqueeze(-2).unsqueeze(-3)                            # [*B, 1, 1, d]
+            span = span.unsqueeze(-2).unsqueeze(-3)
+            # 1 / scale ~ |N(0, span^2)|;  mean ~ U(0, 0.5 / finest spacing);  weights std(y) / Q
+            self.mixture_scales = torch.randn_like(self.raw_mixture_scales).mul_(span).abs_().reciprocal_()
+            self.mixture_means = torch.rand_like(self.raw_mixture_means).mul_(0.5).div(finest)
+            self.mixture_weights = train_y.std().div(self.num_mixtures)
+
+    def initialize_from_data_empspect(self, train_x, train_y):
+        """Means, scales and weights from a diagonal Gaussian mixture (scikit-learn, imported here) fitted to 1000 frequencies drawn
+        from the empirical spectrum |FFT(y)|^2 / N of the outputs (numpy's global generator draws the uniforms).  Assumes evenly
+        spaced inputs, as the reference does."""
+        import numpy as np
+
+        with torch.no_grad():
+            self._training_inputs(train_x, train_y)
+            y = train_y.detach().reshape(-1).cpu()
+            N = y.numel()
+            M = N // 2
+            spect = (torch.fft.fft(y).abs() ** 2 / N)[: M + 1].double().numpy()
+            freq = np.arange(M + 1, dtype=np.float64) / N
+            # inverse-CDF sampling of the frequencies: the spectrum's trapezoidal CDF, linear between the grid frequencies
+            cdf = np.concatenate([[0.0], np.cumsum(0.5 * (spect[1:] + spect[:-1]) * np.diff(freq))])
+            cdf = cdf / cdf[-1]
+            u = np.random.rand(1000, self.ard_num_dims)
+            samples = np.interp(u, cdf, freq)
+            from sklearn.mixture import GaussianMixture
+
+            gmm = GaussianMixture(n_components=self.num_mixtures, covariance_type="diag").fit(samples)
+            like = dict(dtype=self.raw_mixture_means.dtype, device=self.raw_mixture_means.device)
+            self.mixture_means = torch.tensor(gmm.means_, **like).unsqueeze(-2)
+            self.mixture_scales = torch.tensor(gmm.covariances_, **like).unsqueeze(-2)
+            self.mixture_weights = torch.tensor(gmm.weights_, **like)
+
+    def _check_dims(self, x1):
+        d = len(self.active_dims) if self.active_dims is not None else (1 if x1.dim() == 1 else x1.size(-1))
+        if d != self.ard_num_dims:
+            raise RuntimeError(f"The SpectralMixtureKernel expected the input to have {self.ard_num_dims} dimensionality "
+                               f"(based on the ard_num_dims argument). Got {d}.")
+
+    def __call__(self, x1, x2=None, diag=False, **params):
+        self._check_dims(x1)
+        return Kernel.__call__(self, x1, x2, diag=diag, **params)
+
+    def _parameters_of(self, batch_index):
+        w, mu, v = self.mixture_weights, self.mixture_means, self.mixture_scales
+        if batch_index is not None:
+            w, mu, v = w[batch_index], mu[batch_index], v[batch_index]
+        return w, mu, v
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, outputscale=None, **params):
+        from .operators import SpectralMixtureKernelLinearOperator
+        self._check_dims(x1)
+        if diag and not (_same or x1.size(0) == x2.size(0)):
+            raise RuntimeError("diag=True needs x1 and x2 of equal sizes")
+        op = SpectralMixtureKernelLinearOperator(x1, None if _same else x2, *self._parameters_of(_batch_index), outputscale)
+        return op.diagonal() if diag else op
+
+
 def _is_m52_grad(k):
     """k is a Matern52KernelGrad, or a ScaleKernel around one."""
     return isinstance(k, Matern52KernelGrad) or isinstance(getattr(k, "base_kernel", None), Matern52KernelGrad)
@@ -255,6 +398,9 @@ class ScaleKernel(Kernel):
             first = KernelLinearOperator(f[0].x1, f[0].x2, f[0].kind, f[0].lengthscale, self.outputscale * f[0].outputscale)
             op = ProductKernelLinearOperator([first, *f[1:]])
             return op.diagonal() if diag else op
+        if isinstance(self.base_kernel, SpectralMixtureKernel):   # S folded into the same spectral mixture operator
+            os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
+            return self.base_kernel.forward(x1, x2, diag=diag, _same=_same, _batch_index=bi, outputscale=os_)
         if isinstance(self.base_kernel, GridInterpolationKernel):
             base = self.base_kernel.forward(x1, x2, diag=False, _same=_same, **params)
         else:
@@ -454,6 +600,9 @@ class GridInterpolationKernel(Kernel):
 
     def __init__(self, base_kernel, grid_size, num_dims=None, grid_bounds=None, active_dims=None):
         super().__init__(active_dims=active_dims)
+        if isinstance(base_kernel, SpectralMixtureKernel):
+            raise NotImplementedError("a SpectralMixtureKernel base kernel of a GridInterpolationKernel is not available on the "
+                                      "accelerated path")
         if not isinstance(base_kernel, _StationaryKernel):
             raise RuntimeError("GridInterpolationKernel needs an RBFKernel or MaternKernel base kernel on the accelerated path")
         if isinstance(base_kernel, Matern52KernelGrad):

@@ -433,6 +433,8 @@ class KernelLinearOperator(_SamplingMixin):
             return AddedDiagLinearOperator(self, other)
         if isinstance(other, AdditiveKernelLinearOperator):
             raise NotImplementedError("sums that contain additive operators are not available on the accelerated path")
+        if isinstance(other, SpectralMixtureKernelLinearOperator):
+            raise NotImplementedError("sums that contain spectral mixture operators are not available on the accelerated path")
         if isinstance(other, KernelLinearOperator) and not isinstance(other, (SKIKernelLinearOperator, ProductKernelLinearOperator)) \
                 and not isinstance(self, SKIKernelLinearOperator):
             return SumKernelLinearOperator([self, other])     # K_1 + K_2 stays lazy: one engine operator (csrc/sum.cu)
@@ -881,6 +883,8 @@ class SumKernelLinearOperator(KernelLinearOperator):
         if any(isinstance(o, AdditiveKernelLinearOperator) for o in flat):
             # a term is re-wrapped from its inputs, kind and (single) hyper-parameters below, which an additive operator does not have
             raise NotImplementedError("sums that contain additive operators are not available on the accelerated path")
+        if any(isinstance(o, SpectralMixtureKernelLinearOperator) for o in flat):
+            raise NotImplementedError("sums that contain spectral mixture operators are not available on the accelerated path")
         first = flat[0]
         for o in flat[1:]:
             if o.shape != first.shape or o.same != first.same:
@@ -1308,6 +1312,144 @@ class AdditiveKernelLinearOperator(KernelLinearOperator):
 
     def mul(self, other):
         raise NotImplementedError("products that contain an additive operator are not available on the accelerated path")
+
+    __mul__ = mul
+
+
+SPECTRAL_MAX_MIXTURES = 16
+SPECTRAL_MAX_DIMS = 8
+SPECTRAL_MAX_QD = 32
+_SPECTRAL_SLOT = 20        # plan-cache slot of spectral mixture operators (the other operator families use 1..8, 16, 24 and 28)
+# plan-cache slot of the spectral base of a low-rank operator (LOVE's K** - U U^T): its plan carries U, so it must never serve an
+# ordinary spectral operator over the same points; nor may it share the plain low-rank slot, whose operators would inherit the
+# plan's spectral setting when the cache re-points it
+_SPECTRAL_LOWRANK_SLOT = 21
+
+
+class SpectralMixtureKernelLinearOperator(KernelLinearOperator):
+    """S prod_d sum_q w_q exp(-2 pi^2 v_qd^2 tau_d^2) cos(2 pi mu_qd tau_d), tau = x1 - x2 (kernels/spectral_mixture_kernel.py, which
+    sums the components of each dimension and multiplies over the dimensions, through dense [Q, n, m, d] temporaries) as ONE engine
+    plan (gp_plan_set_spectral): products, solves, the preconditioner and SLQ never hold an N x N matrix.  weights [Q], means and
+    scales [Q, 1, d] (or [Q, d]) are the constrained parameter tensors, or their slices for one element of a batch; autograd reaches
+    them through _bilinear_derivative_list.  S is the outputscale of a ScaleKernel around the kernel (None: 1, no gradient).
+    1 <= Q <= 16, 1 <= d <= 8, Q d <= 32; gradients with respect to the inputs are not available."""
+
+    def __init__(self, x1, x2, weights, means, scales, outputscale=None):
+        super().__init__(x1, x2, "rbf", torch.ones((), device=x1.device), outputscale)
+        Q, d = weights.numel(), x1.size(-1)
+        if means.numel() != Q * d or scales.numel() != Q * d:
+            raise RuntimeError(f"spectral mixture: means {tuple(means.shape)} and scales {tuple(scales.shape)} do not hold {Q} x {d} "
+                               "values")
+        if not (1 <= Q <= SPECTRAL_MAX_MIXTURES and 1 <= d <= SPECTRAL_MAX_DIMS and Q * d <= SPECTRAL_MAX_QD):
+            raise NotImplementedError(f"a spectral mixture operator takes 1 <= num_mixtures <= {SPECTRAL_MAX_MIXTURES} over 1 <= d <= "
+                                      f"{SPECTRAL_MAX_DIMS} input dimensions with num_mixtures * d <= {SPECTRAL_MAX_QD} on the "
+                                      f"accelerated path (got {Q} and d = {d})")
+        if x1.requires_grad or (x2 is not None and x2.requires_grad):
+            raise NotImplementedError("gradients with respect to the inputs of a spectral mixture operator (deep kernel learning, "
+                                      "test-input gradients) are not available on the accelerated path")
+        self.weights, self.means, self.scales = weights, means, scales
+        self._scaled = outputscale is not None
+        self.num_mixtures = Q
+
+    def hyper_tensors(self):
+        return [self.weights, self.means, self.scales] + ([self.outputscale] if self._scaled else [])
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    @property
+    def requires_grad(self):
+        return any(t.requires_grad for t in self.hyper_tensors())
+
+    def representation(self):
+        return (self.x1, self.x2, *self.hyper_tensors())
+
+    def _host_hypers(self, noise_t=None):
+        """(weights, means, scales, S, noise) as host lists with one device -> host read."""
+        cached = getattr(self, "_hyp_host", None)
+        if cached is None or (noise_t is not None and cached[5] is not noise_t):
+            parts = [t.detach().reshape(-1).float() for t in (self.weights, self.means, self.scales)]
+            parts.append(self.outputscale.detach().reshape(1).float().to(self.weights.device))
+            if noise_t is not None:
+                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.weights.device))
+            vals = torch.cat(parts).tolist()
+            Q, k = self.num_mixtures, self.means.numel()
+            cached = (vals[:Q], vals[Q:Q + k], vals[Q + k:Q + 2 * k], vals[Q + 2 * k], vals[Q + 2 * k + 1] if noise_t is not None else None,
+                      noise_t)
+            self._hyp_host = cached
+        return cached
+
+    def plan(self, noise=0.0) -> Plan:
+        fresh = False
+        if self._plan is None:
+            slot = _SPECTRAL_LOWRANK_SLOT if getattr(self, "_plan_slot", None) == _LOWRANK_SLOT else _SPECTRAL_SLOT
+            self._plan = _get_plan(self.x1, None if self.same else self.x2, "auto", 0, 0, None, slot, owner=self)
+            fresh = True
+        if torch.is_tensor(noise):
+            w, mu, v, os_, nz, _ = self._host_hypers(noise)
+        else:
+            w, mu, v, os_, _, _ = self._host_hypers(None)
+            nz = float(noise)
+        p = self._plan
+        key = ("rbf", (1.0,), os_, nz)
+        if fresh or getattr(p, "_hyp_key", None) != key:
+            p.set_hypers("rbf", 1.0, os_, nz)   # outputscale and noise; the kind and lengthscale are not used
+            p._hyp_key = key
+        skey = (tuple(w), tuple(mu), tuple(v))
+        if fresh or getattr(p, "_sm_key", None) != skey:   # re-sent only when the parameters' host values change
+            p.set_spectral(w, torch.tensor(mu).reshape(len(w), -1), torch.tensor(v).reshape(len(w), -1))
+            p._sm_key = skey
+        return p
+
+    def _bilinear_derivative_list(self, left, right):
+        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
+        vals = torch.tensor(gl, device=self.device, dtype=self.weights.dtype)
+        Q, k = self.num_mixtures, self.means.numel()
+        out = [vals[:Q].reshape(self.weights.shape), vals[Q:Q + k].reshape(self.means.shape), vals[Q + k:].reshape(self.scales.shape)]
+        if self._scaled:
+            out.append(torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape))
+        return out
+
+    def _bilinear_derivative(self, left, right):
+        raise NotImplementedError("a spectral mixture operator has weight, mean and scale gradients: use _bilinear_derivative_list")
+
+    def _input_grad_list(self, *args):
+        raise NotImplementedError("gradients with respect to the inputs of a spectral mixture operator are not available on the "
+                                  "accelerated path")
+
+    _dense_input_grad_list = _input_grad_list
+
+    def _with(self, x1, x2, detach=False):
+        f = (lambda t: t.detach()) if detach else (lambda t: t)
+        return SpectralMixtureKernelLinearOperator(f(x1), None if x2 is None else f(x2), f(self.weights), f(self.means),
+                                                   f(self.scales), f(self.outputscale) if self._scaled else None)
+
+    def _transpose_nonbatch(self):
+        return self if self.same else self._with(self.x2, self.x1)
+
+    def detach(self):
+        return self._with(self.x1, None if self.same else self.x2, detach=True)
+
+    def __getitem__(self, index):
+        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("a spectral mixture operator adds a (Constant)DiagLinearOperator only: sums that contain spectral "
+                                  "mixture operators are not available on the accelerated path")
+
+    def mul(self, other):
+        raise NotImplementedError("products that contain a spectral mixture operator are not available on the accelerated path")
 
     __mul__ = mul
 

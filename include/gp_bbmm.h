@@ -164,6 +164,29 @@ int gp_plan_set_product(gp_plan* plan, gp_plan* const* factors, int n_factors);
  * gp_plan_set_deriv is refused the same way.  A SKI, sum, product, multitask, derivative or row-sharded plan cannot become additive. */
 int gp_plan_set_additive(gp_plan* plan, int max_degree, const float* comp_scale, int n_comp);
 
+/* Spectral mixture kernels (the reference's SpectralMixtureKernel, kernels/spectral_mixture_kernel.py, dense over [Q, n, m, d]):
+ * `plan` becomes the operator
+ *   K(x, x') = S prod_{c<d} sum_{q<Q} w_q exp(-2 pi^2 v_qc^2 tau_c^2) cos(2 pi mu_qc tau_c),   tau = x - x'
+ * (+ its noise / per-row diagonal where a call adds it), with w = weights[Q], mu = means[Q][d] and v = scales[Q][d] (host arrays,
+ * row-major) and S the outputscale of gp_plan_set_hypers, which also gives the noise; the kind and lengthscale it passes are not
+ * used.  As in the reference, the components of each dimension are summed before the product over the dimensions; for d = 1 this is
+ * S sum_q w_q exp(-2 pi^2 v_q^2 tau^2) cos(2 pi mu_q tau).  The square diagonal is the constant S (sum_q w_q)^d.  A plain plan,
+ * square or cross, after gp_plan_set_data, whose data has d columns.  1 <= Q <= 16, 1 <= d <= 8, Q d <= 32; anything else returns
+ * GP_E_SHAPE.  Parameters are not checked: non-positive or non-finite values give what the formula gives.  Call it again whenever
+ * the parameters change; weights = NULL or Q = 0 clears the setting.  The plan runs its own CUDA-core kernels on packed rows of the
+ * fp32 inputs and their reduced phases frac(mu_qc x_c) (formed in fp64), so the cosine's argument stays below 2 pi in magnitude and
+ * an entry's error does not grow with |x|.
+ * gp_kmv, gp_krows, gp_kdiag, gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos,
+ * gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond, gp_plan_set_noise_diag, gp_plan_set_lowrank and
+ * gp_time_kmv_kernel run on it.  gp_bilinear_grad returns Q (1 + 2d) doubles in grad_ls: dF/dw_q (Q), then dF/dmu_qc and dF/dv_qc
+ * (Q d each, row-major); grad_os receives dF/dS.  A non-finite input makes products, rows, the diagonal and gradients NaN.  On a
+ * spectral plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv, gp_plan_set_deriv_kind, gp_plan_set_sum,
+ * gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_backend, gp_plan_set_comm with more than one rank,
+ * gp_kmv_input_grad and gp_kdense_input_grad return GP_E_STATE with a message naming the call; a spectral plan as a term of
+ * gp_plan_set_sum, a factor of gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.
+ * A SKI, sum, product, multitask, derivative, additive or row-sharded plan cannot become a spectral plan. */
+int gp_plan_set_spectral(gp_plan* plan, int Q, const float* weights, const float* means, const float* scales, int d);
+
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
  * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
  * (+ its noise / per-row diagonal where a call adds it).  U: device [n, r] fp32, leading dimension ldu, caller-owned, must outlive
