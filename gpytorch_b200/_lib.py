@@ -77,6 +77,7 @@ PROTOTYPES = {
     "gp_plan_set_product": (_I, [_P, C.POINTER(_P), _I]),
     "gp_plan_set_additive": (_I, [_P, _I, C.POINTER(_F), _I]),
     "gp_plan_set_spectral": (_I, [_P, _I, C.POINTER(_F), C.POINTER(_F), C.POINTER(_F), _I]),
+    "gp_plan_set_periodic": (_I, [_P, C.POINTER(_F), _I, _I]),
     "gp_plan_set_lowrank": (_I, [_P, _P, _L, _I]),
     "gp_plan_set_tasks": (_I, [_P, _P, _P, _I]),
     "gp_plan_set_task_covar": (_I, [_P, C.POINTER(_F), _I]),

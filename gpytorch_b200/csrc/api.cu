@@ -175,6 +175,7 @@ extern "C" int gp_plan_set_hypers(gp_plan* p, int kind, const float* lengthscale
   for (int i = 0; i < n_ls; ++i)
     GP_REQUIRE(lengthscale[i] > 0.f && isfinite(lengthscale[i]), GP_E_SHAPE, "lengthscale[%d]=%g must be positive", i, lengthscale[i]);
   GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
+  GP_REQUIRE(p->per_n == 0 || kind == GP_RBF, GP_E_STATE, "gp_plan_set_hypers on a periodic plan (gp_plan_set_periodic) takes the kind GP_RBF (got %d)", kind);
   GP_CUDA(cudaSetDevice(p->device));
   p->kind = kind;
   p->ls.assign(lengthscale, lengthscale + n_ls);
@@ -219,6 +220,8 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
              "gp_plan_set_comm with more than one rank is not available on an additive plan (gp_plan_set_additive)");
   GP_REQUIRE(!(p->sm_Q && comm && comm->world > 1), GP_E_STATE,
              "gp_plan_set_comm with more than one rank is not available on a spectral mixture plan (gp_plan_set_spectral)");
+  GP_REQUIRE(!(p->per_n && comm && comm->world > 1), GP_E_STATE,
+             "gp_plan_set_comm with more than one rank is not available on a periodic plan (gp_plan_set_periodic)");
   p->comm = comm;
   return GP_OK;
 }

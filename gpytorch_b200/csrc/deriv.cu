@@ -507,8 +507,10 @@ static int deriv_set(gp_plan* p, gp_plan* data, int kind, const char* what) {
   if (data) GP_REQUIRE(data->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "%s (as the data plan) is not available on a kernel-product plan (gp_plan_set_product)", what);
   GP_REFUSE_ADDITIVE(p, what);
   GP_REFUSE_SPECTRAL(p, what);
+  GP_REFUSE_PERIODIC(p, what);
   if (data) GP_REQUIRE(data->add_M == 0, GP_E_STATE, "%s (as the data plan) is not available on an additive plan (gp_plan_set_additive)", what);
   if (data) GP_REQUIRE(data->sm_Q == 0, GP_E_STATE, "%s (as the data plan) is not available on a spectral mixture plan (gp_plan_set_spectral)", what);
+  if (data) GP_REQUIRE(data->per_n == 0, GP_E_STATE, "%s (as the data plan) is not available on a periodic plan (gp_plan_set_periodic)", what);
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   gp_deriv_state* ds = p->deriv ? p->deriv : new gp_deriv_state();
   gp_plan* old = ds->data;

@@ -281,6 +281,11 @@ struct gp_plan {
   int sm_Q = 0;
   std::vector<float> sm_w, sm_mu, sm_v;   // weights [Q], means and scales [Q][d]
   double sm_diag = 0.0;           // S (sum_q w_q)^d: the constant diagonal of a square operator
+  // periodic kernels (periodic.cu): S exp(-2 sum_d sin^2(pi tau_d / p_d) / l_d) as the RBF kernel of unit lengthscale over the
+  // embedding u_d(x) = (cos, sin)(2 pi x_d / p_d) / sqrt(l_d); from the packing on the plan is a plain RBF plan of 2d packed
+  // columns (packed_dims).  per_n = 0 is a plain plan, else 1 (one shared period) or d
+  int per_n = 0;
+  std::vector<float> per_p;       // the per_n periods
   int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
@@ -399,6 +404,13 @@ int spectral_kdiag(gp_plan* p, float* OUT);
 int spectral_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
 #define GP_REFUSE_SPECTRAL(p, what) \
   GP_REQUIRE((p)->sm_Q == 0, GP_E_STATE, "%s is not available on a spectral mixture plan (gp_plan_set_spectral)", what)
+// periodic.cu
+int periodic_pack(gp_plan* p);                                          // embeds the inputs into Z1 / Z2 (and the tensor-core tiles)
+int periodic_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+#define GP_REFUSE_PERIODIC(p, what) \
+  GP_REQUIRE((p)->per_n == 0, GP_E_STATE, "%s is not available on a periodic plan (gp_plan_set_periodic)", what)
+// columns of the packed rows the plain kernels see: the d inputs, or the 2d embedding columns of a periodic plan
+inline int packed_dims(const gp_plan* p) { return p->per_n ? 2 * p->d : p->d; }
 inline bool plan_is_tc(const gp_plan* p) {
   return p->backend == GP_BACKEND_TCGEN05 || (p->backend == GP_BACKEND_SUM && p->sum_tc) || (p->backend == GP_BACKEND_PRODUCT && p->prod_tc);
 }

@@ -523,6 +523,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   if (p->deriv) return deriv_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->add_M) return additive_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->sm_Q) return spectral_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
+  if (p->per_n) return periodic_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   // before any launch: the SIMT derivative kernel is instantiated up to DP = 64
   GP_REQUIRE(p->backend == GP_BACKEND_SKI || p->DP <= 64, GP_E_SHAPE, "bilinear gradient supports d <= 64 (d=%d)", p->d);
   const bool ard = p->ls.size() > 1;

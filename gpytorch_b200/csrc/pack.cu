@@ -142,9 +142,10 @@ static int round_dp(int d) {
 }
 
 int choose_geometry(gp_plan* p) {
-  p->DP = round_dp(p->d);
+  const int w = packed_dims(p);   // 2d embedding columns on a periodic plan
+  p->DP = round_dp(w);
   GP_REQUIRE(p->DP > 0, GP_E_SHAPE, "input dimension d=%d > 128 is not supported", p->d);
-  int kp = 3 * p->d + 4;
+  int kp = 3 * w + 4;
   p->KP = ((kp + 7) / 8) * 8;
   int want = p->backend_req;
   if (want == GP_BACKEND_AUTO) want = (p->KP <= KP_MAX) ? GP_BACKEND_TCGEN05 : GP_BACKEND_SIMT;
@@ -193,6 +194,7 @@ int pack_inputs(gp_plan* p) {
   p->pack_gen++;   // a kernel product over this plan re-reads its scale, geometry and flag (product.cu)
   GP_CHECK(choose_geometry(p));
   if (p->sm_Q) return spectral_pack(p);
+  if (p->per_n) return periodic_pack(p);
   cudaStream_t st = p->stream;
   const int d = p->d, DP = p->DP;
   GP_CHECK(p->mean.ensure(sizeof(float) * (d + 4)));
@@ -257,8 +259,9 @@ int to_v16(gp_plan* p, const float* V, int64_t ldv, int t, int64_t n, float* V16
 
 // tensor-core operand tiles of rows [0, npad) of Z (rows >= nvalid zero): the A side (XA layout) or the B side (XB layout)
 int pack_tc_rows(gp_plan* p, const float* Z, int64_t nvalid, int64_t npad, bool is_a, float* out) {
-  if (is_a) pack_tc_kernel<true><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, p->d, p->DP, p->KP, TILE_I, out);
-  else pack_tc_kernel<false><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, p->d, p->DP, p->KP, TILE_J, out);
+  const int w = packed_dims(p);
+  if (is_a) pack_tc_kernel<true><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, w, p->DP, p->KP, TILE_I, out);
+  else pack_tc_kernel<false><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, w, p->DP, p->KP, TILE_J, out);
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;

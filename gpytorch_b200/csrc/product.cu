@@ -446,6 +446,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   GP_REFUSE_LOWRANK(p, "gp_plan_set_product");
   GP_REFUSE_ADDITIVE(p, "gp_plan_set_product");
   GP_REFUSE_SPECTRAL(p, "gp_plan_set_product");
+  GP_REFUSE_PERIODIC(p, "gp_plan_set_product");
   GP_CUDA(cudaSetDevice(p->device));
   if (factors == nullptr || n_factors == 0) {   // back to a plain plan
     if (p->backend_req != GP_BACKEND_PRODUCT) return GP_OK;
@@ -461,6 +462,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
     GP_REQUIRE(factors[f]->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "kernel product: a factor that is itself a kernel product is not available");
     GP_REQUIRE(factors[f]->add_M == 0, GP_E_STATE, "gp_plan_set_product: an additive plan as a factor is not available (gp_plan_set_additive)");
     GP_REQUIRE(factors[f]->sm_Q == 0, GP_E_STATE, "gp_plan_set_product: a spectral mixture plan as a factor is not available (gp_plan_set_spectral)");
+    GP_REQUIRE(factors[f]->per_n == 0, GP_E_STATE, "gp_plan_set_product: a periodic plan as a factor is not available (gp_plan_set_periodic)");
   }
   p->factors.assign(factors, factors + n_factors);
   p->backend_req = GP_BACKEND_PRODUCT;

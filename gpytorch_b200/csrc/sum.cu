@@ -125,6 +125,7 @@ extern "C" int gp_plan_set_sum(gp_plan* p, gp_plan* const* terms, int n_terms) {
   GP_REFUSE_PRODUCT(p, "gp_plan_set_sum");
   GP_REFUSE_ADDITIVE(p, "gp_plan_set_sum");
   GP_REFUSE_SPECTRAL(p, "gp_plan_set_sum");
+  GP_REFUSE_PERIODIC(p, "gp_plan_set_sum");
   for (int t = 0; t < n_terms; ++t)
     GP_REQUIRE(terms[t] == nullptr || terms[t]->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE,
                "gp_plan_set_sum: a kernel product as a term is not available (gp_plan_set_product)");

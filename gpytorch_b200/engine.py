@@ -115,9 +115,10 @@ class Plan:
     def set_hypers(self, kind: str, lengthscale, outputscale: float = 1.0, noise: float = 0.0):
         ls = [float(v) for v in (lengthscale if hasattr(lengthscale, "__len__") else [lengthscale])]
         arr = (C.c_float * len(ls))(*ls)
-        self.kind, self.lengthscale, self.outputscale, self.noise = kind, ls, float(outputscale), float(noise)
         with torch.cuda.device(self.device):
             check(self.lib.gp_plan_set_hypers(self._h, KIND[kind], arr, len(ls), float(outputscale), float(noise)))
+        # recorded once the engine took them: bilinear_grad sizes its output by these lengthscales
+        self.kind, self.lengthscale, self.outputscale, self.noise = kind, ls, float(outputscale), float(noise)
         return self
 
     def set_ski(self, grid_sizes, grid_lo, grid_step):
@@ -236,6 +237,21 @@ class Plan:
             check(self.lib.gp_plan_set_spectral(self._h, Q, (C.c_float * Q)(*w), (C.c_float * (Q * d))(*mu.reshape(-1).tolist()),
                                                 (C.c_float * (Q * d))(*sc.reshape(-1).tolist()), d))
         self._spectral = (Q, d)
+        return self
+
+    def set_periodic(self, period=None):
+        """Periodic kernel: this plan's operator becomes S exp(-2 sum_d sin^2(pi tau_d / p_d) / l_d) over tau = x - x', with the
+        lengthscales l, outputscale S and noise of set_hypers (kind "rbf").  period: 1 or d values (a host sequence or tensor);
+        None clears it.  bilinear_grad then returns [dl (1 or d) | dp (1 or d)] and dF/dS."""
+        if period is None:
+            self._periodic = None
+            with torch.cuda.device(self.device):
+                check(self.lib.gp_plan_set_periodic(self._h, None, 0, 0))
+            return self
+        per = [float(v) for v in (period.reshape(-1).tolist() if torch.is_tensor(period) else period)]
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_periodic(self._h, (C.c_float * len(per))(*per), len(per), self.d))
+        self._periodic = len(per)
         return self
 
     def set_noise_diag(self, diag: torch.Tensor | None):
@@ -366,7 +382,7 @@ class Plan:
         """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right)) for left [row_count, s], right [n2, s].  On a kernel
         product: the factors' lengthscale gradients one after the other, and the gradient of the combined scale S.  On an additive
         plan: the D lengthscale gradients and the list of the D component-scale gradients.  On a spectral plan: the Q (1 + 2d)
-        gradients [dw | dmu | dv] and dF/dS."""
+        gradients [dw | dmu | dv] and dF/dS.  On a periodic plan: [dl | dp] and dF/dS."""
         if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.row_count or right.size(0) != self.n2 \
                 or left.size(1) != right.size(1) or left.size(1) < 1:
             raise RuntimeError(f"bilinear_grad: left must be [{self.row_count}, s] and right [{self.n2}, s] with s >= 1 "
@@ -385,6 +401,9 @@ class Plan:
             Q, d = self._spectral
             nls = Q * (1 + 2 * d)
             gl = (C.c_double * nls)()
+        if getattr(self, "_periodic", None) is not None:   # [dl | dp] and dF/dS
+            nls = len(self.lengthscale) + self._periodic
+            gl = (C.c_double * (2 * self.d))()   # the engine writes at most d + d values, whatever this side recorded
         if getattr(self, "_additive", None) is not None:   # D component-scale gradients
             go = (C.c_double * len(self._additive[1]))()
             with torch.cuda.device(self.device):

@@ -1,5 +1,5 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, SpectralMixtureKernel, ScaleKernel,
-AdditiveKernel, ProductKernel, GridInterpolationKernel} for the accelerated path.
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, SpectralMixtureKernel, PeriodicKernel,
+ScaleKernel, AdditiveKernel, ProductKernel, GridInterpolationKernel} for the accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
 rbf_kernel.py:68-85; matern_kernel.py:79-110; scale_kernel.py:64-118), but `forward` returns an
@@ -348,6 +348,55 @@ class SpectralMixtureKernel(Kernel):
         return op.diagonal() if diag else op
 
 
+class PeriodicKernel(Kernel):
+    """k(x, x') = exp(-2 sum_d sin^2(pi (x_d - x'_d) / p_d) / l_d) (kernels/periodic_kernel.py; the lengthscale is not squared).
+    Parameters as in the reference: raw_lengthscale and raw_period_length [*B, 1, ard_num_dims or 1], each with a Positive()
+    constraint unless one is given.  forward returns one engine PeriodicKernelLinearOperator (gp_plan_set_periodic), which runs as
+    an RBF kernel over the embedding (cos, sin)(2 pi x / p) on tensor cores; inside a ScaleKernel the outputscale multiplies it,
+    and scaled or not it may be a term of an AdditiveKernel.  1 <= d <= 16, one batch dimension at most, no priors.  Products,
+    SKI, multitask and derivative kernels do not take it, and the inputs get no gradient."""
+
+    has_lengthscale = True
+
+    def __init__(self, period_length_prior=None, period_length_constraint=None, lengthscale_prior=None, **kwargs):
+        if period_length_prior is not None or lengthscale_prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        super().__init__(**kwargs)
+        n = self.ard_num_dims or 1
+        self.register_parameter("raw_period_length", torch.nn.Parameter(torch.zeros(*self.batch_shape, 1, n)))
+        self.register_constraint("raw_period_length", period_length_constraint or Positive())
+
+    @property
+    def period_length(self):
+        return self.raw_period_length_constraint.transform(self.raw_period_length)
+
+    @period_length.setter
+    def period_length(self, value):
+        self._set_period_length(value)
+
+    def _set_period_length(self, value):
+        self._set_constrained("raw_period_length", value)
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, outputscale=None, last_dim_is_batch=False, **params):
+        from .operators import PeriodicKernelLinearOperator
+        if last_dim_is_batch:
+            raise NotImplementedError("last_dim_is_batch is not available for a PeriodicKernel on the accelerated path")
+        if diag and not (_same or x1.size(0) == x2.size(0)):
+            raise RuntimeError("diag=True needs x1 and x2 of equal sizes")
+        ls, per = self.lengthscale, self.period_length
+        if _batch_index is not None:
+            ls, per = ls[_batch_index], per[_batch_index]
+        ls, per = ls.reshape(-1), per.reshape(-1)
+        op = PeriodicKernelLinearOperator(x1, None if _same else x2, ls[0] if ls.numel() == 1 else ls,
+                                          per[0] if per.numel() == 1 else per, outputscale)
+        return op.diagonal() if diag else op
+
+
+def _is_periodic(k):
+    """k is a PeriodicKernel, or a ScaleKernel around one."""
+    return isinstance(k, PeriodicKernel) or isinstance(getattr(k, "base_kernel", None), PeriodicKernel)
+
+
 def _is_m52_grad(k):
     """k is a Matern52KernelGrad, or a ScaleKernel around one."""
     return isinstance(k, Matern52KernelGrad) or isinstance(getattr(k, "base_kernel", None), Matern52KernelGrad)
@@ -384,9 +433,10 @@ class ScaleKernel(Kernel):
             from .operators import SumKernelLinearOperator
             if _batch_index is not None:
                 raise NotImplementedError("batched ScaleKernel over an AdditiveKernel")
+            from .operators import with_outputscale
             inner = self.base_kernel(x1, None if _same else x2)
             terms = inner.ops if isinstance(inner, SumKernelLinearOperator) else [inner]
-            scaled = [KernelLinearOperator(t.x1, t.x2, t.kind, t.lengthscale, self.outputscale * t.outputscale) for t in terms]
+            scaled = [with_outputscale(t, self.outputscale * t.outputscale) for t in terms]   # periodic terms keep their period
             op = scaled[0] if len(scaled) == 1 else SumKernelLinearOperator(scaled)
             return op.diagonal() if diag else op
         if isinstance(self.base_kernel, ProductKernel):
@@ -398,9 +448,9 @@ class ScaleKernel(Kernel):
             first = KernelLinearOperator(f[0].x1, f[0].x2, f[0].kind, f[0].lengthscale, self.outputscale * f[0].outputscale)
             op = ProductKernelLinearOperator([first, *f[1:]])
             return op.diagonal() if diag else op
-        if isinstance(self.base_kernel, SpectralMixtureKernel):   # S folded into the same spectral mixture operator
+        if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel)):   # S folded into the same operator
             os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
-            return self.base_kernel.forward(x1, x2, diag=diag, _same=_same, _batch_index=bi, outputscale=os_)
+            return self.base_kernel.forward(x1, x2, diag=diag, _same=_same, _batch_index=bi, outputscale=os_, **params)
         if isinstance(self.base_kernel, GridInterpolationKernel):
             base = self.base_kernel.forward(x1, x2, diag=False, _same=_same, **params)
         else:
@@ -412,6 +462,14 @@ class ScaleKernel(Kernel):
             return op.diagonal() if diag else op
         if isinstance(base, SKIKernelLinearOperator):
             op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
+            return op.diagonal() if diag else op
+        from .operators import PeriodicKernelLinearOperator, SumKernelLinearOperator, with_outputscale
+        if isinstance(base, PeriodicKernelLinearOperator):   # a nested ScaleKernel: both scales folded in, the period kept
+            op = with_outputscale(base, os_ * base.outputscale)
+            return op.diagonal() if diag else op
+        if isinstance(base, SumKernelLinearOperator) and any(isinstance(t, PeriodicKernelLinearOperator) for t in base.ops):
+            # a ScaleKernel around a scaled sum with periodic terms: the scale folded into every term, the periods kept
+            op = SumKernelLinearOperator([with_outputscale(t, os_ * t.outputscale) for t in base.ops])
             return op.diagonal() if diag else op
         op = KernelLinearOperator(base.x1, base.x2, base.kind, base.lengthscale, os_)
         return op.diagonal() if diag else op
@@ -478,6 +536,8 @@ class ProductKernel(Kernel):
         for k in kernels:
             if not isinstance(k, Kernel):
                 raise RuntimeError("ProductKernel factors must be kernels")
+            if _is_periodic(k):
+                raise NotImplementedError("products with a PeriodicKernel factor are not available on the accelerated path")
             base = k.base_kernel if isinstance(k, ScaleKernel) else k
             if not isinstance(base, _StationaryKernel) or isinstance(base, (RBFKernelGrad, Matern52KernelGrad)):
                 raise NotImplementedError("ProductKernel factors must be RBF / Matern kernels (optionally scaled) on the accelerated "
@@ -575,6 +635,8 @@ class MultitaskKernel(Kernel):
             raise NotImplementedError("a batched MultitaskKernel is not available on the accelerated path")
         dm = self.data_covar_module
         base = dm.base_kernel if isinstance(dm, ScaleKernel) else dm
+        if isinstance(base, PeriodicKernel):
+            raise NotImplementedError("a PeriodicKernel data kernel of a MultitaskKernel is not available on the accelerated path")
         if not isinstance(base, _StationaryKernel) or len(dm.batch_shape):
             raise NotImplementedError("the accelerated MultitaskKernel takes an RBFKernel / MaternKernel data kernel, optionally "
                                       "inside a ScaleKernel")
@@ -603,6 +665,9 @@ class GridInterpolationKernel(Kernel):
         if isinstance(base_kernel, SpectralMixtureKernel):
             raise NotImplementedError("a SpectralMixtureKernel base kernel of a GridInterpolationKernel is not available on the "
                                       "accelerated path")
+        if isinstance(base_kernel, PeriodicKernel):
+            raise NotImplementedError("a PeriodicKernel base kernel of a GridInterpolationKernel is not available on the accelerated "
+                                      "path")
         if not isinstance(base_kernel, _StationaryKernel):
             raise RuntimeError("GridInterpolationKernel needs an RBFKernel or MaternKernel base kernel on the accelerated path")
         if isinstance(base_kernel, Matern52KernelGrad):

@@ -893,8 +893,13 @@ class SumKernelLinearOperator(KernelLinearOperator):
         # own) and give every term its own slot of the plan cache
         self.ops = []
         for i, o in enumerate(flat):
-            t = KernelLinearOperator(o.x1, o.x2, o.kind, o.lengthscale, o.outputscale, comm=o._comm, row_begin=o._row_begin, row_count=o._row_count)
-            t._plan_slot = 1 + i
+            if isinstance(o, PeriodicKernelLinearOperator):   # keeps its period, on a slot no plain term uses
+                t = o._with(o.x1, None if o.same else o.x2)
+                t._plan_slot = _PERIODIC_SUM_SLOT + i
+            else:
+                t = KernelLinearOperator(o.x1, o.x2, o.kind, o.lengthscale, o.outputscale, comm=o._comm, row_begin=o._row_begin,
+                                         row_count=o._row_count)
+                t._plan_slot = 1 + i
             self.ops.append(t)
         self.x1, self.x2, self.same = first.x1, first.x2, first.same
         self.kind = "sum"
@@ -1452,6 +1457,144 @@ class SpectralMixtureKernelLinearOperator(KernelLinearOperator):
         raise NotImplementedError("products that contain a spectral mixture operator are not available on the accelerated path")
 
     __mul__ = mul
+
+
+PERIODIC_MAX_DIMS = 16
+_PERIODIC_SLOT = 32        # plan-cache slot of periodic operators (the other operator families use 0..8, 16, 20/21, 24 and 28)
+# the periodic base of a low-rank operator (LOVE's K** - U U^T) carries U: it never serves an ordinary periodic operator, and a
+# periodic plan is never handed to a plain low-rank operator (a plan the cache re-points keeps its periodic setting)
+_PERIODIC_LOWRANK_SLOT = 33
+_PERIODIC_SUM_SLOT = 34    # periodic terms of a kernel sum: 34 + term index, as plain terms take 1 + term index
+
+
+class PeriodicKernelLinearOperator(KernelLinearOperator):
+    """S exp(-2 sum_d sin^2(pi tau_d / p_d) / l_d), tau = x1 - x2 (kernels/periodic_kernel.py, which forms the dense matrix) as ONE
+    engine plan (gp_plan_set_periodic).  The engine runs it as the RBF kernel of unit lengthscale over the embedding
+    (cos, sin)(2 pi x_d / p_d) / sqrt(l_d), so products, solves, the preconditioner and SLQ run on the plain tensor-core path.
+    lengthscale and period hold 1 or d values (the parameter tensors or their slices for one element of a batch); autograd reaches
+    them through _bilinear_derivative_list.  S is the outputscale of a ScaleKernel around the kernel (None: 1, no gradient).
+    1 <= d <= 16; gradients with respect to the inputs are not available."""
+
+    def __init__(self, x1, x2, lengthscale, period, outputscale=None, comm=None, row_begin=0, row_count=0):
+        super().__init__(x1, x2, "rbf", lengthscale, outputscale, comm=comm, row_begin=row_begin, row_count=row_count)
+        d = x1.size(-1)
+        if not 1 <= d <= PERIODIC_MAX_DIMS:
+            raise NotImplementedError(f"a periodic operator takes 1 <= d <= {PERIODIC_MAX_DIMS} input dimensions on the accelerated "
+                                      f"path (got d = {d})")
+        if lengthscale.numel() not in (1, d) or period.numel() not in (1, d):
+            raise RuntimeError(f"periodic kernel: lengthscale {tuple(lengthscale.shape)} and period {tuple(period.shape)} must hold 1 "
+                               f"or {d} values")
+        if x1.requires_grad or (x2 is not None and x2.requires_grad):
+            raise NotImplementedError("gradients with respect to the inputs of a periodic operator (deep kernel learning, test-input "
+                                      "gradients) are not available on the accelerated path")
+        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
+            raise NotImplementedError("a row-sharded periodic operator is not available on the accelerated path")
+        self.period = period
+
+    def hyper_tensors(self):
+        return [self.lengthscale, self.period, self.outputscale]
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    @property
+    def requires_grad(self):
+        return any(t.requires_grad for t in self.hyper_tensors())
+
+    def representation(self):
+        return (self.x1, self.x2, *self.hyper_tensors())
+
+    def _host_hypers(self, noise_t=None):
+        """(lengthscale list, outputscale, noise, noise tensor, period list) with one device -> host read."""
+        cached = getattr(self, "_hyp_host", None)
+        if cached is None or (noise_t is not None and cached[3] is not noise_t):
+            parts = [t.detach().reshape(-1).float().to(self.device) for t in (self.lengthscale, self.outputscale, self.period)]
+            if noise_t is not None:
+                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.device))
+            vals = torch.cat(parts).tolist()
+            nl, npr = self.lengthscale.numel(), self.period.numel()
+            cached = (vals[:nl], vals[nl], vals[nl + 1 + npr] if noise_t is not None else None, noise_t, vals[nl + 1:nl + 1 + npr])
+            self._hyp_host = cached
+        return cached
+
+    def _slot(self):
+        slot = getattr(self, "_plan_slot", None)
+        if slot is None:
+            return _PERIODIC_SLOT
+        return _PERIODIC_LOWRANK_SLOT if slot == _LOWRANK_SLOT else slot
+
+    def plan(self, noise=0.0) -> Plan:
+        if self._plan is None:
+            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None, self._slot(),
+                                   owner=self)
+        if torch.is_tensor(noise):
+            ls, os_, nz, _, per = self._host_hypers(noise)
+        else:
+            ls, os_, _, _, per = self._host_hypers(None)
+            nz = float(noise)
+        p = self._plan
+        # re-sent only when the host values change: a cached plan keeps the setting (and packing) its keys record, so a new
+        # operator over the same plan with the same parameters packs nothing
+        if getattr(p, "_per_key", None) != tuple(per):
+            p.set_periodic(per)
+            p._per_key = tuple(per)
+        key = ("rbf", tuple(ls), os_, nz)
+        if getattr(p, "_hyp_key", None) != key:
+            p.set_hypers("rbf", ls, os_, nz)
+            p._hyp_key = key
+        return p
+
+    def _bilinear_derivative_list(self, left, right):
+        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
+        vals = torch.tensor(gl, device=self.device, dtype=self.lengthscale.dtype)
+        nl = self.lengthscale.numel()
+        return [vals[:nl].reshape(self.lengthscale.shape), vals[nl:].to(self.period.dtype).reshape(self.period.shape),
+                torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape)]
+
+    def _bilinear_derivative(self, left, right):
+        raise NotImplementedError("a periodic operator has lengthscale, period and outputscale gradients: use _bilinear_derivative_list")
+
+    def _input_grad_list(self, *args):
+        raise NotImplementedError("gradients with respect to the inputs of a periodic operator are not available on the accelerated "
+                                  "path")
+
+    _dense_input_grad_list = _input_grad_list
+
+    def _with(self, x1, x2, detach=False, outputscale=None):
+        f = (lambda t: t.detach()) if detach else (lambda t: t)
+        return PeriodicKernelLinearOperator(f(x1), None if x2 is None else f(x2), f(self.lengthscale), f(self.period),
+                                            f(self.outputscale if outputscale is None else outputscale))
+
+    def _transpose_nonbatch(self):
+        return self if self.same else self._with(self.x2, self.x1)
+
+    def detach(self):
+        return self._with(self.x1, None if self.same else self.x2, detach=True)
+
+    def __getitem__(self, index):
+        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
+
+    def mul(self, other):
+        raise NotImplementedError("products that contain a periodic operator are not available on the accelerated path")
+
+    __mul__ = mul
+
+
+def with_outputscale(op, outputscale):
+    """A plain or periodic kernel operator with its outputscale replaced (a ScaleKernel folded into the terms of a sum or into the
+    first factor of a product); the operator's other parameters are kept."""
+    if isinstance(op, PeriodicKernelLinearOperator):
+        return op._with(op.x1, None if op.same else op.x2, outputscale=outputscale)
+    return KernelLinearOperator(op.x1, op.x2, op.kind, op.lengthscale, outputscale)
 
 
 class SKIKernelLinearOperator(KernelLinearOperator):

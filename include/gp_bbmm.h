@@ -187,6 +187,29 @@ int gp_plan_set_additive(gp_plan* plan, int max_degree, const float* comp_scale,
  * A SKI, sum, product, multitask, derivative, additive or row-sharded plan cannot become a spectral plan. */
 int gp_plan_set_spectral(gp_plan* plan, int Q, const float* weights, const float* means, const float* scales, int d);
 
+/* Periodic kernels (the reference's PeriodicKernel, kernels/periodic_kernel.py): `plan` becomes the operator
+ *   K(x, x') = S exp(-2 sum_{c<d} sin^2(pi tau_c / p_c) / l_c),   tau = x - x'   (l_c not squared, as in the reference)
+ * (+ its noise / per-row diagonal where a call adds it), with the n_period periods p = period[] (1: one period shared by every
+ * dimension, or d), and the lengthscales l (1 or d), the outputscale S and the noise of gp_plan_set_hypers, whose kind must be
+ * GP_RBF.  A plain plan, square or cross, after gp_plan_set_data, whose data has d columns; 1 <= d <= 16 and every period > 0 and
+ * finite, else GP_E_SHAPE; a plan whose gp_plan_set_hypers kind is not GP_RBF returns GP_E_STATE, and so does gp_plan_set_hypers
+ * with another kind on a periodic plan.  A failed call leaves the plan's previous setting in place.  Call it again whenever the
+ * periods change; period = NULL or n_period = 0 clears the setting.  The
+ * kernel is the RBF kernel of unit lengthscale over the embedding u_c(x) = (cos, sin)(2 pi x_c / p_c) / sqrt(l_c): the plan packs
+ * u (2d columns, from phases reduced in fp64, so an entry's error does not grow with |x|) and from then on runs as a plain RBF
+ * plan of width 2d, on the tensor-core backend (kpad = pad8(6d + 4)) or the CUDA-core one.
+ * gp_kmv, gp_krows, gp_kdiag (the square diagonal is S), gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg,
+ * gp_slq_logdet, gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond, gp_plan_set_backend,
+ * gp_plan_set_noise_diag, gp_plan_set_lowrank and gp_time_kmv_kernel run on it, and it may be a term of gp_plan_set_sum.
+ * gp_bilinear_grad returns n_ls + n_period doubles in grad_ls, [dF/dl (n_ls) | dF/dp (n_period)] (a shared parameter receives the
+ * sum over the dimensions), and dF/dS in grad_os; it is formed from tau directly, not through the embedding.  A non-finite input
+ * makes the gradients NaN.  On a periodic plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv, gp_plan_set_deriv_kind,
+ * gp_plan_set_sum, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_spectral, gp_plan_set_comm with more
+ * than one rank, gp_kmv_input_grad and gp_kdense_input_grad return GP_E_STATE with a message naming the call; a periodic plan as a
+ * factor of gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.  A SKI, sum,
+ * product, multitask, derivative, additive, spectral or row-sharded plan cannot become a periodic plan. */
+int gp_plan_set_periodic(gp_plan* plan, const float* period, int n_period, int d);
+
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
  * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
  * (+ its noise / per-row diagonal where a call adds it).  U: device [n, r] fp32, leading dimension ldu, caller-owned, must outlive
