@@ -169,6 +169,7 @@ extern "C" int gp_plan_set_data(gp_plan* p, const float* X1, int64_t n1, int64_t
 
 extern "C" int gp_plan_set_hypers(gp_plan* p, int kind, const float* lengthscale, int n_ls, float outputscale, float noise) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  GP_REQUIRE(kind != GP_RQ, GP_E_SHAPE, "the rational quadratic kind takes alpha: call gp_plan_set_hypers_rq");
   GP_REQUIRE(kind >= GP_RBF && kind <= GP_MATERN52, GP_E_SHAPE, "nu expected to be 0.5, 1.5, or 2.5 (kind=%d)", kind);
   GP_REQUIRE(lengthscale && n_ls >= 1, GP_E_SHAPE, "lengthscale missing");
   GP_REQUIRE(!p->data_set || n_ls == 1 || n_ls == p->d, GP_E_SHAPE, "lengthscale count %d does not match d=%d", n_ls, p->d);
@@ -184,6 +185,51 @@ extern "C" int gp_plan_set_hypers(gp_plan* p, int kind, const float* lengthscale
   p->hypers_set = true;
   if (p->data_set) return pack_inputs(p);
   return GP_OK;
+}
+
+extern "C" int gp_plan_set_hypers_rq(gp_plan* p, const float* lengthscale, int n_ls, float alpha, float outputscale, float noise) {
+  GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  GP_REQUIRE(lengthscale && n_ls >= 1, GP_E_SHAPE, "lengthscale missing");
+  GP_REQUIRE(!p->data_set || n_ls == 1 || n_ls == p->d, GP_E_SHAPE, "lengthscale count %d does not match d=%d", n_ls, p->d);
+  for (int i = 0; i < n_ls; ++i)
+    GP_REQUIRE(lengthscale[i] > 0.f && isfinite(lengthscale[i]), GP_E_SHAPE, "lengthscale[%d]=%g must be positive", i, lengthscale[i]);
+  GP_REQUIRE(alpha > 0.f && isfinite(alpha), GP_E_SHAPE, "alpha=%g must be positive and finite", alpha);
+  GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
+  GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "gp_plan_set_hypers_rq is not available on a SKI plan (gp_plan_set_ski)");
+  GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "gp_plan_set_hypers_rq is not available on a kernel-sum plan: give the kind to a term");
+  GP_REFUSE_TASKS(p, "gp_plan_set_hypers_rq");
+  GP_REFUSE_KRON(p, "gp_plan_set_hypers_rq");
+  GP_REFUSE_DERIV(p, "gp_plan_set_hypers_rq");
+  GP_REFUSE_PRODUCT(p, "gp_plan_set_hypers_rq");
+  GP_REFUSE_ADDITIVE(p, "gp_plan_set_hypers_rq");
+  GP_REFUSE_SPECTRAL(p, "gp_plan_set_hypers_rq");
+  GP_REFUSE_PERIODIC(p, "gp_plan_set_hypers_rq");
+  GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_STATE, "gp_plan_set_hypers_rq is not available on a row-sharded plan (gp_plan_set_comm)");
+  GP_CUDA(cudaSetDevice(p->device));
+  // all or nothing: a failed pack restores the previous hyper-parameters (and packing), so the number of gradient values a caller
+  // sizes from the kind it asked for always matches what the engine writes
+  const int old_kind = p->kind;
+  const std::vector<float> old_ls = p->ls;
+  const float old_alpha = p->rq_alpha, old_os = p->outputscale, old_noise = p->noise;
+  const bool old_set = p->hypers_set;
+  p->kind = GP_RQ;
+  p->ls.assign(lengthscale, lengthscale + n_ls);
+  p->rq_alpha = alpha;
+  p->outputscale = outputscale;
+  p->noise = noise;
+  p->hypers_set = true;
+  if (!p->data_set) return GP_OK;
+  const int st = pack_inputs(p);
+  if (st != GP_OK) {
+    p->kind = old_kind;
+    p->ls = old_ls;
+    p->rq_alpha = old_alpha;
+    p->outputscale = old_os;
+    p->noise = old_noise;
+    p->hypers_set = old_set;
+    if (old_set) pack_inputs(p);   // the previous packing; the error reported is the first one
+  }
+  return st;
 }
 
 extern "C" int gp_plan_set_noise_diag(gp_plan* p, const float* diag, int64_t n) {
@@ -222,6 +268,8 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
              "gp_plan_set_comm with more than one rank is not available on a spectral mixture plan (gp_plan_set_spectral)");
   GP_REQUIRE(!(p->per_n && comm && comm->world > 1), GP_E_STATE,
              "gp_plan_set_comm with more than one rank is not available on a periodic plan (gp_plan_set_periodic)");
+  GP_REQUIRE(!(p->kind == GP_RQ && comm && comm->world > 1), GP_E_STATE,
+             "gp_plan_set_comm with more than one rank is not available on a rational quadratic plan (gp_plan_set_hypers_rq)");
   p->comm = comm;
   return GP_OK;
 }

@@ -286,6 +286,8 @@ struct gp_plan {
   // columns (packed_dims).  per_n = 0 is a plain plan, else 1 (one shared period) or d
   int per_n = 0;
   std::vector<float> per_p;       // the per_n periods
+  // rational quadratic kernels (kind GP_RQ, gp_plan_set_hypers_rq): (1 + r^2 / (2 alpha))^-alpha over z = (x - mean) / l
+  float rq_alpha = 0.f;
   int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
@@ -306,7 +308,7 @@ int pack_inputs(gp_plan* p);                                            // pack.
 int to_v16(gp_plan* p, const float* V, int64_t ldv, int t, int64_t n, float* V16);
 int pack_v_tiles(gp_plan* p, const float* V16);                         // pack.cu (tensor-core B operand of GEMM2)
 int kmv_partials(gp_plan* p, const float* V16, const int* done_flag);   // dispatch simt / tensor cores
-int kmv_tc_launch_kind(gp_plan* p, int kind, const int* done_flag);     // kind may be GP_DERIV + kind
+int kmv_tc_launch_kind(gp_plan* p, int kind, const int* done_flag);     // kind may be GP_DERIV + kind, or RQ_DL / RQ_DA on an RQ plan
 int product_tc_launch(gp_plan* p, const int* done_flag);                // kmv_tc.cu: the two tensor-core factors of a product plan
 int kmv_simt_launch(gp_plan* p, const float* V16, const int* done_flag);
 int kmv_tc_launch(gp_plan* p, const int* done_flag);
@@ -409,6 +411,8 @@ int periodic_pack(gp_plan* p);                                          // embed
 int periodic_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
 #define GP_REFUSE_PERIODIC(p, what) \
   GP_REQUIRE((p)->per_n == 0, GP_E_STATE, "%s is not available on a periodic plan (gp_plan_set_periodic)", what)
+#define GP_REFUSE_RQ(p, what) \
+  GP_REQUIRE((p)->kind != GP_RQ, GP_E_STATE, "%s is not available on a rational quadratic plan (gp_plan_set_hypers_rq)", what)
 // columns of the packed rows the plain kernels see: the d inputs, or the 2d embedding columns of a periodic plan
 inline int packed_dims(const gp_plan* p) { return p->per_n ? 2 * p->d : p->d; }
 inline bool plan_is_tc(const gp_plan* p) {
@@ -416,6 +420,16 @@ inline bool plan_is_tc(const gp_plan* p) {
 }
 
 __host__ __device__ inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// Per-plan parameters of the covariance, passed by value to every kernel that evaluates it; only GP_RQ reads them (the other
+// kinds' code does not change with it).
+struct CovParam {
+  float alpha;    // RQ: alpha > 0
+  float ialpha;   // RQ: 1 / alpha, rounded once from fp64
+};
+inline CovParam cov_param(const gp_plan* p) {
+  return p->kind == GP_RQ ? CovParam{p->rq_alpha, (float)(1.0 / (double)p->rq_alpha)} : CovParam{0.f, 0.f};
+}
 
 // ---- device helpers -----------------------------------------------------------------------
 #if defined(__CUDACC__)
@@ -436,19 +450,76 @@ __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float((__fl
 // covariance from a = -0.5 |z_i - z_j|^2 in the pre-scaled units of pack.cu:
 //   RBF     z = (x - mean) sqrt(log2 e) / l      k = 2^a                (rbf_covariance.py:19)
 //   Matern  z = (x - mean) sqrt(4 nu) / l        rho^2 = -a = 2 nu r^2  (matern_covariance.py:21-47)
+//   RQ      z = (x - mean) / l               t = -a / alpha = r^2 / (2 alpha),  k = (1 + t)^-alpha   (rq_kernel.py)
 // internal "derivative kinds": the same tile loop evaluates g = l dk/dl (scalar lengthscale) instead of k, so that
 // the bilinear derivative  sum_ij (L_i . R_j) g_ij = sum_i L_i . (G R)_i  is one more fused K.V launch
 // (lazy_evaluated_kernel_tensor.py:69-105, functions/rbf_covariance.py:20-29, functions/matern_covariance.py:27-56)
-constexpr int GP_DERIV = 4;   // GP_DERIV + kind
+// GP_DERIV + kind covers the four RBF / Matern kinds only: its codes 4..7 are the template arguments of the existing derivative
+// instantiations (kmv_tc_kernel<4..7>).  The public GP_RQ = 4 is the same number, so it never reaches a template or a GP_DERIV +
+// kind switch: every dispatcher first maps a plan of kind GP_RQ to the RQ codes below (rq_code), which no other kind uses.
+constexpr int GP_DERIV = 4;   // GP_DERIV + kind, kind in GP_RBF .. GP_MATERN52
+constexpr int RQ_K = 16;      // RQ: k
+constexpr int RQ_DL = 17;     // RQ: l dk/dl (scalar lengthscale)
+constexpr int RQ_DA = 18;     // RQ: dk/dalpha
+__host__ __device__ constexpr bool is_rq_code(int code) { return code >= RQ_K && code <= RQ_DA; }
+// the code a dispatcher evaluates for `kind` on plan p: on an RQ plan GP_RQ (the plan's own kind) is RQ_K
+inline int rq_code(const gp_plan* p, int kind) { return (p->kind == GP_RQ && kind == GP_RQ) ? RQ_K : kind; }
+
+#if defined(__CUDACC__)
+__device__ __forceinline__ float lg2_approx(float x) {
+  float y;
+  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+#endif
+// RQ (DESIGN 4.20).  t = max(-a, 0) / alpha >= 0.  log2(1 + t) with an absolute error O(2^-24 t): the degree-6 Taylor polynomial of
+// log1p on the FMA pipe below 1/16 (truncation t^7 / 7 < 2^-26 t), MUFU lg2 above, selected without a branch; the rounding of
+// 1 + t and lg2's absolute error would otherwise be multiplied by alpha.  k = 2^(-alpha log2(1 + t)): two MUFU operations per entry.
+__device__ __forceinline__ float rq_t(float a, CovParam cp) { return fmaxf(-a, 0.f) * cp.ialpha; }
+#if defined(__CUDACC__)
+__device__ __forceinline__ float rq_lg2_1p(float t) {
+  float p = fmaf(t, -0.16666667f, 0.2f);
+  p = fmaf(t, p, -0.25f);
+  p = fmaf(t, p, 0.33333334f);
+  p = fmaf(t, p, -0.5f);
+  p = fmaf(t, p, 1.f);
+  const float small = LOG2E * (t * p);
+  const float big = lg2_approx(1.f + t);
+  return t < 0.0625f ? small : big;
+}
+__device__ __forceinline__ float rq_k(float t, CovParam cp) { return ex2_approx(-cp.alpha * rq_lg2_1p(t)); }
+// phi(t) = log1p(t) - t / (1 + t) = sum_{n>=2} (-1)^n (n-1)/n t^n  (dk/dalpha = -k phi) without cancellation: the series to n = 9
+// below 1/8 (truncation 1.8 t^8 relative), the difference of the accurate log1pf and t / (1 + t) above (cancels at most a factor 18)
+__device__ __forceinline__ float rq_phi(float t) {
+  float s = fmaf(t, -0.88888889f, 0.875f);
+  s = fmaf(t, s, -0.85714286f);
+  s = fmaf(t, s, 0.83333333f);
+  s = fmaf(t, s, -0.8f);
+  s = fmaf(t, s, 0.75f);
+  s = fmaf(t, s, -0.66666667f);
+  s = fmaf(t, s, 0.5f);
+  const float ser = (t * t) * s;
+  const float dif = log1pf(t) - __fdividef(t, 1.f + t);
+  return t < 0.125f ? ser : dif;
+}
+#endif
 
 template <int KIND>
-__device__ __forceinline__ float dcov_from_arg(float a, float* kout);
+__device__ __forceinline__ float dcov_from_arg(float a, float* kout, CovParam cp);
 
 template <int KIND>
-__device__ __forceinline__ float cov_from_arg(float a) {
-  if (KIND >= GP_DERIV) {
+__device__ __forceinline__ float cov_from_arg(float a, CovParam cp) {
+  if (KIND == RQ_K) {
+    return rq_k(rq_t(a, cp), cp);
+  } else if (KIND == RQ_DL) {
     float k;
-    return dcov_from_arg<KIND - GP_DERIV>(a, &k);
+    return dcov_from_arg<RQ_K>(a, &k, cp);
+  } else if (KIND == RQ_DA) {   // dk/dalpha = -k phi(t)
+    const float t = rq_t(a, cp);
+    return -rq_k(t, cp) * rq_phi(t);
+  } else if (KIND >= GP_DERIV) {
+    float k;
+    return dcov_from_arg<KIND - GP_DERIV>(a, &k, cp);
   } else if (KIND == GP_RBF) {
     return ex2_approx(fminf(a, 0.f));
   } else {
@@ -460,10 +531,15 @@ __device__ __forceinline__ float cov_from_arg(float a) {
   }
 }
 // derivative factor: dk/d(log-ish) pieces for the bilinear gradient.  Returns g with
-// dk/dl = g / l (scalar lengthscale):  RBF: sq*k ; M12: rho e ; M32: rho^2 e ; M52: (1+rho) rho^2/3 e
+// dk/dl = g / l (scalar lengthscale):  RBF: sq*k ; M12: rho e ; M32: rho^2 e ; M52: (1+rho) rho^2/3 e ; RQ: r^2 k / (1 + t)
 template <int KIND>
-__device__ __forceinline__ float dcov_from_arg(float a, float* kout) {
-  if (KIND == GP_RBF) {
+__device__ __forceinline__ float dcov_from_arg(float a, float* kout, CovParam cp) {
+  if (KIND == RQ_K) {
+    const float t = rq_t(a, cp);
+    const float k = rq_k(t, cp);
+    *kout = k;
+    return (-2.f * fminf(a, 0.f)) * __fdividef(k, 1.f + t);   // r^2 = -2 a in the packed units (C = 1)
+  } else if (KIND == GP_RBF) {
     float am = fminf(a, 0.f);
     float k = ex2_approx(am);
     *kout = k;
@@ -590,12 +666,15 @@ __device__ __forceinline__ float sm_pair(const SmHyp& h, const float* za, const 
 }
 SmHyp spectral_hyp(const gp_plan* p);   // spectral.cu: the kernel argument of a spectral plan
 // input-derivative factor q = dk/da of the same covariance (xgrad.cu): dk/dz_i = -q (z_i - z_j) in the packed units.
-//   RBF: ln2 2^a ; M12: e / (2 rho) ; M32: e / 2 ; M52: (1 + rho) e / 6      (e = exp(-rho), rho^2 = -a)
+//   RBF: ln2 2^a ; M12: e / (2 rho) ; M32: e / 2 ; M52: (1 + rho) e / 6 ; RQ: k / (1 + t)      (e = exp(-rho), rho^2 = -a)
 // q is the h of the raw-unit form  dk/dx_i = -h (x_i - x_j) / l^2  times l^2 / C (C = log2 e, 2, 6, 10 as in pack.cu).  A pair at
 // distance 0 contributes 0 (its direction is 0; Matern-1/2's q is unbounded there): the caller masks a == 0.
 template <int KIND>
-__device__ __forceinline__ float hcov_from_arg(float a) {
-  if (KIND == GP_RBF) {
+__device__ __forceinline__ float hcov_from_arg(float a, CovParam cp) {
+  if (KIND == RQ_K) {
+    const float t = rq_t(a, cp);
+    return __fdividef(rq_k(t, cp), 1.f + t);
+  } else if (KIND == GP_RBF) {
     return 0.69314718f * ex2_approx(fminf(a, 0.f));
   } else {
     float rho = sqrt_approx(fmaxf(-a, 0.f));

@@ -13,10 +13,10 @@ namespace gp {
 
 // grid (row blocks, nsplit); 128 threads, one output row each; partial[split][row][16]
 template <int KIND, int DP>
-__global__ void __launch_bounds__(SIMT_TI)
-kmv_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ V16,
-                float* __restrict__ partial, int64_t n1, int64_t n2, int64_t rows_pad, int64_t cols_per_split,
-                int same, int64_t row_begin, const int* __restrict__ done_flag) {
+__device__ __forceinline__ void kmv_simt_body(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ V16,
+                                              float* __restrict__ partial, int64_t n1, int64_t n2, int64_t rows_pad,
+                                              int64_t cols_per_split, int same, int64_t row_begin, const int* __restrict__ done_flag,
+                                              CovParam cp) {
   if (done_flag && *done_flag) return;
   __shared__ __align__(16) float zj[SIMT_TJ][DP];
   __shared__ __align__(16) float vj[SIMT_TJ][TP];
@@ -56,7 +56,7 @@ kmv_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
       }
       float a = -0.5f * s;
       if (same && (j0 + jj) == gi) a = 0.f;  // exact diagonal (kernel.py:44-45)
-      float k = cov_from_arg<KIND>(a);
+      float k = cov_from_arg<KIND>(a, cp);
 #pragma unroll
       for (int c = 0; c < TP; ++c) acc[c] = fmaf(k, vj[jj][c], acc[c]);
     }
@@ -66,6 +66,21 @@ kmv_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
 #pragma unroll
     for (int q = 0; q < 4; ++q) dst[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
   }
+}
+template <int KIND, int DP>
+__global__ void __launch_bounds__(SIMT_TI)
+kmv_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ V16,
+                float* __restrict__ partial, int64_t n1, int64_t n2, int64_t rows_pad, int64_t cols_per_split,
+                int same, int64_t row_begin, const int* __restrict__ done_flag) {
+  kmv_simt_body<KIND, DP>(Z1, Z2, V16, partial, n1, n2, rows_pad, cols_per_split, same, row_begin, done_flag, CovParam{});
+}
+// the RQ kernel with its per-plan alpha
+template <int DP>
+__global__ void __launch_bounds__(SIMT_TI)
+rq_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ V16,
+               float* __restrict__ partial, int64_t n1, int64_t n2, int64_t rows_pad, int64_t cols_per_split,
+               int same, int64_t row_begin, const int* __restrict__ done_flag, CovParam cp) {
+  kmv_simt_body<RQ_K, DP>(Z1, Z2, V16, partial, n1, n2, rows_pad, cols_per_split, same, row_begin, done_flag, cp);
 }
 
 struct SimtLaunch {
@@ -83,9 +98,14 @@ static int launch_simt_kind(gp_plan* p, const SimtLaunch& a, const int* done_fla
   dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)a.nsplit);
 #define GP_SIMT_CASE(D)                                                                                          \
   case D:                                                                                                        \
-    kmv_simt_kernel<KIND, D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count,        \
-                                                              a.n2, rows_pad, a.cps, p->same ? 1 : 0,            \
-                                                              a.row_begin, done_flag);                           \
+    if constexpr (KIND == RQ_K)                                                                                  \
+      rq_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2,       \
+                                                         rows_pad, a.cps, p->same ? 1 : 0, a.row_begin, done_flag, \
+                                                         cov_param(p));                                          \
+    else                                                                                                         \
+      kmv_simt_kernel<KIND, D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count,      \
+                                                                a.n2, rows_pad, a.cps, p->same ? 1 : 0,          \
+                                                                a.row_begin, done_flag);                         \
     break;
   switch (p->DP) {
     GP_SIMT_CASE(4) GP_SIMT_CASE(8) GP_SIMT_CASE(12) GP_SIMT_CASE(16) GP_SIMT_CASE(24) GP_SIMT_CASE(32)
@@ -101,11 +121,12 @@ static int launch_simt_kind(gp_plan* p, const SimtLaunch& a, const int* done_fla
 }
 
 static int launch_simt_any(gp_plan* p, int kind, const SimtLaunch& a, const int* done_flag) {
-  switch (kind) {
+  switch (rq_code(p, kind)) {
     case GP_RBF: return launch_simt_kind<GP_RBF>(p, a, done_flag);
     case GP_MATERN12: return launch_simt_kind<GP_MATERN12>(p, a, done_flag);
     case GP_MATERN32: return launch_simt_kind<GP_MATERN32>(p, a, done_flag);
     case GP_MATERN52: return launch_simt_kind<GP_MATERN52>(p, a, done_flag);
+    case RQ_K: return launch_simt_kind<RQ_K>(p, a, done_flag);
   }
   set_error("bad kernel kind %d", kind);
   return GP_E_SHAPE;
@@ -192,7 +213,7 @@ int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t
 template <int KIND>
 __global__ void krows_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP,
                              const int64_t* __restrict__ idx, int64_t n1_local, int64_t n2, float os, int same,
-                             int64_t row_begin, float* __restrict__ OUT, int64_t ldo, const int* __restrict__ xbad) {
+                             int64_t row_begin, float* __restrict__ OUT, int64_t ldo, const int* __restrict__ xbad, CovParam cp) {
   extern __shared__ float zi[];
   const int64_t r = blockIdx.y;
   const int64_t i = idx[r];
@@ -214,14 +235,14 @@ __global__ void krows_kernel(const float* __restrict__ Z1, const float* __restri
   }
   float a = -0.5f * s;
   if (same && (i + row_begin) == j) a = 0.f;
-  OUT[r * ldo + j] = os * cov_from_arg<KIND>(a);
+  OUT[r * ldo + j] = os * cov_from_arg<KIND>(a, cp);
 }
 
 // diagonal of a cross-covariance K(x1, x2) (n1 == n2): OUT[i] = os * k(x1_i, x2_i)   (kernel(x1, x2, diag=True),
 // lazy_evaluated_kernel_tensor.py:107-133 / kernels/kernel.py:307-352 with diag=True)
 template <int KIND>
 __global__ void kdiag_cross_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP, int64_t n, float os,
-                                   float* __restrict__ OUT) {
+                                   float* __restrict__ OUT, CovParam cp) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float s = 0.f;
@@ -229,7 +250,7 @@ __global__ void kdiag_cross_kernel(const float* __restrict__ Z1, const float* __
     float df = Z1[i * DP + c] - Z2[i * DP + c];
     s = fmaf(df, df, s);
   }
-  OUT[i] = os * cov_from_arg<KIND>(-0.5f * s);
+  OUT[i] = os * cov_from_arg<KIND>(-0.5f * s, cp);
 }
 
 __global__ void fill_kernel(float* __restrict__ p, int64_t n, float v) {
@@ -241,11 +262,13 @@ __global__ void fill_kernel(float* __restrict__ p, int64_t n, float v) {
 // grid (row blocks, col splits); per-thread row, staged columns; outputs per block partial sums
 //   gout[block][0]      = sum_ij w_ij k_ij                 (-> d/d outputscale)
 //   gout[block][1 + c]  = sum_ij w_ij g_ij (z_ic-z_jc)^2   (ARD)  or  gout[block][1] = sum w_ij g_ij (scalar l)
+//   RQ: gout[block][1 + n_ls] = sum_ij w_ij dk_ij/dalpha    (n_ls = d (ARD) or 1)
 template <int KIND, int DP, bool ARD>
 __global__ void __launch_bounds__(SIMT_TI)
 bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ L16,
                 const float* __restrict__ R16, int64_t n1, int64_t n2, int64_t cols_per_split, int same,
-                int64_t row_begin, int d, double* __restrict__ gout, int gstride) {
+                int64_t row_begin, int d, double* __restrict__ gout, int gstride, CovParam cp) {
+  constexpr bool RQ = KIND == RQ_K;
   __shared__ __align__(16) float zj[SIMT_TJ][DP];
   __shared__ __align__(16) float rj[SIMT_TJ][TP];
   const int tid = threadIdx.x;
@@ -259,7 +282,7 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
 #pragma unroll
   for (int c = 0; c < TP; ++c) li[c] = rv ? L16[i * TP + c] : 0.f;
   constexpr int NG = ARD ? DP : 1;
-  float gk = 0.f, gl[NG];
+  float gk = 0.f, gl[NG], ga = 0.f;
 #pragma unroll
   for (int c = 0; c < NG; ++c) gl[c] = 0.f;
   const int64_t gi = i + row_begin;
@@ -284,8 +307,9 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
       float a = -0.5f * s;
       if (same && (j0 + jj) == gi) a = 0.f;
       float k;
-      float g = dcov_from_arg<KIND>(a, &k);
+      float g = dcov_from_arg<KIND>(a, &k, cp);
       gk = fmaf(w, k, gk);
+      if (RQ) ga = fmaf(w, -k * rq_phi(rq_t(a, cp)), ga);
       if (ARD) {
         // dk/dl_c = g * (z_ic - z_jc)^2 / (s * l_c)   (g/l is the scalar-lengthscale derivative)
         float gs = (s > 0.f) ? w * g / s : 0.f;
@@ -298,7 +322,8 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
   }
   // block reduction in double
   __shared__ double red[SIMT_TI];
-  const int nout = 1 + (ARD ? d : 1);
+  const int nls = ARD ? d : 1;
+  const int nout = 1 + nls + (RQ ? 1 : 0);
   const int64_t blk = (int64_t)blockIdx.y * gridDim.x + blockIdx.x;
   for (int o = 0; o < nout; ++o) {
     float v = (o == 0) ? gk : 0.f;
@@ -307,6 +332,7 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
       for (int c = 0; c < NG; ++c)
         if (c == o - 1) v = gl[c];
     }
+    if (RQ && o == 1 + nls) v = ga;   // after the loop: an ARD thread holds DP >= d + 1 (padding) accumulators
     __syncthreads();
     red[tid] = (double)v;
     __syncthreads();
@@ -367,7 +393,7 @@ static int launch_bilinear(gp_plan* p, const BilinLaunch& a, const float* L16, c
 #define GP_BL_CASE(D)                                                                                              \
   case D:                                                                                                          \
     bilinear_kernel<KIND, D, ARD><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, L16, R16, p->row_count, a.n2, cps,  \
-                                                                   p->same ? 1 : 0, a.row_begin, p->d, gout, gstride); \
+                                                                   p->same ? 1 : 0, a.row_begin, p->d, gout, gstride, cov_param(p)); \
     break;
   switch (p->DP) {   // DP <= 64: gp_bilinear_grad refuses wider plans before any launch
     GP_BL_CASE(4) GP_BL_CASE(8) GP_BL_CASE(12) GP_BL_CASE(16) GP_BL_CASE(24) GP_BL_CASE(32) GP_BL_CASE(48) GP_BL_CASE(64)
@@ -394,6 +420,7 @@ static int launch_bilinear_any(gp_plan* p, const BilinLaunch& a, const float* L1
     case GP_RBF: return launch_bilinear<GP_RBF, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
     case GP_MATERN12: return launch_bilinear<GP_MATERN12, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
     case GP_MATERN32: return launch_bilinear<GP_MATERN32, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
+    case GP_RQ: return launch_bilinear<RQ_K, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
     default: return launch_bilinear<GP_MATERN52, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
   }
 }
@@ -445,12 +472,16 @@ static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int
   const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
   dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
   size_t sh = sizeof(float) * p->DP;
+  const CovParam cp = cov_param(p);
+#define GP_KROWS(KK) krows_kernel<KK><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad, cp)
   switch (p->kind) {
-    case GP_RBF: krows_kernel<GP_RBF><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
-    case GP_MATERN12: krows_kernel<GP_MATERN12><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
-    case GP_MATERN32: krows_kernel<GP_MATERN32><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
-    default: krows_kernel<GP_MATERN52><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad); break;
+    case GP_RBF: GP_KROWS(GP_RBF); break;
+    case GP_MATERN12: GP_KROWS(GP_MATERN12); break;
+    case GP_MATERN32: GP_KROWS(GP_MATERN32); break;
+    case GP_RQ: GP_KROWS(RQ_K); break;
+    default: GP_KROWS(GP_MATERN52); break;
   }
+#undef GP_KROWS
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -496,12 +527,16 @@ static int kdiag_base(gp_plan* p, float* OUT) {
     const unsigned g = (unsigned)cdiv(p->n1, 256);
     const float* Z1 = p->Z1.as<float>();
     const float* Z2 = p->Z2.as<float>();
+    const CovParam cp = cov_param(p);
+#define GP_KDIAG(KK) kdiag_cross_kernel<KK><<<g, 256, 0, p->stream>>>(Z1, Z2, p->DP, p->n1, p->outputscale, OUT, cp)
     switch (p->kind) {
-      case GP_RBF: kdiag_cross_kernel<GP_RBF><<<g, 256, 0, p->stream>>>(Z1, Z2, p->DP, p->n1, p->outputscale, OUT); break;
-      case GP_MATERN12: kdiag_cross_kernel<GP_MATERN12><<<g, 256, 0, p->stream>>>(Z1, Z2, p->DP, p->n1, p->outputscale, OUT); break;
-      case GP_MATERN32: kdiag_cross_kernel<GP_MATERN32><<<g, 256, 0, p->stream>>>(Z1, Z2, p->DP, p->n1, p->outputscale, OUT); break;
-      default: kdiag_cross_kernel<GP_MATERN52><<<g, 256, 0, p->stream>>>(Z1, Z2, p->DP, p->n1, p->outputscale, OUT); break;
+      case GP_RBF: GP_KDIAG(GP_RBF); break;
+      case GP_MATERN12: GP_KDIAG(GP_MATERN12); break;
+      case GP_MATERN32: GP_KDIAG(GP_MATERN32); break;
+      case GP_RQ: GP_KDIAG(RQ_K); break;
+      default: GP_KDIAG(GP_MATERN52); break;
     }
+#undef GP_KDIAG
   }
   p->launches++;
   GP_CUDA(cudaGetLastError());
@@ -548,7 +583,9 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
     }
     return GP_OK;
   }
-  const int nout = 1 + (ard ? p->d : 1);
+  const bool rq = p->kind == GP_RQ;   // one more output: dF/dalpha
+  const int nls = ard ? p->d : 1;
+  const int nout = 1 + nls + (rq ? 1 : 0);
   std::vector<double> total(nout, 0.0);
   if (p->tasks && (ard || p->backend != GP_BACKEND_TCGEN05)) {
     // K o B on the SIMT derivative kernel: one pass per column task with B folded into the rows (tasks.cu)
@@ -571,8 +608,8 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
     double* gout = p->misc.as<double>();
     double* gsum = gout + nblk * nout;
     // scalar lengthscale on the tensor-core backend: sum_ij (L_i . R_j) f_ij = sum_i L_i . (F R)_i, i.e. two launches of
-    // the fused K.V kernel (f = k, then f = g = l dk/dl through the derivative kinds) + a dot product with L.  ARD needs d
-    // weighted sums per pair and stays on the SIMT kernel.
+    // the fused K.V kernel (f = k, then f = g = l dk/dl through the derivative kinds) + a dot product with L; an RQ plan adds a
+    // third (f = dk/dalpha).  ARD needs d weighted sums per pair and stays on the SIMT kernel.
     const bool use_tc = !ard && p->backend == GP_BACKEND_TCGEN05;
     const int64_t rows_pad = p->rows_pad;
     const int dot_blocks = (int)std::min<int64_t>(nblk, 2 * p->n_sm);
@@ -582,8 +619,8 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
       GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
       if (use_tc) {
         if (!p->tasks) GP_CHECK(pack_v_tiles(p, p->misc3.as<float>()));
-        for (int pass = 0; pass < 2; ++pass) {
-          const int kind = pass == 0 ? p->kind : GP_DERIV + p->kind;
+        for (int pass = 0; pass < nout; ++pass) {
+          const int kind = pass == 0 ? p->kind : !rq ? GP_DERIV + p->kind : pass == 1 ? RQ_DL : RQ_DA;
           // a multitask plan runs both passes on K o B (tasks.cu), combined into slot 0 in user row order
           GP_CHECK(p->tasks ? tasks_kmv_partials(p, p->misc3.as<float>(), kind, nullptr) : kmv_tc_launch_kind(p, kind, nullptr));
           bilin_dot_kernel<<<dot_blocks, 256, 0, p->stream>>>(p->partial.as<float>(), p->nparts, p->row_count, rows_pad,
@@ -616,5 +653,6 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
     for (int c = 0; c < p->d; ++c) grad_ls[c] = p->outputscale * total[1 + c] / (double)p->ls[c];
   else
     grad_ls[0] = p->outputscale * total[1] / (double)p->ls[0];
+  if (rq) grad_ls[nls] = p->outputscale * total[1 + nls];   // [dF/dl | dF/dalpha]
   return GP_OK;
 }

@@ -38,7 +38,7 @@
 // The same pipeline (tc_pipeline) also runs the product of two tensor-core factors (product_tc_kernel, product.cu): a second
 // GEMM1 operand with its own A tile and its own B tile per stage, a second GEMM1 chain in the same batch (S_b into hi, dead once
 // GEMM2 of the previous tile has read P_hi, so the live set stays s, hi, o1, o2, acc) and the product covariance in the
-// epilogue.  What a kernel computes per entry is its covariance source (TcOne, TcProduct); the protocol exists once.
+// epilogue.  What a kernel computes per entry is its covariance source (TcOne, TcRq, TcProduct); the protocol exists once.
 #include "gp_common.cuh"
 #include "tc_ptx.cuh"
 
@@ -65,7 +65,7 @@ __device__ __forceinline__ float cov_tc(float a) {
   // points.  GEMM1 forms a = z_i.z_j + n_i + n_j, so that rounding is up to (1 + KP/4) 2^-21 (|z_i|^2 + |z_j|^2), a few 1e-6
   // for unit-cube data but more for inputs spanning many lengthscales (DESIGN 4.1); k then exceeds 1 by as much relative,
   // which the entry bound of tests/kmv_oracle.py allows for.  The exact diagonal is forced to a = 0 in diagonal tiles.
-  return (KIND == GP_RBF) ? ex2_approx(a) : cov_from_arg<KIND>(a);
+  return (KIND == GP_RBF) ? ex2_approx(a) : cov_from_arg<KIND>(a, CovParam{});
 }
 
 // Covariance sources of the pipeline.  TWO: a second GEMM1 operand (S_b into hi); pair(a, b): the covariance of one entry from
@@ -74,6 +74,12 @@ template <int KIND>
 struct TcOne {   // one operand of kind KIND (GP_DERIV + kind: l dk/dl for gp_bilinear_grad)
   static constexpr bool TWO = false;
   __device__ __forceinline__ float pair(float a, float) const { return cov_tc<KIND>(a); }
+};
+template <int KIND>
+struct TcRq {    // the RQ kernel: KIND = RQ_K (k), RQ_DL (l dk/dl) or RQ_DA (dk/dalpha); lg2 + ex2 per entry
+  static constexpr bool TWO = false;
+  CovParam cp;
+  __device__ __forceinline__ float pair(float a, float) const { return cov_from_arg<KIND>(a, cp); }
 };
 template <bool RBF_A, bool RBF_B>
 struct TcProduct {   // k_a k_b = poly_a poly_b ex2(e_a + e_b): one ex2 per entry (cov_poly_exp, gp_common.cuh)
@@ -313,6 +319,16 @@ kmv_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const 
               done_flag);
 }
 
+// the RQ kernel (CODE = RQ_K, RQ_DL or RQ_DA) with its per-plan alpha
+template <int CODE>
+__global__ void __maxnreg__(128)
+rq_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const float* __restrict__ Vt,
+             float* __restrict__ partial, int KP, int NS, int64_t ntile_j, int64_t tiles_per_split,
+             int64_t rows_pad, int same, int64_t row_begin, const int* __restrict__ done_flag, CovParam cp) {
+  tc_pipeline(TcRq<CODE>{cp}, XA, nullptr, XB, nullptr, Vt, partial, KP, 0, NS, ntile_j, tiles_per_split, rows_pad, same, row_begin,
+              done_flag);
+}
+
 // two factors of a kernel product (product.cu), each from its own packed tiles XA_f / XB_f of width KP_f
 template <bool RBF_A, bool RBF_B>
 __global__ void __maxnreg__(128)
@@ -349,16 +365,32 @@ static int launch_tc_kind(gp_plan* p, const TcLaunch& a, const int* done_flag) {
   int ns = 0;
   int smem_bytes = tc_smem_bytes(p->KP, &ns);
   GP_REQUIRE(ns >= 2, GP_E_SHAPE, "tensor-core path: smem ring too small for KP=%d", p->KP);
-  GP_CHECK(opt_in_smem<kmv_tc_kernel<KIND>>(p->device, 227 * 1024));
   dim3 grid((unsigned)p->ntile_i, (unsigned)a.nsplit);
-  kmv_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
-      a.XA, a.XB, a.Vt, a.partial, p->KP, ns, a.ntile_j, a.tiles_per_split, p->rows_pad, p->same ? 1 : 0, a.row_begin, done_flag);
+  if constexpr (is_rq_code(KIND)) {
+    GP_CHECK(opt_in_smem<rq_tc_kernel<KIND>>(p->device, 227 * 1024));
+    rq_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
+        a.XA, a.XB, a.Vt, a.partial, p->KP, ns, a.ntile_j, a.tiles_per_split, p->rows_pad, p->same ? 1 : 0, a.row_begin, done_flag,
+        cov_param(p));
+  } else {
+    GP_CHECK(opt_in_smem<kmv_tc_kernel<KIND>>(p->device, 227 * 1024));
+    kmv_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
+        a.XA, a.XB, a.Vt, a.partial, p->KP, ns, a.ntile_j, a.tiles_per_split, p->rows_pad, p->same ? 1 : 0, a.row_begin, done_flag);
+  }
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
 
 static int launch_tc_any(gp_plan* p, int kind, const TcLaunch& a, const int* done_flag) {
+  if (p->kind == GP_RQ) {   // the plan's kind first: GP_RQ is the number of GP_DERIV + GP_RBF
+    switch (rq_code(p, kind)) {
+      case RQ_K: return launch_tc_kind<RQ_K>(p, a, done_flag);
+      case RQ_DL: return launch_tc_kind<RQ_DL>(p, a, done_flag);
+      case RQ_DA: return launch_tc_kind<RQ_DA>(p, a, done_flag);
+    }
+    set_error("bad kernel code %d for a rational quadratic plan", kind);
+    return GP_E_SHAPE;
+  }
   switch (kind) {
     case GP_RBF: return launch_tc_kind<GP_RBF>(p, a, done_flag);
     case GP_MATERN12: return launch_tc_kind<GP_MATERN12>(p, a, done_flag);

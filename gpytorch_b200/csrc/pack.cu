@@ -203,7 +203,9 @@ int pack_inputs(gp_plan* p) {
   GP_CHECK(p->scale.ensure(sizeof(float) * d));
   // scale_c = sqrt(const) / l_c
   std::vector<float> sc(d);
-  double cst = (p->kind == GP_RBF) ? 1.4426950408889634 : (p->kind == GP_MATERN12 ? 2.0 : (p->kind == GP_MATERN32 ? 6.0 : 10.0));
+  // RQ: C = 1 (alpha stays out of the packing, so the value and both derivatives read the same a = -r^2 / 2)
+  double cst = (p->kind == GP_RBF) ? 1.4426950408889634
+               : (p->kind == GP_MATERN12 ? 2.0 : (p->kind == GP_MATERN32 ? 6.0 : (p->kind == GP_RQ ? 1.0 : 10.0)));
   for (int c = 0; c < d; ++c) {
     double l = (p->ls.size() == 1) ? p->ls[0] : p->ls[c];
     sc[c] = (float)(sqrt(cst) / l);

@@ -41,7 +41,7 @@ template <int KIND>
 __global__ void __launch_bounds__(PC_THREADS)
 pc_step_kernel(const float* __restrict__ Z, int DP, float os, float* __restrict__ Lt, int64_t n, int m, int max_rank,
                float tol, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos, PcState* __restrict__ st,
-               int64_t* __restrict__ piv_out, float* __restrict__ pval, int* __restrict__ ppos, double* __restrict__ psum) {
+               int64_t* __restrict__ piv_out, float* __restrict__ pval, int* __restrict__ ppos, double* __restrict__ psum, CovParam cp) {
   if (st->done) return;
   extern __shared__ float sh[];
   float* zp = sh;           // [DP]
@@ -73,7 +73,7 @@ pc_step_kernel(const float* __restrict__ Z, int DP, float os, float* __restrict_
         float df = zp[c] - Z[j * DP + c];
         s = fmaf(df, df, s);
       }
-      float v = os * cov_from_arg<KIND>(-0.5f * s);
+      float v = os * cov_from_arg<KIND>(-0.5f * s, cp);
       {
         // independent partial sums keep 8 L2 loads in flight per thread (the step is latency bound, not bandwidth bound)
         float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -216,14 +216,16 @@ struct PcTerms {
   const DerivHyp* dh;   // PC_KIND_DERIV / PC_KIND_M52GRAD
   AddHyp ah;            // PC_KIND_ADDITIVE
   SmHyp sh;             // PC_KIND_SPECTRAL
+  CovParam cp[4];       // each term's (PC_KIND_SUM) or the plain plan's (cp[0]) covariance parameters: an RQ term's alpha
 };
 __device__ __forceinline__ int pc_task_of(const PcTerms& tt, int r) { return tt.task ? tt.task[r] : r % tt.rep; }
-__device__ __forceinline__ float pc_cov_rt(int kind, float a) {
+__device__ __forceinline__ float pc_cov_rt(int kind, float a, CovParam cp) {
   switch (kind) {
-    case GP_RBF: return cov_from_arg<GP_RBF>(a);
-    case GP_MATERN12: return cov_from_arg<GP_MATERN12>(a);
-    case GP_MATERN32: return cov_from_arg<GP_MATERN32>(a);
-    default: return cov_from_arg<GP_MATERN52>(a);
+    case GP_RBF: return cov_from_arg<GP_RBF>(a, cp);
+    case GP_MATERN12: return cov_from_arg<GP_MATERN12>(a, cp);
+    case GP_MATERN32: return cov_from_arg<GP_MATERN32>(a, cp);
+    case GP_RQ: return cov_from_arg<RQ_K>(a, cp);
+    default: return cov_from_arg<GP_MATERN52>(a, cp);
   }
 }
 
@@ -303,7 +305,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
               float df = zp[off + c] - zj[c];
               s = fmaf(df, df, s);
             }
-            v = fmaf(tt.os[t], pc_cov_rt(tt.kind[t], -0.5f * s), v);
+            v = fmaf(tt.os[t], pc_cov_rt(tt.kind[t], -0.5f * s, tt.cp[t]), v);
             off += tt.DP[t];
           }
         } else if (KIND == PC_KIND_PRODUCT) {
@@ -316,7 +318,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
               float df = zp[off + c] - zj[c];
               s = fmaf(df, df, s);
             }
-            v *= pc_cov_rt(tt.kind[t], -0.5f * s);
+            v *= pc_cov_rt(tt.kind[t], -0.5f * s, CovParam{});
             off += tt.DP[t];
           }
         } else if (KIND == PC_KIND_SKI) {
@@ -332,7 +334,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             float df = zp[c] - zj[c];
             s = fmaf(df, df, s);
           }
-          v = os * tt.B[pc_task_of(tt, pi) * tt.T + pc_task_of(tt, (int)j)] * pc_cov_rt(tt.kind[0], -0.5f * s);
+          v = os * tt.B[pc_task_of(tt, pi) * tt.T + pc_task_of(tt, (int)j)] * pc_cov_rt(tt.kind[0], -0.5f * s, CovParam{});
         } else if (KIND == PC_KIND_DERIV || KIND == PC_KIND_M52GRAD) {
           using K = DerivTable<KIND == PC_KIND_M52GRAD ? GP_MATERN52 : GP_RBF>;
           const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
@@ -351,7 +353,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             float df = zp[c] - Z[j * DP + c];
             s = fmaf(df, df, s);
           }
-          v = os * cov_from_arg<(KIND >= PC_KIND_SUM ? GP_RBF : KIND)>(-0.5f * s);
+          v = os * cov_from_arg<(KIND >= PC_KIND_SUM ? GP_RBF : KIND)>(-0.5f * s, tt.cp[0]);
         }
         {
           float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -848,11 +850,14 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     tt.n = (int)p->terms.size();
     for (int t = 0; t < tt.n; ++t) {
       const gp_plan* q = p->terms[t];
-      tt.kind[t] = q->kind; tt.DP[t] = q->DP; tt.os[t] = q->outputscale; tt.Z[t] = q->Z2.as<float>();
+      tt.kind[t] = q->kind; tt.DP[t] = q->DP; tt.os[t] = q->outputscale; tt.Z[t] = q->Z2.as<float>(); tt.cp[t] = cov_param(q);
       os_total += q->outputscale;
       dp_total += q->DP;
     }
-  } else if (prod) {   // os_total = S, dp_total = the factors' widths back to back (product_pack)
+  } else {
+    tt.cp[0] = cov_param(p);
+  }
+  if (prod) {   // os_total = S, dp_total = the factors' widths back to back (product_pack)
     tt.n = (int)p->factors.size();
     for (int t = 0; t < tt.n; ++t) {
       const gp_plan* q = p->factors[t];
@@ -930,6 +935,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
       case GP_MATERN12: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN12>; break;
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
+      case GP_RQ: fn1 = (const void*)pc_persistent1_kernel<RQ_K>; break;
       case PC_KIND_SUM: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SUM>; break;
       case PC_KIND_PRODUCT: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_PRODUCT>; break;
       case PC_KIND_SKI: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SKI>; break;
@@ -951,8 +957,9 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   } else {
   for (int m = 0; m < rank; ++m) {
     size_t sh = sizeof(float) * (p->DP + m);
-#define GP_PC_LAUNCH(KK) pc_step_kernel<KK><<<gb, PC_THREADS, sh, st>>>(Z, p->DP, p->outputscale, Lt, n, m, rank, error_tol, diag, perm, pos, S, piv, pval, ppos, psum)
+#define GP_PC_LAUNCH(KK) pc_step_kernel<KK><<<gb, PC_THREADS, sh, st>>>(Z, p->DP, p->outputscale, Lt, n, m, rank, error_tol, diag, perm, pos, S, piv, pval, ppos, psum, cov_param(p))
     switch (p->kind) {
+      case GP_RQ: GP_PC_LAUNCH(RQ_K); break;
       case GP_RBF: GP_PC_LAUNCH(GP_RBF); break;
       case GP_MATERN12: GP_PC_LAUNCH(GP_MATERN12); break;
       case GP_MATERN32: GP_PC_LAUNCH(GP_MATERN32); break;

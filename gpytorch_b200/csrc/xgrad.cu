@@ -28,7 +28,7 @@ template <int KIND, int DP, int TW>
 __global__ void __launch_bounds__(SIMT_TI)
 xgrad_kernel(const float* __restrict__ Zo, const float* __restrict__ Zt, int64_t no, int64_t nt,
              const float* __restrict__ Lo, const float* __restrict__ Rt, const float* __restrict__ W, int64_t sr, int64_t sc,
-             int sym, int64_t cols_per_split, int accumulate, float* __restrict__ partial) {
+             int sym, int64_t cols_per_split, int accumulate, float* __restrict__ partial, CovParam cp) {
   constexpr int TWS = TW > 0 ? TW : 1;
   __shared__ __align__(16) float zj[SIMT_TJ][DP];
   __shared__ __align__(16) float rj[SIMT_TJ][TWS];
@@ -75,7 +75,7 @@ xgrad_kernel(const float* __restrict__ Zo, const float* __restrict__ Zt, int64_t
       const float a = -0.5f * s;
       // distance 0 (coinciding points, the diagonal of a square plan) contributes 0; a NaN argument fails the test too and is
       // reported through the plan's xbad flag by the finish kernel
-      const float wq = (a < 0.f) ? w * hcov_from_arg<KIND>(a) : 0.f;
+      const float wq = (a < 0.f) ? w * hcov_from_arg<KIND>(a, cp) : 0.f;
 #pragma unroll
       for (int c = 0; c < DP; ++c) acc[c] = fmaf(wq, zi[c] - zj[jj][c], acc[c]);
     }
@@ -133,7 +133,7 @@ static int launch_xgrad(gp_plan* p, dim3 grid, const XgArgs& a) {
 #define GP_XG_CASE(D)                                                                                                     \
   case D:                                                                                                                 \
     xgrad_kernel<KIND, D, TW><<<grid, SIMT_TI, 0, p->stream>>>(a.Zo, a.Zt, a.no, a.nt, a.Lo, a.Rt, a.W, a.sr, a.sc, a.sym, \
-                                                               a.cps, a.accumulate, a.partial);                           \
+                                                               a.cps, a.accumulate, a.partial, cov_param(p));             \
     break;
   switch (p->DP) {
     GP_XG_CASE(4) GP_XG_CASE(8) GP_XG_CASE(12) GP_XG_CASE(16) GP_XG_CASE(24) GP_XG_CASE(32) GP_XG_CASE(48) GP_XG_CASE(64)
@@ -154,6 +154,7 @@ static int launch_xgrad_kind(gp_plan* p, dim3 grid, const XgArgs& a) {
     case GP_MATERN12: return launch_xgrad<GP_MATERN12, TW>(p, grid, a);
     case GP_MATERN32: return launch_xgrad<GP_MATERN32, TW>(p, grid, a);
     case GP_MATERN52: return launch_xgrad<GP_MATERN52, TW>(p, grid, a);
+    case GP_RQ: return launch_xgrad<RQ_K, TW>(p, grid, a);
   }
   set_error("bad kernel kind %d", p->kind);
   return GP_E_SHAPE;

@@ -119,6 +119,19 @@ class Plan:
             check(self.lib.gp_plan_set_hypers(self._h, KIND[kind], arr, len(ls), float(outputscale), float(noise)))
         # recorded once the engine took them: bilinear_grad sizes its output by these lengthscales
         self.kind, self.lengthscale, self.outputscale, self.noise = kind, ls, float(outputscale), float(noise)
+        self.alpha = None
+        return self
+
+    def set_hypers_rq(self, lengthscale, alpha: float, outputscale: float = 1.0, noise: float = 0.0):
+        """Rational quadratic kernel S (1 + r^2 / (2 alpha))^-alpha (gp_plan_set_hypers_rq): kind, lengthscales (1 or d), alpha,
+        outputscale and noise in one engine call.  bilinear_grad then returns [dl (1 or d) | dalpha] and dF/dS."""
+        ls = [float(v) for v in (lengthscale if hasattr(lengthscale, "__len__") else [lengthscale])]
+        arr = (C.c_float * len(ls))(*ls)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_hypers_rq(self._h, arr, len(ls), float(alpha), float(outputscale), float(noise)))
+        # recorded once the engine took them: bilinear_grad sizes its output by the lengthscales and alpha
+        self.kind, self.lengthscale, self.outputscale, self.noise = "rq", ls, float(outputscale), float(noise)
+        self.alpha = float(alpha)
         return self
 
     def set_ski(self, grid_sizes, grid_lo, grid_step):
@@ -382,7 +395,8 @@ class Plan:
         """(d/d lengthscale[*], d/d outputscale) of sum(left * (K @ right)) for left [row_count, s], right [n2, s].  On a kernel
         product: the factors' lengthscale gradients one after the other, and the gradient of the combined scale S.  On an additive
         plan: the D lengthscale gradients and the list of the D component-scale gradients.  On a spectral plan: the Q (1 + 2d)
-        gradients [dw | dmu | dv] and dF/dS.  On a periodic plan: [dl | dp] and dF/dS."""
+        gradients [dw | dmu | dv] and dF/dS.  On a periodic plan: [dl | dp] and dF/dS.  On a rational quadratic plan: [dl | dalpha]
+        and dF/dS."""
         if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.row_count or right.size(0) != self.n2 \
                 or left.size(1) != right.size(1) or left.size(1) < 1:
             raise RuntimeError(f"bilinear_grad: left must be [{self.row_count}, s] and right [{self.n2}, s] with s >= 1 "
@@ -396,6 +410,8 @@ class Plan:
         s = left.size(1)
         factors = getattr(self, "_factors", None)
         nls = sum(len(f.lengthscale) for f in factors) if factors else len(self.lengthscale)
+        if not factors and getattr(self, "alpha", None) is not None:   # [dl | dalpha] and dF/dS
+            nls += 1
         gl = (C.c_double * nls)()
         if getattr(self, "_spectral", None) is not None:   # [dw | dmu | dv] and dF/dS
             Q, d = self._spectral

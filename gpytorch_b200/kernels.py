@@ -1,5 +1,5 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, SpectralMixtureKernel, PeriodicKernel,
-ScaleKernel, AdditiveKernel, ProductKernel, GridInterpolationKernel} for the accelerated path.
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, RQKernel, SpectralMixtureKernel,
+PeriodicKernel, ScaleKernel, AdditiveKernel, ProductKernel, GridInterpolationKernel} for the accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
 rbf_kernel.py:68-85; matern_kernel.py:79-110; scale_kernel.py:64-118), but `forward` returns an
@@ -172,6 +172,51 @@ class MaternKernel(_StationaryKernel):
     @property
     def kind(self):
         return {0.5: "matern12", 1.5: "matern32", 2.5: "matern52"}[self.nu]
+
+
+class RQKernel(_StationaryKernel):
+    """k = (1 + |x1 - x2|^2 / (2 alpha l^2))^-alpha (kernels/rq_kernel.py).  Parameters as in the reference: raw_lengthscale
+    [*B, 1, ard_num_dims or 1] and raw_alpha [*B, 1], each with a Positive() constraint unless one is given.  forward returns one
+    engine RQKernelLinearOperator (gp_plan_set_hypers_rq) on the tensor-core or CUDA-core K.V; inside a ScaleKernel the outputscale
+    multiplies it, and scaled or not it may be a term of an AdditiveKernel.  One batch dimension at most, no priors.  Products, SKI,
+    multitask, additive-component and derivative kernels do not take it."""
+    kind = "rq"
+
+    def __init__(self, alpha_constraint=None, lengthscale_prior=None, **kwargs):
+        if lengthscale_prior is not None or kwargs.pop("alpha_prior", None) is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        super().__init__(**kwargs)
+        self.register_parameter("raw_alpha", torch.nn.Parameter(torch.zeros(*self.batch_shape, 1)))
+        self.register_constraint("raw_alpha", alpha_constraint or Positive())
+
+    @property
+    def alpha(self):
+        return self.raw_alpha_constraint.transform(self.raw_alpha)
+
+    @alpha.setter
+    def alpha(self, value):
+        self._set_alpha(value)
+
+    def _set_alpha(self, value):
+        self._set_constrained("raw_alpha", value)
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, outputscale=None, last_dim_is_batch=False, **params):
+        from .operators import RQKernelLinearOperator
+        if last_dim_is_batch:
+            raise NotImplementedError("last_dim_is_batch is not available for an RQKernel on the accelerated path")
+        if diag and not (_same or x1.size(0) == x2.size(0)):
+            raise RuntimeError("diag=True needs x1 and x2 of equal sizes")
+        ls, al = self.lengthscale, self.alpha
+        if _batch_index is not None:
+            ls, al = ls[_batch_index], al[_batch_index]
+        ls = ls.reshape(-1)
+        op = RQKernelLinearOperator(x1, None if _same else x2, ls[0] if ls.numel() == 1 else ls, al.reshape(-1)[0], outputscale)
+        return op.diagonal() if diag else op
+
+
+def _is_rq(k):
+    """k is an RQKernel, or a ScaleKernel around one."""
+    return isinstance(k, RQKernel) or isinstance(getattr(k, "base_kernel", None), RQKernel)
 
 
 class Matern52KernelGrad(MaternKernel):
@@ -448,7 +493,7 @@ class ScaleKernel(Kernel):
             first = KernelLinearOperator(f[0].x1, f[0].x2, f[0].kind, f[0].lengthscale, self.outputscale * f[0].outputscale)
             op = ProductKernelLinearOperator([first, *f[1:]])
             return op.diagonal() if diag else op
-        if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel)):   # S folded into the same operator
+        if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel, RQKernel)):   # S folded into the same operator
             os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
             return self.base_kernel.forward(x1, x2, diag=diag, _same=_same, _batch_index=bi, outputscale=os_, **params)
         if isinstance(self.base_kernel, GridInterpolationKernel):
@@ -463,12 +508,13 @@ class ScaleKernel(Kernel):
         if isinstance(base, SKIKernelLinearOperator):
             op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
             return op.diagonal() if diag else op
-        from .operators import PeriodicKernelLinearOperator, SumKernelLinearOperator, with_outputscale
-        if isinstance(base, PeriodicKernelLinearOperator):   # a nested ScaleKernel: both scales folded in, the period kept
+        from .operators import PeriodicKernelLinearOperator, RQKernelLinearOperator, SumKernelLinearOperator, with_outputscale
+        keep = (PeriodicKernelLinearOperator, RQKernelLinearOperator)   # operators with parameters beyond lengthscale and scale
+        if isinstance(base, keep):   # a nested ScaleKernel: both scales folded in, the period / alpha kept
             op = with_outputscale(base, os_ * base.outputscale)
             return op.diagonal() if diag else op
-        if isinstance(base, SumKernelLinearOperator) and any(isinstance(t, PeriodicKernelLinearOperator) for t in base.ops):
-            # a ScaleKernel around a scaled sum with periodic terms: the scale folded into every term, the periods kept
+        if isinstance(base, SumKernelLinearOperator) and any(isinstance(t, keep) for t in base.ops):
+            # a ScaleKernel around a scaled sum with periodic or RQ terms: the scale folded into every term, periods and alphas kept
             op = SumKernelLinearOperator([with_outputscale(t, os_ * t.outputscale) for t in base.ops])
             return op.diagonal() if diag else op
         op = KernelLinearOperator(base.x1, base.x2, base.kind, base.lengthscale, os_)
@@ -538,6 +584,8 @@ class ProductKernel(Kernel):
                 raise RuntimeError("ProductKernel factors must be kernels")
             if _is_periodic(k):
                 raise NotImplementedError("products with a PeriodicKernel factor are not available on the accelerated path")
+            if _is_rq(k):
+                raise NotImplementedError("products with an RQKernel factor are not available on the accelerated path")
             base = k.base_kernel if isinstance(k, ScaleKernel) else k
             if not isinstance(base, _StationaryKernel) or isinstance(base, (RBFKernelGrad, Matern52KernelGrad)):
                 raise NotImplementedError("ProductKernel factors must be RBF / Matern kernels (optionally scaled) on the accelerated "
@@ -637,6 +685,8 @@ class MultitaskKernel(Kernel):
         base = dm.base_kernel if isinstance(dm, ScaleKernel) else dm
         if isinstance(base, PeriodicKernel):
             raise NotImplementedError("a PeriodicKernel data kernel of a MultitaskKernel is not available on the accelerated path")
+        if isinstance(base, RQKernel):
+            raise NotImplementedError("an RQKernel data kernel of a MultitaskKernel is not available on the accelerated path")
         if not isinstance(base, _StationaryKernel) or len(dm.batch_shape):
             raise NotImplementedError("the accelerated MultitaskKernel takes an RBFKernel / MaternKernel data kernel, optionally "
                                       "inside a ScaleKernel")
@@ -668,6 +718,9 @@ class GridInterpolationKernel(Kernel):
         if isinstance(base_kernel, PeriodicKernel):
             raise NotImplementedError("a PeriodicKernel base kernel of a GridInterpolationKernel is not available on the accelerated "
                                       "path")
+        if isinstance(base_kernel, RQKernel):
+            raise NotImplementedError("an RQKernel base kernel of a GridInterpolationKernel is not available on the accelerated path: "
+                                      "its heavy tails leave nothing for the band-limited grid products to skip")
         if not isinstance(base_kernel, _StationaryKernel):
             raise RuntimeError("GridInterpolationKernel needs an RBFKernel or MaternKernel base kernel on the accelerated path")
         if isinstance(base_kernel, Matern52KernelGrad):

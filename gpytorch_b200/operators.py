@@ -448,6 +448,8 @@ class KernelLinearOperator(_SamplingMixin):
         (gp_plan_set_tasks).  RBF / Matern operators, optionally scaled, only.  With another RBF / Matern kernel operator (or a
         product of them) of the same shape: the elementwise product K_1 o K_2 as one engine operator (gp_plan_set_product)."""
         plain = (KernelLinearOperator, ProductKernelLinearOperator)
+        if isinstance(other, RQKernelLinearOperator):
+            return other.mul(self)   # refused, naming RQ
         if type(self) in plain and type(other) in plain:
             return ProductKernelLinearOperator([self, other])
         if not isinstance(other, IndexLinearOperator) or type(self) is not KernelLinearOperator:
@@ -896,6 +898,9 @@ class SumKernelLinearOperator(KernelLinearOperator):
             if isinstance(o, PeriodicKernelLinearOperator):   # keeps its period, on a slot no plain term uses
                 t = o._with(o.x1, None if o.same else o.x2)
                 t._plan_slot = _PERIODIC_SUM_SLOT + i
+            elif isinstance(o, RQKernelLinearOperator):       # keeps alpha, on the plain term slot (kind and alpha are in its key)
+                t = o._with(o.x1, None if o.same else o.x2)
+                t._plan_slot = 1 + i
             else:
                 t = KernelLinearOperator(o.x1, o.x2, o.kind, o.lengthscale, o.outputscale, comm=o._comm, row_begin=o._row_begin,
                                          row_count=o._row_count)
@@ -1020,6 +1025,9 @@ class ProductKernelLinearOperator(KernelLinearOperator):
             raise NotImplementedError(f"a kernel product takes 2 to 4 factors on the accelerated path (got {len(flat)})")
         first = flat[0]
         for o in flat:
+            if isinstance(o, RQKernelLinearOperator):
+                raise NotImplementedError("products that contain a rational quadratic (RQ) operator are not available on the "
+                                          "accelerated path")
             if type(o) is not KernelLinearOperator:
                 raise NotImplementedError("the factors of a kernel product must be RBF / Matern kernel operators (optionally scaled) "
                                           "on the accelerated path")
@@ -1589,10 +1597,103 @@ class PeriodicKernelLinearOperator(KernelLinearOperator):
     __mul__ = mul
 
 
+class RQKernelLinearOperator(KernelLinearOperator):
+    """S (1 + r^2 / (2 alpha))^-alpha, r^2 = |(x1 - x2) / l|^2 (kernels/rq_kernel.py, which forms the dense matrix) as ONE engine
+    plan of kind GP_RQ (gp_plan_set_hypers_rq): products, solves, the preconditioner, SLQ, rows and input gradients run on the plain
+    tensor-core / CUDA-core kernels with the RQ covariance in their epilogue.  lengthscale holds 1 or d values and alpha one (the
+    parameter tensors or their slices for one element of a batch); autograd reaches them through _bilinear_derivative_list.  S is
+    the outputscale of a ScaleKernel around the kernel (None: 1, no gradient).  The plan-cache slots are the plain ones: the kind
+    and alpha are part of the plan's hyper-parameter key, so a plan re-sends them whenever another kind used it last."""
+
+    def __init__(self, x1, x2, lengthscale, alpha, outputscale=None, comm=None, row_begin=0, row_count=0):
+        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
+            raise NotImplementedError("a row-sharded rational quadratic (RQ) operator is not available on the accelerated path")
+        super().__init__(x1, x2, "rq", lengthscale, outputscale)
+        if alpha.numel() != 1:
+            raise RuntimeError(f"RQ kernel: alpha must hold one value (got shape {tuple(alpha.shape)})")
+        self.alpha = alpha
+
+    def hyper_tensors(self):
+        return [self.lengthscale, self.alpha, self.outputscale]
+
+    @property
+    def requires_grad(self):
+        return any(t.requires_grad for t in self.hyper_tensors())
+
+    def representation(self):
+        return (self.x1, self.x2, *self.hyper_tensors())
+
+    def _host_hypers(self, noise_t=None):
+        """(lengthscale list, outputscale, noise, noise tensor, alpha) with one device -> host read."""
+        cached = getattr(self, "_hyp_host", None)
+        if cached is None or (noise_t is not None and cached[3] is not noise_t):
+            parts = [t.detach().reshape(-1).float().to(self.device) for t in (self.lengthscale, self.outputscale, self.alpha)]
+            if noise_t is not None:
+                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.device))
+            vals = torch.cat(parts).tolist()
+            nl = self.lengthscale.numel()
+            cached = (vals[:nl], vals[nl], vals[nl + 2] if noise_t is not None else None, noise_t, vals[nl + 1])
+            self._hyp_host = cached
+        return cached
+
+    def plan(self, noise=0.0) -> Plan:
+        fresh = False
+        if self._plan is None:
+            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None,
+                                   getattr(self, "_plan_slot", 0), owner=self)
+            fresh = True
+        if torch.is_tensor(noise):
+            ls, os_, nz, _, al = self._host_hypers(noise)
+        else:
+            ls, os_, _, _, al = self._host_hypers(None)
+            nz = float(noise)
+        key = ("rq", tuple(ls), al, os_, nz)
+        if fresh or getattr(self._plan, "_hyp_key", None) != key:
+            self._plan.set_hypers_rq(ls, al, os_, nz)
+            self._plan._hyp_key = key
+        return self._plan
+
+    def _bilinear_derivative_list(self, left, right):
+        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
+        vals = torch.tensor(gl, device=self.device, dtype=self.lengthscale.dtype)
+        nl = self.lengthscale.numel()
+        return [vals[:nl].reshape(self.lengthscale.shape), vals[nl:].to(self.alpha.dtype).reshape(self.alpha.shape),
+                torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape)]
+
+    def _bilinear_derivative(self, left, right):
+        raise NotImplementedError("an RQ operator has lengthscale, alpha and outputscale gradients: use _bilinear_derivative_list")
+
+    def _with(self, x1, x2, detach=False, outputscale=None):
+        f = (lambda t: t.detach()) if detach else (lambda t: t)
+        return RQKernelLinearOperator(f(x1), None if x2 is None else f(x2), f(self.lengthscale), f(self.alpha),
+                                      f(self.outputscale if outputscale is None else outputscale))
+
+    def _transpose_nonbatch(self):
+        return self if self.same else self._with(self.x2, self.x1)
+
+    def detach(self):
+        return self._with(self.x1, None if self.same else self.x2, detach=True)
+
+    def __getitem__(self, index):
+        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
+
+    def mul(self, other):
+        raise NotImplementedError("products that contain a rational quadratic (RQ) operator (kernel products, IndexKernel "
+                                  "multitask models) are not available on the accelerated path")
+
+    __mul__ = mul
+
+
 def with_outputscale(op, outputscale):
-    """A plain or periodic kernel operator with its outputscale replaced (a ScaleKernel folded into the terms of a sum or into the
-    first factor of a product); the operator's other parameters are kept."""
-    if isinstance(op, PeriodicKernelLinearOperator):
+    """A plain, periodic or RQ kernel operator with its outputscale replaced (a ScaleKernel folded into the terms of a sum or into
+    the first factor of a product); the operator's other parameters are kept."""
+    if isinstance(op, (PeriodicKernelLinearOperator, RQKernelLinearOperator)):
         return op._with(op.x1, None if op.same else op.x2, outputscale=outputscale)
     return KernelLinearOperator(op.x1, op.x2, op.kind, op.lengthscale, outputscale)
 

@@ -40,8 +40,9 @@ enum {
   GP_W_EIG_NOT_CONVERGED = 8 /* tridiagonal QL iteration hit its sweep limit: the SLQ log-det is unreliable (NumericalWarning) */
 };
 
-/* covariance function kinds: kernels/rbf_kernel.py:68-85, kernels/matern_kernel.py:85-110 */
-enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3 };
+/* covariance function kinds: kernels/rbf_kernel.py:68-85, kernels/matern_kernel.py:85-110, kernels/rq_kernel.py (GP_RQ is set
+ * through gp_plan_set_hypers_rq only, which also gives alpha) */
+enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3, GP_RQ = 4 };
 
 /* which fused K.V kernel runs: GP_BACKEND_TCGEN05 = wgmma/bulk-TMA 3xTF32 tensor-core kernel
  * (the name is historical),
@@ -209,6 +210,27 @@ int gp_plan_set_spectral(gp_plan* plan, int Q, const float* weights, const float
  * factor of gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.  A SKI, sum,
  * product, multitask, derivative, additive, spectral or row-sharded plan cannot become a periodic plan. */
 int gp_plan_set_periodic(gp_plan* plan, const float* period, int n_period, int d);
+
+/* Rational quadratic kernels (the reference's RQKernel, kernels/rq_kernel.py): kind GP_RQ with its alpha, set together with the
+ * lengthscales (1 or d), the outputscale S and the noise in one call:
+ *   K(x, x') = S (1 + r^2 / (2 alpha))^-alpha,   r^2 = |(x - x') / l|^2
+ * (+ its noise / per-row diagonal where a call adds it).  alpha must be > 0 and finite, and the lengthscales as for
+ * gp_plan_set_hypers, else GP_E_SHAPE.  The call is all or nothing: a failed call leaves the plan's previous hyper-parameters in
+ * place.  gp_plan_set_hypers with kind GP_RQ returns GP_E_SHAPE, so a plan never holds kind GP_RQ without its alpha; a later
+ * gp_plan_set_hypers with another kind makes the plan a plain plan of that kind.  A plain plan, square or cross, on the tensor-core
+ * backend or the CUDA-core one; the inputs are packed as for RBF with the constant C = 1, and alpha stays out of the packing.  Its
+ * K.V evaluates log2(1 + t), t = r^2 / (2 alpha), with an absolute error O(2^-24 t) (a polynomial below t = 1/16), so an entry's
+ * error does not grow with alpha (DESIGN 4.20).
+ * gp_kmv, gp_krows, gp_kdiag (the square diagonal is S), gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg,
+ * gp_slq_logdet, gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond, gp_plan_set_backend,
+ * gp_plan_set_noise_diag, gp_plan_set_lowrank (as the base), gp_kmv_input_grad, gp_kdense_input_grad and gp_time_kmv_kernel run on
+ * it, and it may be a term of gp_plan_set_sum.  gp_bilinear_grad returns n_ls + 1 doubles in grad_ls, [dF/dl (n_ls) | dF/dalpha],
+ * and dF/dS in grad_os; a non-finite input makes them NaN.  On an RQ plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv,
+ * gp_plan_set_deriv_kind, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_spectral, gp_plan_set_periodic
+ * and gp_plan_set_comm with more than one rank return GP_E_STATE with a message naming the call; an RQ plan as a factor of
+ * gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.  A SKI, sum, product,
+ * multitask, derivative, additive, spectral, periodic or row-sharded plan cannot take this call (GP_E_STATE). */
+int gp_plan_set_hypers_rq(gp_plan* plan, const float* lengthscale, int n_ls, float alpha, float outputscale, float noise);
 
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
  * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
