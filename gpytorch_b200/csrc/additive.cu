@@ -376,6 +376,7 @@ extern "C" int gp_plan_set_additive(gp_plan* p, int max_degree, const float* com
   GP_REFUSE_SPECTRAL(p, "gp_plan_set_additive");
   GP_REFUSE_PERIODIC(p, "gp_plan_set_additive");
   GP_REFUSE_RQ(p, "gp_plan_set_additive");
+  GP_REFUSE_POLY(p, "gp_plan_set_additive");
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,
              "an additive plan is not available on a row-sharded plan");
   GP_REQUIRE(n_comp >= 1 && n_comp <= ADD_DMAX, GP_E_SHAPE, "an additive plan takes 1 to %d components (got %d)", ADD_DMAX, n_comp);

@@ -170,6 +170,7 @@ extern "C" int gp_plan_set_data(gp_plan* p, const float* X1, int64_t n1, int64_t
 extern "C" int gp_plan_set_hypers(gp_plan* p, int kind, const float* lengthscale, int n_ls, float outputscale, float noise) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(kind != GP_RQ, GP_E_SHAPE, "the rational quadratic kind takes alpha: call gp_plan_set_hypers_rq");
+  GP_REQUIRE(kind != GP_POLY, GP_E_SHAPE, "the polynomial kind takes a power and an offset: call gp_plan_set_hypers_poly");
   GP_REQUIRE(kind >= GP_RBF && kind <= GP_MATERN52, GP_E_SHAPE, "nu expected to be 0.5, 1.5, or 2.5 (kind=%d)", kind);
   GP_REQUIRE(lengthscale && n_ls >= 1, GP_E_SHAPE, "lengthscale missing");
   GP_REQUIRE(!p->data_set || n_ls == 1 || n_ls == p->d, GP_E_SHAPE, "lengthscale count %d does not match d=%d", n_ls, p->d);
@@ -232,6 +233,49 @@ extern "C" int gp_plan_set_hypers_rq(gp_plan* p, const float* lengthscale, int n
   return st;
 }
 
+extern "C" int gp_plan_set_hypers_poly(gp_plan* p, int power, float offset, float outputscale, float noise) {
+  GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  GP_REQUIRE(power >= 1 && power <= 8, GP_E_SHAPE, "power=%d must be an integer in [1, 8]", power);
+  GP_REQUIRE(offset >= 0.f && isfinite(offset), GP_E_SHAPE, "offset=%g must be finite and >= 0", offset);
+  GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
+  GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "gp_plan_set_hypers_poly is not available on a SKI plan (gp_plan_set_ski)");
+  GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "gp_plan_set_hypers_poly is not available on a kernel-sum plan: give the kind to a term");
+  GP_REFUSE_TASKS(p, "gp_plan_set_hypers_poly");
+  GP_REFUSE_KRON(p, "gp_plan_set_hypers_poly");
+  GP_REFUSE_DERIV(p, "gp_plan_set_hypers_poly");
+  GP_REFUSE_PRODUCT(p, "gp_plan_set_hypers_poly");
+  GP_REFUSE_ADDITIVE(p, "gp_plan_set_hypers_poly");
+  GP_REFUSE_SPECTRAL(p, "gp_plan_set_hypers_poly");
+  GP_REFUSE_PERIODIC(p, "gp_plan_set_hypers_poly");
+  GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_STATE, "gp_plan_set_hypers_poly is not available on a row-sharded plan (gp_plan_set_comm)");
+  GP_CUDA(cudaSetDevice(p->device));
+  // all or nothing, as gp_plan_set_hypers_rq: a failed pack restores the previous hyper-parameters (and packing)
+  const int old_kind = p->kind, old_power = p->poly_power;
+  const std::vector<float> old_ls = p->ls;
+  const float old_off = p->poly_offset, old_os = p->outputscale, old_noise = p->noise;
+  const bool old_set = p->hypers_set;
+  p->kind = GP_POLY;
+  p->ls.assign(1, 1.f);   // no lengthscale: the inputs are packed raw (pack.cu)
+  p->poly_power = power;
+  p->poly_offset = offset;
+  p->outputscale = outputscale;
+  p->noise = noise;
+  p->hypers_set = true;
+  if (!p->data_set) return GP_OK;
+  const int st = pack_inputs(p);
+  if (st != GP_OK) {
+    p->kind = old_kind;
+    p->ls = old_ls;
+    p->poly_power = old_power;
+    p->poly_offset = old_off;
+    p->outputscale = old_os;
+    p->noise = old_noise;
+    p->hypers_set = old_set;
+    if (old_set) pack_inputs(p);   // the previous packing; the error reported is the first one
+  }
+  return st;
+}
+
 extern "C" int gp_plan_set_noise_diag(gp_plan* p, const float* diag, int64_t n) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(diag == nullptr || (p->data_set && p->same && n == p->n2), GP_E_SHAPE,
@@ -270,6 +314,8 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
              "gp_plan_set_comm with more than one rank is not available on a periodic plan (gp_plan_set_periodic)");
   GP_REQUIRE(!(p->kind == GP_RQ && comm && comm->world > 1), GP_E_STATE,
              "gp_plan_set_comm with more than one rank is not available on a rational quadratic plan (gp_plan_set_hypers_rq)");
+  GP_REQUIRE(!(p->kind == GP_POLY && comm && comm->world > 1), GP_E_STATE,
+             "gp_plan_set_comm with more than one rank is not available on a polynomial plan (gp_plan_set_hypers_poly)");
   p->comm = comm;
   return GP_OK;
 }

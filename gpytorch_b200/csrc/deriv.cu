@@ -513,6 +513,8 @@ static int deriv_set(gp_plan* p, gp_plan* data, int kind, const char* what) {
   if (data) GP_REQUIRE(data->per_n == 0, GP_E_STATE, "%s (as the data plan) is not available on a periodic plan (gp_plan_set_periodic)", what);
   GP_REFUSE_RQ(p, what);
   if (data) GP_REQUIRE(data->kind != GP_RQ, GP_E_STATE, "%s (as the data plan) is not available on a rational quadratic plan (gp_plan_set_hypers_rq)", what);
+  GP_REFUSE_POLY(p, what);
+  if (data) GP_REQUIRE(data->kind != GP_POLY, GP_E_STATE, "%s (as the data plan) is not available on a polynomial plan (gp_plan_set_hypers_poly)", what);
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   gp_deriv_state* ds = p->deriv ? p->deriv : new gp_deriv_state();
   gp_plan* old = ds->data;

@@ -288,6 +288,9 @@ struct gp_plan {
   std::vector<float> per_p;       // the per_n periods
   // rational quadratic kernels (kind GP_RQ, gp_plan_set_hypers_rq): (1 + r^2 / (2 alpha))^-alpha over z = (x - mean) / l
   float rq_alpha = 0.f;
+  // polynomial kernels (kind GP_POLY, gp_plan_set_hypers_poly): S (x.x' + c)^p over the raw inputs (no centring, no lengthscale)
+  int poly_power = 0;
+  float poly_offset = 0.f;
   int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
@@ -340,6 +343,8 @@ int kmv_tc_launch_cols(gp_plan* p, int kind, const float* XA, const float* XB, c
 int kmv_simt_launch_cols(gp_plan* p, int kind, const float* Z1, const float* Z2, const float* V16, float* partial, int64_t n2,
                          int64_t cols_per_split, int nsplit, int64_t diag_row_begin, const int* done_flag);
 int sum_partials_double(gp_plan* p, const double* in, int64_t nblk, int stride, int nout, double* out);   // out[o] = sum_b in[b][o], NaN when xbad
+bool sum_has_poly(const gp_plan* p);                                    // kmv_simt.cu: a kernel sum with a polynomial term
+int sum_kdiag_terms(gp_plan* p, float* OUT);                            // kmv_simt.cu: its per-row diagonal, term by term
 int64_t bilinear_blocks(const gp_plan* p, int64_t n2);                      // CTAs of one SIMT derivative launch over n2 columns
 void bilinear_split(const gp_plan* p, int64_t n2, dim3* grid, int64_t* cps);  // its grid and columns per split (kmv_simt.cu)
 int bilinear_launch_cols(gp_plan* p, bool ard, const float* Z1, const float* Z2, const float* L16, const float* R16, int64_t n2,
@@ -413,6 +418,8 @@ int periodic_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float*
   GP_REQUIRE((p)->per_n == 0, GP_E_STATE, "%s is not available on a periodic plan (gp_plan_set_periodic)", what)
 #define GP_REFUSE_RQ(p, what) \
   GP_REQUIRE((p)->kind != GP_RQ, GP_E_STATE, "%s is not available on a rational quadratic plan (gp_plan_set_hypers_rq)", what)
+#define GP_REFUSE_POLY(p, what) \
+  GP_REQUIRE((p)->kind != GP_POLY, GP_E_STATE, "%s is not available on a polynomial plan (gp_plan_set_hypers_poly)", what)
 // columns of the packed rows the plain kernels see: the d inputs, or the 2d embedding columns of a periodic plan
 inline int packed_dims(const gp_plan* p) { return p->per_n ? 2 * p->d : p->d; }
 inline bool plan_is_tc(const gp_plan* p) {
@@ -421,14 +428,17 @@ inline bool plan_is_tc(const gp_plan* p) {
 
 __host__ __device__ inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// Per-plan parameters of the covariance, passed by value to every kernel that evaluates it; only GP_RQ reads them (the other
-// kinds' code does not change with it).
+// Per-plan parameters of the covariance, passed by value to every kernel that evaluates it; only GP_RQ and GP_POLY read them (the
+// other kinds' code does not change with it).
 struct CovParam {
   float alpha;    // RQ: alpha > 0
   float ialpha;   // RQ: 1 / alpha, rounded once from fp64
+  float offset;   // POLY: c >= 0 (packed into the GEMM1 operands on the tensor-core path, added to the dot product on the CUDA cores)
+  int power;      // POLY: 1 <= p <= 8
 };
 inline CovParam cov_param(const gp_plan* p) {
-  return p->kind == GP_RQ ? CovParam{p->rq_alpha, (float)(1.0 / (double)p->rq_alpha)} : CovParam{0.f, 0.f};
+  if (p->kind == GP_POLY) return CovParam{0.f, 0.f, p->poly_offset, p->poly_power};
+  return p->kind == GP_RQ ? CovParam{p->rq_alpha, (float)(1.0 / (double)p->rq_alpha), 0.f, 0} : CovParam{0.f, 0.f, 0.f, 0};
 }
 
 // ---- device helpers -----------------------------------------------------------------------
@@ -462,8 +472,29 @@ constexpr int RQ_K = 16;      // RQ: k
 constexpr int RQ_DL = 17;     // RQ: l dk/dl (scalar lengthscale)
 constexpr int RQ_DA = 18;     // RQ: dk/dalpha
 __host__ __device__ constexpr bool is_rq_code(int code) { return code >= RQ_K && code <= RQ_DA; }
-// the code a dispatcher evaluates for `kind` on plan p: on an RQ plan GP_RQ (the plan's own kind) is RQ_K
-inline int rq_code(const gp_plan* p, int kind) { return (p->kind == GP_RQ && kind == GP_RQ) ? RQ_K : kind; }
+// Polynomial kernels (DESIGN 4.21): the kernel argument is not a distance but a = x_i . x_j + c over the raw inputs, and
+// k = a^p, dk/dc = p a^(p-1) (FMA pipe only, no MUFU).  The public GP_POLY = 5 is the number of GP_DERIV + GP_MATERN12, so, as for
+// RQ, only these codes of their own (two digits) reach a template.
+constexpr int POLY_K = 24;    // POLY: k = a^p
+constexpr int POLY_DC = 25;   // POLY: dk/dc = p a^(p-1)
+__host__ __device__ constexpr bool is_poly_code(int code) { return code == POLY_K || code == POLY_DC; }
+// the code a dispatcher evaluates for `kind` on plan p: on an RQ plan GP_RQ (the plan's own kind) is RQ_K, on a polynomial plan
+// GP_POLY is POLY_K
+inline int rq_code(const gp_plan* p, int kind) {
+  if (p->kind == GP_POLY && kind == GP_POLY) return POLY_K;
+  return (p->kind == GP_RQ && kind == GP_RQ) ? RQ_K : kind;
+}
+// a^q for 0 <= q <= 8 by squaring: a^2, a^4, a^8 and the product of the ones q selects.  Every tree of multiplies that forms a^q
+// carries at most (q - 1) roundings of 2^-24 relative (each product adds one to the sum of its factors'), as q - 1 multiplies in
+// a row would; a negative a keeps the sign of a^q for odd q (torch.pow with an integral exponent)
+__host__ __device__ __forceinline__ float poly_pow(float a, int q) {
+  const float a2 = a * a, a4 = a2 * a2;
+  float r = (q & 1) ? a : 1.f;
+  if (q & 2) r *= a2;
+  if (q & 4) r *= a4;
+  if (q & 8) r = a4 * a4;   // q = 8 exactly (q <= 8)
+  return r;
+}
 
 #if defined(__CUDACC__)
 __device__ __forceinline__ float lg2_approx(float x) {
@@ -509,7 +540,11 @@ __device__ __forceinline__ float dcov_from_arg(float a, float* kout, CovParam cp
 
 template <int KIND>
 __device__ __forceinline__ float cov_from_arg(float a, CovParam cp) {
-  if (KIND == RQ_K) {
+  if (KIND == POLY_K) {   // a = x_i . x_j + c (no clamp: a may be negative)
+    return poly_pow(a, cp.power);
+  } else if (KIND == POLY_DC) {
+    return (float)cp.power * poly_pow(a, cp.power - 1);
+  } else if (KIND == RQ_K) {
     return rq_k(rq_t(a, cp), cp);
   } else if (KIND == RQ_DL) {
     float k;
@@ -534,7 +569,11 @@ __device__ __forceinline__ float cov_from_arg(float a, CovParam cp) {
 // dk/dl = g / l (scalar lengthscale):  RBF: sq*k ; M12: rho e ; M32: rho^2 e ; M52: (1+rho) rho^2/3 e ; RQ: r^2 k / (1 + t)
 template <int KIND>
 __device__ __forceinline__ float dcov_from_arg(float a, float* kout, CovParam cp) {
-  if (KIND == RQ_K) {
+  if (KIND == POLY_K) {   // k and dk/dc = p a^(p-1): k = a a^(p-1)
+    const float km1 = poly_pow(a, cp.power - 1);
+    *kout = a * km1;
+    return (float)cp.power * km1;
+  } else if (KIND == RQ_K) {
     const float t = rq_t(a, cp);
     const float k = rq_k(t, cp);
     *kout = k;
@@ -665,13 +704,23 @@ __device__ __forceinline__ float sm_pair(const SmHyp& h, const float* za, const 
   return k;
 }
 SmHyp spectral_hyp(const gp_plan* p);   // spectral.cu: the kernel argument of a spectral plan
+// the argument a = x_i . x_j + c of a polynomial pair from two packed (raw, zero-padded) rows, fp32 FMAs in column order
+__device__ __forceinline__ float poly_arg(const float* za, const float* zb, int n, float offset) {
+  float s = 0.f;
+  for (int c = 0; c < n; ++c) s = fmaf(za[c], zb[c], s);
+  return s + offset;
+}
 // input-derivative factor q = dk/da of the same covariance (xgrad.cu): dk/dz_i = -q (z_i - z_j) in the packed units.
 //   RBF: ln2 2^a ; M12: e / (2 rho) ; M32: e / 2 ; M52: (1 + rho) e / 6 ; RQ: k / (1 + t)      (e = exp(-rho), rho^2 = -a)
 // q is the h of the raw-unit form  dk/dx_i = -h (x_i - x_j) / l^2  times l^2 / C (C = log2 e, 2, 6, 10 as in pack.cu).  A pair at
 // distance 0 contributes 0 (its direction is 0; Matern-1/2's q is unbounded there): the caller masks a == 0.
+//   POLY: not the difference form.  q = dk/da = p a^(p-1) with a = x_i . x_j + c and dk/dx_i = q x_j, so every pair contributes,
+//   the diagonal of a square plan too (2 q_ii x_i from both arguments, which are the same point); xgrad.cu takes that branch.
 template <int KIND>
 __device__ __forceinline__ float hcov_from_arg(float a, CovParam cp) {
-  if (KIND == RQ_K) {
+  if (KIND == POLY_K) {
+    return (float)cp.power * poly_pow(a, cp.power - 1);
+  } else if (KIND == RQ_K) {
     const float t = rq_t(a, cp);
     return __fdividef(rq_k(t, cp), 1.f + t);
   } else if (KIND == GP_RBF) {

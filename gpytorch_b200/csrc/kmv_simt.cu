@@ -48,14 +48,22 @@ __device__ __forceinline__ void kmv_simt_body(const float* __restrict__ Z1, cons
     __syncthreads();
 #pragma unroll 4
     for (int jj = 0; jj < SIMT_TJ; ++jj) {
-      float s = 0.f;
+      float a;
+      if constexpr (is_poly_code(KIND)) {   // a = x_i . x_j + c: every entry, the diagonal too, from the raw inputs
+        float s = 0.f;
 #pragma unroll
-      for (int c = 0; c < DP; ++c) {
-        float df = zi[c] - zj[jj][c];
-        s = fmaf(df, df, s);
+        for (int c = 0; c < DP; ++c) s = fmaf(zi[c], zj[jj][c], s);
+        a = s + cp.offset;
+      } else {
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < DP; ++c) {
+          float df = zi[c] - zj[jj][c];
+          s = fmaf(df, df, s);
+        }
+        a = -0.5f * s;
+        if (same && (j0 + jj) == gi) a = 0.f;  // exact diagonal (kernel.py:44-45)
       }
-      float a = -0.5f * s;
-      if (same && (j0 + jj) == gi) a = 0.f;  // exact diagonal (kernel.py:44-45)
       float k = cov_from_arg<KIND>(a, cp);
 #pragma unroll
       for (int c = 0; c < TP; ++c) acc[c] = fmaf(k, vj[jj][c], acc[c]);
@@ -82,6 +90,14 @@ rq_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const
                int same, int64_t row_begin, const int* __restrict__ done_flag, CovParam cp) {
   kmv_simt_body<RQ_K, DP>(Z1, Z2, V16, partial, n1, n2, rows_pad, cols_per_split, same, row_begin, done_flag, cp);
 }
+// the polynomial kernel with its per-plan power and offset
+template <int DP>
+__global__ void __launch_bounds__(SIMT_TI)
+poly_simt_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, const float* __restrict__ V16,
+                 float* __restrict__ partial, int64_t n1, int64_t n2, int64_t rows_pad, int64_t cols_per_split,
+                 int same, int64_t row_begin, const int* __restrict__ done_flag, CovParam cp) {
+  kmv_simt_body<POLY_K, DP>(Z1, Z2, V16, partial, n1, n2, rows_pad, cols_per_split, same, row_begin, done_flag, cp);
+}
 
 struct SimtLaunch {
   const float* Z1;
@@ -98,7 +114,11 @@ static int launch_simt_kind(gp_plan* p, const SimtLaunch& a, const int* done_fla
   dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)a.nsplit);
 #define GP_SIMT_CASE(D)                                                                                          \
   case D:                                                                                                        \
-    if constexpr (KIND == RQ_K)                                                                                  \
+    if constexpr (KIND == POLY_K)                                                                                \
+      poly_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2,     \
+                                                           rows_pad, a.cps, p->same ? 1 : 0, a.row_begin, done_flag, \
+                                                           cov_param(p));                                        \
+    else if constexpr (KIND == RQ_K)                                                                             \
       rq_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2,       \
                                                          rows_pad, a.cps, p->same ? 1 : 0, a.row_begin, done_flag, \
                                                          cov_param(p));                                          \
@@ -127,6 +147,7 @@ static int launch_simt_any(gp_plan* p, int kind, const SimtLaunch& a, const int*
     case GP_MATERN32: return launch_simt_kind<GP_MATERN32>(p, a, done_flag);
     case GP_MATERN52: return launch_simt_kind<GP_MATERN52>(p, a, done_flag);
     case RQ_K: return launch_simt_kind<RQ_K>(p, a, done_flag);
+    case POLY_K: return launch_simt_kind<POLY_K>(p, a, done_flag);
   }
   set_error("bad kernel kind %d", kind);
   return GP_E_SHAPE;
@@ -228,13 +249,18 @@ __global__ void krows_kernel(const float* __restrict__ Z1, const float* __restri
   __syncthreads();
   int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n2) return;
-  float s = 0.f;
-  for (int c = 0; c < DP; ++c) {
-    float df = zi[c] - Z2[j * DP + c];
-    s = fmaf(df, df, s);
+  float a;
+  if constexpr (is_poly_code(KIND)) {
+    a = poly_arg(zi, Z2 + j * DP, DP, cp.offset);
+  } else {
+    float s = 0.f;
+    for (int c = 0; c < DP; ++c) {
+      float df = zi[c] - Z2[j * DP + c];
+      s = fmaf(df, df, s);
+    }
+    a = -0.5f * s;
+    if (same && (i + row_begin) == j) a = 0.f;
   }
-  float a = -0.5f * s;
-  if (same && (i + row_begin) == j) a = 0.f;
   OUT[r * ldo + j] = os * cov_from_arg<KIND>(a, cp);
 }
 
@@ -245,6 +271,10 @@ __global__ void kdiag_cross_kernel(const float* __restrict__ Z1, const float* __
                                    float* __restrict__ OUT, CovParam cp) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  if constexpr (is_poly_code(KIND)) {   // also the square diagonal S (|x_i|^2 + c)^p (Z1 = Z2)
+    OUT[i] = os * cov_from_arg<KIND>(poly_arg(Z1 + i * DP, Z2 + i * DP, DP, cp.offset), cp);
+    return;
+  }
   float s = 0.f;
   for (int c = 0; c < DP; ++c) {
     float df = Z1[i * DP + c] - Z2[i * DP + c];
@@ -258,6 +288,16 @@ __global__ void fill_kernel(float* __restrict__ p, int64_t n, float v) {
   if (i < n) p[i] = v;
 }
 
+// the diagonal of a square kernel sum with a polynomial term, term by term in term order: OUT[i] (+)= os_t k_t(x_i, x_i), the
+// constant os_t for a stationary term, os_t (|x_i|^2 + c_t)^p_t for a polynomial one (Z: its packed rows)
+__global__ void sum_diag_term_kernel(const float* __restrict__ Z, int DP, int64_t n, float os, CovParam cp, int first,
+                                     float* __restrict__ OUT) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float v = Z ? os * cov_from_arg<POLY_K>(poly_arg(Z + i * DP, Z + i * DP, DP, cp.offset), cp) : os;
+  OUT[i] = first ? v : OUT[i] + v;
+}
+
 // ---- bilinear derivative: sum_ij (Lf_i . Rt_j) dk_ij/dtheta ---------------------------------
 // grid (row blocks, col splits); per-thread row, staged columns; outputs per block partial sums
 //   gout[block][0]      = sum_ij w_ij k_ij                 (-> d/d outputscale)
@@ -269,6 +309,7 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
                 const float* __restrict__ R16, int64_t n1, int64_t n2, int64_t cols_per_split, int same,
                 int64_t row_begin, int d, double* __restrict__ gout, int gstride, CovParam cp) {
   constexpr bool RQ = KIND == RQ_K;
+  constexpr bool POLY = KIND == POLY_K;   // g = dk/dc, one output beside dF/dS (ARD is not used)
   __shared__ __align__(16) float zj[SIMT_TJ][DP];
   __shared__ __align__(16) float rj[SIMT_TJ][TP];
   const int tid = threadIdx.x;
@@ -298,19 +339,26 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
       for (int c = 0; c < TP; ++c) w = fmaf(li[c], rj[jj][c], w);
       float s = 0.f;
       float df2[DP];
+      float a;
+      if constexpr (POLY) {
 #pragma unroll
-      for (int c = 0; c < DP; ++c) {
-        float df = zi[c] - zj[jj][c];
-        df2[c] = df * df;
-        s += df2[c];
+        for (int c = 0; c < DP; ++c) s = fmaf(zi[c], zj[jj][c], s);
+        a = s + cp.offset;
+      } else {
+#pragma unroll
+        for (int c = 0; c < DP; ++c) {
+          float df = zi[c] - zj[jj][c];
+          df2[c] = df * df;
+          s += df2[c];
+        }
+        a = -0.5f * s;
+        if (same && (j0 + jj) == gi) a = 0.f;
       }
-      float a = -0.5f * s;
-      if (same && (j0 + jj) == gi) a = 0.f;
       float k;
       float g = dcov_from_arg<KIND>(a, &k, cp);
       gk = fmaf(w, k, gk);
       if (RQ) ga = fmaf(w, -k * rq_phi(rq_t(a, cp)), ga);
-      if (ARD) {
+      if (ARD && !POLY) {
         // dk/dl_c = g * (z_ic - z_jc)^2 / (s * l_c)   (g/l is the scalar-lengthscale derivative)
         float gs = (s > 0.f) ? w * g / s : 0.f;
 #pragma unroll
@@ -421,8 +469,28 @@ static int launch_bilinear_any(gp_plan* p, const BilinLaunch& a, const float* L1
     case GP_MATERN12: return launch_bilinear<GP_MATERN12, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
     case GP_MATERN32: return launch_bilinear<GP_MATERN32, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
     case GP_RQ: return launch_bilinear<RQ_K, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
+    case GP_POLY: return launch_bilinear<POLY_K, false>(p, a, L16, R16, gout, gstride, grid, cps);
     default: return launch_bilinear<GP_MATERN52, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
   }
+}
+
+bool sum_has_poly(const gp_plan* p) {
+  for (const gp_plan* t : p->terms)
+    if (t->kind == GP_POLY) return true;
+  return false;
+}
+
+// per-row diagonal of a square kernel sum with a polynomial term: the terms' diagonals added in term order
+int sum_kdiag_terms(gp_plan* p, float* OUT) {
+  const unsigned g = (unsigned)cdiv(p->row_count, 256);
+  for (size_t t = 0; t < p->terms.size(); ++t) {
+    const gp_plan* q = p->terms[t];
+    const float* Z = q->kind == GP_POLY ? q->Z2.as<float>() + p->row_begin * q->DP : nullptr;
+    sum_diag_term_kernel<<<g, 256, 0, p->stream>>>(Z, q->DP, p->row_count, q->outputscale, cov_param(q), t == 0 ? 1 : 0, OUT);
+    p->launches++;
+  }
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
 }
 
 int64_t bilinear_blocks(const gp_plan* p, int64_t n2) {
@@ -479,6 +547,7 @@ static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int
     case GP_MATERN12: GP_KROWS(GP_MATERN12); break;
     case GP_MATERN32: GP_KROWS(GP_MATERN32); break;
     case GP_RQ: GP_KROWS(RQ_K); break;
+    case GP_POLY: GP_KROWS(POLY_K); break;
     default: GP_KROWS(GP_MATERN52); break;
   }
 #undef GP_KROWS
@@ -499,7 +568,9 @@ extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
   if (p->kron) return kron_kdiag(p, OUT);
   if (p->deriv) return deriv_kdiag(p, OUT);
   if (p->lr_U) {   // diag(s K) - sum_j U_ij^2
-    if (p->backend == GP_BACKEND_SUM) {
+    if (p->backend == GP_BACKEND_SUM && sum_has_poly(p)) {
+      GP_CHECK(sum_kdiag_terms(p, OUT));   // a polynomial term's diagonal is not constant
+    } else if (p->backend == GP_BACKEND_SUM) {
       // a low-rank plan is square: every stationary term contributes its constant outputscale, added in term order
       float os = 0.f;
       for (gp_plan* t : p->terms) os += t->outputscale;
@@ -518,7 +589,12 @@ static int kdiag_base(gp_plan* p, float* OUT) {
   if (p->backend == GP_BACKEND_SKI) return ski_kdiag(p, OUT);   // not constant: w_i^T K_uu w_i (ski_rows.cuh)
   if (p->add_M) return additive_kdiag(p, OUT);   // square: the constant sum_m e_m(s); cross: per pair
   if (p->sm_Q) return spectral_kdiag(p, OUT);    // square: the constant S (sum_q w_q)^d; cross: per pair
-  if (p->same) {
+  if (p->same && p->kind == GP_POLY) {
+    // a dot-product kernel: S (|x_i|^2 + c)^p, row by row
+    const float* Z = p->Z2.as<float>() + p->row_begin * p->DP;
+    kdiag_cross_kernel<POLY_K><<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(Z, Z, p->DP, p->row_count, p->outputscale,
+                                                                                        OUT, cov_param(p));
+  } else if (p->same) {
     // stationary kernels: k(x,x) = outputscale (lazy_evaluated_kernel_tensor.py:107-133 evaluates kernel(diag=True))
     fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, p->outputscale);
   } else {
@@ -534,6 +610,7 @@ static int kdiag_base(gp_plan* p, float* OUT) {
       case GP_MATERN12: GP_KDIAG(GP_MATERN12); break;
       case GP_MATERN32: GP_KDIAG(GP_MATERN32); break;
       case GP_RQ: GP_KDIAG(RQ_K); break;
+      case GP_POLY: GP_KDIAG(POLY_K); break;
       default: GP_KDIAG(GP_MATERN52); break;
     }
 #undef GP_KDIAG
@@ -561,7 +638,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   if (p->per_n) return periodic_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   // before any launch: the SIMT derivative kernel is instantiated up to DP = 64
   GP_REQUIRE(p->backend == GP_BACKEND_SKI || p->DP <= 64, GP_E_SHAPE, "bilinear gradient supports d <= 64 (d=%d)", p->d);
-  const bool ard = p->ls.size() > 1;
+  bool ard = p->ls.size() > 1;
   if (p->backend == GP_BACKEND_SKI) {
     // interpolated operator: everything happens on the grid (ski.cu); one sweep per 16 columns
     std::vector<double> tot(1 + p->d, 0.0);
@@ -584,6 +661,8 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
     return GP_OK;
   }
   const bool rq = p->kind == GP_RQ;   // one more output: dF/dalpha
+  const bool poly = p->kind == GP_POLY;   // [dF/dc] and dF/dS: no lengthscale (ARD does not apply)
+  if (poly) ard = false;
   const int nls = ard ? p->d : 1;
   const int nout = 1 + nls + (rq ? 1 : 0);
   std::vector<double> total(nout, 0.0);
@@ -620,7 +699,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
       if (use_tc) {
         if (!p->tasks) GP_CHECK(pack_v_tiles(p, p->misc3.as<float>()));
         for (int pass = 0; pass < nout; ++pass) {
-          const int kind = pass == 0 ? p->kind : !rq ? GP_DERIV + p->kind : pass == 1 ? RQ_DL : RQ_DA;
+          const int kind = pass == 0 ? p->kind : poly ? POLY_DC : !rq ? GP_DERIV + p->kind : pass == 1 ? RQ_DL : RQ_DA;
           // a multitask plan runs both passes on K o B (tasks.cu), combined into slot 0 in user row order
           GP_CHECK(p->tasks ? tasks_kmv_partials(p, p->misc3.as<float>(), kind, nullptr) : kmv_tc_launch_kind(p, kind, nullptr));
           bilin_dot_kernel<<<dot_blocks, 256, 0, p->stream>>>(p->partial.as<float>(), p->nparts, p->row_count, rows_pad,
@@ -649,7 +728,9 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   }
   // d/d outputscale of os*k = k ; d/dl: scalar -> sum w g / l ; ARD -> sum w g dz_c^2/s / l_c ; both times os
   *grad_os = total[0];
-  if (ard)
+  if (poly)
+    grad_ls[0] = p->outputscale * total[1];   // dF/dc = S sum_ij w_ij p a_ij^(p-1)
+  else if (ard)
     for (int c = 0; c < p->d; ++c) grad_ls[c] = p->outputscale * total[1 + c] / (double)p->ls[c];
   else
     grad_ls[0] = p->outputscale * total[1] / (double)p->ls[0];

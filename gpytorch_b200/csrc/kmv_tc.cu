@@ -38,7 +38,9 @@
 // The same pipeline (tc_pipeline) also runs the product of two tensor-core factors (product_tc_kernel, product.cu): a second
 // GEMM1 operand with its own A tile and its own B tile per stage, a second GEMM1 chain in the same batch (S_b into hi, dead once
 // GEMM2 of the previous tile has read P_hi, so the live set stays s, hi, o1, o2, acc) and the product covariance in the
-// epilogue.  What a kernel computes per entry is its covariance source (TcOne, TcRq, TcProduct); the protocol exists once.
+// epilogue.  What a kernel computes per entry is its covariance source (TcOne, TcRq, TcPoly, TcProduct); the protocol exists once.
+// A source also says whether the exact diagonal of a square plan is forced to a = 0 (the stationary kinds) or not (TcPoly, whose
+// a_ii = |x_i|^2 + c comes out of GEMM1 like any other entry).
 #include "gp_common.cuh"
 #include "tc_ptx.cuh"
 
@@ -69,21 +71,31 @@ __device__ __forceinline__ float cov_tc(float a) {
 }
 
 // Covariance sources of the pipeline.  TWO: a second GEMM1 operand (S_b into hi); pair(a, b): the covariance of one entry from
-// its GEMM1 results (b = S_b, read only when TWO).
+// its GEMM1 results (b = S_b, read only when TWO); EXACT_DIAG: a square plan's diagonal entries are evaluated at a = 0.
 template <int KIND>
 struct TcOne {   // one operand of kind KIND (GP_DERIV + kind: l dk/dl for gp_bilinear_grad)
   static constexpr bool TWO = false;
+  static constexpr bool EXACT_DIAG = true;
   __device__ __forceinline__ float pair(float a, float) const { return cov_tc<KIND>(a); }
 };
 template <int KIND>
 struct TcRq {    // the RQ kernel: KIND = RQ_K (k), RQ_DL (l dk/dl) or RQ_DA (dk/dalpha); lg2 + ex2 per entry
   static constexpr bool TWO = false;
+  static constexpr bool EXACT_DIAG = true;
+  CovParam cp;
+  __device__ __forceinline__ float pair(float a, float) const { return cov_from_arg<KIND>(a, cp); }
+};
+template <int KIND>
+struct TcPoly {  // the polynomial kernel: KIND = POLY_K (a^p) or POLY_DC (p a^(p-1)), a = x_i.x_j + c from GEMM1; FMA pipe only
+  static constexpr bool TWO = false;
+  static constexpr bool EXACT_DIAG = false;
   CovParam cp;
   __device__ __forceinline__ float pair(float a, float) const { return cov_from_arg<KIND>(a, cp); }
 };
 template <bool RBF_A, bool RBF_B>
 struct TcProduct {   // k_a k_b = poly_a poly_b ex2(e_a + e_b): one ex2 per entry (cov_poly_exp, gp_common.cuh)
   static constexpr bool TWO = true;
+  static constexpr bool EXACT_DIAG = true;
   CovPoly ca, cb;
   __device__ __forceinline__ float pair(float a, float b) const {
     float pa, ea, pb, eb;
@@ -225,7 +237,7 @@ __device__ __forceinline__ void tc_pipeline(const Src src, const float* __restri
   // covariance P of tile u (S in s, S_b in hi) and its tf32 part P_hi (the fp32 residual P_lo is formed in run_gemm2)
   auto epilogue = [&](int u) {
     const int64_t d = diag_off - (int64_t)u * TILE_J;   // first row of this warpgroup - first column of the tile
-    if (same && d > -64 && d < TILE_J) {
+    if (Src::EXACT_DIAG && same && d > -64 && d < TILE_J) {
       const int dr = (int)d + wq * 16 + g - t;           // global row of register 0 - global column of register 0
 #pragma unroll
       for (int i = 0; i < 32; ++i)   // a_ii = 0 exactly (kernel.py:44-45 fills the diagonal with 0), for both operands
@@ -329,6 +341,16 @@ rq_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const f
               done_flag);
 }
 
+// the polynomial kernel (CODE = POLY_K or POLY_DC) with its per-plan power
+template <int CODE>
+__global__ void __maxnreg__(128)
+poly_tc_kernel(const float* __restrict__ XA, const float* __restrict__ XB, const float* __restrict__ Vt,
+               float* __restrict__ partial, int KP, int NS, int64_t ntile_j, int64_t tiles_per_split,
+               int64_t rows_pad, int same, int64_t row_begin, const int* __restrict__ done_flag, CovParam cp) {
+  tc_pipeline(TcPoly<CODE>{cp}, XA, nullptr, XB, nullptr, Vt, partial, KP, 0, NS, ntile_j, tiles_per_split, rows_pad, same,
+              row_begin, done_flag);
+}
+
 // two factors of a kernel product (product.cu), each from its own packed tiles XA_f / XB_f of width KP_f
 template <bool RBF_A, bool RBF_B>
 __global__ void __maxnreg__(128)
@@ -366,7 +388,12 @@ static int launch_tc_kind(gp_plan* p, const TcLaunch& a, const int* done_flag) {
   int smem_bytes = tc_smem_bytes(p->KP, &ns);
   GP_REQUIRE(ns >= 2, GP_E_SHAPE, "tensor-core path: smem ring too small for KP=%d", p->KP);
   dim3 grid((unsigned)p->ntile_i, (unsigned)a.nsplit);
-  if constexpr (is_rq_code(KIND)) {
+  if constexpr (is_poly_code(KIND)) {
+    GP_CHECK(opt_in_smem<poly_tc_kernel<KIND>>(p->device, 227 * 1024));
+    poly_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
+        a.XA, a.XB, a.Vt, a.partial, p->KP, ns, a.ntile_j, a.tiles_per_split, p->rows_pad, p->same ? 1 : 0, a.row_begin, done_flag,
+        cov_param(p));
+  } else if constexpr (is_rq_code(KIND)) {
     GP_CHECK(opt_in_smem<rq_tc_kernel<KIND>>(p->device, 227 * 1024));
     rq_tc_kernel<KIND><<<grid, TC_THREADS, smem_bytes, p->stream>>>(
         a.XA, a.XB, a.Vt, a.partial, p->KP, ns, a.ntile_j, a.tiles_per_split, p->rows_pad, p->same ? 1 : 0, a.row_begin, done_flag,
@@ -389,6 +416,14 @@ static int launch_tc_any(gp_plan* p, int kind, const TcLaunch& a, const int* don
       case RQ_DA: return launch_tc_kind<RQ_DA>(p, a, done_flag);
     }
     set_error("bad kernel code %d for a rational quadratic plan", kind);
+    return GP_E_SHAPE;
+  }
+  if (p->kind == GP_POLY) {   // GP_POLY is the number of GP_DERIV + GP_MATERN12
+    switch (rq_code(p, kind)) {
+      case POLY_K: return launch_tc_kind<POLY_K>(p, a, done_flag);
+      case POLY_DC: return launch_tc_kind<POLY_DC>(p, a, done_flag);
+    }
+    set_error("bad kernel code %d for a polynomial plan", kind);
     return GP_E_SHAPE;
   }
   switch (kind) {

@@ -164,6 +164,7 @@ int kron_refresh(gp_plan* p) {
   const gp_plan* q = ks->data;
   GP_CHECK(kron_check_data(p, q));
   GP_REFUSE_RQ(q, "a Kronecker operator (as the data plan)");
+  GP_REFUSE_POLY(q, "a Kronecker operator (as the data plan)");
   GP_REQUIRE(p->n1 == q->n1 * ks->T && p->n2 == q->n2 * ks->T && p->same == q->same, GP_E_STATE,
              "Kronecker plan: the data plan changed its size; call gp_plan_set_kron again");
   p->kind = q->kind;
@@ -375,6 +376,8 @@ extern "C" int gp_plan_set_kron(gp_plan* p, gp_plan* data, int T) {
   if (data) GP_REFUSE_PERIODIC(data, "gp_plan_set_kron (as the data plan)");
   GP_REFUSE_RQ(p, "gp_plan_set_kron");
   if (data) GP_REFUSE_RQ(data, "gp_plan_set_kron (as the data plan)");
+  GP_REFUSE_POLY(p, "gp_plan_set_kron");
+  if (data) GP_REFUSE_POLY(data, "gp_plan_set_kron (as the data plan)");
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   gp_kron_state* ks = p->kron ? p->kron : new gp_kron_state();
   const bool keep_b = p->kron && ks->T == T && ks->b_set;

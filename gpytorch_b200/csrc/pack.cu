@@ -50,9 +50,11 @@ __global__ void pack_simt_kernel(const float* __restrict__ X, int64_t n, int64_t
 }
 
 // one thread per (padded) row; writes KP floats as KP/4 float4 (coalesced across rows)
+// off >= 0: a polynomial plan (DESIGN 4.21).  Its rows are the raw inputs and the spare columns carry the offset instead of the
+// norms: A [z_hi | z_lo | z_hi | c_hi c_lo 1 1 | 0..], B [z_hi | z_hi | z_lo | 1 1 0 0 | 0..], so GEMM1 gives a = z_i.z_j + c
 template <bool IS_A>
 __global__ void pack_tc_kernel(const float* __restrict__ Z, int64_t row0, int64_t nrows_valid, int64_t nrows_pad,
-                               int d, int DP, int KP, int tile_rows, float* __restrict__ out) {
+                               int d, int DP, int KP, int tile_rows, float* __restrict__ out, float off) {
   int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;  // local padded row
   if (r >= nrows_pad) return;
   int64_t tile = r / tile_rows;
@@ -61,10 +63,12 @@ __global__ void pack_tc_kernel(const float* __restrict__ Z, int64_t row0, int64_
   float4* dst = reinterpret_cast<float4*>(out + tile * (int64_t)tile_rows * KP);
   const bool valid = r < nrows_valid;
   const float* z = Z + (row0 + r) * DP;
+  const bool poly = off >= 0.f;
   double nn = 0.0;
-  if (valid)
+  if (valid && !poly)
     for (int c = 0; c < d; ++c) nn += (double)z[c] * (double)z[c];
   nn *= -0.5;
+  if (poly && IS_A) nn = (double)off;   // B keeps n = 0: its columns (1, 1, 0, 0) pick c_hi + c_lo
   float n_hi = tf32_hi((float)nn);
   float n_lo = tf32_hi((float)(nn - (double)n_hi));
   for (int kc = 0; kc < KP / 4; ++kc) {
@@ -206,14 +210,19 @@ int pack_inputs(gp_plan* p) {
   // RQ: C = 1 (alpha stays out of the packing, so the value and both derivatives read the same a = -r^2 / 2)
   double cst = (p->kind == GP_RBF) ? 1.4426950408889634
                : (p->kind == GP_MATERN12 ? 2.0 : (p->kind == GP_MATERN32 ? 6.0 : (p->kind == GP_RQ ? 1.0 : 10.0)));
+  const bool poly = p->kind == GP_POLY;   // a dot-product kernel: the raw inputs, no centring and no scale (DESIGN 4.21)
   for (int c = 0; c < d; ++c) {
     double l = (p->ls.size() == 1) ? p->ls[0] : p->ls[c];
-    sc[c] = (float)(sqrt(cst) / l);
+    sc[c] = poly ? 1.f : (float)(sqrt(cst) / l);
   }
   GP_CUDA(cudaMemcpyAsync(p->scale.p, sc.data(), sizeof(float) * d, cudaMemcpyHostToDevice, st));
   GP_CUDA(cudaStreamSynchronize(st));  // sc is a stack-lifetime vector
-  col_mean_kernel<<<d, 256, 0, st>>>(p->X1, p->n1, p->ld1, d, p->mean.as<float>());
-  p->launches++;
+  if (poly) {
+    GP_CUDA(cudaMemsetAsync(p->mean.p, 0, sizeof(float) * d, st));
+  } else {
+    col_mean_kernel<<<d, 256, 0, st>>>(p->X1, p->n1, p->ld1, d, p->mean.as<float>());
+    p->launches++;
+  }
   const float* X2 = p->same ? p->X1 : p->X2;
   int64_t ld2 = p->same ? p->ld1 : p->ld2;
   GP_CHECK(p->Z2.ensure(sizeof(float) * p->n2 * DP));
@@ -239,8 +248,9 @@ int pack_inputs(gp_plan* p) {
     GP_CHECK(p->XB.ensure(sizeof(float) * padB * KP));
     const float* ZA = p->same ? p->Z2.as<float>() : p->Z1.as<float>();
     int64_t rowA0 = p->same ? p->row_begin : 0;
-    pack_tc_kernel<true><<<(unsigned)cdiv(padA, 128), 128, 0, st>>>(ZA, rowA0, p->row_count, padA, d, DP, KP, TILE_I, p->XA.as<float>());
-    pack_tc_kernel<false><<<(unsigned)cdiv(padB, 128), 128, 0, st>>>(p->Z2.as<float>(), 0, p->n2, padB, d, DP, KP, TILE_J, p->XB.as<float>());
+    const float off = poly ? p->poly_offset : -1.f;
+    pack_tc_kernel<true><<<(unsigned)cdiv(padA, 128), 128, 0, st>>>(ZA, rowA0, p->row_count, padA, d, DP, KP, TILE_I, p->XA.as<float>(), off);
+    pack_tc_kernel<false><<<(unsigned)cdiv(padB, 128), 128, 0, st>>>(p->Z2.as<float>(), 0, p->n2, padB, d, DP, KP, TILE_J, p->XB.as<float>(), off);
     p->launches += 2;
     GP_CHECK(p->Vtiles.ensure(sizeof(float) * p->ntile_j * (2 * TILE_J * TP + TILE_J * TP / 2)));
   }
@@ -262,8 +272,8 @@ int to_v16(gp_plan* p, const float* V, int64_t ldv, int t, int64_t n, float* V16
 // tensor-core operand tiles of rows [0, npad) of Z (rows >= nvalid zero): the A side (XA layout) or the B side (XB layout)
 int pack_tc_rows(gp_plan* p, const float* Z, int64_t nvalid, int64_t npad, bool is_a, float* out) {
   const int w = packed_dims(p);
-  if (is_a) pack_tc_kernel<true><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, w, p->DP, p->KP, TILE_I, out);
-  else pack_tc_kernel<false><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, w, p->DP, p->KP, TILE_J, out);
+  if (is_a) pack_tc_kernel<true><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, w, p->DP, p->KP, TILE_I, out, -1.f);
+  else pack_tc_kernel<false><<<(unsigned)cdiv(npad, 128), 128, 0, p->stream>>>(Z, 0, nvalid, npad, w, p->DP, p->KP, TILE_J, out, -1.f);
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;

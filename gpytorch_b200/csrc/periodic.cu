@@ -281,6 +281,7 @@ extern "C" int gp_plan_set_periodic(gp_plan* p, const float* period, int n_perio
   GP_REFUSE_ADDITIVE(p, "gp_plan_set_periodic");
   GP_REFUSE_SPECTRAL(p, "gp_plan_set_periodic");
   GP_REFUSE_RQ(p, "gp_plan_set_periodic");
+  GP_REFUSE_POLY(p, "gp_plan_set_periodic");
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_STATE,
              "a periodic plan is not available on a row-sharded plan");
   GP_REQUIRE(d >= 1 && d <= PER_DMAX, GP_E_SHAPE, "a periodic plan takes 1 <= d <= %d input dimensions (got d=%d)", PER_DMAX, d);

@@ -217,6 +217,7 @@ struct PcTerms {
   AddHyp ah;            // PC_KIND_ADDITIVE
   SmHyp sh;             // PC_KIND_SPECTRAL
   CovParam cp[4];       // each term's (PC_KIND_SUM) or the plain plan's (cp[0]) covariance parameters: an RQ term's alpha
+  int rank_stop;        // a polynomial plan or a sum with a polynomial term: a non-positive largest residual ends the factor
 };
 __device__ __forceinline__ int pc_task_of(const PcTerms& tt, int r) { return tt.task ? tt.task[r] : r % tt.rep; }
 __device__ __forceinline__ float pc_cov_rt(int kind, float a, CovParam cp) {
@@ -227,6 +228,20 @@ __device__ __forceinline__ float pc_cov_rt(int kind, float a, CovParam cp) {
     case GP_RQ: return cov_from_arg<RQ_K>(a, cp);
     default: return cov_from_arg<GP_MATERN52>(a, cp);
   }
+}
+// the initial diagonal of a plain polynomial plan (tt.n = 1) or of a sum with a polynomial term, term by term in term order:
+// os_t for a stationary term, os_t (|x_j|^2 + c_t)^p_t for a polynomial one; identity permutation; then pc_first_pivot_kernel
+__global__ void pc_init_dot_kernel(const PcTerms tt, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos, int64_t n) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  float v = 0.f;
+  for (int t = 0; t < tt.n; ++t) {
+    const float* z = tt.Z[t] + j * tt.DP[t];
+    v = fmaf(tt.os[t], tt.kind[t] == GP_POLY ? cov_from_arg<POLY_K>(poly_arg(z, z, tt.DP[t], tt.cp[t].offset), tt.cp[t]) : 1.f, v);
+  }
+  diag[j] = v;
+  perm[j] = (int)j;
+  pos[j] = (int)j;
 }
 
 struct PcPart {
@@ -300,6 +315,11 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
           int off = 0;
           for (int t = 0; t < tt.n; ++t) {
             const float* zj = tt.Z[t] + j * tt.DP[t];
+            if (tt.kind[t] == GP_POLY) {   // a polynomial term: a = x_pivot . x_j + c
+              v = fmaf(tt.os[t], cov_from_arg<POLY_K>(poly_arg(zp + off, zj, tt.DP[t], tt.cp[t].offset), tt.cp[t]), v);
+              off += tt.DP[t];
+              continue;
+            }
             float s = 0.f;
             for (int c = 0; c < tt.DP[t]; ++c) {
               float df = zp[off + c] - zj[c];
@@ -347,6 +367,8 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
           const float ua = a ? (zp[a - 1] - zj[a - 1]) * tt.dh->w[a - 1] : 0.f;
           const float ub = b ? (zp[b - 1] - zj[b - 1]) * tt.dh->w[b - 1] : 0.f;
           v = K::entry(K::pair(s).scaled(os), a, b, ua, ub, *tt.dh);
+        } else if constexpr (KIND == POLY_K) {
+          v = os * cov_from_arg<POLY_K>(poly_arg(zp, Z + j * DP, DP, tt.cp[0].offset), tt.cp[0]);
         } else {
           float s = 0.f;
           for (int c = 0; c < DP; ++c) {
@@ -430,7 +452,10 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
     const int ppw = s_pos[0], inew = s_idx[0], iold = s_old;
     bool stop = false, nan = false;
     if (m + 1 >= max_rank || (int64_t)(m + 1) >= n || !(err > tol)) stop = true;
-    else if (ppw < 0 || !(mx > 0.f)) { stop = true; nan = true; }
+    else if (ppw < 0 || !(mx > 0.f)) {   // NaN, or nothing positive left: on a polynomial operator (rank_stop) its rank is spent
+      stop = true;
+      nan = (KIND == POLY_K || KIND == PC_KIND_SUM) ? (ppw < 0 || !tt.rank_stop) : true;
+    }
     if (blockIdx.x == 0 && tid == 0) {
       st->rank = m + 1;
       st->err = err;
@@ -857,6 +882,12 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   } else {
     tt.cp[0] = cov_param(p);
   }
+  // a dot-product kernel's diagonal is not constant: a plain polynomial plan is staged as a one-term sum for the initial diagonal
+  const bool dot = p->kind == GP_POLY || (sum && sum_has_poly(p));
+  if (dot && !sum) {
+    tt.n = 1; tt.kind[0] = GP_POLY; tt.DP[0] = p->DP; tt.os[0] = p->outputscale; tt.Z[0] = p->Z2.as<float>();
+  }
+  tt.rank_stop = dot ? 1 : 0;
   if (prod) {   // os_total = S, dp_total = the factors' widths back to back (product_pack)
     tt.n = (int)p->factors.size();
     for (int t = 0; t < tt.n; ++t) {
@@ -908,6 +939,10 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     pc_init_ski_kernel<<<gb, PC_THREADS, 0, st>>>(sk, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;
+  } else if (dot) {
+    pc_init_dot_kernel<<<gb, PC_THREADS, 0, st>>>(tt, diag, perm, pos, n);
+    pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
+    p->launches += 2;
   } else {
     pc_init_kernel<<<gb, PC_THREADS, 0, st>>>(diag, perm, pos, n, os_total, S, piv);   // stationary terms: constant initial diagonal
     p->launches += 1;
@@ -923,6 +958,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_REQUIRE(!deriv || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a derivative operator needs the cooperative kernel");
   GP_REQUIRE(!add || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of an additive operator needs the cooperative kernel");
   GP_REQUIRE(!spec || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a spectral mixture operator needs the cooperative kernel");
+  GP_REQUIRE(!dot || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a polynomial operator needs the cooperative kernel");
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
@@ -936,6 +972,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       case GP_MATERN12: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN12>; break;
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
       case GP_RQ: fn1 = (const void*)pc_persistent1_kernel<RQ_K>; break;
+      case GP_POLY: fn1 = (const void*)pc_persistent1_kernel<POLY_K>; break;
       case PC_KIND_SUM: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SUM>; break;
       case PC_KIND_PRODUCT: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_PRODUCT>; break;
       case PC_KIND_SKI: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SKI>; break;
@@ -1039,6 +1076,21 @@ extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, do
   return GP_OK;
 }
 
+// sum of the per-row diagonal (gp_kdiag's) of a polynomial plan or of a sum with a polynomial term, in fp64 in row order
+static int dot_diag_sum(gp_plan* p, double* out) {
+  const int64_t n = p->n2;
+  GP_CHECK(p->misc.ensure(sizeof(float) * n));
+  if (p->backend == GP_BACKEND_SUM) GP_CHECK(sum_kdiag_terms(p, p->misc.as<float>()));
+  else GP_CHECK(gp_kdiag(p, p->misc.as<float>()));
+  std::vector<float> h(n);
+  GP_CUDA(cudaMemcpyAsync(h.data(), p->misc.p, sizeof(float) * n, cudaMemcpyDeviceToHost, p->stream));
+  GP_CUDA(cudaStreamSynchronize(p->stream));
+  double s = 0.0;
+  for (int64_t i = 0; i < n; ++i) s += (double)h[i];
+  *out = s;
+  return GP_OK;
+}
+
 extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U, double* trace_resid_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_REFUSE_LOWRANK(p, "gp_ciq_precond_build");
@@ -1101,7 +1153,9 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   // w_i^T K_uu w_i varies from row to row and is summed in fp64
   if (p->backend == GP_BACKEND_PRODUCT) GP_CHECK(product_refresh(p));   // the constant diagonal S = prod_f s_f
   double tr_k = (double)n * p->outputscale;
-  if (p->backend == GP_BACKEND_SUM) {
+  if (p->kind == GP_POLY || (p->backend == GP_BACKEND_SUM && sum_has_poly(p))) {
+    GP_CHECK(dot_diag_sum(p, &tr_k));   // a polynomial diagonal S (|x_i|^2 + c)^p varies from row to row
+  } else if (p->backend == GP_BACKEND_SUM) {
     double os_total = 0.0;
     for (const gp_plan* q : p->terms) os_total += q->outputscale;
     tr_k = (double)n * os_total;

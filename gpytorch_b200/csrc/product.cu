@@ -294,6 +294,7 @@ int product_pack(gp_plan* p) {
                "kernel product: a factor must be a plain kernel plan (not SKI, not a sum, not a product, not multitask, not derivative)");
     GP_REQUIRE(q->tasks == nullptr, GP_E_STATE, "kernel product: a factor with task indices is not available");
     GP_REQUIRE(q->kind != GP_RQ, GP_E_STATE, "kernel product: a rational quadratic factor is not available (gp_plan_set_hypers_rq)");
+    GP_REQUIRE(q->kind != GP_POLY, GP_E_STATE, "kernel product: a polynomial factor is not available (gp_plan_set_hypers_poly)");
     GP_REQUIRE(q->lr_U == nullptr, GP_E_STATE, "kernel product: a factor with a low-rank correction is not available");
     GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
                "kernel product: a row-sharded factor is not available");
@@ -449,6 +450,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   GP_REFUSE_SPECTRAL(p, "gp_plan_set_product");
   GP_REFUSE_PERIODIC(p, "gp_plan_set_product");
   GP_REFUSE_RQ(p, "gp_plan_set_product");
+  GP_REFUSE_POLY(p, "gp_plan_set_product");
   GP_CUDA(cudaSetDevice(p->device));
   if (factors == nullptr || n_factors == 0) {   // back to a plain plan
     if (p->backend_req != GP_BACKEND_PRODUCT) return GP_OK;
@@ -468,6 +470,9 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   for (int f = 0; f < n_factors; ++f)
     GP_REQUIRE(factors[f] == nullptr || factors[f]->kind != GP_RQ, GP_E_STATE,
                "gp_plan_set_product: a rational quadratic plan as a factor is not available (gp_plan_set_hypers_rq)");
+  for (int f = 0; f < n_factors; ++f)
+    GP_REQUIRE(factors[f] == nullptr || factors[f]->kind != GP_POLY, GP_E_STATE,
+               "gp_plan_set_product: a polynomial plan as a factor is not available (gp_plan_set_hypers_poly)");
   }
   p->factors.assign(factors, factors + n_factors);
   p->backend_req = GP_BACKEND_PRODUCT;

@@ -453,6 +453,7 @@ extern "C" int gp_plan_set_spectral(gp_plan* p, int Q, const float* weights, con
   GP_REFUSE_ADDITIVE(p, "gp_plan_set_spectral");
   GP_REFUSE_PERIODIC(p, "gp_plan_set_spectral");
   GP_REFUSE_RQ(p, "gp_plan_set_spectral");
+  GP_REFUSE_POLY(p, "gp_plan_set_spectral");
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,
              "a spectral plan is not available on a row-sharded plan");
   GP_REQUIRE(Q >= 1 && Q <= SM_QMAX && d >= 1 && d <= SM_DMAX && Q * d <= SM_QDMAX, GP_E_SHAPE,

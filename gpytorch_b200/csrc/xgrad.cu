@@ -9,6 +9,10 @@
 // so  DX1_i = -s sqrt(C)/l (.) sum_j w_ij q_ij (z_i - z_j)  and DX2_j the same with the roles swapped.  On a square plan both
 // arguments are the same points: DX_i = -s sqrt(C)/l (.) sum_j (w_ij + w_ji) q_ij (z_i - z_j).  A pair at distance 0 contributes 0
 // (the clamps of kernels/kernel.py:52-60 give the same; the stationary diagonal has zero input gradient).
+// Polynomial plans (DESIGN 4.21) are not of the difference form: over the raw inputs (scale 1, no centring) a = x_i . x_j + c and
+//   dk_ij/dx_i = s q_ij x_j,   q = p a^(p-1)  (hcov_from_arg<POLY_K>)
+// so the kernel accumulates -w q x_j (the finish kernel's sign turns it back) and no pair is masked: on a square plan the diagonal
+// pair adds (w_ii + w_ii) q_ii x_i, the derivative of k(x_i, x_i) = (|x_i|^2 + c)^p through both of its arguments.
 //
 // One kernel, two roles: a thread owns the row that receives the gradient ("own" side, Zo) and streams staged 64-row tiles of the
 // other side (Zt), forming z_i - z_j by direct differences as kmv_simt_kernel does (no cancellation).  The reduced side is split
@@ -65,6 +69,15 @@ xgrad_kernel(const float* __restrict__ Zo, const float* __restrict__ Zt, int64_t
         const int64_t j = j0 + jj;
         w = W[i * sr + j * sc];
         if (sym) w += W[j * sr + i * sc];
+      }
+      if constexpr (KIND == POLY_K) {
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < DP; ++c) s = fmaf(zi[c], zj[jj][c], s);
+        const float wq = -w * hcov_from_arg<KIND>(s + cp.offset, cp);
+#pragma unroll
+        for (int c = 0; c < DP; ++c) acc[c] = fmaf(wq, zj[jj][c], acc[c]);
+        continue;
       }
       float s = 0.f;
 #pragma unroll
@@ -155,6 +168,7 @@ static int launch_xgrad_kind(gp_plan* p, dim3 grid, const XgArgs& a) {
     case GP_MATERN32: return launch_xgrad<GP_MATERN32, TW>(p, grid, a);
     case GP_MATERN52: return launch_xgrad<GP_MATERN52, TW>(p, grid, a);
     case GP_RQ: return launch_xgrad<RQ_K, TW>(p, grid, a);
+    case GP_POLY: return launch_xgrad<POLY_K, TW>(p, grid, a);
   }
   set_error("bad kernel kind %d", p->kind);
   return GP_E_SHAPE;

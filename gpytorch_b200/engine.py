@@ -120,6 +120,18 @@ class Plan:
         # recorded once the engine took them: bilinear_grad sizes its output by these lengthscales
         self.kind, self.lengthscale, self.outputscale, self.noise = kind, ls, float(outputscale), float(noise)
         self.alpha = None
+        self.poly = None
+        return self
+
+    def set_hypers_poly(self, power: int, offset: float, outputscale: float = 1.0, noise: float = 0.0):
+        """Polynomial kernel S (x.x' + c)^p over the raw inputs (gp_plan_set_hypers_poly): kind, integer power 1..8, offset c >= 0,
+        outputscale and noise in one engine call.  bilinear_grad then returns [dc] and dF/dS (the power is not learned)."""
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_hypers_poly(self._h, int(power), float(offset), float(outputscale), float(noise)))
+        # recorded once the engine took them: bilinear_grad sizes its output by the kind
+        self.kind, self.lengthscale, self.outputscale, self.noise = "poly", [], float(outputscale), float(noise)
+        self.alpha = None
+        self.poly = (int(power), float(offset))
         return self
 
     def set_hypers_rq(self, lengthscale, alpha: float, outputscale: float = 1.0, noise: float = 0.0):
@@ -132,6 +144,7 @@ class Plan:
         # recorded once the engine took them: bilinear_grad sizes its output by the lengthscales and alpha
         self.kind, self.lengthscale, self.outputscale, self.noise = "rq", ls, float(outputscale), float(noise)
         self.alpha = float(alpha)
+        self.poly = None
         return self
 
     def set_ski(self, grid_sizes, grid_lo, grid_step):
@@ -396,7 +409,7 @@ class Plan:
         product: the factors' lengthscale gradients one after the other, and the gradient of the combined scale S.  On an additive
         plan: the D lengthscale gradients and the list of the D component-scale gradients.  On a spectral plan: the Q (1 + 2d)
         gradients [dw | dmu | dv] and dF/dS.  On a periodic plan: [dl | dp] and dF/dS.  On a rational quadratic plan: [dl | dalpha]
-        and dF/dS."""
+        and dF/dS.  On a polynomial plan: [dc] and dF/dS."""
         if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.row_count or right.size(0) != self.n2 \
                 or left.size(1) != right.size(1) or left.size(1) < 1:
             raise RuntimeError(f"bilinear_grad: left must be [{self.row_count}, s] and right [{self.n2}, s] with s >= 1 "
@@ -412,6 +425,8 @@ class Plan:
         nls = sum(len(f.lengthscale) for f in factors) if factors else len(self.lengthscale)
         if not factors and getattr(self, "alpha", None) is not None:   # [dl | dalpha] and dF/dS
             nls += 1
+        if not factors and getattr(self, "poly", None) is not None:    # [dc] and dF/dS
+            nls = 1
         gl = (C.c_double * nls)()
         if getattr(self, "_spectral", None) is not None:   # [dw | dmu | dv] and dF/dS
             Q, d = self._spectral

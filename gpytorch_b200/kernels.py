@@ -1,4 +1,4 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, RQKernel, SpectralMixtureKernel,
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, RQKernel, PolynomialKernel, SpectralMixtureKernel,
 PeriodicKernel, ScaleKernel, AdditiveKernel, ProductKernel, GridInterpolationKernel} for the accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
@@ -217,6 +217,54 @@ class RQKernel(_StationaryKernel):
 def _is_rq(k):
     """k is an RQKernel, or a ScaleKernel around one."""
     return isinstance(k, RQKernel) or isinstance(getattr(k, "base_kernel", None), RQKernel)
+
+
+class PolynomialKernel(Kernel):
+    """k = (x1 . x2 + c)^p over the raw inputs (kernels/polynomial_kernel.py).  Parameters as in the reference: the integer power
+    (an int, an integral float or a one-element tensor, 1..8 on the accelerated path) and raw_offset [*B, 1] with a Positive()
+    constraint unless one is given.  forward returns one engine PolynomialKernelLinearOperator (gp_plan_set_hypers_poly) on the
+    tensor-core or CUDA-core K.V; inside a ScaleKernel the outputscale multiplies it, and scaled or not it may be a term of an
+    AdditiveKernel.  One batch dimension at most, no priors.  The kernel is not stationary (no lengthscale, no centring), so it is
+    not a _StationaryKernel: products, SKI, multitask, additive-component and derivative kernels do not take it."""
+    kind = "poly"
+
+    def __init__(self, power, offset_prior=None, offset_constraint=None, **kwargs):
+        if offset_prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        super().__init__(**kwargs)
+        if torch.is_tensor(power):
+            if power.numel() != 1:
+                raise NotImplementedError("PolynomialKernel: power must be one integer")
+            power = power.item()
+        if isinstance(power, bool) or not isinstance(power, (int, float)) or float(power) != int(power):
+            raise NotImplementedError(f"PolynomialKernel: power must be an integer (got {power!r})")
+        power = int(power)
+        if not 1 <= power <= 8:
+            raise NotImplementedError(f"PolynomialKernel: power {power} is not available on the accelerated path (1 to 8)")
+        self.power = power
+        self.register_parameter("raw_offset", torch.nn.Parameter(torch.zeros(*self.batch_shape, 1)))
+        self.register_constraint("raw_offset", offset_constraint or Positive())
+
+    @property
+    def offset(self):
+        return self.raw_offset_constraint.transform(self.raw_offset)
+
+    @offset.setter
+    def offset(self, value):
+        self._set_offset(value)
+
+    def _set_offset(self, value):
+        self._set_constrained("raw_offset", value)
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, outputscale=None, last_dim_is_batch=False, **params):
+        from .operators import PolynomialKernelLinearOperator
+        if last_dim_is_batch:
+            raise NotImplementedError("last_dim_is_batch is not available for a PolynomialKernel on the accelerated path")
+        if diag and not (_same or x1.size(0) == x2.size(0)):
+            raise RuntimeError("diag=True needs x1 and x2 of equal sizes")
+        off = self.offset if _batch_index is None else self.offset[_batch_index]
+        op = PolynomialKernelLinearOperator(x1, None if _same else x2, self.power, off.reshape(-1)[0], outputscale)
+        return op.diagonal() if diag else op
 
 
 class Matern52KernelGrad(MaternKernel):
@@ -493,7 +541,7 @@ class ScaleKernel(Kernel):
             first = KernelLinearOperator(f[0].x1, f[0].x2, f[0].kind, f[0].lengthscale, self.outputscale * f[0].outputscale)
             op = ProductKernelLinearOperator([first, *f[1:]])
             return op.diagonal() if diag else op
-        if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel, RQKernel)):   # S folded into the same operator
+        if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel, RQKernel, PolynomialKernel)):   # S folded in
             os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
             return self.base_kernel.forward(x1, x2, diag=diag, _same=_same, _batch_index=bi, outputscale=os_, **params)
         if isinstance(self.base_kernel, GridInterpolationKernel):
@@ -508,8 +556,10 @@ class ScaleKernel(Kernel):
         if isinstance(base, SKIKernelLinearOperator):
             op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
             return op.diagonal() if diag else op
-        from .operators import PeriodicKernelLinearOperator, RQKernelLinearOperator, SumKernelLinearOperator, with_outputscale
-        keep = (PeriodicKernelLinearOperator, RQKernelLinearOperator)   # operators with parameters beyond lengthscale and scale
+        from .operators import (PeriodicKernelLinearOperator, PolynomialKernelLinearOperator, RQKernelLinearOperator,
+                                SumKernelLinearOperator, with_outputscale)
+        # operators with parameters beyond lengthscale and scale
+        keep = (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator)
         if isinstance(base, keep):   # a nested ScaleKernel: both scales folded in, the period / alpha kept
             op = with_outputscale(base, os_ * base.outputscale)
             return op.diagonal() if diag else op

@@ -448,8 +448,8 @@ class KernelLinearOperator(_SamplingMixin):
         (gp_plan_set_tasks).  RBF / Matern operators, optionally scaled, only.  With another RBF / Matern kernel operator (or a
         product of them) of the same shape: the elementwise product K_1 o K_2 as one engine operator (gp_plan_set_product)."""
         plain = (KernelLinearOperator, ProductKernelLinearOperator)
-        if isinstance(other, RQKernelLinearOperator):
-            return other.mul(self)   # refused, naming RQ
+        if isinstance(other, (RQKernelLinearOperator, PolynomialKernelLinearOperator)):
+            return other.mul(self)   # refused, naming the kernel
         if type(self) in plain and type(other) in plain:
             return ProductKernelLinearOperator([self, other])
         if not isinstance(other, IndexLinearOperator) or type(self) is not KernelLinearOperator:
@@ -898,7 +898,8 @@ class SumKernelLinearOperator(KernelLinearOperator):
             if isinstance(o, PeriodicKernelLinearOperator):   # keeps its period, on a slot no plain term uses
                 t = o._with(o.x1, None if o.same else o.x2)
                 t._plan_slot = _PERIODIC_SUM_SLOT + i
-            elif isinstance(o, RQKernelLinearOperator):       # keeps alpha, on the plain term slot (kind and alpha are in its key)
+            elif isinstance(o, (RQKernelLinearOperator, PolynomialKernelLinearOperator)):
+                # keeps alpha / power and offset, on the plain term slot (the kind and those parameters are in its key)
                 t = o._with(o.x1, None if o.same else o.x2)
                 t._plan_slot = 1 + i
             else:
@@ -1028,6 +1029,9 @@ class ProductKernelLinearOperator(KernelLinearOperator):
             if isinstance(o, RQKernelLinearOperator):
                 raise NotImplementedError("products that contain a rational quadratic (RQ) operator are not available on the "
                                           "accelerated path")
+            if isinstance(o, PolynomialKernelLinearOperator):
+                raise NotImplementedError("products that contain a PolynomialKernel operator are not available on the accelerated "
+                                          "path")
             if type(o) is not KernelLinearOperator:
                 raise NotImplementedError("the factors of a kernel product must be RBF / Matern kernel operators (optionally scaled) "
                                           "on the accelerated path")
@@ -1690,10 +1694,102 @@ class RQKernelLinearOperator(KernelLinearOperator):
     __mul__ = mul
 
 
+class PolynomialKernelLinearOperator(KernelLinearOperator):
+    """S (x1 . x2 + c)^p (kernels/polynomial_kernel.py, which forms the dense matrix with addmm(...).pow(p)) as ONE engine plan of
+    kind GP_POLY (gp_plan_set_hypers_poly) over the raw inputs: products, solves, the preconditioner, SLQ, rows and input gradients
+    run on the plain tensor-core / CUDA-core kernels with (x . x' + c)^p in their epilogue.  power is a Python int in [1, 8], offset
+    one value (the parameter tensor or its slice for one element of a batch); autograd reaches the offset and S through
+    _bilinear_derivative_list.  The kernel is not stationary: diagonal() is S (|x_i|^2 + c)^p from the plan.  The plan-cache slots
+    are the plain ones: kind, power and offset are part of the plan's hyper-parameter key."""
+
+    def __init__(self, x1, x2, power, offset, outputscale=None, comm=None, row_begin=0, row_count=0):
+        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
+            raise NotImplementedError("a row-sharded polynomial operator is not available on the accelerated path")
+        if offset.numel() != 1:
+            raise RuntimeError(f"polynomial kernel: offset must hold one value (got shape {tuple(offset.shape)})")
+        # no lengthscale: a constant stands in where the generic code reads one (device / dtype only)
+        super().__init__(x1, x2, "poly", torch.ones((), device=x1.device, dtype=offset.dtype), outputscale)
+        self.power = int(power)
+        self.offset = offset
+
+    def hyper_tensors(self):
+        return [self.offset, self.outputscale]
+
+    @property
+    def requires_grad(self):
+        return any(t.requires_grad for t in self.hyper_tensors())
+
+    def representation(self):
+        return (self.x1, self.x2, *self.hyper_tensors())
+
+    def _host_hypers(self, noise_t=None):
+        """(offset, outputscale, noise, noise tensor) with one device -> host read."""
+        cached = getattr(self, "_hyp_host", None)
+        if cached is None or (noise_t is not None and cached[3] is not noise_t):
+            parts = [t.detach().reshape(-1).float().to(self.device) for t in (self.offset, self.outputscale)]
+            if noise_t is not None:
+                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.device))
+            vals = torch.cat(parts).tolist()
+            cached = (vals[0], vals[1], vals[2] if noise_t is not None else None, noise_t)
+            self._hyp_host = cached
+        return cached
+
+    def plan(self, noise=0.0) -> Plan:
+        fresh = False
+        if self._plan is None:
+            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None,
+                                   getattr(self, "_plan_slot", 0), owner=self)
+            fresh = True
+        if torch.is_tensor(noise):
+            off, os_, nz, _ = self._host_hypers(noise)
+        else:
+            off, os_, _, _ = self._host_hypers(None)
+            nz = float(noise)
+        key = ("poly", self.power, off, os_, nz)
+        if fresh or getattr(self._plan, "_hyp_key", None) != key:
+            self._plan.set_hypers_poly(self.power, off, os_, nz)
+            self._plan._hyp_key = key
+        return self._plan
+
+    def _bilinear_derivative_list(self, left, right):
+        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
+        return [torch.tensor(gl[0], device=self.device, dtype=self.offset.dtype).reshape(self.offset.shape),
+                torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape)]
+
+    def _bilinear_derivative(self, left, right):
+        raise NotImplementedError("a polynomial operator has offset and outputscale gradients: use _bilinear_derivative_list")
+
+    def _with(self, x1, x2, detach=False, outputscale=None):
+        f = (lambda t: t.detach()) if detach else (lambda t: t)
+        return PolynomialKernelLinearOperator(f(x1), None if x2 is None else f(x2), self.power, f(self.offset),
+                                              f(self.outputscale if outputscale is None else outputscale))
+
+    def _transpose_nonbatch(self):
+        return self if self.same else self._with(self.x2, self.x1)
+
+    def detach(self):
+        return self._with(self.x1, None if self.same else self.x2, detach=True)
+
+    def __getitem__(self, index):
+        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
+
+    def mul(self, other):
+        raise NotImplementedError("products that contain a PolynomialKernel operator (kernel products, IndexKernel multitask "
+                                  "models) are not available on the accelerated path")
+
+    __mul__ = mul
+
+
 def with_outputscale(op, outputscale):
-    """A plain, periodic or RQ kernel operator with its outputscale replaced (a ScaleKernel folded into the terms of a sum or into
-    the first factor of a product); the operator's other parameters are kept."""
-    if isinstance(op, (PeriodicKernelLinearOperator, RQKernelLinearOperator)):
+    """A plain, periodic, RQ or polynomial kernel operator with its outputscale replaced (a ScaleKernel folded into the terms of a
+    sum or into the first factor of a product); the operator's other parameters are kept."""
+    if isinstance(op, (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator)):
         return op._with(op.x1, None if op.same else op.x2, outputscale=outputscale)
     return KernelLinearOperator(op.x1, op.x2, op.kind, op.lengthscale, outputscale)
 

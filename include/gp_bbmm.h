@@ -41,8 +41,9 @@ enum {
 };
 
 /* covariance function kinds: kernels/rbf_kernel.py:68-85, kernels/matern_kernel.py:85-110, kernels/rq_kernel.py (GP_RQ is set
- * through gp_plan_set_hypers_rq only, which also gives alpha) */
-enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3, GP_RQ = 4 };
+ * through gp_plan_set_hypers_rq only, which also gives alpha), kernels/polynomial_kernel.py (GP_POLY is set through
+ * gp_plan_set_hypers_poly only, which also gives the power and the offset) */
+enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3, GP_RQ = 4, GP_POLY = 5 };
 
 /* which fused K.V kernel runs: GP_BACKEND_TCGEN05 = wgmma/bulk-TMA 3xTF32 tensor-core kernel
  * (the name is historical),
@@ -232,6 +233,31 @@ int gp_plan_set_periodic(gp_plan* plan, const float* period, int n_period, int d
  * multitask, derivative, additive, spectral, periodic or row-sharded plan cannot take this call (GP_E_STATE). */
 int gp_plan_set_hypers_rq(gp_plan* plan, const float* lengthscale, int n_ls, float alpha, float outputscale, float noise);
 
+/* Polynomial kernels (the reference's PolynomialKernel, kernels/polynomial_kernel.py): kind GP_POLY with its integer power p and
+ * offset c, set together with the outputscale S and the noise in one call:
+ *   K(x, x') = S (x . x' + c)^p
+ * (+ its noise / per-row diagonal where a call adds it) over the raw inputs: no lengthscale and no centring.  x . x' + c may be
+ * negative; an odd power keeps its sign.  1 <= p <= 8 and c finite and >= 0, else GP_E_SHAPE.  The call is all or nothing: a failed
+ * call leaves the plan's previous hyper-parameters in place.  gp_plan_set_hypers with kind GP_POLY returns GP_E_SHAPE, so a plan
+ * never holds kind GP_POLY without its power; a later gp_plan_set_hypers with another kind makes the plan a plain plan of that kind.
+ * A plain plan, square or cross, on the tensor-core backend (the same widths as RBF: 3d + 4 <= the tensor-core limit) or the CUDA-core
+ * one.  The tensor-core operands carry c in their spare columns, so GEMM1 gives a = x_i . x_j + c in 3xTF32 and the epilogue is
+ * p - 1 multiplies at most (DESIGN 4.21).  The kernel is not stationary: its diagonal S (|x_i|^2 + c)^p varies from row to row.
+ * gp_kmv, gp_krows, gp_kdiag (square: S (|x_i|^2 + c)^p per row; on a low-rank-corrected base that minus sum_j U_ij^2; on a sum with
+ * a polynomial term the per-row sum of the terms' diagonals), gp_pivoted_cholesky (from that diagonal, first pivot its argmax,
+ * earliest index on ties; a factor of a rank-deficient K ends, without GP_W_PIVCHOL_NAN, where no positive residual is left),
+ * gp_precond_build, gp_precond_probes, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build (its
+ * trace from the same diagonal), gp_ciq_sqrt_matmul_precond, gp_plan_set_backend, gp_plan_set_noise_diag, gp_plan_set_lowrank (as
+ * the base), gp_kmv_input_grad, gp_kdense_input_grad and gp_time_kmv_kernel run on it, and it may be a term of gp_plan_set_sum.
+ * gp_bilinear_grad returns one double in grad_ls, [dF/dc], and dF/dS in grad_os (the power is not learned); a non-finite input makes
+ * them NaN.  The input gradients use dk/dx_i = S p (x_i . x_j + c)^(p-1) x_j: every pair contributes, and on a square plan the
+ * diagonal pair contributes 2 S p (|x_i|^2 + c)^(p-1) x_i.  On a polynomial plan gp_plan_set_tasks, gp_plan_set_kron,
+ * gp_plan_set_deriv, gp_plan_set_deriv_kind, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_spectral,
+ * gp_plan_set_periodic and gp_plan_set_comm with more than one rank return GP_E_STATE with a message naming the call; a polynomial
+ * plan as a factor of gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.  A SKI,
+ * sum, product, multitask, derivative, additive, spectral, periodic or row-sharded plan cannot take this call (GP_E_STATE). */
+int gp_plan_set_hypers_poly(gp_plan* plan, int power, float offset, float outputscale, float noise);
+
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
  * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
  * (+ its noise / per-row diagonal where a call adds it).  U: device [n, r] fp32, leading dimension ldu, caller-owned, must outlive
@@ -335,7 +361,8 @@ int gp_bilinear_grad(gp_plan* plan, const float* Lf, int64_t ldl, const float* R
  * kernels/matern_kernel.py:86-107, w.r.t. x1 / x2): DX1 = dF/dX1 [n1][d] (ld1), DX2 = dF/dX2 [n2][d] (ld2), in raw input units
  * with the outputscale folded in and the noise excluded, for F = sum_ic G_ic (K V)_ic; G [n1, t] ldg, V [n2, t] ldv, any t >= 1.
  * Either output may be NULL; on a square plan (X2 == X1) DX1 gets the total gradient and DX2 must be NULL.  A pair at distance 0
- * contributes 0; a non-finite input gives NaN outputs.  Repeated calls give identical bits (no atomics).
+ * contributes 0 for the stationary kinds; on a polynomial plan (GP_POLY) every pair contributes S p a^(p-1) x_j, a = x_i . x_j + c,
+ * the diagonal pair of a square plan 2 S p a_ii^(p-1) x_i.  A non-finite input gives NaN outputs.  Repeated calls give identical bits (no atomics).
  * GP_E_SHAPE on SKI, kernel-sum (call on every term) and row-sharded plans, for bad shapes, t < 1 or d > 64; GP_E_STATE on a
  * plan with a low-rank correction. */
 int gp_kmv_input_grad(gp_plan* plan, const float* G, int64_t ldg, const float* V, int64_t ldv, int t,
