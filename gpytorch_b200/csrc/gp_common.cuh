@@ -454,8 +454,12 @@ __device__ __forceinline__ float sqrt_approx(float x) {
   return y;
 }
 // round-to-nearest (ties away) to tf32: the tensor core truncates fp32 containers to their top 19 bits,
-// so operands are pre-rounded and the 2-term split x = hi + lo is exact to ~2^-24 |x|.
-__device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
+// so operands are pre-rounded and the 2-term split x = hi + lo is exact to ~2^-24 |x|.  A NaN keeps its bits: the rounding add
+// would carry the payload of CUDA's canonical NaN 0x7fffffff (what fmaf returns for a NaN operand) into the sign bit, giving -0.
+__device__ __forceinline__ float tf32_hi(float x) {
+  const uint32_t u = __float_as_uint(x);
+  return (u & 0x7fffffffu) > 0x7f800000u ? x : __uint_as_float((u + 0x1000u) & 0xFFFFE000u);
+}
 
 // covariance from a = -0.5 |z_i - z_j|^2 in the pre-scaled units of pack.cu:
 //   RBF     z = (x - mean) sqrt(log2 e) / l      k = 2^a                (rbf_covariance.py:19)

@@ -52,18 +52,9 @@ def ring_depth(KP):
     return min(MAX_NS, (226 * 1024 - a_bytes - TC_BARS_BYTES) // stage)
 
 
-def geometry(n1, n2, d, backend="auto", n_sm=132, row_count=None):
-    """pack.cu's choose_geometry for a plan over row_count (default n1) rows and n2 columns: the backend, DP, KP, the ring depth
-    NS (tensor cores), nsplit, the tiles per split T, the tiles of the last split and the columns per SIMT split."""
-    rows = row_count or n1
-    DP, KP = bo.dp_of(d), bo.kp_of(d)
-    if backend == "auto":
-        backend = "tcgen05" if KP <= KP_MAX else "simt"
-    tc = backend == "tcgen05"
-    rows_pad = cdiv(rows, 2 * TILE_I) * 2 * TILE_I
-    ntile_i, ntile_j = rows_pad // TILE_I, cdiv(n2, TILE_J)
-    nti = ntile_i if tc else cdiv(rows, SIMT_TI)
-    ntj = ntile_j                                   # SIMT_TJ == TILE_J
+def split_rule(nti, ntj, n_sm, tc):
+    """(tiles per split, nsplit) of choose_geometry (pack.cu) and segment_split (tasks.cu) for nti row units and ntj column
+    tiles: the fewest splits of at least 8 tiles that best fill 2 (tensor cores) or 1 (SIMT) CTAs per SM."""
     slots = n_sm * (2 if tc else 1)
     best, best_eff = 1, -1.0
     for s in range(1, 17):
@@ -77,7 +68,22 @@ def geometry(n1, n2, d, backend="auto", n_sm=132, row_count=None):
         if eff > best_eff + 0.02:
             best_eff, best = eff, s
     tps = cdiv(ntj, best)
-    nsplit = cdiv(ntj, tps)
+    return tps, cdiv(ntj, tps)
+
+
+def geometry(n1, n2, d, backend="auto", n_sm=132, row_count=None):
+    """pack.cu's choose_geometry for a plan over row_count (default n1) rows and n2 columns: the backend, DP, KP, the ring depth
+    NS (tensor cores), nsplit, the tiles per split T, the tiles of the last split and the columns per SIMT split."""
+    rows = row_count or n1
+    DP, KP = bo.dp_of(d), bo.kp_of(d)
+    if backend == "auto":
+        backend = "tcgen05" if KP <= KP_MAX else "simt"
+    tc = backend == "tcgen05"
+    rows_pad = cdiv(rows, 2 * TILE_I) * 2 * TILE_I
+    ntile_i, ntile_j = rows_pad // TILE_I, cdiv(n2, TILE_J)
+    nti = ntile_i if tc else cdiv(rows, SIMT_TI)
+    ntj = ntile_j                                   # SIMT_TJ == TILE_J
+    tps, nsplit = split_rule(nti, ntj, n_sm, tc)
     return {"backend": backend, "DP": DP, "KP": KP, "NS": ring_depth(KP) if tc else None, "rows_pad": rows_pad,
             "ntile_i": ntile_i, "ntile_j": ntile_j, "nsplit": nsplit, "T": tps, "T_last": ntj - (nsplit - 1) * tps,
             "cps": tps * TILE_J}
@@ -106,8 +112,10 @@ def _tf32_trunc(t):
 
 
 def _tf32_round(t):
-    """gp_common.cuh's tf32_hi: fp32(t) rounded to 10 mantissa bits, ties away."""
-    return ((t.float().view(torch.int32) + 0x1000) & -8192).view(torch.float32).double()
+    """gp_common.cuh's tf32_hi: fp32(t) rounded to 10 mantissa bits, ties away; a NaN keeps its bits."""
+    f = t.float()
+    r = ((f.view(torch.int32) + 0x1000) & -8192).view(torch.float32)
+    return torch.where(torch.isnan(f), f, r).double()
 
 
 def _n_lo(kind, x1, xs, lengthscale):
@@ -207,10 +215,12 @@ def exact(kind, x1, x2, lengthscale, outputscale, noise, V, same=False, row_begi
 
 # ---- the bound ----------------------------------------------------------------------------------------------------------------
 def bound(kind, x1, x2, lengthscale, outputscale, noise, V, path, nsplit, T_per_split, same=False, row_begin=0, row_count=None,
-          block=None):
+          block=None, diag=None):
     """Worst-case |engine - exact| [row_count, t] for every entry of Plan.kmv on the same fp32 inputs (module docstring).
     path "tc" (kmv_tc_kernel) or "simt" (kmv_simt_kernel); nsplit and T_per_split from geometry() (a kernel sum passes the
-    number of partial slots of all its terms as nsplit)."""
+    number of partial slots of all its terms as nsplit).  diag [rows] (cross form only): the column of x2 that is each row's own
+    point, masked to a = 0 by the kernel as on a square plan (-1: none), for columns that are a subset of the rows (one task
+    segment of a Hadamard plan, tests/multitask_oracle.py)."""
     zr, zc, grow = _packed(kind, x1, x2, lengthscale, same, row_begin, row_count)
     dev = zr.device
     n2, d = zc.size(0), zc.size(1)
@@ -227,10 +237,10 @@ def bound(kind, x1, x2, lengthscale, outputscale, noise, V, path, nsplit, T_per_
     block = block or _block_rows(n2, d, 256)
     for b in bo._blocks(zr.size(0), block):
         _, _, _, _, m, da = bo.pair_arg(zr[b], zc, nr, path, DP, KP)
-        if same:   # exact diagonal: a = 0 on both paths
+        if same or diag is not None:   # exact diagonal: a = 0 on both paths
             rows = torch.arange(b.stop - b.start, device=dev)
-            g = grow[b]
-            ok = g < n2
+            g = grow[b] if diag is None else diag[b].to(dev)
+            ok = (g >= 0) & (g < n2)
             m[rows[ok], g[ok]] = 0.0
             da[rows[ok], g[ok]] = 0.0
         k, _ = bo._kg(kind, m)
