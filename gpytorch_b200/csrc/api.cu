@@ -18,6 +18,24 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+uint32_t plan_settings(const gp_plan* p) {
+  return (p->lr_U ? PS_LOWRANK : 0u) | (p->tasks ? PS_TASKS : 0u) | (p->kron ? PS_KRON : 0u) | (p->deriv ? PS_DERIV : 0u) |
+         (p->backend_req == GP_BACKEND_PRODUCT ? PS_PRODUCT : 0u) | (p->add_M ? PS_ADDITIVE : 0u) | (p->sm_Q ? PS_SPECTRAL : 0u) |
+         (p->per_n ? PS_PERIODIC : 0u) | (p->kind == GP_RQ ? PS_RQ : 0u) | (p->kind == GP_POLY ? PS_POLY : 0u);
+}
+
+int refuse_settings(const gp_plan* p, CallId call) {
+  const CallRow& c = CALL_ROWS[call];
+  const uint32_t hit = plan_settings(p) & c.refuses;
+  if (hit == 0) return GP_OK;
+  const SettingName& s = SETTING_NAMES[__builtin_ctz(hit)];   // the first refused setting in check order
+  if (c.as)
+    set_error("%s: %s as a %s is not available (%s)", c.name, s.noun, c.as, s.setter);
+  else
+    set_error("%s is not available on %s (%s)", c.name, s.noun, s.setter);
+  return GP_E_STATE;
+}
+
 __global__ void concat_rhs_kernel(const float* __restrict__ probes, int tp, const float* __restrict__ y, int64_t n,
                                   float* __restrict__ rhs, float* __restrict__ pn_part) {
   // rhs[r][0..tp) = probes (normalised later), rhs[r][tp] = y
@@ -126,10 +144,7 @@ extern "C" int gp_plan_set_backend(gp_plan* p, int backend) {
   GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_STATE, "the SKI backend is selected by gp_plan_set_ski");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel sum runs the backends of its terms");
   GP_REQUIRE(p->kron == nullptr, GP_E_STATE, "a Kronecker plan runs the backend of its data plan");
-  GP_REFUSE_DERIV(p, "gp_plan_set_backend");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_backend");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_backend");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_backend");
+  GP_CHECK(refuse_settings(p, CALL_SET_BACKEND));
   p->backend_req = backend;
   if (p->data_set && p->hypers_set) return pack_inputs(p);
   return GP_OK;
@@ -198,13 +213,7 @@ extern "C" int gp_plan_set_hypers_rq(gp_plan* p, const float* lengthscale, int n
   GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "gp_plan_set_hypers_rq is not available on a SKI plan (gp_plan_set_ski)");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "gp_plan_set_hypers_rq is not available on a kernel-sum plan: give the kind to a term");
-  GP_REFUSE_TASKS(p, "gp_plan_set_hypers_rq");
-  GP_REFUSE_KRON(p, "gp_plan_set_hypers_rq");
-  GP_REFUSE_DERIV(p, "gp_plan_set_hypers_rq");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_hypers_rq");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_hypers_rq");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_hypers_rq");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_hypers_rq");
+  GP_CHECK(refuse_settings(p, CALL_SET_HYPERS_RQ));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_STATE, "gp_plan_set_hypers_rq is not available on a row-sharded plan (gp_plan_set_comm)");
   GP_CUDA(cudaSetDevice(p->device));
   // all or nothing: a failed pack restores the previous hyper-parameters (and packing), so the number of gradient values a caller
@@ -240,13 +249,7 @@ extern "C" int gp_plan_set_hypers_poly(gp_plan* p, int power, float offset, floa
   GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "gp_plan_set_hypers_poly is not available on a SKI plan (gp_plan_set_ski)");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "gp_plan_set_hypers_poly is not available on a kernel-sum plan: give the kind to a term");
-  GP_REFUSE_TASKS(p, "gp_plan_set_hypers_poly");
-  GP_REFUSE_KRON(p, "gp_plan_set_hypers_poly");
-  GP_REFUSE_DERIV(p, "gp_plan_set_hypers_poly");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_hypers_poly");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_hypers_poly");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_hypers_poly");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_hypers_poly");
+  GP_CHECK(refuse_settings(p, CALL_SET_HYPERS_POLY));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_STATE, "gp_plan_set_hypers_poly is not available on a row-sharded plan (gp_plan_set_comm)");
   GP_CUDA(cudaSetDevice(p->device));
   // all or nothing, as gp_plan_set_hypers_rq: a failed pack restores the previous hyper-parameters (and packing)
@@ -304,18 +307,7 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
   GP_REQUIRE(!(p->tasks && comm && comm->world > 1), GP_E_SHAPE, "task indices are not available on a row-sharded plan");
   GP_REQUIRE(!(p->kron && comm && comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   GP_REQUIRE(!(p->deriv && comm && comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
-  GP_REQUIRE(!(p->backend_req == GP_BACKEND_PRODUCT && comm && comm->world > 1), GP_E_STATE,
-             "gp_plan_set_comm with more than one rank is not available on a kernel-product plan (gp_plan_set_product)");
-  GP_REQUIRE(!(p->add_M && comm && comm->world > 1), GP_E_STATE,
-             "gp_plan_set_comm with more than one rank is not available on an additive plan (gp_plan_set_additive)");
-  GP_REQUIRE(!(p->sm_Q && comm && comm->world > 1), GP_E_STATE,
-             "gp_plan_set_comm with more than one rank is not available on a spectral mixture plan (gp_plan_set_spectral)");
-  GP_REQUIRE(!(p->per_n && comm && comm->world > 1), GP_E_STATE,
-             "gp_plan_set_comm with more than one rank is not available on a periodic plan (gp_plan_set_periodic)");
-  GP_REQUIRE(!(p->kind == GP_RQ && comm && comm->world > 1), GP_E_STATE,
-             "gp_plan_set_comm with more than one rank is not available on a rational quadratic plan (gp_plan_set_hypers_rq)");
-  GP_REQUIRE(!(p->kind == GP_POLY && comm && comm->world > 1), GP_E_STATE,
-             "gp_plan_set_comm with more than one rank is not available on a polynomial plan (gp_plan_set_hypers_poly)");
+  if (comm && comm->world > 1) GP_CHECK(refuse_settings(p, CALL_SET_COMM_SHARDED));
   p->comm = comm;
   return GP_OK;
 }

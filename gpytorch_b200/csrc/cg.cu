@@ -543,7 +543,7 @@ int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, fl
   GP_REQUIRE(max_tridiag_iter <= max_iter, GP_E_SHAPE,
              "Getting a tridiagonalization larger than the number of CG iterations run is not possible!");
   GP_REQUIRE(W == nullptr || (k >= 1 && k <= KMAX), GP_E_SHAPE, "preconditioner rank %d not in [1,%d]", k, KMAX);
-  if (W != nullptr) GP_REFUSE_LOWRANK(p, "gp_mbcg with a preconditioner");
+  if (W != nullptr) GP_CHECK(refuse_settings(p, CALL_MBCG_PRECOND));
   cudaStream_t st = p->stream;
   const int64_t n = p->row_count;       // local rows
   const int64_t N = p->n2;              // global size

@@ -258,8 +258,7 @@ static int deriv_check_data(const gp_plan* p, const gp_plan* q) {
     GP_REQUIRE(q->kind == GP_MATERN52, GP_E_SHAPE, "Matern-5/2 derivative plan: the data plan must be a Matern-5/2 plan (kind=%d)", q->kind);
   else
     GP_REQUIRE(q->kind == GP_RBF, GP_E_SHAPE, "derivative observations are available for the RBF kernel only (kind=%d)", q->kind);
-  GP_REQUIRE(q->tasks == nullptr, GP_E_STATE, "derivative plan: a data plan with task indices is not available");
-  GP_REQUIRE(q->lr_U == nullptr, GP_E_STATE, "derivative plan: a data plan with a low-rank correction is not available");
+  GP_CHECK(refuse_settings(q, CALL_DERIV_DATA_REFRESH));
   GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
              "derivative plan: a row-sharded data plan is not available");
   GP_REQUIRE(q->device == p->device && q->stream == p->stream, GP_E_STATE, "derivative plan: the data plan must live on the same device and stream");
@@ -484,8 +483,8 @@ static void deriv_release(gp_plan* p) {
   p->deriv = nullptr;
 }
 
-// gp_plan_set_deriv (RBF) and gp_plan_set_deriv_kind: `what` names the C call in the refusals
-static int deriv_set(gp_plan* p, gp_plan* data, int kind, const char* what) {
+// gp_plan_set_deriv (RBF) and gp_plan_set_deriv_kind: `call` and `data_role` name the C call in the refusals
+static int deriv_set(gp_plan* p, gp_plan* data, int kind, CallId call, CallId data_role) {
   GP_CUDA(cudaSetDevice(p->device));
   if (data == nullptr) {
     if (p->deriv) {
@@ -500,21 +499,8 @@ static int deriv_set(gp_plan* p, gp_plan* data, int kind, const char* what) {
   GP_REQUIRE(data != p, GP_E_STATE, "a derivative plan cannot be its own data plan");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a derivative plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a derivative plan");
-  GP_REFUSE_TASKS(p, what);
-  GP_REFUSE_LOWRANK(p, what);
-  GP_REFUSE_KRON(p, what);
-  GP_REFUSE_PRODUCT(p, what);
-  if (data) GP_REQUIRE(data->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "%s (as the data plan) is not available on a kernel-product plan (gp_plan_set_product)", what);
-  GP_REFUSE_ADDITIVE(p, what);
-  GP_REFUSE_SPECTRAL(p, what);
-  GP_REFUSE_PERIODIC(p, what);
-  if (data) GP_REQUIRE(data->add_M == 0, GP_E_STATE, "%s (as the data plan) is not available on an additive plan (gp_plan_set_additive)", what);
-  if (data) GP_REQUIRE(data->sm_Q == 0, GP_E_STATE, "%s (as the data plan) is not available on a spectral mixture plan (gp_plan_set_spectral)", what);
-  if (data) GP_REQUIRE(data->per_n == 0, GP_E_STATE, "%s (as the data plan) is not available on a periodic plan (gp_plan_set_periodic)", what);
-  GP_REFUSE_RQ(p, what);
-  if (data) GP_REQUIRE(data->kind != GP_RQ, GP_E_STATE, "%s (as the data plan) is not available on a rational quadratic plan (gp_plan_set_hypers_rq)", what);
-  GP_REFUSE_POLY(p, what);
-  if (data) GP_REQUIRE(data->kind != GP_POLY, GP_E_STATE, "%s (as the data plan) is not available on a polynomial plan (gp_plan_set_hypers_poly)", what);
+  GP_CHECK(refuse_settings(p, call));
+  GP_CHECK(refuse_settings(data, data_role));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   gp_deriv_state* ds = p->deriv ? p->deriv : new gp_deriv_state();
   gp_plan* old = ds->data;
@@ -540,12 +526,12 @@ using namespace gp;
 
 extern "C" int gp_plan_set_deriv(gp_plan* p, gp_plan* data) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
-  return deriv_set(p, data, GP_RBF, "gp_plan_set_deriv");
+  return deriv_set(p, data, GP_RBF, CALL_SET_DERIV, CALL_DERIV_DATA);
 }
 
 extern "C" int gp_plan_set_deriv_kind(gp_plan* p, gp_plan* data, int kind) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(kind == GP_RBF || kind == GP_MATERN52, GP_E_SHAPE,
              "derivative observations are available for the RBF and Matern-5/2 kernels (kind=%d)", kind);
-  return deriv_set(p, data, kind, "gp_plan_set_deriv_kind");
+  return deriv_set(p, data, kind, CALL_SET_DERIV_KIND, CALL_DERIV_KIND_DATA);
 }

@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "../../include/gp_bbmm.h"
+#include "plan_settings.h"
 
 #ifndef __CUDA_ARCH_FEAT_SM90_ALL
 #if defined(__CUDA_ARCH__)
@@ -306,6 +307,10 @@ struct KronColsScope {
 
 namespace gp {
 
+// ---- plan settings (plan_settings.h), api.cu ---------------------------------------------
+uint32_t plan_settings(const gp_plan* p);              // the PlanSetting bits p carries
+int refuse_settings(const gp_plan* p, CallId call);    // GP_E_STATE naming the first setting of p that `call` refuses, else GP_OK
+
 // ---- launches implemented across the .cu files -------------------------------------------
 int pack_inputs(gp_plan* p);                                            // pack.cu
 int to_v16(gp_plan* p, const float* V, int64_t ldv, int t, int64_t n, float* V16);
@@ -330,8 +335,6 @@ int product_kmv_launch(gp_plan* p, const float* V16, const int* done_flag);   //
 int product_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);   // the factors' rows multiplied in order
 int product_kdiag_cross(gp_plan* p, float* OUT);                        // diagonal of a cross product: the factors' diagonals multiplied
 int product_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
-#define GP_REFUSE_PRODUCT(p, what) \
-  GP_REQUIRE((p)->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "%s is not available on a kernel-product plan (gp_plan_set_product)", what)
 int lowrank_partials(gp_plan* p, const float* V16, const int* done_flag);   // lowrank.cu: -U U^T V into the last slot (no-op without U)
 int lowrank_kdiag(gp_plan* p, float* OUT);                              // OUT[i] -= sum_j U_ij^2
 int lowrank_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);   // OUT[r] -= U[idx_r] U^T
@@ -356,8 +359,6 @@ int tasks_kmv_partials(gp_plan* p, const float* V16, int kind, const int* done_f
 int tasks_kdiag_scale(gp_plan* p, float* OUT);                               // OUT[i] *= B[t1_i, t2_i]
 int tasks_krows_scale(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
 int tasks_bilinear(gp_plan* p, const float* L16, const float* R16, bool ard, std::vector<double>& total);
-#define GP_REFUSE_TASKS(p, what) \
-  GP_REQUIRE((p)->tasks == nullptr, GP_E_STATE, "%s is not available on a plan with task indices (gp_plan_set_tasks)", what)
 int kron_pack(gp_plan* p);                                                   // kron.cu
 int kron_kmv_partials(gp_plan* p, const float* V16, const int* done_flag);   // (s K) (x) B V into partial slot 0 (unscaled)
 int kron_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
@@ -366,8 +367,6 @@ int kron_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, 
 int kron_refresh(gp_plan* p);                                                // re-check the data plan, take its scale / kind / flag
 int kron_set_task_covar(gp_plan* p, const float* B, int T);                  // gp_plan_set_task_covar on a Kronecker plan
 int kron_task_covar_grad_checked(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB);
-#define GP_REFUSE_KRON(p, what) \
-  GP_REQUIRE((p)->kron == nullptr, GP_E_STATE, "%s is not available on a Kronecker multitask plan (gp_plan_set_kron)", what)
 int deriv_pack(gp_plan* p);                                                  // deriv.cu
 int deriv_kmv_partials(gp_plan* p, const float* V16, const int* done_flag);  // K_grad V into partial slot 0 (unscaled)
 int deriv_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
@@ -375,8 +374,6 @@ int deriv_kdiag(gp_plan* p, float* OUT);
 int deriv_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
 int deriv_refresh(gp_plan* p);                                               // re-check the data plan, take its scale / lengthscales / flag
 double deriv_trace(const gp_plan* p);                                        // s N (1 + c sum_c 1 / l_c^2) in fp64, c = 1 or 5/3
-#define GP_REFUSE_DERIV(p, what) \
-  GP_REQUIRE((p)->deriv == nullptr, GP_E_STATE, "%s is not available on a derivative-observation plan (gp_plan_set_deriv)", what)
 int mbcg_run(gp_plan* p, const float* RHS, int64_t ldr, int t, int n_tridiag, float tol, int max_iter,   // cg.cu
              int max_tridiag_iter, const float* W, int k, float* SOLVES, int64_t lds, float* TMAT, int* iters_out,
              int* tridiag_size, float* resid_out);
@@ -390,8 +387,6 @@ inline int nslots(const gp_plan* p) { return p->nparts + (p->lr_U ? 1 : 0); }
 inline const float* part_scale_ptr(gp_plan* p) {
   return (p->backend == GP_BACKEND_SUM || p->lr_U) ? p->part_scale.as<float>() : nullptr;
 }
-#define GP_REFUSE_LOWRANK(p, what) \
-  GP_REQUIRE((p)->lr_U == nullptr, GP_E_STATE, "%s is not available on a plan with a low-rank correction (gp_plan_set_lowrank)", what)
 // the scale the finish kernels apply to the backend's slots: the outputscale, or 1 on an additive plan (whose components carry
 // their own scales)
 inline float kernel_scale(const gp_plan* p) { return p->add_M ? 1.f : p->outputscale; }
@@ -401,25 +396,15 @@ int additive_kmv_launch(gp_plan* p, const float* V16, const int* done_flag);
 int additive_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
 int additive_kdiag(gp_plan* p, float* OUT);
 int additive_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
-#define GP_REFUSE_ADDITIVE(p, what) \
-  GP_REQUIRE((p)->add_M == 0, GP_E_STATE, "%s is not available on an additive plan (gp_plan_set_additive)", what)
 // spectral.cu
 int spectral_pack(gp_plan* p);                                          // packs [x | reduced phases] into Z1 / Z2, forms sm_diag
 int spectral_kmv_launch(gp_plan* p, const float* V16, const int* done_flag);
 int spectral_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo);
 int spectral_kdiag(gp_plan* p, float* OUT);
 int spectral_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
-#define GP_REFUSE_SPECTRAL(p, what) \
-  GP_REQUIRE((p)->sm_Q == 0, GP_E_STATE, "%s is not available on a spectral mixture plan (gp_plan_set_spectral)", what)
 // periodic.cu
 int periodic_pack(gp_plan* p);                                          // embeds the inputs into Z1 / Z2 (and the tensor-core tiles)
 int periodic_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
-#define GP_REFUSE_PERIODIC(p, what) \
-  GP_REQUIRE((p)->per_n == 0, GP_E_STATE, "%s is not available on a periodic plan (gp_plan_set_periodic)", what)
-#define GP_REFUSE_RQ(p, what) \
-  GP_REQUIRE((p)->kind != GP_RQ, GP_E_STATE, "%s is not available on a rational quadratic plan (gp_plan_set_hypers_rq)", what)
-#define GP_REFUSE_POLY(p, what) \
-  GP_REQUIRE((p)->kind != GP_POLY, GP_E_STATE, "%s is not available on a polynomial plan (gp_plan_set_hypers_poly)", what)
 // columns of the packed rows the plain kernels see: the d inputs, or the 2d embedding columns of a periodic plan
 inline int packed_dims(const gp_plan* p) { return p->per_n ? 2 * p->d : p->d; }
 inline bool plan_is_tc(const gp_plan* p) {

@@ -623,7 +623,7 @@ static int kdiag_base(gp_plan* p, float* OUT) {
 extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float* Rt, int64_t ldr, int s,
                                 double* grad_ls, double* grad_os) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REFUSE_LOWRANK(p, "gp_bilinear_grad");
+  GP_CHECK(refuse_settings(p, CALL_BILINEAR_GRAD));
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "gradients of a kernel sum: call gp_bilinear_grad on every term");
   GP_REQUIRE(s >= 1, GP_E_SHAPE, "s must be >= 1");
   GP_REQUIRE(Lf && Rt, GP_E_SHAPE, "gp_bilinear_grad: null factor");

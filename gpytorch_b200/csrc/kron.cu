@@ -129,8 +129,7 @@ static int kron_check_data(const gp_plan* p, const gp_plan* q) {
   GP_REQUIRE(q->data_set && q->hypers_set, GP_E_STATE, "Kronecker plan: the data plan needs set_data + set_hypers");
   GP_REQUIRE(q->backend == GP_BACKEND_TCGEN05 || q->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
              "Kronecker plan: the data plan must be a plain kernel plan (not SKI, not a kernel sum, not Kronecker)");
-  GP_REQUIRE(q->tasks == nullptr, GP_E_STATE, "Kronecker plan: a data plan with task indices is not available");
-  GP_REQUIRE(q->lr_U == nullptr, GP_E_STATE, "Kronecker plan: a data plan with a low-rank correction is not available");
+  GP_CHECK(refuse_settings(q, CALL_KRON_DATA_REFRESH));
   GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
              "Kronecker plan: a row-sharded data plan is not available");
   GP_REQUIRE(q->device == p->device && q->stream == p->stream, GP_E_STATE, "Kronecker plan: the data plan must live on the same device and stream");
@@ -163,8 +162,6 @@ int kron_refresh(gp_plan* p) {
   gp_kron_state* ks = p->kron;
   const gp_plan* q = ks->data;
   GP_CHECK(kron_check_data(p, q));
-  GP_REFUSE_RQ(q, "a Kronecker operator (as the data plan)");
-  GP_REFUSE_POLY(q, "a Kronecker operator (as the data plan)");
   GP_REQUIRE(p->n1 == q->n1 * ks->T && p->n2 == q->n2 * ks->T && p->same == q->same, GP_E_STATE,
              "Kronecker plan: the data plan changed its size; call gp_plan_set_kron again");
   p->kind = q->kind;
@@ -363,21 +360,8 @@ extern "C" int gp_plan_set_kron(gp_plan* p, gp_plan* data, int T) {
   GP_REQUIRE(data != p, GP_E_STATE, "a Kronecker plan cannot be its own data plan");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a Kronecker plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a Kronecker plan");
-  GP_REFUSE_TASKS(p, "gp_plan_set_kron");
-  GP_REFUSE_LOWRANK(p, "gp_plan_set_kron");
-  GP_REFUSE_DERIV(p, "gp_plan_set_kron");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_kron");
-  if (data) GP_REFUSE_PRODUCT(data, "gp_plan_set_kron (as the data plan)");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_kron");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_kron");
-  if (data) GP_REFUSE_ADDITIVE(data, "gp_plan_set_kron (as the data plan)");
-  if (data) GP_REFUSE_SPECTRAL(data, "gp_plan_set_kron (as the data plan)");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_kron");
-  if (data) GP_REFUSE_PERIODIC(data, "gp_plan_set_kron (as the data plan)");
-  GP_REFUSE_RQ(p, "gp_plan_set_kron");
-  if (data) GP_REFUSE_RQ(data, "gp_plan_set_kron (as the data plan)");
-  GP_REFUSE_POLY(p, "gp_plan_set_kron");
-  if (data) GP_REFUSE_POLY(data, "gp_plan_set_kron (as the data plan)");
+  GP_CHECK(refuse_settings(p, CALL_SET_KRON));
+  GP_CHECK(refuse_settings(data, CALL_KRON_DATA));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   gp_kron_state* ks = p->kron ? p->kron : new gp_kron_state();
   const bool keep_b = p->kron && ks->T == T && ks->b_set;

@@ -179,10 +179,7 @@ extern "C" int gp_plan_set_lowrank(gp_plan* p, const float* U, int64_t ldu, int 
     return GP_OK;
   }
   GP_REQUIRE(p->data_set, GP_E_STATE, "low-rank correction: call gp_plan_set_data first");
-  GP_REFUSE_TASKS(p, "gp_plan_set_lowrank");
-  GP_REFUSE_KRON(p, "gp_plan_set_lowrank");
-  GP_REFUSE_DERIV(p, "gp_plan_set_lowrank");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_lowrank");
+  GP_CHECK(refuse_settings(p, CALL_SET_LOWRANK));
   GP_REQUIRE(r >= 1 && r <= LR_RMAX, GP_E_SHAPE, "low-rank correction of rank %d: 1 <= r <= %d", r, LR_RMAX);
   GP_REQUIRE(ldu >= r, GP_E_SHAPE, "low-rank correction: ldu=%lld < r=%d", (long long)ldu, r);
   GP_REQUIRE(p->same, GP_E_SHAPE, "a low-rank correction needs a square operator (X2 == X1)");

@@ -596,7 +596,7 @@ extern "C" int gp_ciq_sqrt_matmul_precond(gp_plan* plan, const float* B, int64_t
                                           const double* w, int Q, float tol, int max_iter, float* OUT, int64_t ldo, int* iters_out,
                                           float* resid_out) {
   GP_REQUIRE(plan != nullptr, GP_E_STATE, "null plan");
-  GP_REFUSE_LOWRANK(plan, "gp_ciq_sqrt_matmul_precond");
+  GP_CHECK(gp::refuse_settings(plan, gp::CALL_CIQ_SQRT_MATMUL_PRECOND));
   GP_REQUIRE(U != nullptr, GP_E_SHAPE, "preconditioned CIQ without a factor U (k=%d)", k);
   return gp::ciq_run(plan, B, ldb, t, U, k, tau, w, Q, tol, max_iter, OUT, ldo, iters_out, resid_out);
 }

@@ -835,7 +835,7 @@ using namespace gp;
 
 extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float* Lt, int64_t* piv, int* rank_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REFUSE_LOWRANK(p, "gp_pivoted_cholesky");
+  GP_CHECK(refuse_settings(p, CALL_PIVOTED_CHOLESKY));
   GP_REQUIRE(p->same, GP_E_SHAPE, "pivoted Cholesky needs a square operator");
   GP_CHECK(slot_scales_prepare(p));
   const bool prod = p->backend == GP_BACKEND_PRODUCT;
@@ -1033,7 +1033,7 @@ static GramSplit gram_split(const gp_plan* p, int k, int64_t n) {
 
 extern "C" int gp_precond_build(gp_plan* p, const float* Lt, int k, float* W, double* logdet_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REFUSE_LOWRANK(p, "gp_precond_build");
+  GP_CHECK(refuse_settings(p, CALL_PRECOND_BUILD));
   GP_REQUIRE(k >= 1 && k <= 128, GP_E_SHAPE, "preconditioner rank %d not in [1,128]", k);
   const float* dvec = p->noise_diag;
   GP_REQUIRE(dvec != nullptr || p->noise > 0.f, GP_E_SHAPE, "preconditioner needs noise > 0");
@@ -1093,7 +1093,7 @@ static int dot_diag_sum(gp_plan* p, double* out) {
 
 extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U, double* trace_resid_out) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REFUSE_LOWRANK(p, "gp_ciq_precond_build");
+  GP_CHECK(refuse_settings(p, CALL_CIQ_PRECOND_BUILD));
   GP_REQUIRE(k >= 1 && k <= 128, GP_E_SHAPE, "preconditioner rank %d not in [1,128]", k);
   GP_REQUIRE(Lt != nullptr && U != nullptr, GP_E_SHAPE, "Lt / U missing");
   GP_REQUIRE(p->same, GP_E_SHAPE, "the CIQ preconditioner needs a square operator");
@@ -1186,7 +1186,7 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
 
 extern "C" int gp_precond_probes(gp_plan* p, const float* Lt, int k, const float* eps1, const float* eps2, int tp, float* Z) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REFUSE_LOWRANK(p, "gp_precond_probes");
+  GP_CHECK(refuse_settings(p, CALL_PRECOND_PROBES));
   GP_REQUIRE(k >= 1 && tp >= 1 && (size_t)k * tp * 4 <= 40 * 1024, GP_E_SHAPE, "bad probe shape k=%d tp=%d", k, tp);
   int64_t tot = p->row_count * tp;
   probes_kernel<<<(unsigned)cdiv(tot, 256), 256, sizeof(float) * k * tp, p->stream>>>(Lt, k, p->n2, p->row_begin, p->row_count,

@@ -292,10 +292,7 @@ int product_pack(gp_plan* p) {
     GP_REQUIRE(q && q != p && q->data_set && q->hypers_set, GP_E_STATE, "kernel product: every factor needs set_data + set_hypers");
     GP_REQUIRE(q->backend == GP_BACKEND_TCGEN05 || q->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
                "kernel product: a factor must be a plain kernel plan (not SKI, not a sum, not a product, not multitask, not derivative)");
-    GP_REQUIRE(q->tasks == nullptr, GP_E_STATE, "kernel product: a factor with task indices is not available");
-    GP_REQUIRE(q->kind != GP_RQ, GP_E_STATE, "kernel product: a rational quadratic factor is not available (gp_plan_set_hypers_rq)");
-    GP_REQUIRE(q->kind != GP_POLY, GP_E_STATE, "kernel product: a polynomial factor is not available (gp_plan_set_hypers_poly)");
-    GP_REQUIRE(q->lr_U == nullptr, GP_E_STATE, "kernel product: a factor with a low-rank correction is not available");
+    GP_CHECK(refuse_settings(q, CALL_PRODUCT_FACTOR_REFRESH));
     GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
                "kernel product: a row-sharded factor is not available");
     GP_REQUIRE(q->n1 == p->n1 && q->n2 == p->n2 && q->same == p->same, GP_E_SHAPE,
@@ -442,15 +439,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   GP_REQUIRE(p && p->data_set, GP_E_STATE, "kernel product: call gp_plan_set_data on the product first");
   GP_REQUIRE(p->ski == nullptr, GP_E_STATE, "a SKI plan cannot become a kernel product");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a kernel product");
-  GP_REFUSE_TASKS(p, "gp_plan_set_product");
-  GP_REFUSE_KRON(p, "gp_plan_set_product");
-  GP_REFUSE_DERIV(p, "gp_plan_set_product");
-  GP_REFUSE_LOWRANK(p, "gp_plan_set_product");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_product");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_product");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_product");
-  GP_REFUSE_RQ(p, "gp_plan_set_product");
-  GP_REFUSE_POLY(p, "gp_plan_set_product");
+  GP_CHECK(refuse_settings(p, CALL_SET_PRODUCT));
   GP_CUDA(cudaSetDevice(p->device));
   if (factors == nullptr || n_factors == 0) {   // back to a plain plan
     if (p->backend_req != GP_BACKEND_PRODUCT) return GP_OK;
@@ -463,16 +452,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   GP_REQUIRE(n_factors >= 2 && n_factors <= 4, GP_E_SHAPE, "a kernel product takes 2 to 4 factors (got %d)", n_factors);
   for (int f = 0; f < n_factors; ++f) {
     GP_REQUIRE(factors[f] != nullptr && factors[f] != p, GP_E_STATE, "kernel product: factor %d is null or the product itself", f);
-    GP_REQUIRE(factors[f]->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE, "kernel product: a factor that is itself a kernel product is not available");
-    GP_REQUIRE(factors[f]->add_M == 0, GP_E_STATE, "gp_plan_set_product: an additive plan as a factor is not available (gp_plan_set_additive)");
-    GP_REQUIRE(factors[f]->sm_Q == 0, GP_E_STATE, "gp_plan_set_product: a spectral mixture plan as a factor is not available (gp_plan_set_spectral)");
-    GP_REQUIRE(factors[f]->per_n == 0, GP_E_STATE, "gp_plan_set_product: a periodic plan as a factor is not available (gp_plan_set_periodic)");
-  for (int f = 0; f < n_factors; ++f)
-    GP_REQUIRE(factors[f] == nullptr || factors[f]->kind != GP_RQ, GP_E_STATE,
-               "gp_plan_set_product: a rational quadratic plan as a factor is not available (gp_plan_set_hypers_rq)");
-  for (int f = 0; f < n_factors; ++f)
-    GP_REQUIRE(factors[f] == nullptr || factors[f]->kind != GP_POLY, GP_E_STATE,
-               "gp_plan_set_product: a polynomial plan as a factor is not available (gp_plan_set_hypers_poly)");
+    GP_CHECK(refuse_settings(factors[f], CALL_PRODUCT_FACTOR));
   }
   p->factors.assign(factors, factors + n_factors);
   p->backend_req = GP_BACKEND_PRODUCT;

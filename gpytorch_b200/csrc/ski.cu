@@ -1347,15 +1347,7 @@ using namespace gp;
 // (utils/grid.py:142-180 create_grid: linspace(lo - step, hi + step, size) per dimension)
 extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* grid_lo, const float* grid_step, int d) {
   GP_REQUIRE(p != nullptr && p->data_set, GP_E_STATE, "set_data must precede set_ski");
-  GP_REFUSE_TASKS(p, "gp_plan_set_ski");
-  GP_REFUSE_KRON(p, "gp_plan_set_ski");
-  GP_REFUSE_DERIV(p, "gp_plan_set_ski");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_ski");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_ski");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_ski");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_ski");
-  GP_REFUSE_RQ(p, "gp_plan_set_ski");
-  GP_REFUSE_POLY(p, "gp_plan_set_ski");
+  GP_CHECK(refuse_settings(p, CALL_SET_SKI));
   GP_REQUIRE(d == p->d && d >= 1 && d <= SKI_MAXD, GP_E_SHAPE, "SKI: grid dimension %d does not match the data (d=%d, max %d)", d, p->d, SKI_MAXD);
   int64_t M = 1;
   bool large = false;
@@ -1384,11 +1376,7 @@ extern "C" int gp_ski_grid_matmul(gp_plan* p, const float* V, int64_t ldv, int t
 
 extern "C" int gp_ski_input_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, float* DX, int64_t lddx) {
   GP_CHECK(ski_predict_check(p, t, ldl, ldr, "gp_ski_input_grad"));
-  GP_REFUSE_LOWRANK(p, "gp_ski_input_grad");
-  GP_REFUSE_TASKS(p, "gp_ski_input_grad");
-  GP_REFUSE_KRON(p, "gp_ski_input_grad");
-  GP_REFUSE_DERIV(p, "gp_ski_input_grad");
-  GP_REFUSE_PRODUCT(p, "gp_ski_input_grad");
+  GP_CHECK(refuse_settings(p, CALL_SKI_INPUT_GRAD));
   GP_REQUIRE(L && R && DX && lddx >= p->d, GP_E_SHAPE, "gp_ski_input_grad: bad output (leading dimension %lld, d=%d)", (long long)lddx, p->d);
   return ski_with_d(p->d, [&](auto D) { return ski_input_grad_d<D>(p, L, ldl, R, ldr, t, DX, lddx); });
 }

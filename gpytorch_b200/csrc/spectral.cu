@@ -446,14 +446,7 @@ extern "C" int gp_plan_set_spectral(gp_plan* p, int Q, const float* weights, con
   GP_REQUIRE(p->data_set, GP_E_STATE, "spectral plan: call gp_plan_set_data first");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a spectral plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a spectral plan");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_spectral");
-  GP_REFUSE_TASKS(p, "gp_plan_set_spectral");
-  GP_REFUSE_KRON(p, "gp_plan_set_spectral");
-  GP_REFUSE_DERIV(p, "gp_plan_set_spectral");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_spectral");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_spectral");
-  GP_REFUSE_RQ(p, "gp_plan_set_spectral");
-  GP_REFUSE_POLY(p, "gp_plan_set_spectral");
+  GP_CHECK(refuse_settings(p, CALL_SET_SPECTRAL));
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,
              "a spectral plan is not available on a row-sharded plan");
   GP_REQUIRE(Q >= 1 && Q <= SM_QMAX && d >= 1 && d <= SM_DMAX && Q * d <= SM_QDMAX, GP_E_SHAPE,

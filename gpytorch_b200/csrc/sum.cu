@@ -24,7 +24,7 @@ int sum_pack(gp_plan* p) {
     GP_REQUIRE(t && t != p && t->data_set && t->hypers_set, GP_E_STATE, "kernel sum: every term needs set_data + set_hypers");
     GP_REQUIRE(t->backend == GP_BACKEND_TCGEN05 || t->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
                "kernel sum: a term must be a plain kernel plan (not SKI, not a sum)");
-    GP_REQUIRE(t->tasks == nullptr, GP_E_STATE, "kernel sum: a term with task indices is not available");
+    GP_CHECK(refuse_settings(t, CALL_SUM_TERM_REFRESH));
     GP_REQUIRE(t->n1 == p->n1 && t->n2 == p->n2 && t->same == p->same && t->row_begin == p->row_begin && t->row_count == p->row_count,
                GP_E_SHAPE, "kernel sum: term shape %lld x %lld (rows [%lld,+%lld)) differs from the sum's %lld x %lld (rows [%lld,+%lld))",
                (long long)t->n1, (long long)t->n2, (long long)t->row_begin, (long long)t->row_count, (long long)p->n1, (long long)p->n2,
@@ -119,22 +119,9 @@ extern "C" int gp_plan_set_sum(gp_plan* p, gp_plan* const* terms, int n_terms) {
   GP_REQUIRE(p && p->data_set, GP_E_STATE, "kernel sum: call gp_plan_set_data on the sum first");
   GP_REQUIRE(terms != nullptr && n_terms >= 1 && n_terms <= 4, GP_E_SHAPE, "a kernel sum takes 1 to 4 terms (got %d)", n_terms);
   GP_REQUIRE(p->ski == nullptr, GP_E_STATE, "a SKI plan cannot become a kernel sum");
-  GP_REFUSE_TASKS(p, "gp_plan_set_sum");
-  GP_REFUSE_KRON(p, "gp_plan_set_sum");
-  GP_REFUSE_DERIV(p, "gp_plan_set_sum");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_sum");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_sum");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_sum");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_sum");
+  GP_CHECK(refuse_settings(p, CALL_SET_SUM));
   for (int t = 0; t < n_terms; ++t)
-    GP_REQUIRE(terms[t] == nullptr || terms[t]->backend_req != GP_BACKEND_PRODUCT, GP_E_STATE,
-               "gp_plan_set_sum: a kernel product as a term is not available (gp_plan_set_product)");
-  for (int t = 0; t < n_terms; ++t)
-    GP_REQUIRE(terms[t] == nullptr || terms[t]->add_M == 0, GP_E_STATE,
-               "gp_plan_set_sum: an additive plan as a term is not available (gp_plan_set_additive)");
-  for (int t = 0; t < n_terms; ++t)
-    GP_REQUIRE(terms[t] == nullptr || terms[t]->sm_Q == 0, GP_E_STATE,
-               "gp_plan_set_sum: a spectral mixture plan as a term is not available (gp_plan_set_spectral)");
+    if (terms[t]) GP_CHECK(refuse_settings(terms[t], CALL_SUM_TERM));
   GP_CUDA(cudaSetDevice(p->device));
   p->terms.assign(terms, terms + n_terms);
   p->backend_req = GP_BACKEND_SUM;

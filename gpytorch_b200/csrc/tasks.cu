@@ -312,19 +312,12 @@ extern "C" int gp_plan_set_tasks(gp_plan* p, const int32_t* task1, const int32_t
     }
     return GP_OK;
   }
-  GP_REFUSE_KRON(p, "gp_plan_set_tasks");
-  GP_REFUSE_DERIV(p, "gp_plan_set_tasks");
-  GP_REFUSE_PRODUCT(p, "gp_plan_set_tasks");
-  GP_REFUSE_ADDITIVE(p, "gp_plan_set_tasks");
-  GP_REFUSE_SPECTRAL(p, "gp_plan_set_tasks");
-  GP_REFUSE_PERIODIC(p, "gp_plan_set_tasks");
-  GP_REFUSE_RQ(p, "gp_plan_set_tasks");
-  GP_REFUSE_POLY(p, "gp_plan_set_tasks");
+  GP_CHECK(refuse_settings(p, CALL_SET_TASKS));
   GP_REQUIRE(p->data_set, GP_E_STATE, "gp_plan_set_tasks: call gp_plan_set_data first");
   GP_REQUIRE(T >= 1 && T <= 32, GP_E_SHAPE, "number of tasks T=%d not in [1, 32]", T);
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "task indices are not available on a SKI plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "task indices are not available on a kernel-sum plan");
-  GP_REQUIRE(p->lr_U == nullptr, GP_E_STATE, "task indices are not available on a plan with a low-rank correction");
+  GP_CHECK(refuse_settings(p, CALL_SET_TASKS_LOWRANK));
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,
              "task indices are not available on a row-sharded plan");
   GP_REQUIRE(p->same ? (task2 == nullptr || task2 == task1) : task2 != nullptr, GP_E_SHAPE,

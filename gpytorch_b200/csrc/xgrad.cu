@@ -219,16 +219,10 @@ static int xgrad_role(gp_plan* p, const float* Zo, int64_t no, const float* Zt, 
   return GP_OK;
 }
 
-static int xgrad_check(gp_plan* p, const char* what, float* DX1, int64_t ld1, float* DX2, int64_t ld2) {
+static int xgrad_check(gp_plan* p, CallId call, float* DX1, int64_t ld1, float* DX2, int64_t ld2) {
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
-  GP_REFUSE_LOWRANK(p, what);
-  GP_REFUSE_TASKS(p, what);
-  GP_REFUSE_KRON(p, what);
-  GP_REFUSE_DERIV(p, what);
-  GP_REFUSE_PRODUCT(p, what);
-  GP_REFUSE_ADDITIVE(p, what);
-  GP_REFUSE_SPECTRAL(p, what);
-  GP_REFUSE_PERIODIC(p, what);
+  GP_CHECK(refuse_settings(p, call));
+  const char* what = CALL_ROWS[call].name;
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "%s of a kernel sum: call it on every term", what);
   GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "%s is not available on a SKI plan", what);
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,
@@ -245,7 +239,7 @@ using namespace gp;
 
 extern "C" int gp_kmv_input_grad(gp_plan* p, const float* G, int64_t ldg, const float* V, int64_t ldv, int t, float* DX1,
                                  int64_t ld1, float* DX2, int64_t ld2) {
-  GP_CHECK(xgrad_check(p, "gp_kmv_input_grad", DX1, ld1, DX2, ld2));
+  GP_CHECK(xgrad_check(p, CALL_KMV_INPUT_GRAD, DX1, ld1, DX2, ld2));
   GP_REQUIRE(t >= 1 && ldg >= t && ldv >= t && G && V, GP_E_SHAPE, "gp_kmv_input_grad: bad shape t=%d ldg=%lld ldv=%lld", t,
              (long long)ldg, (long long)ldv);
   GP_CUDA(cudaSetDevice(p->device));
@@ -261,7 +255,7 @@ extern "C" int gp_kmv_input_grad(gp_plan* p, const float* G, int64_t ldg, const 
 }
 
 extern "C" int gp_kdense_input_grad(gp_plan* p, const float* W, int64_t ldw, float* DX1, int64_t ld1, float* DX2, int64_t ld2) {
-  GP_CHECK(xgrad_check(p, "gp_kdense_input_grad", DX1, ld1, DX2, ld2));
+  GP_CHECK(xgrad_check(p, CALL_KDENSE_INPUT_GRAD, DX1, ld1, DX2, ld2));
   GP_REQUIRE(W && ldw >= p->n2, GP_E_SHAPE, "gp_kdense_input_grad: bad W (ldw=%lld, n2=%lld)", (long long)ldw, (long long)p->n2);
   GP_CUDA(cudaSetDevice(p->device));
   const float* Z2 = p->Z2.as<float>();

@@ -40,6 +40,53 @@ enum {
   GP_W_EIG_NOT_CONVERGED = 8 /* tridiagonal QL iteration hit its sweep limit: the SLQ log-det is unreliable (NumericalWarning) */
 };
 
+/* Plan settings.  Ten settings change what a plan's operator is: a low-rank correction (lr, gp_plan_set_lowrank), task indices
+ * (tsk, gp_plan_set_tasks), Kronecker (krn, gp_plan_set_kron), derivative observations (drv, gp_plan_set_deriv), a kernel product
+ * (prd, gp_plan_set_product), additive (add, gp_plan_set_additive), spectral mixture (spm, gp_plan_set_spectral), periodic (per,
+ * gp_plan_set_periodic), rational quadratic (rq, gp_plan_set_hypers_rq) and polynomial (ply, gp_plan_set_hypers_poly).  A call on a
+ * plan carrying a setting it does not support (x below) returns GP_E_STATE with "<call> is not available on <plan> (<setter>)", naming
+ * the call, the setting and its setter; a plan another plan takes in is refused the same way, as a data plan, or with "<call>: <plan>
+ * as a factor|term is not available (<setter>)".  The low-rank correction, the one setting that coexists with others, is named first.
+ * A re-check runs before every call on the taking plan once the plan it took in was re-packed.  SKI, kernel-sum and row-sharded
+ * plans are checked separately, as each call describes.
+ *                                                 lr  tsk krn drv prd add spm per rq  ply
+ *   gp_plan_set_backend                           .   .   .   x   x   x   x   .   .   .
+ *   gp_plan_set_hypers_rq                         .   x   x   x   x   x   x   x   .   .
+ *   gp_plan_set_hypers_poly                       .   x   x   x   x   x   x   x   .   .
+ *   gp_plan_set_comm with more than one rank      .   .   .   .   x   x   x   x   x   x
+ *   gp_plan_set_ski                               .   x   x   x   x   x   x   x   x   x
+ *   gp_ski_input_grad                             x   x   x   x   x   .   .   .   .   .
+ *   gp_plan_set_tasks                             .   .   x   x   x   x   x   x   x   x
+ *   gp_plan_set_tasks (after SKI / sum checks)    x   .   .   .   .   .   .   .   .   .
+ *   gp_plan_set_additive                          .   x   x   x   x   .   x   x   x   x
+ *   gp_plan_set_spectral                          .   x   x   x   x   x   .   x   x   x
+ *   gp_plan_set_periodic                          .   x   x   x   x   x   x   .   x   x
+ *   gp_plan_set_sum                               .   x   x   x   x   x   x   x   .   .
+ *   gp_plan_set_product                           x   x   x   x   .   x   x   x   x   x
+ *   gp_plan_set_kron                              x   x   .   x   x   x   x   x   x   x
+ *   gp_plan_set_deriv                             x   x   x   .   x   x   x   x   x   x
+ *   gp_plan_set_deriv_kind                        x   x   x   .   x   x   x   x   x   x
+ *   gp_plan_set_lowrank                           .   x   x   x   x   .   .   .   .   .
+ *   gp_kmv_input_grad                             x   x   x   x   x   x   x   x   .   .
+ *   gp_kdense_input_grad                          x   x   x   x   x   x   x   x   .   .
+ *   gp_pivoted_cholesky                           x   .   .   .   .   .   .   .   .   .
+ *   gp_precond_build                              x   .   .   .   .   .   .   .   .   .
+ *   gp_ciq_precond_build                          x   .   .   .   .   .   .   .   .   .
+ *   gp_precond_probes                             x   .   .   .   .   .   .   .   .   .
+ *   gp_bilinear_grad                              x   .   .   .   .   .   .   .   .   .
+ *   gp_mbcg with a preconditioner                 x   .   .   .   .   .   .   .   .   .
+ *   gp_ciq_sqrt_matmul_precond                    x   .   .   .   .   .   .   .   .   .
+ *   gp_plan_set_kron (as the data plan)           .   .   .   .   x   x   x   x   x   x
+ *   gp_plan_set_deriv (as the data plan)          .   .   .   .   x   x   x   x   x   x
+ *   gp_plan_set_deriv_kind (as the data plan)     .   .   .   .   x   x   x   x   x   x
+ *   gp_plan_set_kron data plan (re-check)         x   x   .   .   .   .   .   .   x   x
+ *   gp_plan_set_deriv(_kind) data plan (re-check) x   x   .   .   .   .   .   .   .   .
+ *   gp_plan_set_product, a factor                 .   .   .   .   x   x   x   x   x   x
+ *   kernel product, a factor (re-check)           x   x   .   .   .   .   .   .   x   x
+ *   gp_plan_set_sum, a term                       .   .   .   .   x   x   x   .   .   .
+ *   kernel sum, a term (re-check)                 .   x   .   .   .   .   .   .   .   .
+ */
+
 /* covariance function kinds: kernels/rbf_kernel.py:68-85, kernels/matern_kernel.py:85-110, kernels/rq_kernel.py (GP_RQ is set
  * through gp_plan_set_hypers_rq only, which also gives alpha), kernels/polynomial_kernel.py (GP_POLY is set through
  * gp_plan_set_hypers_poly only, which also gives the power and the offset) */
@@ -140,10 +187,7 @@ int gp_plan_set_sum(gp_plan* plan, gp_plan* const* terms, int n_terms);
  * gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond, gp_plan_set_noise_diag and
  * gp_time_kmv_kernel run on it.  gp_bilinear_grad returns, factor after factor, the gradients of that factor's lengthscale(s)
  * (1 or d_f entries, sum_f n_ls_f in all; total padded width <= 64) and in grad_os dF/dS of the combined scale (dF/ds_f = S / s_f
- * dF/dS).  A factor that is SKI, a sum, a product, multitask, derivative, low-rank-corrected or row-sharded is refused
- * (GP_E_SHAPE / GP_E_STATE); on a product plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv, gp_plan_set_sum,
- * gp_plan_set_ski, gp_plan_set_lowrank, gp_plan_set_backend, gp_plan_set_comm with more than one rank and the input-gradient
- * calls return GP_E_STATE. */
+ * dF/dS).  A SKI, sum, Kronecker, derivative or row-sharded factor returns GP_E_SHAPE. */
 int gp_plan_set_product(gp_plan* plan, gp_plan* const* factors, int n_factors);
 
 /* Additive GPs (the reference's ScaleKernel(RBFKernel(batch_shape=[D], ard_num_dims=1)) over X.mT.unsqueeze(-1), then .sum(dim=-3)
@@ -159,11 +203,7 @@ int gp_plan_set_product(gp_plan* plan, gp_plan* const* factors, int n_factors);
  * gp_precond_probes, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build,
  * gp_ciq_sqrt_matmul_precond, gp_plan_set_noise_diag, gp_plan_set_lowrank and gp_time_kmv_kernel run on it.  gp_bilinear_grad returns
  * the D lengthscale gradients dF/dl_i in grad_ls and the D component-scale gradients dF/ds_i in grad_os, which must hold D doubles.
- * A non-finite input makes products, rows, the diagonal and gradients NaN.  On an additive plan gp_plan_set_tasks, gp_plan_set_kron,
- * gp_plan_set_deriv, gp_plan_set_deriv_kind, gp_plan_set_sum, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_backend,
- * gp_plan_set_comm with more than one rank, gp_kmv_input_grad and gp_kdense_input_grad return GP_E_STATE with a message naming the
- * call; an additive plan as a term of gp_plan_set_sum, a factor of gp_plan_set_product or the data plan of gp_plan_set_kron /
- * gp_plan_set_deriv is refused the same way.  A SKI, sum, product, multitask, derivative or row-sharded plan cannot become additive. */
+ * A non-finite input makes products, rows, the diagonal and gradients NaN.  A SKI, sum or row-sharded plan cannot become additive. */
 int gp_plan_set_additive(gp_plan* plan, int max_degree, const float* comp_scale, int n_comp);
 
 /* Spectral mixture kernels (the reference's SpectralMixtureKernel, kernels/spectral_mixture_kernel.py, dense over [Q, n, m, d]):
@@ -181,12 +221,8 @@ int gp_plan_set_additive(gp_plan* plan, int max_degree, const float* comp_scale,
  * gp_kmv, gp_krows, gp_kdiag, gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos,
  * gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond, gp_plan_set_noise_diag, gp_plan_set_lowrank and
  * gp_time_kmv_kernel run on it.  gp_bilinear_grad returns Q (1 + 2d) doubles in grad_ls: dF/dw_q (Q), then dF/dmu_qc and dF/dv_qc
- * (Q d each, row-major); grad_os receives dF/dS.  A non-finite input makes products, rows, the diagonal and gradients NaN.  On a
- * spectral plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv, gp_plan_set_deriv_kind, gp_plan_set_sum,
- * gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_backend, gp_plan_set_comm with more than one rank,
- * gp_kmv_input_grad and gp_kdense_input_grad return GP_E_STATE with a message naming the call; a spectral plan as a term of
- * gp_plan_set_sum, a factor of gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.
- * A SKI, sum, product, multitask, derivative, additive or row-sharded plan cannot become a spectral plan. */
+ * (Q d each, row-major); grad_os receives dF/dS.  A non-finite input makes products, rows, the diagonal and gradients NaN.  A SKI, sum or
+ * row-sharded plan cannot become a spectral plan. */
 int gp_plan_set_spectral(gp_plan* plan, int Q, const float* weights, const float* means, const float* scales, int d);
 
 /* Periodic kernels (the reference's PeriodicKernel, kernels/periodic_kernel.py): `plan` becomes the operator
@@ -205,11 +241,7 @@ int gp_plan_set_spectral(gp_plan* plan, int Q, const float* weights, const float
  * gp_plan_set_noise_diag, gp_plan_set_lowrank and gp_time_kmv_kernel run on it, and it may be a term of gp_plan_set_sum.
  * gp_bilinear_grad returns n_ls + n_period doubles in grad_ls, [dF/dl (n_ls) | dF/dp (n_period)] (a shared parameter receives the
  * sum over the dimensions), and dF/dS in grad_os; it is formed from tau directly, not through the embedding.  A non-finite input
- * makes the gradients NaN.  On a periodic plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv, gp_plan_set_deriv_kind,
- * gp_plan_set_sum, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_spectral, gp_plan_set_comm with more
- * than one rank, gp_kmv_input_grad and gp_kdense_input_grad return GP_E_STATE with a message naming the call; a periodic plan as a
- * factor of gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.  A SKI, sum,
- * product, multitask, derivative, additive, spectral or row-sharded plan cannot become a periodic plan. */
+ * makes the gradients NaN.  A SKI, sum or row-sharded plan cannot become a periodic plan. */
 int gp_plan_set_periodic(gp_plan* plan, const float* period, int n_period, int d);
 
 /* Rational quadratic kernels (the reference's RQKernel, kernels/rq_kernel.py): kind GP_RQ with its alpha, set together with the
@@ -226,11 +258,7 @@ int gp_plan_set_periodic(gp_plan* plan, const float* period, int n_period, int d
  * gp_slq_logdet, gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond, gp_plan_set_backend,
  * gp_plan_set_noise_diag, gp_plan_set_lowrank (as the base), gp_kmv_input_grad, gp_kdense_input_grad and gp_time_kmv_kernel run on
  * it, and it may be a term of gp_plan_set_sum.  gp_bilinear_grad returns n_ls + 1 doubles in grad_ls, [dF/dl (n_ls) | dF/dalpha],
- * and dF/dS in grad_os; a non-finite input makes them NaN.  On an RQ plan gp_plan_set_tasks, gp_plan_set_kron, gp_plan_set_deriv,
- * gp_plan_set_deriv_kind, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_spectral, gp_plan_set_periodic
- * and gp_plan_set_comm with more than one rank return GP_E_STATE with a message naming the call; an RQ plan as a factor of
- * gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.  A SKI, sum, product,
- * multitask, derivative, additive, spectral, periodic or row-sharded plan cannot take this call (GP_E_STATE). */
+ * and dF/dS in grad_os; a non-finite input makes them NaN.  A SKI, sum or row-sharded plan cannot take this call (GP_E_STATE). */
 int gp_plan_set_hypers_rq(gp_plan* plan, const float* lengthscale, int n_ls, float alpha, float outputscale, float noise);
 
 /* Polynomial kernels (the reference's PolynomialKernel, kernels/polynomial_kernel.py): kind GP_POLY with its integer power p and
@@ -251,11 +279,8 @@ int gp_plan_set_hypers_rq(gp_plan* plan, const float* lengthscale, int n_ls, flo
  * the base), gp_kmv_input_grad, gp_kdense_input_grad and gp_time_kmv_kernel run on it, and it may be a term of gp_plan_set_sum.
  * gp_bilinear_grad returns one double in grad_ls, [dF/dc], and dF/dS in grad_os (the power is not learned); a non-finite input makes
  * them NaN.  The input gradients use dk/dx_i = S p (x_i . x_j + c)^(p-1) x_j: every pair contributes, and on a square plan the
- * diagonal pair contributes 2 S p (|x_i|^2 + c)^(p-1) x_i.  On a polynomial plan gp_plan_set_tasks, gp_plan_set_kron,
- * gp_plan_set_deriv, gp_plan_set_deriv_kind, gp_plan_set_product, gp_plan_set_ski, gp_plan_set_additive, gp_plan_set_spectral,
- * gp_plan_set_periodic and gp_plan_set_comm with more than one rank return GP_E_STATE with a message naming the call; a polynomial
- * plan as a factor of gp_plan_set_product or the data plan of gp_plan_set_kron / gp_plan_set_deriv is refused the same way.  A SKI,
- * sum, product, multitask, derivative, additive, spectral, periodic or row-sharded plan cannot take this call (GP_E_STATE). */
+ * diagonal pair contributes 2 S p (|x_i|^2 + c)^(p-1) x_i.  A SKI, sum or
+ * row-sharded plan cannot take this call (GP_E_STATE). */
 int gp_plan_set_hypers_poly(gp_plan* plan, int power, float offset, float outputscale, float noise);
 
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
@@ -265,8 +290,7 @@ int gp_plan_set_hypers_poly(gp_plan* plan, int power, float offset, float output
  * SIMT, kernel sum, SKI); GP_E_SHAPE otherwise.  The correction is one more partial slot of every product (U^T V reduced in a
  * fixed order: repeated products are bit-identical), so gp_kmv, gp_mbcg without W, gp_lanczos, gp_slq_logdet, gp_ciq_sqrt_matmul
  * and gp_mll (unpreconditioned) run on it; gp_kdiag returns diag(s K) - sum_j U_ij^2 and gp_krows the rows of s K - U U^T (also
- * for kernel sums).  gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond,
- * gp_bilinear_grad and gp_mbcg with W return GP_E_STATE while a correction is set; gp_mll skips its preconditioner.  A later
+ * for kernel sums); gp_mll skips its preconditioner.  A later
  * gp_plan_set_data / gp_plan_set_comm that changes the size or shards the plan makes every call that applies the correction
  * return GP_E_STATE until gp_plan_set_lowrank is called again. */
 int gp_plan_set_lowrank(gp_plan* plan, const float* U, int64_t ldu, int r);
@@ -276,14 +300,14 @@ int gp_plan_set_lowrank(gp_plan* plan, const float* U, int64_t ldu, int r);
  *     s K(x_i, x'_j) B[t_i, t'_j]   (+ its noise / per-row diagonal where a call adds it).
  * gp_plan_set_tasks: device int32 task ids, task1 [n1] and task2 [n2] (task2 = NULL on a square plan), 1 <= T <= 32; ids outside
  *   [0, T) return GP_E_SHAPE.  Call after gp_plan_set_data (new data drops the tasks); task1 = NULL clears them.  The ids are copied:
- *   the caller's arrays need not outlive the call.  GP_E_STATE on SKI, kernel-sum and low-rank-corrected plans, GP_E_SHAPE on a
- *   row-sharded plan.
+ *   the caller's arrays need not outlive the call.  GP_E_STATE on SKI and kernel-sum plans, GP_E_SHAPE on a row-sharded
+ *   plan.
  * gp_plan_set_task_covar: B as a host array, row-major T x T (need not be symmetric or PSD: not checked); call again whenever it
  *   changes, like gp_plan_set_hypers.  Every call that applies the operator returns GP_E_STATE until it has been set.
  * Tensor-core and SIMT plans, square and cross: gp_kmv, gp_krows, gp_kdiag (s B[t_i, t_i]: not constant), gp_pivoted_cholesky
  * (first pivot = argmax of that diagonal, as for SKI), gp_precond_build / gp_precond_probes, gp_mbcg, gp_slq_logdet, gp_mll,
  * gp_lanczos, gp_ciq_* and gp_bilinear_grad (lengthscale(s) and outputscale of s K o B).  The input gradients (gp_kmv_input_grad,
- * gp_kdense_input_grad, gp_ski_input_grad) return GP_E_STATE.  One K.V is one launch of the plain fused kernel per column task over
+ * gp_kdense_input_grad, gp_ski_input_grad) are refused.  One K.V is one launch of the plain fused kernel per column task over
  * that task's columns (rows and columns packed in task order), then B is applied row by row: no atomics, repeated calls agree bit
  * for bit.
  * gp_task_covar_grad: dB [T][T] (host, row-major) with dB[a][b] = s sum_{i: t_i = a} sum_{j: t'_j = b} (L_i . R_j) k(x_i, x'_j),
@@ -304,8 +328,7 @@ int gp_task_covar_grad(gp_plan* plan, const float* L, int64_t ldl, const float* 
  * outputscale.  One K.V of [N T, t] columns is ceil(T t / 16) launches of data's fused kernel on the B-mixed blocks
  * W[j, a t + c] = sum_b B[a, b] V[j T + b, c]: no atomics, repeated calls agree bit for bit.  gp_kmv, gp_krows, gp_kdiag,
  * gp_pivoted_cholesky, the preconditioner calls, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos and gp_ciq_* run on it.
- * GP_E_STATE / GP_E_SHAPE: a SKI, kernel-sum, multitask, low-rank-corrected or row-sharded data plan; gp_plan_set_comm with more
- * than one rank, gp_plan_set_lowrank, gp_plan_set_tasks and the input gradients on `plan`. */
+ * GP_E_SHAPE: a SKI, kernel-sum or row-sharded data plan, and gp_plan_set_comm with more than one rank on `plan`. */
 int gp_plan_set_kron(gp_plan* plan, gp_plan* data, int T);
 
 /* GPs with derivative observations (RBFKernelGrad, kernels/rbf_kernel_grad.py:60-115, with the perfect shuffle of :99-102, as in
@@ -322,9 +345,8 @@ int gp_plan_set_kron(gp_plan* plan, gp_plan* data, int T);
  * gp_kmv, gp_krows, gp_kdiag (s, s / l_a^2 on a square plan), gp_pivoted_cholesky (first pivot = argmax of that diagonal), the
  * preconditioner calls, gp_mbcg, gp_slq_logdet, gp_mll, gp_lanczos and gp_ciq_* run on it; gp_bilinear_grad returns the gradients of
  * data's lengthscale(s) and outputscale.  A non-finite input makes products, rows, the diagonal and gradients NaN.
- * GP_E_STATE / GP_E_SHAPE: a non-RBF, SKI, kernel-sum, multitask, Kronecker, derivative, low-rank-corrected or row-sharded data
- * plan, d > 16; gp_plan_set_comm with more than one rank, gp_plan_set_lowrank, gp_plan_set_tasks, gp_plan_set_kron and the input
- * gradients on `plan`. */
+ * GP_E_SHAPE: a non-RBF, SKI, kernel-sum, Kronecker, derivative or row-sharded data plan, d > 16, and gp_plan_set_comm with more
+ * than one rank on `plan`. */
 int gp_plan_set_deriv(gp_plan* plan, gp_plan* data);
 
 /* The same value / gradient operator for another covariance (kernels/matern52_kernel_grad.py): kind = GP_RBF is

@@ -188,20 +188,12 @@ def test_refusals():
         sum_interaction_terms([1, 2])
 
 
-def test_c_abi_declares_set_additive_and_every_refusal():
+def test_c_abi_declares_set_additive():
     hdr = open(os.path.join(ROOT, "include", "gp_bbmm.h")).read()
     assert re.search(r"int gp_plan_set_additive\(gp_plan\* plan, int max_degree, const float\* comp_scale, int n_comp\);", hdr)
     from gpytorch_b200 import _lib
 
     assert _lib.PROTOTYPES["gp_plan_set_additive"][1][1:] == [_lib._I, _lib.C.POINTER(_lib._F), _lib._I]
-    src = open(SRC).read() + "".join(open(os.path.join(ROOT, "gpytorch_b200", "csrc", f)).read()
-                                      for f in ("api.cu", "xgrad.cu", "tasks.cu", "kron.cu", "deriv.cu", "sum.cu", "product.cu", "ski.cu"))
-    for call in ("gp_plan_set_backend", "gp_plan_set_tasks", "gp_plan_set_kron", "gp_plan_set_sum", "gp_plan_set_product",
-                 "gp_plan_set_ski"):
-        assert f'GP_REFUSE_ADDITIVE(p, "{call}")' in src, call
-    assert "GP_REFUSE_ADDITIVE(p, what)" in src   # the input-gradient calls and gp_plan_set_deriv(_kind)
-    assert "gp_plan_set_comm with more than one rank is not available on an additive plan" in src
-    assert "an additive plan as a term is not available" in src and "an additive plan as a factor is not available" in src
 
 
 def _tool():

@@ -1,7 +1,6 @@
 """Periodic kernels without a GPU: the fp64 oracle against the reference's own PeriodicKernel (tests/golden/periodic_golden.npz), the
 bound's independence of |x|, the kernel's parameters, constraints, setters and refusals, operator construction and slots, the C
 ABI and the gradient kernel's ptxas report."""
-import glob
 import os
 import re
 
@@ -133,20 +132,12 @@ def test_plan_slots_are_disjoint():
     assert op._slot() == ops._PERIODIC_LOWRANK_SLOT
 
 
-def test_c_abi_declares_periodic_and_refusals():
+def test_c_abi_declares_periodic():
     h = open(os.path.join(ROOT, "include", "gp_bbmm.h")).read()
     assert "int gp_plan_set_periodic(gp_plan* plan, const float* period, int n_period, int d);" in h
     from gpytorch_b200 import _lib
 
     assert "gp_plan_set_periodic" in _lib.PROTOTYPES
-    src = {os.path.basename(f): open(f).read() for f in glob.glob(os.path.join(ROOT, "gpytorch_b200", "csrc", "*.cu"))}
-    for f, call in [("tasks.cu", "gp_plan_set_tasks"), ("kron.cu", "gp_plan_set_kron"), ("product.cu", "gp_plan_set_product"),
-                    ("ski.cu", "gp_plan_set_ski"), ("sum.cu", "gp_plan_set_sum"), ("additive.cu", "gp_plan_set_additive"),
-                    ("spectral.cu", "gp_plan_set_spectral")]:
-        assert f'GP_REFUSE_PERIODIC(p, "{call}")' in src[f], f
-    assert "GP_REFUSE_PERIODIC(p, what)" in src["xgrad.cu"] and "GP_REFUSE_PERIODIC(p, what)" in src["deriv.cu"]
-    assert "data->per_n == 0" in src["deriv.cu"] and 'GP_REFUSE_PERIODIC(data, "gp_plan_set_kron (as the data plan)")' in src["kron.cu"]
-    assert "factors[f]->per_n == 0" in src["product.cu"] and "p->per_n && comm" in src["api.cu"]
 
 
 def test_ptxas_reports_no_spills_in_periodic_kernels():

@@ -99,14 +99,12 @@ def test_class_surface_and_wrappers():
         gp.kernels.MultitaskKernel(gp.kernels.PolynomialKernel(2), num_tasks=2)(x)
 
 
-def test_header_and_sources_document_the_call():
+def test_header_and_api_document_the_call():
     h = open(os.path.join(ROOT, "include", "gp_bbmm.h")).read()
     assert "GP_POLY = 5" in h
     assert re.search(r"int gp_plan_set_hypers_poly\(gp_plan\* plan, int power, float offset, float outputscale, float noise\);", h)
     api = open(os.path.join(ROOT, "gpytorch_b200", "csrc", "api.cu")).read()
     assert "call gp_plan_set_hypers_poly" in api
-    for f in ("additive.cu", "periodic.cu", "ski.cu", "spectral.cu", "tasks.cu", "product.cu", "kron.cu", "deriv.cu"):
-        assert "GP_REFUSE_POLY" in open(os.path.join(ROOT, "gpytorch_b200", "csrc", f)).read(), f
 
 
 def _tool(name):

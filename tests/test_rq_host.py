@@ -200,15 +200,23 @@ def test_plan_key_contains_alpha():
 
 
 # ---- header, C ABI, compiled kernels ------------------------------------------------------------------------------------------
-def test_header_documents_the_call():
+def test_header_and_settings_table_document_the_call():
     h = open(os.path.join(ROOT, "include", "gp_bbmm.h")).read()
     assert "GP_RQ = 4" in h
     assert re.search(r"int gp_plan_set_hypers_rq\(gp_plan\* plan, const float\* lengthscale, int n_ls, float alpha,", h)
     doc = h[h.index("Rational quadratic kernels"):h.index("int gp_plan_set_hypers_rq")]
-    for call in ("gp_plan_set_tasks", "gp_plan_set_kron", "gp_plan_set_deriv", "gp_plan_set_product", "gp_plan_set_ski",
-                 "gp_plan_set_additive", "gp_plan_set_spectral", "gp_plan_set_periodic", "gp_plan_set_comm", "gp_plan_set_sum",
-                 "gp_kmv_input_grad", "[dF/dl (n_ls) | dF/dalpha]"):
+    for call in ("gp_plan_set_sum", "gp_kmv_input_grad", "[dF/dl (n_ls) | dF/dalpha]"):
         assert call in doc, call
+    # the calls an RQ plan refuses: an x in the rq column of the plan-settings table
+    table = h[h.index("Plan settings."):h.index("*/", h.index("Plan settings."))]
+    head = next(ln for ln in table.splitlines() if ln.rstrip().endswith("rq  ply"))
+    col = head.index(" rq ") + 1
+    refusing = {ln[5:col].split("  ")[0].strip() for ln in table.splitlines() if len(ln) > col and ln[col] == "x"}
+    for call in ("gp_plan_set_tasks", "gp_plan_set_kron", "gp_plan_set_deriv", "gp_plan_set_deriv_kind", "gp_plan_set_product",
+                 "gp_plan_set_ski", "gp_plan_set_additive", "gp_plan_set_spectral", "gp_plan_set_periodic",
+                 "gp_plan_set_comm with more than one rank", "gp_plan_set_kron (as the data plan)", "gp_plan_set_deriv (as the data plan)",
+                 "gp_plan_set_product, a factor"):
+        assert call in refusing, call
 
 
 def _tool(name):

@@ -263,7 +263,7 @@ def test_plan_slots_keep_low_rank_spectral_plans_apart(monkeypatch):
     assert len(set(slots)) == 3
 
 
-def test_c_abi_declares_set_spectral_and_every_refusal():
+def test_c_abi_declares_set_spectral():
     hdr = open(os.path.join(ROOT, "include", "gp_bbmm.h")).read()
     assert re.search(r"int gp_plan_set_spectral\(gp_plan\* plan, int Q, const float\* weights, const float\* means, "
                      r"const float\* scales, int d\);", hdr)
@@ -271,16 +271,6 @@ def test_c_abi_declares_set_spectral_and_every_refusal():
 
     F = _lib.C.POINTER(_lib._F)
     assert _lib.PROTOTYPES["gp_plan_set_spectral"] == (_lib._I, [_lib._P, _lib._I, F, F, F, _lib._I])
-    src = "".join(open(os.path.join(ROOT, "gpytorch_b200", "csrc", f)).read()
-                  for f in ("api.cu", "xgrad.cu", "tasks.cu", "kron.cu", "deriv.cu", "sum.cu", "product.cu", "ski.cu", "additive.cu"))
-    for call in ("gp_plan_set_backend", "gp_plan_set_tasks", "gp_plan_set_kron", "gp_plan_set_sum", "gp_plan_set_product",
-                 "gp_plan_set_ski", "gp_plan_set_additive"):
-        assert f'GP_REFUSE_SPECTRAL(p, "{call}")' in src, call
-    assert src.count("GP_REFUSE_SPECTRAL(p, what)") == 2   # the input-gradient calls and gp_plan_set_deriv(_kind)
-    assert "gp_plan_set_comm with more than one rank is not available on a spectral mixture plan" in src
-    assert "a spectral mixture plan as a term is not available" in src and "a spectral mixture plan as a factor is not available" in src
-    assert 'GP_REFUSE_SPECTRAL(data, "gp_plan_set_kron (as the data plan)")' in src
-    assert "(as the data plan) is not available on a spectral mixture plan" in src
 
 
 def test_ptxas_reports_no_spills_for_any_instantiation():
