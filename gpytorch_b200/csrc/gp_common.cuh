@@ -185,6 +185,14 @@ struct gp_kron_state {
   gp::DevBuf Bd;                           // B on the device
   gp::DevBuf W, Vt, part;                  // mixed chunks [nchunk][npad][16] | their packed V tiles | data's slots per chunk
   gp::DevBuf Lw, red, idx, rows;           // gradient / row-extraction scratch
+  // observed rows / columns (gp_plan_set_kron_observed): the operator is P_r ((s K) (x) B) P_c^T.  Host index lists (empty: all
+  // observed), on the device the maps and their inverses (-1 where an interleaved row is not observed) as int32 (N T < 2^31)
+  bool masked = false;
+  int64_t mask_n1 = 0, mask_n2 = 0;        // data plan sizes N1, N2 the mask was given for
+  std::vector<int> obs_r, obs_c;
+  gp::DevBuf rowmap, colmap, rowpos, colpos;
+  gp::DevBuf Lx, Rx, full, gidx;           // gradient operands expanded to N T rows | full rows / diagonal before the gather |
+                                           // the interleaved row of each requested row
 };
 
 // Derivative-observation state (deriv.cu, deriv_table.cuh): the RBF or Matern-5/2 value / gradient operator over interleaved rows

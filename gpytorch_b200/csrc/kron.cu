@@ -25,9 +25,12 @@ namespace gp {
 constexpr int KRON_RED_ROWS = 2048;   // points per block of the dB reduction
 
 // W[q][j][cc] = sum_b B[a][b] V16[j T + b][c] for the column col = 16 q + cc = a t + c (B == nullptr: V16[j T + a][c], the
-// unmixed chunks); zero for col >= T t and for the padding rows j >= n
+// unmixed chunks); zero for col >= T t and for the padding rows j >= n.  MASKED: V16 holds the observed rows only, and row j T + b
+// is V16[colpos[j T + b]], or 0 where colpos is -1 (a missing column of P_r ((s K) (x) B) P_c^T)
+template <bool MASKED>
 __global__ void kron_mix_kernel(const float* __restrict__ V16, int64_t n, int64_t npad, int T, int t, int nchunk,
-                                const float* __restrict__ B, float* __restrict__ W, const int* __restrict__ done_flag) {
+                                const float* __restrict__ B, float* __restrict__ W, const int* __restrict__ done_flag,
+                                const int* __restrict__ colpos) {
   if (done_flag && *done_flag) return;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (int64_t)nchunk * npad * TP) return;
@@ -38,26 +41,43 @@ __global__ void kron_mix_kernel(const float* __restrict__ V16, int64_t n, int64_
   float s = 0.f;
   if (j < n && col < T * t) {
     const int a = col / t, c = col % t;
-    const float* v = V16 + j * T * TP + c;
-    if (B) {
-      const float* br = B + a * T;
-      for (int b = 0; b < T; ++b) s = fmaf(br[b], v[b * TP], s);
+    if constexpr (MASKED) {
+      const int* cp = colpos + j * T;
+      if (B) {
+        const float* br = B + a * T;
+        for (int b = 0; b < T; ++b) {
+          const int r = cp[b];
+          s = fmaf(br[b], r >= 0 ? V16[(int64_t)r * TP + c] : 0.f, s);
+        }
+      } else {
+        const int r = cp[a];
+        s = r >= 0 ? V16[(int64_t)r * TP + c] : 0.f;
+      }
     } else {
-      s = v[a * TP];
+      const float* v = V16 + j * T * TP + c;
+      if (B) {
+        const float* br = B + a * T;
+        for (int b = 0; b < T; ++b) s = fmaf(br[b], v[b * TP], s);
+      } else {
+        s = v[a * TP];
+      }
     }
   }
   W[idx] = s;
 }
 
 // out[(i T + a)][c] = sum_sp part[q][sp][i][cc] for col = a t + c = 16 q + cc (c < t), 0 for c >= t; NaN for non-finite inputs or
-// a non-finite B (the fused kernels' clamps and operand splits need not carry a NaN of the mixed block through)
+// a non-finite B (the fused kernels' clamps and operand splits need not carry a NaN of the mixed block through).  MASKED: out has
+// the nrows observed rows, and observed row r is interleaved row rowmap[r] = i T + a
+template <bool MASKED>
 __global__ void kron_scatter_kernel(const float* __restrict__ part, int nsplit, int64_t rows_pad, int64_t n1, int T, int t,
-                                    float* __restrict__ out, const int* __restrict__ xbad, int bbad, const int* __restrict__ done_flag) {
+                                    float* __restrict__ out, const int* __restrict__ xbad, int bbad, const int* __restrict__ done_flag,
+                                    const int* __restrict__ rowmap, int64_t nrows) {
   if (done_flag && *done_flag) return;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n1 * T * TP) return;
+  if (idx >= (MASKED ? nrows : n1 * T) * TP) return;
   const int c = (int)(idx % TP);
-  const int64_t r = idx / TP;
+  const int64_t r = MASKED ? (int64_t)rowmap[idx / TP] : idx / TP;
   const int64_t i = r / T;
   const int a = (int)(r % T);
   float s = 0.f;
@@ -125,6 +145,34 @@ __global__ void kron_expand_diag_kernel(const float* __restrict__ d, int64_t n1,
   OUT[e] = d[e / T] * B[a * T + a];
 }
 
+// masked plans: OUT[r][e] = SRC[r][map[e]] (observed columns of full rows, or observed entries of the full diagonal with m = 1)
+__global__ void masked_kron_gather_kernel(const float* __restrict__ SRC, int64_t lds, const int* __restrict__ map, int64_t ncols,
+                                   float* __restrict__ OUT, int64_t ldo) {
+  const int64_t r = blockIdx.y;
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= ncols) return;
+  OUT[r * ldo + e] = SRC[r * lds + map[e]];
+}
+
+// masked plans: the interleaved row rowmap[v] of each requested observed row v (-1 outside [0, nrows): a NaN row, as unmasked)
+__global__ void masked_kron_idx_kernel(const int64_t* __restrict__ idx, int64_t m, const int* __restrict__ rowmap, int64_t nrows,
+                                    int64_t* __restrict__ out) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= m) return;
+  const int64_t v = idx[r];
+  out[r] = (v >= 0 && v < nrows) ? (int64_t)rowmap[v] : -1;
+}
+
+// masked plans: OUT [nfull][s] = the observed rows of SRC [.][ld] at their interleaved rows, zero on the missing rows (the gradients
+// of P_r ((s K) (x) B) P_c^T are those of (s K) (x) B with L and R zero there)
+__global__ void masked_kron_expand_kernel(const float* __restrict__ SRC, int64_t ld, int s, const int* __restrict__ pos, int64_t nfull,
+                                       float* __restrict__ OUT) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= nfull * s) return;
+  const int r = pos[e / s];
+  OUT[e] = r >= 0 ? SRC[(int64_t)r * ld + (int)(e % s)] : 0.f;
+}
+
 static int kron_check_data(const gp_plan* p, const gp_plan* q) {
   GP_REQUIRE(q->data_set && q->hypers_set, GP_E_STATE, "Kronecker plan: the data plan needs set_data + set_hypers");
   GP_REQUIRE(q->backend == GP_BACKEND_TCGEN05 || q->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
@@ -143,8 +191,8 @@ static void kron_geometry(gp_plan* p) {
   const gp_plan* q = p->kron->data;
   const int T = p->kron->T;
   p->backend = GP_BACKEND_KRON;
-  p->n1 = q->n1 * T;
-  p->n2 = q->n2 * T;
+  p->n1 = p->kron->masked ? (int64_t)p->kron->obs_r.size() : q->n1 * T;
+  p->n2 = p->kron->masked ? (int64_t)p->kron->obs_c.size() : q->n2 * T;
   p->same = q->same;
   p->d = q->d;
   p->row_begin = 0;
@@ -162,7 +210,8 @@ int kron_refresh(gp_plan* p) {
   gp_kron_state* ks = p->kron;
   const gp_plan* q = ks->data;
   GP_CHECK(kron_check_data(p, q));
-  GP_REQUIRE(p->n1 == q->n1 * ks->T && p->n2 == q->n2 * ks->T && p->same == q->same, GP_E_STATE,
+  const int64_t n1 = ks->masked ? (int64_t)ks->obs_r.size() : q->n1 * ks->T, n2 = ks->masked ? (int64_t)ks->obs_c.size() : q->n2 * ks->T;
+  GP_REQUIRE(p->n1 == n1 && p->n2 == n2 && p->same == q->same && (!ks->masked || (q->n1 == ks->mask_n1 && q->n2 == ks->mask_n2)), GP_E_STATE,
              "Kronecker plan: the data plan changed its size; call gp_plan_set_kron again");
   p->kind = q->kind;
   p->outputscale = q->outputscale;   // the finish kernels scale the unscaled product by the data plan's s
@@ -182,6 +231,8 @@ int kron_pack(gp_plan* p) {
 static int64_t kron_npad(const gp_plan* q) { return q->backend == GP_BACKEND_TCGEN05 ? q->ntile_j * TILE_J : q->n2; }
 
 // V16 [N2 T][16] with t live columns, mixed by B (or not: B == nullptr) -> nchunk data-kernel products in ks->part
+// MASKED: V16 holds the observed columns only (ks->colpos places them)
+template <bool MASKED>
 static int kron_chunks(gp_plan* p, const float* V16, int t, const float* B, int kind, const int* done_flag, int* nchunk_out) {
   gp_kron_state* ks = p->kron;
   gp_plan* q = ks->data;
@@ -193,7 +244,8 @@ static int kron_chunks(gp_plan* p, const float* V16, int t, const float* B, int 
   GP_CHECK(ks->W.ensure(sizeof(float) * (size_t)nchunk * npad * TP));
   GP_CHECK(ks->part.ensure(sizeof(float) * (size_t)nchunk * q->nsplit * slot_floats));
   const int64_t tot = (int64_t)nchunk * npad * TP;
-  kron_mix_kernel<<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(V16, q->n2, npad, T, t, nchunk, B, ks->W.as<float>(), done_flag);
+  kron_mix_kernel<MASKED><<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(V16, q->n2, npad, T, t, nchunk, B, ks->W.as<float>(), done_flag,
+                                                                            ks->colpos.as<int>());
   p->launches++;
   GP_CUDA(cudaGetLastError());
   if (tc) {
@@ -223,9 +275,16 @@ int kron_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   const gp_plan* q = ks->data;
   const int t = p->kron_cols;
   int nchunk = 0;
-  GP_CHECK(kron_chunks(p, V16, t, ks->Bd.as<float>(), q->kind, done_flag, &nchunk));
-  kron_scatter_kernel<<<(unsigned)cdiv(p->n1 * TP, 256), 256, 0, p->stream>>>(ks->part.as<float>(), q->nsplit, q->rows_pad, q->n1, ks->T, t,
-                                                                             p->partial.as<float>(), q->xbad, ks->b_bad ? 1 : 0, done_flag);
+  const unsigned grid = (unsigned)cdiv(p->n1 * TP, 256);
+  if (ks->masked) {
+    GP_CHECK(kron_chunks<true>(p, V16, t, ks->Bd.as<float>(), q->kind, done_flag, &nchunk));
+    kron_scatter_kernel<true><<<grid, 256, 0, p->stream>>>(ks->part.as<float>(), q->nsplit, q->rows_pad, q->n1, ks->T, t, p->partial.as<float>(),
+                                                           q->xbad, ks->b_bad ? 1 : 0, done_flag, ks->rowmap.as<int>(), p->n1);
+  } else {
+    GP_CHECK(kron_chunks<false>(p, V16, t, ks->Bd.as<float>(), q->kind, done_flag, &nchunk));
+    kron_scatter_kernel<false><<<grid, 256, 0, p->stream>>>(ks->part.as<float>(), q->nsplit, q->rows_pad, q->n1, ks->T, t, p->partial.as<float>(),
+                                                            q->xbad, ks->b_bad ? 1 : 0, done_flag, nullptr, 0);
+  }
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -237,14 +296,28 @@ int kron_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ld
   GP_REQUIRE(m <= 65535, GP_E_SHAPE, "rows of a Kronecker plan: at most 65535 rows per call (m=%lld)", (long long)m);
   GP_CHECK(kron_refresh(p));
   gp_plan* q = ks->data;
+  const int64_t n1f = q->n1 * ks->T, n2f = q->n2 * ks->T;
   GP_CHECK(ks->idx.ensure(sizeof(int64_t) * m));
   GP_CHECK(ks->rows.ensure(sizeof(float) * (size_t)m * q->n2));
-  kron_point_idx_kernel<<<(unsigned)cdiv(m, 256), 256, 0, p->stream>>>(idx, m, ks->T, p->n1, ks->idx.as<int64_t>());
+  if (ks->masked) {   // requested observed rows -> interleaved rows; full rows into scratch, then the observed columns
+    GP_CHECK(ks->gidx.ensure(sizeof(int64_t) * m));
+    GP_CHECK(ks->full.ensure(sizeof(float) * (size_t)m * n2f));
+    masked_kron_idx_kernel<<<(unsigned)cdiv(m, 256), 256, 0, p->stream>>>(idx, m, ks->rowmap.as<int>(), p->n1, ks->gidx.as<int64_t>());
+    p->launches++;
+    idx = ks->gidx.as<int64_t>();
+  }
+  kron_point_idx_kernel<<<(unsigned)cdiv(m, 256), 256, 0, p->stream>>>(idx, m, ks->T, n1f, ks->idx.as<int64_t>());
   p->launches++;
   GP_CHECK(gp_krows(q, ks->idx.as<int64_t>(), m, ks->rows.as<float>(), q->n2));
-  kron_expand_rows_kernel<<<dim3((unsigned)cdiv(p->n2, 256), (unsigned)m), 256, 0, p->stream>>>(ks->rows.as<float>(), q->n2, idx, p->n1,
-                                                                                             ks->Bd.as<float>(), ks->T, OUT, ldo);
+  float* dst = ks->masked ? ks->full.as<float>() : OUT;
+  kron_expand_rows_kernel<<<dim3((unsigned)cdiv(n2f, 256), (unsigned)m), 256, 0, p->stream>>>(ks->rows.as<float>(), q->n2, idx, n1f,
+                                                                                          ks->Bd.as<float>(), ks->T, dst,
+                                                                                          ks->masked ? n2f : ldo);
   p->launches++;
+  if (ks->masked) {
+    masked_kron_gather_kernel<<<dim3((unsigned)cdiv(p->n2, 256), (unsigned)m), 256, 0, p->stream>>>(dst, n2f, ks->colmap.as<int>(), p->n2, OUT, ldo);
+    p->launches++;
+  }
   GP_CUDA(cudaGetLastError());
   return GP_OK;
 }
@@ -256,9 +329,34 @@ int kron_kdiag(gp_plan* p, float* OUT) {
   gp_plan* q = ks->data;
   GP_CHECK(ks->rows.ensure(sizeof(float) * q->n1));
   GP_CHECK(gp_kdiag(q, ks->rows.as<float>()));
-  kron_expand_diag_kernel<<<(unsigned)cdiv(p->n1, 256), 256, 0, p->stream>>>(ks->rows.as<float>(), q->n1, ks->Bd.as<float>(), ks->T, OUT);
+  const int64_t n1f = q->n1 * ks->T;
+  if (ks->masked) GP_CHECK(ks->full.ensure(sizeof(float) * n1f));
+  float* dst = ks->masked ? ks->full.as<float>() : OUT;
+  kron_expand_diag_kernel<<<(unsigned)cdiv(n1f, 256), 256, 0, p->stream>>>(ks->rows.as<float>(), q->n1, ks->Bd.as<float>(), ks->T, dst);
   p->launches++;
+  if (ks->masked) {   // s B[a, a] k_ii gathered by the row map
+    masked_kron_gather_kernel<<<dim3((unsigned)cdiv(p->n1, 256), 1u), 256, 0, p->stream>>>(dst, 0, ks->rowmap.as<int>(), p->n1, OUT, 0);
+    p->launches++;
+  }
   GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
+// masked plans: L [n_rows][.] and R [n_cols][.] expanded with zeros to the N1 T and N2 T interleaved rows (ld = s), so that the
+// unmasked gradient passes below run on them unchanged; unmasked plans pass L and R through
+static int kron_expand_operands(gp_plan* p, const float** L, int64_t* ldl, const float** R, int64_t* ldr, int s) {
+  gp_kron_state* ks = p->kron;
+  if (!ks->masked) return GP_OK;
+  const gp_plan* q = ks->data;
+  const int64_t n1f = q->n1 * ks->T, n2f = q->n2 * ks->T;
+  GP_CHECK(ks->Lx.ensure(sizeof(float) * (size_t)n1f * s));
+  GP_CHECK(ks->Rx.ensure(sizeof(float) * (size_t)n2f * s));
+  masked_kron_expand_kernel<<<(unsigned)cdiv(n1f * s, 256), 256, 0, p->stream>>>(*L, *ldl, s, ks->rowpos.as<int>(), n1f, ks->Lx.as<float>());
+  masked_kron_expand_kernel<<<(unsigned)cdiv(n2f * s, 256), 256, 0, p->stream>>>(*R, *ldr, s, ks->colpos.as<int>(), n2f, ks->Rx.as<float>());
+  p->launches += 2;
+  GP_CUDA(cudaGetLastError());
+  *L = ks->Lx.as<float>(); *R = ks->Rx.as<float>();
+  *ldl = s; *ldr = s;
   return GP_OK;
 }
 
@@ -269,22 +367,26 @@ int kron_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, 
   GP_CHECK(kron_refresh(p));
   gp_plan* q = ks->data;
   const int T = ks->T;
+  const int64_t n1f = q->n1 * T, n2f = q->n2 * T;
+  GP_CHECK(kron_expand_operands(p, &L, &ldl, &R, &ldr, s));
   const int nls = (int)q->ls.size();
   std::vector<double> gl(nls, 0.0), tot(nls, 0.0);
   double go = 0.0, tot_os = 0.0;
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->n1 * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
+  GP_CHECK(p->misc2.ensure(sizeof(float) * n1f * TP));
+  GP_CHECK(p->misc3.ensure(sizeof(float) * n2f * TP));
   for (int c0 = 0; c0 < s; c0 += TP) {
     const int tc = std::min(TP, s - c0);
-    GP_CHECK(to_v16(p, L + c0, ldl, tc, p->n1, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, R + c0, ldr, tc, p->n2, p->misc3.as<float>()));
+    GP_CHECK(to_v16(p, L + c0, ldl, tc, n1f, p->misc2.as<float>()));
+    GP_CHECK(to_v16(p, R + c0, ldr, tc, n2f, p->misc3.as<float>()));
     const int nchunk = (int)cdiv((int64_t)T * tc, TP);
     GP_CHECK(ks->Lw.ensure(sizeof(float) * (size_t)nchunk * q->n1 * TP));
     GP_CHECK(ks->W.ensure(sizeof(float) * (size_t)nchunk * q->n2 * TP));
-    kron_mix_kernel<<<(unsigned)cdiv((int64_t)nchunk * q->n1 * TP, 256), 256, 0, p->stream>>>(p->misc2.as<float>(), q->n1, q->n1, T, tc, nchunk,
-                                                                                             nullptr, ks->Lw.as<float>(), nullptr);
-    kron_mix_kernel<<<(unsigned)cdiv((int64_t)nchunk * q->n2 * TP, 256), 256, 0, p->stream>>>(p->misc3.as<float>(), q->n2, q->n2, T, tc, nchunk,
-                                                                                             ks->Bd.as<float>(), ks->W.as<float>(), nullptr);
+    kron_mix_kernel<false><<<(unsigned)cdiv((int64_t)nchunk * q->n1 * TP, 256), 256, 0, p->stream>>>(p->misc2.as<float>(), q->n1, q->n1, T, tc,
+                                                                                                    nchunk, nullptr, ks->Lw.as<float>(), nullptr,
+                                                                                                    nullptr);
+    kron_mix_kernel<false><<<(unsigned)cdiv((int64_t)nchunk * q->n2 * TP, 256), 256, 0, p->stream>>>(p->misc3.as<float>(), q->n2, q->n2, T, tc,
+                                                                                                    nchunk, ks->Bd.as<float>(), ks->W.as<float>(),
+                                                                                                    nullptr, nullptr);
     p->launches += 2;
     GP_CUDA(cudaGetLastError());
     for (int c = 0; c < nchunk; ++c) {
@@ -307,17 +409,19 @@ static int kron_task_covar_grad(gp_plan* p, const float* L, int64_t ldl, const f
   GP_CHECK(kron_refresh(p));
   gp_plan* q = ks->data;
   const int T = ks->T;
+  const int64_t n1f = q->n1 * T, n2f = q->n2 * T;
+  GP_CHECK(kron_expand_operands(p, &L, &ldl, &R, &ldr, t));
   const int nz = (int)cdiv(q->n1, KRON_RED_ROWS);
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->n1 * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
+  GP_CHECK(p->misc2.ensure(sizeof(float) * n1f * TP));
+  GP_CHECK(p->misc3.ensure(sizeof(float) * n2f * TP));
   GP_CHECK(ks->red.ensure(sizeof(double) * (size_t)nz * T * T));
   std::vector<double> acc((size_t)T * T, 0.0), h((size_t)nz * T * T);
   for (int c0 = 0; c0 < t; c0 += TP) {
     const int tc = std::min(TP, t - c0);
-    GP_CHECK(to_v16(p, L + c0, ldl, tc, p->n1, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, R + c0, ldr, tc, p->n2, p->misc3.as<float>()));
+    GP_CHECK(to_v16(p, L + c0, ldl, tc, n1f, p->misc2.as<float>()));
+    GP_CHECK(to_v16(p, R + c0, ldr, tc, n2f, p->misc3.as<float>()));
     int nchunk = 0;
-    GP_CHECK(kron_chunks(p, p->misc3.as<float>(), tc, nullptr, q->kind, nullptr, &nchunk));
+    GP_CHECK(kron_chunks<false>(p, p->misc3.as<float>(), tc, nullptr, q->kind, nullptr, &nchunk));
     kron_dB_kernel<<<dim3((unsigned)nz, (unsigned)(T * T)), 256, 0, p->stream>>>(ks->part.as<float>(), q->nsplit, q->rows_pad,
                                                                                 p->misc2.as<float>(), q->n1, T, tc, ks->red.as<double>(), q->xbad);
     p->launches++;
@@ -333,7 +437,8 @@ static int kron_task_covar_grad(gp_plan* p, const float* L, int64_t ldl, const f
 
 static void kron_release(gp_plan* p) {
   gp_kron_state* ks = p->kron;
-  gp::DevBuf* bufs[] = {&ks->Bd, &ks->W, &ks->Vt, &ks->part, &ks->Lw, &ks->red, &ks->idx, &ks->rows};
+  gp::DevBuf* bufs[] = {&ks->Bd, &ks->W, &ks->Vt, &ks->part, &ks->Lw, &ks->red, &ks->idx, &ks->rows, &ks->rowmap, &ks->colmap,
+                        &ks->rowpos, &ks->colpos, &ks->Lx, &ks->Rx, &ks->full, &ks->gidx};
   for (auto* b : bufs) b->release();
   delete ks;
   p->kron = nullptr;
@@ -377,10 +482,78 @@ extern "C" int gp_plan_set_kron(gp_plan* p, gp_plan* data, int T) {
     return st;
   }
   if (!keep_b) ks->b_set = false;
+  if (ks->masked && !(oldT == T && data->n1 == ks->mask_n1 && data->n2 == ks->mask_n2)) {   // the mask was for other sizes
+    ks->masked = false;
+    ks->obs_r.clear();
+    ks->obs_c.clear();
+    p->noise_diag = nullptr;
+  }
   p->backend_req = GP_BACKEND_KRON;
   kron_geometry(p);
   p->data_set = true;
   return p->hypers_set ? kron_pack(p) : GP_OK;   // without the noise yet: packed by gp_plan_set_hypers
+}
+
+// host index list -> int32 vector; nullptr: every one of the nfull rows (empty vector)
+static int kron_obs_list(const int64_t* idx, int64_t m, int64_t nfull, const char* what, std::vector<int>* out) {
+  out->clear();
+  if (idx == nullptr) return GP_OK;
+  GP_REQUIRE(m >= 1 && m <= nfull, GP_E_SHAPE, "gp_plan_set_kron_observed: %lld observed %s not in [1, %lld]", (long long)m, what,
+             (long long)nfull);
+  for (int64_t r = 0; r < m; ++r) {
+    GP_REQUIRE(idx[r] >= 0 && idx[r] < nfull && (r == 0 || idx[r] > idx[r - 1]), GP_E_SHAPE,
+               "gp_plan_set_kron_observed: %s must be strictly increasing in [0, %lld) (entry %lld is %lld)", what, (long long)nfull,
+               (long long)r, (long long)idx[r]);
+  }
+  if (m == nfull) return GP_OK;   // every row observed: the unmasked operator
+  out->resize((size_t)m);
+  for (int64_t r = 0; r < m; ++r) (*out)[(size_t)r] = (int)idx[r];
+  return GP_OK;
+}
+
+// map [m] and its inverse [nfull] (-1 where missing) on the device; an empty list stands for the identity
+static int kron_obs_upload(const std::vector<int>& obs, int64_t nfull, gp::DevBuf* map, gp::DevBuf* pos, cudaStream_t st) {
+  std::vector<int> m(obs), inv((size_t)nfull, -1);
+  if (m.empty()) {
+    m.resize((size_t)nfull);
+    for (int64_t r = 0; r < nfull; ++r) m[(size_t)r] = (int)r;
+  }
+  for (size_t r = 0; r < m.size(); ++r) inv[(size_t)m[r]] = (int)r;
+  GP_CHECK(map->ensure(sizeof(int) * m.size()));
+  GP_CHECK(pos->ensure(sizeof(int) * inv.size()));
+  GP_CUDA(cudaMemcpyAsync(map->p, m.data(), sizeof(int) * m.size(), cudaMemcpyHostToDevice, st));
+  GP_CUDA(cudaMemcpyAsync(pos->p, inv.data(), sizeof(int) * inv.size(), cudaMemcpyHostToDevice, st));
+  GP_CUDA(cudaStreamSynchronize(st));   // the host vectors go out of scope
+  return GP_OK;
+}
+
+extern "C" int gp_plan_set_kron_observed(gp_plan* p, const int64_t* rows, int64_t n_rows, const int64_t* cols, int64_t n_cols) {
+  GP_REQUIRE(p != nullptr && p->kron != nullptr, GP_E_STATE, "gp_plan_set_kron_observed: not a Kronecker plan (gp_plan_set_kron)");
+  GP_CUDA(cudaSetDevice(p->device));
+  gp_kron_state* ks = p->kron;
+  const gp_plan* q = ks->data;
+  const int64_t n1f = q->n1 * ks->T, n2f = q->n2 * ks->T;
+  std::vector<int> r, c;
+  GP_CHECK(kron_obs_list(rows, n_rows, n1f, "rows", &r));
+  GP_CHECK(kron_obs_list(cols, n_cols, n2f, "columns", &c));
+  GP_REQUIRE(!q->same || r == c, GP_E_SHAPE, "gp_plan_set_kron_observed: a square plan takes equal row and column masks");
+  GP_CUDA(cudaStreamSynchronize(p->stream));   // in-flight products may read the old maps
+  const bool masked = !r.empty() || !c.empty();
+  if (masked) {
+    GP_CHECK(kron_obs_upload(r, n1f, &ks->rowmap, &ks->rowpos, p->stream));
+    GP_CHECK(kron_obs_upload(c, n2f, &ks->colmap, &ks->colpos, p->stream));
+    if (r.empty()) { r.resize((size_t)n1f); for (int64_t i = 0; i < n1f; ++i) r[(size_t)i] = (int)i; }
+    if (c.empty()) { c.resize((size_t)n2f); for (int64_t i = 0; i < n2f; ++i) c[(size_t)i] = (int)i; }
+  }
+  const int64_t old_n1 = p->n1;
+  ks->masked = masked;
+  ks->obs_r.swap(r);
+  ks->obs_c.swap(c);
+  ks->mask_n1 = q->n1;
+  ks->mask_n2 = q->n2;
+  kron_geometry(p);
+  if (p->n1 != old_n1) p->noise_diag = nullptr;   // it had one entry per row of the old operator
+  return p->hypers_set ? kron_pack(p) : GP_OK;
 }
 
 // gp_plan_set_task_covar / gp_task_covar_grad on a Kronecker plan (tasks.cu forwards them here)

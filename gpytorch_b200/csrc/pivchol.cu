@@ -204,6 +204,9 @@ constexpr int PC_KIND_M52GRAD = 69;
 constexpr int PC_KIND_ADDITIVE = 70;
 // spectral mixture kernels (spectral.cu): K[pivot, j] = S prod_d sum_q w_q e_qd cos_qd from the plan's packed rows
 constexpr int PC_KIND_SPECTRAL = 71;
+// Kronecker with observed rows (kron.cu, gp_plan_set_kron_observed): row r is interleaved row g = task[r] (the row map), point
+// g / T, task g mod T; entries as PC_KIND_TASK
+constexpr int PC_KIND_KRON_OBS = 72;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -286,6 +289,9 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
       }
     } else if (KIND == PC_KIND_SKI) {
       ski_stage_u(sk, pi, zp, tid, PCP_THREADS);
+    } else if constexpr (KIND == PC_KIND_KRON_OBS) {
+      const int64_t zr = tt.task[pi] / tt.T;
+      for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[zr * DP + c];
     } else {
       const int64_t zr = (KIND == PC_KIND_TASK || KIND == PC_KIND_DERIV || KIND == PC_KIND_M52GRAD) ? pi / tt.rep : pi;
       for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[zr * DP + c];
@@ -355,6 +361,15 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             s = fmaf(df, df, s);
           }
           v = os * tt.B[pc_task_of(tt, pi) * tt.T + pc_task_of(tt, (int)j)] * pc_cov_rt(tt.kind[0], -0.5f * s, CovParam{});
+        } else if constexpr (KIND == PC_KIND_KRON_OBS) {
+          const int gp_ = tt.task[pi], gj = tt.task[j];
+          const float* zj = Z + (int64_t)(gj / tt.T) * DP;
+          float s = 0.f;
+          for (int c = 0; c < DP; ++c) {
+            float df = zp[c] - zj[c];
+            s = fmaf(df, df, s);
+          }
+          v = os * tt.B[(gp_ % tt.T) * tt.T + gj % tt.T] * pc_cov_rt(tt.kind[0], -0.5f * s, CovParam{});
         } else if (KIND == PC_KIND_DERIV || KIND == PC_KIND_M52GRAD) {
           using K = DerivTable<KIND == PC_KIND_M52GRAD ? GP_MATERN52 : GP_RBF>;
           const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
@@ -500,6 +515,17 @@ __global__ void pc_init_task_kernel(const PcTerms tt, float os, float* __restric
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   const int a = pc_task_of(tt, (int)j);
+  diag[j] = os * tt.B[a * tt.T + a];
+  perm[j] = (int)j;
+  pos[j] = (int)j;
+}
+
+// Kronecker with observed rows: diag[j] = s B[a, a], a = rowmap[j] mod T (tt.task = the row map); then pc_first_pivot_kernel
+__global__ void pc_init_kron_obs_kernel(const PcTerms tt, float os, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos,
+                                        int64_t n) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int a = tt.task[j] % tt.T;
   diag[j] = os * tt.B[a * tt.T + a];
   perm[j] = (int)j;
   pos[j] = (int)j;
@@ -897,6 +923,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   }
   const bool kron = p->kron != nullptr;
   const bool tasks = p->tasks != nullptr || kron;
+  const bool kron_obs = kron && p->kron->masked;
   const bool deriv = p->deriv != nullptr;
   const float* Zsrc = p->Z2.as<float>();
   if (deriv) {   // entries of the value / gradient operator from the data plan's packed rows
@@ -911,6 +938,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     GP_CHECK(kron_refresh(p));
     const gp_plan* q = p->kron->data;
     tt.kind[0] = q->kind; tt.task = nullptr; tt.B = p->kron->Bd.as<float>(); tt.T = p->kron->T; tt.rep = p->kron->T;
+    if (p->kron->masked) tt.task = p->kron->rowmap.as<int>();   // PC_KIND_KRON_OBS
     Zsrc = q->Z2.as<float>();
     dp_total = q->DP;
     os_total = q->outputscale;
@@ -927,6 +955,10 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   if (deriv) {
     const float c = (float)deriv_with_kind(p->deriv->kind, [](auto K) { return decltype(K)::DIAG; });
     pc_init_deriv_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, c, diag, perm, pos, n);
+    pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
+    p->launches += 2;
+  } else if (kron_obs) {
+    pc_init_kron_obs_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;
   } else if (tasks) {
@@ -962,10 +994,11 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : spec ? PC_KIND_SPECTRAL : p->kind) {
+    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : kron_obs ? PC_KIND_KRON_OBS : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : spec ? PC_KIND_SPECTRAL : p->kind) {
       case PC_KIND_ADDITIVE: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_ADDITIVE>; break;
       case PC_KIND_SPECTRAL: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SPECTRAL>; break;
       case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
+      case PC_KIND_KRON_OBS: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_KRON_OBS>; break;
       case PC_KIND_DERIV: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_DERIV>; break;
       case PC_KIND_M52GRAD: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_M52GRAD>; break;
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
@@ -1164,6 +1197,11 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   } else if (p->deriv) {    // s N (1 + c sum_c 1 / l_c^2), c = 1 RBF, 5/3 Matern-5/2
     GP_CHECK(deriv_refresh(p));
     tr_k = deriv_trace(p);
+  } else if (p->kron && p->kron->masked) {   // s sum_r B[a_r, a_r] over the observed rows r, a_r = rowmap[r] mod T
+    const gp_kron_state* ks = p->kron;
+    double bt = 0.0;
+    for (int g : ks->obs_r) bt += (double)ks->B[(size_t)(g % ks->T) * ks->T + g % ks->T];
+    tr_k = (double)ks->data->outputscale * bt;
   } else if (p->kron) {     // s N sum_a B[a, a]
     const gp_kron_state* ks = p->kron;
     double bt = 0.0;

@@ -638,11 +638,17 @@ class KronPlan(_DataPlanOperator):
         super().__init__(data, num_tasks)
 
     def attach(self, data: Plan, num_tasks: int):
-        """(Re-)attach the data plan: validation and geometry only; a B of the same size stays set."""
+        """(Re-)attach the data plan: validation and geometry only; a B of the same size stays set, and so does a mask of the same
+        N1, N2 and T (set_observed)."""
         T = int(num_tasks)
+        obs = getattr(self, "_observed", None)
+        if obs is not None and (obs[2], obs[3], obs[4]) != (data.n1, data.n2, T):
+            obs = None                    # the engine drops the mask with the sizes it was given for
+        self._observed = obs
         self.data, self.num_tasks = data, T
         self.same, self.d = data.same, data.d
-        self.n1, self.n2 = data.n1 * T, data.n2 * T
+        self.n1 = data.n1 * T if obs is None or obs[0] is None else obs[0].numel()
+        self.n2 = data.n2 * T if obs is None or obs[1] is None else obs[1].numel()
         self.row_begin, self.row_count = 0, self.n1
         with torch.cuda.device(self.device):
             check(self.lib.gp_plan_set_kron(self._h, data._h, T))
@@ -650,6 +656,29 @@ class KronPlan(_DataPlanOperator):
 
     def refresh_data(self):
         return self.attach(self.data, self.num_tasks)
+
+    def set_observed(self, rows: torch.Tensor | None, cols: torch.Tensor | None):
+        """Keep the interleaved rows `rows` and columns `cols` only (strictly increasing int64 indices; None: all), so the operator
+        becomes P_r ((s K) (x) B) P_c^T (gp_plan_set_kron_observed).  rows = cols = None removes the mask.  The indices are copied
+        to the host and from there to the device once.  On a square plan the two masks are equal: cols = None takes rows."""
+        rh = None if rows is None else rows.detach().to(device="cpu", dtype=torch.int64).contiguous()
+        ch = None if cols is None else cols.detach().to(device="cpu", dtype=torch.int64).contiguous()
+        if self.same and ch is None:
+            ch = rh
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_kron_observed(self._h, _ptr(rh), 0 if rh is None else rh.numel(),
+                                                      _ptr(ch), 0 if ch is None else ch.numel()))
+        T = self.num_tasks
+        n1f, n2f = self.data.n1 * T, self.data.n2 * T
+        rh = None if rh is None or rh.numel() == n1f else rh     # a list of every row is no mask (as in the engine)
+        ch = None if ch is None or ch.numel() == n2f else ch
+        self._observed = None if rh is None and ch is None else (rh, ch, self.data.n1, self.data.n2, T)
+        self.n1 = n1f if rh is None else rh.numel()
+        self.n2 = n2f if ch is None else ch.numel()
+        self.row_count = self.n1
+        if getattr(self, "_noise_diag", None) is not None and self._noise_diag.numel() != self.n1:
+            self._noise_diag = None       # the engine dropped it with the old row count
+        return self
 
 
 class DerivPlan(_DataPlanOperator):

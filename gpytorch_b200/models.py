@@ -7,7 +7,7 @@ from . import settings
 from .distributions import MultitaskMultivariateNormal, MultivariateNormal
 from .likelihoods import _GaussianLikelihoodBase
 from .module import Module
-from .operators import LOWRANK_MAX_RANK, LowRankUpdatedKernelLinearOperator, SKIKernelLinearOperator
+from .operators import LOWRANK_MAX_RANK, LowRankUpdatedKernelLinearOperator, MaskedLinearOperator, SKIKernelLinearOperator
 
 # Largest grid LOVE cache C = s K_uu W^T R (M x J fp32) the grid path builds; above it the covariance takes the joint path.  At
 # the 100^3 grid of a 10^6-point KISS-GP model and J = 100 the cache is 400 MB; a 128^4 grid would need 100 GB.
@@ -76,6 +76,7 @@ class ExactGP(Module):
 
     def _clear_caches(self):
         self._mean_cache = self._covar_cache = None
+        self._cache_observed = None   # the observed-row mask the two caches were built for (None: every row)
         self._grid_mean_cache = self._grid_covar_cache = None   # c = s K_uu W^T alpha [M], C = s K_uu W^T R [M, J]
 
     def train(self, mode=True):
@@ -132,27 +133,46 @@ class ExactGP(Module):
         # a Kronecker multitask model (MultitaskMultivariateNormal): every covariance block is over the interleaved rows i T + a,
         # so the joint operator is sliced at n T and the means are [n, T] (flattened row-major for the solves)
         multitask = isinstance(train_out, MultitaskMultivariateNormal)
+        # settings.observation_nan_policy "mask" / "fill" (the same posterior here): condition on the observed rows only
+        # (exact_prediction_strategies.py:278-321, :393-410); the rows of a multitask model are the interleaved i T + a
+        observed = None
+        if settings.observation_nan_policy.value() != "ignore":
+            event = self.train_targets.shape[-2:] if multitask else self.train_targets.shape[-1:]
+            obs = settings.observation_nan_policy._get_observed(self.train_targets, event).reshape(-1)
+            observed = None if bool(obs.all()) else obs
+        if (observed is None) != (self._cache_observed is None) or (observed is not None and not torch.equal(observed, self._cache_observed)):
+            self._clear_caches()
+            self._cache_observed = observed
         with settings._use_eval_tolerance(True):
             khat = self.likelihood(train_out, *lik_params).lazy_covariance_matrix
             if multitask:
                 T = train_out.num_tasks
                 n_rows = n * T
-                if self._mean_cache is None:
-                    resid = (self.train_targets - train_out.mean).reshape(-1, 1)
-                    self._mean_cache = khat.solve(resid).squeeze(-1)
+                resid = (self.train_targets - train_out.mean).reshape(-1, 1)
                 k_star = full_covar[n_rows:, :n_rows]
                 k_ss = full_covar[n_rows:, n_rows:]
-                test_mean = (full_mean[n:].reshape(-1) + k_star.matmul(self._mean_cache)).reshape(-1, T)
                 m = test_x.size(-2) * T
             else:
                 n_rows = n
-                if self._mean_cache is None:
-                    resid = (self.train_targets - train_out.mean).unsqueeze(-1)
-                    self._mean_cache = khat.solve(resid).squeeze(-1)  # exact_prediction_strategies.py:286
+                resid = (self.train_targets - train_out.mean).unsqueeze(-1)
                 k_star = full_covar[n:, :n]                           # K(test, train)
                 k_ss = full_covar[n:, n:]
-                test_mean = full_mean[..., n:] + k_star.matmul(self._mean_cache)  # :396
                 m = test_x.size(-2)
+            if observed is not None:   # K_hat over the observed rows, the observed columns of K(test, train)
+                khat = MaskedLinearOperator(khat, observed, observed)
+                k_star = MaskedLinearOperator(k_star, None, observed)
+            if self._mean_cache is None:
+                if observed is None:
+                    self._mean_cache = khat.solve(resid).squeeze(-1)  # exact_prediction_strategies.py:286
+                else:                                                 # NaN on the missing rows, as :298-307
+                    cache = torch.full((n_rows,), float("nan"), device=resid.device, dtype=resid.dtype)
+                    cache[observed] = khat.solve(resid[observed]).squeeze(-1)
+                    self._mean_cache = cache
+            cache = self._mean_cache if observed is None else self._mean_cache[observed]
+            if multitask:
+                test_mean = (full_mean[n:].reshape(-1) + k_star.matmul(cache)).reshape(-1, T)
+            else:
+                test_mean = full_mean[..., n:] + k_star.matmul(cache)  # :396
             mode = _posterior_covar_mode(k_ss)
             if mode == "skip":                               # exact_prediction_strategies.py:432-433
                 covar = torch.zeros(m, m, device=test_x.device)
@@ -164,6 +184,8 @@ class ExactGP(Module):
                     covar = _dense(k_ss) - root @ root.transpose(-1, -2)
             else:
                 rhs = _dense(full_covar[:n_rows, n_rows:])   # K(train, test) [n, m]
+                if observed is not None:
+                    rhs = rhs[observed]
                 corr = k_star.matmul(khat.solve(rhs))        # exact predictive covariance, :435-462
                 covar = _dense(k_ss) - corr
         if multitask:

@@ -633,7 +633,7 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
     hyper-parameters are lengthscale, outputscale and B; B's gradient comes from gp_task_covar_grad and autograd carries it to the
     IndexKernel's covar_factor / raw_var.  Input gradients are not available: inputs that require grad are refused."""
 
-    def __init__(self, x1, x2, kind, lengthscale, outputscale, B):
+    def __init__(self, x1, x2, kind, lengthscale, outputscale, B, rows=None, cols=None):
         if x1.requires_grad or (x2 is not None and x2.requires_grad):
             raise RuntimeError("gradients with respect to the inputs of a Kronecker multitask operator (K (x) B) are not implemented: "
                                "pass inputs that do not require grad")
@@ -644,11 +644,35 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
         self.num_tasks = int(B.shape[-1])
         self._data_op = KernelLinearOperator(x1, x2, kind, lengthscale, outputscale)
         self._data_op._plan_slot = _KRON_SLOT
+        # observed interleaved rows / columns (int64 index tensors, strictly increasing; None: all): the operator is
+        # P_r ((s K) (x) B) P_c^T (masked())
+        if self.same and cols is not None and cols is not rows and (rows is None or not torch.equal(rows, cols)):
+            raise RuntimeError("a square Kronecker operator takes equal row and column masks")
+        self.rows, self.cols = rows, (rows if self.same else cols)
+        self._obs_host = None
+
+    def masked(self, rows, cols):
+        """P_r ((s K) (x) B) P_c^T: the interleaved rows `rows` and columns `cols` (int64 indices, strictly increasing; None: all)
+        as one engine operator on the same data plan (gp_plan_set_kron_observed).  On a square operator the two must be equal."""
+        if self.rows is not None or self.cols is not None:
+            raise NotImplementedError("a masked Kronecker operator cannot be masked again")
+        if self.same and rows is not None and cols is not None and rows is not cols and not torch.equal(rows, cols):
+            raise NotImplementedError("a square Kronecker operator takes equal row and column masks")
+        return KroneckerKernelLinearOperator(self.x1, None if self.same else self.x2, self.kind, self.lengthscale, self.outputscale,
+                                             self.B, rows, cols)
 
     @property
     def shape(self):
         n2 = self.x1.size(0) if self.same else self.x2.size(0)
-        return torch.Size([self.x1.size(0) * self.num_tasks, n2 * self.num_tasks])
+        T = self.num_tasks
+        return torch.Size([self.x1.size(0) * T if self.rows is None else self.rows.numel(),
+                           n2 * T if self.cols is None else self.cols.numel()])
+
+    def _observed_host(self):
+        """(rows, cols) on the host, read once per operator."""
+        if self._obs_host is None:
+            self._obs_host = tuple(None if v is None else v.detach().to(device="cpu", dtype=torch.int64) for v in (self.rows, self.cols))
+        return self._obs_host
 
     def plan(self, noise=0.0) -> Plan:
         data = self._data_op.plan(0.0)
@@ -656,18 +680,29 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
             data.set_noise_diag(None)
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
         T = self.num_tasks
+        masked = self.rows is not None or self.cols is not None
         with _PLAN_LOCK:
-            key = (id(data), T)
+            # a parent that holds a mask never serves an unmasked operator, nor the other way round; masked parents are
+            # re-masked below only when the indices change
+            key = (id(data), T, masked)
             parent = _KRON_PLANS.pop(key, None)
             if parent is None:
                 parent = KronPlan(data, T)
                 parent._hyp_key = None
                 parent._b_key = None
+                parent._obs_key = None
             _KRON_PLANS[key] = parent
             while len(_KRON_PLANS) > 16:
                 _KRON_PLANS.pop(next(iter(_KRON_PLANS))).close()
         # the data plan may have been re-packed or re-pointed since the last use: re-attach it (validation, no allocation)
         parent.attach(data, T)
+        if masked:
+            rh, ch = self._observed_host()
+            ok = parent._observed is not None and parent._obs_key is not None and all(
+                (a is None and b is None) or (a is not None and b is not None and torch.equal(a, b)) for a, b in zip(parent._obs_key, (rh, ch)))
+            if not ok:
+                parent.set_observed(rh, ch)
+                parent._obs_key = (rh, ch)
         hk = (nz, data.kind, tuple(data.lengthscale), data.outputscale)
         if parent._hyp_key != hk:
             parent.set_noise(nz)
@@ -712,11 +747,12 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
     def _transpose_nonbatch(self):
         if self.same:
             return self
-        return KroneckerKernelLinearOperator(self.x2, self.x1, self.kind, self.lengthscale, self.outputscale, self.B.transpose(-1, -2))
+        return KroneckerKernelLinearOperator(self.x2, self.x1, self.kind, self.lengthscale, self.outputscale, self.B.transpose(-1, -2),
+                                             self.cols, self.rows)
 
     def detach(self):
         return KroneckerKernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.kind,
-                                             self.lengthscale.detach(), self.outputscale.detach(), self.B.detach())
+                                             self.lengthscale.detach(), self.outputscale.detach(), self.B.detach(), self.rows, self.cols)
 
     def to_dense(self):
         return _KernelDense.apply(self)
@@ -736,6 +772,8 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
         ri, ci = index
         if isinstance(ri, int):
             return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        if self.rows is not None or self.cols is not None:
+            raise NotImplementedError("a masked Kronecker operator takes no slices: mask the sliced operator instead")
         T = self.num_tasks
         x2 = self.x1 if self.same else self.x2
         rs, cs = _aligned(ri, T, self.x1.size(0)), _aligned(ci, T, x2.size(0))
@@ -756,6 +794,76 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
 
 
 _KRON_PLANS: "dict[tuple, Plan]" = {}
+
+
+def _mask_index(mask, n, what):
+    """Strictly increasing int64 indices of a boolean mask [n] (None: every index)."""
+    if mask is None:
+        return None
+    mask = torch.as_tensor(mask)
+    if mask.dtype != torch.bool or mask.dim() != 1 or mask.numel() != n:
+        raise RuntimeError(f"the {what} mask must be a boolean vector of {n} entries (got {mask.dtype}, {tuple(mask.shape)})")
+    return mask.nonzero().reshape(-1)
+
+
+def _take_square(op, idx, memo):
+    """op[idx, idx] of a square operator with every input indexed ONCE, so that the result is square again (x2 is x1): two
+    fancy indexes of x1 would give two tensors and a cross plan.  The terms of a sum or product and the components of an additive
+    operator share their indexed inputs through memo."""
+    def take(x):
+        if id(x) not in memo:
+            memo[id(x)] = (x, x[idx])    # x is kept so that its id stays unique while memo lives
+        return memo[id(x)][1]
+
+    if getattr(op, "_comm", None) is not None or getattr(op, "_row_begin", 0) != 0:
+        raise NotImplementedError(f"an observation mask on a row-sharded {type(op).__name__} is not available")
+    t = type(op)
+    if t is KernelLinearOperator:
+        return KernelLinearOperator(take(op.x1), None, op.kind, op.lengthscale, op.outputscale)
+    if t is HadamardKernelLinearOperator:
+        return HadamardKernelLinearOperator(take(op.x1), None, op.kind, op.lengthscale, op.outputscale, take(op.t1), None, op.B)
+    if t is SumKernelLinearOperator:
+        return SumKernelLinearOperator([_take_square(o, idx, memo) for o in op.ops])
+    if t is ProductKernelLinearOperator:
+        return ProductKernelLinearOperator([_take_square(o, idx, memo) for o in op.ops])
+    if t is AdditiveKernelLinearOperator:
+        return AdditiveKernelLinearOperator([_take_square(o, idx, memo) for o in op.ops], op.max_degree)
+    if t in (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator, SpectralMixtureKernelLinearOperator):
+        return op._with(take(op.x1), None)
+    raise NotImplementedError(f"observation masks are not available for {t.__name__}")
+
+
+def MaskedLinearOperator(base, row_mask, col_mask):
+    """base restricted to the rows where row_mask and the columns where col_mask is True (linear_operator's MaskedLinearOperator,
+    used by settings.observation_nan_policy("mask")), as an engine operator:
+      * AddedDiagLinearOperator: the kernel and the diagonal are masked separately;
+      * KroneckerKernelLinearOperator: the same operator on a plan with the mask set (gp_plan_set_kron_observed);
+      * plain, sum, product, additive, periodic, RQ, polynomial, spectral and Hadamard operators: their inputs (and task ids)
+        re-indexed; a square operator with equal masks stays square (its inputs are indexed once);
+      * derivative, SKI and batched operators: NotImplementedError.
+    row_mask / col_mask are boolean vectors over the rows / columns (None: all)."""
+    n1, n2 = int(base.shape[-2]), int(base.shape[-1])
+    ri, ci = _mask_index(row_mask, n1, "row"), _mask_index(col_mask, n2, "column")
+    if isinstance(base, AddedDiagLinearOperator):
+        if not ((ri is None and ci is None) or (ri is not None and ci is not None and torch.equal(ri, ci))):
+            raise NotImplementedError("a masked K + D takes equal row and column masks")
+        if ri is None:
+            return base
+        if base.per_row:
+            diag = DiagLinearOperator(base.diag.diag_vec[..., ri])
+        else:
+            diag = ConstantDiagLinearOperator(base.diag.diag_value, ri.numel())
+        return AddedDiagLinearOperator(MaskedLinearOperator(base.kernel_op, row_mask, col_mask), diag)
+    if isinstance(base, KroneckerKernelLinearOperator):
+        equal = (ri is None and ci is None) or (ri is not None and ci is not None and torch.equal(ri, ci))
+        if base.same and not equal:
+            raise NotImplementedError("a square Kronecker operator takes equal row and column masks")
+        return base.masked(ri, None if base.same else ci)
+    if not isinstance(base, KernelLinearOperator) or isinstance(base, (DerivKernelLinearOperator, SKIKernelLinearOperator)):
+        raise NotImplementedError(f"observation masks are not available for {type(base).__name__}")
+    if base.same and ri is not None and ci is not None and torch.equal(ri, ci):
+        return _take_square(base, ri, {})
+    return base[slice(None) if ri is None else ri, slice(None) if ci is None else ci]
 
 _DERIV_SLOT = 28   # plan-cache slot of the data plans of derivative operators
 
@@ -2753,3 +2861,4 @@ class _InvQuadLogdet(torch.autograd.Function):
         elif any(need_x) and left_cols:
             xgrads = op.kernel_op._input_grad_list(left, right, need_x)
         return (None, grad_rhs, None, gn, *grads, *xgrads)
+

@@ -135,6 +135,41 @@ class minres_tolerance(_value_context):
     _global_value = 1e-4
 
 
+class observation_nan_policy(_value_context):
+    """NaN handling policy for observations (settings.py:407-450).
+
+    * ``ignore``: do not check for NaN values (the default).
+    * ``mask``: mask out NaN values during calculation: ExactMarginalLogLikelihood and the exact prediction strategy use the
+      observed entries of the mean, the target and the covariance rows and columns (an entry that is NaN in one batch element is
+      masked for the whole batch).  A Kronecker multitask model keeps one engine operator, P ((s K) (x) B + D) P^T over the
+      observed interleaved rows.  With no NaN in the targets every call returns what ``ignore`` returns.
+    * ``fill``: fill in NaN values with a dummy value for prediction; refused by ExactMarginalLogLikelihood.  Prediction gives
+      the mean ``mask`` gives (the two are the same posterior; the engine never builds the dense masked kernel).
+
+    Deviation: the reference's predictive covariance and LOVE cache solve with the full training covariance even under ``mask``;
+    here both condition on the observed rows only, which is the posterior of the masked model."""
+
+    _fill_value = -999.0
+    _global_value = "ignore"
+
+    def __init__(self, value):
+        if value not in {"ignore", "mask", "fill"}:
+            raise ValueError(f"NaN handling policy {value} not supported!")
+        super().__init__(value)
+
+    @staticmethod
+    def _get_observed(observations, event_shape):
+        """The mask over event_shape of the entries that are not NaN in any batch element (settings.py:428-440)."""
+        import torch
+        return ~torch.any(torch.isnan(observations.reshape(-1, *event_shape)), dim=0)
+
+    @classmethod
+    def _fill_tensor(cls, observations):
+        """observations with every NaN replaced by _fill_value (settings.py:442-450)."""
+        import torch
+        return torch.nan_to_num(observations, nan=cls._fill_value)
+
+
 class skip_logdet_forward(_feature_flag):
     _default = False
 

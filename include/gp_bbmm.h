@@ -331,6 +331,18 @@ int gp_task_covar_grad(gp_plan* plan, const float* L, int64_t ldl, const float* 
  * GP_E_SHAPE: a SKI, kernel-sum or row-sharded data plan, and gp_plan_set_comm with more than one rank on `plan`. */
 int gp_plan_set_kron(gp_plan* plan, gp_plan* data, int T);
 
+/* Missing observations on a Kronecker plan (settings.observation_nan_policy("mask") of the Python package): `plan` becomes the
+ * n_rows x n_cols operator  P_r ((s K_data) (x) B) P_c^T  that keeps the interleaved rows `rows` and columns `cols` (host arrays,
+ * strictly increasing, inside [0, N1 T) and [0, N2 T); copied to the device once).  NULL keeps every row or column; rows = cols =
+ * NULL, or lists that name every row, remove the mask.  On a square plan the two masks must be equal (GP_E_SHAPE otherwise).  The
+ * mask is part of the Kronecker setting: it survives gp_plan_set_kron with the same N1, N2 and T, as B does, and is dropped
+ * otherwise.  gp_plan_set_noise_diag then takes n_rows entries (a diagonal set before is dropped when the row count changes).
+ * Every call that runs on a Kronecker plan runs on the masked operator: K.V mixes the observed columns (zero elsewhere) through
+ * the same launches of data's fused kernel and scatters the observed rows; gp_krows takes observed row indices and returns the
+ * observed columns; gp_kdiag, gp_pivoted_cholesky (first pivot = argmax of the diagonal s B[a, a]), gp_bilinear_grad and
+ * gp_task_covar_grad (L and R of n_rows and n_cols rows) are those of the masked operator.  GP_E_STATE: not a Kronecker plan. */
+int gp_plan_set_kron_observed(gp_plan* plan, const int64_t* rows, int64_t n_rows, const int64_t* cols, int64_t n_cols);
+
 /* GPs with derivative observations (RBFKernelGrad, kernels/rbf_kernel_grad.py:60-115, with the perfect shuffle of :99-102, as in
  * examples/08_Advanced_Usage/Simple_GP_Regression_Derivative_Information_{1d,2d}.ipynb): `plan` becomes the N1 (d+1) x N2 (d+1)
  * operator over interleaved rows i (d+1) + a (a = 0: f(x_i); a = 1..d: df/dx_a at x_i) with, for D = x_i - x'_j,
