@@ -86,6 +86,9 @@ PROTOTYPES = {
     "gp_task_covar_grad": (_I, [_P, _P, _L, _P, _L, _I, C.POINTER(C.c_double)]),
     "gp_plan_set_kron": (_I, [_P, _P, _I]),
     "gp_plan_set_kron_observed": (_I, [_P, _P, _L, _P, _L]),
+    "gp_plan_set_kron_terms": (_I, [_P, C.POINTER(_P), _I, _I]),
+    "gp_plan_set_kron_term_covars": (_I, [_P, C.POINTER(_F), _I, _I]),
+    "gp_kron_terms_grad": (_I, [_P, _P, _L, _P, _L, _I, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "gp_plan_set_deriv": (_I, [_P, _P]),
     "gp_plan_set_deriv_kind": (_I, [_P, _P, _I]),
     "gp_ski_grid_matmul": (_I, [_P, _P, _L, _I, _P, _L]),

@@ -173,6 +173,8 @@ struct gp_task_state {
   int* d_slot0 = nullptr;
 };
 
+constexpr int KRON_MAX_TERMS = 4;   // latent processes of one Kronecker plan (gp_plan_set_kron_terms)
+
 // Kronecker multitask state (kron.cu): the operator is (s K_data) (x) B over interleaved rows i T + a.  One K.V mixes the block by
 // B into ceil(T t / 16) zero-padded [N2, 16] column chunks, runs the data plan's fused kernel once per chunk into its own partial
 // slots, and scatters the chunks back to rows i T + a of partial slot 0.
@@ -193,6 +195,10 @@ struct gp_kron_state {
   gp::DevBuf rowmap, colmap, rowpos, colpos;
   gp::DevBuf Lx, Rx, full, gidx;           // gradient operands expanded to N T rows | full rows / diagonal before the gather |
                                            // the interleaved row of each requested row
+  // several latent processes (gp_plan_set_kron_terms, LCM): sum_q (s_q K_q) (x) B_q with Q = nterm terms; data == term[0], B and Bd
+  // hold the Q blocks back to back (gp_plan_set_kron_term_covars).  nterm = 1 is the single-term operator above
+  int nterm = 1;
+  gp_plan* term[KRON_MAX_TERMS] = {};
 };
 
 // Derivative-observation state (deriv.cu, deriv_table.cuh): the RBF or Matern-5/2 value / gradient operator over interleaved rows

@@ -13,10 +13,15 @@
 // Gradients.  sum L . ((d(sK) (x) B) R) is the data plan's bilinear derivative with L viewed as [N1, T t] and R mixed by B, run
 // chunk by chunk.  dB[a][b] = s sum_i L[i T + a] . (K R_b)[i] with R_b[j] = R[j T + b] is the data kernel over the unmixed chunks,
 // reduced in fp64 in a fixed tree.  Nothing here uses atomics: repeated calls on one plan give identical bits.
+//
+// Several terms (gp_plan_set_kron_terms; LCMKernel, kernels/lcm_kernel.py): sum_q (s_q K_q) (x) B_q.  Each term runs the pipeline
+// above up to its own partial slots (its B_q mix, its data plan's launches); lcm_scatter_kernel sums s_q times each term's slots in
+// term order.  Rows, the diagonal and the gradients run the single-term passes per term with that term's B_q.
 #include <math.h>
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 
 #include "gp_common.cuh"
 
@@ -145,6 +150,69 @@ __global__ void kron_expand_diag_kernel(const float* __restrict__ d, int64_t n1,
   OUT[e] = d[e / T] * B[a * T + a];
 }
 
+// ---- several terms (gp_plan_set_kron_terms): sum_q (s_q K_q) (x) B_q ----
+struct LcmTerms {
+  const float* part[KRON_MAX_TERMS];   // each term's partial slots [nchunk][nsplit][rows_pad][16]
+  int nsplit[KRON_MAX_TERMS];
+  int64_t rows_pad[KRON_MAX_TERMS];
+  float s[KRON_MAX_TERMS];             // the term data plan's outputscale
+  const int* xbad[KRON_MAX_TERMS];
+  int Q;
+};
+
+// out[(i T + a)][c] = sum_q s_q sum_sp part_q[q'][sp][i][cc] for col = a t + c = 16 q' + cc (c < t), 0 for c >= t; terms outer,
+// splits inner.  NaN when any term has non-finite inputs, or a B_q a non-finite entry (bbad)
+__global__ void lcm_scatter_kernel(const LcmTerms lt, int64_t n1, int T, int t, float* __restrict__ out, int bbad,
+                                   const int* __restrict__ done_flag) {
+  if (done_flag && *done_flag) return;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n1 * T * TP) return;
+  const int c = (int)(idx % TP);
+  const int64_t r = idx / TP;
+  const int64_t i = r / T;
+  const int a = (int)(r % T);
+  float s = 0.f;
+  bool bad = bbad != 0;
+  for (int q = 0; q < lt.Q; ++q) {
+    bad = bad || *lt.xbad[q];
+    if (c < t) {
+      const int col = a * t + c;
+      const int64_t rp = lt.rows_pad[q];
+      const float* base = lt.part[q] + ((int64_t)(col / TP) * lt.nsplit[q] * rp + i) * TP + col % TP;
+      float v = 0.f;
+      for (int sp = 0; sp < lt.nsplit[q]; ++sp) v += base[(int64_t)sp * rp * TP];
+      s = fmaf(lt.s[q], v, s);
+    }
+  }
+  if (bad) s = __int_as_float(0x7fc00000);
+  out[idx] = s;
+}
+
+// OUT[r][j T + b] = sum_q rows[q][r][j] B_q[a][b], a = idx[r] mod T: row i T + a of sum_q (s_q K_q) (x) B_q from row i of every s_q K_q
+__global__ void lcm_expand_rows_kernel(const float* __restrict__ rows, int Q, int64_t m, int64_t n2, const int64_t* __restrict__ idx,
+                                       int64_t n, const float* __restrict__ B, int T, float* __restrict__ OUT, int64_t ldo) {
+  const int64_t r = blockIdx.y;
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n2 * T) return;
+  const int64_t v = idx[r];
+  const int a = (v >= 0 && v < n) ? (int)(v % T) : 0;
+  const int b = (int)(e % T);
+  float s = 0.f;
+  for (int q = 0; q < Q; ++q) s = fmaf(rows[((int64_t)q * m + r) * n2 + e / T], B[((int64_t)q * T + a) * T + b], s);
+  OUT[r * ldo + e] = s;
+}
+
+// OUT[i T + a] = sum_q d[q][i] B_q[a][a]
+__global__ void lcm_expand_diag_kernel(const float* __restrict__ d, int Q, int64_t n1, const float* __restrict__ B, int T,
+                                       float* __restrict__ OUT) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n1 * T) return;
+  const int a = (int)(e % T);
+  float s = 0.f;
+  for (int q = 0; q < Q; ++q) s = fmaf(d[(int64_t)q * n1 + e / T], B[((int64_t)q * T + a) * T + a], s);
+  OUT[e] = s;
+}
+
 // masked plans: OUT[r][e] = SRC[r][map[e]] (observed columns of full rows, or observed entries of the full diagonal with m = 1)
 __global__ void masked_kron_gather_kernel(const float* __restrict__ SRC, int64_t lds, const int* __restrict__ map, int64_t ncols,
                                    float* __restrict__ OUT, int64_t ldo) {
@@ -173,7 +241,7 @@ __global__ void masked_kron_expand_kernel(const float* __restrict__ SRC, int64_t
   OUT[e] = r >= 0 ? SRC[(int64_t)r * ld + (int)(e % s)] : 0.f;
 }
 
-static int kron_check_data(const gp_plan* p, const gp_plan* q) {
+static int kron_check_data(const gp_plan* p, const gp_plan* q, int T) {
   GP_REQUIRE(q->data_set && q->hypers_set, GP_E_STATE, "Kronecker plan: the data plan needs set_data + set_hypers");
   GP_REQUIRE(q->backend == GP_BACKEND_TCGEN05 || q->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
              "Kronecker plan: the data plan must be a plain kernel plan (not SKI, not a kernel sum, not Kronecker)");
@@ -181,7 +249,7 @@ static int kron_check_data(const gp_plan* p, const gp_plan* q) {
   GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
              "Kronecker plan: a row-sharded data plan is not available");
   GP_REQUIRE(q->device == p->device && q->stream == p->stream, GP_E_STATE, "Kronecker plan: the data plan must live on the same device and stream");
-  GP_REQUIRE(q->n1 * p->kron->T < ((int64_t)1 << 31) && q->n2 * p->kron->T < ((int64_t)1 << 31), GP_E_SHAPE,
+  GP_REQUIRE(q->n1 * T < ((int64_t)1 << 31) && q->n2 * T < ((int64_t)1 << 31), GP_E_SHAPE,
              "Kronecker plan: N T must stay below 2^31");
   return GP_OK;
 }
@@ -209,18 +277,25 @@ static void kron_geometry(gp_plan* p) {
 int kron_refresh(gp_plan* p) {
   gp_kron_state* ks = p->kron;
   const gp_plan* q = ks->data;
-  GP_CHECK(kron_check_data(p, q));
+  GP_CHECK(kron_check_data(p, q, ks->T));
   const int64_t n1 = ks->masked ? (int64_t)ks->obs_r.size() : q->n1 * ks->T, n2 = ks->masked ? (int64_t)ks->obs_c.size() : q->n2 * ks->T;
   GP_REQUIRE(p->n1 == n1 && p->n2 == n2 && p->same == q->same && (!ks->masked || (q->n1 == ks->mask_n1 && q->n2 == ks->mask_n2)), GP_E_STATE,
              "Kronecker plan: the data plan changed its size; call gp_plan_set_kron again");
   p->kind = q->kind;
   p->outputscale = q->outputscale;   // the finish kernels scale the unscaled product by the data plan's s
   p->xbad = q->xbad;
+  for (int t = 1; t < ks->nterm; ++t) {
+    const gp_plan* qt = ks->term[t];
+    GP_CHECK(kron_check_data(p, qt, ks->T));
+    GP_REQUIRE(qt->n1 == q->n1 && qt->n2 == q->n2 && qt->same == q->same, GP_E_STATE,
+               "Kronecker plan: a term's data plan changed its size; call gp_plan_set_kron_terms again");
+  }
+  if (ks->nterm > 1) p->outputscale = 1.f;   // every term's s_q is applied in the scatter (lcm_scatter_kernel)
   return GP_OK;
 }
 
 int kron_pack(gp_plan* p) {
-  GP_CHECK(kron_check_data(p, p->kron->data));
+  GP_CHECK(kron_check_data(p, p->kron->data, p->kron->T));
   kron_geometry(p);
   GP_CHECK(kron_refresh(p));
   GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)nslots(p) * p->rows_pad * TP));
@@ -230,19 +305,24 @@ int kron_pack(gp_plan* p) {
 // W-chunk pitch of the data plan: whole 64-row tiles on the tensor-core path (one pack call covers every chunk)
 static int64_t kron_npad(const gp_plan* q) { return q->backend == GP_BACKEND_TCGEN05 ? q->ntile_j * TILE_J : q->n2; }
 
-// V16 [N2 T][16] with t live columns, mixed by B (or not: B == nullptr) -> nchunk data-kernel products in ks->part
-// MASKED: V16 holds the observed columns only (ks->colpos places them)
+// floats of the partial slots of data plan q's products over nchunk column chunks
+static size_t kron_part_floats(const gp_plan* q, int nchunk) { return (size_t)nchunk * q->nsplit * q->rows_pad * TP; }
+
+// V16 [N2 T][16] with t live columns, mixed by B (or not: B == nullptr) -> nchunk products of data plan q in ks->part from float
+// part_off on (a Kronecker plan with several terms puts the terms' products back to back; ks->W and ks->Vt are re-used term after
+// term in stream order).  MASKED: V16 holds the observed columns only (ks->colpos places them)
 template <bool MASKED>
-static int kron_chunks(gp_plan* p, const float* V16, int t, const float* B, int kind, const int* done_flag, int* nchunk_out) {
+static int kron_chunks(gp_plan* p, gp_plan* q, const float* V16, int t, const float* B, const int* done_flag, size_t part_off,
+                       int* nchunk_out) {
   gp_kron_state* ks = p->kron;
-  gp_plan* q = ks->data;
+  const int kind = q->kind;
   const bool tc = q->backend == GP_BACKEND_TCGEN05;
   const int T = ks->T;
   const int nchunk = (int)cdiv((int64_t)T * t, TP);
   const int64_t npad = kron_npad(q);
   const size_t slot_floats = (size_t)q->rows_pad * TP;
   GP_CHECK(ks->W.ensure(sizeof(float) * (size_t)nchunk * npad * TP));
-  GP_CHECK(ks->part.ensure(sizeof(float) * (size_t)nchunk * q->nsplit * slot_floats));
+  GP_CHECK(ks->part.ensure(sizeof(float) * (part_off + kron_part_floats(q, nchunk))));
   const int64_t tot = (int64_t)nchunk * npad * TP;
   kron_mix_kernel<MASKED><<<(unsigned)cdiv(tot, 256), 256, 0, p->stream>>>(V16, q->n2, npad, T, t, nchunk, B, ks->W.as<float>(), done_flag,
                                                                             ks->colpos.as<int>());
@@ -253,7 +333,7 @@ static int kron_chunks(gp_plan* p, const float* V16, int t, const float* B, int 
     GP_CHECK(pack_v_tiles_rows(p, ks->W.as<float>(), (int64_t)nchunk * npad, (int64_t)nchunk * q->ntile_j, ks->Vt.as<float>()));
   }
   for (int c = 0; c < nchunk; ++c) {
-    float* part = ks->part.as<float>() + (size_t)c * q->nsplit * slot_floats;
+    float* part = ks->part.as<float>() + part_off + (size_t)c * q->nsplit * slot_floats;
     if (tc) {
       GP_CHECK(kmv_tc_launch_cols(q, kind, q->XA.as<float>(), q->XB.as<float>(), ks->Vt.as<float>() + (size_t)c * q->ntile_j * V_TILE_FLOATS,
                                   part, q->ntile_j, q->tiles_per_split, q->nsplit, q->row_begin, done_flag));
@@ -268,20 +348,57 @@ static int kron_chunks(gp_plan* p, const float* V16, int t, const float* B, int 
   return GP_OK;
 }
 
+// several terms: every term's mixed chunks through its own data kernel, then one scatter of sum_q s_q (its slots) into slot 0
+static int lcm_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
+  gp_kron_state* ks = p->kron;
+  const int T = ks->T, t = p->kron_cols, Q = ks->nterm;
+  const int nchunk = (int)cdiv((int64_t)T * t, TP);
+  size_t off[KRON_MAX_TERMS], tot = 0, wmax = 0, vtmax = 0;
+  for (int k = 0; k < Q; ++k) {   // one allocation of each buffer up front: no term's ensure frees a buffer in use
+    const gp_plan* q = ks->term[k];
+    off[k] = tot;
+    tot += kron_part_floats(q, nchunk);
+    wmax = std::max(wmax, (size_t)nchunk * kron_npad(q) * TP);
+    if (q->backend == GP_BACKEND_TCGEN05) vtmax = std::max(vtmax, (size_t)nchunk * q->ntile_j * V_TILE_FLOATS);
+  }
+  GP_CHECK(ks->part.ensure(sizeof(float) * tot));
+  GP_CHECK(ks->W.ensure(sizeof(float) * wmax));
+  if (vtmax) GP_CHECK(ks->Vt.ensure(sizeof(float) * vtmax));
+  LcmTerms lt;
+  memset(&lt, 0, sizeof(lt));
+  lt.Q = Q;
+  for (int k = 0; k < Q; ++k) {
+    gp_plan* q = ks->term[k];
+    int nc = 0;
+    GP_CHECK(kron_chunks<false>(p, q, V16, t, ks->Bd.as<float>() + (size_t)k * T * T, done_flag, off[k], &nc));
+    lt.part[k] = ks->part.as<float>() + off[k];
+    lt.nsplit[k] = q->nsplit;
+    lt.rows_pad[k] = q->rows_pad;
+    lt.s[k] = q->outputscale;
+    lt.xbad[k] = q->xbad;
+  }
+  lcm_scatter_kernel<<<(unsigned)cdiv(p->n1 * TP, 256), 256, 0, p->stream>>>(lt, ks->data->n1, T, t, p->partial.as<float>(),
+                                                                             ks->b_bad ? 1 : 0, done_flag);
+  p->launches++;
+  GP_CUDA(cudaGetLastError());
+  return GP_OK;
+}
+
 int kron_kmv_partials(gp_plan* p, const float* V16, const int* done_flag) {
   gp_kron_state* ks = p->kron;
   GP_REQUIRE(ks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
   GP_CHECK(kron_refresh(p));
-  const gp_plan* q = ks->data;
+  if (ks->nterm > 1) return lcm_kmv_partials(p, V16, done_flag);
+  gp_plan* q = ks->data;
   const int t = p->kron_cols;
   int nchunk = 0;
   const unsigned grid = (unsigned)cdiv(p->n1 * TP, 256);
   if (ks->masked) {
-    GP_CHECK(kron_chunks<true>(p, V16, t, ks->Bd.as<float>(), q->kind, done_flag, &nchunk));
+    GP_CHECK(kron_chunks<true>(p, q, V16, t, ks->Bd.as<float>(), done_flag, 0, &nchunk));
     kron_scatter_kernel<true><<<grid, 256, 0, p->stream>>>(ks->part.as<float>(), q->nsplit, q->rows_pad, q->n1, ks->T, t, p->partial.as<float>(),
                                                            q->xbad, ks->b_bad ? 1 : 0, done_flag, ks->rowmap.as<int>(), p->n1);
   } else {
-    GP_CHECK(kron_chunks<false>(p, V16, t, ks->Bd.as<float>(), q->kind, done_flag, &nchunk));
+    GP_CHECK(kron_chunks<false>(p, q, V16, t, ks->Bd.as<float>(), done_flag, 0, &nchunk));
     kron_scatter_kernel<false><<<grid, 256, 0, p->stream>>>(ks->part.as<float>(), q->nsplit, q->rows_pad, q->n1, ks->T, t, p->partial.as<float>(),
                                                             q->xbad, ks->b_bad ? 1 : 0, done_flag, nullptr, 0);
   }
@@ -298,6 +415,19 @@ int kron_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ld
   gp_plan* q = ks->data;
   const int64_t n1f = q->n1 * ks->T, n2f = q->n2 * ks->T;
   GP_CHECK(ks->idx.ensure(sizeof(int64_t) * m));
+  if (ks->nterm > 1) {   // every term's rows of s_q K_q back to back, then one expand-and-accumulate pass
+    const int Q = ks->nterm;
+    GP_CHECK(ks->rows.ensure(sizeof(float) * (size_t)Q * m * q->n2));
+    kron_point_idx_kernel<<<(unsigned)cdiv(m, 256), 256, 0, p->stream>>>(idx, m, ks->T, n1f, ks->idx.as<int64_t>());
+    p->launches++;
+    for (int k = 0; k < Q; ++k)
+      GP_CHECK(gp_krows(ks->term[k], ks->idx.as<int64_t>(), m, ks->rows.as<float>() + (size_t)k * m * q->n2, q->n2));
+    lcm_expand_rows_kernel<<<dim3((unsigned)cdiv(n2f, 256), (unsigned)m), 256, 0, p->stream>>>(ks->rows.as<float>(), Q, m, q->n2, idx, n1f,
+                                                                                            ks->Bd.as<float>(), ks->T, OUT, ldo);
+    p->launches++;
+    GP_CUDA(cudaGetLastError());
+    return GP_OK;
+  }
   GP_CHECK(ks->rows.ensure(sizeof(float) * (size_t)m * q->n2));
   if (ks->masked) {   // requested observed rows -> interleaved rows; full rows into scratch, then the observed columns
     GP_CHECK(ks->gidx.ensure(sizeof(int64_t) * m));
@@ -327,9 +457,18 @@ int kron_kdiag(gp_plan* p, float* OUT) {
   GP_REQUIRE(ks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
   GP_CHECK(kron_refresh(p));
   gp_plan* q = ks->data;
+  const int64_t n1f = q->n1 * ks->T;
+  if (ks->nterm > 1) {   // sum_q s_q k_q(x_i, x_i) B_q[a, a]
+    const int Q = ks->nterm;
+    GP_CHECK(ks->rows.ensure(sizeof(float) * (size_t)Q * q->n1));
+    for (int k = 0; k < Q; ++k) GP_CHECK(gp_kdiag(ks->term[k], ks->rows.as<float>() + (size_t)k * q->n1));
+    lcm_expand_diag_kernel<<<(unsigned)cdiv(n1f, 256), 256, 0, p->stream>>>(ks->rows.as<float>(), Q, q->n1, ks->Bd.as<float>(), ks->T, OUT);
+    p->launches++;
+    GP_CUDA(cudaGetLastError());
+    return GP_OK;
+  }
   GP_CHECK(ks->rows.ensure(sizeof(float) * q->n1));
   GP_CHECK(gp_kdiag(q, ks->rows.as<float>()));
-  const int64_t n1f = q->n1 * ks->T;
   if (ks->masked) GP_CHECK(ks->full.ensure(sizeof(float) * n1f));
   float* dst = ks->masked ? ks->full.as<float>() : OUT;
   kron_expand_diag_kernel<<<(unsigned)cdiv(n1f, 256), 256, 0, p->stream>>>(ks->rows.as<float>(), q->n1, ks->Bd.as<float>(), ks->T, dst);
@@ -360,15 +499,13 @@ static int kron_expand_operands(gp_plan* p, const float** L, int64_t* ldl, const
   return GP_OK;
 }
 
-// lengthscale(s) and outputscale: the data plan's bilinear derivative over chunk pairs (L unmixed, R mixed by B), summed in order
-int kron_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os) {
+// lengthscale(s) and outputscale of one term: data plan q's bilinear derivative over chunk pairs (L unmixed, R mixed by B, the
+// term's T x T block on the device), summed in order.  L [N1 T][ldl], R [N2 T][ldr] over the interleaved rows
+static int kron_bilinear_term(gp_plan* p, gp_plan* q, const float* B, const float* L, int64_t ldl, const float* R, int64_t ldr, int s,
+                              double* grad_ls, double* grad_os) {
   gp_kron_state* ks = p->kron;
-  GP_REQUIRE(ks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
-  GP_CHECK(kron_refresh(p));
-  gp_plan* q = ks->data;
   const int T = ks->T;
   const int64_t n1f = q->n1 * T, n2f = q->n2 * T;
-  GP_CHECK(kron_expand_operands(p, &L, &ldl, &R, &ldr, s));
   const int nls = (int)q->ls.size();
   std::vector<double> gl(nls, 0.0), tot(nls, 0.0);
   double go = 0.0, tot_os = 0.0;
@@ -385,8 +522,7 @@ int kron_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, 
                                                                                                     nchunk, nullptr, ks->Lw.as<float>(), nullptr,
                                                                                                     nullptr);
     kron_mix_kernel<false><<<(unsigned)cdiv((int64_t)nchunk * q->n2 * TP, 256), 256, 0, p->stream>>>(p->misc3.as<float>(), q->n2, q->n2, T, tc,
-                                                                                                    nchunk, ks->Bd.as<float>(), ks->W.as<float>(),
-                                                                                                    nullptr, nullptr);
+                                                                                                    nchunk, B, ks->W.as<float>(), nullptr, nullptr);
     p->launches += 2;
     GP_CUDA(cudaGetLastError());
     for (int c = 0; c < nchunk; ++c) {
@@ -401,16 +537,11 @@ int kron_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, 
   return GP_OK;
 }
 
-static int kron_task_covar_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB) {
+// dB of one term: dB[a][b] = s sum_i L[i T + a] . (K R_b)[i] over data plan q's products of the unmixed chunks, in fp64
+static int kron_dB_term(gp_plan* p, gp_plan* q, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB) {
   gp_kron_state* ks = p->kron;
-  GP_REQUIRE(t >= 1 && L && R && dB, GP_E_SHAPE, "gp_task_covar_grad: bad arguments");
-  GP_REQUIRE((ldl >= t || p->n1 == 1) && (ldr >= t || p->n2 == 1), GP_E_SHAPE,
-             "gp_task_covar_grad: leading dimensions must be >= t (ldl=%lld, ldr=%lld, t=%d)", (long long)ldl, (long long)ldr, t);
-  GP_CHECK(kron_refresh(p));
-  gp_plan* q = ks->data;
   const int T = ks->T;
   const int64_t n1f = q->n1 * T, n2f = q->n2 * T;
-  GP_CHECK(kron_expand_operands(p, &L, &ldl, &R, &ldr, t));
   const int nz = (int)cdiv(q->n1, KRON_RED_ROWS);
   GP_CHECK(p->misc2.ensure(sizeof(float) * n1f * TP));
   GP_CHECK(p->misc3.ensure(sizeof(float) * n2f * TP));
@@ -421,7 +552,7 @@ static int kron_task_covar_grad(gp_plan* p, const float* L, int64_t ldl, const f
     GP_CHECK(to_v16(p, L + c0, ldl, tc, n1f, p->misc2.as<float>()));
     GP_CHECK(to_v16(p, R + c0, ldr, tc, n2f, p->misc3.as<float>()));
     int nchunk = 0;
-    GP_CHECK(kron_chunks<false>(p, p->misc3.as<float>(), tc, nullptr, q->kind, nullptr, &nchunk));
+    GP_CHECK(kron_chunks<false>(p, q, p->misc3.as<float>(), tc, nullptr, nullptr, 0, &nchunk));
     kron_dB_kernel<<<dim3((unsigned)nz, (unsigned)(T * T)), 256, 0, p->stream>>>(ks->part.as<float>(), q->nsplit, q->rows_pad,
                                                                                 p->misc2.as<float>(), q->n1, T, tc, ks->red.as<double>(), q->xbad);
     p->launches++;
@@ -433,6 +564,33 @@ static int kron_task_covar_grad(gp_plan* p, const float* L, int64_t ldl, const f
   }
   for (int e = 0; e < T * T; ++e) dB[e] = (double)q->outputscale * acc[(size_t)e];
   return GP_OK;
+}
+
+// a call that takes one task covariance, on a plan with several terms
+static int kron_refuse_terms(const gp_plan* p, const char* call, const char* instead) {
+  GP_REQUIRE(p->kron->nterm == 1, GP_E_STATE, "%s is not available on a Kronecker plan with %d terms (gp_plan_set_kron_terms): call %s",
+             call, p->kron->nterm, instead);
+  return GP_OK;
+}
+
+// lengthscale(s) and outputscale: the data plan's bilinear derivative over chunk pairs (L unmixed, R mixed by B), summed in order
+int kron_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os) {
+  gp_kron_state* ks = p->kron;
+  GP_CHECK(kron_refuse_terms(p, "gp_bilinear_grad", "gp_kron_terms_grad"));
+  GP_REQUIRE(ks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
+  GP_CHECK(kron_refresh(p));
+  GP_CHECK(kron_expand_operands(p, &L, &ldl, &R, &ldr, s));
+  return kron_bilinear_term(p, ks->data, ks->Bd.as<float>(), L, ldl, R, ldr, s, grad_ls, grad_os);
+}
+
+static int kron_task_covar_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB) {
+  gp_kron_state* ks = p->kron;
+  GP_REQUIRE(t >= 1 && L && R && dB, GP_E_SHAPE, "gp_task_covar_grad: bad arguments");
+  GP_REQUIRE((ldl >= t || p->n1 == 1) && (ldr >= t || p->n2 == 1), GP_E_SHAPE,
+             "gp_task_covar_grad: leading dimensions must be >= t (ldl=%lld, ldr=%lld, t=%d)", (long long)ldl, (long long)ldr, t);
+  GP_CHECK(kron_refresh(p));
+  GP_CHECK(kron_expand_operands(p, &L, &ldl, &R, &ldr, t));
+  return kron_dB_term(p, ks->data, L, ldl, R, ldr, t, dB);
 }
 
 static void kron_release(gp_plan* p) {
@@ -448,6 +606,42 @@ static void kron_release(gp_plan* p) {
 
 using namespace gp;
 
+// gp_plan_set_kron (Q = 1) and gp_plan_set_kron_terms: every check before the plan changes, so a refused call leaves it as it was
+static int kron_attach(gp_plan* p, gp_plan* const* data, int Q, int T) {
+  GP_REQUIRE(T >= 1 && T <= 32, GP_E_SHAPE, "number of tasks T=%d not in [1, 32]", T);
+  for (int k = 0; k < Q; ++k) GP_REQUIRE(data[k] != p, GP_E_STATE, "a Kronecker plan cannot be its own data plan");
+  GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a Kronecker plan");
+  GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a Kronecker plan");
+  GP_CHECK(refuse_settings(p, CALL_SET_KRON));
+  for (int k = 0; k < Q; ++k) GP_CHECK(refuse_settings(data[k], CALL_KRON_DATA));
+  GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
+  for (int k = 0; k < Q; ++k) GP_CHECK(kron_check_data(p, data[k], T));
+  for (int k = 1; k < Q; ++k)
+    GP_REQUIRE(data[k]->n1 == data[0]->n1 && data[k]->n2 == data[0]->n2 && data[k]->same == data[0]->same, GP_E_SHAPE,
+               "gp_plan_set_kron_terms: term %d has %lld x %lld points, term 0 %lld x %lld (the terms share their points' count)", k,
+               (long long)data[k]->n1, (long long)data[k]->n2, (long long)data[0]->n1, (long long)data[0]->n2);
+  gp_kron_state* ks = p->kron ? p->kron : new gp_kron_state();
+  const bool keep_b = p->kron && ks->T == T && ks->b_set && ks->nterm == Q;
+  const int oldT = ks->T;
+  ks->data = data[0];
+  ks->T = T;
+  ks->nterm = Q;
+  for (int k = 0; k < KRON_MAX_TERMS; ++k) ks->term[k] = k < Q ? data[k] : nullptr;
+  p->kron = ks;
+  if (!keep_b) ks->b_set = false;
+  // the mask was for other sizes, or the plan now has several terms (which take no mask)
+  if (ks->masked && !(Q == 1 && oldT == T && data[0]->n1 == ks->mask_n1 && data[0]->n2 == ks->mask_n2)) {
+    ks->masked = false;
+    ks->obs_r.clear();
+    ks->obs_c.clear();
+    p->noise_diag = nullptr;
+  }
+  p->backend_req = GP_BACKEND_KRON;
+  kron_geometry(p);
+  p->data_set = true;
+  return p->hypers_set ? kron_pack(p) : GP_OK;   // without the noise yet: packed by gp_plan_set_hypers
+}
+
 extern "C" int gp_plan_set_kron(gp_plan* p, gp_plan* data, int T) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_CUDA(cudaSetDevice(p->device));
@@ -461,37 +655,16 @@ extern "C" int gp_plan_set_kron(gp_plan* p, gp_plan* data, int T) {
     }
     return GP_OK;
   }
-  GP_REQUIRE(T >= 1 && T <= 32, GP_E_SHAPE, "number of tasks T=%d not in [1, 32]", T);
-  GP_REQUIRE(data != p, GP_E_STATE, "a Kronecker plan cannot be its own data plan");
-  GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a Kronecker plan");
-  GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a Kronecker plan");
-  GP_CHECK(refuse_settings(p, CALL_SET_KRON));
-  GP_CHECK(refuse_settings(data, CALL_KRON_DATA));
-  GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
-  gp_kron_state* ks = p->kron ? p->kron : new gp_kron_state();
-  const bool keep_b = p->kron && ks->T == T && ks->b_set;
-  gp_plan* old = ks->data;
-  const int oldT = ks->T;
-  ks->data = data;
-  ks->T = T;
-  p->kron = ks;
-  const int st = kron_check_data(p, data);
-  if (st != GP_OK) {
-    if (old) { ks->data = old; ks->T = oldT; }
-    else kron_release(p);
-    return st;
-  }
-  if (!keep_b) ks->b_set = false;
-  if (ks->masked && !(oldT == T && data->n1 == ks->mask_n1 && data->n2 == ks->mask_n2)) {   // the mask was for other sizes
-    ks->masked = false;
-    ks->obs_r.clear();
-    ks->obs_c.clear();
-    p->noise_diag = nullptr;
-  }
-  p->backend_req = GP_BACKEND_KRON;
-  kron_geometry(p);
-  p->data_set = true;
-  return p->hypers_set ? kron_pack(p) : GP_OK;   // without the noise yet: packed by gp_plan_set_hypers
+  return kron_attach(p, &data, 1, T);
+}
+
+extern "C" int gp_plan_set_kron_terms(gp_plan* p, gp_plan* const* data, int Q, int T) {
+  GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
+  if (data == nullptr) return gp_plan_set_kron(p, nullptr, 0);
+  GP_REQUIRE(Q >= 1 && Q <= KRON_MAX_TERMS, GP_E_SHAPE, "number of terms Q=%d not in [1, %d]", Q, KRON_MAX_TERMS);
+  for (int k = 0; k < Q; ++k) GP_REQUIRE(data[k] != nullptr, GP_E_SHAPE, "gp_plan_set_kron_terms: data plan of term %d missing", k);
+  GP_CUDA(cudaSetDevice(p->device));
+  return kron_attach(p, data, Q, T);
 }
 
 // host index list -> int32 vector; nullptr: every one of the nfull rows (empty vector)
@@ -529,6 +702,7 @@ static int kron_obs_upload(const std::vector<int>& obs, int64_t nfull, gp::DevBu
 
 extern "C" int gp_plan_set_kron_observed(gp_plan* p, const int64_t* rows, int64_t n_rows, const int64_t* cols, int64_t n_cols) {
   GP_REQUIRE(p != nullptr && p->kron != nullptr, GP_E_STATE, "gp_plan_set_kron_observed: not a Kronecker plan (gp_plan_set_kron)");
+  GP_CHECK(kron_refuse_terms(p, "gp_plan_set_kron_observed", "gp_plan_set_kron with one data plan first"));
   GP_CUDA(cudaSetDevice(p->device));
   gp_kron_state* ks = p->kron;
   const gp_plan* q = ks->data;
@@ -556,22 +730,63 @@ extern "C" int gp_plan_set_kron_observed(gp_plan* p, const int64_t* rows, int64_
   return p->hypers_set ? kron_pack(p) : GP_OK;
 }
 
-// gp_plan_set_task_covar / gp_task_covar_grad on a Kronecker plan (tasks.cu forwards them here)
-int gp::kron_set_task_covar(gp_plan* p, const float* B, int T) {
+// the Q task covariance blocks, row-major T x T each, to the host copy and the device
+static int kron_set_blocks(gp_plan* p, const float* B, int Q, int T) {
   gp_kron_state* ks = p->kron;
   GP_REQUIRE(B != nullptr && T == ks->T, GP_E_SHAPE, "task covariance must be %d x %d (got T=%d)", ks->T, ks->T, T);
   GP_CUDA(cudaSetDevice(p->device));
-  ks->B.assign(B, B + (size_t)T * T);
+  const size_t nb = (size_t)Q * T * T;
+  ks->B.assign(B, B + nb);
   ks->b_bad = false;
   for (float v : ks->B) ks->b_bad = ks->b_bad || !std::isfinite(v);
-  GP_CHECK(ks->Bd.ensure(sizeof(float) * T * T));
-  GP_CUDA(cudaMemcpyAsync(ks->Bd.p, ks->B.data(), sizeof(float) * T * T, cudaMemcpyHostToDevice, p->stream));
+  GP_CHECK(ks->Bd.ensure(sizeof(float) * nb));
+  GP_CUDA(cudaMemcpyAsync(ks->Bd.p, ks->B.data(), sizeof(float) * nb, cudaMemcpyHostToDevice, p->stream));
   GP_CUDA(cudaStreamSynchronize(p->stream));   // the next call may replace ks->B
   ks->b_set = true;
   return GP_OK;
 }
 
+extern "C" int gp_plan_set_kron_term_covars(gp_plan* p, const float* B, int Q, int T) {
+  GP_REQUIRE(p != nullptr && p->kron != nullptr, GP_E_STATE, "gp_plan_set_kron_term_covars: not a Kronecker plan (gp_plan_set_kron_terms)");
+  GP_REQUIRE(Q == p->kron->nterm, GP_E_SHAPE, "gp_plan_set_kron_term_covars: the plan has %d terms (got Q=%d)", p->kron->nterm, Q);
+  return kron_set_blocks(p, B, Q, T);
+}
+
+extern "C" int gp_kron_terms_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* grad_ls,
+                                  double* grad_os, double* dB) {
+  GP_REQUIRE(p != nullptr && p->kron != nullptr, GP_E_STATE, "gp_kron_terms_grad: not a Kronecker plan (gp_plan_set_kron_terms)");
+  GP_REQUIRE(p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
+  GP_REQUIRE(t >= 1 && L && R && grad_ls && grad_os && dB, GP_E_SHAPE, "gp_kron_terms_grad: bad arguments");
+  GP_REQUIRE((ldl >= t || p->n1 == 1) && (ldr >= t || p->n2 == 1), GP_E_SHAPE,
+             "gp_kron_terms_grad: leading dimensions must be >= t (ldl=%lld, ldr=%lld, t=%d)", (long long)ldl, (long long)ldr, t);
+  gp_kron_state* ks = p->kron;
+  GP_REQUIRE(ks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_kron_term_covars)");
+  GP_CUDA(cudaSetDevice(p->device));
+  if (ks->nterm == 1) {   // the single-term passes, observed-row masks included
+    GP_CHECK(kron_bilinear_grad(p, L, ldl, R, ldr, t, grad_ls, grad_os));
+    return kron_task_covar_grad(p, L, ldl, R, ldr, t, dB);
+  }
+  GP_CHECK(kron_refresh(p));
+  const int T = ks->T;
+  int ls_off = 0;
+  for (int k = 0; k < ks->nterm; ++k) {   // term order; each term's sums are fp64 in a fixed order
+    gp_plan* q = ks->term[k];
+    const float* Bk = ks->Bd.as<float>() + (size_t)k * T * T;
+    GP_CHECK(kron_bilinear_term(p, q, Bk, L, ldl, R, ldr, t, grad_ls + ls_off, grad_os + k));
+    GP_CHECK(kron_dB_term(p, q, L, ldl, R, ldr, t, dB + (size_t)k * T * T));
+    ls_off += (int)q->ls.size();
+  }
+  return GP_OK;
+}
+
+// gp_plan_set_task_covar / gp_task_covar_grad on a Kronecker plan (tasks.cu forwards them here)
+int gp::kron_set_task_covar(gp_plan* p, const float* B, int T) {
+  GP_CHECK(kron_refuse_terms(p, "gp_plan_set_task_covar", "gp_plan_set_kron_term_covars"));
+  return kron_set_blocks(p, B, 1, T);
+}
+
 int gp::kron_task_covar_grad_checked(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* dB) {
+  GP_CHECK(kron_refuse_terms(p, "gp_task_covar_grad", "gp_kron_terms_grad"));
   GP_REQUIRE(p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_REQUIRE(p->kron->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
   GP_CUDA(cudaSetDevice(p->device));

@@ -207,6 +207,10 @@ constexpr int PC_KIND_SPECTRAL = 71;
 // Kronecker with observed rows (kron.cu, gp_plan_set_kron_observed): row r is interleaved row g = task[r] (the row map), point
 // g / T, task g mod T; entries as PC_KIND_TASK
 constexpr int PC_KIND_KRON_OBS = 72;
+// Kronecker with several terms (kron.cu, gp_plan_set_kron_terms): row r is point r / rep, task r mod rep (rep = T); K[r, r'] =
+// sum_t os_t B_t[a, b] k_t(|z_t,point(r) - z_t,point(r')|^2) with B the terms' T x T blocks back to back; the pivot rows of all
+// terms are staged back to back, as PC_KIND_SUM does
+constexpr int PC_KIND_KRON_TERMS = 73;
 struct PcTerms {
   int n;
   int kind[4], DP[4];
@@ -292,6 +296,13 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
     } else if constexpr (KIND == PC_KIND_KRON_OBS) {
       const int64_t zr = tt.task[pi] / tt.T;
       for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[zr * DP + c];
+    } else if constexpr (KIND == PC_KIND_KRON_TERMS) {
+      const int64_t zr = pi / tt.rep;
+      int off = 0;
+      for (int t = 0; t < tt.n; ++t) {
+        for (int c = tid; c < tt.DP[t]; c += PCP_THREADS) zp[off + c] = tt.Z[t][zr * tt.DP[t] + c];
+        off += tt.DP[t];
+      }
     } else {
       const int64_t zr = (KIND == PC_KIND_TASK || KIND == PC_KIND_DERIV || KIND == PC_KIND_M52GRAD) ? pi / tt.rep : pi;
       for (int c = tid; c < DP; c += PCP_THREADS) zp[c] = Z[zr * DP + c];
@@ -370,6 +381,21 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             s = fmaf(df, df, s);
           }
           v = os * tt.B[(gp_ % tt.T) * tt.T + gj % tt.T] * pc_cov_rt(tt.kind[0], -0.5f * s, CovParam{});
+        } else if constexpr (KIND == PC_KIND_KRON_TERMS) {
+          const int64_t zr = (int)j / tt.rep;
+          const int a = pi % tt.rep, b = (int)j % tt.rep;
+          v = 0.f;
+          int off = 0;
+          for (int t = 0; t < tt.n; ++t) {
+            const float* zj = tt.Z[t] + zr * tt.DP[t];
+            float s = 0.f;
+            for (int c = 0; c < tt.DP[t]; ++c) {
+              float df = zp[off + c] - zj[c];
+              s = fmaf(df, df, s);
+            }
+            v = fmaf(tt.os[t] * tt.B[(t * tt.T + a) * tt.T + b], pc_cov_rt(tt.kind[t], -0.5f * s, CovParam{}), v);
+            off += tt.DP[t];
+          }
         } else if (KIND == PC_KIND_DERIV || KIND == PC_KIND_M52GRAD) {
           using K = DerivTable<KIND == PC_KIND_M52GRAD ? GP_MATERN52 : GP_RBF>;
           const float* zj = Z + (int64_t)((int)j / tt.rep) * DP;
@@ -527,6 +553,19 @@ __global__ void pc_init_kron_obs_kernel(const PcTerms tt, float os, float* __res
   if (j >= n) return;
   const int a = tt.task[j] % tt.T;
   diag[j] = os * tt.B[a * tt.T + a];
+  perm[j] = (int)j;
+  pos[j] = (int)j;
+}
+
+// Kronecker with several terms: diag[j] = sum_t os_t B_t[a, a], a = j mod T (not constant across tasks); then pc_first_pivot_kernel
+__global__ void pc_init_kron_terms_kernel(const PcTerms tt, float* __restrict__ diag, int* __restrict__ perm, int* __restrict__ pos,
+                                          int64_t n) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int a = (int)(j % tt.rep);
+  float v = 0.f;
+  for (int t = 0; t < tt.n; ++t) v = fmaf(tt.os[t], tt.B[(t * tt.T + a) * tt.T + a], v);
+  diag[j] = v;
   perm[j] = (int)j;
   pos[j] = (int)j;
 }
@@ -924,6 +963,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   const bool kron = p->kron != nullptr;
   const bool tasks = p->tasks != nullptr || kron;
   const bool kron_obs = kron && p->kron->masked;
+  const bool kron_terms = kron && p->kron->nterm > 1;
   const bool deriv = p->deriv != nullptr;
   const float* Zsrc = p->Z2.as<float>();
   if (deriv) {   // entries of the value / gradient operator from the data plan's packed rows
@@ -942,6 +982,15 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     Zsrc = q->Z2.as<float>();
     dp_total = q->DP;
     os_total = q->outputscale;
+    if (kron_terms) {   // PC_KIND_KRON_TERMS: every term's packed rows, widths back to back
+      tt.n = p->kron->nterm;
+      dp_total = 0;
+      for (int t = 0; t < tt.n; ++t) {
+        const gp_plan* qt = p->kron->term[t];
+        tt.kind[t] = qt->kind; tt.DP[t] = qt->DP; tt.os[t] = qt->outputscale; tt.Z[t] = qt->Z2.as<float>();
+        dp_total += qt->DP;
+      }
+    }
   } else if (tasks) {
     GP_REQUIRE(p->tasks->b_set, GP_E_STATE, "task covariance not set (gp_plan_set_task_covar)");
     tt.kind[0] = p->kind; tt.task = p->tasks->d_t1; tt.B = p->tasks->Bd.as<float>(); tt.T = p->tasks->T; tt.rep = 1;
@@ -955,6 +1004,10 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   if (deriv) {
     const float c = (float)deriv_with_kind(p->deriv->kind, [](auto K) { return decltype(K)::DIAG; });
     pc_init_deriv_kernel<<<gb, PC_THREADS, 0, st>>>(tt, os_total, c, diag, perm, pos, n);
+    pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
+    p->launches += 2;
+  } else if (kron_terms) {
+    pc_init_kron_terms_kernel<<<gb, PC_THREADS, 0, st>>>(tt, diag, perm, pos, n);
     pc_first_pivot_kernel<<<1, PC_FIRST_THREADS, 0, st>>>(diag, perm, pos, n, S, piv);
     p->launches += 2;
   } else if (kron_obs) {
@@ -994,11 +1047,12 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   if (coop && !stepwise) {
     const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
-    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : kron_obs ? PC_KIND_KRON_OBS : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : spec ? PC_KIND_SPECTRAL : p->kind) {
+    switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : kron_terms ? PC_KIND_KRON_TERMS : kron_obs ? PC_KIND_KRON_OBS : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : spec ? PC_KIND_SPECTRAL : p->kind) {
       case PC_KIND_ADDITIVE: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_ADDITIVE>; break;
       case PC_KIND_SPECTRAL: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SPECTRAL>; break;
       case PC_KIND_TASK: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_TASK>; break;
       case PC_KIND_KRON_OBS: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_KRON_OBS>; break;
+      case PC_KIND_KRON_TERMS: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_KRON_TERMS>; break;
       case PC_KIND_DERIV: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_DERIV>; break;
       case PC_KIND_M52GRAD: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_M52GRAD>; break;
       case GP_RBF: fn1 = (const void*)pc_persistent1_kernel<GP_RBF>; break;
@@ -1197,6 +1251,14 @@ extern "C" int gp_ciq_precond_build(gp_plan* p, const float* Lt, int k, float* U
   } else if (p->deriv) {    // s N (1 + c sum_c 1 / l_c^2), c = 1 RBF, 5/3 Matern-5/2
     GP_CHECK(deriv_refresh(p));
     tr_k = deriv_trace(p);
+  } else if (p->kron && p->kron->nterm > 1) {   // N sum_q s_q sum_a B_q[a, a]
+    const gp_kron_state* ks = p->kron;
+    tr_k = 0.0;
+    for (int q = 0; q < ks->nterm; ++q) {
+      double bt = 0.0;
+      for (int a = 0; a < ks->T; ++a) bt += (double)ks->B[((size_t)q * ks->T + a) * ks->T + a];
+      tr_k += (double)ks->term[q]->outputscale * (double)ks->term[q]->n2 * bt;
+    }
   } else if (p->kron && p->kron->masked) {   // s sum_r B[a_r, a_r] over the observed rows r, a_r = rowmap[r] mod T
     const gp_kron_state* ks = p->kron;
     double bt = 0.0;

@@ -681,6 +681,71 @@ class KronPlan(_DataPlanOperator):
         return self
 
 
+class LcmPlan(_DataPlanOperator):
+    """The linear model of coregionalisation sum_q (s_q K_q) (x) B_q over interleaved rows i T + a (gp_plan_set_kron_terms): N1 T x
+    N2 T, built on Q = 1..4 ready data Plans over the same number of points (kept alive here), each with its own kind, lengthscales,
+    outputscale s_q, backend and inputs.  set_noise supplies the noise; set_term_covars / terms_grad take the B_q and return every
+    gradient.  Every product, solve and sample call of Plan works on it."""
+
+    def __init__(self, datas, num_tasks: int):
+        super().__init__(list(datas)[0], list(datas), num_tasks)
+
+    def attach(self, first: Plan, datas, num_tasks: int):
+        """(Re-)attach the data plans: validation and geometry only; B_q of the same Q and T stay set."""
+        datas = list(datas)
+        T = int(num_tasks)
+        arr = (C.c_void_p * len(datas))(*[d._h.value for d in datas])
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_kron_terms(self._h, arr, len(datas), T))
+        self.data, self.datas, self.num_tasks = datas[0], datas, T
+        self.same, self.d = datas[0].same, datas[0].d
+        self.n1, self.n2 = datas[0].n1 * T, datas[0].n2 * T
+        self.row_begin, self.row_count = 0, self.n1
+        return self
+
+    def refresh_data(self):
+        return self.attach(self.data, self.datas, self.num_tasks)
+
+    def set_noise(self, noise: float):
+        """The noise of this plan; each term keeps its own kind, lengthscales and outputscale."""
+        arr = (C.c_float * 1)(1.0)
+        self.kind, self.lengthscale, self.noise, self.outputscale = self.data.kind, [1.0], float(noise), 1.0
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_hypers(self._h, KIND[self.kind], arr, 1, 1.0, float(noise)))
+        return self
+
+    def set_term_covars(self, b: torch.Tensor):
+        """B_q [Q, T, T] (any device; copied to the host).  Call again whenever one changes."""
+        Q, T = len(self.datas), self.num_tasks
+        bh = b.detach().to(device="cpu", dtype=torch.float32).contiguous()
+        if tuple(bh.shape) != (Q, T, T):
+            raise RuntimeError(f"the task covariances must be [{Q}, {T}, {T}] (got {tuple(b.shape)})")
+        arr = (C.c_float * (Q * T * T))(*bh.reshape(-1).tolist())
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_kron_term_covars(self._h, arr, Q, T))
+        return self
+
+    def terms_grad(self, left: torch.Tensor, right: torch.Tensor):
+        """([dl_q] per term, [ds_q], dB [Q, T, T] float64 on the CPU) of sum(left * (K @ right)), left [n1, s], right [n2, s]."""
+        if left.dim() != 2 or right.dim() != 2 or left.size(0) != self.n1 or right.size(0) != self.n2 \
+                or left.size(1) != right.size(1) or left.size(1) < 1:
+            raise RuntimeError(f"terms_grad: left must be [{self.n1}, s] and right [{self.n2}, s] "
+                               f"(got {tuple(left.shape)}, {tuple(right.shape)})")
+        _require_cuda_f32(left, "left")
+        _require_cuda_f32(right, "right")
+        left, right = _row_block(left), _row_block(right)
+        Q, T = len(self.datas), self.num_tasks
+        nls = [len(d.lengthscale) for d in self.datas]
+        gl, go, db = (C.c_double * sum(nls))(), (C.c_double * Q)(), (C.c_double * (Q * T * T))()
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_kron_terms_grad(self._h, _ptr(left), _ld(left), _ptr(right), _ld(right), left.size(1), gl, go, db))
+        out, o = [], 0
+        for k in nls:
+            out.append([gl[o + i] for i in range(k)])
+            o += k
+        return out, [go[q] for q in range(Q)], torch.tensor(list(db), dtype=torch.float64).reshape(Q, T, T)
+
+
 class DerivPlan(_DataPlanOperator):
     """The value / gradient operator over interleaved rows i (d+1) + a: N1 (d+1) x N2 (d+1), built on a ready plain data Plan of
     covariance `kind` (kept alive here): "rbf" (gp_plan_set_deriv, RBFKernelGrad) or "matern52" (gp_plan_set_deriv_kind,

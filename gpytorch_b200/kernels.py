@@ -1,5 +1,6 @@
 """gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, RQKernel, PolynomialKernel, SpectralMixtureKernel,
-PeriodicKernel, ScaleKernel, AdditiveKernel, ProductKernel, GridInterpolationKernel} for the accelerated path.
+PeriodicKernel, ScaleKernel, AdditiveKernel, ProductKernel, IndexKernel, MultitaskKernel, LCMKernel, GridInterpolationKernel} for the
+accelerated path.
 
 Same constructor kwargs and call contract as the reference (kernels/kernel.py:163-171, :454-534;
 rbf_kernel.py:68-85; matern_kernel.py:79-110; scale_kernel.py:64-118), but `forward` returns an
@@ -499,6 +500,8 @@ class ScaleKernel(Kernel):
     """K <- outputscale * base(K)  (kernels/scale_kernel.py:64-118); the scale is folded into the fused kernel."""
 
     def __init__(self, base_kernel, outputscale_prior=None, outputscale_constraint=None, **kwargs):
+        if isinstance(base_kernel, LCMKernel):
+            raise NotImplementedError("ScaleKernel(LCMKernel(...)) is not available on the accelerated path: scale the base kernels")
         if base_kernel.active_dims is not None:
             kwargs["active_dims"] = base_kernel.active_dims
         super().__init__(**kwargs)
@@ -751,6 +754,57 @@ class MultitaskKernel(Kernel):
     def num_outputs_per_input(self, x1, x2):
         """An n x m data covariance becomes an (n T) x (m T) multitask covariance."""
         return self.num_tasks
+
+
+class LCMKernel(Kernel):
+    """Linear model of coregionalisation (kernels/lcm_kernel.py): K = sum_q K_q(x1, x2) (x) B_q over interleaved rows i T + a, one
+    MultitaskKernel per base kernel in `covar_module_list` (the reference's names, so state-dict keys match), each with its own
+    IndexKernel B_q = F_q F_q^T + diag(v_q) of rank `rank` (an int, or one per base kernel).  Base kernels are what MultitaskKernel
+    takes (RBFKernel / MaternKernel, optionally inside a ScaleKernel).  forward returns one engine operator: the term's
+    KroneckerKernelLinearOperator for one base kernel, an LCMKernelLinearOperator (gp_plan_set_kron_terms) for 2 to 4.  Unbatched, no
+    prior."""
+
+    def __init__(self, base_kernels, num_tasks, rank=1, task_covar_prior=None):
+        if len(base_kernels) < 1:
+            raise ValueError("At least one base kernel must be provided.")
+        for k in base_kernels:
+            if not isinstance(k, Kernel):
+                raise ValueError("base_kernels must only contain Kernel objects")
+        if len(base_kernels) > 4:
+            raise NotImplementedError(f"an LCMKernel takes up to 4 base kernels on the accelerated path (got {len(base_kernels)})")
+        if task_covar_prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        if not isinstance(rank, list):
+            rank = [rank] * len(base_kernels)
+        if len(rank) != len(base_kernels):
+            raise ValueError(f"rank has {len(rank)} entries for {len(base_kernels)} base kernels")
+        super().__init__()
+        self.covar_module_list = torch.nn.ModuleList(
+            [MultitaskKernel(k, num_tasks=num_tasks, rank=r, task_covar_prior=task_covar_prior) for k, r in zip(base_kernels, rank)])
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, last_dim_is_batch=False, **params):
+        if _batch_index is not None:
+            raise NotImplementedError("a batched LCMKernel is not available on the accelerated path")
+        terms = [m.forward(x1, x2, diag=diag, _same=_same, last_dim_is_batch=last_dim_is_batch, **params) for m in self.covar_module_list]
+        if diag:
+            out = terms[0]
+            for t in terms[1:]:
+                out = out + t
+            return out
+        if len(terms) == 1:
+            return terms[0]
+        from .operators import LCMKernelLinearOperator
+        return LCMKernelLinearOperator(terms)
+
+    def _batchable(self):
+        return False
+
+    def _unbatched_name(self):
+        return "LCMKernel"
+
+    def num_outputs_per_input(self, x1, x2):
+        """An n x m data covariance becomes an (n T) x (m T) multitask covariance."""
+        return self.covar_module_list[0].num_outputs_per_input(x1, x2)
 
 
 class GridInterpolationKernel(Kernel):

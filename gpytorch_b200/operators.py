@@ -21,7 +21,7 @@ import torch
 
 from . import settings
 from ._lib import NanError
-from .engine import DerivPlan, KronPlan, Plan
+from .engine import DerivPlan, KronPlan, LcmPlan, Plan
 from .sampling import contour_quadrature, psd_safe_cholesky
 
 
@@ -88,6 +88,8 @@ def clear_plan_cache():
             _PRODUCT_PLANS.popitem()[1].close()
         while _KRON_PLANS:
             _KRON_PLANS.popitem()[1].close()
+        while _LCM_PLANS:
+            _LCM_PLANS.popitem()[1].close()
         while _DERIV_PLANS:
             _DERIV_PLANS.popitem()[1].close()
         while _PLAN_CACHE:
@@ -794,6 +796,143 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
 
 
 _KRON_PLANS: "dict[tuple, Plan]" = {}
+
+
+_LCM_SLOT = 40   # plan-cache slots of the term data plans of LCM operators: 40 + term index (the other families use 0..8, 16,
+                 # 20/21, 24, 28 and 32..37), so two terms over the same inputs never share one plan and its hyper-parameters
+_LCM_PLANS: "dict[tuple, Plan]" = {}
+
+
+class LCMKernelLinearOperator(KernelLinearOperator):
+    """sum_q (s_q K_q(x1, x2)) (x) B_q over interleaved rows i T + a, Q = 1..4 (LCMKernel, kernels/lcm_kernel.py; the reference sums
+    KroneckerProductLinearOperators into a SumLinearOperator): ONE engine operator (gp_plan_set_kron_terms) on the terms' data plans.
+    `terms` are unmasked KroneckerKernelLinearOperators of one shape and T; each keeps its own inputs (active dimensions), kind,
+    lengthscale, outputscale and B.  The hyper-parameters are [l_1, s_1, B_1, ..., l_Q, s_Q, B_Q]; their gradients come from
+    gp_kron_terms_grad.  Input gradients are not available: the terms refuse inputs that require grad."""
+
+    def __init__(self, terms):
+        terms = list(terms)
+        if not 1 <= len(terms) <= 4:
+            raise NotImplementedError(f"an LCM operator takes 1 to 4 terms on the accelerated path (got {len(terms)})")
+        for t in terms:
+            if type(t) is not KroneckerKernelLinearOperator or t.rows is not None or t.cols is not None:
+                raise NotImplementedError(f"the terms of an LCM operator are unmasked Kronecker operators (got {type(t).__name__})")
+        first = terms[0]
+        if any(tuple(t.shape) != tuple(first.shape) or t.num_tasks != first.num_tasks or t.same != first.same for t in terms):
+            raise RuntimeError("the terms of an LCM operator must share their shape, number of tasks and squareness")
+        super().__init__(first.x1, None if first.same else first.x2, first.kind, first.lengthscale, first.outputscale)
+        self.terms = terms
+        self.num_tasks = first.num_tasks
+        self.same = first.same
+        self._data_ops = []
+        for i, t in enumerate(terms):
+            op = KernelLinearOperator(t.x1, None if t.same else t.x2, t.kind, t.lengthscale, t.outputscale)
+            op._plan_slot = _LCM_SLOT + i
+            self._data_ops.append(op)
+
+    @property
+    def shape(self):
+        return self.terms[0].shape
+
+    def plan(self, noise=0.0) -> Plan:
+        datas = []
+        for op in self._data_ops:
+            d = op.plan(0.0)
+            if getattr(d, "_noise_diag", None) is not None:
+                d.set_noise_diag(None)
+            datas.append(d)
+        nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
+        T = self.num_tasks
+        with _PLAN_LOCK:
+            key = (tuple(id(d) for d in datas), T)
+            parent = _LCM_PLANS.pop(key, None)
+            if parent is None:
+                parent = LcmPlan(datas, T)
+                parent._hyp_key = None
+                parent._b_key = None
+            _LCM_PLANS[key] = parent
+            while len(_LCM_PLANS) > 16:
+                _LCM_PLANS.pop(next(iter(_LCM_PLANS))).close()
+        # the data plans may have been re-packed or re-pointed since the last use: re-attach them (validation, no allocation)
+        parent.attach(datas[0], datas, T)
+        hk = (nz, tuple((d.kind, tuple(d.lengthscale), d.outputscale) for d in datas))
+        if parent._hyp_key != hk:
+            parent.set_noise(nz)
+            parent._hyp_key = hk
+        bh = getattr(self, "_b_host", None)
+        if bh is None:
+            bh = self._b_host = torch.stack([t.B.detach().float() for t in self.terms]).cpu()
+        if parent._b_key is None or not torch.equal(parent._b_key, bh):
+            parent.set_term_covars(bh)
+            parent._b_key = bh
+        self._plan = parent
+        return parent
+
+    @property
+    def requires_grad(self):
+        return any(t.requires_grad for t in self.terms)
+
+    def representation(self):
+        return tuple(v for t in self.terms for v in t.representation())
+
+    def hyper_tensors(self):
+        return [h for t in self.terms for h in (t.lengthscale, t.outputscale, t.B)]
+
+    def input_tensors(self):
+        return []
+
+    def solve_input_tensors(self):
+        return []
+
+    def _bilinear_derivative_list(self, left, right):
+        gl, go, dB = self.plan(getattr(self, "_last_noise", 0.0)).terms_grad(left, right)
+        out = []
+        for t, l, o, b in zip(self.terms, gl, go, dB):
+            out += [torch.tensor(l, device=self.device, dtype=self.dtype).reshape(t.lengthscale.shape),
+                    torch.tensor(o, device=self.device, dtype=self.dtype).reshape(t.outputscale.shape),
+                    b.to(device=self.device, dtype=t.B.dtype)]
+        return out
+
+    def _bilinear_derivative(self, left, right):
+        raise NotImplementedError("an LCM operator has one lengthscale and outputscale per term: use _bilinear_derivative_list")
+
+    def _transpose_nonbatch(self):
+        if self.same:
+            return self
+        return LCMKernelLinearOperator([t._transpose_nonbatch() for t in self.terms])
+
+    def detach(self):
+        return LCMKernelLinearOperator([t.detach() for t in self.terms])
+
+    def to_dense(self):
+        return _KernelDense.apply(self)
+
+    def diagonal(self, dim1=-2, dim2=-1):
+        """sum_q s_q k_q(x1_i, x2_i) B_q[a, a] at row i T + a."""
+        if self.shape[0] != self.shape[1]:
+            raise RuntimeError(f"diagonal of a non-square operator {tuple(self.shape)} is undefined")
+        return self.plan().diag()
+
+    _diagonal = diagonal
+
+    def __getitem__(self, index):
+        """Slices that start and stop on multiples of T slice every term (prediction slices the joint operator at n T)."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        return LCMKernelLinearOperator([t[ri, ci] for t in self.terms])
+
+    def mul(self, other):
+        raise NotImplementedError("an LCM operator takes no further factor")
+
+    __mul__ = mul
+
+    def __add__(self, other):
+        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
+            return AddedDiagLinearOperator(self, other)
+        raise NotImplementedError("an LCM operator adds a (Constant)DiagLinearOperator only")
 
 
 def _mask_index(mask, n, what):
@@ -2104,6 +2243,7 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
         """A plan-backed non-SKI kernel operator (or kernel sum) without batch dimension on an unsharded square plan."""
         return (isinstance(base, KernelLinearOperator) and not isinstance(base, (SKIKernelLinearOperator, HadamardKernelLinearOperator,
                                                                                           KroneckerKernelLinearOperator,
+                                                                                          LCMKernelLinearOperator,
                                                                                           DerivKernelLinearOperator,
                                                                                           ProductKernelLinearOperator))
                 and base.same

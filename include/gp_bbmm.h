@@ -343,6 +343,30 @@ int gp_plan_set_kron(gp_plan* plan, gp_plan* data, int T);
  * gp_task_covar_grad (L and R of n_rows and n_cols rows) are those of the masked operator.  GP_E_STATE: not a Kronecker plan. */
 int gp_plan_set_kron_observed(gp_plan* plan, const int64_t* rows, int64_t n_rows, const int64_t* cols, int64_t n_cols);
 
+/* Several latent processes (the linear model of coregionalisation, LCMKernel, kernels/lcm_kernel.py): `plan` becomes the
+ * N1 T x N2 T operator
+ *     sum_q (s_q K_q) (x) B_q,   q = 0 .. Q-1,   over interleaved rows i T + a   (+ its noise / per-row diagonal),
+ * where K_q is data[q]'s operator and s_q its outputscale.  1 <= Q <= 4 (GP_E_SHAPE otherwise); every data[q] is a data plan as
+ * gp_plan_set_kron takes it (the same roles and refusals), and the terms may differ in kind, lengthscale, backend and input rows
+ * (active dimensions), but share N1, N2, squareness, device and stream (GP_E_SHAPE / GP_E_STATE otherwise).  data = NULL clears the
+ * operator; Q = 1 is gp_plan_set_kron(plan, data[0], T).  One K.V is, per term, a B_q mix and ceil(T t / 16) launches of data[q]'s
+ * fused kernel, then one scatter of sum_q s_q (term's product) in a fixed order (terms outer, splits inner); it is NaN when any
+ * term has non-finite inputs or any B_q a non-finite entry.  gp_krows, gp_kdiag, gp_pivoted_cholesky (entries
+ * sum_q s_q B_q[a, b] k_q, first pivot = argmax of the diagonal), the preconditioner calls, gp_mbcg, gp_slq_logdet, gp_mll,
+ * gp_lanczos and gp_ciq_* run on it.  On a plan with Q > 1, gp_plan_set_task_covar, gp_task_covar_grad, gp_bilinear_grad and
+ * gp_plan_set_kron_observed return GP_E_STATE (naming the call to use instead). */
+int gp_plan_set_kron_terms(gp_plan* plan, gp_plan* const* data, int Q, int T);
+
+/* B_0 .. B_{Q-1} of a plan set by gp_plan_set_kron_terms: Q row-major T x T host blocks back to back, in term order (copied). */
+int gp_plan_set_kron_term_covars(gp_plan* plan, const float* B, int Q, int T);
+
+/* Gradients of F = sum(L * (K R)) for L [N1 T, t] (leading dimension ldl) and R [N2 T, t] (ldr) on a Kronecker plan, in term
+ * order: grad_ls = every term's lengthscale gradient(s) concatenated (1 or d per term), grad_os = the Q outputscale gradients,
+ * dB = the Q T x T blocks dF/dB_q (row-major, back to back).  Per term these are gp_bilinear_grad's and gp_task_covar_grad's
+ * passes with that term's B_q; the sums are fp64 in a fixed order, without atomics: repeated calls agree bit for bit. */
+int gp_kron_terms_grad(gp_plan* plan, const float* L, int64_t ldl, const float* R, int64_t ldr, int t, double* grad_ls, double* grad_os,
+                       double* dB);
+
 /* GPs with derivative observations (RBFKernelGrad, kernels/rbf_kernel_grad.py:60-115, with the perfect shuffle of :99-102, as in
  * examples/08_Advanced_Usage/Simple_GP_Regression_Derivative_Information_{1d,2d}.ipynb): `plan` becomes the N1 (d+1) x N2 (d+1)
  * operator over interleaved rows i (d+1) + a (a = 0: f(x_i); a = 1..d: df/dx_a at x_i) with, for D = x_i - x'_j,
