@@ -14,9 +14,11 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("GPBBMM_LIB") or os.path.join(_HERE, "lib", "libgpbbmm.so")   # GPBBMM_LIB: see INTEGRATION.md
 
 GP_OK, GP_E_SHAPE, GP_E_CUDA, GP_E_NAN_MVM, GP_W_NOT_CONVERGED, GP_W_PIVCHOL_NAN, GP_E_NCCL, GP_E_STATE, GP_W_EIG_NOT_CONVERGED = range(9)
-GP_RBF, GP_MATERN12, GP_MATERN32, GP_MATERN52, GP_RQ, GP_POLY = range(6)
-GP_BACKEND_AUTO, GP_BACKEND_TCGEN05, GP_BACKEND_SIMT, GP_BACKEND_SKI, GP_BACKEND_SUM, GP_BACKEND_KRON, GP_BACKEND_DERIV, GP_BACKEND_PRODUCT = range(8)
-KIND = {"rbf": GP_RBF, "matern12": GP_MATERN12, "matern32": GP_MATERN32, "matern52": GP_MATERN52, "rq": GP_RQ, "poly": GP_POLY}
+GP_RBF, GP_MATERN12, GP_MATERN32, GP_MATERN52, GP_RQ, GP_POLY, GP_PPOLY = range(7)
+GP_BACKEND_AUTO, GP_BACKEND_TCGEN05, GP_BACKEND_SIMT, GP_BACKEND_SKI, GP_BACKEND_SUM, GP_BACKEND_KRON, GP_BACKEND_DERIV, GP_BACKEND_PRODUCT, \
+    GP_BACKEND_COMPACT = range(9)
+KIND = {"rbf": GP_RBF, "matern12": GP_MATERN12, "matern32": GP_MATERN32, "matern52": GP_MATERN52, "rq": GP_RQ, "poly": GP_POLY,
+        "ppoly": GP_PPOLY}
 BACKEND = {"auto": GP_BACKEND_AUTO, "tcgen05": GP_BACKEND_TCGEN05, "simt": GP_BACKEND_SIMT}
 
 
@@ -80,6 +82,8 @@ PROTOTYPES = {
     "gp_plan_set_periodic": (_I, [_P, C.POINTER(_F), _I, _I]),
     "gp_plan_set_hypers_rq": (_I, [_P, C.POINTER(_F), _I, _F, _F, _F]),
     "gp_plan_set_hypers_poly": (_I, [_P, _I, _F, _F, _F]),
+    "gp_plan_set_hypers_pp": (_I, [_P, _I, C.POINTER(_F), _I, _F, _F]),
+    "gp_plan_tile_pairs": (_I, [_P, C.POINTER(_L), C.POINTER(_L)]),
     "gp_plan_set_lowrank": (_I, [_P, _P, _L, _I]),
     "gp_plan_set_tasks": (_I, [_P, _P, _P, _I]),
     "gp_plan_set_task_covar": (_I, [_P, C.POINTER(_F), _I]),

@@ -370,6 +370,7 @@ extern "C" int gp_plan_set_additive(gp_plan* p, int max_degree, const float* com
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become an additive plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become an additive plan");
   GP_CHECK(refuse_settings(p, CALL_SET_ADDITIVE));
+  GP_CHECK(refuse_compact(p, "gp_plan_set_additive"));
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,
              "an additive plan is not available on a row-sharded plan");
   GP_REQUIRE(n_comp >= 1 && n_comp <= ADD_DMAX, GP_E_SHAPE, "an additive plan takes 1 to %d components (got %d)", ADD_DMAX, n_comp);

@@ -133,6 +133,7 @@ extern "C" int gp_plan_destroy(gp_plan* p) {
   }
   if (p->kron) gp_plan_set_kron(p, nullptr, 0);   // the data plan stays the caller's
   if (p->deriv) gp_plan_set_deriv(p, nullptr);
+  compact_release(p);
   if (p->pinned) cudaFreeHost(p->pinned);
   delete p;
   return GP_OK;
@@ -142,6 +143,7 @@ extern "C" int gp_plan_set_backend(gp_plan* p, int backend) {
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(backend >= GP_BACKEND_AUTO && backend <= GP_BACKEND_SIMT, GP_E_SHAPE, "bad backend %d", backend);
   GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_STATE, "the SKI backend is selected by gp_plan_set_ski");
+  GP_CHECK(refuse_compact(p, "gp_plan_set_backend"));
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel sum runs the backends of its terms");
   GP_REQUIRE(p->kron == nullptr, GP_E_STATE, "a Kronecker plan runs the backend of its data plan");
   GP_CHECK(refuse_settings(p, CALL_SET_BACKEND));
@@ -162,6 +164,7 @@ extern "C" int gp_plan_set_data(gp_plan* p, const float* X1, int64_t n1, int64_t
     p->data_set = false;   // no re-pack of the old layout on the way out
     GP_CHECK(gp_plan_set_tasks(p, nullptr, nullptr, 0));
   }
+  if (p->compact) p->compact->order_stale = true;   // new points: a new Morton order at the next packing
   p->X1 = X1; p->n1 = n1; p->ld1 = ld1; p->d = d;
   p->same = (X2 == nullptr) || (X2 == X1 && n2 == n1 && ld2 == ld1);
   if (p->same) { p->X2 = X1; p->n2 = n1; p->ld2 = ld1; }
@@ -186,6 +189,7 @@ extern "C" int gp_plan_set_hypers(gp_plan* p, int kind, const float* lengthscale
   GP_REQUIRE(p != nullptr, GP_E_STATE, "null plan");
   GP_REQUIRE(kind != GP_RQ, GP_E_SHAPE, "the rational quadratic kind takes alpha: call gp_plan_set_hypers_rq");
   GP_REQUIRE(kind != GP_POLY, GP_E_SHAPE, "the polynomial kind takes a power and an offset: call gp_plan_set_hypers_poly");
+  GP_REQUIRE(kind != GP_PPOLY, GP_E_SHAPE, "the piecewise polynomial kind takes q and runs its own backend: call gp_plan_set_hypers_pp");
   GP_REQUIRE(kind >= GP_RBF && kind <= GP_MATERN52, GP_E_SHAPE, "nu expected to be 0.5, 1.5, or 2.5 (kind=%d)", kind);
   GP_REQUIRE(lengthscale && n_ls >= 1, GP_E_SHAPE, "lengthscale missing");
   GP_REQUIRE(!p->data_set || n_ls == 1 || n_ls == p->d, GP_E_SHAPE, "lengthscale count %d does not match d=%d", n_ls, p->d);
@@ -194,6 +198,7 @@ extern "C" int gp_plan_set_hypers(gp_plan* p, int kind, const float* lengthscale
   GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
   GP_REQUIRE(p->per_n == 0 || kind == GP_RBF, GP_E_STATE, "gp_plan_set_hypers on a periodic plan (gp_plan_set_periodic) takes the kind GP_RBF (got %d)", kind);
   GP_CUDA(cudaSetDevice(p->device));
+  compact_release(p);   // another kind: a plain plan again
   p->kind = kind;
   p->ls.assign(lengthscale, lengthscale + n_ls);
   p->outputscale = outputscale;
@@ -213,6 +218,7 @@ extern "C" int gp_plan_set_hypers_rq(gp_plan* p, const float* lengthscale, int n
   GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "gp_plan_set_hypers_rq is not available on a SKI plan (gp_plan_set_ski)");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "gp_plan_set_hypers_rq is not available on a kernel-sum plan: give the kind to a term");
+  GP_CHECK(refuse_compact(p, "gp_plan_set_hypers_rq"));
   GP_CHECK(refuse_settings(p, CALL_SET_HYPERS_RQ));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_STATE, "gp_plan_set_hypers_rq is not available on a row-sharded plan (gp_plan_set_comm)");
   GP_CUDA(cudaSetDevice(p->device));
@@ -249,6 +255,7 @@ extern "C" int gp_plan_set_hypers_poly(gp_plan* p, int power, float offset, floa
   GP_REQUIRE(outputscale > 0.f && noise >= 0.f, GP_E_SHAPE, "outputscale must be > 0 and noise >= 0");
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "gp_plan_set_hypers_poly is not available on a SKI plan (gp_plan_set_ski)");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "gp_plan_set_hypers_poly is not available on a kernel-sum plan: give the kind to a term");
+  GP_CHECK(refuse_compact(p, "gp_plan_set_hypers_poly"));
   GP_CHECK(refuse_settings(p, CALL_SET_HYPERS_POLY));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_STATE, "gp_plan_set_hypers_poly is not available on a row-sharded plan (gp_plan_set_comm)");
   GP_CUDA(cudaSetDevice(p->device));
@@ -308,6 +315,7 @@ extern "C" int gp_plan_set_comm(gp_plan* p, gp_comm* comm) {
   GP_REQUIRE(!(p->kron && comm && comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   GP_REQUIRE(!(p->deriv && comm && comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   if (comm && comm->world > 1) GP_CHECK(refuse_settings(p, CALL_SET_COMM_SHARDED));
+  if (comm && comm->world > 1) GP_CHECK(refuse_compact(p, "gp_plan_set_comm with more than one rank"));
   p->comm = comm;
   return GP_OK;
 }
@@ -340,6 +348,7 @@ extern "C" int gp_time_kmv_kernel(gp_plan* p, const float* V, int64_t ldv, int t
     // a derivative plan: the derivative kernel over the live column chunks and the split sum
     if (p->deriv) return deriv_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, p->V16.as<float>(), nullptr);
+    if (p->compact) return compact_kmv_partials(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_SUM) return sum_kmv_launch(p, p->V16.as<float>(), nullptr);
     if (p->backend == GP_BACKEND_PRODUCT) return product_kmv_launch(p, p->V16.as<float>(), nullptr);
     if (p->add_M) return additive_kmv_launch(p, p->V16.as<float>(), nullptr);

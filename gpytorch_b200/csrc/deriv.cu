@@ -259,6 +259,7 @@ static int deriv_check_data(const gp_plan* p, const gp_plan* q) {
   else
     GP_REQUIRE(q->kind == GP_RBF, GP_E_SHAPE, "derivative observations are available for the RBF kernel only (kind=%d)", q->kind);
   GP_CHECK(refuse_settings(q, CALL_DERIV_DATA_REFRESH));
+  GP_CHECK(refuse_compact(q, "a derivative operator's data plan"));
   GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
              "derivative plan: a row-sharded data plan is not available");
   GP_REQUIRE(q->device == p->device && q->stream == p->stream, GP_E_STATE, "derivative plan: the data plan must live on the same device and stream");
@@ -500,7 +501,9 @@ static int deriv_set(gp_plan* p, gp_plan* data, int kind, CallId call, CallId da
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a derivative plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a derivative plan");
   GP_CHECK(refuse_settings(p, call));
+  GP_CHECK(refuse_compact(p, "gp_plan_set_deriv"));
   GP_CHECK(refuse_settings(data, data_role));
+  GP_CHECK(refuse_compact(data, "gp_plan_set_deriv (the data plan)"));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a derivative plan is not available on a row-sharded plan");
   gp_deriv_state* ds = p->deriv ? p->deriv : new gp_deriv_state();
   gp_plan* old = ds->data;

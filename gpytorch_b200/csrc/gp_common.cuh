@@ -222,6 +222,25 @@ struct gp_deriv_state {
   gp::DevBuf part, gout, hypd;             // split partials [nsplit][N1 (d+1)][16] | gradient CTA partials | hyp on the device
 };
 
+// Compact-support backend (compact.cu, GP_BACKEND_COMPACT): piecewise polynomial kernels over points in Morton order.  Row tiles
+// of 128 and column tiles of 64 sorted points; per row tile the CSR list of the column tiles within reach (box gap < 1 in x / l).
+constexpr int PP_DMAX = 16;      // input dimensions: bounds the template cases and the exponent j + q <= 15
+constexpr int PP_TI = 128;       // sorted rows per row tile (one per thread)
+constexpr int PP_TJ = 64;        // sorted columns per column tile
+constexpr int PP_MAX_SLOTS = 32; // partial slots one row tile's list is split across
+struct gp_compact_state {
+  int q = 2;
+  bool order_stale = true;         // set by gp_plan_set_data: the Morton order and the raw tile boxes are redone at the next packing
+  int64_t ntile_i = 0, ntile_j = 0;
+  int64_t pairs = 0;               // evaluated tile pairs of the current schedule
+  int chunk = 1;                   // column tiles per partial slot of one row tile
+  gp::DevBuf perm1, perm2;         // sorted position -> caller's row (int32) of the row / column side (perm2 aliases perm1 square)
+  gp::DevBuf box1, box2;           // raw fp32 tile boxes [ntile][2][d] (lo | hi) of each side
+  gp::DevBuf Zs1, Zs2;             // packed rows (x - mean) / l in sorted order [n][DP]
+  gp::DevBuf rowptr, cols, cnt;    // CSR schedule: int64 [ntile_i + 1], int32 column tiles, int32 per-row-tile counts
+  gp::DevBuf sortbuf, lohi, lsd;   // sort keys / values / CUB scratch; per-dimension lo / hi of the raw inputs; l_c in fp64
+};
+
 struct gp_comm {
   void* nccl_comm = nullptr;
   int rank = 0, world = 1;
@@ -306,6 +325,7 @@ struct gp_plan {
   // polynomial kernels (kind GP_POLY, gp_plan_set_hypers_poly): S (x.x' + c)^p over the raw inputs (no centring, no lengthscale)
   int poly_power = 0;
   float poly_offset = 0.f;
+  gp_compact_state* compact = nullptr;   // non-null: piecewise polynomial kernel on GP_BACKEND_COMPACT (gp_plan_set_hypers_pp)
   int kron_cols = 16;             // columns of V16 a Kronecker or derivative product computes (KronColsScope); the rest must be zero or unused
   void* pinned = nullptr;  // small pinned host scratch: PINNED_BYTES, one PIN_* slot per user
 };
@@ -419,6 +439,12 @@ int spectral_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float*
 // periodic.cu
 int periodic_pack(gp_plan* p);                                          // embeds the inputs into Z1 / Z2 (and the tensor-core tiles)
 int periodic_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+// compact.cu
+int compact_pack(gp_plan* p);                                           // Morton order (when stale), sorted rows, tile lists, slots
+int compact_kmv_partials(gp_plan* p, const float* V16, const int* done_flag);
+int compact_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os);
+int refuse_compact(const gp_plan* p, const char* call);                 // GP_E_STATE when p runs on GP_BACKEND_COMPACT
+void compact_release(gp_plan* p);                                       // back to a plain plan (frees the backend state)
 // columns of the packed rows the plain kernels see: the d inputs, or the 2d embedding columns of a periodic plan
 inline int packed_dims(const gp_plan* p) { return p->per_n ? 2 * p->d : p->d; }
 inline bool plan_is_tc(const gp_plan* p) {
@@ -434,8 +460,12 @@ struct CovParam {
   float ialpha;   // RQ: 1 / alpha, rounded once from fp64
   float offset;   // POLY: c >= 0 (packed into the GEMM1 operands on the tensor-core path, added to the dot product on the CUDA cores)
   int power;      // POLY: 1 <= p <= 8
+  int pp_e;       // PPOLY: exponent j + q <= 15
+  float pp_c1, pp_c2, pp_c3;   // PPOLY: poly_q(r) = 1 + c1 r + c2 r^2 + c3 r^3, rounded once from fp64
 };
+CovParam pp_param(int q, int d);   // compact.cu: the piecewise polynomial's exponent and coefficients for d input columns
 inline CovParam cov_param(const gp_plan* p) {
+  if (p->kind == GP_PPOLY) return pp_param(p->compact ? p->compact->q : 0, p->d);
   if (p->kind == GP_POLY) return CovParam{0.f, 0.f, p->poly_offset, p->poly_power};
   return p->kind == GP_RQ ? CovParam{p->rq_alpha, (float)(1.0 / (double)p->rq_alpha), 0.f, 0} : CovParam{0.f, 0.f, 0.f, 0};
 }
@@ -481,9 +511,13 @@ __host__ __device__ constexpr bool is_rq_code(int code) { return code >= RQ_K &&
 constexpr int POLY_K = 24;    // POLY: k = a^p
 constexpr int POLY_DC = 25;   // POLY: dk/dc = p a^(p-1)
 __host__ __device__ constexpr bool is_poly_code(int code) { return code == POLY_K || code == POLY_DC; }
+// Piecewise polynomial kernels (DESIGN 4.24): k = (1 - r)_+^e poly_q(r) with r = sqrt(-2 a) in the packed units (C = 1).  The public
+// GP_PPOLY = 6 is the number of GP_DERIV + GP_MATERN32, so only this code of its own reaches a template.
+constexpr int PP_K = 32;
 // the code a dispatcher evaluates for `kind` on plan p: on an RQ plan GP_RQ (the plan's own kind) is RQ_K, on a polynomial plan
 // GP_POLY is POLY_K
 inline int rq_code(const gp_plan* p, int kind) {
+  if (p->kind == GP_PPOLY && kind == GP_PPOLY) return PP_K;
   if (p->kind == GP_POLY && kind == GP_POLY) return POLY_K;
   return (p->kind == GP_RQ && kind == GP_RQ) ? RQ_K : kind;
 }
@@ -497,6 +531,28 @@ __host__ __device__ __forceinline__ float poly_pow(float a, int q) {
   if (q & 4) r *= a4;
   if (q & 8) r = a4 * a4;   // q = 8 exactly (q <= 8)
   return r;
+}
+
+// m^e for 0 <= e <= 15 by squaring (m^2, m^4, m^8 and the product of the ones e selects)
+__host__ __device__ __forceinline__ float pp_pow(float m, int e) {
+  const float m2 = m * m, m4 = m2 * m2, m8 = m4 * m4;
+  float r = (e & 1) ? m : 1.f;
+  if (e & 2) r *= m2;
+  if (e & 4) r *= m4;
+  if (e & 8) r *= m8;
+  return r;
+}
+// (1 - r)_+^e poly_q(r): exactly 0 for r >= 1, exactly 1 at r = 0
+__host__ __device__ __forceinline__ float pp_k(float r, CovParam cp) {
+  const float m = fmaxf(1.f - r, 0.f);
+  return pp_pow(m, cp.pp_e) * fmaf(fmaf(fmaf(cp.pp_c3, r, cp.pp_c2), r, cp.pp_c1), r, 1.f);
+}
+// -dk/dr = m^(e-1) (e poly - m poly'), 0 for r >= 1 (m = 0, also where e = 1 leaves a kink at r = 1)
+__host__ __device__ __forceinline__ float pp_mdk(float r, CovParam cp) {
+  const float m = fmaxf(1.f - r, 0.f);
+  const float P = fmaf(fmaf(fmaf(cp.pp_c3, r, cp.pp_c2), r, cp.pp_c1), r, 1.f);
+  const float dP = fmaf(fmaf(3.f * cp.pp_c3, r, 2.f * cp.pp_c2), r, cp.pp_c1);
+  return m > 0.f ? pp_pow(m, cp.pp_e - 1) * ((float)cp.pp_e * P - m * dP) : 0.f;
 }
 
 #if defined(__CUDACC__)
@@ -543,7 +599,9 @@ __device__ __forceinline__ float dcov_from_arg(float a, float* kout, CovParam cp
 
 template <int KIND>
 __device__ __forceinline__ float cov_from_arg(float a, CovParam cp) {
-  if (KIND == POLY_K) {   // a = x_i . x_j + c (no clamp: a may be negative)
+  if (KIND == PP_K) {   // a = -r^2 / 2 from direct differences: r = 0 on the diagonal, k = 1
+    return pp_k(sqrtf(fmaxf(-2.f * a, 0.f)), cp);
+  } else if (KIND == POLY_K) {   // a = x_i . x_j + c (no clamp: a may be negative)
     return poly_pow(a, cp.power);
   } else if (KIND == POLY_DC) {
     return (float)cp.power * poly_pow(a, cp.power - 1);

@@ -170,6 +170,7 @@ static int kmv_partials_base(gp_plan* p, const float* V16, const int* done_flag)
   if (p->deriv) return deriv_kmv_partials(p, V16, done_flag);
   if (p->tasks) return tasks_kmv_partials(p, V16, p->kind, done_flag);
   if (p->backend == GP_BACKEND_SKI) return ski_kmv_partials(p, V16, done_flag);
+  if (p->compact) return compact_kmv_partials(p, V16, done_flag);
   if (p->backend == GP_BACKEND_PRODUCT) {
     GP_CHECK(product_refresh(p));   // before the V tiles are packed: a re-packed factor can change the backend
     if (p->prod_tc) GP_CHECK(pack_v_tiles(p, V16));
@@ -548,6 +549,7 @@ static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int
     case GP_MATERN32: GP_KROWS(GP_MATERN32); break;
     case GP_RQ: GP_KROWS(RQ_K); break;
     case GP_POLY: GP_KROWS(POLY_K); break;
+    case GP_PPOLY: GP_KROWS(PP_K); break;
     default: GP_KROWS(GP_MATERN52); break;
   }
 #undef GP_KROWS
@@ -611,6 +613,7 @@ static int kdiag_base(gp_plan* p, float* OUT) {
       case GP_MATERN32: GP_KDIAG(GP_MATERN32); break;
       case GP_RQ: GP_KDIAG(RQ_K); break;
       case GP_POLY: GP_KDIAG(POLY_K); break;
+      case GP_PPOLY: GP_KDIAG(PP_K); break;
       default: GP_KDIAG(GP_MATERN52); break;
     }
 #undef GP_KDIAG
@@ -631,6 +634,7 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   GP_REQUIRE((ldl >= s || p->row_count == 1) && (ldr >= s || p->n2 == 1), GP_E_SHAPE,
              "gp_bilinear_grad: leading dimensions must be >= s (ldl=%lld, ldr=%lld, s=%d)", (long long)ldl, (long long)ldr, s);
   if (p->backend == GP_BACKEND_PRODUCT) return product_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
+  if (p->compact) return compact_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->kron) return kron_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->deriv) return deriv_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);
   if (p->add_M) return additive_bilinear_grad(p, Lf, ldl, Rt, ldr, s, grad_ls, grad_os);

@@ -246,6 +246,7 @@ static int kron_check_data(const gp_plan* p, const gp_plan* q, int T) {
   GP_REQUIRE(q->backend == GP_BACKEND_TCGEN05 || q->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
              "Kronecker plan: the data plan must be a plain kernel plan (not SKI, not a kernel sum, not Kronecker)");
   GP_CHECK(refuse_settings(q, CALL_KRON_DATA_REFRESH));
+  GP_CHECK(refuse_compact(q, "a Kronecker operator's data plan"));
   GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
              "Kronecker plan: a row-sharded data plan is not available");
   GP_REQUIRE(q->device == p->device && q->stream == p->stream, GP_E_STATE, "Kronecker plan: the data plan must live on the same device and stream");
@@ -613,7 +614,9 @@ static int kron_attach(gp_plan* p, gp_plan* const* data, int Q, int T) {
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a Kronecker plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a Kronecker plan");
   GP_CHECK(refuse_settings(p, CALL_SET_KRON));
+  GP_CHECK(refuse_compact(p, "gp_plan_set_kron"));
   for (int k = 0; k < Q; ++k) GP_CHECK(refuse_settings(data[k], CALL_KRON_DATA));
+  for (int k = 0; k < Q; ++k) GP_CHECK(refuse_compact(data[k], "gp_plan_set_kron (the data plan)"));
   GP_REQUIRE(!(p->comm && p->comm->world > 1), GP_E_SHAPE, "a Kronecker plan is not available on a row-sharded plan");
   for (int k = 0; k < Q; ++k) GP_CHECK(kron_check_data(p, data[k], T));
   for (int k = 1; k < Q; ++k)

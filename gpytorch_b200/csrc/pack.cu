@@ -155,6 +155,7 @@ int choose_geometry(gp_plan* p) {
   if (want == GP_BACKEND_AUTO) want = (p->KP <= KP_MAX) ? GP_BACKEND_TCGEN05 : GP_BACKEND_SIMT;
   if (p->add_M) want = GP_BACKEND_SIMT;   // additive plans run their own CUDA-core kernels on Z (additive.cu)
   if (p->sm_Q) want = GP_BACKEND_SIMT;    // so do spectral plans, on their own packed rows (spectral.cu)
+  if (p->compact) want = GP_BACKEND_COMPACT;   // piecewise polynomial plans run their tile-pair lists (compact.cu)
   GP_REQUIRE(!(want == GP_BACKEND_TCGEN05 && p->KP > KP_MAX), GP_E_SHAPE,
              "tcgen05 (tensor-core) backend needs 3d+4 <= %d (d=%d)", KP_MAX, p->d);
   p->backend = want;
@@ -209,7 +210,7 @@ int pack_inputs(gp_plan* p) {
   std::vector<float> sc(d);
   // RQ: C = 1 (alpha stays out of the packing, so the value and both derivatives read the same a = -r^2 / 2)
   double cst = (p->kind == GP_RBF) ? 1.4426950408889634
-               : (p->kind == GP_MATERN12 ? 2.0 : (p->kind == GP_MATERN32 ? 6.0 : (p->kind == GP_RQ ? 1.0 : 10.0)));
+               : (p->kind == GP_MATERN12 ? 2.0 : (p->kind == GP_MATERN32 ? 6.0 : (p->kind == GP_RQ || p->kind == GP_PPOLY ? 1.0 : 10.0)));
   const bool poly = p->kind == GP_POLY;   // a dot-product kernel: the raw inputs, no centring and no scale (DESIGN 4.21)
   for (int c = 0; c < d; ++c) {
     double l = (p->ls.size() == 1) ? p->ls[0] : p->ls[c];
@@ -256,6 +257,7 @@ int pack_inputs(gp_plan* p) {
   }
   p->nparts = p->tasks ? 1 : p->nsplit;   // a Hadamard product is combined into one slot in user row order
   if (p->add_M) GP_CHECK(additive_pack(p));
+  if (p->compact) GP_CHECK(compact_pack(p));   // sets nparts: the slots of the longest tile-pair list
   GP_CHECK(p->partial.ensure(sizeof(float) * (size_t)nslots(p) * p->rows_pad * TP));
   GP_CUDA(cudaGetLastError());
   return GP_OK;

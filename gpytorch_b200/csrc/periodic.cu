@@ -275,6 +275,7 @@ extern "C" int gp_plan_set_periodic(gp_plan* p, const float* period, int n_perio
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "a SKI plan cannot become a periodic plan");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a periodic plan");
   GP_CHECK(refuse_settings(p, CALL_SET_PERIODIC));
+  GP_CHECK(refuse_compact(p, "gp_plan_set_periodic"));
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_STATE,
              "a periodic plan is not available on a row-sharded plan");
   GP_REQUIRE(d >= 1 && d <= PER_DMAX, GP_E_SHAPE, "a periodic plan takes 1 <= d <= %d input dimensions (got d=%d)", PER_DMAX, d);

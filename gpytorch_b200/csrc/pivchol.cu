@@ -1060,6 +1060,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       case GP_MATERN32: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN32>; break;
       case GP_RQ: fn1 = (const void*)pc_persistent1_kernel<RQ_K>; break;
       case GP_POLY: fn1 = (const void*)pc_persistent1_kernel<POLY_K>; break;
+      case GP_PPOLY: fn1 = (const void*)pc_persistent1_kernel<PP_K>; break;
       case PC_KIND_SUM: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SUM>; break;
       case PC_KIND_PRODUCT: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_PRODUCT>; break;
       case PC_KIND_SKI: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SKI>; break;
@@ -1084,6 +1085,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
 #define GP_PC_LAUNCH(KK) pc_step_kernel<KK><<<gb, PC_THREADS, sh, st>>>(Z, p->DP, p->outputscale, Lt, n, m, rank, error_tol, diag, perm, pos, S, piv, pval, ppos, psum, cov_param(p))
     switch (p->kind) {
       case GP_RQ: GP_PC_LAUNCH(RQ_K); break;
+      case GP_PPOLY: GP_PC_LAUNCH(PP_K); break;
       case GP_RBF: GP_PC_LAUNCH(GP_RBF); break;
       case GP_MATERN12: GP_PC_LAUNCH(GP_MATERN12); break;
       case GP_MATERN32: GP_PC_LAUNCH(GP_MATERN32); break;

@@ -293,6 +293,7 @@ int product_pack(gp_plan* p) {
     GP_REQUIRE(q->backend == GP_BACKEND_TCGEN05 || q->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
                "kernel product: a factor must be a plain kernel plan (not SKI, not a sum, not a product, not multitask, not derivative)");
     GP_CHECK(refuse_settings(q, CALL_PRODUCT_FACTOR_REFRESH));
+    GP_CHECK(refuse_compact(q, "a kernel product's factor"));
     GP_REQUIRE(q->row_begin == 0 && q->row_count == q->n1 && !(q->comm && q->comm->world > 1), GP_E_SHAPE,
                "kernel product: a row-sharded factor is not available");
     GP_REQUIRE(q->n1 == p->n1 && q->n2 == p->n2 && q->same == p->same, GP_E_SHAPE,
@@ -440,6 +441,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   GP_REQUIRE(p->ski == nullptr, GP_E_STATE, "a SKI plan cannot become a kernel product");
   GP_REQUIRE(p->backend_req != GP_BACKEND_SUM, GP_E_STATE, "a kernel-sum plan cannot become a kernel product");
   GP_CHECK(refuse_settings(p, CALL_SET_PRODUCT));
+  GP_CHECK(refuse_compact(p, "gp_plan_set_product"));
   GP_CUDA(cudaSetDevice(p->device));
   if (factors == nullptr || n_factors == 0) {   // back to a plain plan
     if (p->backend_req != GP_BACKEND_PRODUCT) return GP_OK;
@@ -453,6 +455,7 @@ extern "C" int gp_plan_set_product(gp_plan* p, gp_plan* const* factors, int n_fa
   for (int f = 0; f < n_factors; ++f) {
     GP_REQUIRE(factors[f] != nullptr && factors[f] != p, GP_E_STATE, "kernel product: factor %d is null or the product itself", f);
     GP_CHECK(refuse_settings(factors[f], CALL_PRODUCT_FACTOR));
+    GP_CHECK(refuse_compact(factors[f], "gp_plan_set_product (a factor)"));
   }
   p->factors.assign(factors, factors + n_factors);
   p->backend_req = GP_BACKEND_PRODUCT;

@@ -1348,6 +1348,7 @@ using namespace gp;
 extern "C" int gp_plan_set_ski(gp_plan* p, const int* grid_sizes, const float* grid_lo, const float* grid_step, int d) {
   GP_REQUIRE(p != nullptr && p->data_set, GP_E_STATE, "set_data must precede set_ski");
   GP_CHECK(refuse_settings(p, CALL_SET_SKI));
+  GP_CHECK(refuse_compact(p, "gp_plan_set_ski"));
   GP_REQUIRE(d == p->d && d >= 1 && d <= SKI_MAXD, GP_E_SHAPE, "SKI: grid dimension %d does not match the data (d=%d, max %d)", d, p->d, SKI_MAXD);
   int64_t M = 1;
   bool large = false;

@@ -25,6 +25,7 @@ int sum_pack(gp_plan* p) {
     GP_REQUIRE(t->backend == GP_BACKEND_TCGEN05 || t->backend == GP_BACKEND_SIMT, GP_E_SHAPE,
                "kernel sum: a term must be a plain kernel plan (not SKI, not a sum)");
     GP_CHECK(refuse_settings(t, CALL_SUM_TERM_REFRESH));
+    GP_CHECK(refuse_compact(t, "a kernel sum's term"));
     GP_REQUIRE(t->n1 == p->n1 && t->n2 == p->n2 && t->same == p->same && t->row_begin == p->row_begin && t->row_count == p->row_count,
                GP_E_SHAPE, "kernel sum: term shape %lld x %lld (rows [%lld,+%lld)) differs from the sum's %lld x %lld (rows [%lld,+%lld))",
                (long long)t->n1, (long long)t->n2, (long long)t->row_begin, (long long)t->row_count, (long long)p->n1, (long long)p->n2,
@@ -120,8 +121,11 @@ extern "C" int gp_plan_set_sum(gp_plan* p, gp_plan* const* terms, int n_terms) {
   GP_REQUIRE(terms != nullptr && n_terms >= 1 && n_terms <= 4, GP_E_SHAPE, "a kernel sum takes 1 to 4 terms (got %d)", n_terms);
   GP_REQUIRE(p->ski == nullptr, GP_E_STATE, "a SKI plan cannot become a kernel sum");
   GP_CHECK(refuse_settings(p, CALL_SET_SUM));
-  for (int t = 0; t < n_terms; ++t)
+  GP_CHECK(refuse_compact(p, "gp_plan_set_sum"));
+  for (int t = 0; t < n_terms; ++t) {
     if (terms[t]) GP_CHECK(refuse_settings(terms[t], CALL_SUM_TERM));
+    if (terms[t]) GP_CHECK(refuse_compact(terms[t], "gp_plan_set_sum (a term)"));
+  }
   GP_CUDA(cudaSetDevice(p->device));
   p->terms.assign(terms, terms + n_terms);
   p->backend_req = GP_BACKEND_SUM;

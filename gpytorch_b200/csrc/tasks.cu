@@ -313,6 +313,7 @@ extern "C" int gp_plan_set_tasks(gp_plan* p, const int32_t* task1, const int32_t
     return GP_OK;
   }
   GP_CHECK(refuse_settings(p, CALL_SET_TASKS));
+  GP_CHECK(refuse_compact(p, "gp_plan_set_tasks"));
   GP_REQUIRE(p->data_set, GP_E_STATE, "gp_plan_set_tasks: call gp_plan_set_data first");
   GP_REQUIRE(T >= 1 && T <= 32, GP_E_SHAPE, "number of tasks T=%d not in [1, 32]", T);
   GP_REQUIRE(p->ski == nullptr && p->backend != GP_BACKEND_SKI, GP_E_STATE, "task indices are not available on a SKI plan");

@@ -223,6 +223,7 @@ static int xgrad_check(gp_plan* p, CallId call, float* DX1, int64_t ld1, float* 
   GP_REQUIRE(p && p->data_set && p->hypers_set, GP_E_STATE, "plan not ready");
   GP_CHECK(refuse_settings(p, call));
   const char* what = CALL_ROWS[call].name;
+  GP_CHECK(refuse_compact(p, what));
   GP_REQUIRE(p->backend != GP_BACKEND_SUM, GP_E_SHAPE, "%s of a kernel sum: call it on every term", what);
   GP_REQUIRE(p->backend != GP_BACKEND_SKI, GP_E_SHAPE, "%s is not available on a SKI plan", what);
   GP_REQUIRE(p->row_begin == 0 && p->row_count == p->n1 && !(p->comm && p->comm->world > 1), GP_E_SHAPE,

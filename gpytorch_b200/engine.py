@@ -134,6 +134,19 @@ class Plan:
         self.poly = (int(power), float(offset))
         return self
 
+    def set_hypers_pp(self, q: int, lengthscale, outputscale: float = 1.0, noise: float = 0.0):
+        """Piecewise polynomial kernel S (1 - r)_+^(j+q) poly_q(r) on the compact-support backend (gp_plan_set_hypers_pp): q in
+        {0, 1, 2, 3}, lengthscales (1 or d), outputscale and noise in one engine call.  bilinear_grad then returns [dl (1 or d)] and
+        dF/dS; info() adds the evaluated and total tile pairs."""
+        ls = [float(v) for v in (lengthscale if hasattr(lengthscale, "__len__") else [lengthscale])]
+        arr = (C.c_float * len(ls))(*ls)
+        with torch.cuda.device(self.device):
+            check(self.lib.gp_plan_set_hypers_pp(self._h, int(q), arr, len(ls), float(outputscale), float(noise)))
+        self.kind, self.lengthscale, self.outputscale, self.noise = "ppoly", ls, float(outputscale), float(noise)
+        self.alpha = None
+        self.poly = None
+        return self
+
     def set_hypers_rq(self, lengthscale, alpha: float, outputscale: float = 1.0, noise: float = 0.0):
         """Rational quadratic kernel S (1 + r^2 / (2 alpha))^-alpha (gp_plan_set_hypers_rq): kind, lengthscales (1 or d), alpha,
         outputscale and noise in one engine call.  bilinear_grad then returns [dl (1 or d) | dalpha] and dF/dS."""
@@ -369,7 +382,13 @@ class Plan:
     def info(self):
         b, s, k, m = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         check(self.lib.gp_plan_info(self._h, C.byref(b), C.byref(s), C.byref(k), C.byref(m)))
-        return {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum", 5: "kron", 6: "deriv", 7: "product"}.get(b.value, "?"), "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
+        out = {"backend": {1: "tcgen05", 2: "simt", 3: "ski", 4: "sum", 5: "kron", 6: "deriv", 7: "product", 8: "compact"}.get(b.value, "?"),
+               "nsplit": s.value, "kpad": k.value, "n_sm": m.value}
+        if b.value == _lib.GP_BACKEND_COMPACT:   # tile pairs of 128 rows x 64 columns: evaluated per K.V, and all of them
+            ev, tot = C.c_int64(), C.c_int64()
+            check(self.lib.gp_plan_tile_pairs(self._h, C.byref(ev), C.byref(tot)))
+            out["tile_pairs"], out["tile_pairs_total"] = ev.value, tot.value
+        return out
 
     def time_kmv_kernel(self, v: torch.Tensor, warmup: int = 3, reps: int = 20) -> float:
         """Average device time (ms) of ONE launch of the fused K.V kernel alone (CUDA events on the plan stream)."""

@@ -1,4 +1,5 @@
-"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, RQKernel, PolynomialKernel, SpectralMixtureKernel,
+"""gpytorch.kernels.{Kernel, RBFKernel, RBFKernelGrad, MaternKernel, Matern52KernelGrad, RQKernel, PolynomialKernel,
+PiecewisePolynomialKernel, SpectralMixtureKernel,
 PeriodicKernel, ScaleKernel, AdditiveKernel, ProductKernel, IndexKernel, MultitaskKernel, LCMKernel, GridInterpolationKernel} for the
 accelerated path.
 
@@ -266,6 +267,42 @@ class PolynomialKernel(Kernel):
         off = self.offset if _batch_index is None else self.offset[_batch_index]
         op = PolynomialKernelLinearOperator(x1, None if _same else x2, self.power, off.reshape(-1)[0], outputscale)
         return op.diagonal() if diag else op
+
+
+class PiecewisePolynomialKernel(Kernel):
+    """k = (1 - r)_+^(j+q) poly_q(r), r = |x1 - x2| / l, j = floor(D / 2) + q + 1 with D the input columns after active_dims
+    (kernels/piecewise_polynomial_kernel.py, with the module's own q = 2 coefficient (5 j + 3) / 3, DESIGN 4.24).  Parameters as in
+    the reference: q in {0, 1, 2, 3} and raw_lengthscale [*B, 1, ard_num_dims or 1] with a Positive() constraint unless one is given.
+    forward returns one engine PiecewisePolynomialKernelLinearOperator (gp_plan_set_hypers_pp) on the compact-support backend, whose
+    products evaluate only the point pairs within one lengthscale; inside a ScaleKernel the outputscale multiplies it.  1 <= D <= 16,
+    one batch dimension at most, no priors.  Not a _StationaryKernel on this path: sums, products, SKI, multitask and derivative
+    kernels do not take it, and neither do inputs that require grad."""
+    has_lengthscale = True
+    kind = "ppoly"
+
+    def __init__(self, q=2, lengthscale_prior=None, **kwargs):
+        if lengthscale_prior is not None:
+            raise NotImplementedError("priors are not available on the accelerated path")
+        super().__init__(**kwargs)
+        if q not in {0, 1, 2, 3}:
+            raise ValueError("q expected to be 0, 1, 2 or 3")
+        self.q = q
+
+    def forward(self, x1, x2, diag=False, _same=False, _batch_index=None, outputscale=None, last_dim_is_batch=False, **params):
+        from .operators import PiecewisePolynomialKernelLinearOperator
+        if last_dim_is_batch:
+            raise NotImplementedError("last_dim_is_batch is not available for a PiecewisePolynomialKernel on the accelerated path")
+        if diag and not (_same or x1.size(0) == x2.size(0)):
+            raise RuntimeError("diag=True needs x1 and x2 of equal sizes")
+        ls = self.lengthscale if _batch_index is None else self.lengthscale[_batch_index]
+        ls = ls.reshape(-1)
+        op = PiecewisePolynomialKernelLinearOperator(x1, None if _same else x2, self.q, ls[0] if ls.numel() == 1 else ls, outputscale)
+        return op.diagonal() if diag else op
+
+
+def _is_pp(k):
+    """k is a PiecewisePolynomialKernel, or a ScaleKernel around one."""
+    return isinstance(k, PiecewisePolynomialKernel) or isinstance(getattr(k, "base_kernel", None), PiecewisePolynomialKernel)
 
 
 class Matern52KernelGrad(MaternKernel):
@@ -544,7 +581,7 @@ class ScaleKernel(Kernel):
             first = KernelLinearOperator(f[0].x1, f[0].x2, f[0].kind, f[0].lengthscale, self.outputscale * f[0].outputscale)
             op = ProductKernelLinearOperator([first, *f[1:]])
             return op.diagonal() if diag else op
-        if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel, RQKernel, PolynomialKernel)):   # S folded in
+        if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel, RQKernel, PolynomialKernel, PiecewisePolynomialKernel)):
             os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
             return self.base_kernel.forward(x1, x2, diag=diag, _same=_same, _batch_index=bi, outputscale=os_, **params)
         if isinstance(self.base_kernel, GridInterpolationKernel):
@@ -559,10 +596,10 @@ class ScaleKernel(Kernel):
         if isinstance(base, SKIKernelLinearOperator):
             op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
             return op.diagonal() if diag else op
-        from .operators import (PeriodicKernelLinearOperator, PolynomialKernelLinearOperator, RQKernelLinearOperator,
-                                SumKernelLinearOperator, with_outputscale)
+        from .operators import (PeriodicKernelLinearOperator, PiecewisePolynomialKernelLinearOperator, PolynomialKernelLinearOperator,
+                                RQKernelLinearOperator, SumKernelLinearOperator, with_outputscale)
         # operators with parameters beyond lengthscale and scale
-        keep = (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator)
+        keep = (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator, PiecewisePolynomialKernelLinearOperator)
         if isinstance(base, keep):   # a nested ScaleKernel: both scales folded in, the period / alpha kept
             op = with_outputscale(base, os_ * base.outputscale)
             return op.diagonal() if diag else op
@@ -604,6 +641,8 @@ class AdditiveKernel(Kernel):
                 raise NotImplementedError("sums that contain a ProductKernel are not available on the accelerated path")
             if _is_m52_grad(k):
                 raise NotImplementedError("sums that contain a Matern52KernelGrad are not available on the accelerated path")
+            if _is_pp(k):
+                raise NotImplementedError("sums that contain a PiecewisePolynomialKernel are not available on the accelerated path")
         self.kernels = torch.nn.ModuleList(kernels)
 
     def forward(self, x1, x2, diag=False, **params):
@@ -639,6 +678,8 @@ class ProductKernel(Kernel):
                 raise NotImplementedError("products with a PeriodicKernel factor are not available on the accelerated path")
             if _is_rq(k):
                 raise NotImplementedError("products with an RQKernel factor are not available on the accelerated path")
+            if _is_pp(k):
+                raise NotImplementedError("products with a PiecewisePolynomialKernel factor are not available on the accelerated path")
             base = k.base_kernel if isinstance(k, ScaleKernel) else k
             if not isinstance(base, _StationaryKernel) or isinstance(base, (RBFKernelGrad, Matern52KernelGrad)):
                 raise NotImplementedError("ProductKernel factors must be RBF / Matern kernels (optionally scaled) on the accelerated "
@@ -822,6 +863,9 @@ class GridInterpolationKernel(Kernel):
         if isinstance(base_kernel, PeriodicKernel):
             raise NotImplementedError("a PeriodicKernel base kernel of a GridInterpolationKernel is not available on the accelerated "
                                       "path")
+        if isinstance(base_kernel, PiecewisePolynomialKernel):
+            raise NotImplementedError("a PiecewisePolynomialKernel base kernel of a GridInterpolationKernel is not available on the "
+                                      "accelerated path: it runs its own compact-support backend")
         if isinstance(base_kernel, RQKernel):
             raise NotImplementedError("an RQKernel base kernel of a GridInterpolationKernel is not available on the accelerated path: "
                                       "its heavy tails leave nothing for the band-limited grid products to skip")

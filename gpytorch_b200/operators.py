@@ -450,7 +450,7 @@ class KernelLinearOperator(_SamplingMixin):
         (gp_plan_set_tasks).  RBF / Matern operators, optionally scaled, only.  With another RBF / Matern kernel operator (or a
         product of them) of the same shape: the elementwise product K_1 o K_2 as one engine operator (gp_plan_set_product)."""
         plain = (KernelLinearOperator, ProductKernelLinearOperator)
-        if isinstance(other, (RQKernelLinearOperator, PolynomialKernelLinearOperator)):
+        if isinstance(other, (RQKernelLinearOperator, PolynomialKernelLinearOperator, PiecewisePolynomialKernelLinearOperator)):
             return other.mul(self)   # refused, naming the kernel
         if type(self) in plain and type(other) in plain:
             return ProductKernelLinearOperator([self, other])
@@ -967,7 +967,8 @@ def _take_square(op, idx, memo):
         return ProductKernelLinearOperator([_take_square(o, idx, memo) for o in op.ops])
     if t is AdditiveKernelLinearOperator:
         return AdditiveKernelLinearOperator([_take_square(o, idx, memo) for o in op.ops], op.max_degree)
-    if t in (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator, SpectralMixtureKernelLinearOperator):
+    if t in (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator, SpectralMixtureKernelLinearOperator,
+             PiecewisePolynomialKernelLinearOperator):
         return op._with(take(op.x1), None)
     raise NotImplementedError(f"observation masks are not available for {t.__name__}")
 
@@ -1134,6 +1135,9 @@ class SumKernelLinearOperator(KernelLinearOperator):
             raise NotImplementedError("sums that contain additive operators are not available on the accelerated path")
         if any(isinstance(o, SpectralMixtureKernelLinearOperator) for o in flat):
             raise NotImplementedError("sums that contain spectral mixture operators are not available on the accelerated path")
+        if any(isinstance(o, PiecewisePolynomialKernelLinearOperator) for o in flat):
+            raise NotImplementedError("sums that contain a PiecewisePolynomialKernel operator are not available on the accelerated "
+                                      "path: it runs its own compact-support backend")
         first = flat[0]
         for o in flat[1:]:
             if o.shape != first.shape or o.same != first.same:
@@ -2033,10 +2037,90 @@ class PolynomialKernelLinearOperator(KernelLinearOperator):
     __mul__ = mul
 
 
+_PP_SLOT = 44           # plan-cache slot of piecewise polynomial operators (the other families use 0..8, 16, 20/21, 24, 28, 32..37
+_PP_LOWRANK_SLOT = 45   # and 40..43); their low-rank-corrected plans (lazy LOVE), as periodic operators keep theirs apart
+
+
+class PiecewisePolynomialKernelLinearOperator(KernelLinearOperator):
+    """S (1 - r)_+^(j+q) poly_q(r), r = |(x1 - x2) / l|, j = floor(d / 2) + q + 1 (kernels/piecewise_polynomial_kernel.py, which forms
+    the dense matrix) as ONE engine plan on the compact-support backend (gp_plan_set_hypers_pp): the points are kept in Morton order
+    inside the engine and a product evaluates only the tile pairs within one lengthscale, so its cost follows the sparsity of K.
+    Solves, the preconditioner, SLQ, rows, the diagonal, Lanczos and CIQ run on the plan as on a plain one.  q is a Python int in
+    {0, 1, 2, 3}, lengthscale holds 1 or d values, S is the outputscale of a ScaleKernel around the kernel (None: 1, no gradient);
+    autograd reaches the lengthscale and S through _bilinear_derivative_list.  Sums, products, multitask use, row sharding and
+    gradients with respect to the inputs are refused."""
+
+    def __init__(self, x1, x2, q, lengthscale, outputscale=None, comm=None, row_begin=0, row_count=0):
+        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
+            raise NotImplementedError("a row-sharded PiecewisePolynomialKernel operator is not available on the accelerated path")
+        if torch.is_grad_enabled() and (x1.requires_grad or (x2 is not None and x2.requires_grad)):
+            raise NotImplementedError("gradients with respect to the inputs of a PiecewisePolynomialKernel (deep kernel learning, "
+                                      "posterior input gradients) are not available on the accelerated path")
+        super().__init__(x1, x2, "ppoly", lengthscale, outputscale)
+        self.q = int(q)
+
+    def _slot(self):
+        slot = getattr(self, "_plan_slot", None)
+        return _PP_LOWRANK_SLOT if slot == _LOWRANK_SLOT else _PP_SLOT
+
+    def plan(self, noise=0.0) -> Plan:
+        fresh = False
+        if self._plan is None:
+            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None, self._slot(),
+                                   owner=self)
+            fresh = True
+        if torch.is_tensor(noise):
+            ls, os_, nz, _ = self._host_hypers(noise)
+        else:
+            ls, os_, _, _ = self._host_hypers(None)
+            nz = float(noise)
+        key = ("ppoly", self.q, tuple(ls), os_, nz)
+        if fresh or getattr(self._plan, "_hyp_key", None) != key:
+            self._plan.set_hypers_pp(self.q, ls, os_, nz)
+            self._plan._hyp_key = key
+        return self._plan
+
+    def _input_grad_list(self, *args):   # (left, right, needs) or (w, needs)
+        needs = args[-1]
+        if any(needs):
+            raise NotImplementedError("gradients with respect to the inputs of a PiecewisePolynomialKernel are not available on the "
+                                      "accelerated path")
+        return [None] * len(needs)
+
+    _dense_input_grad_list = _input_grad_list
+
+    def _with(self, x1, x2, detach=False, outputscale=None):
+        f = (lambda t: t.detach()) if detach else (lambda t: t)
+        return PiecewisePolynomialKernelLinearOperator(f(x1), None if x2 is None else f(x2), self.q, f(self.lengthscale),
+                                                       f(self.outputscale if outputscale is None else outputscale))
+
+    def _transpose_nonbatch(self):
+        return self if self.same else self._with(self.x2, self.x1)
+
+    def detach(self):
+        return self._with(self.x1, None if self.same else self.x2, detach=True)
+
+    def __getitem__(self, index):
+        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
+        if not isinstance(index, tuple):
+            index = (index, slice(None))
+        ri, ci = index
+        if isinstance(ri, int):
+            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
+        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
+
+    def mul(self, other):
+        raise NotImplementedError("products that contain a PiecewisePolynomialKernel operator (kernel products, IndexKernel "
+                                  "multitask models) are not available on the accelerated path")
+
+    __mul__ = mul
+
+
 def with_outputscale(op, outputscale):
     """A plain, periodic, RQ or polynomial kernel operator with its outputscale replaced (a ScaleKernel folded into the terms of a
     sum or into the first factor of a product); the operator's other parameters are kept."""
-    if isinstance(op, (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator)):
+    if isinstance(op, (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator,
+                       PiecewisePolynomialKernelLinearOperator)):
         return op._with(op.x1, None if op.same else op.x2, outputscale=outputscale)
     return KernelLinearOperator(op.x1, op.x2, op.kind, op.lengthscale, outputscale)
 

@@ -90,14 +90,15 @@ enum {
 /* covariance function kinds: kernels/rbf_kernel.py:68-85, kernels/matern_kernel.py:85-110, kernels/rq_kernel.py (GP_RQ is set
  * through gp_plan_set_hypers_rq only, which also gives alpha), kernels/polynomial_kernel.py (GP_POLY is set through
  * gp_plan_set_hypers_poly only, which also gives the power and the offset) */
-enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3, GP_RQ = 4, GP_POLY = 5 };
+enum { GP_RBF = 0, GP_MATERN12 = 1, GP_MATERN32 = 2, GP_MATERN52 = 3, GP_RQ = 4, GP_POLY = 5, GP_PPOLY = 6 };
 
 /* which fused K.V kernel runs: GP_BACKEND_TCGEN05 = wgmma/bulk-TMA 3xTF32 tensor-core kernel
  * (the name is historical),
  * GP_BACKEND_SIMT = fp32 CUDA-core kernel (bring-up / cross-check / d > 41). */
 enum { GP_BACKEND_AUTO = 0, GP_BACKEND_TCGEN05 = 1, GP_BACKEND_SIMT = 2, GP_BACKEND_SKI = 3 /* set by gp_plan_set_ski */,
        GP_BACKEND_SUM = 4 /* set by gp_plan_set_sum */, GP_BACKEND_KRON = 5 /* set by gp_plan_set_kron */,
-       GP_BACKEND_DERIV = 6 /* set by gp_plan_set_deriv */, GP_BACKEND_PRODUCT = 7 /* set by gp_plan_set_product */ };
+       GP_BACKEND_DERIV = 6 /* set by gp_plan_set_deriv */, GP_BACKEND_PRODUCT = 7 /* set by gp_plan_set_product */,
+       GP_BACKEND_COMPACT = 8 /* set by gp_plan_set_hypers_pp */ };
 
 typedef struct gp_plan gp_plan;   /* opaque: repacked X, workspaces, stream, comm */
 typedef struct gp_comm gp_comm;   /* opaque: NCCL communicator for row-sharded runs */
@@ -282,6 +283,29 @@ int gp_plan_set_hypers_rq(gp_plan* plan, const float* lengthscale, int n_ls, flo
  * diagonal pair contributes 2 S p (|x_i|^2 + c)^(p-1) x_i.  A SKI, sum or
  * row-sharded plan cannot take this call (GP_E_STATE). */
 int gp_plan_set_hypers_poly(gp_plan* plan, int power, float offset, float outputscale, float noise);
+
+/* Piecewise polynomial kernels (the reference's PiecewisePolynomialKernel, kernels/piecewise_polynomial_kernel.py): kind GP_PPOLY
+ * with its smoothness q in {0, 1, 2, 3}, set together with the lengthscales (1 or d), the outputscale S and the noise in one call:
+ *   K(x, x') = S (1 - r)_+^(j+q) poly_q(r),   r = |(x - x') / l|,   j = floor(d / 2) + q + 1
+ * with the reference module's polynomials, including its q = 2 coefficient (5 j + 3) / 3 where R&W eq. 4.21 has (j^2 + 4 j + 3) / 3
+ * (DESIGN 4.24).  K is exactly zero beyond r = 1, and the plan runs on its own backend, GP_BACKEND_COMPACT (compact.cu): each side's
+ * points are put in Morton order of their raw inputs once per gp_plan_set_data, grouped into 128-row and 64-column tiles, and every
+ * hyper-parameter update lists, per row tile, the column tiles whose bounding boxes in x / l are closer than 1 (fp64, conservative:
+ * no pair with r < 1 is skipped).  K.V evaluates those tile pairs only, on the CUDA cores, and writes the rows in the caller's order;
+ * every other call sees the caller's order too.  1 <= d <= 16 (else GP_E_SHAPE at the packing), q and the lengthscales as above,
+ * else GP_E_SHAPE.  The call takes a plain plan, square or cross, with an optional low-rank correction, that is not row-sharded;
+ * any other plan returns GP_E_STATE.  The call is all or nothing.  gp_plan_set_hypers with kind GP_PPOLY returns GP_E_SHAPE; a
+ * later gp_plan_set_hypers with another kind makes the plan a plain plan again.
+ * gp_kmv, gp_krows, gp_kdiag (the square diagonal is S), gp_pivoted_cholesky, gp_precond_build, gp_precond_probes, gp_mbcg,
+ * gp_slq_logdet, gp_mll, gp_lanczos, gp_ciq_sqrt_matmul, gp_ciq_precond_build, gp_ciq_sqrt_matmul_precond,
+ * gp_plan_set_noise_diag, gp_plan_set_lowrank and gp_time_kmv_kernel run on it.  gp_bilinear_grad returns n_ls doubles in grad_ls
+ * (dF/dl) and dF/dS in grad_os, summed in fp64 in a fixed order; a non-finite input makes them NaN, as it does K.V and the rows.
+ * Sums, products, task indices, Kronecker and derivative operators, additive, spectral, periodic, RQ and polynomial settings,
+ * gp_plan_set_backend, the input gradients and row sharding do not take a plan on this backend (GP_E_STATE). */
+int gp_plan_set_hypers_pp(gp_plan* plan, int q, const float* lengthscale, int n_ls, float outputscale, float noise);
+/* The tile pairs the last packing of a GP_BACKEND_COMPACT plan evaluates per K.V, and all ntile_i * ntile_j of them (128-row by
+ * 64-column tiles).  GP_E_STATE on any other plan. */
+int gp_plan_tile_pairs(gp_plan* plan, int64_t* evaluated, int64_t* total);
 
 /* Low-rank correction (the lazy LOVE posterior covariance K** - K*x R R^T Kx*, models/exact_prediction_strategies.py:464-478,
  * which the reference keeps as test_test_covar + MatmulLinearOperator(root, -root^T)): the plan's operator becomes  s K - U U^T
