@@ -73,7 +73,7 @@ pc_step_kernel(const float* __restrict__ Z, int DP, float os, float* __restrict_
         float df = zp[c] - Z[j * DP + c];
         s = fmaf(df, df, s);
       }
-      float v = os * cov_from_arg<KIND>(-0.5f * s, cp);
+      float v = (s == s) ? os * cov_from_arg<KIND>(-0.5f * s, cp) : s;   // cov_from_arg's clamp would turn a NaN input into r = 0
       {
         // independent partial sums keep 8 L2 loads in flight per thread (the step is latency bound, not bandwidth bound)
         float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -141,9 +141,12 @@ pc_step_kernel(const float* __restrict__ Z, int DP, float os, float* __restrict_
     const float mx = s_val[0];
     const int pp = s_pos[0];
     // while (m == 0) or (m < max_iter and max(errors) > error_tol): will step m+1 run?
-    if (m + 1 >= max_rank || (int64_t)(m + 1) >= n || !(err > tol)) {
+    if (pp < 0) {   // a NaN residual: L holds it (and err is NaN, which the stop rule would take for convergence)
+      st->nan_flag = 1;
       st->done = 1;
-    } else if (pp < 0 || !(mx > 0.f)) {  // NaN / non-positive pivot: the reference ends up with NaNs in L
+    } else if (m + 1 >= max_rank || (int64_t)(m + 1) >= n || !(err > tol)) {
+      st->done = 1;
+    } else if (!(mx > 0.f)) {  // non-positive pivot: the reference ends up with NaNs in L
       st->nan_flag = 1;
       st->done = 1;
     } else {
@@ -257,14 +260,17 @@ struct PcPart {
   int pos, idx, old;
 };
 
+// a kernel sum is held to 56 registers, as the other stationary kinds compile to: three 384-thread CTAs per SM where the column
+// cache leaves room for them (ranks <= 43).  0 (no minimum) for the rest: an explicit 1 lets ptxas spend over 120 registers
+// per thread
 template <int KIND>
-__global__ void __launch_bounds__(PCP_THREADS)
-pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, int64_t n, int max_rank, float tol,
+__global__ void __launch_bounds__(PCP_THREADS, KIND == PC_KIND_SUM ? 3 : 0)
+pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, int64_t n, int max_rank, int ncache, float tol,
                       float* diag, int* pos, PcState* st, int64_t* piv_out, PcPart* part, const PcTerms tt, const SkiRows sk) {
   extern __shared__ float sh[];
   float* zp = sh;
   float* lp = sh + DP;
-  float* col = lp + max_rank;
+  float* col = lp + max_rank;   // [ncache][PCP_THREADS]: L of steps < ncache for the thread's first row
   __shared__ float s_val[PCP_RED];
   __shared__ int s_pos[PCP_RED];
   __shared__ int s_idx[PCP_RED];
@@ -318,7 +324,7 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
       if ((int)j == fx_new) { pj = m; pos[j] = m; }      // pos[pi_new] = m (this step's pivot)
       else if ((int)j == fx_old) { pj = fx_pp; pos[j] = fx_pp; }
       if (pj == m + 1) s_old = (int)j;                   // exactly one thread of the grid
-      const bool cached = (j == jfirst);
+      const bool cached = (j == jfirst) && m < ncache;   // this step's entry goes to the column cache
       if (pj < m) {
         Lm[j] = 0.f;
         if (cached) col[m * PCP_THREADS + tid] = 0.f;
@@ -416,29 +422,34 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
             float df = zp[c] - Z[j * DP + c];
             s = fmaf(df, df, s);
           }
-          v = os * cov_from_arg<(KIND >= PC_KIND_SUM ? GP_RBF : KIND)>(-0.5f * s, tt.cp[0]);
+          // as pc_step_kernel.  Only the plain kinds propagate a NaN input this way; the composite entry sources above still
+          // pass it through their covariance clamps as distance 0
+          v = (s == s) ? os * cov_from_arg<(KIND >= PC_KIND_SUM ? GP_RBF : KIND)>(-0.5f * s, tt.cp[0]) : s;
         }
         {
+          // steps q < mc come from the column cache, the rest from Lt; the fmaf order and the grouping by q mod 4 are those of
+          // pc_step_kernel either way.  ncache is rank or a multiple of 4, so the tail q >= 4 floor(m / 4) lies on one side of mc.
           float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
           int q = 0;
-          if (cached) {
+          const int mc = (j == jfirst) ? min(m, ncache) : 0;
+          if (mc > 0) {
             const float* cj = col + tid;
-            for (; q + 4 <= m; q += 4) {
+            for (; q + 4 <= mc; q += 4) {
               s0 = fmaf(lp[q], cj[q * PCP_THREADS], s0);
               s1 = fmaf(lp[q + 1], cj[(q + 1) * PCP_THREADS], s1);
               s2 = fmaf(lp[q + 2], cj[(q + 2) * PCP_THREADS], s2);
               s3 = fmaf(lp[q + 3], cj[(q + 3) * PCP_THREADS], s3);
             }
-            for (; q < m; ++q) s0 = fmaf(lp[q], cj[q * PCP_THREADS], s0);
-          } else {
-            for (; q + 4 <= m; q += 4) {
-              s0 = fmaf(lp[q], Lt[(int64_t)q * n + j], s0);
-              s1 = fmaf(lp[q + 1], Lt[(int64_t)(q + 1) * n + j], s1);
-              s2 = fmaf(lp[q + 2], Lt[(int64_t)(q + 2) * n + j], s2);
-              s3 = fmaf(lp[q + 3], Lt[(int64_t)(q + 3) * n + j], s3);
-            }
-            for (; q < m; ++q) s0 = fmaf(lp[q], Lt[(int64_t)q * n + j], s0);
+            if (mc == m)
+              for (; q < m; ++q) s0 = fmaf(lp[q], cj[q * PCP_THREADS], s0);
           }
+          for (; q + 4 <= m; q += 4) {
+            s0 = fmaf(lp[q], Lt[(int64_t)q * n + j], s0);
+            s1 = fmaf(lp[q + 1], Lt[(int64_t)(q + 1) * n + j], s1);
+            s2 = fmaf(lp[q + 2], Lt[(int64_t)(q + 2) * n + j], s2);
+            s3 = fmaf(lp[q + 3], Lt[(int64_t)(q + 3) * n + j], s3);
+          }
+          for (; q < m; ++q) s0 = fmaf(lp[q], Lt[(int64_t)q * n + j], s0);
           v -= (s0 + s1) + (s2 + s3);
         }
         v /= dpiv;
@@ -492,10 +503,11 @@ pc_persistent1_kernel(const float* __restrict__ Z, int DP, float os, float* Lt, 
     const float mx = s_val[0];
     const int ppw = s_pos[0], inew = s_idx[0], iold = s_old;
     bool stop = false, nan = false;
-    if (m + 1 >= max_rank || (int64_t)(m + 1) >= n || !(err > tol)) stop = true;
-    else if (ppw < 0 || !(mx > 0.f)) {   // NaN, or nothing positive left: on a polynomial operator (rank_stop) its rank is spent
+    if (ppw < 0) stop = nan = true;   // a NaN residual: L holds it (and err is NaN, which the stop rule would take for convergence)
+    else if (m + 1 >= max_rank || (int64_t)(m + 1) >= n || !(err > tol)) stop = true;
+    else if (!(mx > 0.f)) {   // nothing positive left: on a polynomial operator (rank_stop) its rank is spent
       stop = true;
-      nan = (KIND == POLY_K || KIND == PC_KIND_SUM) ? (ppw < 0 || !tt.rank_stop) : true;
+      nan = (KIND == POLY_K || KIND == PC_KIND_SUM) ? !tt.rank_stop : true;
     }
     if (blockIdx.x == 0 && tid == 0) {
       st->rank = m + 1;
@@ -1045,7 +1057,6 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
   GP_REQUIRE(!spec || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a spectral mixture operator needs the cooperative kernel");
   GP_REQUIRE(!dot || (coop && !stepwise), GP_E_STATE, "pivoted Cholesky of a polynomial operator needs the cooperative kernel");
   if (coop && !stepwise) {
-    const size_t sh = sizeof(float) * (dp_total + rank + (size_t)rank * PCP_THREADS);
     const void* fn1;
     switch (sum ? PC_KIND_SUM : prod ? PC_KIND_PRODUCT : ski ? PC_KIND_SKI : deriv ? (p->deriv->kind == GP_MATERN52 ? PC_KIND_M52GRAD : PC_KIND_DERIV) : kron_terms ? PC_KIND_KRON_TERMS : kron_obs ? PC_KIND_KRON_OBS : tasks ? PC_KIND_TASK : add ? PC_KIND_ADDITIVE : spec ? PC_KIND_SPECTRAL : p->kind) {
       case PC_KIND_ADDITIVE: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_ADDITIVE>; break;
@@ -1066,6 +1077,18 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
       case PC_KIND_SKI: fn1 = (const void*)pc_persistent1_kernel<PC_KIND_SKI>; break;
       default: fn1 = (const void*)pc_persistent1_kernel<GP_MATERN52>; break;
     }
+    // The column cache keeps ncache = min(rank, what fits) steps of each thread's first row: all of them up to rank 144 (at a
+    // pivot row of up to 108 floats), a multiple of 4 beyond, where the kernel reads the later steps from Lt.
+    int optin = 0;
+    GP_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device));
+    cudaFuncAttributes fa;
+    GP_CUDA(cudaFuncGetAttributes(&fa, fn1));
+    const int64_t fixed = (int64_t)sizeof(float) * ((int64_t)dp_total + rank);
+    const int64_t room = (int64_t)optin - (int64_t)fa.sharedSizeBytes - fixed;
+    GP_REQUIRE(room >= 0, GP_E_SHAPE, "pivoted Cholesky: a pivot row of %d floats and rank %d do not fit in shared memory", dp_total, rank);
+    int ncache = (int)std::min<int64_t>(rank, room / ((int64_t)sizeof(float) * PCP_THREADS));
+    if (ncache < rank) ncache &= ~3;
+    const size_t sh = (size_t)fixed + sizeof(float) * (size_t)ncache * PCP_THREADS;
     GP_CUDA(cudaFuncSetAttribute(fn1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
     int per_sm1 = 0;
     GP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm1, fn1, PCP_THREADS, sh));
@@ -1076,7 +1099,7 @@ extern "C" int gp_pivoted_cholesky(gp_plan* p, int rank, float error_tol, float*
     int DPv = dp_total, rk = rank;
     float osv = os_total, tolv = error_tol;
     int64_t nn = n;
-    void* args[] = {(void*)&Z, &DPv, &osv, &Lt, &nn, &rk, &tolv, &diag, &pos, &S, &piv, &part, &tt, &sk};
+    void* args[] = {(void*)&Z, &DPv, &osv, &Lt, &nn, &rk, &ncache, &tolv, &diag, &pos, &S, &piv, &part, &tt, &sk};
     GP_CUDA(cudaLaunchCooperativeKernel(fn1, dim3(grid1), dim3(PCP_THREADS), args, sh, st));
     p->launches += 1;
   } else {

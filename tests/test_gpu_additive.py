@@ -12,6 +12,7 @@ pytestmark = pytest.mark.gpu
 
 import additive_oracle as ao  # noqa: E402
 from oracle import linalg as ol, mll as om  # noqa: E402
+import pivchol_oracle as po  # noqa: E402
 
 KINDS = ["rbf", "matern12", "matern32", "matern52"]
 
@@ -99,19 +100,6 @@ def test_d1_matches_plain_plan_and_m1_matches_kernel_sum(cuda_dev):
 U32 = 2.0 ** -24
 
 
-def _pivot_gaps(diag, L, piv):
-    """Per step: the winning residual diagonal minus the best of the other unpivoted candidates (fp64)."""
-    res = diag.clone()
-    done = torch.zeros(diag.numel(), dtype=torch.bool)
-    gaps = []
-    for m, pm in enumerate(piv.tolist()):
-        top2 = torch.topk(res.masked_fill(done, -math.inf), 2).values
-        gaps.append(float(top2[0] - top2[1]))
-        done[pm] = True
-        res = res - L[:, m] ** 2
-    return gaps
-
-
 @pytest.mark.parametrize("kind", KINDS)
 def test_pivots_match_fp64_oracle(cuda_dev, kind):
     """PC_KIND_ADDITIVE entries: the same pivot sequence as the fp64 greedy pivoting of the dense operator.  Step 0 is a tie of the
@@ -124,7 +112,7 @@ def test_pivots_match_fp64_oracle(cuda_dev, kind):
     kd = ao.esym_sum([torch.tensor(s, dtype=torch.float64) for s in sc], M).item()
     diag32 = torch.full((n,), float(torch.tensor(kd, dtype=torch.float32)), dtype=torch.float64)
     L, piv_o = ol.pivoted_cholesky(diag32, lambda i: K[i], rank)
-    gaps = _pivot_gaps(diag32, L, piv_o)
+    gaps = po.pivot_gaps(diag32, L, piv_o)
     assert gaps[0] == 0.0 and min(gaps[1:]) > 2 ** 4 * (rank + 1) * U32 * kd
     p = _plan(cuda_dev, kind, x, None, ls, sc, M, noise=0.1)
     lt, piv, st = p.pivoted_cholesky(rank, 1e-3)

@@ -182,14 +182,19 @@ def test_pivoted_cholesky_stops_on_tolerance(Plan, cuda_dev):
 
 def test_pivoted_cholesky_persistent_and_stepwise_paths_agree(Plan, cuda_dev, monkeypatch):
     """The cooperative single-launch kernel and the one-launch-per-step fallback run the same arithmetic per entry:
-    identical pivots and bit-identical factors (also with more rows than resident threads: grid-stride path)."""
-    for n, d, kind, rank in ((5000, 6, "rbf", 60), (3001, 3, "matern32", 25)):
+    identical pivots and bit-identical factors, also with more rows than resident threads (the grid-stride rows of n =
+    2 * 5 * 384 * SMs + 1 read L back from global memory) and at rank 200, past the shared-memory column cache."""
+    sms = torch.cuda.get_device_properties(cuda_dev).multi_processor_count
+    for n, d, kind, rank, tol in ((5000, 6, "rbf", 60, 1e-4), (3001, 3, "matern32", 25, 1e-4),
+                                  (2 * 5 * 384 * sms + 1, 3, "rbf", 100, 0.0), (20000, 4, "matern52", 200, 0.0)):
         x, _ = om.synthetic_problem(n, d, 0, torch.float32)
         p = Plan(x.to(cuda_dev)).set_hypers(kind, 0.8, 1.3, 0.1)
         monkeypatch.delenv("GP_PC_STEPWISE", raising=False)
-        lt1, piv1, _ = p.pivoted_cholesky(rank, 1e-4)
+        lt1, piv1, _ = p.pivoted_cholesky(rank, tol)
+        if tol == 0.0:   # the grid-stride rows and the steps past the column cache were all reached
+            assert lt1.size(0) == rank
         monkeypatch.setenv("GP_PC_STEPWISE", "1")
-        lt2, piv2, _ = p.pivoted_cholesky(rank, 1e-4)
+        lt2, piv2, _ = p.pivoted_cholesky(rank, tol)
         monkeypatch.delenv("GP_PC_STEPWISE", raising=False)
         assert piv1.cpu().tolist() == piv2.cpu().tolist()
         assert torch.equal(lt1, lt2)

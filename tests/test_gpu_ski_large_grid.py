@@ -22,7 +22,8 @@ pytestmark = pytest.mark.gpu
 import ski_large_grid_oracle as lo  # noqa: E402
 import ski_scale_oracle as so  # noqa: E402
 from oracle import linalg as ol  # noqa: E402
-from test_gpu_ski_precond import _pivot_gaps, dense64, interp_and_factors, pow2_points  # noqa: E402
+from test_gpu_ski_precond import dense64, interp_and_factors, pow2_points  # noqa: E402
+import pivchol_oracle as po  # noqa: E402
 
 U = 2.0 ** -24
 NOISE = 0.1
@@ -200,7 +201,7 @@ def test_entries_and_pivoted_cholesky(cuda_dev, sizes, kind, ls, n):
     assert st == 0 and torch.isfinite(lt).all()
     L64, piv64 = ol.pivoted_cholesky(dg, lambda i: p.rows(torch.tensor([i], device=cuda_dev)).double().cpu()[0], k, 0.0)
     mdg = float(dg.max())
-    if min(_pivot_gaps(dg, L64, piv64)) > 2 ** 4 * (k + 1) * U * mdg:   # no near-tie: the fp64 pivoting is the device's
+    if min(po.pivot_gaps(dg, L64, piv64)) > 2 ** 4 * (k + 1) * U * mdg:   # no near-tie: the fp64 pivoting is the device's
         assert piv.cpu().tolist() == piv64.tolist()
     # L L^T reproduces the operator on the pivot columns, whichever order near-ties took
     pv = piv.cpu()

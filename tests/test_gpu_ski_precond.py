@@ -39,6 +39,7 @@ from oracle import linalg as ol, ski  # noqa: E402
 from test_gpu_ciq_precond import _factor64  # noqa: E402
 from test_gpu_sampling import _sqrt_psd  # noqa: E402
 from test_ski_precond_host import per_dim_interp, separable_diag, toeplitz_factors  # noqa: E402
+import pivchol_oracle as po  # noqa: E402
 
 U32 = 2.0 ** -24
 
@@ -143,20 +144,6 @@ def test_ski_entries_match_fp64(cuda_dev, d, sizes, kind, ls, n):
     p.close()
 
 
-def _pivot_gaps(diag, L, piv):
-    """Per step: the winning residual diagonal minus the best of the others (fp64)."""
-    res = diag.clone()
-    done = torch.zeros(diag.numel(), dtype=torch.bool)
-    gaps = []
-    for m, pm in enumerate(piv.tolist()):
-        cand = res.masked_fill(done, -math.inf)
-        top2 = torch.topk(cand, 2).values
-        gaps.append(float(top2[0] - top2[1]))
-        done[pm] = True
-        res = res - L[:, m] ** 2
-    return gaps
-
-
 @pytest.mark.parametrize("d,sizes,kind,ls,n,k,tol,seed", [
     (2, [32, 32], "matern32", 0.25, 600, 15, 1e-3, 2), (3, [16, 12, 10], "matern52", 0.4, 500, 40, 0.0, 7),
     (1, [24], "rbf", 0.3, 1200, 100, 1e-3, 0),          # rank-deficient: prod G_k = 24 < k
@@ -183,7 +170,7 @@ def test_ski_pivoted_cholesky_matches_fp64_pivoting(cuda_dev, d, sizes, kind, ls
         assert float((approx - Kd).abs().max()) <= 1e-3 * mdg
         p.close()
         return
-    gaps = _pivot_gaps(diag, L64, piv64)
+    gaps = po.pivot_gaps(diag, L64, piv64)
     print(f"\nd={d}: rank {lt.size(0)} (fp64 {piv64.numel()}), smallest pivot gap {min(gaps):.3g} x max diag {mdg:.3g}")
     assert min(gaps) > 2 ** 4 * (k + 1) * U32 * mdg
     assert piv.cpu().tolist() == piv64.tolist()
@@ -241,7 +228,7 @@ def test_preconditioned_ski_mll_matches_oracle(cuda_dev):
             outs[dt] = ol.inv_quad_logdet(lambda v: Kt @ v + nz * v, n, y.to(dt), probes, pre, tol, 1000, 20, return_info=True)
         if dt == torch.float64:
             assert pv.tolist() == piv.cpu().tolist()
-            gaps = _pivot_gaps(dg_dev, L, pv)
+            gaps = po.pivot_gaps(dg_dev, L, pv)
             assert min(gaps) > 2 ** 4 * (k + 1) * U32 * float(dg_dev.max())
     (iq64, ld64, info64, _, _), (iq32, ld32, _, _, _) = outs[torch.float64], outs[torch.float32]
     print(f"\niters {info.iters} (oracle {info64.iters}); inv_quad {iq:.6g} / {iq64:.6g}; logdet {ld:.6g} / {ld64:.6g}")

@@ -12,6 +12,7 @@ pytestmark = pytest.mark.gpu
 
 import spectral_oracle as so  # noqa: E402
 from oracle import linalg as ol, mll as om  # noqa: E402
+import pivchol_oracle as po  # noqa: E402
 
 
 def rel(a, b):
@@ -114,18 +115,6 @@ def test_q1_small_mean_matches_rbf_plan(cuda_dev):
     p.close(), q.close()
 
 
-def _pivot_gaps(diag, L, piv):
-    res = diag.clone()
-    done = torch.zeros(diag.numel(), dtype=torch.bool)
-    gaps = []
-    for m, pm in enumerate(piv.tolist()):
-        top2 = torch.topk(res.masked_fill(done, -math.inf), 2).values
-        gaps.append(float(top2[0] - top2[1]))
-        done[pm] = True
-        res = res - L[:, m] ** 2
-    return gaps
-
-
 def test_rows_diag_and_pivots(cuda_dev):
     n, Q, d = 700, 3, 2
     x = _points(n, d, 11)
@@ -150,7 +139,7 @@ def test_rows_diag_and_pivots(cuda_dev):
     diag32 = torch.full((48,), float(torch.tensor(kdp, dtype=torch.float32)), dtype=torch.float64)
     rank = 10
     L, piv_o = ol.pivoted_cholesky(diag32, lambda i: Kp[i], rank)
-    gaps = _pivot_gaps(diag32, L, piv_o)
+    gaps = po.pivot_gaps(diag32, L, piv_o)
     assert gaps[0] == 0.0 and min(gaps[1:]) > 2 * rank * so.entry_bound(xp, xp, wp, mup, vp, S).max().item()
     pp = _plan(cuda_dev, xp, None, wp, mup, vp, S, noise=0.1)
     lt, piv, st = pp.pivoted_cholesky(rank, 1e-3)
