@@ -16,7 +16,7 @@
 //   additive_kmv_kernel       K.V on CUDA cores, partial[split][row][16] like kmv_simt_kernel (finish kernels: scale 1).  D ex2 per
 //                             pair make it MUFU-bound, which tensor cores would not relieve.  M <= 4 compiled as template cases,
 //                             5 <= M <= 8 through the generic recurrence of ADD_MMAX degrees.
-//   additive_krows_kernel / additive_kdiag_cross_kernel   rows and the diagonal of a cross operator
+//   AddEntry                  rows and the diagonal of a cross operator on the shared row kernels (simt_pass.cuh)
 //   additive_bilinear_kernel  one pass over the pairs for the D lengthscale and D component-scale gradients
 #include <math.h>
 #include <string.h>
@@ -24,6 +24,7 @@
 #include <algorithm>
 
 #include "gp_common.cuh"
+#include "simt_pass.cuh"
 
 namespace gp {
 
@@ -91,39 +92,17 @@ additive_kmv_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, 
   }
 }
 
-// ---- rows: OUT[r][j] = K(x1[idx[r]], x2[j]); NaN rows for an index out of range or non-finite inputs (as krows_kernel) ------
+// ---- rows and the diagonal of a cross operator: K(x1_i, x2_j) from two packed rows -----------------------------------------
 template <bool RBF>
-__global__ void additive_krows_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP, const int64_t* __restrict__ idx,
-                                      int64_t n1_local, int64_t n2, const AddHyp h, float* __restrict__ OUT, int64_t ldo,
-                                      const int* __restrict__ xbad) {
-  __shared__ float zi[ADD_DMAX];
-  const int64_t r = blockIdx.y;
-  const int64_t i = idx[r];
-  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 0 || i >= n1_local || *xbad) {
-    if (j < n2) OUT[r * ldo + j] = __int_as_float(0x7fc00000);
-    return;
-  }
-  for (int c = threadIdx.x; c < h.D; c += blockDim.x) zi[c] = Z1[i * DP + c];
-  __syncthreads();
-  if (j >= n2) return;
-  OUT[r * ldo + j] = add_pair<RBF>(h, zi, Z2 + j * DP);
-}
-
-// diagonal of a cross operator (n1 == n2): OUT[i] = K(x1_i, x2_i)
-template <bool RBF>
-__global__ void additive_kdiag_cross_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP, int64_t n, const AddHyp h,
-                                            float* __restrict__ OUT, const int* __restrict__ xbad) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  OUT[i] = *xbad ? __int_as_float(0x7fc00000) : add_pair<RBF>(h, Z1 + i * DP, Z2 + i * DP);
-}
-
-// diagonal of a square operator: the constant sum_m e_m(s), NaN for non-finite inputs
-__global__ void additive_fill_kernel(float* __restrict__ OUT, int64_t n, float v, const int* __restrict__ xbad) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) OUT[i] = *xbad ? __int_as_float(0x7fc00000) : v;
-}
+struct AddEntry {
+  static constexpr bool XBAD = true;
+  const float* Z1;
+  const float* Z2;
+  int64_t ld;   // DP (64-bit: ptxas then keeps both kernels at or below the registers of their former per-family copies)
+  AddHyp h;
+  __host__ __device__ int width() const { return h.D; }
+  __device__ __forceinline__ float entry(const float* za, const float* zb, int64_t, int64_t) const { return add_pair<RBF>(h, za, zb); }
+};
 
 // ---- bilinear derivative: grid (row blocks, column splits, component groups of ADD_G) ---------------------------------------
 // With w_ij = L_i . R_j, dK/dc_q = sum_{m=1}^{M} e_{m-1}(c without c_q) and l dk_q/dl = gpoly_q 2^{e_q} (dcov_poly_exp):
@@ -207,13 +186,7 @@ additive_bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__
 #pragma unroll
   for (int o = 0; o < 2 * ADD_G; ++o) {
     __syncthreads();
-    red[tid] = (double)(o < ADD_G ? gl[o] : gs[o - ADD_G]);
-    __syncthreads();
-    for (int sft = SIMT_TI / 2; sft > 0; sft >>= 1) {
-      if (tid < sft) red[tid] += red[tid + sft];
-      __syncthreads();
-    }
-    if (tid == 0) gout[blk * gstride + grp * 2 * ADD_G + o] = red[0];
+    block_sum_store<SIMT_TI>(red, (double)(o < ADD_G ? gl[o] : gs[o - ADD_G]), gout + blk * gstride + grp * 2 * ADD_G + o);
   }
 }
 
@@ -240,18 +213,14 @@ template <bool RBF, int MT>
 static int add_kmv_dp(gp_plan* p, const AddHyp& h, const float* V16, const int* done_flag) {
   dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)p->nsplit);
   const int64_t cps = p->tiles_per_split * SIMT_TJ;
-#define GP_ADD_CASE(DPV)                                                                                                           \
-  case DPV:                                                                                                                        \
-    additive_kmv_kernel<RBF, MT, DPV><<<grid, SIMT_TI, 0, p->stream>>>(add_z1(p), p->Z2.as<float>(), V16, partial_ptr(p), p->row_count, \
-                                                                       p->n2, p->rows_pad, cps, h, done_flag);                     \
-    break;
-  switch (p->DP) {
-    GP_ADD_CASE(4) GP_ADD_CASE(8) GP_ADD_CASE(12) GP_ADD_CASE(16) GP_ADD_CASE(24) GP_ADD_CASE(32)
-    default:
-      set_error("additive plan: unsupported padded width %d", p->DP);
-      return GP_E_SHAPE;
+  const bool ok = with_width<4, 8, 12, 16, 24, 32>(p->DP, [&](auto w) {
+    additive_kmv_kernel<RBF, MT, decltype(w)::value><<<grid, SIMT_TI, 0, p->stream>>>(add_z1(p), p->Z2.as<float>(), V16, partial_ptr(p),
+                                                                                      p->row_count, p->n2, p->rows_pad, cps, h, done_flag);
+  });
+  if (!ok) {
+    set_error("additive plan: unsupported padded width %d", p->DP);
+    return GP_E_SHAPE;
   }
-#undef GP_ADD_CASE
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -277,44 +246,28 @@ int additive_kmv_launch(gp_plan* p, const float* V16, const int* done_flag) {
 int additive_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   GP_REQUIRE(m <= 65535, GP_E_SHAPE, "rows of an additive plan: at most 65535 rows per call (m=%lld)", (long long)m);
   const AddHyp h = additive_hyp(p);
-  dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
-  if (h.rbf) additive_krows_kernel<true><<<grid, 256, 0, p->stream>>>(add_z1(p), p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, h, OUT, ldo, p->xbad);
-  else additive_krows_kernel<false><<<grid, 256, 0, p->stream>>>(add_z1(p), p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, h, OUT, ldo, p->xbad);
-  p->launches++;
-  GP_CUDA(cudaGetLastError());
-  return GP_OK;
+  if (h.rbf) return launch_krows(p, AddEntry<true>{add_z1(p), p->Z2.as<float>(), p->DP, h}, idx, m, OUT, ldo);
+  return launch_krows(p, AddEntry<false>{add_z1(p), p->Z2.as<float>(), p->DP, h}, idx, m, OUT, ldo);
 }
 
+// square: the constant sum_m e_m(s); cross: per pair.  NaN for non-finite inputs
 int additive_kdiag(gp_plan* p, float* OUT) {
-  if (p->same) {
-    additive_fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, (float)p->add_diag, p->xbad);
-  } else {
-    GP_REQUIRE(p->n1 == p->n2, GP_E_SHAPE, "diagonal of a %lld x %lld cross-covariance is undefined (kernel(x1, x2, diag=True) needs equal sizes)",
-               (long long)p->n1, (long long)p->n2);
-    const AddHyp h = additive_hyp(p);
-    const unsigned g = (unsigned)cdiv(p->n1, 256);
-    if (h.rbf) additive_kdiag_cross_kernel<true><<<g, 256, 0, p->stream>>>(p->Z1.as<float>(), p->Z2.as<float>(), p->DP, p->n1, h, OUT, p->xbad);
-    else additive_kdiag_cross_kernel<false><<<g, 256, 0, p->stream>>>(p->Z1.as<float>(), p->Z2.as<float>(), p->DP, p->n1, h, OUT, p->xbad);
-  }
-  p->launches++;
-  GP_CUDA(cudaGetLastError());
-  return GP_OK;
+  const AddHyp h = additive_hyp(p);
+  const float v = (float)p->add_diag;
+  if (h.rbf) return launch_kdiag(p, OUT, &v, AddEntry<true>{p->Z1.as<float>(), p->Z2.as<float>(), p->DP, h});
+  return launch_kdiag(p, OUT, &v, AddEntry<false>{p->Z1.as<float>(), p->Z2.as<float>(), p->DP, h});
 }
 
 template <bool RBF>
 static int add_bilinear_launch(gp_plan* p, const AddHyp& h, dim3 grid, int64_t cps, const float* L16, const float* R16, double* gout, int gstride) {
-#define GP_ADD_BL_CASE(DPV)                                                                                                      \
-  case DPV:                                                                                                                      \
-    additive_bilinear_kernel<RBF, DPV><<<grid, SIMT_TI, 0, p->stream>>>(add_z1(p), p->Z2.as<float>(), L16, R16, p->row_count, p->n2, \
-                                                                        cps, h, gout, gstride);                                  \
-    break;
-  switch (p->DP) {
-    GP_ADD_BL_CASE(4) GP_ADD_BL_CASE(8) GP_ADD_BL_CASE(12) GP_ADD_BL_CASE(16) GP_ADD_BL_CASE(24) GP_ADD_BL_CASE(32)
-    default:
-      set_error("additive plan: unsupported padded width %d", p->DP);
-      return GP_E_SHAPE;
+  const bool ok = with_width<4, 8, 12, 16, 24, 32>(p->DP, [&](auto w) {
+    additive_bilinear_kernel<RBF, decltype(w)::value><<<grid, SIMT_TI, 0, p->stream>>>(add_z1(p), p->Z2.as<float>(), L16, R16,
+                                                                                       p->row_count, p->n2, cps, h, gout, gstride);
+  });
+  if (!ok) {
+    set_error("additive plan: unsupported padded width %d", p->DP);
+    return GP_E_SHAPE;
   }
-#undef GP_ADD_BL_CASE
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -329,23 +282,10 @@ int additive_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float
   bilinear_split(p, p->n2, &grid, &cps);
   const int64_t nblk = (int64_t)grid.x * grid.y;
   grid.z = (unsigned)ngrp;
-  GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-  double* gout = p->misc.as<double>();
-  double* gsum = gout + nblk * nout;
-  std::vector<double> total(nout, 0.0), hbuf(nout);
-  for (int c0 = 0; c0 < s; c0 += TP) {
-    const int tc = std::min(TP, s - c0);
-    GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-    GP_CHECK(h.rbf ? add_bilinear_launch<true>(p, h, grid, cps, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout)
-                   : add_bilinear_launch<false>(p, h, grid, cps, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout));
-    GP_CHECK(sum_partials_double(p, gout, nblk, nout, nout, gsum));
-    GP_CUDA(cudaMemcpyAsync(hbuf.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-    GP_CUDA(cudaStreamSynchronize(p->stream));
-    for (int o = 0; o < nout; ++o) total[o] += hbuf[o];
-  }
+  std::vector<double> total;
+  GP_CHECK(bilinear_sweep(p, Lf, ldl, Rt, ldr, s, p->row_count, nblk, nout, [&](const float* L16, const float* R16, double* gout) -> int {
+    return h.rbf ? add_bilinear_launch<true>(p, h, grid, cps, L16, R16, gout, nout) : add_bilinear_launch<false>(p, h, grid, cps, L16, R16, gout, nout);
+  }, total));
   for (int c = 0; c < h.D; ++c) {
     const int base = (c / ADD_G) * 2 * ADD_G + c % ADD_G;
     grad_ls[c] = total[base] / (double)p->ls[c];

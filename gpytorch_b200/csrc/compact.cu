@@ -19,6 +19,7 @@
 #include <cub/cub.cuh>
 
 #include "gp_common.cuh"
+#include "simt_pass.cuh"
 
 namespace gp {
 
@@ -307,13 +308,7 @@ pp_bilinear_kernel(PpSched s, const float* __restrict__ L16, const float* __rest
     if (o >= nout) break;
     const double v = o == 0 ? hk : hl[o > 0 ? o - 1 : 0];
     __syncthreads();
-    red[threadIdx.x] = v;
-    __syncthreads();
-    for (int sft = PP_TI / 2; sft > 0; sft >>= 1) {
-      if (threadIdx.x < sft) red[threadIdx.x] += red[threadIdx.x + sft];
-      __syncthreads();
-    }
-    if (threadIdx.x == 0) gout[unit * gstride + o] = red[0];
+    block_sum_store<PP_TI>(red, v, gout + unit * gstride + o);
   }
 }
 
@@ -463,25 +458,12 @@ static int pp_bilinear_launch(gp_plan* p, const PpSched& s, const float* L16, co
 int compact_bilinear_grad(gp_plan* p, const float* L, int64_t ldl, const float* R, int64_t ldr, int s, double* grad_ls, double* grad_os) {
   const bool ard = p->ls.size() > 1;
   const int nout = 1 + (ard ? p->d : 1);
-  const int64_t units = p->compact->ntile_i * p->nparts;
-  GP_CHECK(p->misc.ensure(sizeof(double) * (units * nout + nout)));
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->n1 * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-  double* gout = p->misc.as<double>();
-  double* gsum = gout + units * nout;
   const PpSched sc = pp_sched(p);
-  std::vector<double> total(nout, 0.0), h(nout);
-  for (int c0 = 0; c0 < s; c0 += TP) {
-    const int tc = std::min(TP, s - c0);
-    GP_CHECK(to_v16(p, L + c0, ldl, tc, p->n1, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, R + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-    GP_CHECK(ard ? pp_bilinear_launch<true>(p, sc, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout)
-                 : pp_bilinear_launch<false>(p, sc, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout));
-    GP_CHECK(sum_partials_double(p, gout, units, nout, nout, gsum));   // fixed order; NaN when an input is not finite
-    GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-    GP_CUDA(cudaStreamSynchronize(p->stream));
-    for (int o = 0; o < nout; ++o) total[o] += h[o];
-  }
+  std::vector<double> total;
+  GP_CHECK(bilinear_sweep(p, L, ldl, R, ldr, s, p->n1, p->compact->ntile_i * p->nparts, nout,
+                          [&](const float* L16, const float* R16, double* gout) -> int {
+                            return ard ? pp_bilinear_launch<true>(p, sc, L16, R16, gout, nout) : pp_bilinear_launch<false>(p, sc, L16, R16, gout, nout);
+                          }, total));
   // dk/dl_c = -k'(r) dz_c^2 / (r l_c); one lengthscale: -k'(r) r / l.  Both times S
   *grad_os = total[0];
   if (ard)

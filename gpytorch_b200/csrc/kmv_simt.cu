@@ -7,6 +7,7 @@
 // Reference semantics: LazyEvaluatedKernelTensor._matmul (lazy/lazy_evaluated_kernel_tensor.py:245-276),
 // _getitem (:136-243), _diagonal (:107-133), _bilinear_derivative (:69-105).
 #include "gp_common.cuh"
+#include "simt_pass.cuh"
 #include "ski_rows.cuh"
 
 namespace gp {
@@ -112,29 +113,22 @@ template <int KIND>
 static int launch_simt_kind(gp_plan* p, const SimtLaunch& a, const int* done_flag) {
   int64_t rows_pad = p->rows_pad;
   dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)a.nsplit);
-#define GP_SIMT_CASE(D)                                                                                          \
-  case D:                                                                                                        \
-    if constexpr (KIND == POLY_K)                                                                                \
-      poly_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2,     \
-                                                           rows_pad, a.cps, p->same ? 1 : 0, a.row_begin, done_flag, \
-                                                           cov_param(p));                                        \
-    else if constexpr (KIND == RQ_K)                                                                             \
-      rq_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2,       \
-                                                         rows_pad, a.cps, p->same ? 1 : 0, a.row_begin, done_flag, \
-                                                         cov_param(p));                                          \
-    else                                                                                                         \
-      kmv_simt_kernel<KIND, D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count,      \
-                                                                a.n2, rows_pad, a.cps, p->same ? 1 : 0,          \
-                                                                a.row_begin, done_flag);                         \
-    break;
-  switch (p->DP) {
-    GP_SIMT_CASE(4) GP_SIMT_CASE(8) GP_SIMT_CASE(12) GP_SIMT_CASE(16) GP_SIMT_CASE(24) GP_SIMT_CASE(32)
-    GP_SIMT_CASE(48) GP_SIMT_CASE(64) GP_SIMT_CASE(96) GP_SIMT_CASE(128)
-    default:
-      set_error("unsupported DP=%d", p->DP);
-      return GP_E_SHAPE;
+  const bool ok = with_width<4, 8, 12, 16, 24, 32, 48, 64, 96, 128>(p->DP, [&](auto w) {
+    constexpr int D = decltype(w)::value;
+    if constexpr (KIND == POLY_K)
+      poly_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2, rows_pad, a.cps,
+                                                           p->same ? 1 : 0, a.row_begin, done_flag, cov_param(p));
+    else if constexpr (KIND == RQ_K)
+      rq_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2, rows_pad, a.cps,
+                                                         p->same ? 1 : 0, a.row_begin, done_flag, cov_param(p));
+    else
+      kmv_simt_kernel<KIND, D><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, a.V16, a.partial, p->row_count, a.n2, rows_pad, a.cps,
+                                                                p->same ? 1 : 0, a.row_begin, done_flag);
+  });
+  if (!ok) {
+    set_error("unsupported DP=%d", p->DP);
+    return GP_E_SHAPE;
   }
-#undef GP_SIMT_CASE
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -231,63 +225,46 @@ int kmv_finish_user(gp_plan* p, const float* V16, float* OUT, int64_t ldo, int t
   return GP_OK;
 }
 
-// ---- row extraction: OUT[m][n2] = os * k(x1[idx[r]], x2[j]) -----------------------------------
+// ---- rows and diagonals: os * k(x1_i, x2_j) of one pair of packed rows of width DP ---------------------------------------
 template <int KIND>
-__global__ void krows_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP,
-                             const int64_t* __restrict__ idx, int64_t n1_local, int64_t n2, float os, int same,
-                             int64_t row_begin, float* __restrict__ OUT, int64_t ldo, const int* __restrict__ xbad, CovParam cp) {
-  extern __shared__ float zi[];
-  const int64_t r = blockIdx.y;
-  const int64_t i = idx[r];
-  // out-of-range row index (CTA-uniform): NaN row instead of an out-of-bounds read.  Non-finite inputs: every entry is NaN in
-  // the reference (mean-centring spreads it), while cov_from_arg's clamps would turn it into the constant outputscale
-  if (i < 0 || i >= n1_local || *xbad) {
-    int64_t jj = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (jj < n2) OUT[r * ldo + jj] = __int_as_float(0x7fc00000);
-    return;
-  }
-  for (int c = threadIdx.x; c < DP; c += blockDim.x) zi[c] = Z1[i * DP + c];
-  __syncthreads();
-  int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n2) return;
-  float a;
-  if constexpr (is_poly_code(KIND)) {
-    a = poly_arg(zi, Z2 + j * DP, DP, cp.offset);
-  } else {
-    float s = 0.f;
-    for (int c = 0; c < DP; ++c) {
-      float df = zi[c] - Z2[j * DP + c];
-      s = fmaf(df, df, s);
+struct PlainEntry {
+  static constexpr bool XBAD = false;
+  const float* Z1;
+  const float* Z2;
+  int ld;   // DP
+  float os;
+  int same;
+  int64_t row_begin;
+  CovParam cp;
+  __host__ __device__ int width() const { return ld; }
+  __device__ __forceinline__ float entry(const float* za, const float* zb, int64_t i, int64_t j) const {
+    float a;
+    if constexpr (is_poly_code(KIND)) {   // also the square diagonal S (|x_i|^2 + c)^p (Z1 = Z2)
+      a = poly_arg(za, zb, ld, cp.offset);
+    } else {
+      float s = 0.f;
+      for (int c = 0; c < ld; ++c) {
+        float df = za[c] - zb[c];
+        s = fmaf(df, df, s);
+      }
+      a = -0.5f * s;
+      if (same && (i + row_begin) == j) a = 0.f;
     }
-    a = -0.5f * s;
-    if (same && (i + row_begin) == j) a = 0.f;
+    return os * cov_from_arg<KIND>(a, cp);
   }
-  OUT[r * ldo + j] = os * cov_from_arg<KIND>(a, cp);
-}
+};
 
-// diagonal of a cross-covariance K(x1, x2) (n1 == n2): OUT[i] = os * k(x1_i, x2_i)   (kernel(x1, x2, diag=True),
-// lazy_evaluated_kernel_tensor.py:107-133 / kernels/kernel.py:307-352 with diag=True)
-template <int KIND>
-__global__ void kdiag_cross_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int DP, int64_t n, float os,
-                                   float* __restrict__ OUT, CovParam cp) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+template <bool XB>
+__global__ void fill_kernel(float* __restrict__ OUT, int64_t n, float v, const int* __restrict__ xbad) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  if constexpr (is_poly_code(KIND)) {   // also the square diagonal S (|x_i|^2 + c)^p (Z1 = Z2)
-    OUT[i] = os * cov_from_arg<KIND>(poly_arg(Z1 + i * DP, Z2 + i * DP, DP, cp.offset), cp);
-    return;
-  }
-  float s = 0.f;
-  for (int c = 0; c < DP; ++c) {
-    float df = Z1[i * DP + c] - Z2[i * DP + c];
-    s = fmaf(df, df, s);
-  }
-  OUT[i] = os * cov_from_arg<KIND>(-0.5f * s, cp);
+  if constexpr (XB)
+    OUT[i] = *xbad ? __int_as_float(0x7fc00000) : v;
+  else
+    OUT[i] = v;
 }
-
-__global__ void fill_kernel(float* __restrict__ p, int64_t n, float v) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = v;
-}
+template __global__ void fill_kernel<false>(float* __restrict__, int64_t, float, const int* __restrict__);
+template __global__ void fill_kernel<true>(float* __restrict__, int64_t, float, const int* __restrict__);
 
 // the diagonal of a square kernel sum with a polynomial term, term by term in term order: OUT[i] (+)= os_t k_t(x_i, x_i), the
 // constant os_t for a stationary term, os_t (|x_i|^2 + c_t)^p_t for a polynomial one (Z: its packed rows)
@@ -383,13 +360,7 @@ bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, cons
     }
     if (RQ && o == 1 + nls) v = ga;   // after the loop: an ARD thread holds DP >= d + 1 (padding) accumulators
     __syncthreads();
-    red[tid] = (double)v;
-    __syncthreads();
-    for (int sft = SIMT_TI / 2; sft > 0; sft >>= 1) {
-      if (tid < sft) red[tid] += red[tid + sft];
-      __syncthreads();
-    }
-    if (tid == 0) gout[blk * gstride + o] = red[0];
+    block_sum_store<SIMT_TI>(red, (double)v, gout + blk * gstride + o);
   }
 }
 
@@ -414,13 +385,7 @@ __global__ void bilin_dot_kernel(const float* __restrict__ partial, int nsplit, 
     for (int sp = 0; sp < nsplit; ++sp) s += partial[(int64_t)sp * rows_pad * TP + e];
     acc += (double)L16[e] * (double)s;
   }
-  red[threadIdx.x] = acc;
-  __syncthreads();
-  for (int sft = 128; sft > 0; sft >>= 1) {
-    if (threadIdx.x < sft) red[threadIdx.x] += red[threadIdx.x + sft];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) gout[(int64_t)blockIdx.x * gstride + o] = red[0];
+  block_sum_store<256>(red, acc, gout + (int64_t)blockIdx.x * gstride + o);
 }
 
 int sum_partials_double(gp_plan* p, const double* in, int64_t nblk, int stride, int nout, double* out) {
@@ -439,15 +404,11 @@ struct BilinLaunch {
 template <int KIND, bool ARD>
 static int launch_bilinear(gp_plan* p, const BilinLaunch& a, const float* L16, const float* R16, double* gout, int gstride, dim3 grid,
                            int64_t cps) {
-#define GP_BL_CASE(D)                                                                                              \
-  case D:                                                                                                          \
-    bilinear_kernel<KIND, D, ARD><<<grid, SIMT_TI, 0, p->stream>>>(a.Z1, a.Z2, L16, R16, p->row_count, a.n2, cps,  \
-                                                                   p->same ? 1 : 0, a.row_begin, p->d, gout, gstride, cov_param(p)); \
-    break;
-  switch (p->DP) {   // DP <= 64: gp_bilinear_grad refuses wider plans before any launch
-    GP_BL_CASE(4) GP_BL_CASE(8) GP_BL_CASE(12) GP_BL_CASE(16) GP_BL_CASE(24) GP_BL_CASE(32) GP_BL_CASE(48) GP_BL_CASE(64)
-  }
-#undef GP_BL_CASE
+  // DP <= 64: gp_bilinear_grad refuses wider plans before any launch
+  with_width<4, 8, 12, 16, 24, 32, 48, 64>(p->DP, [&](auto w) {
+    bilinear_kernel<KIND, decltype(w)::value, ARD><<<grid, SIMT_TI, 0, p->stream>>>(
+        a.Z1, a.Z2, L16, R16, p->row_count, a.n2, cps, p->same ? 1 : 0, a.row_begin, p->d, gout, gstride, cov_param(p));
+  });
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -472,6 +433,20 @@ static int launch_bilinear_any(gp_plan* p, const BilinLaunch& a, const float* L1
     case GP_RQ: return launch_bilinear<RQ_K, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
     case GP_POLY: return launch_bilinear<POLY_K, false>(p, a, L16, R16, gout, gstride, grid, cps);
     default: return launch_bilinear<GP_MATERN52, ARD>(p, a, L16, R16, gout, gstride, grid, cps);
+  }
+}
+
+// f(std::integral_constant<int, KIND>()) for the covariance code of a plain plan's rows and diagonal
+template <class F>
+static void with_plain_kind(int kind, F&& f) {
+  switch (kind) {
+    case GP_RBF: return f(std::integral_constant<int, GP_RBF>());
+    case GP_MATERN12: return f(std::integral_constant<int, GP_MATERN12>());
+    case GP_MATERN32: return f(std::integral_constant<int, GP_MATERN32>());
+    case GP_RQ: return f(std::integral_constant<int, RQ_K>());
+    case GP_POLY: return f(std::integral_constant<int, POLY_K>());
+    case GP_PPOLY: return f(std::integral_constant<int, PP_K>());
+    default: return f(std::integral_constant<int, GP_MATERN52>());
   }
 }
 
@@ -539,23 +514,12 @@ static int krows_base(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int
   if (p->add_M) return additive_krows(p, idx, m, OUT, ldo);
   if (p->sm_Q) return spectral_krows(p, idx, m, OUT, ldo);
   const float* Z1 = p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>();
-  dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
-  size_t sh = sizeof(float) * p->DP;
-  const CovParam cp = cov_param(p);
-#define GP_KROWS(KK) krows_kernel<KK><<<grid, 256, sh, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, p->outputscale, p->same, p->row_begin, OUT, ldo, p->xbad, cp)
-  switch (p->kind) {
-    case GP_RBF: GP_KROWS(GP_RBF); break;
-    case GP_MATERN12: GP_KROWS(GP_MATERN12); break;
-    case GP_MATERN32: GP_KROWS(GP_MATERN32); break;
-    case GP_RQ: GP_KROWS(RQ_K); break;
-    case GP_POLY: GP_KROWS(POLY_K); break;
-    case GP_PPOLY: GP_KROWS(PP_K); break;
-    default: GP_KROWS(GP_MATERN52); break;
-  }
-#undef GP_KROWS
-  p->launches++;
-  GP_CUDA(cudaGetLastError());
-  return GP_OK;
+  int st = GP_OK;
+  with_plain_kind(p->kind, [&](auto k) {
+    const PlainEntry<decltype(k)::value> src{Z1, p->Z2.as<float>(), p->DP, p->outputscale, p->same, p->row_begin, cov_param(p)};
+    st = launch_krows(p, src, idx, m, OUT, ldo);
+  });
+  return st;
 }
 
 static int kdiag_base(gp_plan* p, float* OUT);
@@ -576,7 +540,7 @@ extern "C" int gp_kdiag(gp_plan* p, float* OUT) {
       // a low-rank plan is square: every stationary term contributes its constant outputscale, added in term order
       float os = 0.f;
       for (gp_plan* t : p->terms) os += t->outputscale;
-      fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, os);
+      fill_kernel<false><<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, os, nullptr);
       p->launches++;
     } else {
       GP_CHECK(kdiag_base(p, OUT));
@@ -591,36 +555,18 @@ static int kdiag_base(gp_plan* p, float* OUT) {
   if (p->backend == GP_BACKEND_SKI) return ski_kdiag(p, OUT);   // not constant: w_i^T K_uu w_i (ski_rows.cuh)
   if (p->add_M) return additive_kdiag(p, OUT);   // square: the constant sum_m e_m(s); cross: per pair
   if (p->sm_Q) return spectral_kdiag(p, OUT);    // square: the constant S (sum_q w_q)^d; cross: per pair
-  if (p->same && p->kind == GP_POLY) {
-    // a dot-product kernel: S (|x_i|^2 + c)^p, row by row
+  if (p->same && p->kind == GP_POLY) {   // a dot-product kernel: S (|x_i|^2 + c)^p, row by row
     const float* Z = p->Z2.as<float>() + p->row_begin * p->DP;
-    kdiag_cross_kernel<POLY_K><<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(Z, Z, p->DP, p->row_count, p->outputscale,
-                                                                                        OUT, cov_param(p));
-  } else if (p->same) {
-    // stationary kernels: k(x,x) = outputscale (lazy_evaluated_kernel_tensor.py:107-133 evaluates kernel(diag=True))
-    fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, p->outputscale);
-  } else {
-    GP_REQUIRE(p->n1 == p->n2, GP_E_SHAPE, "diagonal of a %lld x %lld cross-covariance is undefined (kernel(x1, x2, diag=True) needs equal sizes)",
-               (long long)p->n1, (long long)p->n2);
-    const unsigned g = (unsigned)cdiv(p->n1, 256);
-    const float* Z1 = p->Z1.as<float>();
-    const float* Z2 = p->Z2.as<float>();
-    const CovParam cp = cov_param(p);
-#define GP_KDIAG(KK) kdiag_cross_kernel<KK><<<g, 256, 0, p->stream>>>(Z1, Z2, p->DP, p->n1, p->outputscale, OUT, cp)
-    switch (p->kind) {
-      case GP_RBF: GP_KDIAG(GP_RBF); break;
-      case GP_MATERN12: GP_KDIAG(GP_MATERN12); break;
-      case GP_MATERN32: GP_KDIAG(GP_MATERN32); break;
-      case GP_RQ: GP_KDIAG(RQ_K); break;
-      case GP_POLY: GP_KDIAG(POLY_K); break;
-      case GP_PPOLY: GP_KDIAG(PP_K); break;
-      default: GP_KDIAG(GP_MATERN52); break;
-    }
-#undef GP_KDIAG
+    return launch_kdiag(p, OUT, nullptr, PlainEntry<POLY_K>{Z, Z, p->DP, p->outputscale, 0, 0, cov_param(p)});
   }
-  p->launches++;
-  GP_CUDA(cudaGetLastError());
-  return GP_OK;
+  // stationary kernels: k(x,x) = outputscale on a square plan (lazy_evaluated_kernel_tensor.py:107-133 evaluates
+  // kernel(diag=True)), per pair on a cross plan
+  int st = GP_OK;
+  with_plain_kind(p->kind, [&](auto k) {
+    const PlainEntry<decltype(k)::value> src{p->Z1.as<float>(), p->Z2.as<float>(), p->DP, p->outputscale, 0, 0, cov_param(p)};
+    st = launch_kdiag(p, OUT, &p->outputscale, src);
+  });
+  return st;
 }
 
 extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float* Rt, int64_t ldr, int s,
@@ -646,14 +592,8 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   if (p->backend == GP_BACKEND_SKI) {
     // interpolated operator: everything happens on the grid (ski.cu); one sweep per 16 columns
     std::vector<double> tot(1 + p->d, 0.0);
-    GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-    GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-    for (int c0 = 0; c0 < s; c0 += TP) {
-      const int tc = std::min(TP, s - c0);
-      GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-      GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-      GP_CHECK(ski_bilinear(p, p->misc2.as<float>(), p->misc3.as<float>(), tot.data()));
-    }
+    GP_CHECK(v16_chunks(p, Lf, ldl, Rt, ldr, s, p->row_count,
+                        [&](const float* L16, const float* R16) { return ski_bilinear(p, L16, R16, tot.data()); }));
     *grad_os = tot[0];
     if (ard) {
       for (int c = 0; c < p->d; ++c) grad_ls[c] = p->outputscale * tot[1 + c] / (double)p->ls[c];
@@ -672,63 +612,36 @@ extern "C" int gp_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const 
   std::vector<double> total(nout, 0.0);
   if (p->tasks && (ard || p->backend != GP_BACKEND_TCGEN05)) {
     // K o B on the SIMT derivative kernel: one pass per column task with B folded into the rows (tasks.cu)
-    GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-    GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-    for (int c0 = 0; c0 < s; c0 += TP) {
-      const int tc = std::min(TP, s - c0);
-      GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-      GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-      GP_CHECK(tasks_bilinear(p, p->misc2.as<float>(), p->misc3.as<float>(), ard, total));
-    }
+    GP_CHECK(v16_chunks(p, Lf, ldl, Rt, ldr, s, p->row_count,
+                        [&](const float* L16, const float* R16) { return tasks_bilinear(p, L16, R16, ard, total); }));
+  } else if (!ard && p->backend == GP_BACKEND_TCGEN05) {
+    // scalar lengthscale on the tensor-core backend: sum_ij (L_i . R_j) f_ij = sum_i L_i . (F R)_i, i.e. two launches of
+    // the fused K.V kernel (f = k, then f = g = l dk/dl through the derivative kinds) + a dot product with L; an RQ plan adds a
+    // third (f = dk/dalpha).  ARD needs d weighted sums per pair and stays on the SIMT kernel.
+    const int dot_blocks = (int)std::min<int64_t>(bilinear_blocks(p, p->n2), 2 * p->n_sm);
+    GP_CHECK(bilinear_sweep(p, Lf, ldl, Rt, ldr, s, p->row_count, dot_blocks, nout, [&](const float* L16, const float* R16, double* gout) -> int {
+      if (!p->tasks) GP_CHECK(pack_v_tiles(p, R16));
+      for (int pass = 0; pass < nout; ++pass) {
+        const int kind = pass == 0 ? p->kind : poly ? POLY_DC : !rq ? GP_DERIV + p->kind : pass == 1 ? RQ_DL : RQ_DA;
+        // a multitask plan runs both passes on K o B (tasks.cu), combined into slot 0 in user row order
+        GP_CHECK(p->tasks ? tasks_kmv_partials(p, R16, kind, nullptr) : kmv_tc_launch_kind(p, kind, nullptr));
+        bilin_dot_kernel<<<dot_blocks, 256, 0, p->stream>>>(p->partial.as<float>(), p->nparts, p->row_count, p->rows_pad, L16, gout, nout,
+                                                            pass);
+        p->launches++;
+      }
+      GP_CUDA(cudaGetLastError());
+      return GP_OK;
+    }, total));
   } else {
     dim3 grid;
     int64_t cps;
     bilinear_split(p, p->n2, &grid, &cps);
-    int64_t nblk = (int64_t)grid.x * grid.y;
-    GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
-    GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-    GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-    double* gout = p->misc.as<double>();
-    double* gsum = gout + nblk * nout;
-    // scalar lengthscale on the tensor-core backend: sum_ij (L_i . R_j) f_ij = sum_i L_i . (F R)_i, i.e. two launches of
-    // the fused K.V kernel (f = k, then f = g = l dk/dl through the derivative kinds) + a dot product with L; an RQ plan adds a
-    // third (f = dk/dalpha).  ARD needs d weighted sums per pair and stays on the SIMT kernel.
-    const bool use_tc = !ard && p->backend == GP_BACKEND_TCGEN05;
-    const int64_t rows_pad = p->rows_pad;
-    const int dot_blocks = (int)std::min<int64_t>(nblk, 2 * p->n_sm);
-    for (int c0 = 0; c0 < s; c0 += TP) {
-      int tc = std::min(TP, s - c0);
-      GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-      GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-      if (use_tc) {
-        if (!p->tasks) GP_CHECK(pack_v_tiles(p, p->misc3.as<float>()));
-        for (int pass = 0; pass < nout; ++pass) {
-          const int kind = pass == 0 ? p->kind : poly ? POLY_DC : !rq ? GP_DERIV + p->kind : pass == 1 ? RQ_DL : RQ_DA;
-          // a multitask plan runs both passes on K o B (tasks.cu), combined into slot 0 in user row order
-          GP_CHECK(p->tasks ? tasks_kmv_partials(p, p->misc3.as<float>(), kind, nullptr) : kmv_tc_launch_kind(p, kind, nullptr));
-          bilin_dot_kernel<<<dot_blocks, 256, 0, p->stream>>>(p->partial.as<float>(), p->nparts, p->row_count, rows_pad,
-                                                              p->misc2.as<float>(), gout, nout, pass);
-          p->launches++;
-        }
-        GP_CUDA(cudaGetLastError());
-        sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, dot_blocks, nout, nout, gsum, p->xbad);
-        p->launches++;
-        std::vector<double> h(nout);
-        GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-        GP_CUDA(cudaStreamSynchronize(p->stream));
-        for (int o = 0; o < nout; ++o) total[o] += h[o];
-        continue;
-      }
-      const BilinLaunch a{p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>(), p->Z2.as<float>(), p->n2, p->row_begin};
-      GP_CHECK(ard ? launch_bilinear_any<true>(p, a, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout, grid, cps)
-                   : launch_bilinear_any<false>(p, a, p->misc2.as<float>(), p->misc3.as<float>(), gout, nout, grid, cps));
-      sum_partials_double_kernel<<<(unsigned)cdiv(nout, 64), 64, 0, p->stream>>>(gout, nblk, nout, nout, gsum, p->xbad);
-      p->launches++;
-      std::vector<double> h(nout);
-      GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-      GP_CUDA(cudaStreamSynchronize(p->stream));
-      for (int o = 0; o < nout; ++o) total[o] += h[o];
-    }
+    const BilinLaunch a{p->same ? p->Z2.as<float>() + p->row_begin * p->DP : p->Z1.as<float>(), p->Z2.as<float>(), p->n2, p->row_begin};
+    GP_CHECK(bilinear_sweep(p, Lf, ldl, Rt, ldr, s, p->row_count, (int64_t)grid.x * grid.y, nout,
+                            [&](const float* L16, const float* R16, double* gout) -> int {
+                              return ard ? launch_bilinear_any<true>(p, a, L16, R16, gout, nout, grid, cps)
+                                         : launch_bilinear_any<false>(p, a, L16, R16, gout, nout, grid, cps);
+                            }, total));
   }
   // d/d outputscale of os*k = k ; d/dl: scalar -> sum w g / l ; ARD -> sum w g dz_c^2/s / l_c ; both times os
   *grad_os = total[0];

@@ -28,6 +28,7 @@
 #include <algorithm>
 
 #include "gp_common.cuh"
+#include "simt_pass.cuh"
 
 namespace gp {
 
@@ -143,13 +144,7 @@ periodic_bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__
 #pragma unroll
   for (int o = 0; o < NO; ++o) {
     __syncthreads();
-    red[tid] = acc[o];
-    __syncthreads();
-    for (int sft = SIMT_TI / 2; sft > 0; sft >>= 1) {
-      if (tid < sft) red[tid] += red[tid + sft];
-      __syncthreads();
-    }
-    if (tid == 0) gout[blk * gstride + blockIdx.z * NO + o] = red[0];
+    block_sum_store<SIMT_TI>(red, acc[o], gout + blk * gstride + blockIdx.z * NO + o);
   }
 }
 
@@ -210,40 +205,23 @@ int periodic_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float
   bilinear_split(p, p->n2, &grid, &cps);
   const int64_t nblk = (int64_t)grid.x * grid.y;
   grid.z = (unsigned)ngrp;
-  GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-  double* gout = p->misc.as<double>();
-  double* gsum = gout + nblk * nout;
-  std::vector<double> total(nout, 0.0), hbuf(nout);
   const float* Z1 = p->same ? p->Z2.as<float>() : p->Z1.as<float>();
   const float* X2 = p->same ? p->X1 : p->X2;
   const int64_t ld2 = p->same ? p->ld1 : p->ld2;
-  for (int c0 = 0; c0 < s; c0 += TP) {
-    const int tc = std::min(TP, s - c0);
-    GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-#define GP_PER_BL(DV)                                                                                                          \
-  case DV:                                                                                                                     \
-    periodic_bilinear_kernel<DV><<<grid, SIMT_TI, 0, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, p->X1, p->ld1, X2, ld2,      \
-                                                                  p->misc2.as<float>(), p->misc3.as<float>(), p->row_count,  \
-                                                                  p->n2, cps, gout, nout);                                   \
-    break;
-    switch (d) {
-      GP_PER_BL(1) GP_PER_BL(2) GP_PER_BL(3) GP_PER_BL(4) GP_PER_BL(5) GP_PER_BL(6) GP_PER_BL(7) GP_PER_BL(8)
-      GP_PER_BL(9) GP_PER_BL(10) GP_PER_BL(11) GP_PER_BL(12) GP_PER_BL(13) GP_PER_BL(14) GP_PER_BL(15) GP_PER_BL(16)
-      default:
-        set_error("periodic plan: no compiled case for d=%d", d);
-        return GP_E_SHAPE;
+  std::vector<double> total;
+  GP_CHECK(bilinear_sweep(p, Lf, ldl, Rt, ldr, s, p->row_count, nblk, nout, [&](const float* L16, const float* R16, double* gout) -> int {
+    const bool ok = with_width<1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16>(d, [&](auto w) {
+      periodic_bilinear_kernel<decltype(w)::value><<<grid, SIMT_TI, 0, p->stream>>>(Z1, p->Z2.as<float>(), p->DP, p->X1, p->ld1, X2, ld2,
+                                                                                     L16, R16, p->row_count, p->n2, cps, gout, nout);
+    });
+    if (!ok) {
+      set_error("periodic plan: no compiled case for d=%d", d);
+      return GP_E_SHAPE;
     }
-#undef GP_PER_BL
     p->launches++;
     GP_CUDA(cudaGetLastError());
-    GP_CHECK(sum_partials_double(p, gout, nblk, nout, nout, gsum));
-    GP_CUDA(cudaMemcpyAsync(hbuf.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-    GP_CUDA(cudaStreamSynchronize(p->stream));
-    for (int o = 0; o < nout; ++o) total[o] += hbuf[o];
-  }
+    return GP_OK;
+  }, total));
   const double S = p->outputscale;
   const int nls = (int)p->ls.size();
   for (int c = 0; c < nls; ++c) grad_ls[c] = 0.0;

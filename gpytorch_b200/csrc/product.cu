@@ -21,6 +21,7 @@
 #include <algorithm>
 
 #include "gp_common.cuh"
+#include "simt_pass.cuh"
 
 namespace gp {
 
@@ -232,13 +233,7 @@ product_bilinear_kernel(const ProdFactors pf, const float* __restrict__ L16, con
         if (c == o - 1) v = gl[c];
     }
     __syncthreads();
-    red[tid] = (double)v;
-    __syncthreads();
-    for (int sft = SIMT_TI / 2; sft > 0; sft >>= 1) {
-      if (tid < sft) red[tid] += red[tid + sft];
-      __syncthreads();
-    }
-    if (tid == 0) gout[blk * (1 + DPT) + o] = red[0];
+    block_sum_store<SIMT_TI>(red, (double)v, gout + blk * (1 + DPT) + o);
   }
 }
 
@@ -340,16 +335,10 @@ int product_kmv_launch(gp_plan* p, const float* V16, const int* done_flag) {
   const ProdFactors pf = prod_factors(p);
   dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)p->nsplit);
   const int64_t cps = p->tiles_per_split * SIMT_TJ;
-#define GP_PROD_SIMT_CASE(D)                                                                                                      \
-  case D:                                                                                                                         \
-    product_simt_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(pf, V16, p->partial.as<float>(), p->row_count, p->n2, p->rows_pad, cps, \
-                                                            p->same ? 1 : 0, p->row_begin, done_flag);                            \
-    break;
-  switch (round_dpt(p->DP)) {
-    GP_PROD_SIMT_CASE(8) GP_PROD_SIMT_CASE(12) GP_PROD_SIMT_CASE(16) GP_PROD_SIMT_CASE(24) GP_PROD_SIMT_CASE(32)
-    GP_PROD_SIMT_CASE(48) GP_PROD_SIMT_CASE(64) GP_PROD_SIMT_CASE(96) GP_PROD_SIMT_CASE(128)
-  }
-#undef GP_PROD_SIMT_CASE
+  with_width<8, 12, 16, 24, 32, 48, 64, 96, 128>(round_dpt(p->DP), [&](auto w) {
+    product_simt_kernel<decltype(w)::value><<<grid, SIMT_TI, 0, p->stream>>>(pf, V16, p->partial.as<float>(), p->row_count, p->n2,
+                                                                             p->rows_pad, cps, p->same ? 1 : 0, p->row_begin, done_flag);
+  });
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -392,30 +381,16 @@ int product_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float*
   int64_t cps;
   bilinear_split(p, p->n2, &grid, &cps);
   const int64_t nblk = (int64_t)grid.x * grid.y;
-  GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-  double* gout = p->misc.as<double>();
-  double* gsum = gout + nblk * nout;
-  std::vector<double> total(nout, 0.0), h(nout);
-  for (int c0 = 0; c0 < s; c0 += TP) {
-    const int tc = std::min(TP, s - c0);
-    GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-#define GP_PROD_BL_CASE(D)                                                                                                          \
-  case D:                                                                                                                           \
-    product_bilinear_kernel<D><<<grid, SIMT_TI, 0, p->stream>>>(pf, p->misc2.as<float>(), p->misc3.as<float>(), p->row_count, p->n2, \
-                                                                cps, p->same ? 1 : 0, p->row_begin, gout);                          \
-    break;
-    switch (DPT) { GP_PROD_BL_CASE(8) GP_PROD_BL_CASE(12) GP_PROD_BL_CASE(16) GP_PROD_BL_CASE(24) GP_PROD_BL_CASE(32) GP_PROD_BL_CASE(48) GP_PROD_BL_CASE(64) }
-#undef GP_PROD_BL_CASE
+  std::vector<double> total;
+  GP_CHECK(bilinear_sweep(p, Lf, ldl, Rt, ldr, s, p->row_count, nblk, nout, [&](const float* L16, const float* R16, double* gout) -> int {
+    with_width<8, 12, 16, 24, 32, 48, 64>(DPT, [&](auto w) {
+      product_bilinear_kernel<decltype(w)::value><<<grid, SIMT_TI, 0, p->stream>>>(pf, L16, R16, p->row_count, p->n2, cps,
+                                                                                   p->same ? 1 : 0, p->row_begin, gout);
+    });
     p->launches++;
     GP_CUDA(cudaGetLastError());
-    GP_CHECK(sum_partials_double(p, gout, nblk, nout, nout, gsum));
-    GP_CUDA(cudaMemcpyAsync(h.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-    GP_CUDA(cudaStreamSynchronize(p->stream));
-    for (int o = 0; o < nout; ++o) total[o] += h[o];
-  }
+    return GP_OK;
+  }, total));
   // dF/dS = sum w prod k ; d/dl_f: S times the factor's column sums over its lengthscale(s)
   *grad_os = total[0];
   int off = 1, g = 0;

@@ -19,7 +19,7 @@
 //                              Q d ex2 and Q d cos of the reduced phase difference, Q d FMAs into the d mixtures, d - 1 products and
 //                              16 FMAs.  2 Q d MUFU operations per pair make it bound by the special-function unit; tensor cores
 //                              would not change that count.  Template cases: d exact (1 .. 8), Q up to QM in {1, 4, min(16, 32/d)}.
-//   spectral_krows_kernel / spectral_kdiag_cross_kernel   rows and the diagonal of a cross operator (runtime Q, d)
+//   SmEntry                    rows and the diagonal of a cross operator (runtime Q, d) on the shared row kernels (simt_pass.cuh)
 //   spectral_bilinear_kernel   one pass over the pairs for the Q (1 + 2d) parameter gradients and dF/dS; fp64 accumulators,
 //                              components in groups of sm_gq(d) on blockIdx.z, a fixed-order block reduction (no atomics)
 #include <math.h>
@@ -28,6 +28,7 @@
 #include <algorithm>
 
 #include "gp_common.cuh"
+#include "simt_pass.cuh"
 
 namespace gp {
 
@@ -137,37 +138,16 @@ spectral_kmv_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, 
   }
 }
 
-// ---- rows: OUT[r][j] = K(x1[idx[r]], x2[j]); NaN rows for an index out of range or non-finite inputs (as krows_kernel) ------
-__global__ void spectral_krows_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int W, const int64_t* __restrict__ idx,
-                                      int64_t n1, int64_t n2, const SmHyp h, float* __restrict__ OUT, int64_t ldo,
-                                      const int* __restrict__ xbad) {
-  __shared__ float zi[SM_WMAX];
-  const int64_t r = blockIdx.y;
-  const int64_t i = idx[r];
-  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 0 || i >= n1 || *xbad) {
-    if (j < n2) OUT[r * ldo + j] = __int_as_float(0x7fc00000);
-    return;
-  }
-  for (int c = threadIdx.x; c < W; c += blockDim.x) zi[c] = Z1[i * W + c];
-  __syncthreads();
-  if (j >= n2) return;
-  OUT[r * ldo + j] = sm_pair(h, zi, Z2 + j * W);
-}
-
-// diagonal of a cross operator (n1 == n2): OUT[i] = K(x1_i, x2_i)
-__global__ void spectral_kdiag_cross_kernel(const float* __restrict__ Z1, const float* __restrict__ Z2, int W, int64_t n, const SmHyp h,
-                                            float* __restrict__ OUT, const int* __restrict__ xbad) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  OUT[i] = *xbad ? __int_as_float(0x7fc00000) : sm_pair(h, Z1 + i * W, Z2 + i * W);
-}
-
-// diagonal of a square operator: the constant S (sum_q w_q)^d, NaN for non-finite inputs
-__global__ void spectral_fill_kernel(float* __restrict__ OUT, int64_t n, float v, const int* __restrict__ xbad) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) OUT[i] = *xbad ? __int_as_float(0x7fc00000) : v;
-}
+// ---- rows and the diagonal of a cross operator: K(x1_i, x2_j) from two packed rows (runtime Q, d) ---------------------------
+struct SmEntry {
+  static constexpr bool XBAD = true;
+  const float* Z1;
+  const float* Z2;
+  int ld;   // W
+  SmHyp h;
+  __host__ __device__ int width() const { return ld; }
+  __device__ __forceinline__ float entry(const float* za, const float* zb, int64_t, int64_t) const { return sm_pair(h, za, zb); }
+};
 
 // ---- bilinear derivative: grid (row blocks, column splits, component groups of GQ = sm_gq(D)) -------------------------------
 // With g = L_i . R_j, the mixtures s_c = sum_q w_q e_qc cos_qc and P_c = prod_{c' != c} s_c' (prefix and suffix products, no
@@ -270,13 +250,7 @@ spectral_bilinear_kernel(const float* __restrict__ Z1, const float* __restrict__
 #pragma unroll
   for (int o = 0; o < NO; ++o) {
     __syncthreads();
-    red[tid] = acc[o];
-    __syncthreads();
-    for (int sft = SIMT_TI / 2; sft > 0; sft >>= 1) {
-      if (tid < sft) red[tid] += red[tid + sft];
-      __syncthreads();
-    }
-    if (tid == 0) gout[blk * gstride + grp * NO + o] = red[0];
+    block_sum_store<SIMT_TI>(red, acc[o], gout + blk * gstride + grp * NO + o);
   }
 }
 
@@ -322,28 +296,26 @@ int spectral_pack(gp_plan* p) {
 
 static const float* sm_z1(const gp_plan* p) { return p->same ? p->Z2.as<float>() : p->Z1.as<float>(); }
 
-#define GP_SM_CASES(X)                                                                                                      \
-  X(1, 1) X(1, 4) X(1, 16) X(2, 1) X(2, 4) X(2, 16) X(3, 1) X(3, 4) X(3, 10) X(4, 1) X(4, 4) X(4, 8) X(5, 1) X(5, 4) X(5, 6) \
-  X(6, 1) X(6, 4) X(6, 5) X(7, 1) X(7, 4) X(8, 1) X(8, 4)
+// the compiled (d, QM) cases, keyed d * 100 + QM
+template <class F>
+static bool with_sm_case(int key, F&& f) {
+  return with_width<101, 104, 116, 201, 204, 216, 301, 304, 310, 401, 404, 408, 501, 504, 506, 601, 604, 605, 701, 704, 801, 804>(key, f);
+}
 
 int spectral_kmv_launch(gp_plan* p, const float* V16, const int* done_flag) {
   GP_REQUIRE(V16 != nullptr, GP_E_STATE, "spectral plan: fp32 rows of V needed");
   const SmHyp h = spectral_hyp(p);
   dim3 grid((unsigned)cdiv(p->row_count, SIMT_TI), (unsigned)p->nsplit);
   const int64_t cps = p->tiles_per_split * SIMT_TJ;
-  const int key = p->d * 100 + sm_qcase(p->d, h.Q);
-#define GP_SM_KMV(DV, QV)                                                                                                          \
-  case DV * 100 + QV:                                                                                                              \
-    spectral_kmv_kernel<DV, QV><<<grid, SIMT_TI, 0, p->stream>>>(sm_z1(p), p->Z2.as<float>(), p->DP, V16, partial_ptr(p), p->row_count, \
-                                                                 p->n2, p->rows_pad, cps, h, done_flag);                         \
-    break;
-  switch (key) {
-    GP_SM_CASES(GP_SM_KMV)
-    default:
-      set_error("spectral plan: no compiled case for d=%d, Q=%d", p->d, h.Q);
-      return GP_E_SHAPE;
+  const bool ok = with_sm_case(p->d * 100 + sm_qcase(p->d, h.Q), [&](auto key) {
+    constexpr int K = decltype(key)::value;
+    spectral_kmv_kernel<K / 100, K % 100><<<grid, SIMT_TI, 0, p->stream>>>(sm_z1(p), p->Z2.as<float>(), p->DP, V16, partial_ptr(p),
+                                                                          p->row_count, p->n2, p->rows_pad, cps, h, done_flag);
+  });
+  if (!ok) {
+    set_error("spectral plan: no compiled case for d=%d, Q=%d", p->d, h.Q);
+    return GP_E_SHAPE;
   }
-#undef GP_SM_KMV
   p->launches++;
   GP_CUDA(cudaGetLastError());
   return GP_OK;
@@ -351,27 +323,13 @@ int spectral_kmv_launch(gp_plan* p, const float* V16, const int* done_flag) {
 
 int spectral_krows(gp_plan* p, const int64_t* idx, int64_t m, float* OUT, int64_t ldo) {
   GP_REQUIRE(m <= 65535, GP_E_SHAPE, "rows of a spectral plan: at most 65535 rows per call (m=%lld)", (long long)m);
-  const SmHyp h = spectral_hyp(p);
-  dim3 grid((unsigned)cdiv(p->n2, 256), (unsigned)m);
-  spectral_krows_kernel<<<grid, 256, 0, p->stream>>>(sm_z1(p), p->Z2.as<float>(), p->DP, idx, p->row_count, p->n2, h, OUT, ldo, p->xbad);
-  p->launches++;
-  GP_CUDA(cudaGetLastError());
-  return GP_OK;
+  return launch_krows(p, SmEntry{sm_z1(p), p->Z2.as<float>(), p->DP, spectral_hyp(p)}, idx, m, OUT, ldo);
 }
 
+// square: the constant S (sum_q w_q)^d; cross: per pair.  NaN for non-finite inputs
 int spectral_kdiag(gp_plan* p, float* OUT) {
-  if (p->same) {
-    spectral_fill_kernel<<<(unsigned)cdiv(p->row_count, 256), 256, 0, p->stream>>>(OUT, p->row_count, (float)p->sm_diag, p->xbad);
-  } else {
-    GP_REQUIRE(p->n1 == p->n2, GP_E_SHAPE, "diagonal of a %lld x %lld cross-covariance is undefined (kernel(x1, x2, diag=True) needs equal sizes)",
-               (long long)p->n1, (long long)p->n2);
-    const SmHyp h = spectral_hyp(p);
-    spectral_kdiag_cross_kernel<<<(unsigned)cdiv(p->n1, 256), 256, 0, p->stream>>>(p->Z1.as<float>(), p->Z2.as<float>(), p->DP, p->n1, h,
-                                                                                    OUT, p->xbad);
-  }
-  p->launches++;
-  GP_CUDA(cudaGetLastError());
-  return GP_OK;
+  const float diag = (float)p->sm_diag;
+  return launch_kdiag(p, OUT, &diag, SmEntry{p->Z1.as<float>(), p->Z2.as<float>(), p->DP, spectral_hyp(p)});
 }
 
 // grad_ls = [dF/dw_q (Q) | dF/dmu_qc (Q d, row-major) | dF/dv_qc (Q d, row-major)], *grad_os = dF/dS
@@ -385,36 +343,21 @@ int spectral_bilinear_grad(gp_plan* p, const float* Lf, int64_t ldl, const float
   bilinear_split(p, p->n2, &grid, &cps);
   const int64_t nblk = (int64_t)grid.x * grid.y;
   grid.z = (unsigned)ngrp;
-  GP_CHECK(p->misc.ensure(sizeof(double) * (nblk * nout + nout)));
-  GP_CHECK(p->misc2.ensure(sizeof(float) * p->row_count * TP));
-  GP_CHECK(p->misc3.ensure(sizeof(float) * p->n2 * TP));
-  double* gout = p->misc.as<double>();
-  double* gsum = gout + nblk * nout;
-  std::vector<double> total(nout, 0.0), hbuf(nout);
-  const int key = d * 100 + sm_qcase(d, Q);
-  for (int c0 = 0; c0 < s; c0 += TP) {
-    const int tc = std::min(TP, s - c0);
-    GP_CHECK(to_v16(p, Lf + c0, ldl, tc, p->row_count, p->misc2.as<float>()));
-    GP_CHECK(to_v16(p, Rt + c0, ldr, tc, p->n2, p->misc3.as<float>()));
-#define GP_SM_BL(DV, QV)                                                                                                        \
-  case DV * 100 + QV:                                                                                                           \
-    spectral_bilinear_kernel<DV, QV><<<grid, SIMT_TI, 0, p->stream>>>(sm_z1(p), p->Z2.as<float>(), p->DP, p->misc2.as<float>(), \
-                                                                      p->misc3.as<float>(), p->row_count, p->n2, cps, h, gout, nout); \
-    break;
-    switch (key) {
-      GP_SM_CASES(GP_SM_BL)
-      default:
-        set_error("spectral plan: no compiled case for d=%d, Q=%d", d, Q);
-        return GP_E_SHAPE;
+  std::vector<double> total;
+  GP_CHECK(bilinear_sweep(p, Lf, ldl, Rt, ldr, s, p->row_count, nblk, nout, [&](const float* L16, const float* R16, double* gout) -> int {
+    const bool ok = with_sm_case(d * 100 + sm_qcase(d, Q), [&](auto key) {
+      constexpr int K = decltype(key)::value;
+      spectral_bilinear_kernel<K / 100, K % 100><<<grid, SIMT_TI, 0, p->stream>>>(sm_z1(p), p->Z2.as<float>(), p->DP, L16, R16,
+                                                                                 p->row_count, p->n2, cps, h, gout, nout);
+    });
+    if (!ok) {
+      set_error("spectral plan: no compiled case for d=%d, Q=%d", d, Q);
+      return GP_E_SHAPE;
     }
-#undef GP_SM_BL
     p->launches++;
     GP_CUDA(cudaGetLastError());
-    GP_CHECK(sum_partials_double(p, gout, nblk, nout, nout, gsum));
-    GP_CUDA(cudaMemcpyAsync(hbuf.data(), gsum, sizeof(double) * nout, cudaMemcpyDeviceToHost, p->stream));
-    GP_CUDA(cudaStreamSynchronize(p->stream));
-    for (int o = 0; o < nout; ++o) total[o] += hbuf[o];
-  }
+    return GP_OK;
+  }, total));
   const double S = p->outputscale;
   *grad_os = total[0];
   for (int q = 0; q < Q; ++q) {
