@@ -566,10 +566,9 @@ class ScaleKernel(Kernel):
             from .operators import SumKernelLinearOperator
             if _batch_index is not None:
                 raise NotImplementedError("batched ScaleKernel over an AdditiveKernel")
-            from .operators import with_outputscale
             inner = self.base_kernel(x1, None if _same else x2)
             terms = inner.ops if isinstance(inner, SumKernelLinearOperator) else [inner]
-            scaled = [with_outputscale(t, self.outputscale * t.outputscale) for t in terms]   # periodic terms keep their period
+            scaled = [t.with_outputscale(self.outputscale * t.outputscale) for t in terms]   # periodic terms keep their period
             op = scaled[0] if len(scaled) == 1 else SumKernelLinearOperator(scaled)
             return op.diagonal() if diag else op
         if isinstance(self.base_kernel, ProductKernel):
@@ -578,8 +577,7 @@ class ScaleKernel(Kernel):
             if _batch_index is not None:
                 raise NotImplementedError("batched ScaleKernel over a ProductKernel")
             f = self.base_kernel(x1, None if _same else x2).ops
-            first = KernelLinearOperator(f[0].x1, f[0].x2, f[0].kind, f[0].lengthscale, self.outputscale * f[0].outputscale)
-            op = ProductKernelLinearOperator([first, *f[1:]])
+            op = ProductKernelLinearOperator([f[0].with_outputscale(self.outputscale * f[0].outputscale), *f[1:]])
             return op.diagonal() if diag else op
         if isinstance(self.base_kernel, (SpectralMixtureKernel, PeriodicKernel, RQKernel, PolynomialKernel, PiecewisePolynomialKernel)):
             os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
@@ -589,25 +587,13 @@ class ScaleKernel(Kernel):
         else:
             base = self.base_kernel.forward(x1, x2, diag=False, _same=_same, _batch_index=bi, **params)
         os_ = self.outputscale if (_batch_index is None or self.outputscale.dim() == 0) else self.outputscale[_batch_index]
-        from .operators import DerivKernelLinearOperator, SKIKernelLinearOperator
-        if isinstance(base, DerivKernelLinearOperator):   # s folded into the same value / gradient operator
-            op = DerivKernelLinearOperator(base.x1, None if base.same else base.x2, base.lengthscale, os_, base.kind)
-            return op.diagonal() if diag else op
-        if isinstance(base, SKIKernelLinearOperator):
-            op = SKIKernelLinearOperator(base.x1, base.kind, base.lengthscale, os_, base.grid_sizes, base.grid_lo, base.grid_step)
-            return op.diagonal() if diag else op
-        from .operators import (PeriodicKernelLinearOperator, PiecewisePolynomialKernelLinearOperator, PolynomialKernelLinearOperator,
-                                RQKernelLinearOperator, SumKernelLinearOperator, with_outputscale)
-        # operators with parameters beyond lengthscale and scale
-        keep = (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator, PiecewisePolynomialKernelLinearOperator)
-        if isinstance(base, keep):   # a nested ScaleKernel: both scales folded in, the period / alpha kept
-            op = with_outputscale(base, os_ * base.outputscale)
-            return op.diagonal() if diag else op
-        if isinstance(base, SumKernelLinearOperator) and any(isinstance(t, keep) for t in base.ops):
-            # a ScaleKernel around a scaled sum with periodic or RQ terms: the scale folded into every term, periods and alphas kept
-            op = SumKernelLinearOperator([with_outputscale(t, os_ * t.outputscale) for t in base.ops])
-            return op.diagonal() if diag else op
-        op = KernelLinearOperator(base.x1, base.x2, base.kind, base.lengthscale, os_)
+        from .operators import SumKernelLinearOperator
+
+        def fold(op):
+            # s folded into the operator, its other parameters kept; the scale of a nested ScaleKernel multiplies it
+            return op.with_outputscale(os_ * op.outputscale if op._scaled else os_)
+
+        op = SumKernelLinearOperator([fold(t) for t in base.ops]) if isinstance(base, SumKernelLinearOperator) else fold(base)
         return op.diagonal() if diag else op
 
     def _batchable(self):

@@ -36,6 +36,48 @@ _PLAN_CACHE: "dict[tuple, Plan]" = {}
 _PLAN_CACHE_MAX = 64          # a batch of 16 independent operators (+ their cross-covariances) must fit
 _PLAN_LOCK = __import__("threading").RLock()   # BatchLinearOperator drives the cache from worker threads
 
+_SLOT_ROLES = ("own", "lowrank", "sum_term", "product_factor", "data", "lcm_term")
+# RQ and polynomial operators run on the plain kernels: they share the plain slots, and their kind and parameters are part of the
+# plan's hyper-parameter key, so a plan re-sends them whenever another kind used it last
+_SLOT_FAMILY = {"rq": "plain", "poly": "plain"}
+
+
+def _slot(family, role, index=0):
+    """The plan-cache slot of an operator of `family` in `role` (the index-th sum term, product factor or LCM term): operators
+    over the same inputs get one plan per slot, and a plan is only ever re-pointed within its slot, so two families (or roles)
+    never see each other's engine settings."""
+    if role not in _SLOT_ROLES:
+        raise ValueError(f"unknown plan-cache role {role!r}")
+    return (_SLOT_FAMILY.get(family, family), role, int(index))
+
+
+# Parent plans of the operators built on other plans (sum, product, Kronecker, LCM, derivative), one dict per family, each the
+# 16 most recently used
+_SUM_PLANS: "dict[tuple, Plan]" = {}
+_PRODUCT_PLANS: "dict[tuple, Plan]" = {}
+_KRON_PLANS: "dict[tuple, Plan]" = {}
+_LCM_PLANS: "dict[tuple, Plan]" = {}
+_DERIV_PLANS: "dict[tuple, Plan]" = {}
+_PARENT_PLANS = (_SUM_PLANS, _PRODUCT_PLANS, _KRON_PLANS, _LCM_PLANS, _DERIV_PLANS)
+
+
+def _parent_plan(plans, key, make, x1=None, x2=None):
+    """The parent plan of `key` in `plans` (most recently used last, at most 16), make() on a miss.  With x1 (and x2 for a cross
+    operator), a parent whose inputs differ follows its child plans, which the cache re-pointed to new inputs (_get_plan_locked)."""
+    with _PLAN_LOCK:
+        parent = plans.pop(key, None)
+        if parent is None:
+            parent = make()
+            parent._hyp_key = None
+        elif x1 is not None and parent.x1.data_ptr() != x1.data_ptr():
+            parent.x1 = x1.contiguous()
+            parent.x2 = parent.x1 if x2 is None else x2.contiguous()
+            parent.refresh_data()
+        plans[key] = parent
+        while len(plans) > 16:
+            plans.pop(next(iter(plans))).close()
+    return parent
+
 
 def _get_plan(x1, x2, backend, row_begin, row_count, comm, slot=0, owner=None) -> Plan:
     if not x1.is_cuda:
@@ -82,16 +124,9 @@ def _get_plan_locked(x1, x2, backend, row_begin, row_count, comm, slot=0, owner=
 
 def clear_plan_cache():
     with _PLAN_LOCK:
-        while _SUM_PLANS:
-            _SUM_PLANS.popitem()[1].close()
-        while _PRODUCT_PLANS:
-            _PRODUCT_PLANS.popitem()[1].close()
-        while _KRON_PLANS:
-            _KRON_PLANS.popitem()[1].close()
-        while _LCM_PLANS:
-            _LCM_PLANS.popitem()[1].close()
-        while _DERIV_PLANS:
-            _DERIV_PLANS.popitem()[1].close()
+        for plans in _PARENT_PLANS:
+            while plans:
+                plans.popitem()[1].close()
         while _PLAN_CACHE:
             _PLAN_CACHE.popitem()[1].close()
         _ADDITIVE_X.clear()
@@ -251,52 +286,99 @@ class _SamplingMixin:
         return (q.double() @ (evecs * evals.sqrt())).float()
 
 
+def _a(noun):
+    return ("an " if noun[0] in "aeiou" else "a ") + noun
+
+
 class KernelLinearOperator(_SamplingMixin):
-    """K(x1, x2) (outputscale folded in) that never materialises: every product is the fused CUDA kernel."""
+    """K(x1, x2) (outputscale folded in) that never materialises: every product is the fused CUDA kernel.
+
+    This class is also the single-plan operator every kernel family (RQ, polynomial, periodic, piecewise polynomial, spectral
+    mixture) derives from.  A family declares its parameters, its engine calls and what it may take part in; plan(), the host
+    read of the hyper-parameters, their gradients and the re-wrapping methods are the ones below."""
+
+    # -- what a family declares --
+    _family = "plain"          # plan-cache family (_slot)
+    _noun = "RBF / Matern"     # names the family in refusals
+    _sum_term = True           # may be a term of a kernel sum
+    _factor = True             # may be a kernel-product or an IndexKernel factor
+    _input_grads = True        # gradients with respect to the inputs
+    _row_sharding = True
+    _single_plan = True        # one plan, re-wrapped by _with (composite and data-plan operators: False)
+    _params = ("lengthscale",)     # the hyper-parameter tensors before the outputscale, in hyper_tensors() order
+    _plan_backend = None           # None: settings.backend
+    _resend_on_new_plan = True     # re-send every engine setting on a plan newly obtained from the cache
+    _scaled = False                # per operator: it carries the outputscale of a ScaleKernel
 
     def __init__(self, x1, x2, kind, lengthscale, outputscale=None, plan: Plan | None = None, comm=None,
                  row_begin=0, row_count=0):
+        if not self._row_sharding:
+            if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
+                raise NotImplementedError(f"a row-sharded {self._noun} operator is not available on the accelerated path")
+            comm, row_begin, row_count = None, 0, 0
         self.x1, self.x2 = x1, x2
         self.kind = kind
         self.lengthscale = lengthscale          # tensor (scalar or [d]); may require grad
+        self._scaled = outputscale is not None
         self.outputscale = outputscale if outputscale is not None else torch.ones((), device=x1.device)
         self._plan = plan
+        self._plan_slot = _slot(self._family, "own")
         self._comm = comm
         self._row_begin, self._row_count = row_begin, row_count
         self.same = x2 is None or x2 is x1 or (x1.shape == x2.shape and x1.data_ptr() == x2.data_ptr())
 
+    def _ctor_args(self):
+        """The constructor arguments between (x1, x2) and the outputscale (_with rebuilds the operator from them)."""
+        return (self.kind, self.lengthscale)
+
+    def _engine_calls(self, hyp, nz):
+        """[(plan attribute, key, send)] in call order: send(plan) is called when the plan's attribute differs from key.  hyp is
+        the host values of _plan_hypers(), one list per tensor; nz the noise."""
+        ls, (os_,) = hyp
+        return [("_hyp_key", (self.kind, tuple(ls), os_, nz), lambda p: p.set_hypers(self.kind, ls, os_, nz))]
+
     # -- plumbing --
+    @property
+    def _scale_is_hyper(self):
+        return True
+
+    def _plan_hypers(self):
+        """The tensors this operator's own plan is set from: _params, then the outputscale."""
+        return [getattr(self, n) for n in self._params] + ([self.outputscale] if self._scale_is_hyper else [])
+
     def _host_hypers(self, noise_t=None):
-        """(lengthscale list, outputscale, noise) as host floats with ONE device->host read per operator (cached: the
-        parameter tensors of an operator never change; a new forward builds a new operator)."""
+        """([values of each _plan_hypers() tensor], noise, noise tensor) as host floats with ONE device->host read per operator
+        (cached: the parameter tensors of an operator never change; a new forward builds a new operator)."""
         cached = getattr(self, "_hyp_host", None)
-        if cached is None or (noise_t is not None and cached[3] is not noise_t):
-            parts = [self.lengthscale.detach().reshape(-1).float(), self.outputscale.detach().reshape(1).float()]
+        if cached is None or (noise_t is not None and cached[2] is not noise_t):
+            hyp = self._plan_hypers()
+            parts = [t.detach().reshape(-1).float().to(self.device) for t in hyp]
             if noise_t is not None:
-                parts.append(noise_t.detach().reshape(-1)[:1].float())
+                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.device))
             vals = torch.cat(parts).tolist()
-            nl = self.lengthscale.numel()
-            cached = (vals[:nl], vals[nl], vals[nl + 1] if noise_t is not None else None, noise_t)
+            out, k = [], 0
+            for t in hyp:
+                out.append(vals[k:k + t.numel()])
+                k += t.numel()
+            cached = (out, vals[k] if noise_t is not None else None, noise_t)
             self._hyp_host = cached
         return cached
 
     def plan(self, noise=0.0) -> Plan:
         """noise: a host float, or the device tensor of the likelihood (read together with the other hyper-parameters)."""
-        fresh = False
-        if self._plan is None:
-            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(),
-                                   self._row_begin, self._row_count, self._comm, getattr(self, "_plan_slot", 0), owner=self)
-            fresh = True
-        if torch.is_tensor(noise):
-            ls, os_, nz, _ = self._host_hypers(noise)
-        else:
-            ls, os_, _, _ = self._host_hypers(None)
+        fresh = self._plan is None
+        if fresh:
+            self._plan = _get_plan(self.x1, None if self.same else self.x2, self._plan_backend or settings.backend.value(),
+                                   self._row_begin, self._row_count, self._comm, self._plan_slot, owner=self)
+        hyp, nz, _ = self._host_hypers(noise if torch.is_tensor(noise) else None)
+        if not torch.is_tensor(noise):
             nz = float(noise)
-        key = (self.kind, tuple(ls), os_, nz)
-        if fresh or getattr(self._plan, "_hyp_key", None) != key:
-            self._plan.set_hypers(self.kind, ls, os_, nz)
-            self._plan._hyp_key = key
-        return self._plan
+        p = self._plan
+        for attr, key, send in self._engine_calls(hyp, nz):
+            if (fresh and self._resend_on_new_plan) or getattr(p, attr, None) != key:
+                send(p)
+                setattr(p, attr, key)
+        return p
 
     @property
     def shape(self):
@@ -320,22 +402,25 @@ class KernelLinearOperator(_SamplingMixin):
 
     @property
     def requires_grad(self):
-        return bool(self.lengthscale.requires_grad or self.outputscale.requires_grad)
+        return any(t.requires_grad for t in self._plan_hypers())
 
     def evaluate_kernel(self):
         return self  # "meta LinearOperator" branch, lazy_evaluated_kernel_tensor.py:345-348
 
     def representation(self):
-        return (self.x1, self.x2, self.lengthscale, self.outputscale)
+        return (self.x1, self.x2, *self._plan_hypers())
 
     def hyper_tensors(self):
         """The differentiable hyper-parameters of this operator, in the order _bilinear_derivative_list returns their
         gradients (the autograd functions below take them as explicit inputs)."""
-        return [self.lengthscale, self.outputscale]
+        return self._plan_hypers()
 
     def input_tensors(self):
         """The inputs K is differentiated in by the product and dense-block autograd functions below, which take them after
-        the hyper-parameters: [x1] for a square operator (both arguments are the same points), [x1, x2] for a cross-covariance."""
+        the hyper-parameters: [x1] for a square operator (both arguments are the same points), [x1, x2] for a cross-covariance;
+        none for a family without input gradients."""
+        if not self._input_grads:
+            return []
         return [self.x1] if self.same else [self.x1, self.x2]
 
     def solve_input_tensors(self):
@@ -344,13 +429,27 @@ class KernelLinearOperator(_SamplingMixin):
         return self.input_tensors()
 
     def _bilinear_derivative_list(self, left, right):
-        gl, go = self._bilinear_derivative(left, right)
-        return [gl.reshape(self.lengthscale.shape), go.reshape(self.outputscale.shape)]
+        """The gradients of sum(left * (K @ right)) with respect to hyper_tensors(): the engine's flat gradient split over the
+        tensors before the outputscale, then the outputscale's."""
+        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
+        out, k = [], 0
+        for t in self._plan_hypers()[:len(self._params)]:
+            out.append(torch.tensor(gl[k:k + t.numel()], device=self.device, dtype=t.dtype).reshape(t.shape))
+            k += t.numel()
+        if self._scale_is_hyper:
+            out.append(torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape))
+        return out
+
+    def _no_input_grads(self):
+        return NotImplementedError(f"gradients with respect to the inputs of {_a(self._noun)} operator are not available on the "
+                                   "accelerated path")
 
     def _input_grad_list(self, left, right, needs):
         """Gradients of sum(left * (K @ right)) w.r.t. input_tensors(), None where `needs` is False (gp_kmv_input_grad)."""
         if not any(needs):
             return [None] * len(needs)
+        if not self._input_grads:
+            raise self._no_input_grads()
         d1, d2 = self.plan(getattr(self, "_last_noise", 0.0)).kmv_input_grad(left, right, needs[0], len(needs) > 1 and needs[1])
         return [d1, d2][: len(needs)]
 
@@ -358,6 +457,8 @@ class KernelLinearOperator(_SamplingMixin):
         """Gradients of sum(w * K) w.r.t. input_tensors(), None where `needs` is False (gp_kdense_input_grad)."""
         if not any(needs):
             return [None] * len(needs)
+        if not self._input_grads:
+            raise self._no_input_grads()
         d1, d2 = self.plan().dense_input_grad(w, needs[0], len(needs) > 1 and needs[1])
         return [d1, d2][: len(needs)]
 
@@ -377,11 +478,24 @@ class KernelLinearOperator(_SamplingMixin):
     def numel(self):
         return self.shape[0] * self.shape[1]
 
+    def _with(self, x1, x2, detach=False, outputscale=None):
+        """This operator over new inputs (detached, or with the outputscale replaced), rebuilt through its constructor: the
+        new operator has its own plan and no row sharding."""
+        if not self._single_plan:
+            raise NotImplementedError(f"{type(self).__name__} is not rebuilt from its inputs and parameters on the accelerated path")
+        f = (lambda t: t.detach() if torch.is_tensor(t) else t) if detach else (lambda t: t)
+        if outputscale is None and self._scaled:
+            outputscale = self.outputscale
+        return type(self)(f(x1), None if x2 is None else f(x2), *map(f, self._ctor_args()),
+                          None if outputscale is None else f(outputscale))
+
+    def with_outputscale(self, outputscale):
+        """This operator with its outputscale replaced (a ScaleKernel folded in); its other parameters are kept."""
+        return self._with(self.x1, None if self.same else self.x2, outputscale=outputscale)
+
     def _transpose_nonbatch(self):
-        """K(x1, x2)^T = K(x2, x1) for every stationary kernel on this path (no data is moved)."""
-        if self.same:
-            return self
-        return KernelLinearOperator(self.x2, self.x1, self.kind, self.lengthscale, self.outputscale)
+        """K(x1, x2)^T = K(x2, x1) for every kernel on this path (no data is moved)."""
+        return self if self.same else self._with(self.x2, self.x1)
 
     def transpose(self, dim1, dim2):
         return self if dim1 % 2 == dim2 % 2 else self._transpose_nonbatch()
@@ -394,8 +508,7 @@ class KernelLinearOperator(_SamplingMixin):
         return self._transpose_nonbatch()
 
     def detach(self):
-        return KernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.kind, self.lengthscale.detach(),
-                                    self.outputscale.detach())
+        return self._with(self.x1, None if self.same else self.x2, detach=True)
 
     # -- products --
     def matmul(self, rhs):
@@ -426,19 +539,12 @@ class KernelLinearOperator(_SamplingMixin):
         ri, ci = index
         if isinstance(ri, int):
             return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
-        x1 = self.x1[ri]
-        x2 = (self.x1 if self.same else self.x2)[ci]
-        return KernelLinearOperator(x1, x2, self.kind, self.lengthscale, self.outputscale)
+        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
 
     def __add__(self, other):
         if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
             return AddedDiagLinearOperator(self, other)
-        if isinstance(other, AdditiveKernelLinearOperator):
-            raise NotImplementedError("sums that contain additive operators are not available on the accelerated path")
-        if isinstance(other, SpectralMixtureKernelLinearOperator):
-            raise NotImplementedError("sums that contain spectral mixture operators are not available on the accelerated path")
-        if isinstance(other, KernelLinearOperator) and not isinstance(other, (SKIKernelLinearOperator, ProductKernelLinearOperator)) \
-                and not isinstance(self, SKIKernelLinearOperator):
+        if isinstance(other, KernelLinearOperator):
             return SumKernelLinearOperator([self, other])     # K_1 + K_2 stays lazy: one engine operator (csrc/sum.cu)
         raise NotImplementedError("a kernel operator adds a (Constant)DiagLinearOperator or another kernel operator")
 
@@ -449,10 +555,10 @@ class KernelLinearOperator(_SamplingMixin):
         """K o B[t, t'] with an IndexKernel's operator (the Hadamard multitask model, covar_x.mul(covar_i)): one engine operator
         (gp_plan_set_tasks).  RBF / Matern operators, optionally scaled, only.  With another RBF / Matern kernel operator (or a
         product of them) of the same shape: the elementwise product K_1 o K_2 as one engine operator (gp_plan_set_product)."""
-        plain = (KernelLinearOperator, ProductKernelLinearOperator)
-        if isinstance(other, (RQKernelLinearOperator, PolynomialKernelLinearOperator, PiecewisePolynomialKernelLinearOperator)):
-            return other.mul(self)   # refused, naming the kernel
-        if type(self) in plain and type(other) in plain:
+        for o in (self, other):
+            if isinstance(o, KernelLinearOperator) and not o._factor:
+                raise o._no_product()
+        if isinstance(other, KernelLinearOperator):
             return ProductKernelLinearOperator([self, other])
         if not isinstance(other, IndexLinearOperator) or type(self) is not KernelLinearOperator:
             raise NotImplementedError("the accelerated path multiplies an RBF / Matern kernel operator (optionally scaled) by an "
@@ -473,8 +579,16 @@ class KernelLinearOperator(_SamplingMixin):
             p.set_noise_diag(None)
         return p
 
+    def _no_product(self):
+        return NotImplementedError(f"products that contain {_a(self._noun)} operator (kernel products, IndexKernel multitask "
+                                   "models) are not available on the accelerated path: it multiplies an RBF / Matern kernel operator "
+                                   "(optionally scaled) by another one or by an IndexKernel operator only")
+
     def _bilinear_derivative(self, left, right):
         """(d/d lengthscale, d/d outputscale) of sum(left * (K @ right)); lazy_evaluated_kernel_tensor.py:69-105."""
+        if self._params != ("lengthscale",) or not self._scale_is_hyper:
+            names = ", ".join(self._params) + (" and outputscale" if self._scale_is_hyper else "")
+            raise NotImplementedError(f"{_a(self._noun)} operator has {names} gradients: use _bilinear_derivative_list")
         gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
         return torch.tensor(gl, device=self.device, dtype=self.dtype), torch.tensor(go, device=self.device, dtype=self.dtype)
 
@@ -511,14 +625,15 @@ class IndexLinearOperator:
     __mul__ = mul
 
 
-_TASK_SLOT = 16   # plan-cache slot of Hadamard operators: a plain operator over the same inputs never sees their task ids
-
-
 class HadamardKernelLinearOperator(KernelLinearOperator):
     """s K(x1, x2) o B[t1, t2] (the Hadamard multitask model, examples/03_Multitask_Exact_GPs/Hadamard_Multitask_GP_Regression.ipynb):
     one engine operator whose plan carries the task ids (gp_plan_set_tasks) and B (gp_plan_set_task_covar).  The hyper-parameters
     are lengthscale, outputscale and B; B's gradient comes from gp_task_covar_grad and autograd carries it to the IndexKernel's
     covar_factor / raw_var.  Input gradients are not available: inputs that require grad are refused."""
+
+    _family = "task"    # a plain operator over the same inputs never sees the task ids
+    _noun = "Hadamard multitask"
+    _sum_term = _factor = _single_plan = False
 
     def __init__(self, x1, x2, kind, lengthscale, outputscale, t1, t2, B):
         if x1.requires_grad or (x2 is not None and x2.requires_grad):
@@ -532,7 +647,6 @@ class HadamardKernelLinearOperator(KernelLinearOperator):
         if self.t1.numel() != self.shape[0] or self.t2.numel() != self.shape[1]:
             raise RuntimeError(f"task ids of sizes {self.t1.numel()}, {self.t2.numel()} do not match the operator {tuple(self.shape)}")
         self.B = B
-        self._plan_slot = _TASK_SLOT
 
     def plan(self, noise=0.0) -> Plan:
         p = super().plan(noise)
@@ -616,9 +730,6 @@ class HadamardKernelLinearOperator(KernelLinearOperator):
         raise NotImplementedError("a Hadamard multitask operator adds a (Constant)DiagLinearOperator only")
 
 
-_KRON_SLOT = 24   # plan-cache slot of the data plans of Kronecker operators
-
-
 def _aligned(ix, T: int, n: int):
     """The point slice of a row / column slice of a Kronecker operator that starts and stops on multiples of T (None otherwise)."""
     if not isinstance(ix, slice) or ix.step not in (None, 1):
@@ -635,6 +746,10 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
     hyper-parameters are lengthscale, outputscale and B; B's gradient comes from gp_task_covar_grad and autograd carries it to the
     IndexKernel's covar_factor / raw_var.  Input gradients are not available: inputs that require grad are refused."""
 
+    _family = "kron"
+    _noun = "Kronecker multitask"
+    _sum_term = _factor = _single_plan = False
+
     def __init__(self, x1, x2, kind, lengthscale, outputscale, B, rows=None, cols=None):
         if x1.requires_grad or (x2 is not None and x2.requires_grad):
             raise RuntimeError("gradients with respect to the inputs of a Kronecker multitask operator (K (x) B) are not implemented: "
@@ -645,7 +760,7 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
         self.B = B
         self.num_tasks = int(B.shape[-1])
         self._data_op = KernelLinearOperator(x1, x2, kind, lengthscale, outputscale)
-        self._data_op._plan_slot = _KRON_SLOT
+        self._data_op._plan_slot = _slot("kron", "data")
         # observed interleaved rows / columns (int64 index tensors, strictly increasing; None: all): the operator is
         # P_r ((s K) (x) B) P_c^T (masked())
         if self.same and cols is not None and cols is not rows and (rows is None or not torch.equal(rows, cols)):
@@ -683,24 +798,14 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
         T = self.num_tasks
         masked = self.rows is not None or self.cols is not None
-        with _PLAN_LOCK:
-            # a parent that holds a mask never serves an unmasked operator, nor the other way round; masked parents are
-            # re-masked below only when the indices change
-            key = (id(data), T, masked)
-            parent = _KRON_PLANS.pop(key, None)
-            if parent is None:
-                parent = KronPlan(data, T)
-                parent._hyp_key = None
-                parent._b_key = None
-                parent._obs_key = None
-            _KRON_PLANS[key] = parent
-            while len(_KRON_PLANS) > 16:
-                _KRON_PLANS.pop(next(iter(_KRON_PLANS))).close()
+        # a parent that holds a mask never serves an unmasked operator, nor the other way round; masked parents are re-masked
+        # below only when the indices change
+        parent = _parent_plan(_KRON_PLANS, (id(data), T, masked), lambda: KronPlan(data, T))
         # the data plan may have been re-packed or re-pointed since the last use: re-attach it (validation, no allocation)
         parent.attach(data, T)
         if masked:
             rh, ch = self._observed_host()
-            ok = parent._observed is not None and parent._obs_key is not None and all(
+            ok = parent._observed is not None and getattr(parent, "_obs_key", None) is not None and all(
                 (a is None and b is None) or (a is not None and b is not None and torch.equal(a, b)) for a, b in zip(parent._obs_key, (rh, ch)))
             if not ok:
                 parent.set_observed(rh, ch)
@@ -712,7 +817,7 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
         bh = getattr(self, "_b_host", None)
         if bh is None:
             bh = self._b_host = self.B.detach().float().cpu()
-        if parent._b_key is None or not torch.equal(parent._b_key, bh):
+        if getattr(parent, "_b_key", None) is None or not torch.equal(parent._b_key, bh):
             parent.set_task_covar(bh)
             parent._b_key = bh
         self._plan = parent
@@ -795,20 +900,16 @@ class KroneckerKernelLinearOperator(KernelLinearOperator):
         raise NotImplementedError("a Kronecker multitask operator adds a (Constant)DiagLinearOperator only")
 
 
-_KRON_PLANS: "dict[tuple, Plan]" = {}
-
-
-_LCM_SLOT = 40   # plan-cache slots of the term data plans of LCM operators: 40 + term index (the other families use 0..8, 16,
-                 # 20/21, 24, 28 and 32..37), so two terms over the same inputs never share one plan and its hyper-parameters
-_LCM_PLANS: "dict[tuple, Plan]" = {}
-
-
 class LCMKernelLinearOperator(KernelLinearOperator):
     """sum_q (s_q K_q(x1, x2)) (x) B_q over interleaved rows i T + a, Q = 1..4 (LCMKernel, kernels/lcm_kernel.py; the reference sums
     KroneckerProductLinearOperators into a SumLinearOperator): ONE engine operator (gp_plan_set_kron_terms) on the terms' data plans.
     `terms` are unmasked KroneckerKernelLinearOperators of one shape and T; each keeps its own inputs (active dimensions), kind,
     lengthscale, outputscale and B.  The hyper-parameters are [l_1, s_1, B_1, ..., l_Q, s_Q, B_Q]; their gradients come from
     gp_kron_terms_grad.  Input gradients are not available: the terms refuse inputs that require grad."""
+
+    _family = "lcm"
+    _noun = "LCM"
+    _sum_term = _factor = _single_plan = False
 
     def __init__(self, terms):
         terms = list(terms)
@@ -827,7 +928,7 @@ class LCMKernelLinearOperator(KernelLinearOperator):
         self._data_ops = []
         for i, t in enumerate(terms):
             op = KernelLinearOperator(t.x1, None if t.same else t.x2, t.kind, t.lengthscale, t.outputscale)
-            op._plan_slot = _LCM_SLOT + i
+            op._plan_slot = _slot("lcm", "lcm_term", i)   # two terms over the same inputs never share a plan
             self._data_ops.append(op)
 
     @property
@@ -843,16 +944,7 @@ class LCMKernelLinearOperator(KernelLinearOperator):
             datas.append(d)
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
         T = self.num_tasks
-        with _PLAN_LOCK:
-            key = (tuple(id(d) for d in datas), T)
-            parent = _LCM_PLANS.pop(key, None)
-            if parent is None:
-                parent = LcmPlan(datas, T)
-                parent._hyp_key = None
-                parent._b_key = None
-            _LCM_PLANS[key] = parent
-            while len(_LCM_PLANS) > 16:
-                _LCM_PLANS.pop(next(iter(_LCM_PLANS))).close()
+        parent = _parent_plan(_LCM_PLANS, (tuple(id(d) for d in datas), T), lambda: LcmPlan(datas, T))
         # the data plans may have been re-packed or re-pointed since the last use: re-attach them (validation, no allocation)
         parent.attach(datas[0], datas, T)
         hk = (nz, tuple((d.kind, tuple(d.lengthscale), d.outputscale) for d in datas))
@@ -862,7 +954,7 @@ class LCMKernelLinearOperator(KernelLinearOperator):
         bh = getattr(self, "_b_host", None)
         if bh is None:
             bh = self._b_host = torch.stack([t.B.detach().float() for t in self.terms]).cpu()
-        if parent._b_key is None or not torch.equal(parent._b_key, bh):
+        if getattr(parent, "_b_key", None) is None or not torch.equal(parent._b_key, bh):
             parent.set_term_covars(bh)
             parent._b_key = bh
         self._plan = parent
@@ -957,8 +1049,6 @@ def _take_square(op, idx, memo):
     if getattr(op, "_comm", None) is not None or getattr(op, "_row_begin", 0) != 0:
         raise NotImplementedError(f"an observation mask on a row-sharded {type(op).__name__} is not available")
     t = type(op)
-    if t is KernelLinearOperator:
-        return KernelLinearOperator(take(op.x1), None, op.kind, op.lengthscale, op.outputscale)
     if t is HadamardKernelLinearOperator:
         return HadamardKernelLinearOperator(take(op.x1), None, op.kind, op.lengthscale, op.outputscale, take(op.t1), None, op.B)
     if t is SumKernelLinearOperator:
@@ -967,8 +1057,7 @@ def _take_square(op, idx, memo):
         return ProductKernelLinearOperator([_take_square(o, idx, memo) for o in op.ops])
     if t is AdditiveKernelLinearOperator:
         return AdditiveKernelLinearOperator([_take_square(o, idx, memo) for o in op.ops], op.max_degree)
-    if t in (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator, SpectralMixtureKernelLinearOperator,
-             PiecewisePolynomialKernelLinearOperator):
+    if op._single_plan:
         return op._with(take(op.x1), None)
     raise NotImplementedError(f"observation masks are not available for {t.__name__}")
 
@@ -1005,9 +1094,6 @@ def MaskedLinearOperator(base, row_mask, col_mask):
         return _take_square(base, ri, {})
     return base[slice(None) if ri is None else ri, slice(None) if ci is None else ci]
 
-_DERIV_SLOT = 28   # plan-cache slot of the data plans of derivative operators
-
-
 _DERIV_NAMES = {"rbf": "RBFKernelGrad", "matern52": "Matern52KernelGrad"}
 
 
@@ -1017,6 +1103,10 @@ class DerivKernelLinearOperator(KernelLinearOperator):
     perfect shuffle: ONE engine operator (gp_plan_set_deriv / gp_plan_set_deriv_kind) on the plan of the plain kernel of that kind;
     no N (d+1) x N (d+1) matrix is stored.  The hyper-parameters are lengthscale (scalar or ARD) and outputscale.  Input gradients
     are not available: inputs that require grad are refused."""
+
+    _family = "deriv"
+    _noun = "derivative"
+    _sum_term = _factor = _single_plan = False
 
     def __init__(self, x1, x2, lengthscale, outputscale=None, kind="rbf"):
         if kind not in _DERIV_NAMES:
@@ -1031,7 +1121,7 @@ class DerivKernelLinearOperator(KernelLinearOperator):
         super().__init__(x1, x2, kind, lengthscale, outputscale)
         self.num_outputs = d + 1
         self._data_op = KernelLinearOperator(x1, x2, kind, lengthscale, self.outputscale)
-        self._data_op._plan_slot = _DERIV_SLOT
+        self._data_op._plan_slot = _slot("deriv", "data")
 
     @property
     def shape(self):
@@ -1043,15 +1133,8 @@ class DerivKernelLinearOperator(KernelLinearOperator):
         if getattr(data, "_noise_diag", None) is not None:
             data.set_noise_diag(None)
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
-        with _PLAN_LOCK:
-            key = (id(data), self.kind)   # one parent per (data plan, kind): never re-attached to a data plan of another kind
-            parent = _DERIV_PLANS.pop(key, None)
-            if parent is None:
-                parent = DerivPlan(data, self.kind)
-                parent._hyp_key = None
-            _DERIV_PLANS[key] = parent
-            while len(_DERIV_PLANS) > 16:
-                _DERIV_PLANS.pop(next(iter(_DERIV_PLANS))).close()
+        # one parent per (data plan, kind): never re-attached to a data plan of another kind
+        parent = _parent_plan(_DERIV_PLANS, (id(data), self.kind), lambda: DerivPlan(data, self.kind))
         # the data plan may have been re-packed or re-pointed since the last use: re-attach it (validation, no allocation)
         parent.attach(data, self.kind)
         hk = (nz, tuple(data.lengthscale), data.outputscale)
@@ -1076,6 +1159,9 @@ class DerivKernelLinearOperator(KernelLinearOperator):
     def detach(self):
         return DerivKernelLinearOperator(self.x1.detach(), None if self.same else self.x2.detach(), self.lengthscale.detach(),
                                          self.outputscale.detach(), self.kind)
+
+    def with_outputscale(self, outputscale):
+        return DerivKernelLinearOperator(self.x1, None if self.same else self.x2, self.lengthscale, outputscale, self.kind)
 
     def to_dense(self):
         return _KernelDense.apply(self)
@@ -1114,14 +1200,15 @@ class DerivKernelLinearOperator(KernelLinearOperator):
         raise NotImplementedError("a derivative operator adds a (Constant)DiagLinearOperator only")
 
 
-_DERIV_PLANS: "dict[tuple, Plan]" = {}
-
-
 class SumKernelLinearOperator(KernelLinearOperator):
     """K_1 + ... + K_m over the same inputs (AdditiveKernel, kernels/kernel.py:592-621).  The reference evaluates every term
     densely and adds the matrices; here the sum is ONE engine operator (gp_plan_set_sum): a product launches the fused kernel of
     every term into disjoint partial slots, the solves / preconditioner / SLQ run on the sum, and the hyper-parameter gradients
     of each term come from that term's own bilinear derivative with the shared left / right factors."""
+
+    _family = "sum"
+    _noun = "kernel sum"
+    _factor = _single_plan = False
 
     def __init__(self, ops):
         ops = list(ops)
@@ -1130,39 +1217,27 @@ class SumKernelLinearOperator(KernelLinearOperator):
             flat.extend(o.ops if isinstance(o, SumKernelLinearOperator) else [o])
         if not 1 <= len(flat) <= 4:
             raise RuntimeError(f"a kernel sum takes 1 to 4 terms (got {len(flat)})")
-        if any(isinstance(o, AdditiveKernelLinearOperator) for o in flat):
-            # a term is re-wrapped from its inputs, kind and (single) hyper-parameters below, which an additive operator does not have
-            raise NotImplementedError("sums that contain additive operators are not available on the accelerated path")
-        if any(isinstance(o, SpectralMixtureKernelLinearOperator) for o in flat):
-            raise NotImplementedError("sums that contain spectral mixture operators are not available on the accelerated path")
-        if any(isinstance(o, PiecewisePolynomialKernelLinearOperator) for o in flat):
-            raise NotImplementedError("sums that contain a PiecewisePolynomialKernel operator are not available on the accelerated "
-                                      "path: it runs its own compact-support backend")
+        for o in flat:
+            if not o._sum_term:
+                raise NotImplementedError(f"sums that contain {o._noun} operators are not available on the accelerated path")
         first = flat[0]
         for o in flat[1:]:
             if o.shape != first.shape or o.same != first.same:
                 raise RuntimeError(f"cannot add kernels of shapes {tuple(first.shape)} and {tuple(o.shape)}")
         # one engine plan per term even when the terms see the same inputs: re-wrap (the caller's operators stay usable on their
-        # own) and give every term its own slot of the plan cache
+        # own) and give every term its own slot of the plan cache; a term keeps its row sharding
         self.ops = []
         for i, o in enumerate(flat):
-            if isinstance(o, PeriodicKernelLinearOperator):   # keeps its period, on a slot no plain term uses
-                t = o._with(o.x1, None if o.same else o.x2)
-                t._plan_slot = _PERIODIC_SUM_SLOT + i
-            elif isinstance(o, (RQKernelLinearOperator, PolynomialKernelLinearOperator)):
-                # keeps alpha / power and offset, on the plain term slot (the kind and those parameters are in its key)
-                t = o._with(o.x1, None if o.same else o.x2)
-                t._plan_slot = 1 + i
-            else:
-                t = KernelLinearOperator(o.x1, o.x2, o.kind, o.lengthscale, o.outputscale, comm=o._comm, row_begin=o._row_begin,
-                                         row_count=o._row_count)
-                t._plan_slot = 1 + i
+            t = o._with(o.x1, o.x2)
+            t._plan_slot = _slot(o._family, "sum_term", i)
+            t._comm, t._row_begin, t._row_count = o._comm, o._row_begin, o._row_count
             self.ops.append(t)
         self.x1, self.x2, self.same = first.x1, first.x2, first.same
         self.kind = "sum"
         self.lengthscale, self.outputscale = first.lengthscale, first.outputscale   # representative only (device / dtype)
         self._comm, self._row_begin, self._row_count = first._comm, first._row_begin, first._row_count
         self._plan = None
+        self._plan_slot = _slot("sum", "own")
 
     def hyper_tensors(self):
         return [t for o in self.ops for t in o.hyper_tensors()]
@@ -1205,21 +1280,10 @@ class SumKernelLinearOperator(KernelLinearOperator):
     def plan(self, noise=0.0) -> Plan:
         terms = [o.plan(0.0) for o in self.ops]
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
-        with _PLAN_LOCK:
-            key = ("sum", tuple(id(t) for t in terms), getattr(self, "_plan_slot", 0))
-            parent = _SUM_PLANS.pop(key, None)
-            if parent is None:
-                parent = Plan(self.x1, None if self.same else self.x2, backend="auto", row_begin=self._row_begin,
-                              row_count=self._row_count, comm=self._comm)
-                parent._hyp_key = None
-            elif parent.x1.data_ptr() != self.x1.data_ptr():
-                # the term plans were re-pointed to new inputs (_get_plan_locked): follow them
-                parent.x1 = self.x1.contiguous()
-                parent.x2 = parent.x1 if self.same else self.x2.contiguous()
-                parent.refresh_data()
-            _SUM_PLANS[key] = parent
-            while len(_SUM_PLANS) > 16:
-                _SUM_PLANS.pop(next(iter(_SUM_PLANS))).close()
+        x2 = None if self.same else self.x2
+        parent = _parent_plan(_SUM_PLANS, (tuple(id(t) for t in terms), self._plan_slot),
+                              lambda: Plan(self.x1, x2, backend="auto", row_begin=self._row_begin, row_count=self._row_count,
+                                           comm=self._comm), self.x1, x2)
         # the terms may have been re-created / re-packed since the last use: (re-)attach them every time (validation + a
         # 64-float upload, no allocation), then set the noise of the sum
         parent.set_sum(terms)
@@ -1259,15 +1323,16 @@ class SumKernelLinearOperator(KernelLinearOperator):
         raise NotImplementedError("a kernel sum has one (lengthscale, outputscale) pair per term: use _bilinear_derivative_list")
 
 
-_SUM_PLANS: "dict[tuple, Plan]" = {}
-
-
 class ProductKernelLinearOperator(KernelLinearOperator):
     """K_1 o ... o K_m over the same inputs (ProductKernel, kernels/kernel.py:634-690).  The reference evaluates every factor
     densely and multiplies the matrices; here the product is ONE engine operator (gp_plan_set_product): a product with a block of
     vectors is one fused kernel launch that forms prod_f k_f per pair in registers, the solves / preconditioner / SLQ run on it, and
     one engine call returns every factor's hyper-parameter gradients.  2 to 4 RBF / Matern factors; gradients with respect to the
     inputs are not available through a product."""
+
+    _family = "product"
+    _noun = "kernel product"
+    _sum_term = _single_plan = False
 
     def __init__(self, ops):
         flat = []
@@ -1277,15 +1342,8 @@ class ProductKernelLinearOperator(KernelLinearOperator):
             raise NotImplementedError(f"a kernel product takes 2 to 4 factors on the accelerated path (got {len(flat)})")
         first = flat[0]
         for o in flat:
-            if isinstance(o, RQKernelLinearOperator):
-                raise NotImplementedError("products that contain a rational quadratic (RQ) operator are not available on the "
-                                          "accelerated path")
-            if isinstance(o, PolynomialKernelLinearOperator):
-                raise NotImplementedError("products that contain a PolynomialKernel operator are not available on the accelerated "
-                                          "path")
-            if type(o) is not KernelLinearOperator:
-                raise NotImplementedError("the factors of a kernel product must be RBF / Matern kernel operators (optionally scaled) "
-                                          "on the accelerated path")
+            if not o._factor:
+                raise o._no_product()
             if o.shape != first.shape or o.same != first.same:
                 raise RuntimeError(f"cannot multiply kernels of shapes {tuple(first.shape)} and {tuple(o.shape)}")
             if o._comm is not None or o._row_begin != 0 or o._row_count not in (0, o.shape[0]):
@@ -1296,8 +1354,8 @@ class ProductKernelLinearOperator(KernelLinearOperator):
         # one engine plan per factor even when the factors see the same inputs: re-wrap and give each its own plan-cache slot
         self.ops = []
         for i, o in enumerate(flat):
-            t = KernelLinearOperator(o.x1, o.x2, o.kind, o.lengthscale, o.outputscale)
-            t._plan_slot = 5 + i
+            t = o._with(o.x1, o.x2)
+            t._plan_slot = _slot(o._family, "product_factor", i)
             self.ops.append(t)
         self.x1, self.x2, self.same = first.x1, first.x2, first.same
         self.kind = "product"
@@ -1329,7 +1387,7 @@ class ProductKernelLinearOperator(KernelLinearOperator):
 
     def _bilinear_derivative_list(self, left, right):
         gl, go = self.plan(0.0).bilinear_grad(left, right)
-        parts = self._split_grads(gl, go, [o.lengthscale.numel() for o in self.ops], [o._host_hypers()[1] for o in self.ops])
+        parts = self._split_grads(gl, go, [o.lengthscale.numel() for o in self.ops], [o._host_hypers()[0][-1][0] for o in self.ops])
         out = []
         for o, (g, gs) in zip(self.ops, parts):
             out.append(torch.tensor(g, device=self.device, dtype=self.dtype).reshape(o.lengthscale.shape))
@@ -1349,20 +1407,8 @@ class ProductKernelLinearOperator(KernelLinearOperator):
     def plan(self, noise=0.0) -> Plan:
         factors = [o.plan(0.0) for o in self.ops]
         nz = float(noise.detach().reshape(-1)[0]) if torch.is_tensor(noise) else float(noise)
-        with _PLAN_LOCK:
-            key = ("product", tuple(id(f) for f in factors))
-            parent = _PRODUCT_PLANS.pop(key, None)
-            if parent is None:
-                parent = Plan(self.x1, None if self.same else self.x2, backend="auto")
-                parent._hyp_key = None
-            elif parent.x1.data_ptr() != self.x1.data_ptr():
-                # the factor plans were re-pointed to new inputs (_get_plan_locked): follow them
-                parent.x1 = self.x1.contiguous()
-                parent.x2 = parent.x1 if self.same else self.x2.contiguous()
-                parent.refresh_data()
-            _PRODUCT_PLANS[key] = parent
-            while len(_PRODUCT_PLANS) > 16:
-                _PRODUCT_PLANS.pop(next(iter(_PRODUCT_PLANS))).close()
+        x2 = None if self.same else self.x2
+        parent = _parent_plan(_PRODUCT_PLANS, tuple(id(f) for f in factors), lambda: Plan(self.x1, x2, backend="auto"), self.x1, x2)
         # the factors may have been re-created / re-packed since the last use: (re-)attach them every time (validation only),
         # then set the noise of the product
         parent.set_product(factors)
@@ -1394,12 +1440,8 @@ class ProductKernelLinearOperator(KernelLinearOperator):
                                   "available on the accelerated path")
 
 
-_PRODUCT_PLANS: "dict[tuple, Plan]" = {}
-
-
 ADDITIVE_MAX_COMPONENTS = 32
 ADDITIVE_MAX_DEGREE = 8
-_ADDITIVE_SLOT = 16        # plan-cache slot of additive operators (sum terms 1..4, product factors 5..8, low-rank 8)
 _ADDITIVE_KINDS = ("rbf", "matern12", "matern32", "matern52")
 _ADDITIVE_X: "collections.OrderedDict[tuple, list]" = collections.OrderedDict()
 _ADDITIVE_X_ROLES = 8      # stacked inputs kept: the most recently used roles (shape, side, device), two buffers each
@@ -1460,6 +1502,10 @@ class AdditiveKernelLinearOperator(KernelLinearOperator):
     reaches batched [D, 1, 1] / [D] parameters and sums the gradients of a shared one.  1 <= D <= 32, M <= 8 after clamping to D;
     gradients with respect to the inputs are not available."""
 
+    _family = "additive"
+    _noun = "additive"
+    _sum_term = _factor = _single_plan = False
+
     def __init__(self, ops, max_degree=1):
         self.ops = _additive_components(ops, "AdditiveKernelLinearOperator")
         D = len(self.ops)
@@ -1478,6 +1524,7 @@ class AdditiveKernelLinearOperator(KernelLinearOperator):
         self.lengthscale, self.outputscale = first.lengthscale, first.outputscale   # representative only (device / dtype)
         self._comm, self._row_begin, self._row_count = None, 0, 0
         self._plan = None
+        self._plan_slot = _slot("additive", "own")
 
     def hyper_tensors(self):
         return [t for o in self.ops for t in o.hyper_tensors()]
@@ -1506,7 +1553,7 @@ class AdditiveKernelLinearOperator(KernelLinearOperator):
         fresh = False
         if self._plan is None:
             self._plan = _get_plan(self.x1, None if self.same else self.x2, "auto", 0, 0, None,
-                                   getattr(self, "_plan_slot", _ADDITIVE_SLOT), owner=self)
+                                   self._plan_slot, owner=self)
             fresh = True
         if torch.is_tensor(noise):
             ls, sc, nz, _ = self._host_hypers(noise)
@@ -1587,11 +1634,6 @@ class AdditiveKernelLinearOperator(KernelLinearOperator):
 SPECTRAL_MAX_MIXTURES = 16
 SPECTRAL_MAX_DIMS = 8
 SPECTRAL_MAX_QD = 32
-_SPECTRAL_SLOT = 20        # plan-cache slot of spectral mixture operators (the other operator families use 1..8, 16, 24 and 28)
-# plan-cache slot of the spectral base of a low-rank operator (LOVE's K** - U U^T): its plan carries U, so it must never serve an
-# ordinary spectral operator over the same points; nor may it share the plain low-rank slot, whose operators would inherit the
-# plan's spectral setting when the cache re-points it
-_SPECTRAL_LOWRANK_SLOT = 21
 
 
 class SpectralMixtureKernelLinearOperator(KernelLinearOperator):
@@ -1601,6 +1643,12 @@ class SpectralMixtureKernelLinearOperator(KernelLinearOperator):
     scales [Q, 1, d] (or [Q, d]) are the constrained parameter tensors, or their slices for one element of a batch; autograd reaches
     them through _bilinear_derivative_list.  S is the outputscale of a ScaleKernel around the kernel (None: 1, no gradient).
     1 <= Q <= 16, 1 <= d <= 8, Q d <= 32; gradients with respect to the inputs are not available."""
+
+    _family = "spectral"
+    _noun = "spectral mixture"
+    _sum_term = _factor = _input_grads = _row_sharding = False
+    _params = ("weights", "means", "scales")
+    _plan_backend = "auto"
 
     def __init__(self, x1, x2, weights, means, scales, outputscale=None):
         super().__init__(x1, x2, "rbf", torch.ones((), device=x1.device), outputscale)
@@ -1616,118 +1664,27 @@ class SpectralMixtureKernelLinearOperator(KernelLinearOperator):
             raise NotImplementedError("gradients with respect to the inputs of a spectral mixture operator (deep kernel learning, "
                                       "test-input gradients) are not available on the accelerated path")
         self.weights, self.means, self.scales = weights, means, scales
-        self._scaled = outputscale is not None
         self.num_mixtures = Q
 
-    def hyper_tensors(self):
-        return [self.weights, self.means, self.scales] + ([self.outputscale] if self._scaled else [])
-
-    def input_tensors(self):
-        return []
-
-    def solve_input_tensors(self):
-        return []
-
     @property
-    def requires_grad(self):
-        return any(t.requires_grad for t in self.hyper_tensors())
+    def _scale_is_hyper(self):
+        return self._scaled      # without a ScaleKernel S = 1 has no gradient
 
-    def representation(self):
-        return (self.x1, self.x2, *self.hyper_tensors())
+    def _ctor_args(self):
+        return (self.weights, self.means, self.scales)
 
-    def _host_hypers(self, noise_t=None):
-        """(weights, means, scales, S, noise) as host lists with one device -> host read."""
-        cached = getattr(self, "_hyp_host", None)
-        if cached is None or (noise_t is not None and cached[5] is not noise_t):
-            parts = [t.detach().reshape(-1).float() for t in (self.weights, self.means, self.scales)]
-            parts.append(self.outputscale.detach().reshape(1).float().to(self.weights.device))
-            if noise_t is not None:
-                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.weights.device))
-            vals = torch.cat(parts).tolist()
-            Q, k = self.num_mixtures, self.means.numel()
-            cached = (vals[:Q], vals[Q:Q + k], vals[Q + k:Q + 2 * k], vals[Q + 2 * k], vals[Q + 2 * k + 1] if noise_t is not None else None,
-                      noise_t)
-            self._hyp_host = cached
-        return cached
-
-    def plan(self, noise=0.0) -> Plan:
-        fresh = False
-        if self._plan is None:
-            slot = _SPECTRAL_LOWRANK_SLOT if getattr(self, "_plan_slot", None) == _LOWRANK_SLOT else _SPECTRAL_SLOT
-            self._plan = _get_plan(self.x1, None if self.same else self.x2, "auto", 0, 0, None, slot, owner=self)
-            fresh = True
-        if torch.is_tensor(noise):
-            w, mu, v, os_, nz, _ = self._host_hypers(noise)
-        else:
-            w, mu, v, os_, _, _ = self._host_hypers(None)
-            nz = float(noise)
-        p = self._plan
-        key = ("rbf", (1.0,), os_, nz)
-        if fresh or getattr(p, "_hyp_key", None) != key:
-            p.set_hypers("rbf", 1.0, os_, nz)   # outputscale and noise; the kind and lengthscale are not used
-            p._hyp_key = key
-        skey = (tuple(w), tuple(mu), tuple(v))
-        if fresh or getattr(p, "_sm_key", None) != skey:   # re-sent only when the parameters' host values change
-            p.set_spectral(w, torch.tensor(mu).reshape(len(w), -1), torch.tensor(v).reshape(len(w), -1))
-            p._sm_key = skey
-        return p
-
-    def _bilinear_derivative_list(self, left, right):
-        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
-        vals = torch.tensor(gl, device=self.device, dtype=self.weights.dtype)
-        Q, k = self.num_mixtures, self.means.numel()
-        out = [vals[:Q].reshape(self.weights.shape), vals[Q:Q + k].reshape(self.means.shape), vals[Q + k:].reshape(self.scales.shape)]
-        if self._scaled:
-            out.append(torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape))
-        return out
-
-    def _bilinear_derivative(self, left, right):
-        raise NotImplementedError("a spectral mixture operator has weight, mean and scale gradients: use _bilinear_derivative_list")
-
-    def _input_grad_list(self, *args):
-        raise NotImplementedError("gradients with respect to the inputs of a spectral mixture operator are not available on the "
-                                  "accelerated path")
-
-    _dense_input_grad_list = _input_grad_list
-
-    def _with(self, x1, x2, detach=False):
-        f = (lambda t: t.detach()) if detach else (lambda t: t)
-        return SpectralMixtureKernelLinearOperator(f(x1), None if x2 is None else f(x2), f(self.weights), f(self.means),
-                                                   f(self.scales), f(self.outputscale) if self._scaled else None)
-
-    def _transpose_nonbatch(self):
-        return self if self.same else self._with(self.x2, self.x1)
-
-    def detach(self):
-        return self._with(self.x1, None if self.same else self.x2, detach=True)
-
-    def __getitem__(self, index):
-        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
-        if not isinstance(index, tuple):
-            index = (index, slice(None))
-        ri, ci = index
-        if isinstance(ri, int):
-            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
-        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
-
-    def __add__(self, other):
-        if isinstance(other, (ConstantDiagLinearOperator, DiagLinearOperator)):
-            return AddedDiagLinearOperator(self, other)
-        raise NotImplementedError("a spectral mixture operator adds a (Constant)DiagLinearOperator only: sums that contain spectral "
-                                  "mixture operators are not available on the accelerated path")
-
-    def mul(self, other):
-        raise NotImplementedError("products that contain a spectral mixture operator are not available on the accelerated path")
-
-    __mul__ = mul
+    def _engine_calls(self, hyp, nz):
+        w, mu, v = hyp[:3]
+        os_ = hyp[3][0] if self._scaled else 1.0
+        Q = len(w)
+        # set_hypers carries the outputscale and noise (the kind and lengthscale are not used); set_spectral is re-sent only when
+        # the parameters' host values change
+        return [("_hyp_key", ("rbf", (1.0,), os_, nz), lambda p: p.set_hypers("rbf", 1.0, os_, nz)),
+                ("_sm_key", (tuple(w), tuple(mu), tuple(v)),
+                 lambda p: p.set_spectral(w, torch.tensor(mu).reshape(Q, -1), torch.tensor(v).reshape(Q, -1)))]
 
 
 PERIODIC_MAX_DIMS = 16
-_PERIODIC_SLOT = 32        # plan-cache slot of periodic operators (the other operator families use 0..8, 16, 20/21, 24 and 28)
-# the periodic base of a low-rank operator (LOVE's K** - U U^T) carries U: it never serves an ordinary periodic operator, and a
-# periodic plan is never handed to a plain low-rank operator (a plan the cache re-points keeps its periodic setting)
-_PERIODIC_LOWRANK_SLOT = 33
-_PERIODIC_SUM_SLOT = 34    # periodic terms of a kernel sum: 34 + term index, as plain terms take 1 + term index
 
 
 class PeriodicKernelLinearOperator(KernelLinearOperator):
@@ -1738,8 +1695,15 @@ class PeriodicKernelLinearOperator(KernelLinearOperator):
     them through _bilinear_derivative_list.  S is the outputscale of a ScaleKernel around the kernel (None: 1, no gradient).
     1 <= d <= 16; gradients with respect to the inputs are not available."""
 
+    _family = "periodic"
+    _noun = "periodic"
+    _factor = _input_grads = _row_sharding = False
+    _params = ("lengthscale", "period")
+    # set_periodic repacks the embedding: a cached plan keeps the setting its keys record, so a new operator over the same plan
+    # with the same parameters packs nothing
+    _resend_on_new_plan = False
+
     def __init__(self, x1, x2, lengthscale, period, outputscale=None, comm=None, row_begin=0, row_count=0):
-        super().__init__(x1, x2, "rbf", lengthscale, outputscale, comm=comm, row_begin=row_begin, row_count=row_count)
         d = x1.size(-1)
         if not 1 <= d <= PERIODIC_MAX_DIMS:
             raise NotImplementedError(f"a periodic operator takes 1 <= d <= {PERIODIC_MAX_DIMS} input dimensions on the accelerated "
@@ -1750,106 +1714,16 @@ class PeriodicKernelLinearOperator(KernelLinearOperator):
         if x1.requires_grad or (x2 is not None and x2.requires_grad):
             raise NotImplementedError("gradients with respect to the inputs of a periodic operator (deep kernel learning, test-input "
                                       "gradients) are not available on the accelerated path")
-        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
-            raise NotImplementedError("a row-sharded periodic operator is not available on the accelerated path")
+        super().__init__(x1, x2, "rbf", lengthscale, outputscale, comm=comm, row_begin=row_begin, row_count=row_count)
         self.period = period
 
-    def hyper_tensors(self):
-        return [self.lengthscale, self.period, self.outputscale]
+    def _ctor_args(self):
+        return (self.lengthscale, self.period)
 
-    def input_tensors(self):
-        return []
-
-    def solve_input_tensors(self):
-        return []
-
-    @property
-    def requires_grad(self):
-        return any(t.requires_grad for t in self.hyper_tensors())
-
-    def representation(self):
-        return (self.x1, self.x2, *self.hyper_tensors())
-
-    def _host_hypers(self, noise_t=None):
-        """(lengthscale list, outputscale, noise, noise tensor, period list) with one device -> host read."""
-        cached = getattr(self, "_hyp_host", None)
-        if cached is None or (noise_t is not None and cached[3] is not noise_t):
-            parts = [t.detach().reshape(-1).float().to(self.device) for t in (self.lengthscale, self.outputscale, self.period)]
-            if noise_t is not None:
-                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.device))
-            vals = torch.cat(parts).tolist()
-            nl, npr = self.lengthscale.numel(), self.period.numel()
-            cached = (vals[:nl], vals[nl], vals[nl + 1 + npr] if noise_t is not None else None, noise_t, vals[nl + 1:nl + 1 + npr])
-            self._hyp_host = cached
-        return cached
-
-    def _slot(self):
-        slot = getattr(self, "_plan_slot", None)
-        if slot is None:
-            return _PERIODIC_SLOT
-        return _PERIODIC_LOWRANK_SLOT if slot == _LOWRANK_SLOT else slot
-
-    def plan(self, noise=0.0) -> Plan:
-        if self._plan is None:
-            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None, self._slot(),
-                                   owner=self)
-        if torch.is_tensor(noise):
-            ls, os_, nz, _, per = self._host_hypers(noise)
-        else:
-            ls, os_, _, _, per = self._host_hypers(None)
-            nz = float(noise)
-        p = self._plan
-        # re-sent only when the host values change: a cached plan keeps the setting (and packing) its keys record, so a new
-        # operator over the same plan with the same parameters packs nothing
-        if getattr(p, "_per_key", None) != tuple(per):
-            p.set_periodic(per)
-            p._per_key = tuple(per)
-        key = ("rbf", tuple(ls), os_, nz)
-        if getattr(p, "_hyp_key", None) != key:
-            p.set_hypers("rbf", ls, os_, nz)
-            p._hyp_key = key
-        return p
-
-    def _bilinear_derivative_list(self, left, right):
-        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
-        vals = torch.tensor(gl, device=self.device, dtype=self.lengthscale.dtype)
-        nl = self.lengthscale.numel()
-        return [vals[:nl].reshape(self.lengthscale.shape), vals[nl:].to(self.period.dtype).reshape(self.period.shape),
-                torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape)]
-
-    def _bilinear_derivative(self, left, right):
-        raise NotImplementedError("a periodic operator has lengthscale, period and outputscale gradients: use _bilinear_derivative_list")
-
-    def _input_grad_list(self, *args):
-        raise NotImplementedError("gradients with respect to the inputs of a periodic operator are not available on the accelerated "
-                                  "path")
-
-    _dense_input_grad_list = _input_grad_list
-
-    def _with(self, x1, x2, detach=False, outputscale=None):
-        f = (lambda t: t.detach()) if detach else (lambda t: t)
-        return PeriodicKernelLinearOperator(f(x1), None if x2 is None else f(x2), f(self.lengthscale), f(self.period),
-                                            f(self.outputscale if outputscale is None else outputscale))
-
-    def _transpose_nonbatch(self):
-        return self if self.same else self._with(self.x2, self.x1)
-
-    def detach(self):
-        return self._with(self.x1, None if self.same else self.x2, detach=True)
-
-    def __getitem__(self, index):
-        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
-        if not isinstance(index, tuple):
-            index = (index, slice(None))
-        ri, ci = index
-        if isinstance(ri, int):
-            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
-        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
-
-    def mul(self, other):
-        raise NotImplementedError("products that contain a periodic operator are not available on the accelerated path")
-
-    __mul__ = mul
+    def _engine_calls(self, hyp, nz):
+        ls, per, (os_,) = hyp
+        return [("_per_key", tuple(per), lambda p: p.set_periodic(per)),
+                ("_hyp_key", ("rbf", tuple(ls), os_, nz), lambda p: p.set_hypers("rbf", ls, os_, nz))]
 
 
 class RQKernelLinearOperator(KernelLinearOperator):
@@ -1857,92 +1731,25 @@ class RQKernelLinearOperator(KernelLinearOperator):
     plan of kind GP_RQ (gp_plan_set_hypers_rq): products, solves, the preconditioner, SLQ, rows and input gradients run on the plain
     tensor-core / CUDA-core kernels with the RQ covariance in their epilogue.  lengthscale holds 1 or d values and alpha one (the
     parameter tensors or their slices for one element of a batch); autograd reaches them through _bilinear_derivative_list.  S is
-    the outputscale of a ScaleKernel around the kernel (None: 1, no gradient).  The plan-cache slots are the plain ones: the kind
-    and alpha are part of the plan's hyper-parameter key, so a plan re-sends them whenever another kind used it last."""
+    the outputscale of a ScaleKernel around the kernel (None: 1, no gradient).  The plan-cache slots are the plain ones (_slot)."""
+
+    _family = "rq"
+    _noun = "rational quadratic (RQ)"
+    _factor = _row_sharding = False
+    _params = ("lengthscale", "alpha")
 
     def __init__(self, x1, x2, lengthscale, alpha, outputscale=None, comm=None, row_begin=0, row_count=0):
-        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
-            raise NotImplementedError("a row-sharded rational quadratic (RQ) operator is not available on the accelerated path")
-        super().__init__(x1, x2, "rq", lengthscale, outputscale)
+        super().__init__(x1, x2, "rq", lengthscale, outputscale, comm=comm, row_begin=row_begin, row_count=row_count)
         if alpha.numel() != 1:
             raise RuntimeError(f"RQ kernel: alpha must hold one value (got shape {tuple(alpha.shape)})")
         self.alpha = alpha
 
-    def hyper_tensors(self):
-        return [self.lengthscale, self.alpha, self.outputscale]
+    def _ctor_args(self):
+        return (self.lengthscale, self.alpha)
 
-    @property
-    def requires_grad(self):
-        return any(t.requires_grad for t in self.hyper_tensors())
-
-    def representation(self):
-        return (self.x1, self.x2, *self.hyper_tensors())
-
-    def _host_hypers(self, noise_t=None):
-        """(lengthscale list, outputscale, noise, noise tensor, alpha) with one device -> host read."""
-        cached = getattr(self, "_hyp_host", None)
-        if cached is None or (noise_t is not None and cached[3] is not noise_t):
-            parts = [t.detach().reshape(-1).float().to(self.device) for t in (self.lengthscale, self.outputscale, self.alpha)]
-            if noise_t is not None:
-                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.device))
-            vals = torch.cat(parts).tolist()
-            nl = self.lengthscale.numel()
-            cached = (vals[:nl], vals[nl], vals[nl + 2] if noise_t is not None else None, noise_t, vals[nl + 1])
-            self._hyp_host = cached
-        return cached
-
-    def plan(self, noise=0.0) -> Plan:
-        fresh = False
-        if self._plan is None:
-            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None,
-                                   getattr(self, "_plan_slot", 0), owner=self)
-            fresh = True
-        if torch.is_tensor(noise):
-            ls, os_, nz, _, al = self._host_hypers(noise)
-        else:
-            ls, os_, _, _, al = self._host_hypers(None)
-            nz = float(noise)
-        key = ("rq", tuple(ls), al, os_, nz)
-        if fresh or getattr(self._plan, "_hyp_key", None) != key:
-            self._plan.set_hypers_rq(ls, al, os_, nz)
-            self._plan._hyp_key = key
-        return self._plan
-
-    def _bilinear_derivative_list(self, left, right):
-        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
-        vals = torch.tensor(gl, device=self.device, dtype=self.lengthscale.dtype)
-        nl = self.lengthscale.numel()
-        return [vals[:nl].reshape(self.lengthscale.shape), vals[nl:].to(self.alpha.dtype).reshape(self.alpha.shape),
-                torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape)]
-
-    def _bilinear_derivative(self, left, right):
-        raise NotImplementedError("an RQ operator has lengthscale, alpha and outputscale gradients: use _bilinear_derivative_list")
-
-    def _with(self, x1, x2, detach=False, outputscale=None):
-        f = (lambda t: t.detach()) if detach else (lambda t: t)
-        return RQKernelLinearOperator(f(x1), None if x2 is None else f(x2), f(self.lengthscale), f(self.alpha),
-                                      f(self.outputscale if outputscale is None else outputscale))
-
-    def _transpose_nonbatch(self):
-        return self if self.same else self._with(self.x2, self.x1)
-
-    def detach(self):
-        return self._with(self.x1, None if self.same else self.x2, detach=True)
-
-    def __getitem__(self, index):
-        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
-        if not isinstance(index, tuple):
-            index = (index, slice(None))
-        ri, ci = index
-        if isinstance(ri, int):
-            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
-        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
-
-    def mul(self, other):
-        raise NotImplementedError("products that contain a rational quadratic (RQ) operator (kernel products, IndexKernel "
-                                  "multitask models) are not available on the accelerated path")
-
-    __mul__ = mul
+    def _engine_calls(self, hyp, nz):
+        ls, (al,), (os_,) = hyp
+        return [("_hyp_key", ("rq", tuple(ls), al, os_, nz), lambda p: p.set_hypers_rq(ls, al, os_, nz))]
 
 
 class PolynomialKernelLinearOperator(KernelLinearOperator):
@@ -1951,94 +1758,28 @@ class PolynomialKernelLinearOperator(KernelLinearOperator):
     run on the plain tensor-core / CUDA-core kernels with (x . x' + c)^p in their epilogue.  power is a Python int in [1, 8], offset
     one value (the parameter tensor or its slice for one element of a batch); autograd reaches the offset and S through
     _bilinear_derivative_list.  The kernel is not stationary: diagonal() is S (|x_i|^2 + c)^p from the plan.  The plan-cache slots
-    are the plain ones: kind, power and offset are part of the plan's hyper-parameter key."""
+    are the plain ones (_slot)."""
+
+    _family = "poly"
+    _noun = "PolynomialKernel"
+    _factor = _row_sharding = False
+    _params = ("offset",)
 
     def __init__(self, x1, x2, power, offset, outputscale=None, comm=None, row_begin=0, row_count=0):
-        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
-            raise NotImplementedError("a row-sharded polynomial operator is not available on the accelerated path")
+        # no lengthscale: a constant stands in where the generic code reads one (device / dtype only)
+        super().__init__(x1, x2, "poly", torch.ones((), device=x1.device, dtype=offset.dtype), outputscale, comm=comm,
+                         row_begin=row_begin, row_count=row_count)
         if offset.numel() != 1:
             raise RuntimeError(f"polynomial kernel: offset must hold one value (got shape {tuple(offset.shape)})")
-        # no lengthscale: a constant stands in where the generic code reads one (device / dtype only)
-        super().__init__(x1, x2, "poly", torch.ones((), device=x1.device, dtype=offset.dtype), outputscale)
         self.power = int(power)
         self.offset = offset
 
-    def hyper_tensors(self):
-        return [self.offset, self.outputscale]
+    def _ctor_args(self):
+        return (self.power, self.offset)
 
-    @property
-    def requires_grad(self):
-        return any(t.requires_grad for t in self.hyper_tensors())
-
-    def representation(self):
-        return (self.x1, self.x2, *self.hyper_tensors())
-
-    def _host_hypers(self, noise_t=None):
-        """(offset, outputscale, noise, noise tensor) with one device -> host read."""
-        cached = getattr(self, "_hyp_host", None)
-        if cached is None or (noise_t is not None and cached[3] is not noise_t):
-            parts = [t.detach().reshape(-1).float().to(self.device) for t in (self.offset, self.outputscale)]
-            if noise_t is not None:
-                parts.append(noise_t.detach().reshape(-1)[:1].float().to(self.device))
-            vals = torch.cat(parts).tolist()
-            cached = (vals[0], vals[1], vals[2] if noise_t is not None else None, noise_t)
-            self._hyp_host = cached
-        return cached
-
-    def plan(self, noise=0.0) -> Plan:
-        fresh = False
-        if self._plan is None:
-            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None,
-                                   getattr(self, "_plan_slot", 0), owner=self)
-            fresh = True
-        if torch.is_tensor(noise):
-            off, os_, nz, _ = self._host_hypers(noise)
-        else:
-            off, os_, _, _ = self._host_hypers(None)
-            nz = float(noise)
-        key = ("poly", self.power, off, os_, nz)
-        if fresh or getattr(self._plan, "_hyp_key", None) != key:
-            self._plan.set_hypers_poly(self.power, off, os_, nz)
-            self._plan._hyp_key = key
-        return self._plan
-
-    def _bilinear_derivative_list(self, left, right):
-        gl, go = self.plan(getattr(self, "_last_noise", 0.0)).bilinear_grad(left, right)
-        return [torch.tensor(gl[0], device=self.device, dtype=self.offset.dtype).reshape(self.offset.shape),
-                torch.tensor(go, device=self.device, dtype=self.outputscale.dtype).reshape(self.outputscale.shape)]
-
-    def _bilinear_derivative(self, left, right):
-        raise NotImplementedError("a polynomial operator has offset and outputscale gradients: use _bilinear_derivative_list")
-
-    def _with(self, x1, x2, detach=False, outputscale=None):
-        f = (lambda t: t.detach()) if detach else (lambda t: t)
-        return PolynomialKernelLinearOperator(f(x1), None if x2 is None else f(x2), self.power, f(self.offset),
-                                              f(self.outputscale if outputscale is None else outputscale))
-
-    def _transpose_nonbatch(self):
-        return self if self.same else self._with(self.x2, self.x1)
-
-    def detach(self):
-        return self._with(self.x1, None if self.same else self.x2, detach=True)
-
-    def __getitem__(self, index):
-        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
-        if not isinstance(index, tuple):
-            index = (index, slice(None))
-        ri, ci = index
-        if isinstance(ri, int):
-            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
-        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
-
-    def mul(self, other):
-        raise NotImplementedError("products that contain a PolynomialKernel operator (kernel products, IndexKernel multitask "
-                                  "models) are not available on the accelerated path")
-
-    __mul__ = mul
-
-
-_PP_SLOT = 44           # plan-cache slot of piecewise polynomial operators (the other families use 0..8, 16, 20/21, 24, 28, 32..37
-_PP_LOWRANK_SLOT = 45   # and 40..43); their low-rank-corrected plans (lazy LOVE), as periodic operators keep theirs apart
+    def _engine_calls(self, hyp, nz):
+        (off,), (os_,) = hyp
+        return [("_hyp_key", ("poly", self.power, off, os_, nz), lambda p: p.set_hypers_poly(self.power, off, os_, nz))]
 
 
 class PiecewisePolynomialKernelLinearOperator(KernelLinearOperator):
@@ -2050,84 +1791,31 @@ class PiecewisePolynomialKernelLinearOperator(KernelLinearOperator):
     autograd reaches the lengthscale and S through _bilinear_derivative_list.  Sums, products, multitask use, row sharding and
     gradients with respect to the inputs are refused."""
 
+    _family = "ppoly"
+    _noun = "PiecewisePolynomialKernel"
+    _sum_term = _factor = _input_grads = _row_sharding = False
+
     def __init__(self, x1, x2, q, lengthscale, outputscale=None, comm=None, row_begin=0, row_count=0):
-        if comm is not None or row_begin != 0 or row_count not in (0, x1.size(0)):
-            raise NotImplementedError("a row-sharded PiecewisePolynomialKernel operator is not available on the accelerated path")
+        super().__init__(x1, x2, "ppoly", lengthscale, outputscale, comm=comm, row_begin=row_begin, row_count=row_count)
         if torch.is_grad_enabled() and (x1.requires_grad or (x2 is not None and x2.requires_grad)):
             raise NotImplementedError("gradients with respect to the inputs of a PiecewisePolynomialKernel (deep kernel learning, "
                                       "posterior input gradients) are not available on the accelerated path")
-        super().__init__(x1, x2, "ppoly", lengthscale, outputscale)
         self.q = int(q)
 
-    def _slot(self):
-        slot = getattr(self, "_plan_slot", None)
-        return _PP_LOWRANK_SLOT if slot == _LOWRANK_SLOT else _PP_SLOT
+    def _ctor_args(self):
+        return (self.q, self.lengthscale)
 
-    def plan(self, noise=0.0) -> Plan:
-        fresh = False
-        if self._plan is None:
-            self._plan = _get_plan(self.x1, None if self.same else self.x2, settings.backend.value(), 0, 0, None, self._slot(),
-                                   owner=self)
-            fresh = True
-        if torch.is_tensor(noise):
-            ls, os_, nz, _ = self._host_hypers(noise)
-        else:
-            ls, os_, _, _ = self._host_hypers(None)
-            nz = float(noise)
-        key = ("ppoly", self.q, tuple(ls), os_, nz)
-        if fresh or getattr(self._plan, "_hyp_key", None) != key:
-            self._plan.set_hypers_pp(self.q, ls, os_, nz)
-            self._plan._hyp_key = key
-        return self._plan
-
-    def _input_grad_list(self, *args):   # (left, right, needs) or (w, needs)
-        needs = args[-1]
-        if any(needs):
-            raise NotImplementedError("gradients with respect to the inputs of a PiecewisePolynomialKernel are not available on the "
-                                      "accelerated path")
-        return [None] * len(needs)
-
-    _dense_input_grad_list = _input_grad_list
-
-    def _with(self, x1, x2, detach=False, outputscale=None):
-        f = (lambda t: t.detach()) if detach else (lambda t: t)
-        return PiecewisePolynomialKernelLinearOperator(f(x1), None if x2 is None else f(x2), self.q, f(self.lengthscale),
-                                                       f(self.outputscale if outputscale is None else outputscale))
-
-    def _transpose_nonbatch(self):
-        return self if self.same else self._with(self.x2, self.x1)
-
-    def detach(self):
-        return self._with(self.x1, None if self.same else self.x2, detach=True)
-
-    def __getitem__(self, index):
-        """Row / column blocks (the train / test blocks of prediction): a cross plan for x1 != x2."""
-        if not isinstance(index, tuple):
-            index = (index, slice(None))
-        ri, ci = index
-        if isinstance(ri, int):
-            return self.plan().rows(torch.tensor([ri], device=self.device))[0][ci]
-        return self._with(self.x1[ri], (self.x1 if self.same else self.x2)[ci])
-
-    def mul(self, other):
-        raise NotImplementedError("products that contain a PiecewisePolynomialKernel operator (kernel products, IndexKernel "
-                                  "multitask models) are not available on the accelerated path")
-
-    __mul__ = mul
-
-
-def with_outputscale(op, outputscale):
-    """A plain, periodic, RQ or polynomial kernel operator with its outputscale replaced (a ScaleKernel folded into the terms of a
-    sum or into the first factor of a product); the operator's other parameters are kept."""
-    if isinstance(op, (PeriodicKernelLinearOperator, RQKernelLinearOperator, PolynomialKernelLinearOperator,
-                       PiecewisePolynomialKernelLinearOperator)):
-        return op._with(op.x1, None if op.same else op.x2, outputscale=outputscale)
-    return KernelLinearOperator(op.x1, op.x2, op.kind, op.lengthscale, outputscale)
+    def _engine_calls(self, hyp, nz):
+        ls, (os_,) = hyp
+        return [("_hyp_key", ("ppoly", self.q, tuple(ls), os_, nz), lambda p: p.set_hypers_pp(self.q, ls, os_, nz))]
 
 
 class SKIKernelLinearOperator(KernelLinearOperator):
     """K_ski = s W (T_0 x ... x T_{d-1}) W^T (kernels/grid_interpolation_kernel.py:132-213): the engine's SKI backend -- cubic
     interpolation weights kept in compact per-dimension form, Kronecker / Toeplitz grid covariance applied mode by mode."""
+
+    _noun = "SKI"
+    _sum_term = _factor = _single_plan = False
 
     def __init__(self, x1, kind, lengthscale, outputscale, grid_sizes, grid_lo, grid_step):
         super().__init__(x1, None, kind, lengthscale, outputscale)
@@ -2136,15 +1824,13 @@ class SKIKernelLinearOperator(KernelLinearOperator):
     def plan(self, noise=0.0) -> Plan:
         if self._plan is None:
             key = "ski:" + repr((self.grid_sizes, self.grid_lo, self.grid_step))
-            self._plan = _get_plan(self.x1, None, key, 0, 0, None, getattr(self, "_plan_slot", 0), owner=self)
+            self._plan = _get_plan(self.x1, None, key, 0, 0, None, self._plan_slot, owner=self)
             if getattr(self._plan, "_ski_key", None) != key:
                 self._plan.set_ski(self.grid_sizes, self.grid_lo, self.grid_step)
                 self._plan._ski_key = key
                 self._plan._hyp_key = None
-        if torch.is_tensor(noise):
-            ls, os_, nz, _ = self._host_hypers(noise)
-        else:
-            ls, os_, _, _ = self._host_hypers(None)
+        (ls, (os_,)), nz, _ = self._host_hypers(noise if torch.is_tensor(noise) else None)
+        if not torch.is_tensor(noise):
             nz = float(noise)
         hk = (self.kind, tuple(ls), os_, nz)
         if getattr(self._plan, "_hyp_key", None) != hk:
@@ -2176,6 +1862,9 @@ class SKIKernelLinearOperator(KernelLinearOperator):
     def detach(self):
         return SKIKernelLinearOperator(self.x1, self.kind, self.lengthscale.detach(), self.outputscale.detach(), self.grid_sizes,
                                        self.grid_lo, self.grid_step)
+
+    def with_outputscale(self, outputscale):
+        return SKIKernelLinearOperator(self.x1, self.kind, self.lengthscale, outputscale, self.grid_sizes, self.grid_lo, self.grid_step)
 
     def to_dense(self):
         n = self.x1.size(0)
@@ -2277,7 +1966,6 @@ class _SKISliceOperator:
         return self.matmul(torch.eye(self.cols.numel(), device=self.device))
 
 
-_LOWRANK_SLOT = 8   # plan-cache slot of low-rank operators (kernel-sum terms use 1..4): a plain operator never sees their U
 LOWRANK_MAX_RANK = 128
 
 
@@ -2308,7 +1996,7 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
         if U.dim() != 2 or U.size(0) != base.shape[0] or not 1 <= U.size(1) <= LOWRANK_MAX_RANK:
             raise RuntimeError(f"low-rank factor must be [{base.shape[0]}, r] with 1 <= r <= {LOWRANK_MAX_RANK} (got {tuple(U.shape)})")
         self.base = base.detach()
-        self.base._plan_slot = _LOWRANK_SLOT
+        self.base._plan_slot = _slot(self.base._family, "lowrank")   # a plan carrying U never serves an operator without it
         self.U = U.detach().float().contiguous()
 
     @classmethod
@@ -2325,11 +2013,8 @@ class LowRankUpdatedKernelLinearOperator(_SamplingMixin):
     @staticmethod
     def supports(base) -> bool:
         """A plan-backed non-SKI kernel operator (or kernel sum) without batch dimension on an unsharded square plan."""
-        return (isinstance(base, KernelLinearOperator) and not isinstance(base, (SKIKernelLinearOperator, HadamardKernelLinearOperator,
-                                                                                          KroneckerKernelLinearOperator,
-                                                                                          LCMKernelLinearOperator,
-                                                                                          DerivKernelLinearOperator,
-                                                                                          ProductKernelLinearOperator))
+        return (isinstance(base, KernelLinearOperator)
+                and (base._single_plan or isinstance(base, (SumKernelLinearOperator, AdditiveKernelLinearOperator)))
                 and base.same
                 and base._comm is None and base._row_begin == 0 and base._row_count in (0, base.shape[0]))
 

@@ -76,7 +76,7 @@ def test_kernel_parameters_setters_and_refusals():
         mk.forward(torch.zeros(4, 1), torch.zeros(4, 1))
 
 
-def test_operator_dispatch_and_refusals():
+def test_operator_dispatch_refusals_and_slot_keys():
     from gpytorch_b200 import kernels, operators as ops
 
     x = torch.randn(10, 2)
@@ -93,7 +93,7 @@ def test_operator_dispatch_and_refusals():
     so = s(x)
     assert isinstance(so, ops.SumKernelLinearOperator)
     assert isinstance(so.ops[0], ops.PeriodicKernelLinearOperator) and type(so.ops[1]) is ops.KernelLinearOperator
-    assert so.ops[0]._slot() == ops._PERIODIC_SUM_SLOT and so.ops[1]._plan_slot == 2
+    assert so.ops[0]._plan_slot == ops._slot("periodic", "sum_term", 0) and so.ops[1]._plan_slot == ops._slot("plain", "sum_term", 1)
     sc = kernels.ScaleKernel(kernels.PeriodicKernel() + kernels.RBFKernel())(x)
     assert isinstance(sc.ops[0], ops.PeriodicKernelLinearOperator) and sc.ops[0].period is not None
     b = kernels.ScaleKernel(kernels.PeriodicKernel(batch_shape=torch.Size([3])))(torch.randn(3, 10, 1))
@@ -119,17 +119,16 @@ def test_gradients_split_onto_parameter_shapes():
     assert g[0].tolist() == [1.0, 2.0] and g[1].tolist() == [3.0, 4.0] and float(g[2]) == 6.0
 
 
-def test_plan_slots_are_disjoint():
+def test_plan_slot_keys_are_disjoint():
     from gpytorch_b200 import operators as ops
 
-    used = {0, *range(1, 9), ops._TASK_SLOT, ops._SPECTRAL_SLOT, ops._SPECTRAL_LOWRANK_SLOT, ops._KRON_SLOT, ops._DERIV_SLOT,
-            ops._ADDITIVE_SLOT}
-    mine = {ops._PERIODIC_SLOT, ops._PERIODIC_LOWRANK_SLOT, *range(ops._PERIODIC_SUM_SLOT, ops._PERIODIC_SUM_SLOT + 4)}
+    others = ("plain", "rq", "poly", "task", "spectral", "kron", "deriv", "additive", "lcm", "ppoly", "sum", "product")
+    used = {ops._slot(f, r, i) for f in others for r in ops._SLOT_ROLES for i in range(4)}
+    mine = {ops._slot("periodic", "own"), ops._slot("periodic", "lowrank"), *(ops._slot("periodic", "sum_term", i) for i in range(4))}
     assert len(mine) == 6 and not (mine & used)
     op = ops.PeriodicKernelLinearOperator(torch.zeros(4, 1), None, torch.tensor(1.0), torch.tensor(2.0))
-    assert op._slot() == ops._PERIODIC_SLOT
-    op._plan_slot = ops._LOWRANK_SLOT
-    assert op._slot() == ops._PERIODIC_LOWRANK_SLOT
+    assert op._plan_slot == ops._slot("periodic", "own")
+    assert ops.LowRankUpdatedKernelLinearOperator(op, torch.ones(4, 1)).base._plan_slot == ops._slot("periodic", "lowrank")
 
 
 def test_c_abi_declares_periodic():

@@ -59,7 +59,7 @@ def test_mutants_fall_outside_the_bound(path):
     assert bool(((K @ V.double() - ref).abs() <= bnd).all())
 
 
-def test_class_surface_and_wrappers():
+def test_class_surface_and_wrapper_methods():
     import gpytorch_b200 as gp
     from gpytorch_b200.operators import PolynomialKernelLinearOperator, SumKernelLinearOperator
 
@@ -88,7 +88,7 @@ def test_class_surface_and_wrappers():
     assert isinstance(s, SumKernelLinearOperator) and isinstance(s.ops[0], PolynomialKernelLinearOperator)
     s2 = gp.kernels.ScaleKernel(gp.kernels.PolynomialKernel(4) + gp.kernels.RBFKernel())(x)
     assert s2.ops[0].power == 4
-    for o in (op.detach(), op._transpose_nonbatch(), op[1:4, :], gp.operators.with_outputscale(op, torch.tensor(2.0))):
+    for o in (op.detach(), op._transpose_nonbatch(), op[1:4, :], op.with_outputscale(torch.tensor(2.0))):
         assert isinstance(o, PolynomialKernelLinearOperator) and o.power == 2 and abs(float(o.offset) - 0.7) < 1e-6
     assert gp.operators.LowRankUpdatedKernelLinearOperator.supports(op)
     with pytest.raises(NotImplementedError, match="PolynomialKernel"):

@@ -35,7 +35,7 @@ def test_love_posterior_dominates_the_exact_posterior(J):
 
 
 def test_posterior_branch_precedence_and_fallback():
-    from gpytorch_b200 import settings
+    from gpytorch_b200 import operators, settings
     from gpytorch_b200.models import _posterior_covar_mode
     from gpytorch_b200.operators import (BatchLinearOperator, KernelLinearOperator, LowRankUpdatedKernelLinearOperator,
                                          SKIKernelLinearOperator, SumKernelLinearOperator)
@@ -67,7 +67,8 @@ def test_posterior_branch_precedence_and_fallback():
     with pytest.raises(RuntimeError):
         LowRankUpdatedKernelLinearOperator(plain, torch.zeros(50, 129))
     op = LowRankUpdatedKernelLinearOperator(plain, torch.zeros(50, 3))
-    assert op.shape == (50, 50) and op.hyper_tensors() == [] and not op.requires_grad and op.base._plan_slot != 0
+    assert op.shape == (50, 50) and op.hyper_tensors() == [] and not op.requires_grad
+    assert op.base._plan_slot == operators._slot("plain", "lowrank") != plain._plan_slot
 
 
 def test_lowrank_kernels_are_spill_free():

@@ -125,7 +125,7 @@ def test_mutants_fall_outside_the_bound():
         assert bool(((Km @ V.double() - ref).abs() > bnd).any()), name
 
 
-def test_class_surface_and_refusals():
+def test_class_surface_wrapper_methods_and_refusals():
     import gpytorch_b200 as gp
     from gpytorch_b200.operators import PiecewisePolynomialKernelLinearOperator
 
@@ -149,7 +149,7 @@ def test_class_surface_and_refusals():
     k.lengthscale = 0.7
     op = gp.kernels.ScaleKernel(gp.kernels.ScaleKernel(k))(x)
     assert isinstance(op, PiecewisePolynomialKernelLinearOperator) and op.q == 2 and abs(float(op.lengthscale) - 0.7) < 1e-6
-    for o in (op.detach(), op._transpose_nonbatch(), op[1:4, :], gp.operators.with_outputscale(op, torch.tensor(2.0))):
+    for o in (op.detach(), op._transpose_nonbatch(), op[1:4, :], op.with_outputscale(torch.tensor(2.0))):
         assert isinstance(o, PiecewisePolynomialKernelLinearOperator) and o.q == 2
     assert gp.kernels.PiecewisePolynomialKernel(active_dims=[0, 2])(x).x1.shape[1] == 2
     assert gp.operators.LowRankUpdatedKernelLinearOperator.supports(op)

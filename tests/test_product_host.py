@@ -79,7 +79,9 @@ def test_operator_refusals_and_algebra(gp, monkeypatch):
     p = a.mul(b)
     assert isinstance(p, ops.ProductKernelLinearOperator) and [o.kind for o in p.ops] == ["rbf", "matern12"]
     assert [o.kind for o in (p * mk("matern52")).ops] == ["rbf", "matern12", "matern52"]
-    assert len({o._plan_slot for o in p.ops}) == 2 and p.input_tensors() == [] and p.solve_input_tensors() == []
+    assert [o._plan_slot for o in p.ops] == [ops._slot("plain", "product_factor", i) for i in range(2)]
+    assert ops._slot("plain", "lowrank") not in [ops._slot("plain", "product_factor", i) for i in range(4)]
+    assert p.input_tensors() == [] and p.solve_input_tensors() == []
     assert len(p.hyper_tensors()) == 4 and tuple(p.shape) == (6, 6)
     assert isinstance(p + ops.ConstantDiagLinearOperator(torch.tensor(0.1), 6), ops.AddedDiagLinearOperator)
     with pytest.raises(NotImplementedError, match="sums that contain products"):

@@ -146,17 +146,19 @@ def _is_rq_with(o, alpha):
     return isinstance(o, operators.RQKernelLinearOperator) and float(o.alpha) == alpha
 
 
-def test_every_wrapper_keeps_alpha():
+def test_every_wrapper_method_keeps_alpha():
     op = _rq_op(5, 4)
     assert [t is u for t, u in zip(op.hyper_tensors(), [op.lengthscale, op.alpha, op.outputscale])] == [True] * 3
     assert _is_rq_with(op.t(), 3.0) and _is_rq_with(op.mT, 3.0) and _is_rq_with(op.transpose(-1, -2), 3.0)
     assert _is_rq_with(op.detach(), 3.0)
     assert _is_rq_with(op[1:3, :], 3.0) and _is_rq_with(op[:, 0:2], 3.0)
-    w = operators.with_outputscale(op, torch.tensor(2.0))
+    w = op.with_outputscale(torch.tensor(2.0))
     assert _is_rq_with(w, 3.0) and float(w.outputscale) == 2.0
     sq = _rq_op(5)
     s = sq + operators.KernelLinearOperator(sq.x1, None, "rbf", torch.tensor(1.0))
-    assert isinstance(s, operators.SumKernelLinearOperator) and _is_rq_with(s.ops[0], 3.0) and s.ops[0]._plan_slot == 1
+    assert isinstance(s, operators.SumKernelLinearOperator) and _is_rq_with(s.ops[0], 3.0)
+    # the RQ term takes the plain first-term slot, the plain term the second
+    assert [o._plan_slot for o in s.ops] == [operators._slot("plain", "sum_term", 0), operators._slot("plain", "sum_term", 1)]
     assert len(s.hyper_tensors()) == 5
     lr = operators.LowRankUpdatedKernelLinearOperator(sq, torch.randn(5, 2))
     assert _is_rq_with(lr.base, 3.0)
@@ -192,11 +194,21 @@ def test_operator_level_refusals():
         operators._additive_components([op], "additive")
 
 
-def test_plan_key_contains_alpha():
-    import inspect
-    src = inspect.getsource(operators.RQKernelLinearOperator.plan)
-    assert re.search(r'key = \("rq", tuple\(ls\), al, os_, nz\)', src)
-    assert "set_hypers_rq(ls, al, os_, nz)" in src
+def test_plan_resends_when_alpha_changes():
+    """Operators on one plan that differ in alpha alone re-send their hyper-parameters (set_hypers_rq(ls, al, os_, nz)); equal
+    ones do not."""
+    calls = []
+
+    class _P:
+        def set_hypers_rq(self, *args):
+            calls.append(args)
+
+    plan, x = _P(), torch.zeros(4, 1)
+    for al in (1.0, 1.0, 2.0):
+        op = operators.RQKernelLinearOperator(x, None, torch.tensor(0.5), torch.tensor(al), torch.tensor(1.5))
+        op._plan = plan      # an existing plan, as the cache hands out: sent only when its key differs
+        op.plan(0.25)
+    assert calls == [([0.5], 1.0, 1.5, 0.25), ([0.5], 2.0, 1.5, 0.25)]
 
 
 # ---- header, C ABI, compiled kernels ------------------------------------------------------------------------------------------

@@ -111,15 +111,15 @@ def test_flag_default_and_snapshot():
         assert settings.snapshot()[settings.ski_grid_prediction] == [True]
 
 
-def test_lowrank_on_ski_is_a_separate_constructor():
-    from gpytorch_b200.operators import LowRankUpdatedKernelLinearOperator, _LOWRANK_SLOT
+def test_lowrank_on_ski_is_a_separate_constructor_on_its_slot_key():
+    from gpytorch_b200.operators import LowRankUpdatedKernelLinearOperator, _slot
 
     train, test, others = _ops()
     assert not LowRankUpdatedKernelLinearOperator.supports(test)
     with pytest.raises(RuntimeError):
         LowRankUpdatedKernelLinearOperator(test, torch.zeros(30, 3))
     op = LowRankUpdatedKernelLinearOperator.on_ski(test, torch.zeros(30, 3))
-    assert op.shape == (30, 30) and op.base._plan_slot == _LOWRANK_SLOT and getattr(test, "_plan_slot", 0) == 0
+    assert op.shape == (30, 30) and op.base._plan_slot == _slot("plain", "lowrank") and test._plan_slot == _slot("plain", "own")
     with pytest.raises(RuntimeError):
         LowRankUpdatedKernelLinearOperator.on_ski(others["plain"], torch.zeros(30, 3))
     with pytest.raises(RuntimeError):

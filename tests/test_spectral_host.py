@@ -240,7 +240,7 @@ class _SlotPlan:
         return self
 
 
-def test_plan_slots_keep_low_rank_spectral_plans_apart(monkeypatch):
+def test_plan_slot_keys_keep_low_rank_spectral_plans_apart(monkeypatch):
     """An ordinary spectral operator, the spectral base of a low-rank (LOVE) operator and a plain low-rank base ask the plan cache
     for three different slots: a plan carrying U never serves an ordinary spectral operator, and a spectral plan never serves a
     plain one."""
@@ -259,7 +259,7 @@ def test_plan_slots_keep_low_rank_spectral_plans_apart(monkeypatch):
     k(x).plan()
     operators.LowRankUpdatedKernelLinearOperator(k(x), U).base.plan()
     operators.LowRankUpdatedKernelLinearOperator(operators.KernelLinearOperator(x, None, "rbf", torch.tensor(1.0)), U).base.plan()
-    assert slots == [operators._SPECTRAL_SLOT, operators._SPECTRAL_LOWRANK_SLOT, operators._LOWRANK_SLOT]
+    assert slots == [operators._slot("spectral", "own"), operators._slot("spectral", "lowrank"), operators._slot("plain", "lowrank")]
     assert len(set(slots)) == 3
 
 
